@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""bench.py -- headline benchmark of the B200-native slamkit hot path.
+"""bench.py -- headline benchmark of the H100-native (sm_90a) slamkit hot path.
 
 Default workload (BASELINE.json configs[1]): one optimiser step of the SLAM pre-training recipe -- Qwen2.5-0.5B-shaped
 unit LM (358 M params, vocab 502, bf16 params and optimiser state), per-GPU micro-batch [8, 1024] synthetic unit
@@ -9,6 +9,7 @@ peer-memory kernel on one node; `config.dp_comm` in the JSON line says which bac
   python bench.py --gpus N --steps K --warmup W            # our arm (one JSON line on rank 0)
   python bench.py --impl reference --gpus N --steps K ...  # CPU arm: the reference's algorithm on the host cores
   python bench.py --workload cfg4|cfg5 ...                 # BASELINE configs[3] / [4] (see run_cfg4 / run_cfg5)
+  python bench.py ... --dump-outputs DIR                   # also write the last timed step's outputs as DIR/<name>.npy
 
 Both timed legs of the default workload go through the public trainer (`slamkit_b200.trainer.B200Trainer.train_step`, what
 cli/train.py calls): token counting, global item count, forward/backward, overlapped all-reduce, clip + AdamW.
@@ -16,7 +17,7 @@ cli/train.py calls): token counting, global item count, forward/backward, overla
 `value`  : speech-tokens/s, inputs resident in HBM, CUDA-event timed, max over ranks.
 `e2e`    : same metric through the public API with HOST inputs: per step a pinned-host -> device copy of ids/labels
            and a device -> host read of the loss inside the timed region.
-`roofline`: the dominant kernel (tcgen05 GEMM, ~290 launches/step) timed live with CUDA events on its launching stream
+`roofline`: the dominant kernel (wgmma GEMM, ~290 launches/step) timed live with CUDA events on its launching stream
            in a separate profiling step; algorithmic FLOPs = 6 * N_matmul_params * tokens (SURVEY.md §8d).
 `cpu_baseline`: oracle/lm_oracle.OracleTrainer (the pinned restatement of the reference's HF path) on a bounded sample.
 """
@@ -55,6 +56,22 @@ def synth_batch(rank: int, idx: int, B: int = PER_GPU_BATCH, T: int = SEQ) -> to
     return ids
 
 
+DUMP_SAMPLE = 4 << 20   # elements of each sampled flat buffer written by --dump-outputs (16 MB of float32 each)
+
+
+def dump_outputs(out_dir: str, loss: torch.Tensor, model) -> None:
+    """What the last timed train step hands its caller, as .npy files: the step loss (float64), and a fixed, seeded sample
+    of the updated parameters and of that step's gradient buffer (float32).  The inputs are seeded, so two builds run with
+    the same arguments can be compared output for output."""
+    import numpy as np
+    os.makedirs(out_dir, exist_ok=True)
+    np.save(os.path.join(out_dir, "loss.npy"), np.array([float(loss)], dtype=np.float64))
+    g = torch.Generator().manual_seed(0)
+    idx = torch.randint(0, model.n_params, (DUMP_SAMPLE,), generator=g).sort().values.to(model.params.device)
+    np.save(os.path.join(out_dir, "params_sample.npy"), model.params[idx].float().cpu().numpy())
+    np.save(os.path.join(out_dir, "grads_sample.npy"), model.grads[idx].float().cpu().numpy())
+
+
 def usable_cpus() -> int:
     """CPU threads this process may really use: affinity mask, capped by the cgroup CPU quota (a container can see
     hundreds of host cores it is not allowed to run on; oversubscribing them makes the CPU baseline crawl)."""
@@ -74,7 +91,8 @@ def peaks():
         d = json.load(open(p))
         return {"bf16_burst": d.get("bf16_tflops"), "bf16_sustained": d.get("bf16_tflops_sustained"),
                 "hbm_gbs": d.get("hbm_gbs"), "source": "MEASURED_PEAKS.json (of measured)"}
-    return {"bf16_burst": 1590.0, "bf16_sustained": 1400.0, "hbm_gbs": 6650.0, "source": "B200_PROFILING.md (of fallback)"}
+    # NVIDIA H100 SXM data sheet (dense BF16, HBM3) at a 700 W limit: a ceiling, not a measured rate
+    return {"bf16_burst": 989.0, "bf16_sustained": 989.0, "hbm_gbs": 3350.0, "source": "H100 SXM data sheet (fallback)"}
 
 
 class ClockSampler(threading.Thread):
@@ -182,12 +200,19 @@ def run_hubert_gpu(args, rank, local_rank, world, lib, dist):
     l0 = lib.sk_launch_count()
     e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
     e0.record()
+    last = None
     for i in range(n):
-        fe.units_device(devw[i % 2], None)
+        last = fe.units_device(devw[i % 2], None)
     e1.record()
     sync()
     dev_ms = mx(e0.elapsed_time(e1))
     launches = lib.sk_launch_count() - l0
+    if args.dump_outputs and rank == 0 and last is not None:
+        # the last timed batch's unit ids and frame counts (what units_device hands its caller), as float32
+        import numpy as np
+        os.makedirs(args.dump_outputs, exist_ok=True)
+        np.save(os.path.join(args.dump_outputs, "hubert_unit_ids.npy"), last[0].float().cpu().numpy())
+        np.save(os.path.join(args.dump_outputs, "hubert_n_frames.npy"), last[1].float().cpu().numpy())
     def e2e_plain():
         for i in range(n):
             ids, nf = fe.units_device(host[i % 2], None)       # pinned host -> device inside, on the compute stream
@@ -277,13 +302,10 @@ def run_hubert_gpu(args, rank, local_rank, world, lib, dist):
         lib.sk_prof_enable(0)
         conv0_bytes = HUBERT_B * (HUBERT_T0 * 512 * 2 * 2 + (HUBERT_S + 80) * 4)
         gbs = conv0_bytes / (ms[3] / 1e3) / 1e9 if ms[3] > 0 else None
-        out["roofline"] = {"bound": "hbm", "kernel": "conv0_tc_kernel (conv0 taps + GroupNorm affine as a split-bf16 tcgen05 GEMM, "
-                                                     "GELU + hi/lo split in the epilogue, channels-last TMA stores)",
+        out["roofline"] = {"bound": "hbm", "kernel": "conv0_apply_k10s5_kernel (conv0 taps + GroupNorm affine + GELU + hi/lo split, "
+                                                     "channels-last stores)",
                            "achieved": gbs, "peak": pk["hbm_gbs"], "unit": "GB/s",
                            "frac": (gbs / pk["hbm_gbs"]) if gbs else None,
-                           # ncu --set full at batch 16: 3.0865 GB written + 0.0326 GB read per launch -> x4 at batch 64
-                           "traffic": 4 * (3.0865e9 + 0.0326e9), "traffic_unit": "bytes/launch",
-                           "traffic_source": "profiles/r02_ncu_conv0_tc.txt (batch 16, scaled x4)",
                            "algorithmic_bytes_per_launch": conv0_bytes, "peak_source": pk["source"],
                            "breakdown_ms": {"gemm": ms[0], "attention": ms[1], "conv0_apply": ms[3],
                                             "batch": dev_ms / n},
@@ -312,7 +334,7 @@ def workload_config(world: int):
     return {"workload": "SLAM pretrain step: Qwen2.5-0.5B-shaped unit LM (358M, vocab 502), unit_hubert_25 tokens, "
                         "seq=1024, per-GPU micro-batch 8, clip 0.5 + AdamW, bf16 params/state",
             "global_batch": PER_GPU_BATCH * world, "seq_len": SEQ, "parallelism": f"dp{world}",
-            "l2": "working set ~11 GB/step per GPU (activations + params + optimiser state) >> 126 MB L2"}
+            "l2": "working set ~11 GB/step per GPU (activations + params + optimiser state) >> 50 MB L2"}
 
 
 CFG4_VOCAB = 151_665 + 502      # Qwen2.5 tokenizer entries + 500 units + <speech>, <text> (interleaving_tokeniser.py:121-127)
@@ -393,7 +415,7 @@ def run_cfg4(args, rank, local_rank, world, lib, dist):
                                                  "tokens in one row, position_ids restart), clip 0.5 + AdamW, bf16",
                                      "global_batch_tokens": CFG4_TOKENS * world, "seq_len": 2048, "parallelism": f"dp{world}",
                                      "api": "slamkit_b200.trainer.B200Trainer.train_step", "documents": batches[0][1],
-                                     "l2": "working set ~20 GB/step >> 126 MB L2"},
+                                     "l2": "working set ~20 GB/step >> 50 MB L2"},
                           "e2e": {"value": CFG4_TOKENS * world * args.steps / (max(ms2, wall2) / 1e3), "unit": "tokens/s",
                                   "h2d_bytes_per_step": 3 * CFG4_TOKENS * 8, "d2h_bytes_per_step": 4},
                           "gpu_launches": int(launches),
@@ -448,7 +470,7 @@ def run_cfg5(args, rank, local_rank, world, lib, dist):
                           "config": {"workload": "cfg-5: DPO step, policy + frozen reference (358M each), 8 pairs per GPU, rows of 1024 "
                                                  "(256-token shared prompt), beta 0.1, clip 0.5 + AdamW, bf16",
                                      "global_batch_pairs": 8 * world, "seq_len": SEQ, "parallelism": f"dp{world}",
-                                     "api": "slamkit_b200.dpo.B200DPOTrainer.step", "l2": "working set >> 126 MB L2"},
+                                     "api": "slamkit_b200.dpo.B200DPOTrainer.step", "l2": "working set >> 50 MB L2"},
                           "e2e": {"value": tok * world * args.steps / (max(ms2, wall2) / 1e3), "unit": "tokens/s",
                                   "h2d_bytes_per_step": 2 * tok * 8, "d2h_bytes_per_step": 4},
                           "gpu_launches": int(launches),
@@ -473,7 +495,12 @@ def main():
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--skip-hubert", action="store_true", help="skip the secondary HuBERT audio-hours/s measurement")
     ap.add_argument("--hubert-cpu", action="store_true", help=argparse.SUPPRESS)
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="after the timed steps, write the last timed step's outputs (loss, sampled parameters and gradient; "
+                         "the HuBERT leg's unit ids) as DIR/<name>.npy (default workload only)")
     args = ap.parse_args()
+    if args.dump_outputs and (args.workload != "cfg2" or args.impl != "b200"):
+        ap.error("--dump-outputs is implemented for the default workload (--workload cfg2) of the GPU implementation")
     args.warmup = max(args.warmup, 3) if args.impl == "b200" else args.warmup
 
     rank = int(os.environ.get("RANK", "0"))
@@ -516,7 +543,7 @@ def main():
         counts.update({"n_items_global": PER_GPU_BATCH * SEQ * world, "n_tokens_global": PER_GPU_BATCH * SEQ * world})
 
     def step_device(i):
-        trainer.train_step([{"input_ids": devb[i % NB], "labels": devb[i % NB], **counts}])
+        return trainer.train_step([{"input_ids": devb[i % NB], "labels": devb[i % NB], **counts}])
 
     def step_e2e(i):
         # host ids in (one pinned-host -> device copy feeds input_ids and labels: a causal LM's labels ARE its ids),
@@ -547,12 +574,15 @@ def main():
     e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
     barrier()
     e0.record()
+    last = None
     for i in range(args.steps):
-        step_device(i)
+        last = step_device(i)
     e1.record()
     barrier()
     dev_ms = max_over_ranks(e0.elapsed_time(e1))
     launches = lib.sk_launch_count() - launches0
+    if args.dump_outputs and rank == 0 and last is not None:
+        dump_outputs(args.dump_outputs, last, model)
 
     # end-to-end through the public API with host buffers
     for i in range(2):
@@ -593,14 +623,8 @@ def main():
         gemm_ms, attn_ms, opt_ms = ms[0] / reps, ms[1] / reps, ms[2] / reps
         step_ms = dev_ms / args.steps
         gemm_tf = GEMM_FLOP_PER_TOKEN * PER_GPU_BATCH * SEQ / (gemm_ms / 1e3) / 1e12
-        # DRAM bytes per GEMM launch (read + write), mean over the step's GEMM launches: written by tools/profile_lm_step.sh
-        # from an ncu launch list of THIS build (bench.py cannot run under ncu itself)
-        traffic, traffic_src = None, None
-        tpath = os.path.join(ROOT, "profiles", "r02_lm_gemm_traffic.json")
-        if os.path.exists(tpath):
-            tj = json.load(open(tpath))
-            traffic, traffic_src = tj["gemm_dram_bytes_per_launch"], f"profiles/r02_lm_gemm_traffic.json ({tj['source']})"
-        roof = {"bound": "tensor", "kernel": f"gemm_tcgen05_kernel ({cnt[0] // reps} launches/step, fused epilogues included)",
+        traffic, traffic_src = None, None   # DRAM traffic per launch is not measured here
+        roof = {"bound": "tensor", "kernel": f"gemm_wgmma_kernel ({cnt[0] // reps} launches/step, fused epilogues included)",
                 "achieved": gemm_tf, "peak": pk["bf16_sustained"], "unit": "TFLOP/s",
                 "frac": gemm_tf / pk["bf16_sustained"], "frac_of_burst": gemm_tf / pk["bf16_burst"],
                 "traffic": traffic, "traffic_unit": "bytes/launch", "traffic_source": traffic_src,

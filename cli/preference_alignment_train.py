@@ -1,5 +1,5 @@
 """cli/preference_alignment_train.py -- drop-in for the reference entry point (cli/preference_alignment_train.py:18-69):
-DPO of a unit LM on prompt / chosen / rejected unit strings, on the sm_100a train path.
+DPO of a unit LM on prompt / chosen / rejected unit strings, on the sm_90a train path.
 
     torchrun --nproc-per-node N cli/preference_alignment_train.py data.train_path=<pairs.jsonl> data.val_path=<pairs.jsonl> \
         model.pretrained_model=<dir written by cli/train.py> training_args.output_dir=<dir> [+training_args.max_steps=K]
@@ -10,7 +10,7 @@ prompt / chosen / rejected dropped.  Step: `SLAMDPOTrainer` = trl `DPOTrainer` w
 sigmoid loss, beta 0.1, frozen copy of the initial policy as reference (slamkit_b200/dpo.py).  trl and nltk are not in
 the image: truncation uses trl's documented defaults (max_prompt_length 512, max_length 1024 unless given in
 training_args), and the repetition filter splits words with a regular expression instead of nltk's Treebank tokeniser
-(identical n-grams on plain lower-case transcripts; parity otherwise unpinned, DESIGN.md §6)."""
+(identical n-grams on plain lower-case transcripts; parity otherwise unpinned)."""
 import glob
 import json
 import logging

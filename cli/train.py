@@ -1,4 +1,4 @@
-"""cli/train.py -- drop-in for the reference entry point (cli/train.py:16-89), driving the sm_100a train step instead of
+"""cli/train.py -- drop-in for the reference entry point (cli/train.py:16-89), driving the sm_90a train step instead of
 HF Trainer.
 
     torchrun --nproc-per-node 8 cli/train.py data.train_path=<tokens.jsonl> data.val_path=<tokens.jsonl> \
@@ -8,7 +8,7 @@ Data contract of `init_dataset` (slamkit/data/hf_dataset.py:91-118): tokenise `a
 either right-pad with 0 and labels = input_ids with pad -> -100 (DataCollatorForLanguageModeling) or, with
 `data.packing=true`, flatten the mini-batch into one row with restarting `position_ids` and a -100 label at every
 document start (DataCollatorWithFlattening; the reference requires flash_attention_2 for it, cli/train.py:43-45 -- here
-the tcgen05 attention kernels are block-diagonal from the same position_ids).  Schedule / clip / AdamW as
+the attention kernels are block-diagonal from the same position_ids).  Schedule / clip / AdamW as
 config/training_args/default.yaml; evaluation every `eval_steps`, checkpoints `checkpoint-<step>` every `save_steps`
 (HF default 500) keeping `save_total_limit`, `cont_training` = HF `resume_from_checkpoint` (true: latest checkpoint
 in output_dir; a path: that checkpoint), `run_time` / `train_max_tokens` stoppers (slamkit/trainer/callbacks.py).

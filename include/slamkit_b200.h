@@ -1,4 +1,4 @@
-/* slamkit_b200 -- C ABI of the B200-native hot paths of slp-rl/slamkit.
+/* slamkit_b200 -- C ABI of the H100-native (sm_90a) hot paths of slp-rl/slamkit.
  *
  * The reference has no native code and no FFI of its own (SURVEY.md §0, §8b): both hot paths enter third-party
  * Python libraries through two plugin ABCs.  This header is therefore the interface a binding for those two plugin
@@ -25,10 +25,10 @@ extern "C" {
 /* ---- library ------------------------------------------------------------------------------------------------ */
 const char* sk_last_error(void);
 int sk_version(void);                       /* 100*major + minor */
-int sk_device_sm_count(void);               /* multiprocessor count of the current device (148 on B200) */
-int sk_device_cc(void);                     /* 10*major + minor of the current device; kernels require 100 */
+int sk_device_sm_count(void);               /* multiprocessor count of the current device (132 on H100 SXM) */
+int sk_device_cc(void);                     /* 10*major + minor of the current device; kernels require 90 */
 
-/* ---- tensor-core GEMM (tcgen05 + TMA + TMEM) ------------------------------------------------------------------
+/* ---- tensor-core GEMM (wgmma + TMA) ---------------------------------------------------------------------------
  * C[M,N] = A * B^T (+ bias[N]) (+ residual[M,N]); bf16 operands, fp32 accumulation, bf16 (or fp32) output.
  *   a_mn = 0: A is [M,K] row-major (lda = row pitch);  a_mn = 1: A is stored transposed as [K,M] (lda = its pitch).
  *   b_mn = 0: B is [N,K] row-major (a torch Linear weight);  b_mn = 1: B is stored as [K,N].
@@ -108,7 +108,7 @@ int sk_ce_fwd_bwd(const void* logits, const int64_t* labels, void* dlogits, floa
  * (HF:models/qwen2/modeling_qwen2.py:187-246) and HubertAttention (HF:models/hubert/modeling_hubert.py:262-345). */
 int sk_attn_fwd(const void* q, const void* k, const void* v, void* o, float* lse, int B, int T, int H, int KVH, int ld,
                 int ldo, int causal, float scale, void* stream);
-/* tcgen05 / TMEM implementation of the same forward (S and O accumulate in tensor memory, operands staged by TMA).
+/* The same forward on the fused projection (optionally block-diagonal over packed documents).
  * qkv points at the fused [B*T, ld] projection: H q-heads, then KVH k-heads, then KVH v-heads, 64 columns each. */
 int sk_attn_tc_fwd(const void* qkv, void* o, float* lse, int B, int T, int H, int KVH, int ld, int ldo, int causal,
                    float scale, const int32_t* seg_start, void* stream);
@@ -116,11 +116,11 @@ int sk_attn_tc_fwd(const void* qkv, void* o, float* lse, int B, int T, int H, in
  * column 0 and wherever position_ids == 0, exactly how HF derives cu_seqlens for its varlen flash-attention path
  * (HF:modeling_flash_attention_utils.py prepare_fa_kwargs_from_position_ids).  seg_start[b*T+t] = in-row index of the
  * first token of t's document, seg_end = one past its last.  Passing them (NULL = one document per row) to
- * sk_attn_tc_fwd / sk_attn_tc_bwd makes attention block-diagonal causal; key tiles outside a tile's documents are
- * skipped. */
+ * sk_attn_tc_fwd / sk_attn_tc_bwd makes attention block-diagonal causal. */
 int sk_seg_bounds(const int32_t* pos_ids, int32_t* seg_start, int32_t* seg_end, int B, int T, void* stream);
-/* tcgen05 backward: dqkv (same fused layout as qkv, pitch ldg) from d_o; delta fp32 [B,H,T] and partial fp32
- * [B,H,T,128] are caller scratch.  Deterministic (per-head partials reduced over the GQA group in a fixed order). */
+/* Backward on the fused projection: dqkv (same fused layout as qkv, pitch ldg) from d_o; delta fp32 [B,H,T] is caller
+ * scratch; partial is accepted for ABI compatibility, unused, and may be NULL.  Deterministic (dK / dV summed over
+ * the GQA group in a fixed order). */
 int sk_attn_tc_bwd(const void* qkv, const void* o, const void* d_o, const float* lse, float* delta, float* partial,
                    void* dqkv, int B, int T, int H, int KVH, int ld, int ldo, int ldg, int causal, float scale,
                    const int32_t* seg_start, const int32_t* seg_end, void* stream);
@@ -296,13 +296,13 @@ int sk_p2p_wait(void* const* flags, int rank, int world, int slot_lo, int n_slot
  * 1 reduce kernel running, 2 peers ready, 3 last CTA done; row 256: wait kernel start / end); NULL switches it off. */
 int sk_p2p_set_trace(void* buf);
 /* Test hook: `ctas` CTAs with the reduce kernel's footprint (64 threads, <= 64 registers, no shared memory) that hold their
- * slot for `ns` nanoseconds; started_u32 counts the CTAs that got onto an SM (tools/coresidency_check.py). */
+ * slot for `ns` nanoseconds; started_u32 counts the CTAs that got onto an SM. */
 int sk_p2p_debug_hog(int ctas, int64_t ns, void* started_u32, void* stream);
 
 /* number of kernels this library launched since load (bench.py's gpu_launches) */
 int64_t sk_launch_count(void);
 /* Bench-only device timing: when enabled, CUDA events are recorded on the launching stream around every launch of
- * category 0 (tcgen05 GEMM), 1 (attention), 2 (optimiser).  sk_prof_collect synchronises the device and returns the
+ * category 0 (GEMM), 1 (attention), 2 (optimiser).  sk_prof_collect synchronises the device and returns the
  * summed milliseconds and launch-group counts per category (arrays of 4), then resets. */
 int sk_prof_enable(int on);
 int sk_prof_collect(double* ms_by_cat, int64_t* count_by_cat);

@@ -260,6 +260,54 @@ def make_hubert_golden(out_path: str):
     print("hubert golden ->", out_path, "frames", hs.shape, "lens", [len(t) for t in toks])
 
 
+def _param_digest(t: torch.Tensor) -> np.ndarray:
+    """shape-sensitive fingerprint of a parameter: (sum, sum of x * flat index) in float64"""
+    x = t.detach().double().flatten()
+    return np.array([float(x.sum()), float((x * torch.arange(x.numel(), dtype=torch.float64)).sum())])
+
+
+def make_checkpoint_golden(out_path: str):
+    """The reference's own `UnitLM.from_pretrained` on the directory `write_unit_lm_checkpoint` writes (seeded oracle
+    parameters): the state-dict keys it ends up with, a fingerprint of every loaded parameter, and its bf16 logits on seeded
+    tokens."""
+    import types
+    from oracle import lm_oracle as O
+    from slamkit_b200.lm import LMConfig, write_unit_lm_checkpoint
+    import slamkit.model.unit_lm as ref_mod
+    from slamkit.model.unit_lm import UnitLM
+    from transformers import OPTConfig
+    real = ref_mod.AutoConfig.from_pretrained
+    # the reference's default base model is looked up on the hub (unit_lm.py:37,66-70): stand in for that one lookup
+    ref_mod.AutoConfig.from_pretrained = staticmethod(lambda name, *a, **k: OPTConfig() if name == "facebook/opt-350M" else real(name, *a, **k))
+    ocfg = O.OracleLMConfig(vocab_size=502, hidden=128, n_layers=2, n_heads=2, n_kv_heads=1, head_dim=64, ffn=256)
+    p = O.init_params(ocfg, seed=3)
+    tmp = tempfile.mkdtemp()
+    base, ck = os.path.join(tmp, "base"), os.path.join(tmp, "ck")
+    os.makedirs(base)
+    cfg = LMConfig(vocab_size=502, hidden=128, n_layers=2, n_heads=2, n_kv_heads=1, head_dim=64, ffn=256)
+    write_unit_lm_checkpoint(ck, p, cfg, base_model_name=base)
+    json.dump(json.load(open(os.path.join(ck, "config.json")))["base_config"], open(os.path.join(base, "config.json"), "w"))
+    model = UnitLM.from_pretrained(ck, torch_dtype=torch.bfloat16)
+    sd = model.state_dict()
+    keys = sorted(sd)
+    g = torch.Generator().manual_seed(1)
+    ids = torch.randint(2, 502, (2, 24), generator=g)
+    ids[:, 0] = 1
+    with torch.no_grad():
+        logits = model(input_ids=ids).logits.to(torch.bfloat16)
+    np.savez_compressed(out_path, keys=np.array(keys), digests=np.stack([_param_digest(sd[k]) for k in keys]),
+                        shapes=np.array([json.dumps(list(sd[k].shape)) for k in keys]), ids=ids.numpy(),
+                        logits_u16=bf16_to_u16(logits))
+    print("checkpoint golden ->", out_path, len(keys), "keys")
+
+
+def copy_example_audio(out_dir: str):
+    """The reference's example FLAC files (decoder known answers: sample counts and STREAMINFO MD5)."""
+    import shutil
+    for name in ("audio1.flac", "audio2.flac"):
+        shutil.copyfile(os.path.join(REF, "example_data", "audio", name), os.path.join(out_dir, name))
+
+
 if __name__ == "__main__":
     assert os.path.isdir(REF), "the reference is only mounted in the build container"
     _stub_omegaconf()
@@ -277,3 +325,7 @@ if __name__ == "__main__":
         make_tokeniser_golden(os.path.join(gd, "tokeniser.npz"))
     if "hubert" in which:
         make_hubert_golden(os.path.join(gd, "hubert_tiny.npz"))
+    if "checkpoint" in which:
+        make_checkpoint_golden(os.path.join(gd, "unit_lm_checkpoint.npz"))
+    if "audio" in which:
+        copy_example_audio(gd)

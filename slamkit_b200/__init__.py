@@ -1,4 +1,4 @@
-"""slamkit_b200 -- B200-native (sm_100a) hot paths of slp-rl/slamkit behind the reference's plugin interfaces.
+"""slamkit_b200 -- H100-native (sm_90a) hot paths of slp-rl/slamkit behind the reference's plugin interfaces.
 
 Only what the two hot paths need lives here:
   csrc/                hand-written CUDA kernels + the C ABI (libslamkit_b200.so, include/slamkit_b200.h)

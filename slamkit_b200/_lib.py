@@ -97,11 +97,11 @@ def require_cuda():
     import torch
 
     if not torch.cuda.is_available():
-        raise SkError("slamkit_b200 needs a CUDA device (sm_100a); there is no CPU fallback")
+        raise SkError("slamkit_b200 needs a CUDA device (sm_90a); there is no CPU fallback")
     lib = load()
     cc = lib.sk_device_cc()
-    if cc != 100:
-        raise SkError(f"slamkit_b200 kernels are built for sm_100a only; current device reports compute capability {cc}")
+    if cc != 90:
+        raise SkError(f"slamkit_b200 kernels are built for sm_90a only; current device reports compute capability {cc}")
     return lib
 
 

@@ -1,6 +1,6 @@
 """A small Hydra-compatible config loader for the slamkit CLI surface (SURVEY.md §5, §8 b-3).
 
-`hydra-core` / `omegaconf` are not part of the B200 image, and the hot paths must not depend on them, so this module
+`hydra-core` / `omegaconf` are not dependencies of this package, and the hot paths must not depend on them, so this module
 re-implements the subset of Hydra 1.3 semantics that the reference's `config/` tree and README one-liners use:
 `defaults:` lists (group selection, nested `/group: name`, `override /group: name`, `_self_`), the
 `# @package _global_` directive, `group=name` and dotted `key=value` / `+key=value` command-line overrides, `???`

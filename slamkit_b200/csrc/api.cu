@@ -53,7 +53,7 @@ int sk_num_sms() {
     int dev = 0;
     if (cudaGetDevice(&dev) != cudaSuccess ||
         cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || n <= 0)
-      n = 148;
+      n = 132;   // H100 SXM
   }
   return n;
 }
@@ -183,7 +183,7 @@ int sk_seg_bounds(const int32_t* pos_ids, int32_t* seg_start, int32_t* seg_end, 
 int sk_attn_tc_bwd(const void* qkv, const void* o, const void* d_o, const float* lse, float* delta, float* partial,
                    void* dqkv, int B, int T, int H, int KVH, int ld, int ldo, int ldg, int causal, float scale,
                    const int32_t* seg_start, const int32_t* seg_end, void* stream) {
-  SK_REQUIRE(qkv && o && d_o && lse && delta && partial && dqkv, "sk_attn_tc_bwd: null argument");
+  SK_REQUIRE(qkv && o && d_o && lse && delta && dqkv, "sk_attn_tc_bwd: null argument");
   return sk_attn_tc_bwd_launch(CBF(qkv), CBF(o), CBF(d_o), lse, delta, partial, BF(dqkv), B, T, H, KVH, ld, ldo, ldg, causal,
                                scale, S(stream), seg_start, seg_end);
 }

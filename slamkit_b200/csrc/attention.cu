@@ -1,20 +1,29 @@
 // Flash-style attention for the causal-LM path (GQA, head_dim 64; HF:models/qwen2/modeling_qwen2.py:187-246) and the
 // bidirectional HuBERT encoder (HF:models/hubert/modeling_hubert.py:262-345), forward and backward.
 //
-// Round-1 implementation: tiled online-softmax kernels on the warp-level tensor-core path (mma.sync m16n8k16 bf16,
-// ldmatrix from XOR-swizzled shared memory, cp.async double buffering).  S/P never touch HBM; the backward is split
-// in two deterministic kernels (dK/dV per key tile looping over the GQA group, dQ per query tile) so no atomics are
-// needed.  The tcgen05/TMEM version of these kernels is the round-2 item (attention is 5.8 % of the step FLOPs).
+// Tiled online-softmax kernels on the sm_90a warpgroup tensor cores: every 64-row block of scores and every product
+// with P / dS is one wgmma.mma_async chain (m64n64k16 bf16, fp32 accumulate).  Operand tiles are staged by cp.async
+// (double-buffered) into 1024-byte-aligned [rows][64] bf16 tiles in the 128B-swizzled layout wgmma reads directly;
+// P and dS stay in registers and feed the next product as the register A operand.  S/P never touch HBM; the backward
+// is split in two deterministic kernels (dK/dV per key tile looping over the GQA group, dQ per query tile) so no atomics
+// are needed.
+//
+// Packed batches: with seg_start (int32 [B*T], in-row index of the first token of each token's document) the causal
+// kernels mask keys before the query's document start -- block-diagonal causal attention.
 //
 // Layout: q/k/v are column slices of the fused projection output [B*T, ld] (q: H*64 cols, k/v: KVH*64 cols);
 // o is [B*T, H*64]; lse is [B, H, T] fp32 (natural log of the scaled-score softmax denominator); delta likewise.
-#include "common.cuh"
+#include "kernels.h"
 
 namespace {
 
 constexpr int HD = 64;  // head dim
 
+// [rows][64] bf16 tile, 128-byte rows, 16-byte chunks XOR-swizzled by row % 8: with a 1024-byte-aligned base this is the
+// SWIZZLE_128B K-major layout wgmma descriptors describe
 SK_DEVINL uint32_t tile_addr(uint32_t base, int r, int chunk) { return base + r * 128 + ((chunk ^ (r & 7)) << 4); }
+// 1024-byte-aligned start of the dynamic shared memory (launches request 1 KB extra)
+SK_DEVINL uint32_t smem_base_1k(const void* p) { return (smem_u32(p) + 1023u) & ~1023u; }
 
 SK_DEVINL void cp_async16(uint32_t saddr, const void* g, bool pred) {
   const int sz = pred ? 16 : 0;
@@ -26,21 +35,17 @@ SK_DEVINL void cp_async_wait() {
   asm volatile("cp.async.wait_group %0;" ::"n"(N) : "memory");
 }
 
-SK_DEVINL void ldsm_x4(uint32_t& r0, uint32_t& r1, uint32_t& r2, uint32_t& r3, uint32_t addr) {
-  asm volatile("ldmatrix.sync.aligned.m8n8.x4.shared.b16 {%0,%1,%2,%3}, [%4];"
-               : "=r"(r0), "=r"(r1), "=r"(r2), "=r"(r3)
-               : "r"(addr));
-}
-SK_DEVINL void ldsm_x4_t(uint32_t& r0, uint32_t& r1, uint32_t& r2, uint32_t& r3, uint32_t addr) {
-  asm volatile("ldmatrix.sync.aligned.m8n8.x4.trans.shared.b16 {%0,%1,%2,%3}, [%4];"
-               : "=r"(r0), "=r"(r1), "=r"(r2), "=r"(r3)
-               : "r"(addr));
-}
-SK_DEVINL void mma16816(float (&d)[4], const uint32_t (&a)[4], uint32_t b0, uint32_t b1) {
+// m64n64k16 with the A operand in registers (a[4]: the mma.sync m16n8k16 A fragment of this warp's 16 rows)
+SK_DEVINL void wgmma_m64n64_rs(float (&d)[32], const uint32_t (&a)[4], uint64_t db) {
   asm volatile(
-      "mma.sync.aligned.m16n8k16.row.col.f32.bf16.bf16.f32 {%0,%1,%2,%3}, {%4,%5,%6,%7}, {%8,%9}, {%0,%1,%2,%3};"
-      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3])
-      : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "r"(b0), "r"(b1));
+      "{\n\t.reg .pred p;\n\tsetp.eq.u32 p, 1, 1;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n64k16.f32.bf16.bf16 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,"
+      "%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31}, {%32,%33,%34,%35}, %36, p, 1, 1, 1;\n\t}\n"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]),
+        "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]),
+        "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]),
+        "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+      : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(db));
 }
 
 // rows x 64 bf16 tile, global (row pitch ld) -> swizzled smem; rows >= limit are zero-filled
@@ -54,46 +59,31 @@ SK_DEVINL void load_tile(uint32_t sbase, const bf16* g, int ld, int row0, int li
   }
 }
 
-// A fragments (16 rows x 64 k) of a [rows][64] smem tile starting at row r0: a[ks][4]
-SK_DEVINL void load_a_frags(uint32_t sbase, int r0, uint32_t (&a)[4][4]) {
-  const int lane = threadIdx.x & 31;
-  const int r = r0 + (lane & 7) + 8 * ((lane >> 3) & 1);
+// Per warpgroup, acc = this warp's 16 rows x 64 columns of a 64 x 64 fp32 tile in the mma.sync C layout (acc[nt][e]:
+// rows lane/4 (+8 for e >= 2), columns 8 nt + 2 (lane % 4) + (e & 1)), which is also the wgmma m64n64 accumulator layout.
+// All four warps of the warpgroup call these together.
+
+// acc += A * B^T: A = [64 rows][64 k] smem tile (this warpgroup's rows), B = [64 n-rows][64 k] smem tile; both K-major.
+// Used for S = Q K^T, S^T = K Q^T, dP = dO V^T, dP^T = V dO^T.
+SK_DEVINL void wg_a_bT(float (&acc)[8][4], uint32_t sA, uint32_t sB) {
+  float(&d)[32] = reinterpret_cast<float(&)[32]>(acc);
+  wgmma_fence();
 #pragma unroll
-  for (int ks = 0; ks < 4; ++ks) ldsm_x4(a[ks][0], a[ks][1], a[ks][2], a[ks][3], tile_addr(sbase, r, ks * 2 + (lane >> 4)));
+  for (int ks = 0; ks < 4; ++ks)
+    wgmma_m64n64<0, 0>(d, gmma_desc_sw128(sA + ks * 32, 16, 1024), gmma_desc_sw128(sB + ks * 32, 16, 1024));
+  wgmma_commit();
+  wgmma_wait<0>();
 }
 
-// acc[16 x 64] (8 n-tiles) += A(16 x 64 k-frags) * B^T where B tile is [64 n-rows][64 k] in smem (non-transposed
-// ldmatrix): used for S = Q K^T, S^T = K Q^T, dP = dO V^T, dP^T = V dO^T.
-SK_DEVINL void gemm_a_bT(float (&acc)[8][4], const uint32_t (&a)[4][4], uint32_t sB) {
-  const int lane = threadIdx.x & 31;
+// acc += P * B: P = this warp's 16 x 64 bf16 A fragments p[kk][4] (registers), B = [64 k-rows][64 n] smem tile (the n
+// index contiguous: MN-major, 16 k-rows = 2048 bytes per step).  Used for O = P V, dV = P^T dO, dK = dS^T Q, dQ = dS K.
+SK_DEVINL void wg_p_b(float (&acc)[8][4], const uint32_t (&p)[4][4], uint32_t sB) {
+  float(&d)[32] = reinterpret_cast<float(&)[32]>(acc);
+  wgmma_fence();
 #pragma unroll
-  for (int ks = 0; ks < 4; ++ks) {
-#pragma unroll
-    for (int np = 0; np < 4; ++np) {
-      uint32_t b0, b1, b2, b3;
-      const int nrow = np * 16 + (lane & 7) + 8 * (lane >> 4);
-      ldsm_x4(b0, b1, b2, b3, tile_addr(sB, nrow, ks * 2 + ((lane >> 3) & 1)));
-      mma16816(acc[2 * np], a[ks], b0, b1);
-      mma16816(acc[2 * np + 1], a[ks], b2, b3);
-    }
-  }
-}
-
-// acc[16 x 64 dims] += P(16 x 64 k, packed bf16 A frags p[kk][4]) * B where B tile is [64 k-rows][64 n] in smem
-// (transposed ldmatrix): used for O = P V, dV = P^T dO, dK = dS^T Q, dQ = dS K.
-SK_DEVINL void gemm_p_b(float (&acc)[8][4], const uint32_t (&p)[4][4], uint32_t sB) {
-  const int lane = threadIdx.x & 31;
-#pragma unroll
-  for (int kk = 0; kk < 4; ++kk) {
-#pragma unroll
-    for (int dp = 0; dp < 4; ++dp) {
-      uint32_t b0, b1, b2, b3;
-      const int krow = kk * 16 + (lane & 7) + 8 * ((lane >> 3) & 1);
-      ldsm_x4_t(b0, b1, b2, b3, tile_addr(sB, krow, dp * 2 + (lane >> 4)));
-      mma16816(acc[2 * dp], p[kk], b0, b1);
-      mma16816(acc[2 * dp + 1], p[kk], b2, b3);
-    }
-  }
+  for (int kk = 0; kk < 4; ++kk) wgmma_m64n64_rs(d, p[kk], gmma_desc_sw128(sB + kk * 2048, 8192, 1024));
+  wgmma_commit();
+  wgmma_wait<0>();
 }
 
 // accumulator tile (16 x 64, fp32) -> bf16 A fragments for the next matmul
@@ -120,9 +110,10 @@ SK_DEVINL void zero_acc(float (&a)[8][4]) {
 template <bool CAUSAL>
 __global__ void __launch_bounds__(256, 2)
 attn_fwd_kernel(const bf16* __restrict__ q, const bf16* __restrict__ k, const bf16* __restrict__ v, bf16* __restrict__ o,
-                float* __restrict__ lse, int T, int ld, int ldo, int H, int group, float scale) {
+                float* __restrict__ lse, int T, int ld, int ldo, int H, int group, float scale,
+                const int* __restrict__ seg_start) {
   extern __shared__ __align__(128) uint8_t smem_attn[];
-  const uint32_t sQ = smem_u32(smem_attn);
+  const uint32_t sQ = smem_base_1k(smem_attn);
   const uint32_t sK = sQ + 128 * 128;
   const uint32_t sV = sK + 2 * 64 * 128;
   const int b = blockIdx.z, h = blockIdx.y;
@@ -144,11 +135,15 @@ attn_fwd_kernel(const bf16* __restrict__ q, const bf16* __restrict__ k, const bf
   load_tile<64, 256>(sV, vp, ld, 0, T);
   cp_async_commit();
 
-  uint32_t qa[4][4];
+  const uint32_t sQw = sQ + (uint32_t)(warp >> 2) * 8192u;   // this warpgroup's 64 query rows
   float oacc[8][4];
   zero_acc(oacc);
   float m_i[2] = {-INFINITY, -INFINITY}, l_i[2] = {0.f, 0.f};
   const int row_a = q0 + warp * 16 + (lane >> 2);  // this thread's rows: row_a, row_a + 8
+  int seg_r[2] = {0, 0};                            // first key of each row's document
+#pragma unroll
+  for (int r = 0; r < 2; ++r)
+    if (seg_start && row_a + 8 * r < T) seg_r[r] = seg_start[(size_t)b * T + row_a + 8 * r];
 
   for (int j = 0; j < n_kv; ++j) {
     const int st = j & 1;
@@ -161,14 +156,13 @@ attn_fwd_kernel(const bf16* __restrict__ q, const bf16* __restrict__ k, const bf
       cp_async_wait<0>();
     }
     __syncthreads();
-    if (j == 0) load_a_frags(sQ, warp * 16, qa);
 
     float s[8][4];
     zero_acc(s);
-    gemm_a_bT(s, qa, sK + st * 8192);
+    wg_a_bT(s, sQw, sK + st * 8192);
 
     const int k0 = j * 64;
-    const bool need_mask = (CAUSAL && (k0 + 63 > q0 + warp * 16)) || (k0 + 64 > T);
+    const bool need_mask = (CAUSAL && (k0 + 63 > q0 + warp * 16)) || (k0 + 64 > T) || seg_start;
     if (need_mask) {
 #pragma unroll
       for (int nt = 0; nt < 8; ++nt) {
@@ -176,7 +170,7 @@ attn_fwd_kernel(const bf16* __restrict__ q, const bf16* __restrict__ k, const bf
         for (int e = 0; e < 4; ++e) {
           const int key = k0 + nt * 8 + (lane & 3) * 2 + (e & 1);
           const int row = row_a + ((e >> 1) << 3);
-          if (key >= T || (CAUSAL && key > row)) s[nt][e] = -INFINITY;
+          if (key >= T || (CAUSAL && key > row) || key < seg_r[e >> 1]) s[nt][e] = -INFINITY;
         }
       }
     }
@@ -220,7 +214,7 @@ attn_fwd_kernel(const bf16* __restrict__ q, const bf16* __restrict__ k, const bf
     }
     uint32_t pa[4][4];
     acc_to_a(s, pa);
-    gemm_p_b(oacc, pa, sV + st * 8192);
+    wg_p_b(oacc, pa, sV + st * 8192);
     __syncthreads();
   }
   // finalize
@@ -270,7 +264,7 @@ attn_fwd_split_kernel(const bf16* __restrict__ q_hi, const bf16* __restrict__ q_
                       const bf16* __restrict__ k_lo, const bf16* __restrict__ v_hi, const bf16* __restrict__ v_lo,
                       bf16* __restrict__ o_hi, bf16* __restrict__ o_lo, int T, int ld, int ldo, float scale) {
   extern __shared__ __align__(128) uint8_t smem_attn[];
-  const uint32_t sQh = smem_u32(smem_attn);
+  const uint32_t sQh = smem_base_1k(smem_attn);
   const uint32_t sQl = sQh + 128 * 128;
   const uint32_t sKV = sQl + 128 * 128;  // per stage: Kh, Kl, Vh, Vl (4 x 8 KB)
   const int b = blockIdx.z, h = blockIdx.y;
@@ -292,7 +286,7 @@ attn_fwd_split_kernel(const bf16* __restrict__ q_hi, const bf16* __restrict__ q_
   load_kv(0, 0);
   cp_async_commit();
 
-  uint32_t qh[4][4], ql[4][4];
+  const uint32_t qh = sQh + (uint32_t)(warp >> 2) * 8192u, ql = sQl + (uint32_t)(warp >> 2) * 8192u;   // this warpgroup's rows
   float oacc[8][4];
   zero_acc(oacc);
   float m_i[2] = {-INFINITY, -INFINITY}, l_i[2] = {0.f, 0.f};
@@ -308,16 +302,12 @@ attn_fwd_split_kernel(const bf16* __restrict__ q_hi, const bf16* __restrict__ q_
       cp_async_wait<0>();
     }
     __syncthreads();
-    if (j == 0) {
-      load_a_frags(sQh, warp * 16, qh);
-      load_a_frags(sQl, warp * 16, ql);
-    }
     const uint32_t sb = sKV + st * 4 * 8192;
     float s[8][4];
     zero_acc(s);
-    gemm_a_bT(s, ql, sb);          // Ql Kh^T (small terms first)
-    gemm_a_bT(s, qh, sb + 8192);   // Qh Kl^T
-    gemm_a_bT(s, qh, sb);          // Qh Kh^T
+    wg_a_bT(s, ql, sb);          // Ql Kh^T (small terms first)
+    wg_a_bT(s, qh, sb + 8192);   // Qh Kl^T
+    wg_a_bT(s, qh, sb);          // Qh Kh^T
     const int k0 = j * 64;
     if (k0 + 64 > T) {
 #pragma unroll
@@ -364,9 +354,9 @@ attn_fwd_split_kernel(const bf16* __restrict__ q_hi, const bf16* __restrict__ q_
     }
     uint32_t ph[4][4], pl[4][4];
     acc_to_a_split(s, ph, pl);
-    gemm_p_b(oacc, pl, sb + 2 * 8192);  // Pl Vh
-    gemm_p_b(oacc, ph, sb + 3 * 8192);  // Ph Vl
-    gemm_p_b(oacc, ph, sb + 2 * 8192);  // Ph Vh
+    wg_p_b(oacc, pl, sb + 2 * 8192);  // Pl Vh
+    wg_p_b(oacc, ph, sb + 3 * 8192);  // Ph Vl
+    wg_p_b(oacc, ph, sb + 2 * 8192);  // Ph Vh
     __syncthreads();
   }
 #pragma unroll
@@ -437,12 +427,13 @@ __global__ void __launch_bounds__(128, 3)
 attn_bwd_dkdv_kernel(const bf16* __restrict__ q, const bf16* __restrict__ k, const bf16* __restrict__ v,
                      const bf16* __restrict__ d_o, const float* __restrict__ lse, const float* __restrict__ delta,
                      bf16* __restrict__ dk, bf16* __restrict__ dv, int T, int ld, int ldo, int ldg, int H, int group,
-                     float scale) {
+                     float scale, const int* __restrict__ seg_start) {
   extern __shared__ __align__(128) uint8_t smem_attn[];
-  const uint32_t sKV = smem_u32(smem_attn);            // K tile then V tile (each 8 KB), only used for the prologue
+  const uint32_t sKV = smem_base_1k(smem_attn);        // K tile then V tile (each 8 KB)
   const uint32_t sQ = sKV + 2 * 8192;                  // 2 stages
   const uint32_t sdO = sQ + 2 * 8192;                  // 2 stages
-  float* sStat = reinterpret_cast<float*>(smem_attn + 6 * 8192);  // [2 stages][2 (lse, delta)][64]
+  float* sStat = reinterpret_cast<float*>(smem_attn + (sKV - smem_u32(smem_attn)) + 6 * 8192);  // [2 stages][2 (lse, delta)][64]
+  int* sSeg = reinterpret_cast<int*>(sStat + 2 * 2 * 64);          // [2 stages][64] document start of each query row
   const int b = blockIdx.z, g = blockIdx.y;
   const int kt = blockIdx.x;  // tile 0 has the most work under the causal mask and is scheduled first
   const int k0 = kt * 64;
@@ -472,6 +463,7 @@ attn_bwd_dkdv_kernel(const bf16* __restrict__ q, const bf16* __restrict__ k, con
       const size_t off = ((size_t)b * H + h) * T + (row < T ? row : 0);
       sStat[(st * 2 + 0) * 64 + threadIdx.x] = row < T ? lse[off] : 0.f;
       sStat[(st * 2 + 1) * 64 + threadIdx.x] = row < T ? delta[off] : 0.f;
+      sSeg[st * 64 + threadIdx.x] = (seg_start && row < T) ? seg_start[(size_t)b * T + row] : 0;
     }
     cp_async_commit();
   };
@@ -496,14 +488,11 @@ attn_bwd_dkdv_kernel(const bf16* __restrict__ q, const bf16* __restrict__ k, con
     const float* s_lse = sStat + (st * 2 + 0) * 64;
     const float* s_del = sStat + (st * 2 + 1) * 64;
 
-    // K / V A-fragments are re-read from their resident smem tiles each iteration (8 ldmatrix) instead of being
-    // pinned in 32 registers: that keeps the kernel under 170 registers -> 3 CTAs per SM
-    uint32_t fa[4][4];
-    load_a_frags(sKV, warp * 16, fa);
     float st_acc[8][4];  // S^T tile: rows = keys (this warp's 16), cols = 64 query rows
     zero_acc(st_acc);
-    gemm_a_bT(st_acc, fa, sQ + st * 8192);
-    const bool need_mask = (CAUSAL && (q0 < k0 + 64)) || (q0 + 64 > T) || (k0 + 64 > T);
+    wg_a_bT(st_acc, sKV, sQ + st * 8192);
+    const int* s_seg = sSeg + st * 64;
+    const bool need_mask = (CAUSAL && (q0 < k0 + 64)) || (q0 + 64 > T) || (k0 + 64 > T) || seg_start;
 #pragma unroll
     for (int nt = 0; nt < 8; ++nt) {
 #pragma unroll
@@ -513,19 +502,18 @@ attn_bwd_dkdv_kernel(const bf16* __restrict__ q, const bf16* __restrict__ k, con
         float pv = exp2f(st_acc[nt][e] * sl2 - s_lse[qi] * 1.4426950408889634f);
         if (need_mask) {
           const int qrow = q0 + qi;
-          if (qrow >= T || key >= T || (CAUSAL && key > qrow)) pv = 0.f;
+          if (qrow >= T || key >= T || (CAUSAL && key > qrow) || key < s_seg[qi]) pv = 0.f;
         }
         st_acc[nt][e] = pv;
       }
     }
     uint32_t pa[4][4];
     acc_to_a(st_acc, pa);
-    gemm_p_b(dvacc, pa, sdO + st * 8192);  // dV += P^T dO
+    wg_p_b(dvacc, pa, sdO + st * 8192);  // dV += P^T dO
 
     float dp[8][4];
     zero_acc(dp);
-    load_a_frags(sKV + 8192, warp * 16, fa);
-    gemm_a_bT(dp, fa, sdO + st * 8192);  // dP^T = V dO^T
+    wg_a_bT(dp, sKV + 8192, sdO + st * 8192);  // dP^T = V dO^T
 #pragma unroll
     for (int nt = 0; nt < 8; ++nt) {
 #pragma unroll
@@ -535,7 +523,7 @@ attn_bwd_dkdv_kernel(const bf16* __restrict__ q, const bf16* __restrict__ k, con
       }
     }
     acc_to_a(dp, pa);
-    gemm_p_b(dkacc, pa, sQ + st * 8192);  // dK += dS^T Q
+    wg_p_b(dkacc, pa, sQ + st * 8192);  // dK += dS^T Q
     __syncthreads();
   }
 #pragma unroll
@@ -560,9 +548,10 @@ template <bool CAUSAL>
 __global__ void __launch_bounds__(128)
 attn_bwd_dq_kernel(const bf16* __restrict__ q, const bf16* __restrict__ k, const bf16* __restrict__ v,
                    const bf16* __restrict__ d_o, const float* __restrict__ lse, const float* __restrict__ delta,
-                   bf16* __restrict__ dq, int T, int ld, int ldo, int ldg, int H, int group, float scale) {
+                   bf16* __restrict__ dq, int T, int ld, int ldo, int ldg, int H, int group, float scale,
+                   const int* __restrict__ seg_start) {
   extern __shared__ __align__(128) uint8_t smem_attn[];
-  const uint32_t sQdO = smem_u32(smem_attn);  // Q tile, dO tile (prologue only)
+  const uint32_t sQdO = smem_base_1k(smem_attn);  // Q tile, dO tile
   const uint32_t sK = sQdO + 2 * 8192;        // 2 stages
   const uint32_t sV = sK + 2 * 8192;          // 2 stages
   const int b = blockIdx.z, h = blockIdx.y;
@@ -585,14 +574,15 @@ attn_bwd_dq_kernel(const bf16* __restrict__ q, const bf16* __restrict__ k, const
 
   const int row_a = q0 + warp * 16 + (lane >> 2);
   float lse_r[2], del_r[2];
+  int seg_r[2];
 #pragma unroll
   for (int r = 0; r < 2; ++r) {
     const int row = row_a + 8 * r;
     const size_t off = ((size_t)b * H + h) * T + (row < T ? row : 0);
     lse_r[r] = row < T ? lse[off] * 1.4426950408889634f : 0.f;
     del_r[r] = row < T ? delta[off] : 0.f;
+    seg_r[r] = (seg_start && row < T) ? seg_start[(size_t)b * T + row] : 0;
   }
-  uint32_t qa[4][4], doa[4][4];
   float dqacc[8][4];
   zero_acc(dqacc);
 
@@ -607,15 +597,11 @@ attn_bwd_dq_kernel(const bf16* __restrict__ q, const bf16* __restrict__ k, const
       cp_async_wait<0>();
     }
     __syncthreads();
-    if (j == 0) {
-      load_a_frags(sQdO, warp * 16, qa);
-      load_a_frags(sQdO + 8192, warp * 16, doa);
-    }
     const int k0 = j * 64;
     float s[8][4];
     zero_acc(s);
-    gemm_a_bT(s, qa, sK + st * 8192);
-    const bool need_mask = (CAUSAL && (k0 + 63 > q0 + warp * 16)) || (k0 + 64 > T) || (q0 + 64 > T);
+    wg_a_bT(s, sQdO, sK + st * 8192);
+    const bool need_mask = (CAUSAL && (k0 + 63 > q0 + warp * 16)) || (k0 + 64 > T) || (q0 + 64 > T) || seg_start;
 #pragma unroll
     for (int nt = 0; nt < 8; ++nt) {
 #pragma unroll
@@ -624,14 +610,14 @@ attn_bwd_dq_kernel(const bf16* __restrict__ q, const bf16* __restrict__ k, const
         if (need_mask) {
           const int key = k0 + nt * 8 + (lane & 3) * 2 + (e & 1);
           const int row = row_a + ((e >> 1) << 3);
-          if (row >= T || key >= T || (CAUSAL && key > row)) pv = 0.f;
+          if (row >= T || key >= T || (CAUSAL && key > row) || key < seg_r[e >> 1]) pv = 0.f;
         }
         s[nt][e] = pv;
       }
     }
     float dp[8][4];
     zero_acc(dp);
-    gemm_a_bT(dp, doa, sV + st * 8192);  // dP = dO V^T
+    wg_a_bT(dp, sQdO + 8192, sV + st * 8192);  // dP = dO V^T
 #pragma unroll
     for (int nt = 0; nt < 8; ++nt) {
 #pragma unroll
@@ -639,7 +625,7 @@ attn_bwd_dq_kernel(const bf16* __restrict__ q, const bf16* __restrict__ k, const
     }
     uint32_t pa[4][4];
     acc_to_a(dp, pa);
-    gemm_p_b(dqacc, pa, sK + st * 8192);  // dQ += dS K
+    wg_p_b(dqacc, pa, sK + st * 8192);  // dQ += dS K
     __syncthreads();
   }
 #pragma unroll
@@ -654,10 +640,11 @@ attn_bwd_dq_kernel(const bf16* __restrict__ q, const bf16* __restrict__ k, const
   }
 }
 
-constexpr int FWD_SMEM = 128 * 128 + 4 * 8192;        // 48 KB
-constexpr int DKDV_SMEM = 6 * 8192 + 2 * 2 * 64 * 4;  // 49 KB + stats
-constexpr int DQ_SMEM = 6 * 8192;
-constexpr int FWD_SPLIT_SMEM = 2 * 128 * 128 + 8 * 8192;  // 96 KB
+// +1024: the tiles start at the first 1024-byte boundary of the dynamic shared memory
+constexpr int FWD_SMEM = 128 * 128 + 4 * 8192 + 1024;        // 48 KB
+constexpr int DKDV_SMEM = 6 * 8192 + 2 * 2 * 64 * 4 + 2 * 64 * 4 + 1024;  // 48 KB + stats + document starts
+constexpr int DQ_SMEM = 6 * 8192 + 1024;
+constexpr int FWD_SPLIT_SMEM = 2 * 128 * 128 + 8 * 8192 + 1024;  // 96 KB
 
 template <typename K>
 int set_smem(K kernel, int bytes) {
@@ -668,7 +655,8 @@ int set_smem(K kernel, int bytes) {
 }  // namespace
 
 int sk_attn_fwd_launch(const bf16* q, const bf16* k, const bf16* v, bf16* o, float* lse, int B, int T, int H, int KVH,
-                       int ld, int ldo, int causal, float scale, cudaStream_t s) {
+                       int ld, int ldo, int causal, float scale, cudaStream_t s, const int* seg_start) {
+  SK_REQUIRE(seg_start == nullptr || causal, "attention: document segments need the causal kernel");
   SK_REQUIRE(H % KVH == 0, "attention: H must be a multiple of KVH");
   SK_REQUIRE(ld % 8 == 0 && ldo % 8 == 0, "attention: leading dims must be multiples of 8");
   static bool init = false;
@@ -679,8 +667,8 @@ int sk_attn_fwd_launch(const bf16* q, const bf16* k, const bf16* v, bf16* o, flo
   }
   dim3 grid((T + 127) / 128, H, B);
   sk_prof_begin(1, s);
-  if (causal) attn_fwd_kernel<true><<<grid, 256, FWD_SMEM, s>>>(q, k, v, o, lse, T, ld, ldo, H, H / KVH, scale);
-  else attn_fwd_kernel<false><<<grid, 256, FWD_SMEM, s>>>(q, k, v, o, lse, T, ld, ldo, H, H / KVH, scale);
+  if (causal) attn_fwd_kernel<true><<<grid, 256, FWD_SMEM, s>>>(q, k, v, o, lse, T, ld, ldo, H, H / KVH, scale, seg_start);
+  else attn_fwd_kernel<false><<<grid, 256, FWD_SMEM, s>>>(q, k, v, o, lse, T, ld, ldo, H, H / KVH, scale, nullptr);
   sk_prof_end(s);
   SK_LAUNCH_CHECK();
   return 0;
@@ -689,7 +677,8 @@ int sk_attn_fwd_launch(const bf16* q, const bf16* k, const bf16* v, bf16* o, flo
 // dq/dk/dv are column slices of one gradient buffer with row pitch ldg (same layout as the fused qkv activation)
 int sk_attn_bwd_launch(const bf16* q, const bf16* k, const bf16* v, const bf16* o, const bf16* d_o, const float* lse,
                        float* delta, bf16* dq, bf16* dk, bf16* dv, int B, int T, int H, int KVH, int ld, int ldo,
-                       int ldg, int causal, float scale, cudaStream_t s) {
+                       int ldg, int causal, float scale, cudaStream_t s, const int* seg_start) {
+  SK_REQUIRE(seg_start == nullptr || causal, "attention: document segments need the causal kernels");
   SK_REQUIRE(H % KVH == 0, "attention: H must be a multiple of KVH");
   static bool init = false;
   if (!init) {
@@ -706,13 +695,15 @@ int sk_attn_bwd_launch(const bf16* q, const bf16* k, const bf16* v, const bf16* 
   const int group = H / KVH;
   dim3 g1((T + 63) / 64, KVH, B), g2((T + 63) / 64, H, B);
   if (causal) {
-    attn_bwd_dkdv_kernel<true><<<g1, 128, DKDV_SMEM, s>>>(q, k, v, d_o, lse, delta, dk, dv, T, ld, ldo, ldg, H, group, scale);
+    attn_bwd_dkdv_kernel<true><<<g1, 128, DKDV_SMEM, s>>>(q, k, v, d_o, lse, delta, dk, dv, T, ld, ldo, ldg, H, group, scale,
+                                                          seg_start);
     SK_LAUNCH_CHECK();
-    attn_bwd_dq_kernel<true><<<g2, 128, DQ_SMEM, s>>>(q, k, v, d_o, lse, delta, dq, T, ld, ldo, ldg, H, group, scale);
+    attn_bwd_dq_kernel<true><<<g2, 128, DQ_SMEM, s>>>(q, k, v, d_o, lse, delta, dq, T, ld, ldo, ldg, H, group, scale, seg_start);
   } else {
-    attn_bwd_dkdv_kernel<false><<<g1, 128, DKDV_SMEM, s>>>(q, k, v, d_o, lse, delta, dk, dv, T, ld, ldo, ldg, H, group, scale);
+    attn_bwd_dkdv_kernel<false><<<g1, 128, DKDV_SMEM, s>>>(q, k, v, d_o, lse, delta, dk, dv, T, ld, ldo, ldg, H, group, scale,
+                                                           nullptr);
     SK_LAUNCH_CHECK();
-    attn_bwd_dq_kernel<false><<<g2, 128, DQ_SMEM, s>>>(q, k, v, d_o, lse, delta, dq, T, ld, ldo, ldg, H, group, scale);
+    attn_bwd_dq_kernel<false><<<g2, 128, DQ_SMEM, s>>>(q, k, v, d_o, lse, delta, dq, T, ld, ldo, ldg, H, group, scale, nullptr);
   }
   sk_prof_end(s);
   SK_LAUNCH_CHECK();
@@ -744,4 +735,36 @@ int sk_attn_delta_launch(const bf16* o, const bf16* d_o, float* delta, int B, in
   sk_prof_end(s);
   SK_LAUNCH_CHECK();
   return 0;
+}
+
+// ---- fused-projection entry points of the LM step ---------------------------------------------------------------
+// q/k/v: column slices of one [B*T, ld] bf16 buffer starting at `qkv` (q heads first, then KVH k heads, then KVH v heads)
+int sk_attn_tc_fwd_launch(const bf16* qkv, bf16* o, float* lse, int B, int T, int H, int KVH, int ld, int ldo, int causal,
+                          float scale, cudaStream_t s, const int* seg_start) {
+  return sk_attn_fwd_launch(qkv, qkv + H * HD, qkv + (H + KVH) * HD, o, lse, B, T, H, KVH, ld, ldo, causal, scale, s,
+                            seg_start);
+}
+
+// dqkv: same column layout as qkv (row pitch ldg).  seg_end is accepted with seg_start (a packed batch); the masks are
+// fully determined by seg_start.  With rope tables, the inverse rotary embedding is applied to dq / dk afterwards
+// (rope_kernel's inverse mode: the backward of the forward RoPE, same bf16 rounding points).  `partial` is unused here.
+int sk_attn_tc_bwd_launch(const bf16* qkv, const bf16* o, const bf16* d_o, const float* lse, float* delta, float* partial,
+                          bf16* dqkv, int B, int T, int H, int KVH, int ld, int ldo, int ldg, int causal, float scale,
+                          cudaStream_t s, const int* seg_start, const int* seg_end, const bf16* rope_cos,
+                          const bf16* rope_sin, const int* pos_ids, int max_pos) {
+  (void)partial;
+  SK_REQUIRE((seg_start == nullptr) == (seg_end == nullptr), "attn_tc_bwd: seg_start and seg_end go together");
+  SK_REQUIRE((rope_cos == nullptr) == (rope_sin == nullptr) && (rope_cos == nullptr || max_pos > 0), "attn_tc_bwd: rope tables go together");
+  int rc = sk_attn_bwd_launch(qkv, qkv + H * HD, qkv + (H + KVH) * HD, o, d_o, lse, delta, dqkv, dqkv + H * HD,
+                              dqkv + (H + KVH) * HD, B, T, H, KVH, ld, ldo, ldg, causal, scale, s, seg_start);
+  if (rc) return rc;
+  if (rope_cos) return sk_rope_launch(dqkv, rope_cos, rope_sin, pos_ids, B * T, T, ldg, H + KVH, HD, 1, max_pos, s);
+  return 0;
+}
+
+// qkv_hi / qkv_lo: [B*T, ld] with H q-heads, H k-heads, H v-heads (64 columns each); o_hi / o_lo: [B*T, ldo]
+int sk_attn_tc_fwd_split_launch(const bf16* qkv_hi, const bf16* qkv_lo, bf16* o_hi, bf16* o_lo, int B, int T, int H, int ld,
+                                int ldo, float scale, cudaStream_t s) {
+  return sk_attn_fwd_split_launch(qkv_hi, qkv_lo, qkv_hi + H * HD, qkv_lo + H * HD, qkv_hi + 2 * H * HD, qkv_lo + 2 * H * HD,
+                                  o_hi, o_lo, B, T, H, ld, ldo, scale, s);
 }

@@ -1,6 +1,6 @@
-// Common device helpers for the slamkit_b200 sm_100a kernels: PTX wrappers for
-// mbarrier / TMA / tcgen05 / TMEM, warp reductions, 128-bit vector I/O.
-// Everything here is sm_100a-only by design (no multi-arch dispatch).
+// Common device helpers for the slamkit_b200 sm_90a kernels: PTX wrappers for
+// mbarrier / TMA / wgmma, warp reductions, 128-bit vector I/O.
+// Everything here is sm_90a-only by design (no multi-arch dispatch).
 #pragma once
 #include <cuda_runtime.h>
 #include <cuda_bf16.h>
@@ -44,7 +44,7 @@ int sk_num_sms();
 // ----------------------------------------------------------------------------------------------
 // Programmatic dependent launch.  The LM step is ~760 back-to-back launches on one stream; with the
 // programmatic-stream-serialization attribute a kernel's CTAs may become resident -- and run their prologue (barrier
-// init, TMEM allocation, tensor-map prefetch, index math) -- while the previous kernel's last wave drains.  Every
+// init, tensor-map prefetch, index math) -- while the previous kernel's last wave drains.  Every
 // kernel launched this way calls griddep_wait() before its first global-memory access (the wait returns once the
 // previous grid has completed and its writes are visible), so data hazards are exactly those of plain stream order.
 // SK_PDL=0 in the environment turns the attribute off.
@@ -73,7 +73,7 @@ template <typename... KArgs, typename... Args>
 inline cudaError_t sk_launch_pdl(void (*kernel)(KArgs...), dim3 grid, dim3 block, size_t smem, cudaStream_t s, Args... args) {
   return sk_launch_pdl_if(true, kernel, grid, block, smem, s, args...);
 }
-// bench-only device timing hooks (api.cu): category 0 = tcgen05 GEMM, 1 = attention, 2 = optimiser, 3 = other
+// bench-only device timing hooks (api.cu): category 0 = GEMM, 1 = attention, 2 = optimiser, 3 = other
 void sk_prof_begin(int cat, cudaStream_t s);
 void sk_prof_end(cudaStream_t s);
 
@@ -169,37 +169,17 @@ SK_DEVINL float sigmoid_f(float x) {
 SK_DEVINL float silu_f(float x) { return x * sigmoid_f(x); }
 
 // ----------------------------------------------------------------------------------------------
-// Packed fp32 pairs (sm_100a FFMA2 / FMUL2 / FADD2): two fp32 lanes per instruction issue slot.  Same fp32 FLOP rate as
-// the scalar forms (profiles/r01_micro_ffma_vs_ffma2.txt); what they buy is issue bandwidth in element-wise code.
+// fp32 pairs: element-wise code written on two lanes at a time.  sm_90 has no packed fp32 instructions, so each pair
+// operation is two scalar ones with the same per-lane rounding (fma.rn / mul.rn / add.rn / sub.rn).
 // ----------------------------------------------------------------------------------------------
-typedef unsigned long long f32x2;
-SK_DEVINL f32x2 pk2(float a, float b) {
-  f32x2 r;
-  asm("mov.b64 %0, {%1, %2};" : "=l"(r) : "f"(a), "f"(b));
-  return r;
-}
-SK_DEVINL void upk2(f32x2 v, float& a, float& b) { asm("mov.b64 {%0, %1}, %2;" : "=f"(a), "=f"(b) : "l"(v)); }
-SK_DEVINL f32x2 dup2(float c) { return pk2(c, c); }
-SK_DEVINL f32x2 fma2(f32x2 a, f32x2 b, f32x2 c) {
-  f32x2 d;
-  asm("fma.rn.f32x2 %0, %1, %2, %3;" : "=l"(d) : "l"(a), "l"(b), "l"(c));
-  return d;
-}
-SK_DEVINL f32x2 mul2(f32x2 a, f32x2 b) {
-  f32x2 d;
-  asm("mul.rn.f32x2 %0, %1, %2;" : "=l"(d) : "l"(a), "l"(b));
-  return d;
-}
-SK_DEVINL f32x2 add2(f32x2 a, f32x2 b) {
-  f32x2 d;
-  asm("add.rn.f32x2 %0, %1, %2;" : "=l"(d) : "l"(a), "l"(b));
-  return d;
-}
-SK_DEVINL f32x2 sub2(f32x2 a, f32x2 b) {
-  f32x2 d;
-  asm("sub.rn.f32x2 %0, %1, %2;" : "=l"(d) : "l"(a), "l"(b));
-  return d;
-}
+typedef float2 f32x2;
+SK_DEVINL f32x2 pk2(float a, float b) { return make_float2(a, b); }
+SK_DEVINL void upk2(f32x2 v, float& a, float& b) { a = v.x; b = v.y; }
+SK_DEVINL f32x2 dup2(float c) { return make_float2(c, c); }
+SK_DEVINL f32x2 fma2(f32x2 a, f32x2 b, f32x2 c) { return make_float2(__fmaf_rn(a.x, b.x, c.x), __fmaf_rn(a.y, b.y, c.y)); }
+SK_DEVINL f32x2 mul2(f32x2 a, f32x2 b) { return make_float2(__fmul_rn(a.x, b.x), __fmul_rn(a.y, b.y)); }
+SK_DEVINL f32x2 add2(f32x2 a, f32x2 b) { return make_float2(__fadd_rn(a.x, b.x), __fadd_rn(a.y, b.y)); }
+SK_DEVINL f32x2 sub2(f32x2 a, f32x2 b) { return make_float2(__fsub_rn(a.x, b.x), __fsub_rn(a.y, b.y)); }
 // Single-thread role waits (TMA producer / MMA issuer): back off with nanosleep so the spinning lane does not steal
 // issue slots from the compute warps sharing its scheduler.  Still bounded (trap after ~4 s).
 SK_DEVINL void mbar_wait_sleep(uint32_t bar, uint32_t parity) {
@@ -228,6 +208,17 @@ SK_DEVINL void mbar_wait(uint32_t bar, uint32_t parity) {
         __trap();
       }
     }
+  }
+}
+
+// Same bound without the printf: a function call anywhere in a kernel that issues wgmma makes ptxas serialize its wgmma
+// pipeline, so wgmma kernels use this form.
+SK_DEVINL void mbar_wait_nocall(uint32_t bar, uint32_t parity) {
+  if (mbar_try_wait(bar, parity)) return;
+  uint64_t t0 = globaltimer_ns();
+  uint32_t spins = 0;
+  while (!mbar_try_wait(bar, parity)) {
+    if ((++spins & 0x3fffu) == 0 && globaltimer_ns() - t0 > 4000000000ull) __trap();
   }
 }
 
@@ -265,74 +256,61 @@ SK_DEVINL void tma_store_wait() {
 }
 
 // ----------------------------------------------------------------------------------------------
-// tcgen05 / TMEM
+// wgmma (sm_90a warpgroup MMA): D[registers of 4 warps] += A[smem desc] * B[smem desc], bf16 in, fp32 accumulate.
+// The accumulator of m64nN is N/2 floats per thread: warp w of the warpgroup holds rows 16w + lane/4 (d[4j], d[4j+1])
+// and 16w + lane/4 + 8 (d[4j+2], d[4j+3]), columns 8j + 2(lane%4) + {0, 1}.
 // ----------------------------------------------------------------------------------------------
-SK_DEVINL void tmem_alloc(uint32_t smem_dst, uint32_t ncols) {
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_dst), "r"(ncols)
-               : "memory");
+SK_DEVINL void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+SK_DEVINL void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N>
+SK_DEVINL void wgmma_wait() {
+  asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory");
 }
-SK_DEVINL void tmem_relinquish() {
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-SK_DEVINL void tmem_dealloc(uint32_t taddr, uint32_t ncols) {
-  asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-}
-SK_DEVINL void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-SK_DEVINL void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-// tcgen05.commit: arrive on an mbarrier when all previously issued MMAs of this thread retire.
-SK_DEVINL void tc_commit(uint32_t bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(bar)
-               : "memory");
-}
-// D[tmem] (+)= A[smem desc] * B[smem desc], kind::f16 (bf16/fp16 inputs, fp32 accumulate)
-SK_DEVINL void tc_mma_f16(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}\n"
-      ::"r"(tmem_d), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-SK_DEVINL void tc_mma_tf32(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::tf32 [%0], %1, %2, %3, p;\n\t}\n"
-      ::"r"(tmem_d), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// 32 lanes x 32 columns of fp32: thread i of the warp receives lane (quadrant*32+i), columns [c, c+32)
-SK_DEVINL void tmem_ld_32x32(uint32_t taddr, uint32_t (&r)[32]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,"
-      "%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31}, [%32];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]),
-        "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]),
-        "=r"(r[16]), "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]),
-        "=r"(r[24]), "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-      : "r"(taddr)
-      : "memory");
-}
-SK_DEVINL void tmem_ld_wait() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
+// named barrier over the first `threads` threads of the CTA (id 0 is __syncthreads)
+SK_DEVINL void named_bar_sync(int id, int threads) { asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(threads) : "memory"); }
 
-// UMMA shared-memory matrix descriptor (cute::UMMA::SmemDescriptor layout, sm_100):
+// GMMA shared-memory matrix descriptor (sm_90):
 //   [0,14)  start address >> 4      [16,30) leading byte offset >> 4   [32,46) stride byte offset >> 4
-//   [46,48) version = 1             [49,52) base offset = 0            [61,64) layout type (2 = SWIZZLE_128B)
-SK_DEVINL uint64_t umma_desc_sw128(uint32_t smem_addr, uint32_t lbo_bytes, uint32_t sbo_bytes) {
+//   [49,52) base offset = 0         [62,64) layout type (1 = SWIZZLE_128B)
+// Canonical SW128 layouts (bf16, T = 64 elements = 128 bytes):
+//   K-major : rows of 128 B, 8-row groups SBO = 1024 B apart (LBO unused)
+//   MN-major: 64-element MN atoms LBO apart; 8-k-row groups SBO = 1024 B apart
+SK_DEVINL uint64_t gmma_desc_sw128(uint32_t smem_addr, uint32_t lbo_bytes, uint32_t sbo_bytes) {
   uint64_t d = 0;
   d |= (uint64_t)((smem_addr & 0x3ffffu) >> 4);
   d |= (uint64_t)((lbo_bytes >> 4) & 0x3fffu) << 16;
   d |= (uint64_t)((sbo_bytes >> 4) & 0x3fffu) << 32;
-  d |= (uint64_t)1 << 46;
-  d |= (uint64_t)2 << 61;
+  d |= (uint64_t)1 << 62;
   return d;
 }
-// UMMA instruction descriptor for kind::f16 / kind::tf32 (cute::UMMA::InstrDescriptor):
-//   [4,6) D format (1 = f32)  [7,10) A format  [10,13) B format (0 f16, 1 bf16, 2 tf32)
-//   [15] A major (0 K, 1 MN)  [16] B major     [17,23) N>>3           [24,29) M>>4
-SK_DEVINL constexpr uint32_t umma_idesc(uint32_t ab_fmt, uint32_t a_mn_major, uint32_t b_mn_major, uint32_t M,
-                                        uint32_t N) {
-  return (1u << 4) | (ab_fmt << 7) | (ab_fmt << 10) | (a_mn_major << 15) | (b_mn_major << 16) | ((N >> 3) << 17) |
-         ((M >> 4) << 24);
+// m64nNk16, bf16 x bf16 -> fp32, D += A * B.  TA / TB: 0 = K-major operand, 1 = MN-major (transposed) operand.
+template <int TA, int TB>
+SK_DEVINL void wgmma_m64n64(float (&d)[32], uint64_t da, uint64_t db) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\tsetp.eq.u32 p, 1, 1;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n64k16.f32.bf16.bf16 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31}, %32, %33, p, 1, 1, %34, %35;\n\t}\n"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+      : "l"(da), "l"(db), "n"(TA), "n"(TB));
+}
+template <int TA, int TB>
+SK_DEVINL void wgmma_m64n128(float (&d)[64], uint64_t da, uint64_t db) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\tsetp.eq.u32 p, 1, 1;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n128k16.f32.bf16.bf16 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31,%32,%33,%34,%35,%36,%37,%38,%39,%40,%41,%42,%43,%44,%45,%46,%47,%48,%49,%50,%51,%52,%53,%54,%55,%56,%57,%58,%59,%60,%61,%62,%63}, %64, %65, p, 1, 1, %66, %67;\n\t}\n"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+      : "l"(da), "l"(db), "n"(TA), "n"(TB));
+}
+template <int TA, int TB>
+SK_DEVINL void wgmma_m64n256(float (&d)[128], uint64_t da, uint64_t db) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\tsetp.eq.u32 p, 1, 1;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n256k16.f32.bf16.bf16 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31,%32,%33,%34,%35,%36,%37,%38,%39,%40,%41,%42,%43,%44,%45,%46,%47,%48,%49,%50,%51,%52,%53,%54,%55,%56,%57,%58,%59,%60,%61,%62,%63,%64,%65,%66,%67,%68,%69,%70,%71,%72,%73,%74,%75,%76,%77,%78,%79,%80,%81,%82,%83,%84,%85,%86,%87,%88,%89,%90,%91,%92,%93,%94,%95,%96,%97,%98,%99,%100,%101,%102,%103,%104,%105,%106,%107,%108,%109,%110,%111,%112,%113,%114,%115,%116,%117,%118,%119,%120,%121,%122,%123,%124,%125,%126,%127}, %128, %129, p, 1, 1, %130, %131;\n\t}\n"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63]), "+f"(d[64]), "+f"(d[65]), "+f"(d[66]), "+f"(d[67]), "+f"(d[68]), "+f"(d[69]), "+f"(d[70]), "+f"(d[71]), "+f"(d[72]), "+f"(d[73]), "+f"(d[74]), "+f"(d[75]), "+f"(d[76]), "+f"(d[77]), "+f"(d[78]), "+f"(d[79]), "+f"(d[80]), "+f"(d[81]), "+f"(d[82]), "+f"(d[83]), "+f"(d[84]), "+f"(d[85]), "+f"(d[86]), "+f"(d[87]), "+f"(d[88]), "+f"(d[89]), "+f"(d[90]), "+f"(d[91]), "+f"(d[92]), "+f"(d[93]), "+f"(d[94]), "+f"(d[95]), "+f"(d[96]), "+f"(d[97]), "+f"(d[98]), "+f"(d[99]), "+f"(d[100]), "+f"(d[101]), "+f"(d[102]), "+f"(d[103]), "+f"(d[104]), "+f"(d[105]), "+f"(d[106]), "+f"(d[107]), "+f"(d[108]), "+f"(d[109]), "+f"(d[110]), "+f"(d[111]), "+f"(d[112]), "+f"(d[113]), "+f"(d[114]), "+f"(d[115]), "+f"(d[116]), "+f"(d[117]), "+f"(d[118]), "+f"(d[119]), "+f"(d[120]), "+f"(d[121]), "+f"(d[122]), "+f"(d[123]), "+f"(d[124]), "+f"(d[125]), "+f"(d[126]), "+f"(d[127])
+      : "l"(da), "l"(db), "n"(TA), "n"(TB));
+}
+template <int N, int TA, int TB>
+SK_DEVINL void wgmma_bf16(float (&d)[N / 2], uint64_t da, uint64_t db) {
+  if constexpr (N == 256) wgmma_m64n256<TA, TB>(d, da, db);
+  else if constexpr (N == 128) wgmma_m64n128<TA, TB>(d, da, db);
+  else wgmma_m64n64<TA, TB>(d, da, db);
 }

@@ -1,21 +1,20 @@
-// tcgen05 GEMM for sm_100a:  C[M,N] = A[M,K] * B[N,K]^T (+bias[N]) (+residual[M,N]),  bf16 in, fp32 accumulate
-// in TMEM, bf16 (or fp32) out.
+// wgmma GEMM for sm_90a:  C[M,N] = A[M,K] * B[N,K]^T (+bias[N]) (+residual[M,N]),  bf16 in, fp32 accumulate,
+// bf16 (or fp32) out.
 //
-// One persistent CTA per SM, 10 warps, warp-specialised:
-//   warp 0      TMA producer   (cp.async.bulk.tensor -> 128B-swizzled smem ring, mbarrier complete_tx)
-//   warp 1      MMA issuer     (one lane issues tcgen05.mma.cta_group::1.kind::f16, 128 x BN x 16 per instruction;
-//                               tcgen05.commit frees smem slots and publishes accumulators)
-//   warps 2..9  epilogue       (tcgen05.ld 32x32b.x32 from TMEM -> bias / residual / fused element-wise op -> swizzled
-//                               smem -> TMA store).  Two warps per TMEM lane quadrant, each owning one half of the
-//                               tile's columns: with K = 896 (14 k-blocks per tile) the mainloop of a tile lasts ~6 us,
-//                               and a one-warp-per-quadrant epilogue (a single warp per scheduler, latency-bound) took
-//                               longer than that as soon as it did more than convert-and-store.
-// Accumulators are double-buffered in TMEM (2 x BN columns) so the epilogue of tile i overlaps the MMAs of tile i+1.
+// One persistent CTA per SM, 9 warps:
+//   warps 0..7  two consumer warpgroups: warpgroup g issues wgmma.mma_async m64 x BN x 16 on rows [64g, 64g + 64) of
+//               the 128-row tile, accumulating in registers; each warp releases a ring slot once the MMAs that read
+//               it have retired.  After a tile's K loop the fp32 accumulator is parked in the (then idle) stage ring
+//               as a [128][BN] row-major tile, and the epilogue warps read it back one ROW per thread (32 columns at a
+//               time): bias / residual / fused element-wise op -> swizzled smem -> TMA store.  EW = 4 epilogue
+//               warps (one per 32-row quadrant) or EW = 8 (two per quadrant, each owning half of the columns).
+//   warp 8      TMA producer (cp.async.bulk.tensor -> 128B-swizzled smem ring, mbarrier complete_tx); it starts the
+//               next tile's loads once the parked accumulator has been consumed.
 //
 // Operand majors.  "K-major" = the contraction index is contiguous in memory (A row-major [M,K], B row-major [N,K]).
 // "MN-major" = the M (or N) index is contiguous (A stored as [K,M], B stored as [K,N]).  MN-major operands let the
 // backward GEMMs (dgrad: dX = dY * W ; wgrad: dW = dY^T * X) read activations and weights in place, with no
-// transposed copies in HBM.  Layouts follow cute::UMMA canonical SW128 forms:
+// transposed copies in HBM (wgmma's transpose bits).  Layouts are the canonical GMMA SW128 forms:
 //    K-major : ((8,m),(T,2)) : ((8T,SBO),(1,T))          rows of 128 B, 8-row groups SBO=1024 B apart
 //    MN-major: ((T,8,m),(8,k)) : ((1,T,LBO),(8T,SBO))    64-element MN atoms, LBO apart; 8-k-row groups SBO apart
 #include "common.cuh"
@@ -30,7 +29,8 @@ namespace {
 
 constexpr int BM = 128;
 constexpr int BK = 64;
-constexpr int UMMA_K = 16;
+constexpr int MMA_K = 16;
+constexpr int GEMM_THREADS = 288;   // 2 consumer warpgroups + 1 producer warp
 
 
 struct GemmParams {
@@ -78,18 +78,49 @@ struct GemmParams {
 
 template <int BN, int EW = 4>
 struct GemmCfg {
-  static constexpr int THREADS = 64 + 32 * EW;              // TMA warp, MMA warp, EW epilogue warps
   static constexpr int A_BYTES = BM * BK * 2;
   static constexpr int B_ATOMS = (BN + 63) / 64;            // MN-major B is fetched in 64-column atoms
   static constexpr int B_BYTES = B_ATOMS * 64 * BK * 2;
   static constexpr int STAGE_BYTES = A_BYTES + B_BYTES;
   static constexpr int STAGES = (BN > 128) ? 4 : (BN > 64 ? 6 : 8);
-  static constexpr int ACC_STRIDE = (BN <= 32) ? 32 : (BN <= 64 ? 64 : (BN <= 128 ? 128 : 256));
-  static constexpr int TMEM_COLS = 2 * ACC_STRIDE;
   static constexpr int STAGING_BYTES = 4 * 2 * 4096;  // (32 rows x 128 B) TMA-store buffers: 2 per warp (EW = 4) or 1 (EW = 8)
   static constexpr int BAR_BYTES = 256;
   static constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + STAGING_BYTES + BAR_BYTES + 1024;  // +1024: manual alignment
+  static_assert(STAGES * STAGE_BYTES >= BM * BN * 4, "the parked fp32 accumulator must fit in the stage ring");
+  static_assert(SMEM_BYTES <= 227 * 1024, "sm_90 allows 227 KB of shared memory per block");
 };
+
+// Parked accumulator: fp32 [BM][BN] row-major at `base`, 16-byte chunks XOR-swizzled by (row & 7) so that both the
+// fragment-order stores and the row-per-thread loads spread over all banks.
+template <int BN>
+SK_DEVINL uint32_t acc_chunk_addr(uint32_t base, int row, int chunk) {
+  return base + (uint32_t)row * (BN * 4) + (uint32_t)((chunk ^ (row & 7)) << 4);
+}
+// one warpgroup's m64 x BN wgmma accumulator (rows [64 wg, 64 wg + 64)) -> parked tile
+template <int BN>
+SK_DEVINL void acc_park(uint32_t base, const float (&d)[BN / 2], int wg, int warp_in_wg, int lane) {
+  const int r0 = 64 * wg + 16 * warp_in_wg + (lane >> 2);
+#pragma unroll
+  for (int j = 0; j < BN / 8; ++j) {
+    const int chunk = 2 * j + ((lane & 3) >> 1);
+    const uint32_t off = (uint32_t)(lane & 1) * 8u;
+    asm volatile("st.shared.v2.f32 [%0], {%1, %2};" ::"r"(acc_chunk_addr<BN>(base, r0, chunk) + off), "f"(d[4 * j]),
+                 "f"(d[4 * j + 1]) : "memory");
+    asm volatile("st.shared.v2.f32 [%0], {%1, %2};" ::"r"(acc_chunk_addr<BN>(base, r0 + 8, chunk) + off), "f"(d[4 * j + 2]),
+                 "f"(d[4 * j + 3]) : "memory");
+  }
+}
+// row (ta >> 16) + lane, columns [ta & 0xffff, +32) of the parked tile -> r[32]
+template <int BN>
+SK_DEVINL void acc_ld_32x32(uint32_t base, uint32_t ta, uint32_t (&r)[32]) {
+  const int row = (int)(ta >> 16) + (int)(threadIdx.x & 31);
+  const int c0 = (int)(ta & 0xffffu) >> 2;
+#pragma unroll
+  for (int i = 0; i < 8; ++i)
+    asm volatile("ld.shared.v4.b32 {%0, %1, %2, %3}, [%4];"
+                 : "=r"(r[4 * i]), "=r"(r[4 * i + 1]), "=r"(r[4 * i + 2]), "=r"(r[4 * i + 3])
+                 : "r"(acc_chunk_addr<BN>(base, row, c0 + i)) : "memory");
+}
 
 // GELU(erf) for the fused epilogue (HuBERT conv layers and FFN): branch-free Abramowitz-Stegun 7.1.26 erf, folded as
 //   gelu(y) = relu(y) - |y| * (P(t)/2) * exp(-y^2/2),  t = 1/(1 + p|y|/sqrt2)
@@ -289,15 +320,13 @@ SK_DEVINL void sk_fixup_add(uint32_t (&r)[32], const float* ws, int chunk, int r
 }
 
 template <int BN, bool A_MN, bool B_MN, bool SK, int EW>
-// register caps: two (EW = 4) or three (EW = 8) warps of this kernel share an SM sub-partition's 16 K registers; 240 /
-// 160 leave the 1024 that one warp of the peer all-reduce kernel needs (p2p_comm.cu), so it can run alongside
-__global__ void __launch_bounds__(64 + 32 * EW, 1) __maxnreg__(EW == 8 ? 160 : 240)
-gemm_tcgen05_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
-                    const __grid_constant__ CUtensorMap tmA_lo, const __grid_constant__ CUtensorMap tmB_lo,
-                    const __grid_constant__ CUtensorMap tmC, const __grid_constant__ CUtensorMap tmAux, GemmParams p) {
+__global__ void __launch_bounds__(GEMM_THREADS, 1)
+gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
+                  const __grid_constant__ CUtensorMap tmA_lo, const __grid_constant__ CUtensorMap tmB_lo,
+                  const __grid_constant__ CUtensorMap tmC, const __grid_constant__ CUtensorMap tmAux, GemmParams p) {
   using Cfg = GemmCfg<BN, EW>;
   static_assert(EW == 4 || (EW == 8 && BN == 256 && !SK), "8 epilogue warps: plain 256-wide tiles only");
-  constexpr int CS = EW / 4;          // column split: epilogue warps per TMEM lane quadrant
+  constexpr int CS = EW / 4;          // column split: epilogue warps per 32-row quadrant
   griddep_launch();                 // the next kernel on the stream may start its own prologue now
   extern __shared__ uint8_t smem_raw[];
   const uint32_t smem_base = (smem_u32(smem_raw) + 1023u) & ~1023u;
@@ -305,10 +334,7 @@ gemm_tcgen05_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_consta
   const uint32_t bar_base = staging_base + Cfg::STAGING_BYTES;
   auto full_bar = [&](int s) { return bar_base + 8u * s; };
   auto empty_bar = [&](int s) { return bar_base + 8u * (Cfg::STAGES + s); };
-  auto tfull_bar = [&](int s) { return bar_base + 8u * (2 * Cfg::STAGES + s); };
-  auto tempty_bar = [&](int s) { return bar_base + 8u * (2 * Cfg::STAGES + 2 + s); };
-  const uint32_t tmem_slot = bar_base + 8u * (2 * Cfg::STAGES + 4);
-  uint32_t* tmem_slot_ptr = reinterpret_cast<uint32_t*>(smem_raw + (tmem_slot - smem_u32(smem_raw)));
+  const uint32_t acc_free = bar_base + 8u * (2 * Cfg::STAGES);
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
@@ -319,30 +345,20 @@ gemm_tcgen05_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_consta
   // bytes one stage receives: A tile + B tile (a K-major B box is exactly BN rows; MN-major B comes in 64-column atoms)
   constexpr uint32_t STAGE_TX = Cfg::A_BYTES + (B_MN ? Cfg::B_ATOMS * 64 * BK * 2 : BN * BK * 2);
 
-  if (warp == 0 && lane == 0) {
+  if (threadIdx.x == 0) {
     tma_prefetch_desc(&tmA);
     tma_prefetch_desc(&tmB);
     for (int s = 0; s < Cfg::STAGES; ++s) {
       mbar_init(full_bar(s), 1);
-      mbar_init(empty_bar(s), 1);
+      mbar_init(empty_bar(s), 8);   // one arrival per consumer warp
     }
-    for (int s = 0; s < 2; ++s) {
-      mbar_init(tfull_bar(s), 1);
-      mbar_init(tempty_bar(s), EW);
-    }
+    mbar_init(acc_free, 1);
     fence_mbar_init();
   }
-  if (warp == 1) {
-    tmem_alloc(tmem_slot, Cfg::TMEM_COLS);
-    tmem_relinquish();
-  }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot_ptr;
   griddep_wait();                   // prologue done; inputs of this GEMM are complete and visible from here on
 
-  if (warp == 0) {
+  if (warp == 8) {
     // ===== TMA producer =====
     // Split-bf16 mode (passes == 3) pairs two ring slots per k-block: [A_hi | B_hi] [A_lo | B_lo] are fetched once and
     // feed all three products (hi*hi, hi*lo, lo*hi) -- 4 tile loads per k-block instead of the 6 that three separate
@@ -353,15 +369,22 @@ gemm_tcgen05_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_consta
       const uint32_t stage_bytes = split ? 2u * Cfg::STAGE_BYTES : (uint32_t)Cfg::STAGE_BYTES;
       int stage = 0;
       uint32_t phase = 0;
+      uint32_t acc_phase = 0;
+      bool first = true;
       WorkIter<SK> w(p, num_kb_total, kb_per_split, total_items);
       while (w.next()) {
+        if (!first) {   // the previous tile's accumulator is parked in the ring until its epilogue is done
+          mbar_wait_nocall(acc_free, acc_phase);
+          acc_phase ^= 1u;
+        }
+        first = false;
         const int bidx = w.tile / tiles_per_batch;
         const int r = w.tile - bidx * tiles_per_batch;
         const int m0 = (r / p.tiles_n) * BM;
         const int n_blk = r % p.tiles_n;
         const int n0 = n_blk * BN;
         for (int kb = w.kb_begin; kb < w.kb_end; ++kb) {
-          mbar_wait(empty_bar(stage), phase ^ 1u);
+          mbar_wait_nocall(empty_bar(stage), phase ^ 1u);
           const uint32_t fb = full_bar(stage);
           mbar_arrive_expect_tx(fb, split ? 2u * STAGE_TX : STAGE_TX);
           for (int part = 0; part < (split ? 2 : 1); ++part) {
@@ -391,120 +414,118 @@ gemm_tcgen05_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_consta
         }
       }
     }
-  } else if (warp == 1) {
-    // ===== MMA issuer =====
-    if (lane == 0) {
-      constexpr uint32_t idesc = umma_idesc(1u, A_MN ? 1u : 0u, B_MN ? 1u : 0u, BM, BN);
-      const bool split = p.passes == 3;
-      const int n_stage = split ? Cfg::STAGES / 2 : Cfg::STAGES;
-      const uint32_t stage_bytes = split ? 2u * Cfg::STAGE_BYTES : (uint32_t)Cfg::STAGE_BYTES;
-      int stage = 0;
-      uint32_t phase = 0;
-      int as = 0;
-      uint32_t aphase = 0;
-      WorkIter<SK> w(p, num_kb_total, kb_per_split, total_items);
-      while (w.next()) {
-        mbar_wait(tempty_bar(as), aphase ^ 1u);
-        tc_fence_after();
-        const uint32_t tmem_d = tmem_base + as * Cfg::ACC_STRIDE;
+  } else {
+    // ===== consumer warpgroups (MMA) and epilogue warps 0..EW-1 =====
+    const int wg = warp >> 2;
+    const int q = warp & 3;            // 32-row quadrant of the tile this warp's epilogue owns
+    const int chalf = warp >> 2;       // column half (EW == 8)
+    const bool epi_warp = warp < EW;
+    auto acc_ld = [&](uint32_t ta, uint32_t (&r)[32]) { acc_ld_32x32<BN>(smem_base, ta, r); };
+    const bool split = p.passes == 3;
+    const int n_stage = split ? Cfg::STAGES / 2 : Cfg::STAGES;
+    const uint32_t stage_bytes = split ? 2u * Cfg::STAGE_BYTES : (uint32_t)Cfg::STAGE_BYTES;
+    int stage = 0;
+    uint32_t phase = 0;
+    uint32_t store_cnt = 0;
+    // the parked accumulator has been read: the ring may be refilled (async-proxy writes after generic accesses)
+    auto release_acc = [&] {
+      fence_proxy_async();
+      named_bar_sync(1, 256);
+      if (threadIdx.x == 0) mbar_arrive(acc_free);
+    };
+    WorkIter<SK> w(p, num_kb_total, kb_per_split, total_items);
+    while (w.next()) {
+      {
+        // ---- K loop: this warpgroup's 64 rows x BN columns accumulate in registers ----
+        float acc[BN / 2];
+#pragma unroll
+        for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
         const int k_iters = max(0, w.kb_end - w.kb_begin);
+        int prev = -1;
         for (int kb = 0; kb < k_iters; ++kb) {
-          mbar_wait(full_bar(stage), phase);
-          tc_fence_after();
+          mbar_wait_nocall(full_bar(stage), phase);
+          wgmma_fence();
           const uint32_t s_hi = smem_base + stage * stage_bytes;
           // products per k-block: hi*hi, then (split mode) hi*lo and lo*hi
           for (int g = 0; g < (split ? 3 : 1); ++g) {
-            const uint32_t sA = s_hi + (g == 2 ? Cfg::STAGE_BYTES : 0);
+            // this warpgroup's rows: 64 K-major rows of 128 B, or the g-th 64-row MN atom -- 8 KB in both layouts
+            const uint32_t sA = s_hi + (g == 2 ? Cfg::STAGE_BYTES : 0) + (uint32_t)wg * 8192u;
             const uint32_t sB = s_hi + Cfg::A_BYTES + (g == 1 ? Cfg::STAGE_BYTES : 0);
 #pragma unroll
-            for (int k = 0; k < BK / UMMA_K; ++k) {
-              const uint64_t adesc = A_MN ? umma_desc_sw128(sA + k * (UMMA_K * 128), BK * 128, 1024)
-                                          : umma_desc_sw128(sA + k * (UMMA_K * 2), 16, 1024);
-              const uint64_t bdesc = B_MN ? umma_desc_sw128(sB + k * (UMMA_K * 128), BK * 128, 1024)
-                                          : umma_desc_sw128(sB + k * (UMMA_K * 2), 16, 1024);
-              tc_mma_f16(tmem_d, adesc, bdesc, idesc, (kb | g | k) != 0 ? 1u : 0u);
+            for (int k = 0; k < BK / MMA_K; ++k) {
+              const uint64_t adesc = A_MN ? gmma_desc_sw128(sA + k * (MMA_K * 128), BK * 128, 1024)
+                                          : gmma_desc_sw128(sA + k * (MMA_K * 2), 16, 1024);
+              const uint64_t bdesc = B_MN ? gmma_desc_sw128(sB + k * (MMA_K * 128), BK * 128, 1024)
+                                          : gmma_desc_sw128(sB + k * (MMA_K * 2), 16, 1024);
+              wgmma_bf16<BN, A_MN ? 1 : 0, B_MN ? 1 : 0>(acc, adesc, bdesc);
             }
           }
-          tc_commit(empty_bar(stage));
+          wgmma_commit();
+          wgmma_wait<1>();            // the previous k-block's MMAs have retired: its slot can be refilled
+          if (prev >= 0 && lane == 0) mbar_arrive(empty_bar(prev));
+          prev = stage;
           if (++stage == n_stage) { stage = 0; phase ^= 1u; }
         }
-        tc_commit(tfull_bar(as));
-        as ^= 1;
-        if (as == 0) aphase ^= 1u;
+        wgmma_wait<0>();
+        if (prev >= 0 && lane == 0) mbar_arrive(empty_bar(prev));
+        // every k-block of this tile has been consumed and the producer waits for acc_free: the ring is idle
+        named_bar_sync(1, 256);
+        acc_park<BN>(smem_base, acc, wg, warp & 3, lane);
+        named_bar_sync(1, 256);
       }
-    }
-  } else {
-    // ===== epilogue (warps 2..9); TMEM lane quadrant = warp % 4, column half = (warp - 2) / 4 =====
-    const int q = warp & 3;
-    const int chalf = (warp - 2) >> 2;   // 0 when EW == 4
-    uint32_t store_cnt = 0;
-    int as = 0;
-    uint32_t aphase = 0;
-    WorkIter<SK> w(p, num_kb_total, kb_per_split, total_items);
-    if (!SK && p.tma_store && p.epi == 2) {
-      // ===== SwiGLU backward epilogue: acc = d_act; d_gate = bf16(bf16(d_act*u) * silu'(g)), d_up = bf16(d_act * bf16(silu(g)))
-      // The accumulator arrives one ROW per thread, but gu / d_gu must move with coalesced accesses (a thread walking
-      // its own row issues 32 scattered 16-byte requests per instruction: measured slower than the unfused kernels).
-      // So bf16(d_act) goes through the warp's swizzled staging buffer and is re-read in a (4 rows x 8 pieces of
-      // 16 bytes) arrangement -- lane = (row % 4, piece) -- in which every global load / store instruction covers
-      // four full 128-byte row segments.  The gu registers are refilled in place for the NEXT chunk (of this tile or of
-      // the CTA's next tile) as soon as they have been consumed, so a whole chunk of math -- and, across tiles, the wait
-      // for the accumulator -- hides the DRAM latency.  Products of two bf16 values rounded to bf16 are single packed
-      // HMUL2.BF16 (exact product, one rounding: the same value as rounding the fp32 product).
-      const int lpiece = lane & 7, lrsub = lane >> 3;
-      const uint32_t sX = staging_base + (uint32_t)(warp - 2) * (EW == 4 ? 8192u : 4096u);
-      constexpr int NCH = BN / 64 / CS;           // 64-column chunks per warp and tile
-      const int c_lo = chalf * NCH;
-      // byte offset of this lane's gate piece for (tile origin m0/n0, chunk c2, k = 0); rows advance by 4 per k
-      auto piece_off = [&](int bidx, int m0, int n0, int c2, size_t ld) -> size_t {
-        const int acol = n0 + c2 * 64;
-        const int gcol = (acol >> 7) * 256 + (acol & 127) + lpiece * 8;
-        return (((size_t)bidx * p.M + m0 + q * 32 + lrsub) * ld + gcol) * sizeof(bf16);
-      };
-      auto tile_of = [&](const WorkIter<SK>& it, int& bidx, int& m0, int& n0) {
-        bidx = it.tile / tiles_per_batch;
-        const int rr = it.tile - bidx * tiles_per_batch;
-        m0 = (rr / p.tiles_n) * BM;
-        n0 = (rr % p.tiles_n) * BN;
-      };
-      const size_t row4_in = (size_t)4 * p.ld_aux * sizeof(bf16), row4_out = (size_t)4 * p.ldc * sizeof(bf16);
-      uint4 gv[8], uv[8];
-      auto gu_load_k = [&](int k, const uint8_t* base, int m0, int n0, int c2) {
-        const int rin = m0 + q * 32 + 4 * k + lrsub;
-        if (rin < p.M && n0 + c2 * 64 < p.N) {
-          gv[k] = ldg128(base + k * row4_in);
-          uv[k] = ldg128(base + k * row4_in + 256);
-        } else {
-          gv[k] = make_uint4(0u, 0u, 0u, 0u);
-          uv[k] = make_uint4(0u, 0u, 0u, 0u);
-        }
-      };
-      bool have = w.next();
-      if (have) {
-        int bidx, m0, n0;
-        tile_of(w, bidx, m0, n0);
-        const uint8_t* base = reinterpret_cast<const uint8_t*>(p.aux) + piece_off(bidx, m0, n0, c_lo, (size_t)p.ld_aux);
+      if (!epi_warp) {
+        release_acc();
+        continue;
+      }
+      const int split_idx = w.split;
+      const int bidx = w.tile / tiles_per_batch;
+      const int rr = w.tile - bidx * tiles_per_batch;
+      const int m0 = (rr / p.tiles_n) * BM;
+      const int n0 = (rr % p.tiles_n) * BN;
+      if (!SK && p.tma_store && p.epi == 2) {
+        // ===== SwiGLU backward epilogue: acc = d_act; d_gate = bf16(bf16(d_act*u) * silu'(g)), d_up = bf16(d_act * bf16(silu(g)))
+        // The accumulator arrives one ROW per thread, but gu / d_gu must move with coalesced accesses (a thread walking
+        // its own row issues 32 scattered 16-byte requests per instruction: measured slower than the unfused kernels).
+        // So bf16(d_act) goes through the warp's swizzled staging buffer and is re-read in a (4 rows x 8 pieces of
+        // 16 bytes) arrangement -- lane = (row % 4, piece) -- in which every global load / store instruction covers
+        // four full 128-byte row segments.  The gu registers are refilled in place for the NEXT chunk of the tile as
+        // soon as they have been consumed, so a whole chunk of math hides the DRAM latency.  Products of two bf16 values
+        // rounded to bf16 are single packed HMUL2.BF16 (exact product, one rounding: the same value as rounding the fp32 product).
+        const int lpiece = lane & 7, lrsub = lane >> 3;
+        const uint32_t sX = staging_base + (uint32_t)warp * (EW == 4 ? 8192u : 4096u);
+        constexpr int NCH = BN / 64 / CS;           // 64-column chunks per warp and tile
+        const int c_lo = chalf * NCH;
+        // byte offset of this lane's gate piece for (tile origin m0/n0, chunk c2, k = 0); rows advance by 4 per k
+        auto piece_off = [&](int bidx, int m0, int n0, int c2, size_t ld) -> size_t {
+          const int acol = n0 + c2 * 64;
+          const int gcol = (acol >> 7) * 256 + (acol & 127) + lpiece * 8;
+          return (((size_t)bidx * p.M + m0 + q * 32 + lrsub) * ld + gcol) * sizeof(bf16);
+        };
+        const size_t row4_in = (size_t)4 * p.ld_aux * sizeof(bf16), row4_out = (size_t)4 * p.ldc * sizeof(bf16);
+        uint4 gv[8], uv[8];
+        auto gu_load_k = [&](int k, const uint8_t* base, int m0, int n0, int c2) {
+          const int rin = m0 + q * 32 + 4 * k + lrsub;
+          if (rin < p.M && n0 + c2 * 64 < p.N) {
+            gv[k] = ldg128(base + k * row4_in);
+            uv[k] = ldg128(base + k * row4_in + 256);
+          } else {
+            gv[k] = make_uint4(0u, 0u, 0u, 0u);
+            uv[k] = make_uint4(0u, 0u, 0u, 0u);
+          }
+        };
+        {
+          const uint8_t* base = reinterpret_cast<const uint8_t*>(p.aux) + piece_off(bidx, m0, n0, c_lo, (size_t)p.ld_aux);
 #pragma unroll
-        for (int k = 0; k < 8; ++k) gu_load_k(k, base, m0, n0, c_lo);
-      }
-      while (have) {
-        int bidx, m0, n0;
-        tile_of(w, bidx, m0, n0);
-        WorkIter<SK> wn = w;
-        const bool have_next = wn.next();
-        int nb = 0, nm0 = 0, nn0 = 0;
-        if (have_next) tile_of(wn, nb, nm0, nn0);
-        mbar_wait(tfull_bar(as), aphase);
-        tc_fence_after();
-        const uint32_t taddr = tmem_base + (uint32_t(q * 32) << 16) + uint32_t(as * Cfg::ACC_STRIDE);
+          for (int k = 0; k < 8; ++k) gu_load_k(k, base, m0, n0, c_lo);
+        }
+        const uint32_t taddr = (uint32_t)(q * 32) << 16;
 #pragma unroll 1
         for (int c2 = c_lo; c2 < c_lo + NCH; ++c2) {
           const bool col_ok = n0 + c2 * 64 < p.N;
           {
             uint32_t r0[32], r1[32];
-            tmem_ld_32x32(taddr + c2 * 64, r0);
-            tmem_ld_32x32(taddr + c2 * 64 + 32, r1);
-            tmem_ld_wait();
+            acc_ld(taddr + c2 * 64, r0);
+            acc_ld(taddr + c2 * 64 + 32, r1);
 #pragma unroll
             for (int j = 0; j < 8; ++j) {
               const uint32_t* r = j < 4 ? r0 + 8 * j : r1 + 8 * (j - 4);
@@ -518,11 +539,10 @@ gemm_tcgen05_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_consta
             }
           }
           __syncwarp();
-          // where the registers freed below are refilled from: the next chunk of this tile, or the first chunk of the next
-          const bool last = c2 + 1 == c_lo + NCH;
-          const bool refill = last ? have_next : true;
-          const int fm0 = last ? nm0 : m0, fn0 = last ? nn0 : n0, fc2 = last ? c_lo : c2 + 1;
-          const uint8_t* fbase = reinterpret_cast<const uint8_t*>(p.aux) + piece_off(last ? nb : bidx, fm0, fn0, fc2, (size_t)p.ld_aux);
+          // the registers freed below are refilled from the next chunk of this tile
+          const bool refill = c2 + 1 < c_lo + NCH;
+          const int fm0 = m0, fn0 = n0, fc2 = c2 + 1;
+          const uint8_t* fbase = reinterpret_cast<const uint8_t*>(p.aux) + piece_off(bidx, fm0, fn0, fc2, (size_t)p.ld_aux);
           uint8_t* obase = reinterpret_cast<uint8_t*>(p.C) + piece_off(bidx, m0, n0, c2, (size_t)p.ldc);
 #pragma unroll
           for (int k = 0; k < 8; ++k) {
@@ -553,27 +573,14 @@ gemm_tcgen05_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_consta
           }
           __syncwarp();                              // all lanes are done reading sX before the next chunk overwrites it
         }
-        tc_fence_before();
-        __syncwarp();
-        if (lane == 0) mbar_arrive(tempty_bar(as));
-        as ^= 1;
-        if (as == 0) aphase ^= 1u;
-        have = w.next();
+        release_acc();
+        continue;
       }
-    } else
-    while (w.next()) {
-      const int split = w.split;
-      const int bidx = w.tile / tiles_per_batch;
-      const int rr = w.tile - bidx * tiles_per_batch;
-      const int m0 = (rr / p.tiles_n) * BM;
-      const int n0 = (rr % p.tiles_n) * BN;
-      mbar_wait(tfull_bar(as), aphase);
-      tc_fence_after();
       const int row_in_tile = q * 32 + lane;
       const int row_in = m0 + row_in_tile;
       const bool row_ok = row_in < p.M;
       const size_t row = (size_t)bidx * p.M + row_in;
-      const uint32_t taddr = tmem_base + (uint32_t(q * 32) << 16) + uint32_t(as * Cfg::ACC_STRIDE);
+      const uint32_t taddr = (uint32_t)(q * 32) << 16;   // (first row, column) of this warp in the parked tile
       const int first_contrib = (int)blockIdx.x + w.G;   // same member of the next group
       const int n_contrib = (SK && w.role == 2) ? w.n_contrib() : 0;
       if (SK && w.role == 1) {
@@ -582,8 +589,7 @@ gemm_tcgen05_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_consta
 #pragma unroll 1
         for (int c = 0; c < BN / 32; ++c) {
           uint32_t r[32];
-          tmem_ld_32x32(taddr + c * 32, r);
-          tmem_ld_wait();
+          acc_ld(taddr + c * 32, r);
 #pragma unroll
           for (int j = 0; j < 8; ++j)
             __stcg(reinterpret_cast<float4*>(slot + sk_slot_off(c, j, row_in_tile)),
@@ -603,10 +609,7 @@ gemm_tcgen05_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_consta
               const uint64_t t0 = globaltimer_ns();
               while (ld_acquire_u32(f) == 0u) {
                 __nanosleep(64);
-                if (globaltimer_ns() - t0 > 8000000000ull) {
-                  printf("slamkit_b200: stream-K flag wait timed out (cta %d waits for %d)\n", (int)blockIdx.x, c);
-                  __trap();
-                }
+                if (globaltimer_ns() - t0 > 8000000000ull) __trap();   // no printf: a call anywhere in this kernel serialises its wgmma pipeline
               }
             }
           }
@@ -614,7 +617,7 @@ gemm_tcgen05_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_consta
         }
         // one 64-column x 32-row bf16 chunk: registers -> this warp's swizzled staging buffer -> TMA store at (col, rows)
         auto stage_store = [&](const CUtensorMap* map, const uint32_t (&pk)[32], int col) {
-          const uint32_t sbuf = staging_base + (EW == 4 ? (uint32_t)(warp - 2) * 8192u + (store_cnt & 1u) * 4096u : (uint32_t)(warp - 2) * 4096u);
+          const uint32_t sbuf = staging_base + (EW == 4 ? (uint32_t)warp * 8192u + (store_cnt & 1u) * 4096u : (uint32_t)warp * 4096u);
           if (lane == 0) {
             if constexpr (EW == 4) tma_store_wait_read<1>(); else tma_store_wait_read<0>();
           }
@@ -643,9 +646,8 @@ gemm_tcgen05_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_consta
               uint32_t gpk[32], upk[32];
               {
                 uint32_t r0[32], r1[32];
-                tmem_ld_32x32(taddr + i * 64, r0);
-                tmem_ld_32x32(taddr + i * 64 + 32, r1);
-                tmem_ld_wait();
+                acc_ld(taddr + i * 64, r0);
+                acc_ld(taddr + i * 64 + 32, r1);
 #pragma unroll
                 for (int t = 0; t < 16; ++t) {
                   gpk[t] = pack_bf16(__uint_as_float(r0[2 * t]), __uint_as_float(r0[2 * t + 1]));
@@ -655,9 +657,8 @@ gemm_tcgen05_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_consta
               stage_store(&tmC, gpk, n0 + i * 64);
               {
                 uint32_t r0[32], r1[32];
-                tmem_ld_32x32(taddr + 128 + i * 64, r0);
-                tmem_ld_32x32(taddr + 128 + i * 64 + 32, r1);
-                tmem_ld_wait();
+                acc_ld(taddr + 128 + i * 64, r0);
+                acc_ld(taddr + 128 + i * 64 + 32, r1);
 #pragma unroll
                 for (int t = 0; t < 16; ++t) {
                   upk[t] = pack_bf16(__uint_as_float(r0[2 * t]), __uint_as_float(r0[2 * t + 1]));
@@ -693,9 +694,8 @@ gemm_tcgen05_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_consta
             const int col64 = n0 + c2 * 64;
             if (col64 >= p.N) break;
             uint32_t r0[32], r1[32], pk[32];
-            tmem_ld_32x32(taddr + c2 * 64, r0);
-            tmem_ld_32x32(taddr + c2 * 64 + 32, r1);
-            tmem_ld_wait();
+            acc_ld(taddr + c2 * 64, r0);
+            acc_ld(taddr + c2 * 64 + 32, r1);
 #pragma unroll
             for (int g = 0; g < 4; ++g) {
               float v0[8], v1[8];
@@ -741,9 +741,8 @@ gemm_tcgen05_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_consta
 #pragma unroll 1
           for (int c2 = chalf * (BN / 64 / CS); c2 < (chalf + 1) * (BN / 64 / CS); ++c2) {
             uint32_t r0[32], r1[32], pk[32];
-            tmem_ld_32x32(taddr + c2 * 64, r0);
-            tmem_ld_32x32(taddr + c2 * 64 + 32, r1);
-            tmem_ld_wait();
+            acc_ld(taddr + c2 * 64, r0);
+            acc_ld(taddr + c2 * 64 + 32, r1);
             if (SK && n_contrib > 0) {
               sk_fixup_add(r0, p.sk_ws, c2 * 2, row_in_tile, first_contrib, w.G, n_contrib);
               sk_fixup_add(r1, p.sk_ws, c2 * 2 + 1, row_in_tile, first_contrib, w.G, n_contrib);
@@ -772,9 +771,8 @@ gemm_tcgen05_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_consta
               for (int j = 0; j < 8; ++j) rv[j] = make_uint4(0u, 0u, 0u, 0u);
             }
             uint32_t r0[32], r1[32], pk[32];
-            tmem_ld_32x32(taddr + c2 * 64, r0);
-            tmem_ld_32x32(taddr + c2 * 64 + 32, r1);
-            tmem_ld_wait();
+            acc_ld(taddr + c2 * 64, r0);
+            acc_ld(taddr + c2 * 64 + 32, r1);
             if (SK && n_contrib > 0) {
               sk_fixup_add(r0, p.sk_ws, c2 * 2, row_in_tile, first_contrib, w.G, n_contrib);
               sk_fixup_add(r1, p.sk_ws, c2 * 2 + 1, row_in_tile, first_contrib, w.G, n_contrib);
@@ -797,10 +795,10 @@ gemm_tcgen05_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_consta
             stage_store(&tmC, pk, col64);
           }
         } else if (p.tma_store) {
-          // coalesced path: TMEM -> registers -> 128B-swizzled smem (this warp's private 32-row buffer) -> TMA store
+          // coalesced path: parked accumulator -> registers -> 128B-swizzled smem (this warp's private 32-row buffer) -> TMA store
 #pragma unroll 1
           for (int c2 = chalf * (BN / 64 / CS); c2 < (chalf + 1) * (BN / 64 / CS); ++c2) {
-            const uint32_t sbuf = staging_base + (EW == 4 ? (uint32_t)(warp - 2) * 8192u + (store_cnt & 1u) * 4096u : (uint32_t)(warp - 2) * 4096u);
+            const uint32_t sbuf = staging_base + (EW == 4 ? (uint32_t)warp * 8192u + (store_cnt & 1u) * 4096u : (uint32_t)warp * 4096u);
             if (lane == 0) {
               if constexpr (EW == 4) tma_store_wait_read<1>(); else tma_store_wait_read<0>();
             }
@@ -808,8 +806,7 @@ gemm_tcgen05_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_consta
 #pragma unroll
             for (int half = 0; half < 2; ++half) {
               uint32_t r[32];
-              tmem_ld_32x32(taddr + c2 * 64 + half * 32, r);
-              tmem_ld_wait();
+              acc_ld(taddr + c2 * 64 + half * 32, r);
               if (SK && n_contrib > 0) sk_fixup_add(r, p.sk_ws, c2 * 2 + half, row_in_tile, first_contrib, w.G, n_contrib);
 #pragma unroll
               for (int g = 0; g < 4; ++g) {
@@ -841,8 +838,7 @@ gemm_tcgen05_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_consta
 #pragma unroll 1
         for (int c = chalf * (BN / 32 / CS); c < (chalf + 1) * (BN / 32 / CS); ++c) {
           uint32_t r[32];
-          tmem_ld_32x32(taddr + c * 32, r);
-          tmem_ld_wait();
+          acc_ld(taddr + c * 32, r);
           if (SK && n_contrib > 0) sk_fixup_add(r, p.sk_ws, c, row_in_tile, first_contrib, w.G, n_contrib);
           const int col0 = n0 + c * 32;
           if (row_ok && col0 < p.N) {
@@ -854,7 +850,7 @@ gemm_tcgen05_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_consta
 #pragma unroll
                 for (int i = 0; i < 8; ++i) v[i] = __uint_as_float(r[g * 8 + i]);
                 if (p.splits > 1) {
-                  float* dst = p.splitk_ws + ((size_t)split * p.M + row_in) * p.N + col;
+                  float* dst = p.splitk_ws + ((size_t)split_idx * p.M + row_in) * p.N + col;
                   *reinterpret_cast<float4*>(dst) = make_float4(v[0], v[1], v[2], v[3]);
                   *reinterpret_cast<float4*>(dst + 4) = make_float4(v[4], v[5], v[6], v[7]);
                   continue;
@@ -899,20 +895,9 @@ gemm_tcgen05_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_consta
             for (int i = 0; i < n_contrib; ++i) p.sk_flags[(first_contrib + i * w.G) * 4 + q] = 0u;
         }
       }
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(tempty_bar(as));
-      as ^= 1;
-      if (as == 0) aphase ^= 1u;
+      release_acc();
     }
-    if (p.tma_store && lane == 0) tma_store_wait<0>();   // all bulk stores retired before the CTA exits
-  }
-
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) {
-    tc_fence_after();
-    tmem_dealloc(tmem_base, Cfg::TMEM_COLS);
+    if (epi_warp && p.tma_store && lane == 0) tma_store_wait<0>();   // all bulk stores retired before the CTA exits
   }
 }
 
@@ -1011,12 +996,12 @@ int launch_gemm(const CUtensorMap* tm, const GemmParams& p, int grid, cudaStream
   using Cfg = GemmCfg<BN, EW>;
   static bool attr_set = false;
   if (!attr_set) {
-    SK_CUDA_CHECK(cudaFuncSetAttribute(gemm_tcgen05_kernel<BN, A_MN, B_MN, SK, EW>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+    SK_CUDA_CHECK(cudaFuncSetAttribute(gemm_wgmma_kernel<BN, A_MN, B_MN, SK, EW>, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                        Cfg::SMEM_BYTES));
     attr_set = true;
   }
   sk_prof_begin(0, stream);
-  cudaError_t lerr = sk_launch_pdl_if(p.pdl != 0, gemm_tcgen05_kernel<BN, A_MN, B_MN, SK, EW>, dim3(grid), dim3(Cfg::THREADS), (size_t)Cfg::SMEM_BYTES, stream,
+  cudaError_t lerr = sk_launch_pdl_if(p.pdl != 0, gemm_wgmma_kernel<BN, A_MN, B_MN, SK, EW>, dim3(grid), dim3(GEMM_THREADS), (size_t)Cfg::SMEM_BYTES, stream,
                                    tm[0], tm[1], tm[2], tm[3], tm[4], tm[5], p);
   sk_prof_end(stream);
   SK_CUDA_CHECK(lerr);
@@ -1032,12 +1017,11 @@ int dispatch_major(bool a_mn, bool b_mn, const CUtensorMap* tm, const GemmParams
   return launch_gemm<BN, true, true, SK, EW>(tm, p, grid, s);
 }
 
-// Relative cost of one 128 x BN tile (BN=256 == 100), measured on B200 (profiles/r01_gemm_bench.txt): narrow tiles
-// pay the per-tile pipeline fill / epilogue overhead and re-read the A tile from shared memory more often per FLOP.
-// (A 224-wide tile, which would fit N = 896 exactly, was measured no faster per tile than 256: r01_gemm_bench_v3.)
+// Relative cost of one 128 x BN tile (BN=256 == 100), a heuristic: narrow tiles pay the per-tile pipeline fill /
+// epilogue overhead and re-read the A tile from shared memory more often per FLOP.
 inline int tile_cost(int bn) { return bn >= 256 ? 100 : (bn >= 128 ? 61 : 54); }
 
-constexpr size_t SK_FLAG_BYTES = 4096;   // tail of the scratch buffer: stream-K publish flags ([CTA][TMEM lane quadrant])
+constexpr size_t SK_FLAG_BYTES = 4096;   // tail of the scratch buffer: stream-K publish flags ([CTA][32-row quadrant])
 
 }  // namespace
 
@@ -1054,8 +1038,7 @@ int sk_pick_bn(int M, int N, int force_bn) {
     const long tiles = (long)((M + BM - 1) / BM) * ((N + bn - 1) / bn);
     const long waves = (tiles + nsm - 1) / nsm;
     const long cost = waves * tile_cost(bn);
-    // a narrower tile has to be clearly better (>= 25 %) to displace a wider one: measured near-ties favour BN = 256
-    // (profiles/r01_gemm_bench_v2_tma_store.txt: gu_wgrad 145 us at 256 vs 158 us at 128)
+    // a narrower tile has to be clearly better (>= 25 %) to displace a wider one (near-ties favour BN = 256)
     if (best_cost < 0 || cost * 100 < best_cost * 75) {
       best_cost = cost;
       best = bn;
@@ -1078,9 +1061,8 @@ int sk_gemm_ex_launch(const SkGemmEx& g, cudaStream_t stream) {
   const int nsm = sk_num_sms();
   // stream-K needs the plain 2-D form and a scratch buffer of sk_gemm_ws_min_bytes() whose last 4 KB (flags) are zero
   static const int sk_env = [] { const char* e = getenv("SK_STREAMK"); return e ? atoi(e) : 1; }();
-  // measured (profiles/r01_gemm_bench_v3_streamk.txt, A/B inside the LM step): balancing pays when whole-tile waves
-  // would leave >= ~20 % of the SM-time idle (gu_wgrad: 304 tiles = 2.05 waves, 144 -> 125 us); at 13 % idle the
-  // fix-up traffic eats the gain
+  // balancing pays when whole-tile waves would leave a good part (default >= 20 %) of the SM-time idle; with less idle
+  // time the fix-up traffic eats the gain
   static const int sk_min_idle = [] { const char* e = getenv("SK_STREAMK_MIN_IDLE"); return e ? atoi(e) : 20; }();
   static const int sk_min_kb = [] { const char* e = getenv("SK_STREAMK_MIN_KB"); return e ? atoi(e) : 32; }();
   const bool sk_ok = sk_env != 0 && g.batch == 1 && !use3d && g.passes == 1 && g.a_mode == 0 && g.splitk_ws != nullptr &&
@@ -1216,7 +1198,7 @@ int sk_gemm_ex_launch(const SkGemmEx& g, cudaStream_t stream) {
   if (p.sk_units > 0) {
     rc = dispatch_major<256, true>(g.a_mn, g.b_mn, tm, p, grid, stream);
   } else {
-    // 8 epilogue warps (two per TMEM lane quadrant) where the epilogue does real work per element; the plain
+    // 8 epilogue warps (two per 32-row quadrant) where the epilogue does real work per element; the plain
     // convert-and-store epilogue is faster with 4 (fewer warps contending with the TMA / MMA issue threads)
     static const int ew_env = [] { const char* e = getenv("SK_GEMM_EW"); return e ? atoi(e) : 0; }();
     const bool ew8 = BN == 256 && p.tma_store && (ew_env == 8 || (ew_env == 0 && (g.epi == 2 || g.epi == 3)));

@@ -15,7 +15,7 @@ namespace {
 
 SK_DEVINL float gelu_erf(float x) { return 0.5f * x * (1.0f + erff(x * 0.70710678118654752440f)); }
 // Branch-free GELU(erf) for the conv0 front, where it runs on 3.1e9 elements per batch and the kernel is bound by
-// instruction issue, not by HBM (profiles/r01_ncu_conv0_apply_v2.txt).  erf from Abramowitz-Stegun 7.1.26
+// instruction issue, not by HBM.  erf from Abramowitz-Stegun 7.1.26
 // (|error| <= 1.5e-7 absolute, below the 2^-17 relative quantisation of the hi/lo output it feeds), folded into the GELU:
 //   gelu(y) = y/2 (1 + erf(y/sqrt2)),  erf|z| = 1 - P(t) exp(-z^2),  t = 1/(1 + p|z|)
 //           = relu(y) - |y| * (P(t)/2) * exp(-y^2/2)
@@ -307,9 +307,7 @@ conv0_apply_kernel(const float* __restrict__ wav, const float* __restrict__ w, c
 //    iteration; the frames' windows overlap, so 15 samples feed both (8 outputs per thread-iteration).
 //  * The waveform is staged through shared memory in chunks of CONV0_PCH frame pairs (coalesced loads, next chunk
 //    fetched into registers while the current one is computed).  With per-iteration global loads the loop was bound by
-//    the loaded HBM read latency (~0.9 us per iteration while 2.7 TB/s of stores are in flight: one load -> use
-//    dependency per iteration, 16 warps per SM) no matter how the arithmetic was arranged
-//    (profiles/r01_conv0_apply_experiments.txt).
+//    the loaded HBM read latency (one load -> use dependency per iteration) no matter how the arithmetic was arranged.
 //  * GELU runs on packed pairs, stage by stage (gelu_fast_pairs), so the four dependency chains interleave and the
 //    FMA-pipe instruction count of the activation halves.
 constexpr int CONV0_PCH = 256;                       // frame pairs per chunk
@@ -423,243 +421,6 @@ conv0_apply_k10s5_kernel(const float* __restrict__ wav, const float* __restrict_
     if (more) commit(cur ^ 1);
     __syncthreads();
     cur ^= 1;
-  }
-}
-
-// ------------------------------------------------------------------------------------------------
-// conv0 on the tensor cores (kernel 10, stride 5: HuBERT's front).
-//
-// conv0_apply_k10s5_kernel above is bound by instruction issue, not by HBM: 21.5 instructions per output element, 5 of
-// them the ten taps (profiles/r01_conv0_apply_experiments.txt: 86 % of HBM peak without the GELU, 55 % with it).  Here
-// the taps, the GroupNorm scale AND the GroupNorm shift are one tcgen05 GEMM per 128-frame tile, in the same split-bf16
-// arithmetic as conv1..7:
-//     A row (one frame, 128 bytes) = [ x_hi[0..9] 1 0.. | x_hi[0..9] 1 0.. | x_lo[0..9] 0.. | 0.. ]        (4 x 16 bf16)
-//     B row (one channel of one clip) = [ ws_hi[0..9] sh_hi 0.. | ws_lo[0..9] sh_lo 0.. | ws_hi[0..9] 0.. | 0.. ]
-//   with ws = w * gamma * rstd and sh = beta - mean * gamma * rstd of that (clip, channel): three K = 16 MMAs give
-//   x_hi ws_hi + sh_hi + x_hi ws_lo + sh_lo + x_lo ws_hi = conv * scale + shift to ~2^-16 relative, fp32 accumulate in TMEM.
-// What is left for the CUDA cores is the epilogue: GELU on packed pairs, hi/lo split, swizzled staging, TMA stores.
-//   warps 0..3   build the A tile of the NEXT frame tile (one thread per frame: 10 samples -> hi/lo -> 8 swizzled 16-byte
-//                chunks), double-buffered
-//   warp 4       lane 0: TMA load of the clip's B operand when the clip changes; 3 MMAs per channel half and tile
-//   warps 5..12  epilogue, 4 warps (the four TMEM lane quadrants) per 256-channel half; thread = frame
-// One CTA per SM walks a contiguous range of (clip, frame tile) pairs, so B is (re)loaded at most twice per CTA.
-// ------------------------------------------------------------------------------------------------
-constexpr int C0T_THREADS = 416;
-constexpr uint32_t C0T_A_BYTES = 128 * 128;                 // one A tile
-constexpr uint32_t C0T_SMEM = 2 * C0T_A_BYTES + 512 * 128 + 8 * 2 * 4096 + 256 + 1024;
-
-SK_DEVINL void tma_store_3d(const void* tmap, uint32_t smem_src, int32_t c0, int32_t c1, int32_t c2) {
-  asm volatile("cp.async.bulk.tensor.3d.global.shared::cta.bulk_group [%0, {%2, %3, %4}], [%1];" ::"l"(tmap),
-               "r"(smem_src), "r"(c0), "r"(c1), "r"(c2)
-               : "memory");
-}
-
-// per (clip, channel): the 64 bf16 K-entries of the B operand described above
-__global__ void conv0_tc_prep_kernel(const float* __restrict__ w /*[C][10]*/, const float2* __restrict__ affine /*[B][C]*/,
-                                     bf16* __restrict__ bprep /*[B][C][64]*/, int C) {
-  const int b = blockIdx.y;
-  const int c = blockIdx.x * blockDim.x + threadIdx.x;
-  if (c >= C) return;
-  const float2 a = affine[(size_t)b * C + c];
-  uint16_t row[64];
-#pragma unroll
-  for (int k = 0; k < 64; ++k) row[k] = 0;
-  auto bits = [](float v) { return __bfloat16_as_ushort(__float2bfloat16_rn(v)); };
-  auto hi_of = [](float v) { return __bfloat162float(__float2bfloat16_rn(v)); };
-#pragma unroll
-  for (int j = 0; j < 10; ++j) {
-    const float ws = __ldg(w + c * 10 + j) * a.x;
-    const float h = hi_of(ws);
-    row[j] = bits(h);
-    row[16 + j] = bits(ws - h);
-    row[32 + j] = bits(h);
-  }
-  const float sh = hi_of(a.y);
-  row[10] = bits(sh);
-  row[26] = bits(a.y - sh);
-  uint4* dst = reinterpret_cast<uint4*>(bprep + ((size_t)b * C + c) * 64);
-#pragma unroll
-  for (int v = 0; v < 8; ++v)
-    dst[v] = make_uint4(row[8 * v] | (uint32_t)row[8 * v + 1] << 16, row[8 * v + 2] | (uint32_t)row[8 * v + 3] << 16,
-                        row[8 * v + 4] | (uint32_t)row[8 * v + 5] << 16, row[8 * v + 6] | (uint32_t)row[8 * v + 7] << 16);
-}
-
-__global__ void __launch_bounds__(C0T_THREADS, 1)
-conv0_tc_kernel(const __grid_constant__ CUtensorMap tmB, const __grid_constant__ CUtensorMap tmHi,
-                const __grid_constant__ CUtensorMap tmLo, const float* __restrict__ wav, int S, int pad, int T0, int C,
-                int n_clips) {
-  extern __shared__ uint8_t smem_raw[];
-  const uint32_t smem_base = (smem_u32(smem_raw) + 1023u) & ~1023u;
-  const uint32_t sA = smem_base, sB = sA + 2 * C0T_A_BYTES, sStage = sB + 512 * 128, bar = sStage + 8 * 2 * 4096;
-  const uint32_t a_full = bar, a_empty = bar + 16, b_full = bar + 32, t_full = bar + 40, t_empty = bar + 56, tmem_slot = bar + 72;
-  uint32_t* tmem_slot_ptr = reinterpret_cast<uint32_t*>(smem_raw + (tmem_slot - smem_u32(smem_raw)));
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int NT = C < 256 ? C : 256;                      // channels per TMEM buffer / MMA
-  const int n_half = C / NT;                             // 1 or 2
-  const int tpc = (T0 + 127) / 128;                      // frame tiles per clip
-  const long n_tiles = (long)tpc * n_clips;
-  const long tile_begin = n_tiles * blockIdx.x / gridDim.x, tile_end = n_tiles * (blockIdx.x + 1) / gridDim.x;
-
-  if (threadIdx.x == 0) {
-    tma_prefetch_desc(&tmB);
-    tma_prefetch_desc(&tmHi);
-    tma_prefetch_desc(&tmLo);
-    for (int i = 0; i < 2; ++i) {
-      mbar_init(a_full + 8 * i, 4);
-      mbar_init(a_empty + 8 * i, 1);
-      mbar_init(t_full + 8 * i, 1);
-      mbar_init(t_empty + 8 * i, 4);
-    }
-    mbar_init(b_full, 1);
-    fence_mbar_init();
-  }
-  if (warp == 4) {
-    tmem_alloc(tmem_slot, 512);
-    tmem_relinquish();
-  }
-  tc_fence_before();
-  __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot_ptr;
-
-  if (warp < 4) {
-    // ===== A-tile builders: thread r owns frame row r of the tile =====
-    const int r = threadIdx.x;
-    int it = 0;
-    for (long tile = tile_begin; tile < tile_end; ++tile, ++it) {
-      const int b = (int)(tile / tpc), ft = (int)(tile - (long)b * tpc);
-      const int buf = it & 1;
-      mbar_wait(a_empty + 8 * buf, (((uint32_t)it >> 1) & 1u) ^ 1u);
-      const int t = ft * 128 + r;
-      const long g0 = (long)5 * t - pad;
-      const float* wv = wav + (size_t)b * S;
-      uint32_t hb[10], lb[10];
-#pragma unroll
-      for (int j = 0; j < 10; ++j) {
-        const long g = g0 + j;
-        const float x = (t < T0 && g >= 0 && g < S) ? __ldg(wv + g) : 0.f;
-        const bf16 h = __float2bfloat16_rn(x);
-        hb[j] = __bfloat16_as_ushort(h);
-        lb[j] = __bfloat16_as_ushort(__float2bfloat16_rn(x - __bfloat162float(h)));
-      }
-      const uint4 c0 = make_uint4(hb[0] | hb[1] << 16, hb[2] | hb[3] << 16, hb[4] | hb[5] << 16, hb[6] | hb[7] << 16);
-      const uint4 c1 = make_uint4(hb[8] | hb[9] << 16, 0x3f80u, 0u, 0u);                       // x_hi[8], x_hi[9], 1.0, 0...
-      const uint4 c4 = make_uint4(lb[0] | lb[1] << 16, lb[2] | lb[3] << 16, lb[4] | lb[5] << 16, lb[6] | lb[7] << 16);
-      const uint4 c5 = make_uint4(lb[8] | lb[9] << 16, 0u, 0u, 0u);
-      const uint4 z = make_uint4(0u, 0u, 0u, 0u);
-      const uint4 ch[8] = {c0, c1, c0, c1, c4, c5, z, z};
-      const uint32_t row = sA + buf * C0T_A_BYTES + (uint32_t)r * 128u;
-#pragma unroll
-      for (int c = 0; c < 8; ++c)
-        asm volatile("st.shared.v4.b32 [%0], {%1, %2, %3, %4};" ::"r"(row + (uint32_t)((c ^ (r & 7)) << 4)), "r"(ch[c].x),
-                     "r"(ch[c].y), "r"(ch[c].z), "r"(ch[c].w)
-                     : "memory");
-      fence_proxy_async();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(a_full + 8 * buf);
-    }
-  } else if (warp == 4) {
-    // ===== B loader + MMA issuer =====
-    if (lane == 0) {
-      const uint32_t idesc = umma_idesc(1u, 0u, 0u, 128, (uint32_t)NT);
-      int cur_b = -1, it = 0;
-      uint32_t b_phase = 0;
-      for (long tile = tile_begin; tile < tile_end; ++tile, ++it) {
-        const int b = (int)(tile / tpc);
-        const int buf = it & 1;
-        if (b != cur_b) {
-          // the previous tile's MMAs (the last readers of sB) have retired once their commit freed its A buffer
-          if (it > 0) mbar_wait_sleep(a_empty + 8 * ((it - 1) & 1), (((uint32_t)(it - 1) >> 1) & 1u));
-          mbar_arrive_expect_tx(b_full, (uint32_t)C * 128u);
-          for (int hh = 0; hh < n_half; ++hh) tma_load_2d(sB + (uint32_t)hh * NT * 128u, &tmB, b_full, 0, b * C + hh * NT);
-          mbar_wait_sleep(b_full, b_phase);
-          b_phase ^= 1u;
-          cur_b = b;
-        }
-        mbar_wait_sleep(a_full + 8 * buf, ((uint32_t)it >> 1) & 1u);
-        for (int hh = 0; hh < n_half; ++hh) {
-          mbar_wait_sleep(t_empty + 8 * hh, ((uint32_t)it & 1u) ^ 1u);
-          tc_fence_after();
-#pragma unroll
-          for (int k = 0; k < 3; ++k)
-            tc_mma_f16(tmem_base + (uint32_t)hh * 256u, umma_desc_sw128(sA + buf * C0T_A_BYTES + k * 32, 16, 1024),
-                       umma_desc_sw128(sB + (uint32_t)hh * NT * 128u + k * 32, 16, 1024), idesc, k > 0 ? 1u : 0u);
-          tc_commit(t_full + 8 * hh);
-        }
-        tc_commit(a_empty + 8 * buf);
-      }
-    }
-  } else {
-    // ===== epilogue: GELU, hi/lo split, TMA stores; thread = frame =====
-    const int e = warp - 5;
-    const int hh = e >> 2;
-    const int q = warp & 3;
-    const uint32_t sbuf0 = sStage + (uint32_t)e * 8192u;
-    uint32_t store_cnt = 0;
-    auto stage_store = [&](const CUtensorMap* map, const uint32_t (&pk)[32], int col, int row0, int clip) {
-      const uint32_t sbuf = sbuf0 + (store_cnt & 1u) * 4096u;
-      if (lane == 0) tma_store_wait_read<1>();
-      __syncwarp();
-#pragma unroll
-      for (int j = 0; j < 8; ++j)
-        asm volatile("st.shared.v4.b32 [%0], {%1, %2, %3, %4};" ::"r"(sbuf + (uint32_t)lane * 128u + (uint32_t)((j ^ (lane & 7)) << 4)),
-                     "r"(pk[4 * j]), "r"(pk[4 * j + 1]), "r"(pk[4 * j + 2]), "r"(pk[4 * j + 3])
-                     : "memory");
-      fence_proxy_async();
-      __syncwarp();
-      if (lane == 0) {
-        tma_store_3d(map, sbuf, col, row0, clip);
-        tma_store_commit();
-      }
-      ++store_cnt;
-    };
-    if (hh < n_half) {
-      int it = 0;
-      for (long tile = tile_begin; tile < tile_end; ++tile, ++it) {
-        const int b = (int)(tile / tpc), ft = (int)(tile - (long)b * tpc);
-        mbar_wait(t_full + 8 * hh, (uint32_t)it & 1u);
-        tc_fence_after();
-        const uint32_t taddr = tmem_base + (uint32_t)hh * 256u + ((uint32_t)(q * 32) << 16);
-#pragma unroll 1
-        for (int c2 = 0; c2 < NT / 64; ++c2) {
-          uint32_t hpk[32], lpk[32];
-#pragma unroll
-          for (int half = 0; half < 2; ++half) {
-            uint32_t rr[32];
-            tmem_ld_32x32(taddr + c2 * 64 + half * 32, rr);
-            tmem_ld_wait();
-#pragma unroll
-            for (int g4 = 0; g4 < 4; ++g4) {
-              f32x2 y[4];
-#pragma unroll
-              for (int i = 0; i < 4; ++i) y[i] = pk2(__uint_as_float(rr[8 * g4 + 2 * i]), __uint_as_float(rr[8 * g4 + 2 * i + 1]));
-              gelu_fast_pairs<4>(y);
-#pragma unroll
-              for (int i = 0; i < 4; ++i) {
-                float g0, g1, l0, l1;
-                upk2(y[i], g0, g1);
-                const uint32_t h = pack_bf16(g0, g1);
-                upk2(sub2(y[i], pk2(__uint_as_float(h << 16), __uint_as_float(h & 0xffff0000u))), l0, l1);
-                hpk[half * 16 + g4 * 4 + i] = h;
-                lpk[half * 16 + g4 * 4 + i] = pack_bf16(l0, l1);
-              }
-            }
-          }
-          stage_store(&tmHi, hpk, hh * NT + c2 * 64, ft * 128 + q * 32, b);
-          stage_store(&tmLo, lpk, hh * NT + c2 * 64, ft * 128 + q * 32, b);
-        }
-        tc_fence_before();
-        __syncwarp();
-        if (lane == 0) mbar_arrive(t_empty + 8 * hh);
-      }
-      if (lane == 0) tma_store_wait<0>();
-    }
-  }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 4) {
-    tc_fence_after();
-    tmem_dealloc(tmem_base, 512);
   }
 }
 
@@ -869,7 +630,7 @@ int sk_split_f32_launch(const float* x, bf16* hi, bf16* lo, long n, cudaStream_t
 extern "C" int sk_conv0_nstat(void) { return NSTAT; }
 int sk_conv0_launch(const float* wav, const float* w, const float* gamma, const float* beta, double* stats,
                     float2* affine, bf16* out_hi, bf16* out_lo, int B, int S, int pad, int T0, int C, int KW, int ST,
-                    float eps, cudaStream_t s, bf16* bprep) {
+                    float eps, cudaStream_t s) {
   SK_REQUIRE(KW <= KW_MAX, "conv0: kernel width %d > %d", KW, KW_MAX);
   SK_REQUIRE(C % 8 == 0 && C / 4 <= 256, "conv0: channel count must be a multiple of 8 and <= 1024");
   SK_CUDA_CHECK(cudaMemsetAsync(stats, 0, (size_t)B * NSTAT * sizeof(double), s));
@@ -879,31 +640,7 @@ int sk_conv0_launch(const float* wav, const float* w, const float* gamma, const 
   dim3 g2((C + 127) / 128, B);
   conv0_affine_kernel<<<g2, 128, 0, s>>>(stats, w, gamma, beta, affine, C, KW, T0, eps);
   SK_LAUNCH_CHECK();
-  static const int mode = [] { const char* e = getenv("SK_CONV0_MODE"); return e ? atoi(e) : 3; }();
-  // tensor-core path (mode 3, default): HuBERT's kernel 10 / stride 5 front as a split-bf16 tcgen05 GEMM with the
-  // GroupNorm affine folded into the operand and GELU + hi/lo split in the epilogue
-  if (mode == 3 && KW == 10 && ST == 5 && bprep != nullptr && (C == 64 || C == 128 || C == 256 || C == 512)) {
-    conv0_tc_prep_kernel<<<dim3((C + 127) / 128, B), 128, 0, s>>>(w, affine, bprep, C);
-    SK_LAUNCH_CHECK();
-    CUtensorMap tmB, tmHi, tmLo;
-    const int NT = C < 256 ? C : 256;
-    int rc;
-    if ((rc = sk_make_tmap_2d(&tmB, bprep, 2, 64, (uint64_t)B * C, 64, 64, (uint32_t)NT))) return rc;
-    if ((rc = sk_make_tmap_3d(&tmHi, out_hi, (uint64_t)C, (uint64_t)T0, (uint64_t)B, (uint64_t)C, (uint64_t)T0 * C, 32))) return rc;
-    if ((rc = sk_make_tmap_3d(&tmLo, out_lo, (uint64_t)C, (uint64_t)T0, (uint64_t)B, (uint64_t)C, (uint64_t)T0 * C, 32))) return rc;
-    static bool attr = false;
-    if (!attr) {
-      SK_CUDA_CHECK(cudaFuncSetAttribute(conv0_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, C0T_SMEM));
-      attr = true;
-    }
-    const long n_tiles = (long)((T0 + 127) / 128) * B;
-    const int grid = (int)std::min<long>(n_tiles, sk_num_sms());
-    sk_prof_begin(3, s);
-    conv0_tc_kernel<<<grid, C0T_THREADS, C0T_SMEM, s>>>(tmB, tmHi, tmLo, wav, S, pad, T0, C, B);
-    sk_prof_end(s);
-    SK_LAUNCH_CHECK();
-    return 0;
-  }
+  static const int mode = [] { const char* e = getenv("SK_CONV0_MODE"); return e ? atoi(e) : 2; }();
   // CUDA-core paths: HuBERT's kernel 10 / stride 5 front with 4 channels x 2 frames per thread; generic kernel otherwise
   const bool fast = mode == 2 && KW == 10 && ST == 5 && C % 4 == 0 && C / 4 <= 256;
   const int fpb = fast ? 2 * CONV0_PCH : std::max(1, 256 / (C / 8));   // frames per block-iteration (fast: per chunk)

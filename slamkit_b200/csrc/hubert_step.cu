@@ -5,7 +5,7 @@
 // (SK:cluster/_k_means_lloyd.pyx:168-213), with everything device-resident: the only D2H traffic is the int32 labels.
 //
 // All matrix products (7 strided convolutions as windowed GEMMs, projections, grouped positional conv, attention,
-// FFN, k-means distances) run on the tcgen05 GEMM / mma.sync attention kernels in split-bf16 (hi, lo) form, 3 passes,
+// FFN, k-means distances) run on the wgmma GEMM / wgmma attention kernels in split-bf16 (hi, lo) form, 3 passes,
 // fp32 accumulation: the reference computes in fp32 and the unit ids have to agree with it.
 #include "kernels.h"
 #include "../../include/slamkit_b200.h"
@@ -28,7 +28,7 @@ struct LayerOff {
   int64_t wqkv, bqkv, wo, bo, ln1g, ln1b, w1, b1, w2, b2, ln2g, ln2b;
 };
 struct WsLayout {
-  int64_t stats, affine, conv0_b, act0, act1, lnc, x, xp, pc, h0, h1, qkv, ao, t1, ff, dot, n_frames, total;
+  int64_t stats, affine, act0, act1, lnc, x, xp, pc, h0, h1, qkv, ao, t1, ff, dot, n_frames, total;
 };
 int64_t align_up(int64_t v, int64_t a) { return (v + a - 1) / a * a; }
 }  // namespace
@@ -46,7 +46,6 @@ struct SkHubert {
   float* csq = nullptr;
   uint8_t* ws = nullptr;
   int64_t ws_bytes = 0;
-  int attn_tc = 1;   // tcgen05 split-precision attention (SK_HUBERT_ATTN_TC=0 selects the warp-level kernel)
 };
 
 namespace {
@@ -81,7 +80,6 @@ WsLayout make_layout(const SkHubert* h, int B, int S) {
   auto hilo = [&](int64_t elems) { return take(2 * align_up(elems * 2, 256)); };  // hi then lo
   w.stats = take((int64_t)B * sk_conv0_nstat() * 8);
   w.affine = take((int64_t)B * h->C * 8);
-  w.conv0_b = take((int64_t)B * h->C * 64 * 2);   // per-clip B operand of the tensor-core conv0 (hubert_kernels.cu)
   w.act0 = hilo((int64_t)B * T[0] * h->C);
   w.act1 = hilo((int64_t)B * (h->nconv > 1 ? T[1] : 1) * h->C);
   w.lnc = hilo(M * h->C);
@@ -155,7 +153,7 @@ int forward_impl(SkHubert* h, const float* wav, const int64_t* lens, int B, int 
   SK_TRY(sk_conv0_launch(wav, h->w32 + h->conv0_w, h->w32 + h->gn_g, h->w32 + h->gn_b,
                          reinterpret_cast<double*>(h->ws + w.stats), reinterpret_cast<float2*>(h->ws + w.affine),
                          act[0].hi, act[0].lo, B, S, h->cfg.pad, T[0], C, h->cfg.conv_kernel[0], h->cfg.conv_stride[0],
-                         1e-5f, s, reinterpret_cast<bf16*>(h->ws + w.conv0_b)));
+                         1e-5f, s));
   if (dbg_stage == 100) return sk_hilo_to_f32_launch(act[0].hi, act[0].lo, feat_out, (long)B * T[0] * C, s);
   // conv 1..n-1 as strided-window GEMMs (+GELU)
   int cur = 0;
@@ -213,11 +211,7 @@ int forward_impl(SkHubert* h, const float* wav, const int64_t* lens, int B, int 
     const LayerOff& o = h->lo[l];
     const bool last = (l == h->cfg.n_layers - 1) || (dbg_stage == l + 1);
     SK_TRY(linear_split(h, M, 3 * H, H, hb[0], o.wqkv, o.bqkv, 0, nullptr, qkv, nullptr, 3 * H, s));
-    if (h->attn_tc)
-      SK_TRY(sk_attn_tc_fwd_split_launch(qkv.hi, qkv.lo, ao.hi, ao.lo, B, Tf, h->cfg.n_heads, 3 * H, H, scale, s));
-    else
-      SK_TRY(sk_attn_fwd_split_launch(qkv.hi, qkv.lo, qkv.hi + H, qkv.lo + H, qkv.hi + 2 * H, qkv.lo + 2 * H, ao.hi, ao.lo,
-                                      B, Tf, h->cfg.n_heads, 3 * H, H, scale, s));
+    SK_TRY(sk_attn_tc_fwd_split_launch(qkv.hi, qkv.lo, ao.hi, ao.lo, B, Tf, h->cfg.n_heads, 3 * H, H, scale, s));
     SK_TRY(linear_split(h, M, H, H, ao, o.wo, o.bo, 0, &hb[0], t1, nullptr, H, s));
     SK_TRY(sk_layernorm_hilo_launch(t1.hi, t1.lo, nullptr, nullptr, h->w32 + o.ln1g, h->w32 + o.ln1b, hb[1].hi, hb[1].lo,
                                     nullptr, M, H, eps, s));
@@ -253,7 +247,6 @@ int sk_hubert_create(const SkHubertConfig* cfg, SkHubert** out) {
   SK_REQUIRE(cfg->pos_conv_kernel % 2 == 0, "sk_hubert_create: only even positional-conv kernels (HF drops the last frame)");
   SkHubert* h = new SkHubert();
   h->cfg = *cfg;
-  if (const char* e = getenv("SK_HUBERT_ATTN_TC")) h->attn_tc = atoi(e);
   h->C = cfg->conv_dim; h->H = cfg->hidden; h->F = cfg->ffn;
   h->G = cfg->pos_conv_groups; h->cg = cg; h->Kpos = cfg->pos_conv_kernel; h->halo = cfg->pos_conv_kernel / 2;
   h->U = cfg->n_units; h->Upad = (cfg->n_units + 63) / 64 * 64;

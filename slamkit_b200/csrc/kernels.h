@@ -88,15 +88,15 @@ int sk_seg_bounds_launch(const int32_t* pos_ids, int32_t* seg_start, int32_t* se
 
 // attention.cu
 int sk_attn_fwd_launch(const bf16* q, const bf16* k, const bf16* v, bf16* o, float* lse, int B, int T, int H, int KVH,
-                       int ld, int ldo, int causal, float scale, cudaStream_t s);
+                       int ld, int ldo, int causal, float scale, cudaStream_t s, const int* seg_start = nullptr);
 int sk_attn_bwd_launch(const bf16* q, const bf16* k, const bf16* v, const bf16* o, const bf16* d_o, const float* lse,
                        float* delta, bf16* dq, bf16* dk, bf16* dv, int B, int T, int H, int KVH, int ld, int ldo,
-                       int ldg, int causal, float scale, cudaStream_t s);
+                       int ldg, int causal, float scale, cudaStream_t s, const int* seg_start = nullptr);
 int sk_attn_fwd_split_launch(const bf16* q_hi, const bf16* q_lo, const bf16* k_hi, const bf16* k_lo, const bf16* v_hi,
                              const bf16* v_lo, bf16* o_hi, bf16* o_lo, int B, int T, int H, int ld, int ldo, float scale,
                              cudaStream_t s);
 
-// attention_tc.cu (tcgen05 / TMEM flash attention)
+// attention.cu: entry points on the fused q|k|v projection (LM step, HuBERT encoder)
 int sk_attn_tc_fwd_split_launch(const bf16* qkv_hi, const bf16* qkv_lo, bf16* o_hi, bf16* o_lo, int B, int T, int H, int ld,
                                 int ldo, float scale, cudaStream_t s);
 // seg_start / seg_end (optional, int32 [B*T]): in-row index of the first token of each token's document and one past
@@ -115,7 +115,7 @@ int sk_split_f32_launch(const float* x, bf16* hi, bf16* lo, long n, cudaStream_t
 extern "C" int sk_conv0_nstat(void);
 int sk_conv0_launch(const float* wav, const float* w, const float* gamma, const float* beta, double* stats,
                     float2* affine, bf16* out_hi, bf16* out_lo, int B, int S, int pad, int T0, int C, int KW, int ST,
-                    float eps, cudaStream_t s, bf16* bprep = nullptr /* [B][C][64] bf16 scratch: enables the tensor-core front */);
+                    float eps, cudaStream_t s);
 int sk_layernorm_hilo_launch(const bf16* a_hi, const bf16* a_lo, const bf16* b_hi, const bf16* b_lo, const float* gamma,
                              const float* beta, bf16* o_hi, bf16* o_lo, float* o_f32, int M, int D, float eps,
                              cudaStream_t s);

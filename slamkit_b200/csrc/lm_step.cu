@@ -29,7 +29,7 @@ struct WsLayout {
   int64_t X, h1, rstd1, qkv, ao, lse, xmid, h2, rstd2, gu, act;  // per-layer strides below
   int64_t sX, sh, srstd, sqkv, slse, sgu, sact;
   int64_t hf, rstdf, logits, dlogits, dxA, dxB, dh, dao, dqkv, dgu, delta;
-  int64_t dw_partial, colsum_partial, ce_partial, embed_scratch, splitk, splitk_bytes, attn_partial, seg_start, seg_end, total;
+  int64_t dw_partial, colsum_partial, ce_partial, embed_scratch, splitk, splitk_bytes, seg_start, seg_end, total;
 };
 }  // namespace
 
@@ -118,7 +118,6 @@ WsLayout make_layout(const SkLm* lm, int B, int T) {
   w.colsum_partial = take((int64_t)sk_colsum_splits() * lm->qkv_dim * 4);
   w.ce_partial = take((int64_t)sk_ce_blocks((int)M) * 2 * 4);
   w.embed_scratch = take((int64_t)lm->Vp * lm->d * 8);   // 64-bit fixed-point accumulators of the embedding gradient
-  w.attn_partial = take((int64_t)B * lm->H * T * 128 * 4);   // per-head fp32 dK|dV partials (tcgen05 backward)
   w.seg_start = take(M * 4);   // document bounds of packed batches (position_ids given), int32 per token
   w.seg_end = take(M * 4);
   w.total = cur;
@@ -228,7 +227,7 @@ int forward_impl(SkLm* lm, const int64_t* ids, const int64_t* labels, const int3
 // Only [chunk, Vp] logits ever exist (0.6 GB at 2048 rows instead of 2 x 2.5 GB at [8192, 152 k]) and every element
 // moves through HBM as in the one-pass form; the price is one read-modify-write of dE per extra chunk.  (A fully fused
 // "flash" CE would recompute the logits GEMM in the backward pass -- 2.2 TFLOP at this shape, more time than the 7.5 GB
-// of logits traffic it removes: DESIGN.md §4.)  The sums per row meet in `ce_partial`, finalised once.
+// of logits traffic it removes.)  The sums per row meet in `ce_partial`, finalised once.
 int head_chunked(SkLm* lm, const int64_t* labels, int B, int T, float num_items, float dloss, int accumulate, float* stats,
                  const WsLayout& w, cudaStream_t s) {
   const int M = B * T, d = lm->d;
@@ -299,10 +298,10 @@ int backward_impl(SkLm* lm, const int64_t* ids, const int32_t* pos_ids, int B, i
     // attention
     SK_TRY(linear_dgrad(M, d, d, dxB, P + o.wo, dao, s));
     SK_TRY(linear_wgrad(M, d, d, dxB, ao, G + o.wo, accumulate, s, lm->ws + w.splitk, (size_t)w.splitk_bytes));
-    SK_TRY(sk_attn_tc_bwd_launch(qkv, ao, dao, lse, wsp<float>(lm, w.delta), wsp<float>(lm, w.attn_partial), dqkv, B, T,
+    SK_TRY(sk_attn_tc_bwd_launch(qkv, ao, dao, lse, wsp<float>(lm, w.delta), nullptr, dqkv, B, T,
                                  lm->H, lm->KVH, Q, d, Q, 1, scale, s, pos_ids ? wsp<int32_t>(lm, w.seg_start) : nullptr,
                                  pos_ids ? wsp<int32_t>(lm, w.seg_end) : nullptr, lm->rope_cos, lm->rope_sin, pos_ids,
-                                 lm->cfg.max_positions));   // inverse RoPE on dq / dk applied by the attention kernels' epilogues
+                                 lm->cfg.max_positions));   // inverse RoPE on dq / dk applied after the attention backward
     if (lm->cfg.qkv_bias)
       SK_TRY(sk_colsum_launch(dqkv, G + o.bqkv, wsp<float>(lm, w.colsum_partial), M, Q, Q, accumulate, s));
     SK_TRY(linear_dgrad(M, Q, d, dqkv, P + o.wqkv, dh, s));

@@ -3,15 +3,10 @@
 // single NVSwitch node.
 //
 // Why not NCCL here: with the element-wise work fused into GEMM epilogues the backward pass is wall-to-wall persistent
-// CTAs that each own a whole SM's shared memory; NCCL's channel CTAs (hundreds of threads, tens of KB of shared memory)
-// only get an SM when one of those exits, and a persistent 148-CTA GEMM then runs a second wave for the CTAs it lost, so
-// most of the 716 MB moved after the backward pass (profiles/r02_n2_same_box.txt).  The kernels below are built to
-// CO-RESIDE with those CTAs: 4 warps of <= 32 registers per thread and no shared memory.  Registers are allocated per SM
-// sub-partition (16 K each) and a warp is bound to one by its index, so what matters is the room left in EACH
-// sub-partition: two attention-backward CTAs (5 warps x 96 registers each), two 240-register GEMM warps or three
-// 160-register ones leave exactly the 1024 registers one such warp needs (the GEMM kernels are capped at 240 / 160 for
-// this; measured with tools/coresidency_check.py) -- so the reduction rides along with the backward pass instead of
-// waiting for it, and its resident CTAs do not keep the next kernel's CTAs off their SMs.
+// CTAs that each own most of an SM's shared memory; NCCL's channel CTAs (hundreds of threads, tens of KB of shared
+// memory) only get an SM when one of those exits.  The kernels below are built small instead -- 4 warps of <= 32 registers
+// per thread and no shared memory -- so that they can find room next to those CTAs.  How much of the reduction actually
+// overlaps the backward pass on an H100 depends on the resident kernels' register use and is not measured here.
 //
 // Algorithm (one launch per bucket, every rank runs the same code on its own copy of the flat bf16 gradient buffer; all
 // buffers and flag arrays are mapped into every process with CUDA IPC):
@@ -117,10 +112,8 @@ __global__ void __launch_bounds__(256) p2p_wait_kernel(const uint32_t* own_flags
 }
 
 // W = compile-time world size (2, 4, 8) or 0 = run-time `world` (any size up to 8).
-// Register budget: 32 per thread -- one warp then needs 1024 registers of its SM sub-partition, which is what two
-// attention-backward CTAs (5 warps x 96 registers per sub-partition) or two 240-register GEMM warps leave free there.
-// Warps are bound to a sub-partition by their index, so the budget has to hold per sub-partition, not per SM
-// (measured with tools/coresidency_check.py).  Two 16-byte loads are in flight per thread; the memory-level parallelism
+// Register budget: 32 per thread -- one warp then needs 1024 registers of its SM sub-partition, a small enough slice to
+// fit next to the backward kernels.  Two 16-byte loads are in flight per thread; the memory-level parallelism
 // comes from the number of resident warps instead.
 template <int W>
 __global__ void __launch_bounds__(P2P_THREADS, 16)
@@ -182,8 +175,8 @@ p2p_allreduce_kernel(P2PPeers pr, uint32_t* own_flags, int rank, int world, size
 }
 
 // Stand-in with exactly the reduce kernel's footprint (64 threads, <= 64 registers, no shared memory) that just occupies
-// its slot for `ns` nanoseconds: tools/coresidency_check.py times the backward kernels with and without it resident to
-// show which of them share an SM with the reduce kernel.
+// its slot for `ns` nanoseconds: timing the backward kernels with and without it resident shows which of them share an SM
+// with the reduce kernel.
 __global__ void __launch_bounds__(P2P_THREADS, 16) p2p_hog_kernel(unsigned long long ns, unsigned* started, float* sink) {
   if (threadIdx.x == 0) atomicAdd(started, 1u);
   const uint64_t t0 = globaltimer_ns();

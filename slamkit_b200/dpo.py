@@ -1,4 +1,4 @@
-"""DPO step on the B200 train path (SURVEY.md §8 f-2): mirror of `SLAMDPOTrainer` (slamkit/trainer/slam_dpo_trainer.py:4-64,
+"""DPO step on the GPU train path (SURVEY.md §8 f-2): mirror of `SLAMDPOTrainer` (slamkit/trainer/slam_dpo_trainer.py:4-64,
 a `trl.DPOTrainer` whose `tokenize_row` prepends BOS to the prompt and appends EOS to both completions) with trl's default
 sigmoid loss, beta 0.1 (config/training_args/dpo_training_args.yaml:5-6), frozen reference model.
 

@@ -1,4 +1,4 @@
-"""`TokenLM.generate` for the B200 unit LM (slamkit/model/token_lm.py:19-27; `UnitLM.generate` hands the call to HF's
+"""`TokenLM.generate` for the GPU unit LM (slamkit/model/token_lm.py:19-27; `UnitLM.generate` hands the call to HF's
 `GenerationMixin.generate`, slamkit/model/unit_lm.py:196-198; callers: `SpeechLM.generate`, slamkit/model/speech_lm.py:38-55,
 with `config/metric/generate.yaml`'s `temperature / top_k / max_new_tokens / do_sample` and `bad_words_ids`).
 

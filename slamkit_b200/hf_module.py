@@ -1,4 +1,4 @@
-"""HF-Trainer-compatible face of the B200 train step (SURVEY.md §8 b-2): an `nn.Module` whose `forward(input_ids,
+"""HF-Trainer-compatible face of the GPU train step (SURVEY.md §8 b-2): an `nn.Module` whose `forward(input_ids,
 attention_mask, position_ids, labels, num_items_in_batch)` returns `CausalLMOutputWithPast(loss, logits)` under autograd,
 as `slamkit.model.unit_lm.UnitLM.forward` does (slamkit/model/unit_lm.py:135-182), so that `SLAMTrainer` / HF `Trainer`,
 the reference collators and callbacks can drive it unchanged:
@@ -8,7 +8,7 @@ the reference collators and callbacks can drive it unchanged:
     loss.backward()                     # model.flat.grad is the flat bf16 gradient buffer
     torch.optim.AdamW(model.parameters()).step()
 
-The module has ONE parameter, `flat`: the flat bf16 buffer the sm_100a kernels read (same storage as `core.params`), so
+The module has ONE parameter, `flat`: the flat bf16 buffer the sm_90a kernels read (same storage as `core.params`), so
 optimisers and `clip_grad_norm_` see every weight; `state_dict()` / `load_state_dict()` speak the reference's names
 (`lm.model.layers.N...`).  Forward + backward run in one C-ABI call (`sk_lm_forward_backward`) inside the
 `autograd.Function`'s forward -- the gradient of a scalar loss with respect to the flat buffer is known as soon as the

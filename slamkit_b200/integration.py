@@ -41,7 +41,7 @@ def hubert_b200_from_cfg(pretrained_model: str = "facebook/hubert-base-ls960",
 def tlm_b200_from_cfg(cfg, device: str = "cuda:0", max_batch: int = 8, max_seq: Optional[int] = None):
     """`cfg` is the reference's model config node (config/model/*.yaml): context_len, config_args{base_model_name,
     vocab_size, twist_init, rope_theta, ...}.  Raises OSError when the base model cannot be reached (offline box) and
-    ValueError when its architecture has no B200 kernels (anything but Qwen2)."""
+    ValueError when its architecture has no kernels here (anything but Qwen2)."""
     from transformers import AutoConfig
     from .lm import B200UnitLM, LMConfig
 

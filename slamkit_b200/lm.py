@@ -3,7 +3,7 @@
 Mirrors `slamkit.model.unit_lm.UnitLM` (slamkit/model/unit_lm.py:82-212) and the `TokenLM` ABC
 (slamkit/model/token_lm.py:7-27): same `forward(input_ids, attention_mask, position_ids, labels,
 num_items_in_batch)` contract, `log_likelihood`, HF-compatible state-dict names (`lm.model.layers.N...`), but the
-compute is the hand-written sm_100a train step behind the C ABI (`sk_lm_*` in include/slamkit_b200.h).  PyTorch only
+compute is the hand-written sm_90a train step behind the C ABI (`sk_lm_*` in include/slamkit_b200.h).  PyTorch only
 owns the flat bf16 parameter / gradient / workspace buffers.
 """
 from __future__ import annotations
@@ -38,14 +38,14 @@ class LMConfig:
     @staticmethod
     def from_hf(cfg, vocab_size: Optional[int] = None, max_positions: int = 2048) -> "LMConfig":
         """From an HF config of the base model.  Only the Qwen2 decoder architecture (RMSNorm, rotary GQA attention with
-        q/k/v bias, SwiGLU, no o/MLP bias) has sm_100a kernels behind it: anything else (e.g. the OPT-125M of
+        q/k/v bias, SwiGLU, no o/MLP bias) has sm_90a kernels behind it: anything else (e.g. the OPT-125M of
         config/model/twist.yaml) is refused instead of being silently trained as a different model."""
         mt = getattr(cfg, "model_type", None)
         if mt != "qwen2":
-            raise ValueError(f"unsupported base architecture '{mt}': the B200 train path implements the Qwen2 decoder "
+            raise ValueError(f"unsupported base architecture '{mt}': the GPU train path implements the Qwen2 decoder "
                              "(use model=slam, config/model/slam.yaml)")
         if getattr(cfg, "head_dim", None) not in (None, 64) or cfg.hidden_size // cfg.num_attention_heads != 64:
-            raise ValueError("unsupported attention geometry: the sm_100a attention kernels need head_dim 64")
+            raise ValueError("unsupported attention geometry: the sm_90a attention kernels need head_dim 64")
         rp = getattr(cfg, "rope_parameters", None) or {}
         theta = rp.get("rope_theta", getattr(cfg, "rope_theta", 10000.0))
         return LMConfig(
@@ -77,7 +77,7 @@ def write_unit_lm_checkpoint(save_directory: str, state_dict_hf: Dict[str, torch
                              base_model_name: str = "Qwen/Qwen2.5-0.5B") -> None:
     """Writes `model.safetensors` with the `lm.`-prefixed names of `UnitLM.state_dict()` (base_model_prefix = "lm",
     slamkit/model/unit_lm.py:87) and a `config.json` in the `UnitLMConfig` layout (unit_lm.py:32-79), so that the
-    reference's `UnitLM.from_pretrained(dir)` / cli/eval.py consume a B200-trained model.  Pure host code (no CUDA):
+    reference's `UnitLM.from_pretrained(dir)` / cli/eval.py consume a model trained with this package.  Pure host code (no CUDA):
     tests/test_host_cpu.py loads such a directory with the reference's own class."""
     import json
     import os
@@ -110,10 +110,10 @@ def check_right_padded(attention_mask: Optional[torch.Tensor]) -> None:
         return
     m = attention_mask
     if m.dim() != 2:
-        raise ValueError("attention_mask must be [batch, seq] (explicit 4-D masks are not supported on the B200 path)")
+        raise ValueError("attention_mask must be [batch, seq] (explicit 4-D masks are not supported on the GPU path)")
     ok = bool(((m[:, 1:] != 0) <= (m[:, :-1] != 0)).all()) if m.shape[1] > 1 else True
     if not ok:
-        raise ValueError("attention_mask is not right-padding (ones then zeros per row): the B200 attention kernels "
+        raise ValueError("attention_mask is not right-padding (ones then zeros per row): the GPU attention kernels "
                          "implement causal masking only")
 
 

@@ -221,7 +221,7 @@ def seg_bounds(pos_ids: torch.Tensor) -> Tuple[torch.Tensor, torch.Tensor]:
 
 def attn_tc_fwd(qkv: torch.Tensor, B: int, T: int, H: int, KVH: int, causal: bool, scale: float,
                 seg_start: Optional[torch.Tensor] = None):
-    """tcgen05 flash-attention forward (sk_attn_tc_fwd); same contract as attn_fwd.  seg_start (from seg_bounds) makes
+    """Flash-attention forward on the fused projection (sk_attn_tc_fwd); same contract as attn_fwd.  seg_start (from seg_bounds) makes
     it block-diagonal causal for packed batches."""
     lib = L.require_cuda()
     o = torch.empty((B * T, H * 64), device=qkv.device, dtype=torch.bfloat16)
@@ -233,12 +233,11 @@ def attn_tc_fwd(qkv: torch.Tensor, B: int, T: int, H: int, KVH: int, causal: boo
 
 def attn_tc_bwd(qkv, o, d_o, lse, B, T, H, KVH, causal: bool, scale: float, seg_start: Optional[torch.Tensor] = None,
                 seg_end: Optional[torch.Tensor] = None) -> torch.Tensor:
-    """tcgen05 flash-attention backward (sk_attn_tc_bwd); same contract as attn_bwd."""
+    """Flash-attention backward on the fused projection (sk_attn_tc_bwd); same contract as attn_bwd."""
     lib = L.require_cuda()
     dqkv = torch.empty_like(qkv)
     delta = torch.empty_like(lse)
-    partial = torch.empty((B, H, T, 128), device=qkv.device, dtype=torch.float32)
-    L.check(lib.sk_attn_tc_bwd(L.ptr(qkv), L.ptr(o), L.ptr(d_o), L.ptr(lse), L.ptr(delta), L.ptr(partial), L.ptr(dqkv),
+    L.check(lib.sk_attn_tc_bwd(L.ptr(qkv), L.ptr(o), L.ptr(d_o), L.ptr(lse), L.ptr(delta), L.ptr(None), L.ptr(dqkv),
                                B, T, H, KVH, qkv.stride(0), o.stride(0), dqkv.stride(0), int(causal), L.f32(scale),
                                L.ptr(seg_start), L.ptr(seg_end), L.stream_ptr()))
     return dqkv

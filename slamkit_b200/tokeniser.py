@@ -111,7 +111,7 @@ class B200InterleavingTokeniser:
     contract of the interleaved speech-text recipe (config/tokeniser/interleaved_hubert_25.yaml, BASELINE cfg-4): an HF
     text tokenizer extended with `<Un0>..<Un{n-1}>`, `<speech>`, `<text>` (interleaving_tokeniser.py:121-127), so the
     model vocabulary is text + units (~152 k rows for Qwen2.5).  `prepare_sample` / `string_tokenise` / `len` are what
-    cli/train.py needs; `audio_represent` goes through the same B200 feature extractor as the unit tokeniser.  Building
+    cli/train.py needs; `audio_represent` goes through the same GPU feature extractor as the unit tokeniser.  Building
     the interleaved strings from word alignments (`stringify_representation(mode='train')`) is text-side preprocessing
     outside the hot path (SURVEY.md §2) and is not re-implemented: prepare such token files with the reference."""
 
@@ -136,7 +136,7 @@ class B200InterleavingTokeniser:
 
     def stringify_representation(self, reps: List[Dict], mode: str = "test") -> List[str]:
         if mode == "train":
-            raise NotImplementedError("interleaving from word alignments is text-side preprocessing outside the B200 hot "
+            raise NotImplementedError("interleaving from word alignments is text-side preprocessing outside the GPU hot "
                                       "path; prepare interleaved token files with the reference's cli/prepare_tokens.py")
         return ["".join(f"<Un{u}>" for u in cur["units"]) for cur in reps]
 

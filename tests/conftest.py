@@ -10,7 +10,7 @@ GOLDEN = os.path.join(ROOT, "tests", "golden")
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a CUDA device (B200, sm_100a); run with -m gpu on the GPU box")
+    config.addinivalue_line("markers", "gpu: needs a CUDA device (H100, sm_90a); run with -m gpu on a GPU machine")
 
 
 def pytest_collection_modifyitems(config, items):

@@ -117,7 +117,7 @@ full = torch.randint(2, 502, (4, 32), generator=g); full[:, 0] = 1
 full[3, 20:] = 0
 labels = full.clone(); labels[full == 0] = -100
 mine = slice(rank * 2, rank * 2 + 2)
-# the scheme bench.py / B200 trainer use: every rank normalises by the GLOBAL item count, then all-reduce(SUM)
+# the scheme bench.py / B200Trainer use: every rank normalises by the GLOBAL item count, then all-reduce(SUM)
 n_local = torch.tensor([float((labels[mine] != -100).sum())]); n_glob = n_local.clone(); dist.all_reduce(n_glob)
 _, _, grads = O.forward_backward(p, cfg, full[mine], labels[mine], float(n_glob))
 flat = torch.cat([grads[k].float().flatten() for k in sorted(grads)])
@@ -257,13 +257,11 @@ def test_flac_decoder_roundtrip(tmp_path, ch, mode, order, porder, mid_side):
 
 
 def test_flac_decoder_on_reference_example_audio():
-    """The reference's own example_data (present only in the build container): decoded sample counts are the known
+    """The reference's own example_data/audio files (stored under tests/golden/): decoded sample counts are the known
     answers 225360 / 255120 of SURVEY.md §4 and the PCM hashes to the MD5 stored in each file's STREAMINFO."""
     import hashlib
     from slamkit_b200.audio_io import flac_decode_int, flac_info
-    base = "/root/reference/example_data/audio"
-    if not os.path.isdir(base):
-        pytest.skip("reference example data is only mounted in the build container")
+    base = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden")
     for name, n in (("audio1.flac", 225360), ("audio2.flac", 255120)):
         info = flac_info(os.path.join(base, name))
         pcm = flac_decode_int(os.path.join(base, name))

@@ -14,7 +14,6 @@ import torch
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 GOLDEN = os.path.join(ROOT, "tests", "golden")
-REF = "/root/reference"
 
 
 # ------------------------------------------------------------------------------------------------ GradSync
@@ -189,46 +188,33 @@ def test_checkpoint_layout_round_trip(tmp_path):
     assert c["base_config"]["num_key_value_heads"] == 1 and c["vocab_size"] == 502 and c["twist_init"] is False
 
 
-@pytest.mark.skipif(not os.path.isdir(REF), reason="the reference checkout exists only in the build container")
-def test_reference_unit_lm_loads_a_b200_checkpoint(tmp_path, monkeypatch):
-    """SURVEY.md §8 f-4: the reference's own `UnitLM.from_pretrained` consumes the directory `save_pretrained` writes, and
-    its logits / log_likelihood on it equal the oracle's (which the GPU path is tested against)."""
+def test_reference_unit_lm_loads_a_b200_checkpoint(tmp_path):
+    """SURVEY.md §8 f-4: the reference's own `UnitLM.from_pretrained` consumes the directory `save_pretrained` writes.
+    tests/golden/unit_lm_checkpoint.npz holds what it produced on such a directory (oracle/make_goldens.py checkpoint):
+    the state-dict keys it ended up with, a fingerprint of every loaded parameter and its bf16 logits; the checkpoint
+    written here must load to the same parameters, and the oracle (which the GPU path is tested against) must give the
+    same logits."""
     from oracle import lm_oracle as O
+    from oracle.make_goldens import _param_digest
+    from safetensors.torch import load_file
     from slamkit_b200.lm import write_unit_lm_checkpoint
-    m = types.ModuleType("omegaconf")
-    m.DictConfig, m.ListConfig, m.OmegaConf = type("DictConfig", (dict,), {}), type("ListConfig", (list,), {}), type("OmegaConf", (), {})
-    sys.modules.setdefault("omegaconf", m)
-    if REF not in sys.path:
-        sys.path.insert(0, REF)
-    import slamkit.model.unit_lm as ref_mod
-    from slamkit.model.unit_lm import UnitLM
-    from transformers import OPTConfig
-    # HF builds a default-constructed UnitLMConfig() to diff configs, and the reference's default base model is looked up
-    # on the hub (unit_lm.py:37,66-70): stand in for that one lookup, everything else is the reference's own code path
-    real = ref_mod.AutoConfig.from_pretrained
-    monkeypatch.setattr(ref_mod.AutoConfig, "from_pretrained",
-                        staticmethod(lambda name, *a, **k: OPTConfig() if name == "facebook/opt-350M" else real(name, *a, **k)))
+    z = np.load(os.path.join(GOLDEN, "unit_lm_checkpoint.npz"))
     ocfg = O.OracleLMConfig(vocab_size=502, hidden=128, n_layers=2, n_heads=2, n_kv_heads=1, head_dim=64, ffn=256)
     p = O.init_params(ocfg, seed=3)
-    base = tmp_path / "base"
-    os.makedirs(base)
-    ck = tmp_path / "ck"
-    write_unit_lm_checkpoint(str(ck), p, _tiny_cfg(), base_model_name=str(base))
-    json.dump(json.load(open(ck / "config.json"))["base_config"], open(base / "config.json", "w"))   # offline stand-in for the hub
-    model = UnitLM.from_pretrained(str(ck), torch_dtype=torch.bfloat16)
-    sd = model.state_dict()
-    assert all(torch.equal(sd[k], p[k]) for k in p), [k for k in p if not torch.equal(sd[k], p[k])][:3]
-    g = torch.Generator().manual_seed(1)
-    ids = torch.randint(2, 502, (2, 24), generator=g)
-    ids[:, 0] = 1
+    write_unit_lm_checkpoint(str(tmp_path), p, _tiny_cfg(), base_model_name="Qwen/Qwen2.5-0.5B")
+    sd = load_file(str(tmp_path / "model.safetensors"))
+    ref_keys = [str(k) for k in z["keys"]]
+    tied = {"lm.lm_head.weight": "lm.model.embed_tokens.weight"}     # tied to the embedding in the reference's model
+    for k, shape, dig in zip(ref_keys, z["shapes"], z["digests"]):
+        t = sd[k] if k in sd else sd[tied[k]]
+        assert list(t.shape) == json.loads(str(shape)), k
+        assert np.allclose(_param_digest(t), dig, rtol=1e-12, atol=1e-9), k
+    assert set(sd) <= set(ref_keys)
+    ids = torch.from_numpy(z["ids"])
     with torch.no_grad():
-        ref_logits = model(input_ids=ids).logits
-    with torch.no_grad():
-        logits = O.forward_logits(p, ocfg, ids)
-    assert torch.equal(ref_logits.to(torch.bfloat16), logits.to(torch.bfloat16))
-    z = np.load(os.path.join(GOLDEN, "lm_loglik.npz"))
-    ll = model.log_likelihood(torch.from_numpy(z["tokens"]), mean_nll=False)
-    assert np.allclose(ll.float().numpy(), z["ll_sum"], rtol=1e-5, atol=1e-4)
+        logits = O.forward_logits(p, ocfg, ids).to(torch.bfloat16)
+    ref_logits = torch.from_numpy(z["logits_u16"].astype(np.int16)).view(torch.bfloat16)
+    assert torch.equal(ref_logits, logits)
 
 
 def test_checkpoint_rotation_and_listing(tmp_path):

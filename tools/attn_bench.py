@@ -1,4 +1,4 @@
-"""Times the attention kernels at the LM shape (B=8,H=14,KVH=2,T=1024): warp-level (mma.sync) vs tcgen05."""
+"""Times the wgmma attention kernels (forward, backward) at the LM shape (B=8,H=14,KVH=2,T=1024)."""
 import sys, os, math
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import torch
@@ -16,12 +16,6 @@ def timeit(fn, n=20):
     e.record(); torch.cuda.synchronize()
     return s.elapsed_time(e) / n * 1e3
 fl_fwd = 4 * B * H * T * T * 64 / 2
-o, lse = ops.attn_fwd(qkv, B, T, H, KVH, True, scale)
-t = timeit(lambda: ops.attn_fwd(qkv, B, T, H, KVH, True, scale)); print(f"fwd mma.sync {t:8.1f} us {fl_fwd/t/1e6:7.1f} TF/s")
-if hasattr(ops, "attn_tc_fwd"):
-    o2, lse2 = ops.attn_tc_fwd(qkv, B, T, H, KVH, True, scale)
-    print("tc vs warp: max|do|", float((o2.float() - o.float()).abs().max()), "max|dlse|", float((lse2 - lse).abs().max()))
-    t = timeit(lambda: ops.attn_tc_fwd(qkv, B, T, H, KVH, True, scale)); print(f"fwd tcgen05  {t:8.1f} us {fl_fwd/t/1e6:7.1f} TF/s")
-t = timeit(lambda: ops.attn_bwd(qkv, o, d_o, lse, B, T, H, KVH, True, scale)); print(f"bwd mma.sync {t:8.1f} us {2.5*fl_fwd/t/1e6:7.1f} TF/s (5 GEMM-equivalents)")
-if hasattr(ops, "attn_tc_bwd"):
-    t = timeit(lambda: ops.attn_tc_bwd(qkv, o, d_o, lse, B, T, H, KVH, True, scale)); print(f"bwd tcgen05  {t:8.1f} us {2.5*fl_fwd/t/1e6:7.1f} TF/s")
+o, lse = ops.attn_tc_fwd(qkv, B, T, H, KVH, True, scale)
+t = timeit(lambda: ops.attn_tc_fwd(qkv, B, T, H, KVH, True, scale)); print(f"fwd {t:8.1f} us {fl_fwd/t/1e6:7.1f} TF/s")
+t = timeit(lambda: ops.attn_tc_bwd(qkv, o, d_o, lse, B, T, H, KVH, True, scale)); print(f"bwd {t:8.1f} us {2.5*fl_fwd/t/1e6:7.1f} TF/s (5 GEMM-equivalents)")

@@ -44,7 +44,7 @@ def timed(fn, n=20):
     return s.elapsed_time(e) / n * 1e3
 
 
-for ctas in (148, 48):
+for ctas in (lib.sk_device_sm_count(), 48):
     print(f"--- {ctas} stand-in CTAs")
     for name, fn in cases.items():
         for _ in range(3):

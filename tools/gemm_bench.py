@@ -1,4 +1,4 @@
-"""Micro-benchmark of the tcgen05 GEMM on the LM shapes (CUDA events, L2 flushed between iterations).
+"""Micro-benchmark of the wgmma GEMM on the LM shapes (CUDA events, L2 flushed between iterations).
 Prints one line per shape: our TFLOP/s per tile width, and torch.matmul (cuBLAS) for context."""
 import sys, os
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
