@@ -207,6 +207,65 @@ int sk_lm_logits_ld(const SkLm* lm);
 int sk_lm_optimizer_step(SkLm* lm, void* exp_avg, void* exp_avg_sq, float lr, float beta1, float beta2, float eps,
                          float weight_decay, int step, float max_grad_norm, int emulate_bf16_norm, float* stats,
                          void* stream);
+
+/* ---- incremental decoding (TokenLM.generate with a KV cache) -----------------------------------------------------
+ * Replaces HF GenerationMixin's cached greedy / sampling loop behind UnitLM.generate (slamkit/model/unit_lm.py:196-198,
+ * called by SpeechLM.generate, slamkit/model/speech_lm.py:38-55).  sk_lm_decode_step and sk_select_next allocate
+ * nothing, never synchronise and take the same arguments every step (positions, lengths and the step index live in
+ * device memory), so one step can be captured in a CUDA graph and replayed; run one step eagerly before capturing.
+ *
+ * KV cache of all layers, caller-owned: [L][K|V][B][KVH][T_cache][head_dim] bf16, K stored after RoPE. */
+int64_t sk_lm_kv_cache_bytes(const SkLm* lm, int B, int T_cache);
+int64_t sk_lm_decode_workspace_bytes(const SkLm* lm, int B, int T_cache);
+/* ids RIGHT-padded [B,T] (T <= T_cache), lens int32 [B], 1 <= lens[b] <= T real tokens at positions 0..lens[b]-1.  Runs
+ * the forward pass on the bound workspace (sized for [B,T]) without the full-sequence head, copies the K/V of positions
+ * < lens[b] into the cache and writes the bf16 logits of each row's last real token into logits [B, ldl]
+ * (ldl >= sk_lm_logits_ld()).  Also clears the GEMM flag words of decode_ws. */
+int sk_lm_prefill(SkLm* lm, const int64_t* ids, const int32_t* lens, int B, int T, void* kv_cache, int T_cache,
+                  void* logits, int ldl, void* decode_ws, int64_t decode_ws_bytes, void* stream);
+/* One token per row: tokens int64 [B] at positions pos int32 [B] (pos[b] < T_cache): embed, per layer RMSNorm ->
+ * QKV + bias + RoPE GEMM (M = B) -> K/V appended at pos[b] -> decode attention over [0, pos[b]] -> o-proj + residual ->
+ * RMSNorm -> SwiGLU GEMM -> down-proj + residual; final norm, head -> logits [B, ldl]. */
+int sk_lm_decode_step(SkLm* lm, const int64_t* tokens, const int32_t* pos, int B, void* kv_cache, int T_cache,
+                      void* logits, int ldl, void* decode_ws, int64_t decode_ws_bytes, void* stream);
+/* Stand-alone decode attention: o[b, h*64 .. h*64+63] (pitch ldo) = softmax(q k^T * scale) v over keys [0, lens[b]) of
+ * row b; q [B, H*64] pitch ldq; k_cache / v_cache [B][KVH][T_cache][64] bf16.  Flash-decoding over fixed 64-key splits
+ * (one CTA per row, kv head and split serves the H/KVH <= 16 query heads of its group) and a combine pass in split
+ * order: bit-identical run to run, and no key at or past lens[b] is read.  partial: sk_attn_decode_partial_bytes. */
+int64_t sk_attn_decode_partial_bytes(int B, int H, int T_cache);
+int sk_attn_decode(const void* q, int ldq, const void* k_cache, const void* v_cache, const int32_t* lens, void* o, int ldo,
+                   float* partial, int B, int H, int KVH, int T_cache, float scale, void* stream);
+/* Token selection settings (HF GenerationConfig fields). */
+typedef struct SkSampling {
+  uint64_t seed;             /* Philox key of the draws */
+  double top_p;              /* >= 1: off */
+  float temperature;         /* sampling only */
+  int32_t do_sample;         /* 0: greedy (argmax, lowest id on ties; temperature / top-k / top-p unused) */
+  int32_t top_k;             /* <= 0: off */
+  int32_t n_eos;             /* 0..8 */
+  int32_t eos[8];            /* a row finishes after emitting one of these */
+  int32_t pad_token_id;      /* written for rows that have finished */
+  int32_t max_length;        /* a row finishes once prompt + generated tokens reach this length */
+} SkSampling;
+/* Device-resident decode state (pointers to caller-owned device memory). */
+typedef struct SkDecodeState {
+  int64_t* tokens;           /* [B] last token of each row: the next decode step's input */
+  int32_t* pos;              /* [B] its position */
+  int32_t* finished;         /* [B] */
+  int32_t* n_gen;            /* [B] tokens generated */
+  int64_t* out;              /* [B, max_new] generated ids; pad_token_id once a row has finished */
+  int32_t* step;             /* [2] step index and an arrival counter, both zero-initialised */
+  int32_t max_new;
+  int32_t reserved;
+} SkDecodeState;
+/* Selects the next token of every row in HF's order: bans -> (if do_sample) temperature -> top-k (keeps scores >= the
+ * k-th largest) -> top-p (drops the tokens whose ascending cumulative probability is <= 1 - top_p, ties by id, keeps the
+ * most likely one) -> softmax -> inverse-CDF draw in token-id order; greedy: argmax.  ban_bits: uint32 [ceil(V/32)]
+ * bitmask of banned ids or NULL.  uniforms: NULL = Philox4x32-10 keyed by (seed, step, row); else one fp32 uniform in
+ * [0, 1) per row.  Finished rows (or pos[b] + 1 >= max_length) only write pad_token_id.  Otherwise out[b, step],
+ * n_gen[b], tokens[b], pos[b] (+1) and finished[b] (eos) are updated; the step index advances by one per call. */
+int sk_select_next(const void* logits, int ldl, int V, int B, const uint32_t* ban_bits, const SkSampling* cfg,
+                   const float* uniforms, const SkDecodeState* state, void* stream);
 /* ---- HuBERT unit extraction (path (i)) ------------------------------------------------------------------------------
  * One object per device; replaces HubertFeatureExtractor.extract + batch_cluster
  * (slamkit/feature_extractor/hubert_feature_extractor.py:40-50,73-81): F.pad(40,40) -> HF HubertModel conv encoder,

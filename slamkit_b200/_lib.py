@@ -56,6 +56,33 @@ class SkHubertConfig(C.Structure):
     ]
 
 
+class SkSampling(C.Structure):
+    _fields_ = [
+        ("seed", C.c_uint64),
+        ("top_p", C.c_double),
+        ("temperature", C.c_float),
+        ("do_sample", C.c_int32),
+        ("top_k", C.c_int32),
+        ("n_eos", C.c_int32),
+        ("eos", C.c_int32 * 8),
+        ("pad_token_id", C.c_int32),
+        ("max_length", C.c_int32),
+    ]
+
+
+class SkDecodeState(C.Structure):
+    _fields_ = [
+        ("tokens", C.c_void_p),
+        ("pos", C.c_void_p),
+        ("finished", C.c_void_p),
+        ("n_gen", C.c_void_p),
+        ("out", C.c_void_p),
+        ("step", C.c_void_p),
+        ("max_new", C.c_int32),
+        ("reserved", C.c_int32),
+    ]
+
+
 def declared_symbols() -> List[str]:
     """Names of all functions declared in include/slamkit_b200.h (used by the CPU symbol-export test)."""
     text = open(HEADER_PATH).read()
@@ -76,7 +103,8 @@ def load() -> C.CDLL:
     lib = C.CDLL(LIB_PATH)
     lib.sk_last_error.restype = C.c_char_p
     for name in ("sk_lm_param_count", "sk_lm_workspace_bytes", "sk_launch_count", "sk_hubert_param_count", "sk_hubert_prepared_bytes",
-                 "sk_hubert_workspace_bytes", "sk_gemm_ws_bytes"):
+                 "sk_hubert_workspace_bytes", "sk_gemm_ws_bytes", "sk_lm_kv_cache_bytes", "sk_lm_decode_workspace_bytes",
+                 "sk_attn_decode_partial_bytes"):
         if hasattr(lib, name):
             getattr(lib, name).restype = C.c_int64
     for name in ("sk_lm_logits",):

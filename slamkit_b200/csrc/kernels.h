@@ -110,6 +110,21 @@ int sk_attn_tc_bwd_launch(const bf16* qkv, const bf16* o, const bf16* d_o, const
 int sk_attn_tc_fwd_launch(const bf16* qkv, bf16* o, float* lse, int B, int T, int H, int KVH, int ld, int ldo, int causal,
                           float scale, cudaStream_t s, const int* seg_start = nullptr);
 
+// decode.cu: KV cache, decode attention and token selection of incremental decoding (cache layout per layer:
+// [K|V][B][KVH][T_cache][64] bf16)
+int sk_kv_prefill_launch(const bf16* qkv, long layer_stride, int ldq, bf16* cache, const int32_t* lens, int L, int B, int T,
+                         int H, int KVH, int T_cache, cudaStream_t s);
+int sk_kv_append_launch(const bf16* qkv, int ldq, bf16* kc, bf16* vc, const int32_t* pos, int32_t* lens, int B, int H,
+                        int KVH, int T_cache, cudaStream_t s);
+int sk_gather_last_launch(const bf16* x, const int32_t* lens, bf16* out, int B, int T, int D, cudaStream_t s);
+int sk_attn_decode_splits(int T_cache);
+int sk_attn_decode_launch(const bf16* q, int ldq, const bf16* kc, const bf16* vc, const int32_t* lens, bf16* o, int ldo,
+                          float* partial, int B, int H, int KVH, int T_cache, float scale, cudaStream_t s);
+struct SkSampling;
+struct SkDecodeState;
+int sk_select_next_launch(const bf16* logits, int ldl, int V, int B, const uint32_t* ban, const SkSampling& cfg,
+                          const float* uniforms, const SkDecodeState& st, cudaStream_t s);
+
 // hubert_kernels.cu
 int sk_split_f32_launch(const float* x, bf16* hi, bf16* lo, long n, cudaStream_t s);
 extern "C" int sk_conv0_nstat(void);

@@ -315,9 +315,126 @@ int backward_impl(SkLm* lm, const int64_t* ids, const int32_t* pos_ids, int B, i
   return 0;
 }
 
+// byte offsets into the decode workspace for (B, T_cache): one token per row
+struct DecLayout {
+  int64_t gemm, gemm_bytes, x0, x1, h, qkv, ao, gu, act, lens, partial, total;
+};
+
+DecLayout make_dec_layout(const SkLm* lm, int B, int T_cache) {
+  DecLayout w;
+  int64_t cur = 0;
+  auto take = [&](int64_t bytes) {
+    const int64_t o = cur;
+    cur = align_up(cur + bytes, 256);
+    return o;
+  };
+  // GEMM scratch: split-K slabs of the down projection and stream-K partial tiles, flag words in its last 4 KB
+  w.gemm_bytes = align_up((int64_t)sk_gemm_ws_min_bytes(), 256);
+  w.gemm = take(w.gemm_bytes);
+  w.x0 = take((int64_t)B * lm->d * 2);
+  w.x1 = take((int64_t)B * lm->d * 2);
+  w.h = take((int64_t)B * lm->d * 2);
+  w.qkv = take((int64_t)B * lm->qkv_dim * 2);
+  w.ao = take((int64_t)B * lm->d * 2);
+  w.gu = take((int64_t)B * 2 * lm->F * 2);
+  w.act = take((int64_t)B * lm->F * 2);
+  w.lens = take((int64_t)B * 4);
+  w.partial = take(sk_attn_decode_partial_bytes(B, lm->H, T_cache));
+  w.total = cur;
+  return w;
+}
+
+int check_decode(const SkLm* lm, int B, int T_cache, int ldl, const void* kv_cache, const void* logits, const void* ws,
+                 int64_t ws_bytes, const DecLayout& w) {
+  SK_REQUIRE(lm->params && lm->ws, "sk_lm: sk_lm_bind has not been called");
+  SK_REQUIRE(kv_cache && logits && ws, "sk_lm decode: null argument");
+  SK_REQUIRE(B > 0 && T_cache > 0 && T_cache <= lm->cfg.max_positions, "sk_lm decode: bad shape B=%d T_cache=%d (max_positions=%d)",
+             B, T_cache, lm->cfg.max_positions);
+  SK_REQUIRE(ldl >= lm->Vp && ldl % 8 == 0, "sk_lm decode: ldl must be >= %d and a multiple of 8 (got %d)", lm->Vp, ldl);
+  SK_REQUIRE(((uintptr_t)ws & 255) == 0 && ((uintptr_t)kv_cache & 15) == 0 && ((uintptr_t)logits & 15) == 0,
+             "sk_lm decode: decode workspace must be 256-byte, cache and logits 16-byte aligned");
+  SK_REQUIRE(ws_bytes >= w.total, "sk_lm decode: decode workspace too small: need %lld bytes, got %lld", (long long)w.total,
+             (long long)ws_bytes);
+  return 0;
+}
+
 }  // namespace
 
 extern "C" {
+
+int64_t sk_lm_kv_cache_bytes(const SkLm* lm, int B, int T_cache) {
+  if (!lm || B <= 0 || T_cache <= 0) return 0;
+  return (int64_t)lm->L * 2 * B * lm->KVH * T_cache * lm->hd * 2;
+}
+
+int64_t sk_lm_decode_workspace_bytes(const SkLm* lm, int B, int T_cache) {
+  if (!lm || B <= 0 || T_cache <= 0) return 0;
+  return make_dec_layout(lm, B, T_cache).total;
+}
+
+int sk_lm_prefill(SkLm* lm, const int64_t* ids, const int32_t* lens, int B, int T, void* kv_cache, int T_cache,
+                  void* logits, int ldl, void* decode_ws, int64_t decode_ws_bytes, void* stream) {
+  SK_REQUIRE(lm && ids && lens, "sk_lm_prefill: null argument");
+  const DecLayout dl = make_dec_layout(lm, B, T_cache);
+  SK_TRY(check_decode(lm, B, T_cache, ldl, kv_cache, logits, decode_ws, decode_ws_bytes, dl));
+  SK_REQUIRE(T > 0 && T <= T_cache, "sk_lm_prefill: prompt width T=%d must be in [1, T_cache=%d]", T, T_cache);
+  const WsLayout w = make_layout(lm, B, T);
+  SK_TRY(check_bound(lm, B, T, w, nullptr));
+  cudaStream_t s = (cudaStream_t)stream;
+  uint8_t* dws = reinterpret_cast<uint8_t*>(decode_ws);
+  SK_CUDA_CHECK(cudaMemsetAsync(dws + dl.gemm + dl.gemm_bytes - 4096, 0, 4096, s));
+  SK_TRY(forward_impl(lm, ids, nullptr, nullptr, B, T, 0.f, 1.f, false, nullptr, w, s, nullptr, false));
+  SK_TRY(sk_kv_prefill_launch(wsp<bf16>(lm, w.qkv), w.sqkv / 2, lm->qkv_dim, reinterpret_cast<bf16*>(kv_cache), lens, lm->L, B,
+                              T, lm->H, lm->KVH, T_cache, s));
+  bf16* hl = reinterpret_cast<bf16*>(dws + dl.h);
+  SK_TRY(sk_gather_last_launch(wsp<bf16>(lm, w.hf), lens, hl, B, T, lm->d, s));
+  return sk_gemm_launch(B, lm->Vp, lm->d, hl, lm->d, 0, lm->params + lm->off_head, lm->d, 0, logits, ldl, 0, nullptr, nullptr,
+                        0, 0, 0, 0, s);
+}
+
+int sk_lm_decode_step(SkLm* lm, const int64_t* tokens, const int32_t* pos, int B, void* kv_cache, int T_cache,
+                      void* logits, int ldl, void* decode_ws, int64_t decode_ws_bytes, void* stream) {
+  SK_REQUIRE(lm && tokens && pos, "sk_lm_decode_step: null argument");
+  const DecLayout dl = make_dec_layout(lm, B, T_cache);
+  SK_TRY(check_decode(lm, B, T_cache, ldl, kv_cache, logits, decode_ws, decode_ws_bytes, dl));
+  cudaStream_t s = (cudaStream_t)stream;
+  const int d = lm->d, F = lm->F, Q = lm->qkv_dim;
+  const bf16* P = lm->params;
+  uint8_t* dws = reinterpret_cast<uint8_t*>(decode_ws);
+  bf16* x = reinterpret_cast<bf16*>(dws + dl.x0);
+  bf16* xm = reinterpret_cast<bf16*>(dws + dl.x1);
+  bf16* h = reinterpret_cast<bf16*>(dws + dl.h);
+  bf16* qkv = reinterpret_cast<bf16*>(dws + dl.qkv);
+  bf16* ao = reinterpret_cast<bf16*>(dws + dl.ao);
+  bf16* gu = reinterpret_cast<bf16*>(dws + dl.gu);
+  bf16* act = reinterpret_cast<bf16*>(dws + dl.act);
+  int32_t* lens = reinterpret_cast<int32_t*>(dws + dl.lens);
+  float* partial = reinterpret_cast<float*>(dws + dl.partial);
+  void* gemm_ws = dws + dl.gemm;
+  const size_t plane = (size_t)B * lm->KVH * T_cache * lm->hd;
+  const float scale = 1.0f / sqrtf((float)lm->hd);
+  SK_TRY(sk_embed_fwd_launch(tokens, P + lm->off_embed, x, B, d, lm->V, s));
+  for (int l = 0; l < lm->L; ++l) {
+    const LayerOff& o = lm->lo[l];
+    bf16* kc = reinterpret_cast<bf16*>(kv_cache) + (size_t)l * 2 * plane;
+    bf16* vc = kc + plane;
+    SK_TRY(sk_rmsnorm_fwd_launch(x, P + o.ln1, h, nullptr, B, d, lm->cfg.rms_eps, s));
+    SK_TRY(sk_linear_rope_launch(B, Q, d, h, P + o.wqkv, lm->cfg.qkv_bias ? P + o.bqkv : nullptr, qkv, lm->rope_cos,
+                                 lm->rope_sin, pos, 1, (lm->H + lm->KVH) * lm->hd, lm->cfg.max_positions, s));
+    SK_TRY(sk_kv_append_launch(qkv, Q, kc, vc, pos, lens, B, lm->H, lm->KVH, T_cache, s));
+    SK_TRY(sk_attn_decode_launch(qkv, Q, kc, vc, lens, ao, d, partial, B, lm->H, lm->KVH, T_cache, scale, s));
+    SK_TRY(linear_fwd(B, d, d, ao, P + o.wo, xm, nullptr, x, s));
+    SK_TRY(sk_rmsnorm_fwd_launch(xm, P + o.ln2, h, nullptr, B, d, lm->cfg.rms_eps, s));
+    SK_TRY(sk_linear_swiglu_fwd_launch(B, F, d, h, P + o.wgu, gu, act, s));
+    // down projection added in place (residual == output): with M = B there is a single row of output tiles, so the
+    // scratch lets the GEMM split its long K loop over idle SMs (fixed-order reduction)
+    SK_TRY(sk_gemm_launch(B, d, F, act, F, 0, P + o.wd, F, 0, xm, d, 0, nullptr, xm, d, 0, 0, 0, s, gemm_ws,
+                          (size_t)dl.gemm_bytes));
+    std::swap(x, xm);
+  }
+  SK_TRY(sk_rmsnorm_fwd_launch(x, P + lm->off_final_norm, h, nullptr, B, d, lm->cfg.rms_eps, s));
+  return sk_gemm_launch(B, lm->Vp, d, h, d, 0, P + lm->off_head, d, 0, logits, ldl, 0, nullptr, nullptr, 0, 0, 0, 0, s);
+}
 
 int sk_lm_create(const SkLmConfig* cfg, SkLm** out) {
   SK_REQUIRE(cfg && out, "sk_lm_create: null argument");

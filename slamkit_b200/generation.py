@@ -1,17 +1,19 @@
-"""`TokenLM.generate` for the GPU unit LM (slamkit/model/token_lm.py:19-27; `UnitLM.generate` hands the call to HF's
+"""`TokenLM.generate` rules for the GPU unit LM (slamkit/model/token_lm.py:19-27; `UnitLM.generate` hands the call to HF's
 `GenerationMixin.generate`, slamkit/model/unit_lm.py:196-198; callers: `SpeechLM.generate`, slamkit/model/speech_lm.py:38-55,
 with `config/metric/generate.yaml`'s `temperature / top_k / max_new_tokens / do_sample` and `bad_words_ids`).
 
-Decoding is not a hot path of this package (SURVEY.md §2 row 3): there is no KV cache -- every step re-runs the forward
-kernels on the whole prefix of one sequence -- but the interface and the token-selection rules are HF's, so that a model
-trained here can be sampled through the reference's `SpeechLM` without leaving the CUDA path:
+`B200UnitLM.generate` decodes on the device: a prefill pass fills a KV cache, then one batched decode step per token
+(`sk_lm_decode_step`) and on-device token selection (`sk_select_next`), replayed as a CUDA graph.  This module is the
+CPU statement of the rules that path implements, so that a model trained here can be sampled through the reference's
+`SpeechLM` with HF's semantics:
   * decoder-only conventions: prompts arrive LEFT-padded with an `attention_mask` (speech_lm.py:44-45); each row is decoded
-    on its own without the pads (positions start at 0 at the first real token, as HF derives them from the mask) and the
-    result is the padded prompt followed by the continuation, right-padded with `pad_token_id` after `eos_token_id`;
+    without the pads (positions start at 0 at the first real token, as HF derives them from the mask) and the result is
+    the padded prompt followed by the continuation, right-padded with `pad_token_id` after `eos_token_id`;
   * logits processing in HF's order: `bad_words_ids` (single-token entries) -> temperature -> top-k -> top-p -> softmax ->
     multinomial (`do_sample=True`) or argmax.
-`select_next` and `generate_tokens` are pure torch functions of a `next_logits(ids[1,t]) -> [vocab]` callable, which is how
-the CPU tests check them against `transformers`' own `generate` and logits warpers.
+`select_next` and `generate_tokens` are pure torch functions of a `next_logits(ids[1,t]) -> [vocab]` callable (one row at
+a time, no cache), which is how the CPU tests check them against `transformers`' own `generate` and logits warpers and
+how the GPU tests check the device sampler.
 """
 from __future__ import annotations
 
@@ -68,6 +70,20 @@ def _single_token_bans(bad_words_ids) -> List[int]:
                                       "slamkit/model/speech_lm.py:46-48)")
         out.append(int(w[0]))
     return out
+
+
+def ban_bitmask(banned: Sequence[int], vocab_size: int) -> torch.Tensor:
+    """int32 [ceil(V/32)] bitmask of banned ids (bit i % 32 of word i // 32), the form `sk_select_next` takes: one bit per
+    id, so banning every text id of an interleaved 152 k vocabulary costs 19 KB."""
+    n_words = (vocab_size + 31) // 32
+    bits = torch.zeros(n_words * 32, dtype=torch.bool)
+    if len(banned):
+        ids = torch.as_tensor(list(banned), dtype=torch.long)
+        if bool(((ids < 0) | (ids >= vocab_size)).any()):
+            raise ValueError(f"bad_words_ids: ids must be in [0, {vocab_size})")
+        bits[ids] = True
+    words = (bits.view(n_words, 32).long() << torch.arange(32)).sum(1)
+    return torch.where(words >= 2 ** 31, words - 2 ** 32, words).to(torch.int32)
 
 
 def generate_tokens(next_logits: Callable[[torch.Tensor], torch.Tensor], inputs: torch.Tensor,

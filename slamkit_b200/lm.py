@@ -345,9 +345,14 @@ class B200UnitLM:
     @torch.inference_mode()
     def generate(self, inputs: Optional[torch.Tensor] = None, generation_config=None, **kwargs) -> torch.Tensor:
         """TokenLM.generate (slamkit/model/token_lm.py:19-27; UnitLM.generate -> HF GenerationMixin, unit_lm.py:196-198):
-        greedy or sampled continuation of left-padded prompts with HF's logits processing (generation.py).  No KV cache --
-        decoding is not a hot path here -- so every new token re-runs the forward kernels on one sequence's prefix."""
-        from .generation import generate_tokens
+        greedy or sampled continuation of left-padded prompts with HF's logits processing (rules: generation.py).
+
+        All rows decode together on the device: one prefill pass writes the prompts' K/V into a cache, then every new
+        token is one batched decode step plus on-device token selection, captured once as a CUDA graph and replayed.
+        The host looks at the rows' `finished` flags every 16 steps only.  Sampling draws from a Philox stream whose seed
+        comes from `generator` (or torch's default CPU generator), so `torch.manual_seed` makes runs reproducible.
+        Prompt plus continuation is bounded by `max_positions`."""
+        generator = kwargs.pop("generator", None)
         if inputs is None:
             inputs = kwargs.pop("input_ids", None)
         if inputs is None:
@@ -377,14 +382,147 @@ class B200UnitLM:
         opts.setdefault("pad_token_id", self.config.pad_token_id)
         if opts.get("do_sample") and "top_k" not in opts:
             opts["top_k"] = 50                                    # transformers' GenerationConfig default
+        return self._generate_cached(inputs, attention_mask, generator=generator, **opts)
+
+    def _generate_cached(self, inputs: torch.Tensor, attention_mask: Optional[torch.Tensor], max_new_tokens=None,
+                         max_length=None, do_sample=False, temperature=None, top_k=None, top_p=None, eos_token_id=None,
+                         pad_token_id=None, bad_words_ids=None, generator=None) -> torch.Tensor:
+        from .generation import _single_token_bans, ban_bitmask
+        if inputs.dim() != 2:
+            raise ValueError("generate: inputs must be [batch, time]")
+        B, T = inputs.shape
+        if max_new_tokens is None:
+            max_new_tokens = (max_length if max_length is not None else 20) - T      # HF's default: max_length = 20 in total
+        if max_new_tokens < 0:
+            raise ValueError(f"generate: the prompt ({T} tokens) is already longer than max_length={max_length}")
+        eos = [] if eos_token_id is None else ([int(eos_token_id)] if isinstance(eos_token_id, int) else
+                                               [int(e) for e in eos_token_id])
+        eos = sorted(set(eos))
+        if len(eos) > 8:
+            raise NotImplementedError("generate: at most 8 eos_token_id values are supported")
+        if eos and pad_token_id is None:
+            pad_token_id = min(eos)                                   # HF: "Setting pad_token_id to eos_token_id"
+        fill = int(pad_token_id) if pad_token_id is not None else 0
+        banned = _single_token_bans(bad_words_ids)
+        lens = torch.full((B,), T, dtype=torch.long)
+        if attention_mask is not None:
+            m = attention_mask.to("cpu").bool()
+            lens = m.sum(1)
+            left = torch.arange(T)[None, :] >= (T - lens)[:, None]
+            if B and (bool((lens == 0).any()) or not torch.equal(m, left)):
+                raise ValueError("generate: attention_mask must be left-padding (zeros first, then ones) for every row")
+        if B == 0 or max_new_tokens == 0:
+            return inputs.clone()
+        P = self.config.max_positions
+        Lmax = int(lens.max())
+        if Lmax > P:
+            raise L.SkError(f"generate: a prompt of {Lmax} tokens is longer than max_positions = {P}")
+        T_cache = min(Lmax + max_new_tokens, P)
+        # left-padded [B, T] -> right-padded [B, Lmax]: row b's real tokens at positions 0..lens[b]-1
+        cols = torch.arange(Lmax)[None, :]
+        src = ((T - lens)[:, None] + cols).clamp(max=T - 1)
+        ids = torch.where(cols < lens[:, None], inputs.to("cpu").gather(1, src), torch.zeros((), dtype=torch.long))
         V = self.config.vocab_size
+        seed = 0
+        if do_sample:
+            gen = generator if generator is not None else torch.default_generator
+            seed = int(torch.randint(0, 2 ** 62, (1,), generator=gen))
+        cfg = L.SkSampling(seed=seed, top_p=float(top_p) if top_p is not None else 1.0,
+                           temperature=float(temperature) if temperature is not None else 1.0, do_sample=int(bool(do_sample)),
+                           top_k=int(top_k) if top_k else 0, n_eos=len(eos), pad_token_id=fill, max_length=T_cache)
+        for i, e in enumerate(eos):
+            cfg.eos[i] = e
+        if do_sample and cfg.temperature <= 0:
+            raise ValueError("temperature must be > 0")
+        sess = DecodeSession(self, B, T_cache, max_new_tokens, fill)
+        ban = ban_bitmask(banned, V).to(self.device) if banned else None
+        sess.prefill(ids, lens)
+        sess.select(cfg, ban)
+        n_steps = max_new_tokens - 1
+        if n_steps > 0:
+            def step():
+                sess.step()
+                sess.select(cfg, ban)
+            step()                        # eager: sets every one-time kernel attribute before the capture
+            done = 1
+            if done < n_steps and not bool(sess.finished.all()):
+                # captured on a side stream without torch.cuda.graph's gc.collect / empty_cache, which cost more than a
+                # short generation
+                g, cur, side = torch.cuda.CUDAGraph(), torch.cuda.current_stream(), torch.cuda.Stream()
+                side.wait_stream(cur)
+                with torch.cuda.stream(side):
+                    g.capture_begin()
+                    try:
+                        step()
+                    finally:
+                        g.capture_end()
+                cur.wait_stream(side)
+                while done < n_steps:
+                    if done % 16 == 0 and bool(sess.finished.all()):
+                        break
+                    g.replay()
+                    done += 1
+        n_new = int(sess.n_gen.max())
+        out = torch.cat([inputs.to(self.device), sess.out[:, :n_new]], dim=1)
+        return out.to(inputs.device)
 
-        def next_logits(ids: torch.Tensor) -> torch.Tensor:
-            if ids.shape[1] > self.max_seq:
-                raise L.SkError(f"generate: sequence of {ids.shape[1]} tokens exceeds the bound workspace (max_seq = {self.max_seq})")
-            return self.forward(ids).logits[0, -1, :V].float().cpu()
 
-        return generate_tokens(next_logits, inputs, attention_mask=attention_mask, max_positions=self.config.max_positions, **opts)
+class DecodeSession:
+    """Device buffers of one batched incremental decode of a `B200UnitLM`: the KV cache of all layers, the decode
+    workspace, the [B, vocab] logits of the current step and the selection state (`SkDecodeState`).  PyTorch owns the
+    memory; `prefill`, `step` and `select` enqueue `sk_lm_prefill`, `sk_lm_decode_step` and `sk_select_next` on the
+    current stream.  `step` and `select` take the same arguments every call, so they can be captured in a CUDA graph."""
+
+    def __init__(self, model: B200UnitLM, B: int, T_cache: int, max_new: int, pad_token_id: int = 0):
+        self.m, self.B, self.T_cache = model, B, T_cache
+        lib, h, dev = model.lib, model._h, model.device
+        self.ldl = model.vocab_padded
+        self.kv = torch.empty(int(lib.sk_lm_kv_cache_bytes(h, B, T_cache)), device=dev, dtype=torch.uint8)
+        self.ws = torch.empty(int(lib.sk_lm_decode_workspace_bytes(h, B, T_cache)), device=dev, dtype=torch.uint8)
+        self.logits_buf = torch.empty(B, self.ldl, device=dev, dtype=torch.bfloat16)
+        self.tokens = torch.zeros(B, device=dev, dtype=torch.long)
+        self.pos = torch.zeros(B, device=dev, dtype=torch.int32)
+        self.finished = torch.zeros(B, device=dev, dtype=torch.int32)
+        self.n_gen = torch.zeros(B, device=dev, dtype=torch.int32)
+        self.out = torch.full((B, max(max_new, 1)), pad_token_id, device=dev, dtype=torch.long)
+        self.step_ctr = torch.zeros(2, device=dev, dtype=torch.int32)
+        self.state = L.SkDecodeState(self.tokens.data_ptr(), self.pos.data_ptr(), self.finished.data_ptr(),
+                                     self.n_gen.data_ptr(), self.out.data_ptr(), self.step_ctr.data_ptr(), self.out.shape[1], 0)
+
+    @property
+    def logits(self) -> torch.Tensor:
+        """[B, vocab_size] bf16 logits of the last prefill / decode step."""
+        return self.logits_buf[:, :self.m.config.vocab_size]
+
+    def prefill(self, ids: torch.Tensor, lens: torch.Tensor) -> torch.Tensor:
+        """ids: right-padded [B, T] prompts, lens: real tokens per row.  Fills the cache; the next token of row b goes
+        to position lens[b] (its last prompt token, at lens[b] - 1, is the state's current token)."""
+        m = self.m
+        B, T = ids.shape
+        m._ensure(B, T)
+        ids_d = ids.to(m.device, dtype=torch.long).contiguous()
+        lens_d = lens.to(m.device, dtype=torch.int32).contiguous()
+        self.tokens.copy_(ids_d.gather(1, (lens_d.long() - 1).clamp(min=0)[:, None])[:, 0])
+        self.pos.copy_(lens_d - 1)
+        L.check(m.lib.sk_lm_prefill(m._h, L.ptr(ids_d), L.ptr(lens_d), B, T, L.ptr(self.kv), self.T_cache,
+                                    L.ptr(self.logits_buf), self.ldl, L.ptr(self.ws), C.c_int64(self.ws.numel()),
+                                    L.stream_ptr()))
+        return self.logits
+
+    def step(self, tokens: Optional[torch.Tensor] = None, pos: Optional[torch.Tensor] = None) -> torch.Tensor:
+        """One decode step: tokens int64 [B] at positions pos int32 [B] (default: the selection state's)."""
+        m = self.m
+        t = self.tokens if tokens is None else tokens
+        p = self.pos if pos is None else pos
+        L.check(m.lib.sk_lm_decode_step(m._h, L.ptr(t), L.ptr(p), self.B, L.ptr(self.kv), self.T_cache,
+                                        L.ptr(self.logits_buf), self.ldl, L.ptr(self.ws), C.c_int64(self.ws.numel()),
+                                        L.stream_ptr()))
+        return self.logits
+
+    def select(self, cfg: "L.SkSampling", ban: Optional[torch.Tensor] = None, uniforms: Optional[torch.Tensor] = None) -> None:
+        m = self.m
+        L.check(m.lib.sk_select_next(L.ptr(self.logits_buf), self.ldl, m.config.vocab_size, self.B, L.ptr(ban),
+                                     C.byref(cfg), L.ptr(uniforms), C.byref(self.state), L.stream_ptr()))
 
 
 class B200AdamW:
