@@ -55,6 +55,23 @@ int sk_gemm_bf16_ws(int M, int N, int K, const void* A, int lda, int a_mn, const
                     int ldc, int out_f32, const void* bias, const void* residual, int ldr, int round_before_res, int act,
                     int force_bn, void* ws, int64_t ws_bytes, void* stream);
 int64_t sk_gemm_ws_bytes(void);
+/* Test hook: the schedule sk_gemm_bf16_ws would run for these arguments (sk_gemm_bf16 = the same call with ws = NULL),
+ * after the same argument checks.  Nothing is launched and no pointer is dereferenced: only the shapes, the flags,
+ * ws_bytes, which of bias / residual / ws are NULL and whether residual == C matter. */
+typedef struct SkGemmPlan {
+  int32_t bn;                /* tile width: 64, 128 or 256 (tiles are 128 rows) */
+  int32_t epi_warps;         /* 4, or 8 (two per 32-row quadrant) */
+  int32_t splits;            /* > 1: split-K into this many K ranges, fp32 slabs summed by a second kernel */
+  int32_t sk_units;          /* > 0: stream-K over the last sk_units units (rows of tiles, or columns: sk_colunits) */
+  int32_t sk_groups;         /* CTA groups that share the stream-K iteration space (cut into equal K ranges) */
+  int32_t sk_G;              /* tiles per unit = CTAs per group */
+  int32_t sk_colunits;       /* 1: a stream-K unit is a column of tiles (selected by SK_STREAMK=2) */
+  int32_t tma_store;         /* 1: bf16 output through TMA stores; 0: direct stores (fp32 output, split-K slabs) */
+  int32_t grid;              /* CTAs of the GEMM kernel */
+} SkGemmPlan;
+int sk_gemm_plan(int M, int N, int K, const void* A, int lda, int a_mn, const void* B, int ldb, int b_mn, const void* C,
+                 int ldc, int out_f32, const void* bias, const void* residual, int ldr, int round_before_res, int act,
+                 int force_bn, const void* ws, int64_t ws_bytes, SkGemmPlan* plan);
 
 /* Linears of the LM step with the following element-wise op fused into the GEMM epilogue (no extra pass over HBM).
  * sk_linear_swiglu_fwd: gu[M,2F] = x[M,K] * w_gu[2F,K]^T and act[M,F] = bf16(bf16(silu(gate)) * up)  (Qwen2MLP,

@@ -83,6 +83,20 @@ class SkDecodeState(C.Structure):
     ]
 
 
+class SkGemmPlan(C.Structure):
+    _fields_ = [
+        ("bn", C.c_int32),
+        ("epi_warps", C.c_int32),
+        ("splits", C.c_int32),
+        ("sk_units", C.c_int32),
+        ("sk_groups", C.c_int32),
+        ("sk_G", C.c_int32),
+        ("sk_colunits", C.c_int32),
+        ("tma_store", C.c_int32),
+        ("grid", C.c_int32),
+    ]
+
+
 def declared_symbols() -> List[str]:
     """Names of all functions declared in include/slamkit_b200.h (used by the CPU symbol-export test)."""
     text = open(HEADER_PATH).read()

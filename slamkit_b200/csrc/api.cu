@@ -134,6 +134,14 @@ int sk_gemm_bf16_ws(int M, int N, int K, const void* A, int lda, int a_mn, const
                         force_bn, S(stream), ws, (size_t)ws_bytes);
 }
 int64_t sk_gemm_ws_bytes(void) { return (int64_t)sk_gemm_ws_min_bytes(); }
+int sk_gemm_plan(int M, int N, int K, const void* A, int lda, int a_mn, const void* B, int ldb, int b_mn, const void* C,
+                 int ldc, int out_f32, const void* bias, const void* residual, int ldr, int round_before_res, int act,
+                 int force_bn, const void* ws, int64_t ws_bytes, SkGemmPlan* plan) {
+  SK_REQUIRE(plan, "sk_gemm_plan: null plan");
+  return sk_gemm_plan_ex(sk_gemm_desc(M, N, K, A, lda, a_mn, B, ldb, b_mn, const_cast<void*>(C), ldc, out_f32, bias, residual,
+                                      ldr, round_before_res, act, force_bn, const_cast<void*>(ws), (size_t)ws_bytes),
+                         plan);
+}
 int sk_embed_fwd(const int64_t* ids, const void* table, void* out, int M, int D, int V, void* stream) {
   return sk_embed_fwd_launch(ids, CBF(table), BF(out), M, D, V, S(stream));
 }

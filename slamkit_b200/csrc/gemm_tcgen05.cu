@@ -24,6 +24,7 @@
 #include <string.h>
 #include <stdlib.h>
 #include "kernels.h"
+#include "../../include/slamkit_b200.h"
 
 namespace {
 
@@ -901,9 +902,10 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
   }
 }
 
-// C[m,n] = bf16( sum_s ws[s][m][n] ) (+ C when accumulate), fixed summation order -> deterministic split-K
+// C[m,n] = bf16( sum_s ws[s][m][n] (+ C when accumulate) ), fixed summation order -> deterministic split-K; the sum is
+// rounded to bf16 before C is added when round_before_res is set (the same rounding points as the one-pass epilogue)
 __global__ void splitk_reduce_kernel(const float* __restrict__ ws, bf16* __restrict__ C, int M, int N, int ldc, int splits,
-                                     int accumulate) {
+                                     int accumulate, int round_before_res) {
   griddep_launch();
   griddep_wait();
   const long total = (long)M * N / 8;
@@ -924,8 +926,8 @@ __global__ void splitk_reduce_kernel(const float* __restrict__ ws, bf16* __restr
 #pragma unroll
       for (int k = 0; k < 4; ++k) {
         const float2 f = unpack_bf16(ow[k]);
-        acc[2 * k] = bf16_round(acc[2 * k]) + f.x;
-        acc[2 * k + 1] = bf16_round(acc[2 * k + 1]) + f.y;
+        acc[2 * k] = (round_before_res ? bf16_round(acc[2 * k]) : acc[2 * k]) + f.x;
+        acc[2 * k + 1] = (round_before_res ? bf16_round(acc[2 * k + 1]) : acc[2 * k + 1]) + f.y;
       }
     }
     stg128(dst, make_uint4(pack_bf16(acc[0], acc[1]), pack_bf16(acc[2], acc[3]), pack_bf16(acc[4], acc[5]),
@@ -1047,17 +1049,34 @@ int sk_pick_bn(int M, int N, int force_bn) {
   return best;
 }
 
-// General launcher (see SkGemmEx in kernels.h).
-int sk_gemm_ex_launch(const SkGemmEx& g, cudaStream_t stream) {
+namespace {
+
+// Everything the launcher decides before it encodes tensor maps: argument checks, tile width (BN), split-K, TMA-store
+// epilogue, the stream-K partition, epilogue warps (ew) and grid; p receives every kernel parameter.  sk_gemm_ex_launch
+// runs exactly this plan (it only adds the tensor maps); sk_gemm_plan_ex reports it, so tests can tell which schedule ran.
+int plan_gemm(const SkGemmEx& g, GemmParams& p, int& BN, int& ew, int& grid) {
   SK_REQUIRE(g.M > 0 && g.N > 0 && g.K > 0 && g.batch >= 1, "gemm: empty problem M=%d N=%d K=%d batch=%d", g.M, g.N, g.K,
              g.batch);
   SK_REQUIRE(g.N % 8 == 0, "gemm: N must be a multiple of 8 (N=%d)", g.N);
   SK_REQUIRE(g.ldc % 8 == 0 && (g.residual == nullptr || g.ldr % 8 == 0), "gemm: ldc/ldr must be multiples of 8");
   SK_REQUIRE((reinterpret_cast<uintptr_t>(g.C) & 15) == 0, "gemm: C must be 16-byte aligned");
+  SK_REQUIRE(((reinterpret_cast<uintptr_t>(g.A) | reinterpret_cast<uintptr_t>(g.B) | reinterpret_cast<uintptr_t>(g.A_lo) |
+               reinterpret_cast<uintptr_t>(g.B_lo)) & 15) == 0,
+             "gemm: A and B must be 16-byte aligned");
+  SK_REQUIRE((reinterpret_cast<uintptr_t>(g.bias) & 15) == 0 && (reinterpret_cast<uintptr_t>(g.residual) & 15) == 0,
+             "gemm: bias and residual must be 16-byte aligned");
   SK_REQUIRE(g.passes == 1 || (g.passes == 3 && g.A_lo && g.B_lo), "gemm: passes must be 1, or 3 with lo operands");
   const bool use3d = g.a_rows > 0;   // strided-window / batched A view
   SK_REQUIRE(!use3d || !g.a_mn, "gemm: a batched / windowed A operand must be K-major");
   SK_REQUIRE(g.a_mode == 0 || use3d, "gemm: a_mode 1 needs the 3-D A view");
+  // pitches cover the rows they describe (a TMA map would otherwise read the next row's elements as this row's)
+  SK_REQUIRE(use3d || g.lda >= (g.a_mn ? g.M : g.K), "gemm: lda=%d is smaller than the %s of A", g.lda, g.a_mn ? "M" : "K");
+  SK_REQUIRE(g.ldb >= (g.b_mn ? g.N : g.K), "gemm: ldb=%d is smaller than the %s of B", g.ldb, g.b_mn ? "N" : "K");
+  if (g.col_gin == 0) {   // (compacted columns are narrower than N)
+    const int out_cols = g.epi == 2 ? 2 * g.N : g.N;
+    SK_REQUIRE(g.ldc >= out_cols, "gemm: ldc=%d is smaller than the %d output columns", g.ldc, out_cols);
+    SK_REQUIRE(g.residual == nullptr || g.ldr >= g.N, "gemm: ldr=%d is smaller than N=%d", g.ldr, g.N);
+  }
   const int nsm = sk_num_sms();
   // stream-K needs the plain 2-D form and a scratch buffer of sk_gemm_ws_min_bytes() whose last 4 KB (flags) are zero
   static const int sk_env = [] { const char* e = getenv("SK_STREAMK"); return e ? atoi(e) : 1; }();
@@ -1069,28 +1088,8 @@ int sk_gemm_ex_launch(const SkGemmEx& g, cudaStream_t stream) {
                      g.splitk_ws_bytes >= sk_gemm_ws_min_bytes();
   const size_t ws_data_bytes = g.splitk_ws_bytes > SK_FLAG_BYTES ? g.splitk_ws_bytes - SK_FLAG_BYTES : 0;
   // the SwiGLU epilogues need both halves of a [128 gate | 128 up] block in one tile
-  const int BN = (g.a_mode == 1) ? 64 : sk_pick_bn(g.M * g.batch, g.N, (g.epi == 1 || g.epi == 2) ? 256 : g.force_bn);
-  CUtensorMap tm[6];
-  const void* As[2] = {g.A, g.passes == 3 ? g.A_lo : g.A};
-  const void* Bs[2] = {g.B, g.passes == 3 ? g.B_lo : g.B};
-  for (int i = 0; i < 2; ++i) {
-    int rc;
-    CUtensorMap* ta = &tm[i == 0 ? 0 : 2];
-    CUtensorMap* tb = &tm[i == 0 ? 1 : 3];
-    if (use3d) {
-      rc = sk_make_tmap_3d(ta, As[i], (uint64_t)g.a_inner, (uint64_t)g.a_rows, (uint64_t)g.batch, (uint64_t)g.a_row_stride,
-                           (uint64_t)g.a_batch_stride, BM);
-    } else if (!g.a_mn) {
-      rc = sk_make_tmap_2d(ta, As[i], 2, (uint64_t)g.K, (uint64_t)g.M, (uint64_t)g.lda, BK, BM);
-    } else {
-      rc = sk_make_tmap_2d(ta, As[i], 2, (uint64_t)g.M, (uint64_t)g.K, (uint64_t)g.lda, 64, BK);
-    }
-    if (rc) return rc;
-    if (!g.b_mn) rc = sk_make_tmap_2d(tb, Bs[i], 2, (uint64_t)g.K, (uint64_t)g.N, (uint64_t)g.ldb, BK, (uint32_t)BN);
-    else         rc = sk_make_tmap_2d(tb, Bs[i], 2, (uint64_t)g.N, (uint64_t)g.K, (uint64_t)g.ldb, 64, BK);
-    if (rc) return rc;
-  }
-  GemmParams p;
+  BN = (g.a_mode == 1) ? 64 : sk_pick_bn(g.M * g.batch, g.N, (g.epi == 1 || g.epi == 2) ? 256 : g.force_bn);
+  memset(&p, 0, sizeof(p));
   p.M = g.M; p.N = g.N; p.K = g.K;
   p.batch = g.batch;
   p.a_mode = (g.a_mode & 1) | (use3d ? 2 : 0);   // bit 1: A uses the 3-D TMA form
@@ -1130,15 +1129,8 @@ int sk_gemm_ex_launch(const SkGemmEx& g, cudaStream_t stream) {
     }
   }
   // TMA-store epilogue for the plain bf16 outputs (everything on the LM path)
-  p.tma_store = 0;
-  tm[4] = tm[0];
-  if (!g.out_f32 && !g.C_lo && g.col_gin == 0 && p.splits == 1 && g.batch == 1 && !use3d && (g.ldc * 2) % 16 == 0) {
-    // epi 2 writes d_gu [M, 2N] (the accumulator tile is d_act [M, N])
-    const int rc2 = sk_make_tmap_2d(&tm[4], g.C, 2, (uint64_t)(g.epi == 2 ? 2 * g.N : g.N), (uint64_t)g.M, (uint64_t)g.ldc, 64, 32);
-    if (rc2) return rc2;
-    p.tma_store = 1;
-  }
-  tm[5] = tm[4];
+  p.tma_store = (!g.out_f32 && !g.C_lo && g.col_gin == 0 && p.splits == 1 && g.batch == 1 && !use3d && (g.ldc * 2) % 16 == 0)
+                    ? 1 : 0;
   p.epi = g.epi;
   p.aux = reinterpret_cast<const bf16*>(g.aux);
   p.ld_aux = g.ld_aux;
@@ -1152,8 +1144,6 @@ int sk_gemm_ex_launch(const SkGemmEx& g, cudaStream_t stream) {
     if (g.epi == 1) {
       SK_REQUIRE(BN == 256 && g.N % 256 == 0 && g.aux_out && g.ld_aux_out % 8 == 0 && !g.bias,
                  "gemm: SwiGLU-forward epilogue needs N = 2F with F %% 128 == 0 and an act output");
-      const int rc3 = sk_make_tmap_2d(&tm[5], g.aux_out, 2, (uint64_t)g.N / 2, (uint64_t)g.M, (uint64_t)g.ld_aux_out, 64, 32);
-      if (rc3) return rc3;
     } else if (g.epi == 2) {
       SK_REQUIRE(BN == 256 && g.N % 128 == 0 && g.aux && g.ld_aux % 8 == 0 && !g.bias,
                  "gemm: SwiGLU-backward epilogue needs N = F with F %% 128 == 0 and the saved gu activation");
@@ -1166,14 +1156,7 @@ int sk_gemm_ex_launch(const SkGemmEx& g, cudaStream_t stream) {
     }
   }
   // stream-K over the units (rows or columns of tiles) of the last, partial wave -- see WorkIter
-  p.sk_units = 0;
-  p.sk_groups = 0;
   p.sk_G = 1;
-  p.sk_colunits = 0;
-  p.units = 0;
-  p.n_groups = 0;
-  p.sk_ws = nullptr;
-  p.sk_flags = nullptr;
   if (sk_ok && BN == 256 && p.splits == 1 && num_kb >= sk_min_kb && (p.tiles_n <= 8 || (sk_env >= 2 && p.tiles_m <= 8))) {
     const int colunits = p.tiles_n <= 8 ? 0 : 1;
     const int G = colunits ? p.tiles_m : p.tiles_n;
@@ -1193,17 +1176,77 @@ int sk_gemm_ex_launch(const SkGemmEx& g, cudaStream_t stream) {
     }
   }
   const long work = tiles * p.splits;
-  const int grid = p.sk_units > 0 ? p.n_groups * p.sk_G : (int)(work < nsm ? work : nsm);
+  grid = p.sk_units > 0 ? p.n_groups * p.sk_G : (int)(work < nsm ? work : nsm);
+  // 8 epilogue warps (two per 32-row quadrant) where the epilogue does real work per element; the plain
+  // convert-and-store epilogue is faster with 4 (fewer warps contending with the TMA / MMA issue threads)
+  static const int ew_env = [] { const char* e = getenv("SK_GEMM_EW"); return e ? atoi(e) : 0; }();
+  ew = (p.sk_units == 0 && BN == 256 && p.tma_store && (ew_env == 8 || (ew_env == 0 && (g.epi == 2 || g.epi == 3)))) ? 8 : 4;
+  return 0;
+}
+
+}  // namespace
+
+int sk_gemm_plan_ex(const SkGemmEx& g, SkGemmPlan* out) {
+  GemmParams p;
+  int BN = 0, ew = 0, grid = 0;
+  const int rc = plan_gemm(g, p, BN, ew, grid);
+  if (rc) return rc;
+  out->bn = BN;
+  out->epi_warps = ew;
+  out->splits = p.splits;
+  out->sk_units = p.sk_units;
+  out->sk_groups = p.sk_groups;
+  out->sk_G = p.sk_G;
+  out->sk_colunits = p.sk_colunits;
+  out->tma_store = p.tma_store;
+  out->grid = grid;
+  return 0;
+}
+
+// General launcher (see SkGemmEx in kernels.h).
+int sk_gemm_ex_launch(const SkGemmEx& g, cudaStream_t stream) {
+  GemmParams p;
+  int BN = 0, ew = 0, grid = 0;
+  const int rc0 = plan_gemm(g, p, BN, ew, grid);
+  if (rc0) return rc0;
+  const bool use3d = g.a_rows > 0;
+  CUtensorMap tm[6];
+  const void* As[2] = {g.A, g.passes == 3 ? g.A_lo : g.A};
+  const void* Bs[2] = {g.B, g.passes == 3 ? g.B_lo : g.B};
+  for (int i = 0; i < 2; ++i) {
+    int rc;
+    CUtensorMap* ta = &tm[i == 0 ? 0 : 2];
+    CUtensorMap* tb = &tm[i == 0 ? 1 : 3];
+    if (use3d) {
+      rc = sk_make_tmap_3d(ta, As[i], (uint64_t)g.a_inner, (uint64_t)g.a_rows, (uint64_t)g.batch, (uint64_t)g.a_row_stride,
+                           (uint64_t)g.a_batch_stride, BM);
+    } else if (!g.a_mn) {
+      rc = sk_make_tmap_2d(ta, As[i], 2, (uint64_t)g.K, (uint64_t)g.M, (uint64_t)g.lda, BK, BM);
+    } else {
+      rc = sk_make_tmap_2d(ta, As[i], 2, (uint64_t)g.M, (uint64_t)g.K, (uint64_t)g.lda, 64, BK);
+    }
+    if (rc) return rc;
+    if (!g.b_mn) rc = sk_make_tmap_2d(tb, Bs[i], 2, (uint64_t)g.K, (uint64_t)g.N, (uint64_t)g.ldb, BK, (uint32_t)BN);
+    else         rc = sk_make_tmap_2d(tb, Bs[i], 2, (uint64_t)g.N, (uint64_t)g.K, (uint64_t)g.ldb, 64, BK);
+    if (rc) return rc;
+  }
+  tm[4] = tm[0];
+  if (p.tma_store) {
+    // epi 2 writes d_gu [M, 2N] (the accumulator tile is d_act [M, N])
+    const int rc2 = sk_make_tmap_2d(&tm[4], g.C, 2, (uint64_t)(g.epi == 2 ? 2 * g.N : g.N), (uint64_t)g.M, (uint64_t)g.ldc, 64, 32);
+    if (rc2) return rc2;
+  }
+  tm[5] = tm[4];
+  if (g.epi == 1) {
+    const int rc3 = sk_make_tmap_2d(&tm[5], g.aux_out, 2, (uint64_t)g.N / 2, (uint64_t)g.M, (uint64_t)g.ld_aux_out, 64, 32);
+    if (rc3) return rc3;
+  }
   int rc;
   if (p.sk_units > 0) {
     rc = dispatch_major<256, true>(g.a_mn, g.b_mn, tm, p, grid, stream);
+  } else if (ew == 8) {
+    rc = dispatch_major<256, false, 8>(g.a_mn, g.b_mn, tm, p, grid, stream);
   } else {
-    // 8 epilogue warps (two per 32-row quadrant) where the epilogue does real work per element; the plain
-    // convert-and-store epilogue is faster with 4 (fewer warps contending with the TMA / MMA issue threads)
-    static const int ew_env = [] { const char* e = getenv("SK_GEMM_EW"); return e ? atoi(e) : 0; }();
-    const bool ew8 = BN == 256 && p.tma_store && (ew_env == 8 || (ew_env == 0 && (g.epi == 2 || g.epi == 3)));
-    if (ew8) rc = dispatch_major<256, false, 8>(g.a_mn, g.b_mn, tm, p, grid, stream);
-    else
     switch (BN) {
       case 256: rc = dispatch_major<256, false>(g.a_mn, g.b_mn, tm, p, grid, stream); break;
       case 128: rc = dispatch_major<128, false>(g.a_mn, g.b_mn, tm, p, grid, stream); break;
@@ -1216,10 +1259,10 @@ int sk_gemm_ex_launch(const SkGemmEx& g, cudaStream_t stream) {
     SK_REQUIRE(g.residual == nullptr || g.residual == g.C, "gemm: split-K supports only in-place accumulation");
     const long n8 = (long)g.M * g.N / 8;
     int blocks = (int)((n8 + 255) / 256);
-    if (blocks > nsm * 8) blocks = nsm * 8;
+    if (blocks > sk_num_sms() * 8) blocks = sk_num_sms() * 8;
     sk_prof_begin(0, stream);
     SK_CUDA_CHECK(sk_launch_pdl(splitk_reduce_kernel, dim3(blocks), dim3(256), (size_t)(0), stream, p.splitk_ws, reinterpret_cast<bf16*>(g.C), g.M, g.N, g.ldc, p.splits,
-                                                     g.residual != nullptr));
+                                                     g.residual != nullptr, g.round_before_res));
     sk_prof_end(stream);
     SK_LAUNCH_CHECK();
   }
@@ -1228,9 +1271,9 @@ int sk_gemm_ex_launch(const SkGemmEx& g, cudaStream_t stream) {
 
 // Plain entry point.  A: [M,K] (a_mn=0, lda = row pitch of the [M,K] array) or stored [K,M] (a_mn=1, lda = row pitch of
 // the [K,M] array).  B: [N,K] (b_mn=0) or stored [K,N] (b_mn=1).
-int sk_gemm_launch(int M, int N, int K, const void* A, int lda, int a_mn, const void* B, int ldb, int b_mn, void* C,
-                   int ldc, int out_f32, const void* bias, const void* residual, int ldr, int round_before_res, int act,
-                   int force_bn, cudaStream_t stream, void* splitk_ws, size_t splitk_ws_bytes) {
+SkGemmEx sk_gemm_desc(int M, int N, int K, const void* A, int lda, int a_mn, const void* B, int ldb, int b_mn, void* C,
+                      int ldc, int out_f32, const void* bias, const void* residual, int ldr, int round_before_res, int act,
+                      int force_bn, void* splitk_ws, size_t splitk_ws_bytes) {
   SkGemmEx g;
   memset(&g, 0, sizeof(g));
   g.M = M; g.N = N; g.K = K; g.batch = 1; g.passes = 1;
@@ -1242,7 +1285,14 @@ int sk_gemm_launch(int M, int N, int K, const void* A, int lda, int a_mn, const 
   g.pdl = 1;
   g.splitk_ws = splitk_ws;
   g.splitk_ws_bytes = splitk_ws_bytes;
-  return sk_gemm_ex_launch(g, stream);
+  return g;
+}
+int sk_gemm_launch(int M, int N, int K, const void* A, int lda, int a_mn, const void* B, int ldb, int b_mn, void* C,
+                   int ldc, int out_f32, const void* bias, const void* residual, int ldr, int round_before_res, int act,
+                   int force_bn, cudaStream_t stream, void* splitk_ws, size_t splitk_ws_bytes) {
+  return sk_gemm_ex_launch(sk_gemm_desc(M, N, K, A, lda, a_mn, B, ldb, b_mn, C, ldc, out_f32, bias, residual, ldr,
+                                        round_before_res, act, force_bn, splitk_ws, splitk_ws_bytes),
+                           stream);
 }
 
 // ---- fused linears of the LM step (SkGemmEx::epi) ------------------------------------------------------------------

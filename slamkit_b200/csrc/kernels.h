@@ -49,9 +49,15 @@ struct SkGemmEx {
   int rope_T, rope_cols, rope_maxpos;
 };
 int sk_gemm_ex_launch(const SkGemmEx& g, cudaStream_t stream);
+struct SkGemmPlan;
+int sk_gemm_plan_ex(const SkGemmEx& g, SkGemmPlan* out);   // the decisions sk_gemm_ex_launch makes for g, nothing launched
 int sk_gemm_launch(int M, int N, int K, const void* A, int lda, int a_mn, const void* B, int ldb, int b_mn, void* C,
                    int ldc, int out_f32, const void* bias, const void* residual, int ldr, int round_before_res, int act,
                    int force_bn, cudaStream_t stream, void* splitk_ws = nullptr, size_t splitk_ws_bytes = 0);
+// the SkGemmEx that sk_gemm_launch runs
+SkGemmEx sk_gemm_desc(int M, int N, int K, const void* A, int lda, int a_mn, const void* B, int ldb, int b_mn, void* C,
+                      int ldc, int out_f32, const void* bias, const void* residual, int ldr, int round_before_res, int act,
+                      int force_bn, void* splitk_ws, size_t splitk_ws_bytes);
 int sk_linear_swiglu_fwd_launch(int M, int F, int K, const void* x, const void* Wgu, void* gu, void* act, cudaStream_t s);
 int sk_linear_swiglu_bwd_launch(int M, int N, int F, const void* dy, const void* Wd, const void* gu, void* dgu, cudaStream_t s);
 int sk_linear_rope_launch(int M, int N, int K, const void* x, const void* W, const void* bias, void* out, const void* cos_t,

@@ -427,8 +427,9 @@ int sk_lm_decode_step(SkLm* lm, const int64_t* tokens, const int32_t* pos, int B
     SK_TRY(sk_rmsnorm_fwd_launch(xm, P + o.ln2, h, nullptr, B, d, lm->cfg.rms_eps, s));
     SK_TRY(sk_linear_swiglu_fwd_launch(B, F, d, h, P + o.wgu, gu, act, s));
     // down projection added in place (residual == output): with M = B there is a single row of output tiles, so the
-    // scratch lets the GEMM split its long K loop over idle SMs (fixed-order reduction)
-    SK_TRY(sk_gemm_launch(B, d, F, act, F, 0, P + o.wd, F, 0, xm, d, 0, nullptr, xm, d, 0, 0, 0, s, gemm_ws,
+    // scratch lets the GEMM split its long K loop over idle SMs (fixed-order reduction); rounded before the residual
+    // add like the forward pass's down projection
+    SK_TRY(sk_gemm_launch(B, d, F, act, F, 0, P + o.wd, F, 0, xm, d, 0, nullptr, xm, d, 1, 0, 0, s, gemm_ws,
                           (size_t)dl.gemm_bytes));
     std::swap(x, xm);
   }

@@ -31,33 +31,57 @@ def gemm_workspace(device) -> torch.Tensor:
     return _gemm_ws[key]
 
 
-def gemm(a: torch.Tensor, b: torch.Tensor, *, a_mn: bool = False, b_mn: bool = False,
-         bias: Optional[torch.Tensor] = None, residual: Optional[torch.Tensor] = None,
-         out: Optional[torch.Tensor] = None, out_f32: bool = False, round_before_res: bool = False,
-         act: int = 0, force_bn: int = 0, streamk: bool = False) -> torch.Tensor:
-    """C = A @ B^T (+bias) (+residual).  a: [M,K] (or [K,M] if a_mn); b: [N,K] (or [K,N] if b_mn).
-    streamk=True hands the kernel the per-device scratch (sk_gemm_bf16_ws: stream-K balancing, 224-wide tiles)."""
-    lib = L.require_cuda()
+def _gemm_args(a, b, a_mn, b_mn, bias, residual, out, out_f32, round_before_res, act, force_bn):
+    """Leading arguments of sk_gemm_bf16 / sk_gemm_bf16_ws / sk_gemm_plan (M .. force_bn); out may be None (plan only)."""
     _bf16(a), _bf16(b)
     assert a.dim() == 2 and b.dim() == 2 and a.stride(1) == 1 and b.stride(1) == 1
     M, K = (a.shape[1], a.shape[0]) if a_mn else (a.shape[0], a.shape[1])
     N, Kb = (b.shape[1], b.shape[0]) if b_mn else (b.shape[0], b.shape[1])
     assert K == Kb, f"contraction mismatch {K} vs {Kb}"
+    assert out is None or out.stride(1) == 1
+    return (M, N, K, L.ptr(a), a.stride(0), int(a_mn), L.ptr(b), b.stride(0), int(b_mn), L.ptr(out),
+            out.stride(0) if out is not None else N, int(out_f32), L.ptr(bias), L.ptr(residual),
+            residual.stride(0) if residual is not None else 0, int(round_before_res), act, force_bn)
+
+
+def gemm(a: torch.Tensor, b: torch.Tensor, *, a_mn: bool = False, b_mn: bool = False,
+         bias: Optional[torch.Tensor] = None, residual: Optional[torch.Tensor] = None,
+         out: Optional[torch.Tensor] = None, out_f32: bool = False, round_before_res: bool = False,
+         act: int = 0, force_bn: int = 0, streamk: bool = False) -> torch.Tensor:
+    """C = A @ B^T (+bias) (+residual).  a: [M,K] (or [K,M] if a_mn); b: [N,K] (or [K,N] if b_mn).
+    streamk=True hands the kernel the per-device scratch (sk_gemm_bf16_ws: split-K for few tiles and a long K loop,
+    stream-K balancing for a partial last wave)."""
+    lib = L.require_cuda()
     if out is None:
+        M = a.shape[1] if a_mn else a.shape[0]
+        N = b.shape[1] if b_mn else b.shape[0]
         out = torch.empty((M, N), device=a.device, dtype=torch.float32 if out_f32 else torch.bfloat16)
-    assert out.stride(1) == 1
+    M, N, K, pa, lda, am, pb, ldb, bm, pc, ldc, f32, pbias, pres, ldr, rbr, act, fbn = _gemm_args(
+        a, b, a_mn, b_mn, bias, residual, out, out_f32, round_before_res, act, force_bn)
     if streamk:
         ws = gemm_workspace(a.device)
-        L.check(lib.sk_gemm_bf16_ws(M, N, K, L.ptr(a), a.stride(0), int(a_mn), L.ptr(b), b.stride(0), int(b_mn),
-                                    L.ptr(out), out.stride(0), int(out_f32), L.ptr(bias), L.ptr(residual),
-                                    residual.stride(0) if residual is not None else 0, int(round_before_res), act,
-                                    force_bn, L.ptr(ws), C.c_int64(ws.numel()), L.stream_ptr()))
+        L.check(lib.sk_gemm_bf16_ws(M, N, K, pa, lda, am, pb, ldb, bm, pc, ldc, f32, pbias, pres, ldr, rbr, act, fbn,
+                                    L.ptr(ws), C.c_int64(ws.numel()), L.stream_ptr()))
         return out
-    L.check(lib.sk_gemm_bf16(M, N, K, L.ptr(a), a.stride(0), int(a_mn), L.ptr(b), b.stride(0), int(b_mn), L.ptr(out),
-                             out.stride(0), int(out_f32), L.ptr(bias), L.ptr(residual),
-                             residual.stride(0) if residual is not None else 0, int(round_before_res), act, force_bn,
+    L.check(lib.sk_gemm_bf16(M, N, K, pa, lda, am, pb, ldb, bm, pc, ldc, f32, pbias, pres, ldr, rbr, act, fbn,
                              L.stream_ptr()))
     return out
+
+
+def gemm_plan(a: torch.Tensor, b: torch.Tensor, *, a_mn: bool = False, b_mn: bool = False,
+              bias: Optional[torch.Tensor] = None, residual: Optional[torch.Tensor] = None,
+              out: Optional[torch.Tensor] = None, out_f32: bool = False, round_before_res: bool = False,
+              act: int = 0, force_bn: int = 0, streamk: bool = False) -> dict:
+    """The schedule gemm() runs for the same arguments (sk_gemm_plan): bn, epi_warps, splits, sk_units, sk_groups,
+    sk_G, sk_colunits, tma_store, grid.  Nothing is launched.  Pass `out` when it matters (residual is out, pitch)."""
+    lib = L.require_cuda()
+    M, N, K, pa, lda, am, pb, ldb, bm, pc, ldc, f32, pbias, pres, ldr, rbr, act, fbn = _gemm_args(
+        a, b, a_mn, b_mn, bias, residual, out, out_f32, round_before_res, act, force_bn)
+    ws = gemm_workspace(a.device) if streamk else None
+    plan = L.SkGemmPlan()
+    L.check(lib.sk_gemm_plan(M, N, K, pa, lda, am, pb, ldb, bm, pc, ldc, f32, pbias, pres, ldr, rbr, act, fbn, L.ptr(ws),
+                             C.c_int64(ws.numel() if ws is not None else 0), C.byref(plan)))
+    return {name: int(getattr(plan, name)) for name, _ in L.SkGemmPlan._fields_}
 
 
 def gemm_splitk(a: torch.Tensor, b: torch.Tensor, out: torch.Tensor, *, a_mn: bool, b_mn: bool, accumulate: bool,

@@ -86,19 +86,25 @@ def test_gemm_splitk_wgrad(M, N, K, acc):
 
 
 @pytest.mark.parametrize("a_mn,b_mn", [(False, False), (False, True), (True, False), (True, True)])
-@pytest.mark.parametrize("M,N,K,bn", [(2048, 896, 2048, 0), (4224, 1152, 2048, 0), (2560, 896, 4096, 256),
-                                       (2000, 1000, 2304, 256), (640, 4864, 2048, 256), (2048, 896, 2048, 128),
-                                       (1152, 896, 4096, 0), (9728, 896, 2048, 0)])
+@pytest.mark.parametrize("M,N,K,bn", [(5064, 896, 2056, 0), (4224, 1152, 2048, 0), (2560, 896, 4096, 256),
+                                       (3000, 1000, 2304, 256), (4160, 1480, 2056, 256), (6000, 1000, 3000, 256),
+                                       (4104, 2048, 2104, 0), (9728, 896, 2048, 0)])
 def test_gemm_streamk(M, N, K, bn, a_mn, b_mn):
     """Stream-K balancing (sk_gemm_bf16_ws): partial tiles meet in the scratch, fixed-order fix-up -> same result every
-    launch; all four operand layouts, ragged M / N edges, many and few contributors per tile."""
+    launch; all four operand layouts, ragged M / N / K edges, one to four contributors per tile, a single split unit.
+    Every shape is checked to run stream-K (on 132 SMs)."""
     from slamkit_b200 import ops
-    a, b = _randn(M, K, seed=21), _randn(N, K, seed=22)
-    ref = a.float() @ b.float().t()
-    a_dev = a.t().contiguous().to(DEV) if a_mn else a.to(DEV)
-    b_dev = b.t().contiguous().to(DEV) if b_mn else b.to(DEV)
+    import gemm_ref as R
+    a, b = _randn(M, K, seed=21).to(DEV), _randn(N, K, seed=22).to(DEV)
+    a_dev = a.t().contiguous() if a_mn else a
+    b_dev = b.t().contiguous() if b_mn else b
+    plan = ops.gemm_plan(a_dev, b_dev, a_mn=a_mn, b_mn=b_mn, force_bn=bn, streamk=True)
+    assert R.schedule_kind(plan, K) in ("streamk1", "streamk2"), plan
     out = ops.gemm(a_dev, b_dev, a_mn=a_mn, b_mn=b_mn, force_bn=bn, streamk=True)
-    assert rel_err(out.cpu(), ref) < 4e-3, (M, N, K, bn, rel_err(out.cpu(), ref))
+    ref = a.float() @ b.float().t()
+    assert rel_err(out, ref) < 4e-3, (M, N, K, bn, rel_err(out, ref))
+    rep = R.mismatch_random(out, a, b, plan["bn"])
+    assert rep is None, rep
     for _ in range(3):   # flags re-armed by the kernel; bit-identical
         out2 = ops.gemm(a_dev, b_dev, a_mn=a_mn, b_mn=b_mn, force_bn=bn, streamk=True)
         assert torch.equal(out, out2)
@@ -106,12 +112,17 @@ def test_gemm_streamk(M, N, K, bn, a_mn, b_mn):
 
 
 def test_gemm_streamk_epilogues():
+    """Bias + residual, fp32 output (the direct-store fix-up), GELU and in-place accumulation under stream-K."""
     from slamkit_b200 import ops
-    M, N, K = 2048, 896, 2048
+    import gemm_ref as R
+    M, N, K = 5120, 896, 2048
     a, b = _randn(M, K, seed=5), _randn(N, K, seed=6)
     bias, res = _randn(N, seed=7), _randn(M, N, seed=8)
     acc = a.float() @ b.float().t()
     ad, bd = a.to(DEV), b.to(DEV)
+    r = res.to(DEV)
+    for kw in (dict(bias=bias.to(DEV), residual=r), dict(out_f32=True), dict(bias=bias.to(DEV), act=1), dict(residual=r, out=r)):
+        assert R.schedule_kind(ops.gemm_plan(ad, bd, streamk=True, **kw), K) == "streamk2"
     out = ops.gemm(ad, bd, bias=bias.to(DEV), residual=res.to(DEV), round_before_res=True, streamk=True).cpu()
     ref = ((acc + bias.float()).to(torch.bfloat16).float() + res.float())
     assert rel_err(out, ref) < 4e-3
