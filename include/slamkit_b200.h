@@ -283,6 +283,26 @@ typedef struct SkDecodeState {
  * n_gen[b], tokens[b], pos[b] (+1) and finished[b] (eos) are updated; the step index advances by one per call. */
 int sk_select_next(const void* logits, int ldl, int V, int B, const uint32_t* ban_bits, const SkSampling* cfg,
                    const float* uniforms, const SkDecodeState* state, void* stream);
+
+/* ---- sequence scoring (modelling metrics of cli/eval.py) ---------------------------------------------------------------
+ * The tail of UnitLM.log_likelihood (slamkit/model/unit_lm.py:184-194 -> calc_nll, slamkit/utils/calculation_utils.py:5-29)
+ * with the bf16 model's rounding: for logits z bf16 [B*T, ldl] (V valid columns; e.g. sk_lm_logits after sk_lm_forward with
+ * labels = NULL) and tokens ids int64 [B,T], target y = ids[b, t+1] of logits row b*T + t:
+ *   banned columns (ban_bits: uint32 [ceil(V/32)] bitmask as for sk_select_next, or NULL) are -inf;
+ *   y == pad_id is masked: value 0, not counted, its logits row is not read;
+ *   token_nll[b, t] = -bf16((z_y - max) - log(sum exp(z - max))) with fp32 max / sum over the non-banned columns
+ *                     (+inf for a banned target);
+ *   ll_out[b] (bf16) = -bf16(sum_t token_nll[b, t]), or with mean_nll -bf16(bf16(sum) / count) (NaN when count = 0).
+ * Every logits element of an unmasked row is read once; columns >= V are never read.  token_nll: fp32 [B, T-1],
+ * caller-owned (the per-sequence pass sums it in a fixed order).  No atomics: bit-identical run to run.  V in [2, 2^20],
+ * ldl % 8 == 0, logits 16-byte aligned. */
+int sk_seq_loglik(const void* logits, int ldl, int V, const int64_t* ids, int B, int T, int pad_id, const uint32_t* ban_bits,
+                  int mean_nll, float* token_nll, void* ll_out, void* stream);
+/* UnitTokeniser.tokenise on the device (slamkit/tokeniser/unit_tokeniser.py:40-73 with its `<S> $0 <S>` template): sk_rle's
+ * units int32 [B, T_units] and counts int32 [B] -> right-padded ids int64 [B, T_out] = [bos, units + offset..., eos, pad...].
+ * T_out = max(counts) + 2 gives the batch tokenise() builds. */
+int sk_units_to_tokens(const int32_t* units, const int32_t* counts, int B, int T_units, int offset, int bos, int eos, int pad,
+                       int64_t* ids, int T_out, void* stream);
 /* ---- HuBERT unit extraction (path (i)) ------------------------------------------------------------------------------
  * One object per device; replaces HubertFeatureExtractor.extract + batch_cluster
  * (slamkit/feature_extractor/hubert_feature_extractor.py:40-50,73-81): F.pad(40,40) -> HF HubertModel conv encoder,

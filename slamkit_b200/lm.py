@@ -342,6 +342,62 @@ class B200UnitLM:
         ll = tok.sum(-1)
         return ll / mask.sum(-1) if mean_nll else ll
 
+    def _ban_bits(self, ignore_tokens) -> Optional[torch.Tensor]:
+        """Device bitmask (`generation.ban_bitmask` layout) of an ignore list, built once per distinct list."""
+        if ignore_tokens is None:
+            return None
+        key = tuple(int(i) for i in ignore_tokens)
+        cache = self.__dict__.setdefault("_ban_cache", {})
+        bits = cache.get(key)
+        if bits is None:
+            V = self.config.vocab_size
+            ids = torch.as_tensor(key, dtype=torch.long).to(self.device)
+            if ids.numel() and bool(((ids < 0) | (ids >= V)).any()):
+                raise ValueError(f"ignore_tokens: ids must be in [0, {V})")
+            flags = torch.zeros((V + 31) // 32 * 32, dtype=torch.int64, device=self.device)
+            flags[ids] = 1
+            words = (flags.view(-1, 32) << torch.arange(32, device=self.device)).sum(1)
+            bits = torch.where(words >= 2 ** 31, words - 2 ** 32, words).to(torch.int32)
+            if len(cache) >= 4:
+                cache.pop(next(iter(cache)))
+            cache[key] = bits
+        return bits
+
+    @torch.inference_mode()
+    def sequence_log_likelihood(self, tokens: torch.Tensor, mean_nll: bool, ignore_tokens=None,
+                                attention_mask: Optional[torch.Tensor] = None,
+                                return_token_nll: bool = False):
+        """`UnitLM.log_likelihood` of the bf16 reference model (slamkit/model/unit_lm.py:184-194): bf16 [B] per-sequence
+        (mean or summed) log-likelihood on the device, with the reference's bf16 rounding of each token's log-prob, of the
+        sum and of the mean (the metric's 0.5 tie rule sees those roundings).  One forward pass, then `sk_seq_loglik` reads
+        the bf16 logits once; no fp32 copy of the logits is made.  Targets equal to the model's pad id are masked;
+        `ignore_tokens` are -inf columns.  With `return_token_nll`, also returns the fp32 [B, T-1] per-token values."""
+        check_right_padded(attention_mask)
+        if tokens.dim() != 2:
+            raise ValueError("tokens must be [batch, seq]")
+        B, T = tokens.shape
+        if T > self.config.max_positions:
+            raise ValueError(f"sequence_log_likelihood: a row of {T} tokens is longer than max_positions = "
+                             f"{self.config.max_positions} (rows are not truncated)")
+        if B == 0:
+            ll = torch.empty((0,), device=self.device, dtype=torch.bfloat16)
+            return (ll, torch.empty((0, max(T - 1, 0)), device=self.device)) if return_token_nll else ll
+        ids = tokens.to(self.device, dtype=torch.int64).contiguous()
+        self.forward(ids)
+        return self.score_last_forward(ids, mean_nll, ignore_tokens, return_token_nll)
+
+    def score_last_forward(self, ids: torch.Tensor, mean_nll: bool, ignore_tokens=None, return_token_nll: bool = False):
+        """The scoring half of `sequence_log_likelihood`: `sk_seq_loglik` on the logits of the last `forward(ids)`
+        (ids: device int64 [B, T], B >= 1)."""
+        B, T = ids.shape
+        ll = torch.empty((B,), device=self.device, dtype=torch.bfloat16)
+        token_nll = torch.empty((B * max(T - 1, 1),), device=self.device, dtype=torch.float32)
+        ban = self._ban_bits(ignore_tokens)
+        L.check(self.lib.sk_seq_loglik(C.c_void_p(self.lib.sk_lm_logits(self._h)), self.lib.sk_lm_logits_ld(self._h),
+                                       self.config.vocab_size, L.ptr(ids), B, T, int(self.config.pad_token_id), L.ptr(ban),
+                                       int(bool(mean_nll)), L.ptr(token_nll), L.ptr(ll), L.stream_ptr()))
+        return (ll, token_nll[:B * (T - 1)].view(B, T - 1)) if return_token_nll else ll
+
     @torch.inference_mode()
     def generate(self, inputs: Optional[torch.Tensor] = None, generation_config=None, **kwargs) -> torch.Tensor:
         """TokenLM.generate (slamkit/model/token_lm.py:19-27; UnitLM.generate -> HF GenerationMixin, unit_lm.py:196-198):

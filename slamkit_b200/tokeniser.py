@@ -75,6 +75,28 @@ class B200UnitTokeniser:
     def tokenise(self, wav, lens=None):
         return self.string_tokenise(self.audio_stringify(wav, lens), return_tensors="pt", padding=True)
 
+    @torch.inference_mode()
+    def tokenise_device(self, wav: torch.Tensor, lens: Optional[torch.Tensor] = None):
+        """`tokenise()` without the host strings: unit ids -> dedup (`sk_rle`) -> `[BOS, u + offset..., EOS, PAD...]`
+        (`sk_units_to_tokens`), all on the device.  Returns device (ids int64 [B, T], attention_mask int64 [B, T]), equal
+        to tokenise()'s.  The host reads the per-row counts once, to size the batch."""
+        from . import _lib as L
+        fe = self.model
+        if fe is None:
+            raise RuntimeError("This tokeniser does not have a feature extractor")
+        ids, nf = fe.units_device(wav, lens)
+        units, counts = ids, nf
+        if self.dedup:
+            units, _, counts = fe.dedup_device(ids, nf)
+        B, T_units = units.shape
+        T_out = int(counts.max()) + 2 if B else 2
+        out = torch.empty((B, T_out), dtype=torch.int64, device=units.device)
+        if B:
+            L.check(fe.lib.sk_units_to_tokens(L.ptr(units), L.ptr(counts), B, T_units, self.offset, self.bos_token_id,
+                                              self.eos_token_id, self.pad_token_id, L.ptr(out), T_out, L.stream_ptr()))
+        mask = (torch.arange(T_out, device=units.device)[None, :] < (counts.long() + 2)[:, None]).long()
+        return out, mask
+
     def prepare_sample(self, sample: dict, **kw):
         return self.string_tokenise(sample["audio_repr"], **kw)
 
@@ -145,6 +167,31 @@ class B200InterleavingTokeniser:
 
     def prepare_sample(self, sample: dict, **kw) -> Dict:
         return self.string_tokenise(sample["audio_repr"], **kw)
+
+    @property
+    def fe_sample_rate(self) -> int:
+        return B200UnitTokeniser.fe_sample_rate.fget(self)
+
+    def tokenise(self, wav: torch.Tensor, lens: Optional[torch.Tensor] = None) -> Dict:
+        """interleaving_tokeniser.py:230-233, speech-only batch: `<Un…>` strings through the text tokenizer, right-padded."""
+        if not isinstance(wav, torch.Tensor):
+            raise NotImplementedError("interleaved (speech + text) inputs are not supported: pass a speech-only wav batch")
+        self.text_tokeniser.padding_side = "right"
+        strs = self.stringify_representation(self.audio_represent(wav, lens))
+        return self.string_tokenise(strs, return_tensors="pt", padding=True)
+
+    def get_ignore_tokens(self, used_token_modality: Optional[str]) -> Optional[List[int]]:
+        """interleaving_tokeniser.py:295-310: ids excluded from the log-likelihood.  SPEECH bans every text id except
+        bos / eos, plus `<speech>` / `<text>`; TEXT bans the unit ids (not the two markers); anything else bans nothing."""
+        tk = self.text_tokeniser
+        num_text = len(tk) - self.num_units - 2
+        special = [tk.bos_token_id, tk.eos_token_id]
+        markers = [tk.encode(SPEECH_TOKEN)[0], tk.encode(TEXT_TOKEN)[0]]
+        if used_token_modality and used_token_modality.upper() == "SPEECH":
+            return [x for x in range(0, num_text) if x not in special] + markers
+        if used_token_modality and used_token_modality.upper() == "TEXT":
+            return [x for x in range(num_text, len(tk)) if x not in special + markers]
+        return None
 
     def save_pretrained(self, save_directory: str, **_):
         with open(f"{save_directory}/tokeniser_config.json", "w") as f:
