@@ -356,6 +356,58 @@ int sk_kmeans_argmin(const float* dot, const float* centers_sqnorm, int32_t* lab
 /* conv0 statistics buffer length (doubles per clip) */
 int sk_conv0_nstat(void);
 
+/* ---- HiFi-GAN unit vocoder ---------------------------------------------------------------------------------------------
+ * CodeHiFiGANVocoder.forward (slamkit/vocoder/hifigan/vocoder.py:56-88 -> CodeGenerator, generator.py:95-197) in eval
+ * mode with weight norm folded, fp32-grade: convolutions run as split-bf16 (hi*hi + hi*lo + lo*hi) implicit GEMMs on the
+ * tensor cores.  speaker_id = style_id = 0, as vocode() passes them; f0 conditioning and embedder_params are not
+ * supported.  Rows of a batch are packed on one timeline with zero gaps wide enough that a row's waveform is
+ * bit-identical alone, in any batch and at any position.  Weights are one flat fp32 buffer enumerated by
+ * sk_vocoder_tensor_info with the reference's state-dict names and torch shapes (ConvTranspose1d: [Cin, Cout, k]). */
+typedef struct SkVocoderConfig {
+  int32_t num_embeddings;            /* code vocabulary (500) */
+  int32_t embedding_dim;             /* 128; a multiple of 4 */
+  int32_t model_in_dim;              /* embedding_dim * (1 + multispkr + multistyle) */
+  int32_t multispkr, num_speakers;
+  int32_t multistyle, num_styles;
+  int32_t upsample_initial_channel;  /* 512; every stage's channel count must be a multiple of 4 */
+  int32_t n_upsamples;               /* 1..8 */
+  int32_t upsample_rates[8];         /* rate u, kernel k: k - u even, k <= 32 */
+  int32_t upsample_kernel_sizes[8];
+  int32_t n_resblocks;               /* 1..4 ResBlocks per stage, averaged */
+  int32_t resblock_kernel_sizes[4];  /* odd */
+  int32_t resblock_dilations[4][3];
+  int32_t dur_predictor;             /* 1: VariancePredictor durations (dur_prediction=True) */
+  int32_t dur_hidden;                /* var_pred_hidden_dim */
+  int32_t dur_kernel;                /* var_pred_kernel_size: only 3 */
+  int32_t max_rows;                  /* workspace: rows per sub-batch */
+  int32_t max_frames;                /* workspace: unit frames per sub-batch (summed over its rows) */
+} SkVocoderConfig;
+typedef struct SkVocoder SkVocoder;
+
+int sk_vocoder_create(const SkVocoderConfig* cfg, SkVocoder** out);
+void sk_vocoder_destroy(SkVocoder* v);
+int64_t sk_vocoder_param_count(const SkVocoder* v);        /* fp32 elements of the flat weight buffer */
+int sk_vocoder_tensor_info(const SkVocoder* v, int idx, char* name_buf, int name_cap, int64_t* offset,
+                           int64_t* numel);                /* idx < 0 -> number of tensors */
+int sk_vocoder_gap(const SkVocoder* v);                    /* zero frames between packed rows */
+int sk_vocoder_upsampling(const SkVocoder* v);             /* output samples per unit frame (product of the rates) */
+int64_t sk_vocoder_prepared_bytes(const SkVocoder* v);     /* device scratch for the split (hi, lo) conv weights */
+int64_t sk_vocoder_workspace_bytes(const SkVocoder* v);    /* for (max_rows, max_frames) */
+/* weights fp32 [sk_vocoder_param_count] stays referenced; the conv weights are split into `prepared` on `stream`. */
+int sk_vocoder_bind(SkVocoder* v, const float* weights, void* prepared, int64_t prepared_bytes, void* workspace,
+                    int64_t workspace_bytes, void* stream);
+/* codes int64 [B, ld] with counts int32 [B] entries per row; negative codes are dropped.  B <= max_rows,
+ * ld <= max_frames.  dur int32 [B, ld] (per kept unit, or NULL), log_dur fp32 [B, ld] (the predictor's value before
+ * exp / round, or NULL), frames int32 [B] (frames per row).  status int32 [2]: {codes >= num_embeddings, rows with more
+ * units than max_frames}; such codes are read as 0 and never index out of bounds. */
+int sk_vocoder_durations(SkVocoder* v, const int64_t* codes, int ld, const int32_t* counts, int B, int32_t* dur,
+                         float* log_dur, int32_t* frames, int32_t* status, void* stream);
+/* wave fp32 [B, ldw]: row b's frames_host[b] * sk_vocoder_upsampling() samples, then zeros.  frames_host: the frames of
+ * sk_vocoder_durations on the host (the caller reads them once to size wave); rows are vocoded in sub-batches of whole
+ * rows that fit the workspace.  Codes must have passed sk_vocoder_durations with status {0, 0}. */
+int sk_vocoder_run(SkVocoder* v, const int64_t* codes, int ld, const int32_t* counts, int B, const int32_t* frames_host,
+                   float* wave, int64_t ldw, void* stream);
+
 /* ---- host-side FLAC decoding (no audio decoder exists in the image) ------------------------------------------------
  * Replaces torchaudio.info / torchaudio.load in cli/extract_features.py:45-57.  Host pointers. md5_16 receives the
  * STREAMINFO MD5 of the unencoded audio (all zero if the encoder did not set it). */

@@ -118,7 +118,8 @@ def load() -> C.CDLL:
     lib.sk_last_error.restype = C.c_char_p
     for name in ("sk_lm_param_count", "sk_lm_workspace_bytes", "sk_launch_count", "sk_hubert_param_count", "sk_hubert_prepared_bytes",
                  "sk_hubert_workspace_bytes", "sk_gemm_ws_bytes", "sk_lm_kv_cache_bytes", "sk_lm_decode_workspace_bytes",
-                 "sk_attn_decode_partial_bytes"):
+                 "sk_attn_decode_partial_bytes", "sk_vocoder_param_count", "sk_vocoder_prepared_bytes",
+                 "sk_vocoder_workspace_bytes"):
         if hasattr(lib, name):
             getattr(lib, name).restype = C.c_int64
     for name in ("sk_lm_logits",):
@@ -126,6 +127,8 @@ def load() -> C.CDLL:
     lib.sk_lm_destroy.restype = None
     if hasattr(lib, "sk_hubert_destroy"):
         lib.sk_hubert_destroy.restype = None
+    if hasattr(lib, "sk_vocoder_destroy"):
+        lib.sk_vocoder_destroy.restype = None
     _lib = lib
     return lib
 

@@ -5,6 +5,7 @@ defaults: Hann-windowed sinc, lowpass_filter_width 6, rolloff 0.99), THEN averag
 from __future__ import annotations
 
 import math
+import struct
 import wave
 from typing import Tuple
 
@@ -12,9 +13,46 @@ import numpy as np
 import torch
 
 
+def _wav_chunks(path: str):
+    """(format tag, channels, sample rate, bits per sample, data offset, data bytes) of a RIFF/WAVE file; the tag of a
+    WAVE_FORMAT_EXTENSIBLE file is its sub-format's."""
+    with open(path, "rb") as f:
+        head = f.read(12)
+        if len(head) < 12 or head[:4] != b"RIFF" or head[8:12] != b"WAVE":
+            raise ValueError(f"{path}: not a RIFF/WAVE file")
+        fmt = None
+        while True:
+            ch = f.read(8)
+            if len(ch) < 8:
+                raise ValueError(f"{path}: no data chunk")
+            cid, size = ch[:4], struct.unpack("<I", ch[4:])[0]
+            if cid == b"fmt ":
+                body = f.read(size)
+                tag, nch, sr, _, _, bits = struct.unpack("<HHIIHH", body[:16])
+                if tag == 0xFFFE and len(body) >= 26:
+                    tag = struct.unpack("<H", body[24:26])[0]
+                fmt = (tag, nch, sr, bits)
+                f.seek(size & 1, 1)
+            elif cid == b"data":
+                if fmt is None:
+                    raise ValueError(f"{path}: data chunk before fmt chunk")
+                return fmt + (f.tell(), size)
+            else:
+                f.seek(size + (size & 1), 1)
+
+
 def wav_num_frames(path: str) -> int:
-    with wave.open(path, "rb") as w:
-        return w.getnframes()
+    tag, nch, sr, bits, _, size = _wav_chunks(path)
+    return size // (nch * bits // 8)
+
+
+def audio_info(path: str) -> Tuple[int, int]:
+    """(frames, sample rate) of a FLAC or WAV file (what torchaudio.info reports as num_frames / sample_rate)."""
+    if path.lower().endswith(".flac"):
+        i = flac_info(path)
+        return i["num_frames"], i["sample_rate"]
+    tag, nch, sr, bits, _, size = _wav_chunks(path)
+    return size // (nch * bits // 8), sr
 
 
 def resample(x: torch.Tensor, orig_sr: int, new_sr: int, lowpass_filter_width: int = 6, rolloff: float = 0.99) -> torch.Tensor:
@@ -51,10 +89,18 @@ def resample(x: torch.Tensor, orig_sr: int, new_sr: int, lowpass_filter_width: i
 
 
 def load_wav(path: str, target_sr: int = 16000) -> torch.Tensor:
-    with wave.open(path, "rb") as w:
-        sr, ch, width, n = w.getframerate(), w.getnchannels(), w.getsampwidth(), w.getnframes()
-        raw = w.readframes(n)
-    if width == 2:
+    tag, ch, sr, bits, off, size = _wav_chunks(path)
+    width = bits // 8
+    with open(path, "rb") as f:
+        f.seek(off)
+        raw = f.read(size - size % (ch * width))
+    if tag == 3:                                                  # IEEE float, as torchaudio.save writes float32
+        if width != 4:
+            raise ValueError(f"{path}: unsupported float sample width {width}")
+        x = np.frombuffer(raw, dtype="<f4").astype(np.float32)
+    elif tag != 1:
+        raise ValueError(f"{path}: unsupported WAV format tag {tag}")
+    elif width == 2:
         x = np.frombuffer(raw, dtype="<i2").astype(np.float32) / 32768.0
     elif width == 4:
         x = np.frombuffer(raw, dtype="<i4").astype(np.float32) / 2147483648.0
@@ -74,6 +120,17 @@ def write_wav(path: str, x: torch.Tensor, sr: int = 16000) -> None:
         w.setsampwidth(2)
         w.setframerate(sr)
         w.writeframes(pcm.tobytes())
+
+
+def write_wav_float(path: str, x: torch.Tensor, sr: int = 16000) -> None:
+    """Mono 32-bit IEEE-float WAV (format tag 3 with a fact chunk): what torchaudio.save writes for a float32 tensor."""
+    data = x.detach().reshape(-1).to("cpu", torch.float32).numpy().astype("<f4").tobytes()
+    n = len(data) // 4
+    fmt = struct.pack("<HHIIHHH", 3, 1, sr, sr * 4, 4, 32, 0)
+    body = (b"WAVE" + b"fmt " + struct.pack("<I", len(fmt)) + fmt + b"fact" + struct.pack("<II", 4, n)
+            + b"data" + struct.pack("<I", len(data)) + data)
+    with open(path, "wb") as f:
+        f.write(b"RIFF" + struct.pack("<I", len(body)) + body)
 
 
 # ---- FLAC through the library's host-side decoder (sk_flac_*) ---------------------------------------------------------

@@ -5,7 +5,7 @@ from __future__ import annotations
 
 import os
 import warnings
-from typing import Optional
+from typing import Optional, Tuple
 
 
 def hubert_b200_from_cfg(pretrained_model: str = "facebook/hubert-base-ls960",
@@ -62,3 +62,62 @@ def tlm_b200_from_cfg(cfg, device: str = "cuda:0", max_batch: int = 8, max_seq: 
     else:
         model.init_weights(seed=0)
     return model
+
+
+# textlesslib checkpoint names (`<dense>-<quantizer>-<vocab>-hifigan[-<suffix>]`) -> file names under its disk root
+TEXTLESS_VOCODER_FILES = {
+    "mhubert-base-25hz-kmeans-500-hifigan": "hifigan_lj_mhubert_base_25hz.pt",
+    "mhubert-base-25hz-kmeans-500-hifigan-config": "hifigan_lj_mhubert_base_25hz_config.json",
+    "hubert-base-ls960-layer-9-kmeans-500-hifigan": "hifigan_expresso_lj_vctk_hubert_base_ls960_L9_km500_generator.pt",
+    "hubert-base-ls960-layer-9-kmeans-500-hifigan-config": "hifigan_expresso_lj_vctk_hubert_base_ls960_L9_km500_config.json",
+    "hubert-base-ls960-layer-9-kmeans-expresso-2000-hifigan":
+        "hifigan_expresso_lj_vctk_hubert_base_ls960_L9_km2000_expresso_generator.pt",
+    "hubert-base-ls960-layer-9-kmeans-expresso-2000-hifigan-config":
+        "hifigan_expresso_lj_vctk_hubert_base_ls960_L9_km2000_expresso_config.json",
+    "mhubert-base-vp_mls_cv_8lang-kmeans-2000-hifigan":
+        "hifigan_expresso_lj_vctk_mhubert_base_vp_mls_cv_8lang_it3_L12_km2000_generator.pt",
+    "mhubert-base-vp_mls_cv_8lang-kmeans-2000-hifigan-config":
+        "hifigan_expresso_lj_vctk_mhubert_base_vp_mls_cv_8lang_it3_L12_km2000_config.json",
+    "mhubert-base-vp_mls_cv_8lang-kmeans-expresso-2000-hifigan":
+        "hifigan_expresso_lj_vctk_mhubert_base_vp_mls_cv_8lang_it3_L12_km2000_expresso_generator.pt",
+    "mhubert-base-vp_mls_cv_8lang-kmeans-expresso-2000-hifigan-config":
+        "hifigan_expresso_lj_vctk_mhubert_base_vp_mls_cv_8lang_it3_L12_km2000_expresso_config.json",
+}
+
+
+def vocoder_checkpoint_paths(dense_model_name: str, quantizer_model_name: str, vocab_size: int,
+                             vocoder_suffix: Optional[str] = None) -> Tuple[str, str]:
+    """(generator, config) paths where textlesslib's checkpoint manager keeps them: $TEXTLESS_CHECKPOINT_ROOT, default
+    ~/.textless/ (CodeHiFiGANVocoder.by_name, slamkit/vocoder/hifigan/vocoder.py:98-140)."""
+    name = f"{dense_model_name}-{quantizer_model_name}-{vocab_size}-hifigan"
+    if vocoder_suffix is not None:
+        name += "-" + vocoder_suffix
+    root = os.path.expanduser(os.environ.get("TEXTLESS_CHECKPOINT_ROOT", "~/.textless/"))
+    if name not in TEXTLESS_VOCODER_FILES:
+        raise FileNotFoundError(f"unknown textless vocoder checkpoint '{name}': pass model_path= and config_path=")
+    return (os.path.join(root, TEXTLESS_VOCODER_FILES[name]), os.path.join(root, TEXTLESS_VOCODER_FILES[name + "-config"]))
+
+
+def vocoder_b200_from_cfg(cfg, device: str = "cuda:0", max_rows: int = 64, max_frames: int = 16384):
+    """`vocoder_factory` (slamkit/vocoder/audio_vocoder.py:13-25) for `vocoder_type: hifigan` / `hifigan_b200`, with the
+    reference's keys (dense_model_name, quantizer_model_name, vocab_size, vocoder_suffix, speaker_meta, style_meta) or
+    explicit `model_path` / `config_path`.  Nothing is downloaded: a missing file raises FileNotFoundError naming the
+    path it was expected at.  `vocoder_type: null` gives None."""
+    get = cfg.get if hasattr(cfg, "get") else (lambda k, d=None: getattr(cfg, k, d))
+    vt = get("vocoder_type")
+    if vt is None:
+        return None
+    if vt not in ("hifigan", "hifigan_b200"):
+        raise ValueError(f"Unknown vocoder type: {vt}")
+    model_path, config_path = get("model_path"), get("config_path")
+    if not (model_path and config_path):
+        mp, cp = vocoder_checkpoint_paths(get("dense_model_name"), get("quantizer_model_name"), get("vocab_size"),
+                                          get("vocoder_suffix"))
+        model_path, config_path = model_path or mp, config_path or cp
+    for p in (model_path, config_path):
+        if not os.path.exists(p):
+            raise FileNotFoundError(f"vocoder file not found: {p} (this package never downloads; place the textlesslib "
+                                    "checkpoint there or pass vocoder.model_path / vocoder.config_path)")
+    from .vocoder import HifiGanB200Vocoder
+    return HifiGanB200Vocoder.from_checkpoint(model_path, config_path, device=device, max_rows=max_rows,
+                                              max_frames=max_frames)

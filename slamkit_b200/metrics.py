@@ -140,3 +140,96 @@ def _paired(name: str, sep: str):
 swuggy = _paired("sWUGGY", "_")
 sblimp = _paired("sBLIMP", "+")
 storycloze = _paired("StoryCloze", "_")
+
+
+# ---- generative metric (slamkit/metric/generative_metric.py) ----------------------------------------------------------
+def get_cut_location(alignment, prompt_length: float) -> float:
+    """generative_metric.py:18-26: the end time of the aligned word whose end is nearest to `prompt_length` (first on
+    ties)."""
+    endtimes = torch.tensor([word[2] for word in alignment])
+    return endtimes[torch.abs(endtimes - prompt_length).argmin()].item()
+
+
+def _is_shorter(path: str, min_file_length: float) -> bool:
+    from .audio_io import audio_info
+    n, sr = audio_info(path)
+    return n < min_file_length * sr
+
+
+class PromptDataset:
+    """generative_metric.py:34-81: files matched by `glob_path` (recursive), the first `num_files` of `iglob` when it is
+    set, skipping files shorter than `min_file_length` seconds; each prompt is the resampled, channel-averaged clip cut
+    to `int(prompt_length * sample_rate)` samples, or with `use_alignment` to the aligned word end nearest to
+    `prompt_length` (alignments: `<file>.json` next to a `.wav`, or `<alignment_folder>/<stem>.json`)."""
+
+    def __init__(self, glob_path: str, prompt_length: Optional[float] = None, sample_rate: int = 16000,
+                 num_files: Optional[int] = None, min_file_length: Optional[float] = None, use_alignment: bool = False,
+                 alignment_folder: Optional[str] = None):
+        from glob import glob, iglob
+        self.prompt_length, self.sample_rate = prompt_length, sample_rate
+        if num_files is None:
+            self.data = glob(glob_path, recursive=True)
+            if min_file_length is not None:
+                self.data = [p for p in self.data if not _is_shorter(p, min_file_length)]
+        else:
+            self.data = []
+            for path in iglob(glob_path, recursive=True):
+                if len(self.data) >= num_files:
+                    break
+                if min_file_length is not None and _is_shorter(path, min_file_length):
+                    continue
+                self.data.append(path)
+        self.use_alignment, self.alignment_folder = use_alignment, alignment_folder
+
+    def __len__(self) -> int:
+        return len(self.data)
+
+    def crop(self, idx: int) -> Optional[int]:
+        """Samples kept of file `idx` (None: all)."""
+        if self.prompt_length is None:
+            return None
+        if not self.use_alignment:
+            return int(self.prompt_length * self.sample_rate)
+        import json
+        with open(self.get_alignment_path(self.data[idx])) as f:
+            alignment = json.load(f)["aligned_text"]
+        return int(get_cut_location(alignment, self.prompt_length) * self.sample_rate)
+
+    def __getitem__(self, idx: int):
+        from .audio_io import load_audio
+        audio = load_audio(self.data[idx], self.sample_rate)
+        n = self.crop(idx)
+        if n is not None:
+            audio = audio[:n]
+        return audio, audio.shape[-1]
+
+    def get_alignment_path(self, file: str) -> str:
+        if self.alignment_folder is None:
+            return file.replace(".wav", ".json")
+        base = os.path.basename(file)
+        return os.path.join(self.alignment_folder, base[:base.find(".")] + ".json")
+
+
+def generate(model, data_path: str, batch_size: int, used_tokens_modality: Optional[str] = None,
+             prompt_length: Optional[float] = None, min_file_length: Optional[float] = None,
+             alignment_folder: Optional[str] = None, use_alignment: bool = False, sample_rate: int = 16000,
+             num_files: Optional[int] = None, num_workers: int = 8, pin_memory: bool = True, **generate_kwargs) -> dict:
+    """generative_metric.py:89-106: `batch_size` prompts at a time, in dataset order, zero-padded to the batch's longest
+    prompt, each batch continued by `model.generate`.  Audio is decoded ahead of the GPU by `num_workers` threads
+    (cli/extract_features.BatchPrefetcher); the prefetcher decodes whole files, and the crop is applied on the device."""
+    from cli.extract_features import BatchPrefetcher
+    dataset = PromptDataset(data_path, prompt_length=prompt_length, sample_rate=sample_rate, num_files=num_files,
+                            min_file_length=min_file_length, alignment_folder=alignment_folder, use_alignment=use_alignment)
+    assert len(dataset) > 0, f"no samples found for {data_path}"
+    idx = list(range(len(dataset)))
+    batches = [[(dataset.data[i], i) for i in idx[s:s + batch_size]] for s in range(0, len(idx), batch_size)]
+    res, prompts = [], []
+    with torch.inference_mode():
+        for batch, wav, lens in BatchPrefetcher(batches, sample_rate, str(model.device), num_workers=max(1, num_workers)):
+            cut = [dataset.crop(i) for _, i in batch]
+            lens = torch.stack([lens[r].clamp(max=c) if c is not None else lens[r] for r, c in enumerate(cut)])
+            S = int(lens.max())
+            wav = wav[:, :S] * (torch.arange(S, device=wav.device)[None, :] < lens[:, None])
+            res.extend(model.generate(wav, lens, used_tokens_modality or "SPEECH", **generate_kwargs))
+            prompts.extend(wav[r, :int(lens[r])] for r in range(wav.shape[0]))
+    return {"generate": res, "prompts": prompts}

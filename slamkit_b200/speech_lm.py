@@ -1,22 +1,22 @@
-"""B200SpeechLM -- mirror of the reference's `SpeechLM` (slamkit/model/speech_lm.py:8-36) for the modelling metrics:
-a trained `B200UnitLM` plus an audio tokeniser, scoring zero-padded waveform batches.
+"""B200SpeechLM -- mirror of the reference's `SpeechLM` (slamkit/model/speech_lm.py:8-63): a trained `B200UnitLM` plus
+an audio tokeniser and, optionally, a unit vocoder, scoring and continuing zero-padded waveform batches.
 
 With the unit tokeniser the whole chain runs on the device: HuBERT units (`sk_hubert_units`) -> dedup (`sk_rle`) ->
-token ids (`sk_units_to_tokens`) -> LM forward (`sk_lm_forward`) -> per-sequence scores (`sk_seq_loglik`).  The
+token ids (`sk_units_to_tokens`) -> LM forward (`sk_lm_forward`) -> per-sequence scores (`sk_seq_loglik`).  `generate`
+continues left-padded prompts with the cached decoder and vocodes every row in one batched `sk_vocoder_run` call.  The
 interleaved tokeniser builds its ids through the text tokenizer on the host, as the reference does."""
 from __future__ import annotations
 
-from typing import Optional
+from typing import List, Optional
 
 import torch
 
 
 class B200SpeechLM:
     def __init__(self, model, tokeniser, vocoder=None, device: Optional[str] = None):
-        if vocoder is not None:
-            raise NotImplementedError("vocoding needs a vocoder, which this package does not provide")
         self.model = model
         self.tokeniser = tokeniser
+        self.vocoder = vocoder
         self.device = torch.device(device) if device is not None else model.device
 
     def tokenise(self, wavs: torch.Tensor, lens: Optional[torch.Tensor] = None):
@@ -33,3 +33,28 @@ class B200SpeechLM:
         ids, mask = self.tokenise(wavs, lens)
         ignore = self.tokeniser.get_ignore_tokens(used_token_modality)
         return self.model.sequence_log_likelihood(ids, mean_nll, ignore, attention_mask=mask)
+
+    @torch.inference_mode()
+    def generate(self, wavs: torch.Tensor, lens: Optional[torch.Tensor] = None, output_modality: str = "SPEECH",
+                 remove_prompt: bool = False, **kwargs) -> List[torch.Tensor]:
+        """speech_lm.py:38-55: continue each zero-padded prompt clip; with a vocoder, one waveform per row (an empty
+        tensor for an empty continuation), otherwise the decoded unit ids."""
+        if not hasattr(self.tokeniser, "build_prompt"):
+            raise NotImplementedError("generate needs the unit tokeniser: interleaved (speech + text) prompts are not "
+                                      "supported")
+        if output_modality is None or output_modality.upper() != "SPEECH":
+            raise NotImplementedError(f"output_modality={output_modality!r}: only SPEECH continuations are supported")
+        tokens = self.tokeniser.build_prompt(wavs, lens, output_modality=output_modality)
+        ignore = self.tokeniser.get_ignore_tokens(output_modality)
+        if ignore is not None:
+            ignore = [[tok] for tok in ignore]
+        conts = self.model.generate(tokens["input_ids"], attention_mask=tokens["attention_mask"], bad_words_ids=ignore,
+                                    **kwargs)
+        if remove_prompt:
+            conts = conts[..., tokens["input_ids"].size(1):]
+        decoded = [self.tokeniser.decode_sample(c, output_modality=output_modality) for c in conts]
+        if self.vocoder is None:
+            return decoded
+        wave, wl = self.vocoder.vocode_batch(decoded)
+        return [wave[i, :int(wl[i])] if int(wl[i]) > 0 else torch.zeros(0, device=wave.device)
+                for i in range(len(decoded))]

@@ -97,6 +97,33 @@ class B200UnitTokeniser:
         mask = (torch.arange(T_out, device=units.device)[None, :] < (counts.long() + 2)[:, None]).long()
         return out, mask
 
+    def prompt_ids(self, units: torch.Tensor, counts: torch.Tensor) -> Dict[str, torch.Tensor]:
+        """The generation prompt of unit_tokeniser.py:75-80 under the left padding SpeechLM.generate sets: row b is
+        `[PAD..., BOS, units[b, :counts[b]] + offset]` (the template's EOS dropped), with its attention mask.  Works on
+        the tensors' device."""
+        B = units.shape[0]
+        counts = counts.to(units.device).long()
+        T = int(counts.max()) + 1 if B else 1
+        col = torch.arange(T, device=units.device)[None, :]
+        start = T - 1 - counts[:, None]                                   # column of BOS
+        src = (col - start - 1).clamp(0, max(units.shape[1] - 1, 0))
+        vals = units.long().gather(1, src) + self.offset if units.shape[1] else torch.zeros_like(src)
+        ids = torch.where(col > start, vals, torch.full_like(vals, self.pad_token_id))
+        ids = torch.where(col == start, torch.full_like(ids, self.bos_token_id), ids)
+        return {"input_ids": ids, "attention_mask": (col >= start).long()}
+
+    @torch.inference_mode()
+    def build_prompt(self, wav: torch.Tensor, lens: Optional[torch.Tensor] = None,
+                     output_modality: Optional[str] = None) -> Dict[str, torch.Tensor]:
+        """unit_tokeniser.py:75-80 on the device: HuBERT units -> dedup (`sk_rle`) -> left-padded prompt ids."""
+        fe = self.model
+        if fe is None:
+            raise RuntimeError("This tokeniser does not have a feature extractor")
+        ids, nf = fe.units_device(wav, lens)
+        if self.dedup:
+            ids, _, nf = fe.dedup_device(ids, nf)
+        return self.prompt_ids(ids, nf)
+
     def prepare_sample(self, sample: dict, **kw):
         return self.string_tokenise(sample["audio_repr"], **kw)
 
