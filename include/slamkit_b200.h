@@ -32,7 +32,7 @@ int sk_device_cc(void);                     /* 10*major + minor of the current d
  * C[M,N] = A * B^T (+ bias[N]) (+ residual[M,N]); bf16 operands, fp32 accumulation, bf16 (or fp32) output.
  *   a_mn = 0: A is [M,K] row-major (lda = row pitch);  a_mn = 1: A is stored transposed as [K,M] (lda = its pitch).
  *   b_mn = 0: B is [N,K] row-major (a torch Linear weight);  b_mn = 1: B is stored as [K,N].
- *   act: 0 none, 1 GELU(erf) on (acc+bias).  round_before_res: round (acc+bias) to bf16 before adding the residual
+ *   act: 0 none, 1 GELU(erf), 2 ReLU on (acc+bias).  round_before_res: round (acc+bias) to bf16 before adding the residual
  *   (bit-matches an unfused bf16 linear followed by a bf16 add).  force_bn: 0 auto, else 64/128/256.
  * Replaces every torch.nn.Linear / F.linear on both hot paths (HF:models/qwen2/modeling_qwen2.py:35-48,187-246;
  * HF:models/hubert/modeling_hubert.py:216-231,262-405) and their autograd dgrad/wgrad GEMMs. */
@@ -99,6 +99,16 @@ int sk_rmsnorm_fwd(const void* x, const void* w, void* y, float* rstd, int M, in
 int sk_rmsnorm_bwd_blocks(void);
 int sk_rmsnorm_bwd(const void* dy, const void* x, const void* w, const float* rstd, const void* dres, void* dx,
                    void* dw, float* dw_partial, int M, int D, int accumulate_dw, void* stream);
+/* nn.LayerNorm with affine weight w and bias b (the OPT decoder's, HF:models/opt/modeling_opt.py:195-200): fp32 inside,
+ * y = bf16((x - mean) * rstd * w + b).  mean / rstd (fp32 [M], may be NULL) are what the backward reads.  D <= 2048. */
+int sk_layernorm_fwd(const void* x, const void* w, const void* b, void* y, float* mean, float* rstd, int M, int D, float eps,
+                     void* stream);
+/* dx = d(layernorm)(dy) (+ dres); dw (+)= sum_rows dy * xhat, db (+)= sum_rows dy, through fixed-order per-block partials
+ * (deterministic).  dw_partial / db_partial: fp32 [sk_layernorm_bwd_blocks() * D] each. */
+int sk_layernorm_bwd_blocks(void);
+int sk_layernorm_bwd(const void* dy, const void* x, const void* w, const float* mean, const float* rstd, const void* dres,
+                     void* dx, void* dw, void* db, float* dw_partial, float* db_partial, int M, int D, int accumulate,
+                     void* stream);
 /* Column sums of a bf16 matrix (bias gradient). partial: fp32 [sk_colsum_splits()*N]. */
 int sk_colsum_splits(void);
 int sk_colsum(const void* x, void* out, float* partial, int M, int N, int ld, int accumulate, void* stream);
@@ -179,6 +189,31 @@ typedef struct SkLmConfig {
 typedef struct SkLm SkLm;
 
 int sk_lm_create(const SkLmConfig* cfg, SkLm** out);
+/* Pre-LayerNorm OPT decoder (HF OPTForCausalLM with do_layer_norm_before = True and word_embed_proj_dim = hidden, e.g.
+ * facebook/opt-125m, the base of config/model/twist.yaml and gslm.yaml; HF:models/opt/modeling_opt.py):
+ *   x0 = bf16(embed_tokens[id] + embed_positions[pos + 2]);  per layer  h = LN1(x);  q|k|v = h W + b;  causal MHA with
+ *   scale 1/8 (HF multiplies q by 1/8, a power of two);  x += o W_o + b_o;  h = LN2(x);  x += relu(h W_1 + b_1) W_2 + b_2;
+ *   final LN, tied (or separate) lm_head without bias.  LayerNorms are affine, fp32 inside, rounded once to bf16.
+ * Returns the same SkLm handle type: every sk_lm_* entry point runs this decoder on it.  Differences from a Qwen2 handle:
+ *   - the flat layout (sk_lm_tensor_info) lists per layer ln1, ln1_b, wqkv [3*hidden, hidden], bqkv, wo, bo, ln2, ln2_b,
+ *     w1 [ffn, hidden], b1, w2 [hidden, ffn], b2; then final_norm, final_norm_b, embed [Vpad, hidden],
+ *     pos_embed [max_positions + 2, hidden] and, untied, lm_head;
+ *   - sk_lm_bind takes NULL RoPE tables;
+ *   - positions (row % T, pos_ids, or the decode step's pos[b]) select table row position + 2, clamped to the table;
+ *   - the gradient-norm groups are OPTForCausalLM's parameters: q, k, v, out_proj, fc1, fc2 weights and biases and the
+ *     LayerNorm weights and biases each count as one tensor;
+ *   - the KV cache holds n_heads K/V heads per layer (same layout as above with n_kv_heads = n_heads). */
+typedef struct SkOptConfig {
+  int32_t vocab_size;        /* 502 for unit_hubert_25 */
+  int32_t hidden;            /* 768 for opt-125m; n_heads * 64, <= 2048 */
+  int32_t n_layers;          /* 12 */
+  int32_t n_heads;           /* 12 */
+  int32_t ffn;               /* 3072; a multiple of 8 */
+  int32_t max_positions;     /* max_position_embeddings (2048): the position table has max_positions + 2 rows */
+  float ln_eps;              /* 1e-5 */
+  int32_t tie_embeddings;    /* 1: lm_head shares the token embedding table */
+} SkOptConfig;
+int sk_lm_create_opt(const SkOptConfig* cfg, SkLm** out);
 void sk_lm_destroy(SkLm* lm);
 /* Flat parameter layout (bf16 elements). Tensors are enumerated in a fixed order; name_buf receives e.g.
  * "layers.3.wqkv". Returns the number of tensors when idx < 0. */

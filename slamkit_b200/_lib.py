@@ -38,6 +38,19 @@ class SkLmConfig(C.Structure):
     ]
 
 
+class SkOptConfig(C.Structure):
+    _fields_ = [
+        ("vocab_size", C.c_int32),
+        ("hidden", C.c_int32),
+        ("n_layers", C.c_int32),
+        ("n_heads", C.c_int32),
+        ("ffn", C.c_int32),
+        ("max_positions", C.c_int32),
+        ("ln_eps", C.c_float),
+        ("tie_embeddings", C.c_int32),
+    ]
+
+
 class SkHubertConfig(C.Structure):
     _fields_ = [
         ("n_conv", C.c_int32),

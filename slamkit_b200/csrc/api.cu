@@ -157,6 +157,16 @@ int sk_rmsnorm_bwd(const void* dy, const void* x, const void* w, const float* rs
   return sk_rmsnorm_bwd_launch(CBF(dy), CBF(x), CBF(w), rstd, CBF(dres), BF(dx), BF(dw), dw_partial, M, D,
                                accumulate_dw, S(stream));
 }
+int sk_layernorm_fwd(const void* x, const void* w, const void* b, void* y, float* mean, float* rstd, int M, int D, float eps,
+                     void* stream) {
+  return sk_layernorm_fwd_launch(CBF(x), CBF(w), CBF(b), BF(y), mean, rstd, M, D, eps, S(stream));
+}
+int sk_layernorm_bwd(const void* dy, const void* x, const void* w, const float* mean, const float* rstd, const void* dres,
+                     void* dx, void* dw, void* db, float* dw_partial, float* db_partial, int M, int D, int accumulate,
+                     void* stream) {
+  return sk_layernorm_bwd_launch(CBF(dy), CBF(x), CBF(w), mean, rstd, CBF(dres), BF(dx), BF(dw), BF(db), dw_partial, db_partial,
+                                 M, D, accumulate, S(stream));
+}
 int sk_colsum(const void* x, void* out, float* partial, int M, int N, int ld, int accumulate, void* stream) {
   return sk_colsum_launch(CBF(x), BF(out), partial, M, N, ld, accumulate, S(stream));
 }

@@ -50,7 +50,7 @@ struct GemmParams {
   int tiles_m, tiles_n;
   int out_f32;          // 1: C is float
   int round_before_res; // 1: out = bf16(bf16(acc+bias) + res)  (matches an unfused bf16 linear followed by an add)
-  int act;              // 0 none, 1 GELU(erf) applied to acc+bias
+  int act;              // 0 none, 1 GELU(erf), 2 ReLU, applied to acc+bias
   int col_gin, col_gout;  // > 0: output column c -> (c / col_gin) * col_gout + c % col_gin, dropped if c % col_gin >= col_gout
   int splits;           // > 1: split-K; work item = (tile, split), fp32 partial tiles go to splitk_ws[split][M][N]
   float* splitk_ws;
@@ -265,6 +265,9 @@ SK_DEVINL void epi_bias_act(float (&v)[8], const GemmParams& p, int col) {
   if (p.act == 1) {
 #pragma unroll
     for (int i = 0; i < 8; ++i) v[i] = gelu_erf(v[i]);
+  } else if (p.act == 2) {   // ReLU commutes with the bf16 rounding that follows: bf16(relu(v)) == relu(bf16(v))
+#pragma unroll
+    for (int i = 0; i < 8; ++i) v[i] = fmaxf(v[i], 0.0f);
   }
 }
 
@@ -1066,6 +1069,7 @@ int plan_gemm(const SkGemmEx& g, GemmParams& p, int& BN, int& ew, int& grid) {
   SK_REQUIRE((reinterpret_cast<uintptr_t>(g.bias) & 15) == 0 && (reinterpret_cast<uintptr_t>(g.residual) & 15) == 0,
              "gemm: bias and residual must be 16-byte aligned");
   SK_REQUIRE(g.passes == 1 || (g.passes == 3 && g.A_lo && g.B_lo), "gemm: passes must be 1, or 3 with lo operands");
+  SK_REQUIRE(g.act >= 0 && g.act <= 2, "gemm: act must be 0 (none), 1 (GELU) or 2 (ReLU), got %d", g.act);
   const bool use3d = g.a_rows > 0;   // strided-window / batched A view
   SK_REQUIRE(!use3d || !g.a_mn, "gemm: a batched / windowed A operand must be K-major");
   SK_REQUIRE(g.a_mode == 0 || use3d, "gemm: a_mode 1 needs the 3-D A view");

@@ -91,6 +91,19 @@ int sk_adamw_launch(bf16* p, const bf16* g, bf16* m, bf16* v, long n, float lr, 
                     float wd, int step, const float* clip_stats, cudaStream_t s);
 int sk_transpose_launch(const bf16* in, bf16* out, int M, int N, cudaStream_t s);
 int sk_seg_bounds_launch(const int32_t* pos_ids, int32_t* seg_start, int32_t* seg_end, int B, int T, cudaStream_t s);
+// OPT decoder: LayerNorm (fp32 mean / rstd per row saved by the forward), token + learned position embedding
+// (table row = position + 2, clamped), the position-table gradient in the embedding's 64-bit fixed point, ReLU backward
+int sk_layernorm_fwd_launch(const bf16* x, const bf16* w, const bf16* b, bf16* y, float* mean, float* rstd, int M, int D,
+                            float eps, cudaStream_t s);
+extern "C" int sk_layernorm_bwd_blocks(void);
+int sk_layernorm_bwd_launch(const bf16* dy, const bf16* x, const bf16* w, const float* mean, const float* rstd, const bf16* dres,
+                            bf16* dx, bf16* dw, bf16* db, float* dw_partial, float* db_partial, int M, int D, int accumulate,
+                            cudaStream_t s);
+int sk_opt_embed_fwd_launch(const int64_t* ids, const int32_t* pos_ids, const bf16* E, const bf16* P, bf16* out, int M, int T, int D,
+                            int V, int n_pos, cudaStream_t s);
+int sk_opt_pos_bwd_launch(const int32_t* pos_ids, const bf16* dx, float* scratch, bf16* dP, int M, int T, int D, int n_pos,
+                          int accumulate, cudaStream_t s);
+int sk_relu_bwd_launch(bf16* g, const bf16* a, long n, cudaStream_t s);
 
 // attention.cu
 int sk_attn_fwd_launch(const bf16* q, const bf16* k, const bf16* v, bf16* o, float* lse, int B, int T, int H, int KVH,

@@ -937,3 +937,295 @@ int sk_transpose_launch(const bf16* in, bf16* out, int M, int N, cudaStream_t s)
   SK_LAUNCH_CHECK();
   return 0;
 }
+
+// ------------------------------------------------------------------------------------------------
+// OPT decoder (pre-LayerNorm, learned positions, ReLU MLP; HF:models/opt/modeling_opt.py:45-70,170-260,480-560)
+// ------------------------------------------------------------------------------------------------
+namespace {
+
+constexpr int LN_BWD_WARPS = 4;
+
+// LayerNorm forward, one warp per row: y = bf16((x - mean) * rstd * g + b) in fp32 (nn.LayerNorm on a bf16 input, and
+// its autocast form that runs in fp32 and feeds the next linear a bf16 copy, both round once).  The row stays in
+// registers between the mean pass, the variance pass and the output pass.
+template <int MAXV>
+__global__ void __launch_bounds__(WARPS_PER_BLOCK * 32)
+layernorm_fwd_kernel(const bf16* __restrict__ x, const bf16* __restrict__ w, const bf16* __restrict__ b, bf16* __restrict__ y,
+                     float* __restrict__ mean_out, float* __restrict__ rstd_out, int M, int D, float eps) {
+  griddep_launch();
+  griddep_wait();
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int row = blockIdx.x * WARPS_PER_BLOCK + warp;
+  if (row >= M) return;
+  const int nvec = D / 8;
+  uint4 xv[MAXV];
+  float s = 0.f;
+#pragma unroll
+  for (int j = 0; j < MAXV; ++j) {
+    const int c = lane + 32 * j;
+    if (c < nvec) {
+      xv[j] = ldg128_stream(x + (size_t)row * D + c * 8);
+      const uint32_t u[4] = {xv[j].x, xv[j].y, xv[j].z, xv[j].w};
+#pragma unroll
+      for (int k = 0; k < 4; ++k) {
+        const float2 f = unpack_bf16(u[k]);
+        s += f.x + f.y;
+      }
+    }
+  }
+  const float mean = warp_sum(s) / (float)D;
+  float ss = 0.f;
+#pragma unroll
+  for (int j = 0; j < MAXV; ++j) {
+    const int c = lane + 32 * j;
+    if (c < nvec) {
+      const uint32_t u[4] = {xv[j].x, xv[j].y, xv[j].z, xv[j].w};
+#pragma unroll
+      for (int k = 0; k < 4; ++k) {
+        const float2 f = unpack_bf16(u[k]);
+        ss += (f.x - mean) * (f.x - mean) + (f.y - mean) * (f.y - mean);
+      }
+    }
+  }
+  const float rstd = rsqrtf(warp_sum(ss) / (float)D + eps);
+  if (lane == 0) {
+    if (mean_out) mean_out[row] = mean;
+    if (rstd_out) rstd_out[row] = rstd;
+  }
+#pragma unroll
+  for (int j = 0; j < MAXV; ++j) {
+    const int c = lane + 32 * j;
+    if (c < nvec) {
+      const uint4 wv = ldg128(w + c * 8), bv = ldg128(b + c * 8);
+      const uint32_t u[4] = {xv[j].x, xv[j].y, xv[j].z, xv[j].w};
+      const uint32_t wu[4] = {wv.x, wv.y, wv.z, wv.w}, bu[4] = {bv.x, bv.y, bv.z, bv.w};
+      uint32_t o[4];
+#pragma unroll
+      for (int k = 0; k < 4; ++k) {
+        const float2 f = unpack_bf16(u[k]), g = unpack_bf16(wu[k]), bb = unpack_bf16(bu[k]);
+        o[k] = pack_bf16(fmaf((f.x - mean) * rstd, g.x, bb.x), fmaf((f.y - mean) * rstd, g.y, bb.y));
+      }
+      stg128(y + (size_t)row * D + c * 8, make_uint4(o[0], o[1], o[2], o[3]));
+    }
+  }
+}
+
+// LayerNorm backward, one warp per row, grid-stride over rows with a fixed grid:
+//   xhat = (x - mean) * rstd ; g = dy * w ; dx = rstd * (g - mean(g) - xhat * mean(g * xhat)) (+ dres)
+//   dw (+)= sum_rows dy * xhat ; db (+)= sum_rows dy
+// Each warp adds its rows' dw / db terms into its own shared-memory slab (a lane owns its columns: no conflicts); the
+// block writes one partial row per block, and colsum_reduce_kernel sums the partials in a fixed order (deterministic).
+template <int MAXV>
+__global__ void __launch_bounds__(LN_BWD_WARPS * 32)
+layernorm_bwd_kernel(const bf16* __restrict__ dy, const bf16* __restrict__ x, const bf16* __restrict__ w,
+                     const float* __restrict__ mean_in, const float* __restrict__ rstd_in, const bf16* __restrict__ dres,
+                     bf16* __restrict__ dx, float* __restrict__ dw_partial, float* __restrict__ db_partial, int M, int D) {
+  griddep_launch();
+  griddep_wait();
+  extern __shared__ float sacc[];   // [2][LN_BWD_WARPS][D]: dw then db
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int nvec = D / 8;
+  float* sdw = sacc + (size_t)warp * D;
+  float* sdb = sacc + (size_t)(LN_BWD_WARPS + warp) * D;
+  for (int c = lane; c < nvec; c += 32)
+#pragma unroll
+    for (int k = 0; k < 8; ++k) { sdw[c * 8 + k] = 0.f; sdb[c * 8 + k] = 0.f; }
+  for (int row = blockIdx.x * LN_BWD_WARPS + warp; row < M; row += gridDim.x * LN_BWD_WARPS) {
+    uint4 xq[MAXV], dq[MAXV];
+#pragma unroll
+    for (int j = 0; j < MAXV; ++j) {
+      const int c = lane + 32 * j;
+      if (c < nvec) {
+        xq[j] = ldg128_stream(x + (size_t)row * D + c * 8);
+        dq[j] = ldg128_stream(dy + (size_t)row * D + c * 8);
+      }
+    }
+    const float mean = mean_in[row], rstd = rstd_in[row];
+    float s1 = 0.f, s2 = 0.f;
+#pragma unroll
+    for (int j = 0; j < MAXV; ++j) {
+      const int c = lane + 32 * j;
+      if (c < nvec) {
+        const uint4 wv = ldg128(w + c * 8);
+        const uint32_t xu[4] = {xq[j].x, xq[j].y, xq[j].z, xq[j].w}, du[4] = {dq[j].x, dq[j].y, dq[j].z, dq[j].w};
+        const uint32_t wu[4] = {wv.x, wv.y, wv.z, wv.w};
+#pragma unroll
+        for (int k = 0; k < 4; ++k) {
+          const float2 xf = unpack_bf16(xu[k]), df = unpack_bf16(du[k]), wf = unpack_bf16(wu[k]);
+          const float xh0 = (xf.x - mean) * rstd, xh1 = (xf.y - mean) * rstd;
+          const float g0 = df.x * wf.x, g1 = df.y * wf.y;
+          s1 += g0 + g1;
+          s2 = fmaf(g0, xh0, fmaf(g1, xh1, s2));
+          float* pw = sdw + c * 8 + 2 * k;
+          float* pb = sdb + c * 8 + 2 * k;
+          pw[0] = fmaf(df.x, xh0, pw[0]);
+          pw[1] = fmaf(df.y, xh1, pw[1]);
+          pb[0] += df.x;
+          pb[1] += df.y;
+        }
+      }
+    }
+    const float m1 = warp_sum(s1) / (float)D, m2 = warp_sum(s2) / (float)D;
+#pragma unroll
+    for (int j = 0; j < MAXV; ++j) {
+      const int c = lane + 32 * j;
+      if (c < nvec) {
+        const uint4 wv = ldg128(w + c * 8);
+        const uint4 rv = dres ? ldg128_stream(dres + (size_t)row * D + c * 8) : make_uint4(0, 0, 0, 0);
+        const uint32_t xu[4] = {xq[j].x, xq[j].y, xq[j].z, xq[j].w}, du[4] = {dq[j].x, dq[j].y, dq[j].z, dq[j].w};
+        const uint32_t wu[4] = {wv.x, wv.y, wv.z, wv.w}, ru[4] = {rv.x, rv.y, rv.z, rv.w};
+        uint32_t o[4];
+#pragma unroll
+        for (int k = 0; k < 4; ++k) {
+          const float2 xf = unpack_bf16(xu[k]), df = unpack_bf16(du[k]), wf = unpack_bf16(wu[k]), rf = unpack_bf16(ru[k]);
+          const float xh0 = (xf.x - mean) * rstd, xh1 = (xf.y - mean) * rstd;
+          const float d0 = rstd * (df.x * wf.x - m1 - xh0 * m2), d1 = rstd * (df.y * wf.y - m1 - xh1 * m2);
+          o[k] = pack_bf16(d0 + rf.x, d1 + rf.y);
+        }
+        stg128(dx + (size_t)row * D + c * 8, make_uint4(o[0], o[1], o[2], o[3]));
+      }
+    }
+  }
+  __syncthreads();
+  for (int i = threadIdx.x; i < D; i += blockDim.x) {
+    float a = 0.f, bsum = 0.f;
+#pragma unroll
+    for (int wi = 0; wi < LN_BWD_WARPS; ++wi) {
+      a += sacc[(size_t)wi * D + i];
+      bsum += sacc[(size_t)(LN_BWD_WARPS + wi) * D + i];
+    }
+    dw_partial[(size_t)blockIdx.x * D + i] = a;
+    db_partial[(size_t)blockIdx.x * D + i] = bsum;
+  }
+}
+
+// OPTLearnedPositionalEmbedding: table row of a position (offset 2, clamped to the table like the RoPE tables)
+SK_DEVINL int opt_pos_row(const int32_t* pos_ids, int m, int T, int n_rows) {
+  const int p = (pos_ids ? pos_ids[m] : m % T) + 2;
+  return max(0, min(p, n_rows - 1));
+}
+
+// x0 = bf16(E[id] + P[pos + 2]) (embed_tokens + embed_positions in bf16: one rounding)
+__global__ void opt_embed_fwd_kernel(const int64_t* __restrict__ ids, const int32_t* __restrict__ pos_ids, const bf16* __restrict__ E,
+                                     const bf16* __restrict__ P, bf16* __restrict__ out, int M, int T, int D, int V, int n_pos) {
+  const int vec_per_row = D / 8;
+  const long total = (long)M * vec_per_row;
+  for (long i = blockIdx.x * (long)blockDim.x + threadIdx.x; i < total; i += (long)gridDim.x * blockDim.x) {
+    const int m = (int)(i / vec_per_row);
+    const int c = (int)(i % vec_per_row);
+    long id = ids[m];
+    if (id < 0 || id >= V) id = 0;
+    const int pr = opt_pos_row(pos_ids, m, T, n_pos);
+    const uint4 a = ldg128(E + (size_t)id * D + c * 8), b = ldg128(P + (size_t)pr * D + c * 8);
+    const uint32_t au[4] = {a.x, a.y, a.z, a.w}, bu[4] = {b.x, b.y, b.z, b.w};
+    uint32_t o[4];
+#pragma unroll
+    for (int k = 0; k < 4; ++k) {
+      const float2 fa = unpack_bf16(au[k]), fb = unpack_bf16(bu[k]);
+      o[k] = pack_bf16(fa.x + fb.x, fa.y + fb.y);
+    }
+    stg128(out + (size_t)m * D + c * 8, make_uint4(o[0], o[1], o[2], o[3]));
+  }
+}
+
+// dP_fix[pos_row(m)] += dx[m] in the 64-bit fixed point of embed_bwd_scatter_kernel (order-independent)
+__global__ void opt_pos_bwd_scatter_kernel(const int32_t* __restrict__ pos_ids, const bf16* __restrict__ dx,
+                                           unsigned long long* __restrict__ scratch, int M, int T, int D, int n_pos) {
+  const int vec_per_row = D / 8;
+  const long total = (long)M * vec_per_row;
+  for (long i = blockIdx.x * (long)blockDim.x + threadIdx.x; i < total; i += (long)gridDim.x * blockDim.x) {
+    const int m = (int)(i / vec_per_row);
+    const int c = (int)(i % vec_per_row);
+    const int pr = opt_pos_row(pos_ids, m, T, n_pos);
+    const uint4 v = ldg128_stream(dx + (size_t)m * D + c * 8);
+    const uint32_t w[4] = {v.x, v.y, v.z, v.w};
+    unsigned long long* dst = scratch + (size_t)pr * D + c * 8;
+#pragma unroll
+    for (int k = 0; k < 4; ++k) {
+      const float2 f = unpack_bf16(w[k]);
+      if (f.x != 0.f) atomicAdd(dst + 2 * k, (unsigned long long)__float2ll_rn(f.x * EMBED_FIX_SCALE));
+      if (f.y != 0.f) atomicAdd(dst + 2 * k + 1, (unsigned long long)__float2ll_rn(f.y * EMBED_FIX_SCALE));
+    }
+  }
+}
+
+// torch threshold_backward(grad, relu_out, 0): grad where the saved activation is > 0, else 0 (in place on grad)
+__global__ void relu_bwd_kernel(bf16* __restrict__ g, const bf16* __restrict__ a, long n) {
+  griddep_launch();
+  griddep_wait();
+  for (long i = (blockIdx.x * (long)blockDim.x + threadIdx.x) * 8; i < n; i += (long)gridDim.x * blockDim.x * 8) {
+    const uint4 gv = *reinterpret_cast<const uint4*>(g + i);
+    const uint4 av = ldg128_stream(a + i);
+    const uint32_t gu[4] = {gv.x, gv.y, gv.z, gv.w}, au[4] = {av.x, av.y, av.z, av.w};
+    uint32_t o[4];
+#pragma unroll
+    for (int k = 0; k < 4; ++k) {
+      const float2 fa = unpack_bf16(au[k]);
+      o[k] = (fa.x > 0.f ? (gu[k] & 0xffffu) : 0u) | (fa.y > 0.f ? (gu[k] & 0xffff0000u) : 0u);
+    }
+    stg128(g + i, make_uint4(o[0], o[1], o[2], o[3]));
+  }
+}
+
+}  // namespace
+
+int sk_layernorm_fwd_launch(const bf16* x, const bf16* w, const bf16* b, bf16* y, float* mean, float* rstd, int M, int D,
+                            float eps, cudaStream_t s) {
+  SK_REQUIRE(D % 8 == 0 && D <= 2048, "layernorm: D must be a multiple of 8 and <= 2048 (D=%d)", D);
+  const dim3 grid((M + WARPS_PER_BLOCK - 1) / WARPS_PER_BLOCK), block(WARPS_PER_BLOCK * 32);
+  if (D <= 1024) SK_CUDA_CHECK(sk_launch_pdl(layernorm_fwd_kernel<4>, grid, block, (size_t)0, s, x, w, b, y, mean, rstd, M, D, eps));
+  else           SK_CUDA_CHECK(sk_launch_pdl(layernorm_fwd_kernel<8>, grid, block, (size_t)0, s, x, w, b, y, mean, rstd, M, D, eps));
+  SK_LAUNCH_CHECK();
+  return 0;
+}
+// dw_partial / db_partial must each hold sk_layernorm_bwd_blocks() * D floats
+extern "C" int sk_layernorm_bwd_blocks(void) { return sk_num_sms() * 2; }
+int sk_layernorm_bwd_launch(const bf16* dy, const bf16* x, const bf16* w, const float* mean, const float* rstd, const bf16* dres,
+                            bf16* dx, bf16* dw, bf16* db, float* dw_partial, float* db_partial, int M, int D, int accumulate,
+                            cudaStream_t s) {
+  SK_REQUIRE(D % 8 == 0 && D <= 2048, "layernorm: D must be a multiple of 8 and <= 2048 (D=%d)", D);
+  int blocks = sk_layernorm_bwd_blocks();
+  const int need = (M + LN_BWD_WARPS - 1) / LN_BWD_WARPS;
+  if (blocks > need) blocks = need;
+  const size_t smem = (size_t)2 * LN_BWD_WARPS * D * sizeof(float);
+  if (smem > 48 * 1024)   // D > 1536
+    SK_CUDA_CHECK(cudaFuncSetAttribute(layernorm_bwd_kernel<8>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+  if (D <= 1024)
+    SK_CUDA_CHECK(sk_launch_pdl(layernorm_bwd_kernel<4>, dim3(blocks), dim3(LN_BWD_WARPS * 32), smem, s, dy, x, w, mean, rstd, dres, dx,
+                                dw_partial, db_partial, M, D));
+  else
+    SK_CUDA_CHECK(sk_launch_pdl(layernorm_bwd_kernel<8>, dim3(blocks), dim3(LN_BWD_WARPS * 32), smem, s, dy, x, w, mean, rstd, dres, dx,
+                                dw_partial, db_partial, M, D));
+  SK_LAUNCH_CHECK();
+  SK_CUDA_CHECK(sk_launch_pdl(colsum_reduce_kernel, dim3((D + 31) / 32), dim3(1024), (size_t)0, s, (const float*)dw_partial, dw, blocks, D, accumulate));
+  SK_LAUNCH_CHECK();
+  SK_CUDA_CHECK(sk_launch_pdl(colsum_reduce_kernel, dim3((D + 31) / 32), dim3(1024), (size_t)0, s, (const float*)db_partial, db, blocks, D, accumulate));
+  SK_LAUNCH_CHECK();
+  return 0;
+}
+int sk_opt_embed_fwd_launch(const int64_t* ids, const int32_t* pos_ids, const bf16* E, const bf16* P, bf16* out, int M, int T, int D,
+                            int V, int n_pos, cudaStream_t s) {
+  SK_REQUIRE(D % 8 == 0 && n_pos > 0 && T > 0, "opt embed: D must be a multiple of 8");
+  opt_embed_fwd_kernel<<<grid_for((long)M * D / 8, 256), 256, 0, s>>>(ids, pos_ids, E, P, out, M, T, D, V, n_pos);
+  SK_LAUNCH_CHECK();
+  return 0;
+}
+int sk_opt_pos_bwd_launch(const int32_t* pos_ids, const bf16* dx, float* scratch, bf16* dP, int M, int T, int D, int n_pos,
+                          int accumulate, cudaStream_t s) {
+  SK_REQUIRE(D % 8 == 0 && n_pos > 0 && T > 0, "opt positions: D must be a multiple of 8");
+  unsigned long long* fix = reinterpret_cast<unsigned long long*>(scratch);   // n_pos * D 64-bit words
+  const long n = (long)n_pos * D;
+  SK_CUDA_CHECK(cudaMemsetAsync(fix, 0, (size_t)n * sizeof(unsigned long long), s));
+  opt_pos_bwd_scatter_kernel<<<grid_for((long)M * D / 8, 256), 256, 0, s>>>(pos_ids, dx, fix, M, T, D, n_pos);
+  SK_LAUNCH_CHECK();
+  SK_REQUIRE(n % 8 == 0, "opt positions: table size must be a multiple of 8");
+  add_fix_into_bf16_kernel<<<grid_for(n / 8, 256), 256, 0, s>>>(dP, fix, n, accumulate);
+  SK_LAUNCH_CHECK();
+  return 0;
+}
+int sk_relu_bwd_launch(bf16* g, const bf16* a, long n, cudaStream_t s) {
+  SK_REQUIRE(n % 8 == 0, "relu backward: size must be a multiple of 8");
+  SK_CUDA_CHECK(sk_launch_pdl(relu_bwd_kernel, dim3(grid_for(n / 8, 256)), dim3(256), (size_t)0, s, g, a, n));
+  SK_LAUNCH_CHECK();
+  return 0;
+}

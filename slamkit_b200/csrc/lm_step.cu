@@ -24,6 +24,11 @@ struct TensorDesc {
 struct LayerOff {
   int64_t ln1, wqkv, bqkv, wo, ln2, wgu, wd;
 };
+// OPT decoder layer (HF OPTDecoderLayer, do_layer_norm_before = True): every linear has a bias, q|k|v fused as in Qwen2
+struct OptLayerOff {
+  int64_t ln1w, ln1b, wqkv, bqkv, wo, bo, ln2w, ln2b, w1, b1, w2, b2;
+};
+enum { SK_ARCH_QWEN2 = 0, SK_ARCH_OPT = 1 };
 // byte offsets into the workspace for one (B,T)
 struct WsLayout {
   int64_t X, h1, rstd1, qkv, ao, lse, xmid, h2, rstd2, gu, act;  // per-layer strides below
@@ -34,10 +39,14 @@ struct WsLayout {
 }  // namespace
 
 struct SkLm {
-  SkLmConfig cfg;
+  SkLmConfig cfg;      // OPT handles fill it too (n_kv_heads = n_heads, rms_eps = the LayerNorm eps): shape checks are shared
+  int arch = SK_ARCH_QWEN2;
   int d, F, H, KVH, hd, L, V, Vp, qkv_dim;
   std::vector<TensorDesc> tensors;
   std::vector<LayerOff> lo;
+  std::vector<OptLayerOff> olo;   // OPT layers
+  int64_t off_final_norm_b = 0, off_pos = 0;
+  int n_pos = 0;                  // OPT: rows of the learned position table (max_positions + 2)
   int64_t off_final_norm = 0, off_embed = 0, off_head = 0, n_params = 0;
   bf16* params = nullptr;
   bf16* grads = nullptr;
@@ -358,6 +367,258 @@ int check_decode(const SkLm* lm, int B, int T_cache, int ldl, const void* kv_cac
   return 0;
 }
 
+// ---- OPT decoder (HF:models/opt/modeling_opt.py:45-70 positions, :100-182 attention, :185-260 decoder layer,
+// :480-560 decoder).  Separate functions from the Qwen2 ones above; the entry points below pick one by lm->arch.
+
+// The Qwen2 workspace plan with OPT's tensors: rstd slabs hold the LayerNorm mean then rstd (fp32 [2][M]), `gu` holds
+// the ReLU output a = relu(fc1) [M, F] that fc2 and the ReLU backward read, `dgu` its gradient; `act` is unused.
+WsLayout make_opt_layout(const SkLm* lm, int B, int T) {
+  WsLayout w;
+  const int64_t M = (int64_t)B * T;
+  int64_t cur = 0;
+  auto take = [&](int64_t bytes) {
+    const int64_t o = cur;
+    cur = align_up(cur + bytes, 256);
+    return o;
+  };
+  const int L = lm->L;
+  w.sX = align_up(M * lm->d * 2, 256);
+  w.sh = w.sX;
+  w.srstd = align_up(M * 8, 256);
+  w.sqkv = align_up(M * lm->qkv_dim * 2, 256);
+  w.slse = align_up((int64_t)B * lm->H * T * 4, 256);
+  w.sgu = align_up(M * lm->F * 2, 256);
+  w.sact = 0;
+  // GEMM scratch first, at the same fixed offset as in make_layout (sk_lm_bind clears its flag words once)
+  w.splitk_bytes = align_up(std::max<int64_t>((int64_t)8 * lm->qkv_dim * lm->d * 4, (int64_t)sk_gemm_ws_min_bytes()) + 4096, 256);
+  w.splitk = take(w.splitk_bytes);
+  w.X = take(w.sX * (L + 1));
+  w.h1 = take(w.sh * L);
+  w.rstd1 = take(w.srstd * L);
+  w.qkv = take(w.sqkv * L);
+  w.ao = take(w.sX * L);
+  w.lse = take(w.slse * L);
+  w.xmid = take(w.sX * L);
+  w.h2 = take(w.sh * L);
+  w.rstd2 = take(w.srstd * L);
+  w.gu = take(w.sgu * L);
+  w.act = 0;
+  w.hf = take(w.sX);
+  w.rstdf = take(w.srstd);
+  w.logits = take(M * lm->Vp * 2);
+  w.dlogits = lm->head_chunk > 0 ? w.logits : take(M * lm->Vp * 2);
+  w.dxA = take(w.sX);
+  w.dxB = take(w.sX);
+  w.dh = take(w.sX);
+  w.dao = take(w.sX);
+  w.dqkv = take(w.sqkv);
+  w.dgu = take(w.sgu);
+  w.delta = take(w.slse);
+  w.dw_partial = take((int64_t)2 * sk_layernorm_bwd_blocks() * lm->d * 4);   // LayerNorm weight and bias partials
+  w.colsum_partial = take((int64_t)sk_colsum_splits() * std::max(lm->qkv_dim, lm->F) * 4);
+  w.ce_partial = take((int64_t)sk_ce_blocks((int)M) * 2 * 4);
+  // token and position tables share the fixed-point scratch: their gradients are formed one after the other
+  w.embed_scratch = take((int64_t)std::max(lm->Vp, lm->n_pos) * lm->d * 8);
+  w.seg_start = take(M * 4);
+  w.seg_end = take(M * 4);
+  w.total = cur;
+  return w;
+}
+
+WsLayout layout_of(const SkLm* lm, int B, int T) {
+  return lm->arch == SK_ARCH_OPT ? make_opt_layout(lm, B, T) : make_layout(lm, B, T);
+}
+
+int opt_forward(SkLm* lm, const int64_t* ids, const int64_t* labels, const int32_t* pos_ids, int B, int T, float num_items,
+                float dloss, bool want_dlogits, float* stats, const WsLayout& w, cudaStream_t s, float* row_nll = nullptr,
+                bool with_head = true) {
+  const int M = B * T, d = lm->d, F = lm->F, L = lm->L, Q = lm->qkv_dim;
+  const float eps = lm->cfg.rms_eps;
+  const bf16* P = lm->params;
+  SK_TRY(sk_opt_embed_fwd_launch(ids, pos_ids, P + lm->off_embed, P + lm->off_pos, wsp<bf16>(lm, w.X), M, T, d, lm->V, lm->n_pos, s));
+  // q is multiplied by head_dim^-0.5 = 1/8 after q_proj (HF:modeling_opt.py:146); a power of two, so the same value as
+  // scaling the scores inside attention
+  const float scale = 1.0f / sqrtf((float)lm->hd);
+  const int* seg_start = nullptr;
+  if (pos_ids) {
+    SK_TRY(sk_seg_bounds_launch(pos_ids, wsp<int32_t>(lm, w.seg_start), wsp<int32_t>(lm, w.seg_end), B, T, s));
+    seg_start = wsp<int32_t>(lm, w.seg_start);
+  }
+  for (int l = 0; l < L; ++l) {
+    const OptLayerOff& o = lm->olo[l];
+    bf16* x = wsp<bf16>(lm, w.X + w.sX * l);
+    bf16* xn = wsp<bf16>(lm, w.X + w.sX * (l + 1));
+    bf16* h1 = wsp<bf16>(lm, w.h1 + w.sh * l);
+    float* st1 = wsp<float>(lm, w.rstd1 + w.srstd * l);
+    bf16* qkv = wsp<bf16>(lm, w.qkv + w.sqkv * l);
+    bf16* ao = wsp<bf16>(lm, w.ao + w.sX * l);
+    float* lse = wsp<float>(lm, w.lse + w.slse * l);
+    bf16* xmid = wsp<bf16>(lm, w.xmid + w.sX * l);
+    bf16* h2 = wsp<bf16>(lm, w.h2 + w.sh * l);
+    float* st2 = wsp<float>(lm, w.rstd2 + w.srstd * l);
+    bf16* a = wsp<bf16>(lm, w.gu + w.sgu * l);
+
+    SK_TRY(sk_layernorm_fwd_launch(x, P + o.ln1w, P + o.ln1b, h1, st1, st1 + M, M, d, eps, s));
+    SK_TRY(linear_fwd(M, Q, d, h1, P + o.wqkv, qkv, P + o.bqkv, nullptr, s));
+    SK_TRY(sk_attn_tc_fwd_launch(qkv, ao, lse, B, T, lm->H, lm->H, Q, d, 1, scale, s, seg_start));
+    SK_TRY(linear_fwd(M, d, d, ao, P + o.wo, xmid, P + o.bo, x, s));
+    SK_TRY(sk_layernorm_fwd_launch(xmid, P + o.ln2w, P + o.ln2b, h2, st2, st2 + M, M, d, eps, s));
+    SK_TRY(sk_gemm_launch(M, F, d, h2, d, 0, P + o.w1, d, 0, a, F, 0, P + o.b1, nullptr, 0, 0, 2, 0, s));   // relu(fc1)
+    SK_TRY(linear_fwd(M, d, F, a, P + o.w2, xn, P + o.b2, xmid, s));
+  }
+  float* stf = wsp<float>(lm, w.rstdf);
+  SK_TRY(sk_layernorm_fwd_launch(wsp<bf16>(lm, w.X + w.sX * L), P + lm->off_final_norm, P + lm->off_final_norm_b,
+                                 wsp<bf16>(lm, w.hf), stf, stf + M, M, d, eps, s));
+  lm->last_B = B;
+  lm->last_T = T;
+  if (!with_head) return 0;
+  bf16* logits = wsp<bf16>(lm, w.logits);
+  SK_TRY(linear_fwd(M, lm->Vp, d, wsp<bf16>(lm, w.hf), P + lm->off_head, logits, nullptr, nullptr, s));
+  if (labels) {
+    SK_TRY(sk_ce_launch(logits, labels, want_dlogits ? wsp<bf16>(lm, w.dlogits) : nullptr, wsp<float>(lm, w.ce_partial),
+                        row_nll, stats, M, T, lm->V, lm->Vp, num_items, dloss, s));
+  }
+  return 0;
+}
+
+// The embedding table's pad row gets the gradient of every token equal to pad_token_id.  HF's nn.Embedding(padding_idx)
+// drops that row's gradient instead; in right-padded and packed batches the two agree exactly, because the gradient
+// reaching a pad position is zero (pad targets carry no loss and only later pad positions attend to a pad key).
+int opt_backward(SkLm* lm, const int64_t* ids, const int32_t* pos_ids, int B, int T, int accumulate, const WsLayout& w,
+                 cudaStream_t s, bool with_head = true) {
+  const int M = B * T, d = lm->d, F = lm->F, L = lm->L, Q = lm->qkv_dim;
+  const bf16* P = lm->params;
+  bf16* G = lm->grads;
+  float* dwp = wsp<float>(lm, w.dw_partial);
+  float* dbp = dwp + (size_t)sk_layernorm_bwd_blocks() * d;
+  float* csp = wsp<float>(lm, w.colsum_partial);
+  bf16* dxA = wsp<bf16>(lm, w.dxA);
+  bf16* dxB = wsp<bf16>(lm, w.dxB);
+  bf16* dh = wsp<bf16>(lm, w.dh);
+  bf16* dao = wsp<bf16>(lm, w.dao);
+  bf16* dqkv = wsp<bf16>(lm, w.dqkv);
+  bf16* da = wsp<bf16>(lm, w.dgu);
+  bf16* hf = wsp<bf16>(lm, w.hf);
+  void* sws = lm->ws + w.splitk;
+  const size_t swb = (size_t)w.splitk_bytes;
+  const float scale = 1.0f / sqrtf((float)lm->hd);
+  const int* seg_start = pos_ids ? wsp<int32_t>(lm, w.seg_start) : nullptr;
+  const int* seg_end = pos_ids ? wsp<int32_t>(lm, w.seg_end) : nullptr;
+
+  if (with_head) {
+    bf16* dlogits = wsp<bf16>(lm, w.dlogits);
+    SK_TRY(linear_dgrad(M, lm->Vp, d, dlogits, P + lm->off_head, dh, s));
+    SK_TRY(linear_wgrad(M, lm->Vp, d, dlogits, hf, G + lm->off_head, accumulate, s, sws, swb));
+  }
+  const float* stf = wsp<float>(lm, w.rstdf);
+  SK_TRY(sk_layernorm_bwd_launch(dh, wsp<bf16>(lm, w.X + w.sX * L), P + lm->off_final_norm, stf, stf + M, nullptr, dxA,
+                                 G + lm->off_final_norm, G + lm->off_final_norm_b, dwp, dbp, M, d, accumulate, s));
+  if (!lm->bwd_events.empty()) SK_CUDA_CHECK(cudaEventRecord(lm->bwd_events[L], s));
+  for (int l = L - 1; l >= 0; --l) {
+    const OptLayerOff& o = lm->olo[l];
+    const bf16* x = wsp<bf16>(lm, w.X + w.sX * l);
+    const bf16* h1 = wsp<bf16>(lm, w.h1 + w.sh * l);
+    const float* st1 = wsp<float>(lm, w.rstd1 + w.srstd * l);
+    const bf16* qkv = wsp<bf16>(lm, w.qkv + w.sqkv * l);
+    const bf16* ao = wsp<bf16>(lm, w.ao + w.sX * l);
+    const float* lse = wsp<float>(lm, w.lse + w.slse * l);
+    const bf16* xmid = wsp<bf16>(lm, w.xmid + w.sX * l);
+    const bf16* h2 = wsp<bf16>(lm, w.h2 + w.sh * l);
+    const float* st2 = wsp<float>(lm, w.rstd2 + w.srstd * l);
+    const bf16* a = wsp<bf16>(lm, w.gu + w.sgu * l);
+
+    // MLP: dy = dxA.  ReLU backward as one element-wise pass over fc2's dgrad, masked by the saved a = relu(fc1) > 0
+    SK_TRY(linear_dgrad(M, d, F, dxA, P + o.w2, da, s));
+    SK_TRY(sk_relu_bwd_launch(da, a, (long)M * F, s));
+    SK_TRY(linear_wgrad(M, d, F, dxA, a, G + o.w2, accumulate, s, sws, swb));
+    SK_TRY(sk_colsum_launch(dxA, G + o.b2, csp, M, d, d, accumulate, s));
+    SK_TRY(linear_dgrad(M, F, d, da, P + o.w1, dh, s));
+    SK_TRY(linear_wgrad(M, F, d, da, h2, G + o.w1, accumulate, s, sws, swb));
+    SK_TRY(sk_colsum_launch(da, G + o.b1, csp, M, F, F, accumulate, s));
+    SK_TRY(sk_layernorm_bwd_launch(dh, xmid, P + o.ln2w, st2, st2 + M, dxA, dxB, G + o.ln2w, G + o.ln2b, dwp, dbp, M, d,
+                                   accumulate, s));
+    // attention: dy = dxB
+    SK_TRY(linear_dgrad(M, d, d, dxB, P + o.wo, dao, s));
+    SK_TRY(linear_wgrad(M, d, d, dxB, ao, G + o.wo, accumulate, s, sws, swb));
+    SK_TRY(sk_colsum_launch(dxB, G + o.bo, csp, M, d, d, accumulate, s));
+    SK_TRY(sk_attn_tc_bwd_launch(qkv, ao, dao, lse, wsp<float>(lm, w.delta), nullptr, dqkv, B, T, lm->H, lm->H, Q, d, Q, 1,
+                                 scale, s, seg_start, seg_end));
+    SK_TRY(sk_colsum_launch(dqkv, G + o.bqkv, csp, M, Q, Q, accumulate, s));
+    SK_TRY(linear_dgrad(M, Q, d, dqkv, P + o.wqkv, dh, s));
+    SK_TRY(linear_wgrad(M, Q, d, dqkv, h1, G + o.wqkv, accumulate, s, sws, swb));
+    SK_TRY(sk_layernorm_bwd_launch(dh, x, P + o.ln1w, st1, st1 + M, dxB, dxA, G + o.ln1w, G + o.ln1b, dwp, dbp, M, d,
+                                   accumulate, s));
+    if (!lm->bwd_events.empty()) SK_CUDA_CHECK(cudaEventRecord(lm->bwd_events[l], s));
+  }
+  SK_TRY(sk_embed_bwd_launch(ids, dxA, wsp<float>(lm, w.embed_scratch), G + lm->off_embed, M, d, lm->V, lm->Vp,
+                             lm->cfg.tie_embeddings ? 1 : accumulate, s));
+  return sk_opt_pos_bwd_launch(pos_ids, dxA, wsp<float>(lm, w.embed_scratch), G + lm->off_pos, M, T, d, lm->n_pos, accumulate, s);
+}
+
+// One token per row at position pos[b] (read on the device: the step is graph-capturable).  The KV cache layout is the
+// Qwen2 one with KVH = H.
+int opt_decode_step(SkLm* lm, const int64_t* tokens, const int32_t* pos, int B, void* kv_cache, int T_cache, void* logits,
+                    int ldl, uint8_t* dws, const DecLayout& dl, cudaStream_t s) {
+  const int d = lm->d, F = lm->F, Q = lm->qkv_dim;
+  const float eps = lm->cfg.rms_eps;
+  const bf16* P = lm->params;
+  bf16* x = reinterpret_cast<bf16*>(dws + dl.x0);
+  bf16* xm = reinterpret_cast<bf16*>(dws + dl.x1);
+  bf16* h = reinterpret_cast<bf16*>(dws + dl.h);
+  bf16* qkv = reinterpret_cast<bf16*>(dws + dl.qkv);
+  bf16* ao = reinterpret_cast<bf16*>(dws + dl.ao);
+  bf16* a = reinterpret_cast<bf16*>(dws + dl.gu);
+  int32_t* lens = reinterpret_cast<int32_t*>(dws + dl.lens);
+  float* partial = reinterpret_cast<float*>(dws + dl.partial);
+  void* gemm_ws = dws + dl.gemm;
+  const size_t plane = (size_t)B * lm->H * T_cache * lm->hd;
+  const float scale = 1.0f / sqrtf((float)lm->hd);
+  SK_TRY(sk_opt_embed_fwd_launch(tokens, pos, P + lm->off_embed, P + lm->off_pos, x, B, 1, d, lm->V, lm->n_pos, s));
+  for (int l = 0; l < lm->L; ++l) {
+    const OptLayerOff& o = lm->olo[l];
+    bf16* kc = reinterpret_cast<bf16*>(kv_cache) + (size_t)l * 2 * plane;
+    bf16* vc = kc + plane;
+    SK_TRY(sk_layernorm_fwd_launch(x, P + o.ln1w, P + o.ln1b, h, nullptr, nullptr, B, d, eps, s));
+    SK_TRY(linear_fwd(B, Q, d, h, P + o.wqkv, qkv, P + o.bqkv, nullptr, s));
+    SK_TRY(sk_kv_append_launch(qkv, Q, kc, vc, pos, lens, B, lm->H, lm->H, T_cache, s));
+    SK_TRY(sk_attn_decode_launch(qkv, Q, kc, vc, lens, ao, d, partial, B, lm->H, lm->H, T_cache, scale, s));
+    SK_TRY(linear_fwd(B, d, d, ao, P + o.wo, xm, P + o.bo, x, s));
+    SK_TRY(sk_layernorm_fwd_launch(xm, P + o.ln2w, P + o.ln2b, h, nullptr, nullptr, B, d, eps, s));
+    SK_TRY(sk_gemm_launch(B, F, d, h, d, 0, P + o.w1, d, 0, a, F, 0, P + o.b1, nullptr, 0, 0, 2, 0, s));
+    // fc2 + bias + residual into x (not in place): with M = B the scratch lets stream-K spread the long K loop over idle
+    // SMs; rounded before the residual add like the forward pass
+    SK_TRY(sk_gemm_launch(B, d, F, a, F, 0, P + o.w2, F, 0, x, d, 0, P + o.b2, xm, d, 1, 0, 0, s, gemm_ws,
+                          (size_t)dl.gemm_bytes));
+  }
+  SK_TRY(sk_layernorm_fwd_launch(x, P + lm->off_final_norm, P + lm->off_final_norm_b, h, nullptr, nullptr, B, d, eps, s));
+  return sk_gemm_launch(B, lm->Vp, d, h, d, 0, P + lm->off_head, d, 0, logits, ldl, 0, nullptr, nullptr, 0, 0, 0, 0, s);
+}
+
+// gradient-norm groups (one per HF parameter) and their device chunk tables; `groups` lists (offset, n) ranges
+int upload_norm_groups(SkLm* lm, const std::vector<std::vector<std::pair<int64_t, int64_t>>>& groups) {
+  std::vector<long> cs;
+  std::vector<int> cl, tb;
+  for (const auto& g : groups) {
+    tb.push_back((int)cs.size());
+    for (const auto& r : g)
+      for (int64_t o = 0; o < r.second; o += GN_CHUNK) {
+        cs.push_back((long)(r.first + o));
+        cl.push_back((int)((r.second - o) < GN_CHUNK ? (r.second - o) : GN_CHUNK));
+      }
+  }
+  lm->n_norm_groups = (int)tb.size();
+  tb.push_back((int)cs.size());
+  lm->n_chunks = (int)cs.size();
+  SK_CUDA_CHECK(cudaMalloc(&lm->d_chunk_start, cs.size() * sizeof(long)));
+  SK_CUDA_CHECK(cudaMalloc(&lm->d_chunk_len, cl.size() * sizeof(int)));
+  SK_CUDA_CHECK(cudaMalloc(&lm->d_tensor_chunk_begin, tb.size() * sizeof(int)));
+  SK_CUDA_CHECK(cudaMalloc(&lm->d_chunk_partial, cs.size() * sizeof(float)));
+  SK_CUDA_CHECK(cudaMemcpy(lm->d_chunk_start, cs.data(), cs.size() * sizeof(long), cudaMemcpyHostToDevice));
+  SK_CUDA_CHECK(cudaMemcpy(lm->d_chunk_len, cl.data(), cl.size() * sizeof(int), cudaMemcpyHostToDevice));
+  SK_CUDA_CHECK(cudaMemcpy(lm->d_tensor_chunk_begin, tb.data(), tb.size() * sizeof(int), cudaMemcpyHostToDevice));
+  return 0;
+}
+
 }  // namespace
 
 extern "C" {
@@ -378,12 +639,13 @@ int sk_lm_prefill(SkLm* lm, const int64_t* ids, const int32_t* lens, int B, int 
   const DecLayout dl = make_dec_layout(lm, B, T_cache);
   SK_TRY(check_decode(lm, B, T_cache, ldl, kv_cache, logits, decode_ws, decode_ws_bytes, dl));
   SK_REQUIRE(T > 0 && T <= T_cache, "sk_lm_prefill: prompt width T=%d must be in [1, T_cache=%d]", T, T_cache);
-  const WsLayout w = make_layout(lm, B, T);
+  const WsLayout w = layout_of(lm, B, T);
   SK_TRY(check_bound(lm, B, T, w, nullptr));
   cudaStream_t s = (cudaStream_t)stream;
   uint8_t* dws = reinterpret_cast<uint8_t*>(decode_ws);
   SK_CUDA_CHECK(cudaMemsetAsync(dws + dl.gemm + dl.gemm_bytes - 4096, 0, 4096, s));
-  SK_TRY(forward_impl(lm, ids, nullptr, nullptr, B, T, 0.f, 1.f, false, nullptr, w, s, nullptr, false));
+  if (lm->arch == SK_ARCH_OPT) SK_TRY(opt_forward(lm, ids, nullptr, nullptr, B, T, 0.f, 1.f, false, nullptr, w, s, nullptr, false));
+  else                         SK_TRY(forward_impl(lm, ids, nullptr, nullptr, B, T, 0.f, 1.f, false, nullptr, w, s, nullptr, false));
   SK_TRY(sk_kv_prefill_launch(wsp<bf16>(lm, w.qkv), w.sqkv / 2, lm->qkv_dim, reinterpret_cast<bf16*>(kv_cache), lens, lm->L, B,
                               T, lm->H, lm->KVH, T_cache, s));
   bf16* hl = reinterpret_cast<bf16*>(dws + dl.h);
@@ -398,6 +660,8 @@ int sk_lm_decode_step(SkLm* lm, const int64_t* tokens, const int32_t* pos, int B
   const DecLayout dl = make_dec_layout(lm, B, T_cache);
   SK_TRY(check_decode(lm, B, T_cache, ldl, kv_cache, logits, decode_ws, decode_ws_bytes, dl));
   cudaStream_t s = (cudaStream_t)stream;
+  if (lm->arch == SK_ARCH_OPT)
+    return opt_decode_step(lm, tokens, pos, B, kv_cache, T_cache, logits, ldl, reinterpret_cast<uint8_t*>(decode_ws), dl, s);
   const int d = lm->d, F = lm->F, Q = lm->qkv_dim;
   const bf16* P = lm->params;
   uint8_t* dws = reinterpret_cast<uint8_t*>(decode_ws);
@@ -526,6 +790,91 @@ int sk_lm_create(const SkLmConfig* cfg, SkLm** out) {
   return 0;
 }
 
+int sk_lm_create_opt(const SkOptConfig* cfg, SkLm** out) {
+  SK_REQUIRE(cfg && out, "sk_lm_create_opt: null argument");
+  SK_REQUIRE(cfg->n_heads > 0 && cfg->hidden == 64 * cfg->n_heads, "sk_lm_create_opt: only head_dim 64 is supported (hidden %d, %d heads)",
+             cfg->hidden, cfg->n_heads);
+  SK_REQUIRE(cfg->hidden <= 2048, "sk_lm_create_opt: hidden must be <= 2048 (got %d)", cfg->hidden);
+  SK_REQUIRE(cfg->ffn > 0 && cfg->ffn % 8 == 0, "sk_lm_create_opt: ffn must be a positive multiple of 8 (got %d)", cfg->ffn);
+  SK_REQUIRE(cfg->n_layers > 0 && cfg->max_positions > 0, "sk_lm_create_opt: n_layers and max_positions must be positive");
+  SK_REQUIRE(cfg->vocab_size > 0 && cfg->vocab_size <= (1 << 20), "sk_lm_create_opt: vocab_size must be in [1, 2^20]");
+  SkLm* lm = new SkLm();
+  lm->arch = SK_ARCH_OPT;
+  lm->cfg.vocab_size = cfg->vocab_size;
+  lm->cfg.hidden = cfg->hidden;
+  lm->cfg.n_layers = cfg->n_layers;
+  lm->cfg.n_heads = cfg->n_heads;
+  lm->cfg.n_kv_heads = cfg->n_heads;
+  lm->cfg.head_dim = 64;
+  lm->cfg.ffn = cfg->ffn;
+  lm->cfg.max_positions = cfg->max_positions;
+  lm->cfg.rms_eps = cfg->ln_eps;
+  lm->cfg.tie_embeddings = cfg->tie_embeddings;
+  lm->cfg.qkv_bias = 1;
+  lm->d = cfg->hidden;
+  lm->F = cfg->ffn;
+  lm->H = lm->KVH = cfg->n_heads;
+  lm->hd = 64;
+  lm->L = cfg->n_layers;
+  lm->V = cfg->vocab_size;
+  lm->Vp = (cfg->vocab_size + 63) / 64 * 64;
+  lm->qkv_dim = 3 * lm->d;
+  lm->n_pos = cfg->max_positions + 2;   // OPTLearnedPositionalEmbedding: offset 2
+  lm->head_chunk = lm->Vp > 8192 ? 2048 : 0;
+  if (const char* e = getenv("SK_HEAD_CHUNK")) lm->head_chunk = (atoi(e) / 128) * 128;
+  const int d = lm->d, F = lm->F;
+  lm->olo.resize(lm->L);
+  for (int l = 0; l < lm->L; ++l) {
+    const std::string p = "layers." + std::to_string(l) + ".";
+    OptLayerOff& o = lm->olo[l];
+    o.ln1w = add_tensor(lm, p + "ln1", 1, d);
+    o.ln1b = add_tensor(lm, p + "ln1_b", 1, d);
+    o.wqkv = add_tensor(lm, p + "wqkv", 3 * d, d);
+    o.bqkv = add_tensor(lm, p + "bqkv", 1, 3 * d);
+    o.wo = add_tensor(lm, p + "wo", d, d);
+    o.bo = add_tensor(lm, p + "bo", 1, d);
+    o.ln2w = add_tensor(lm, p + "ln2", 1, d);
+    o.ln2b = add_tensor(lm, p + "ln2_b", 1, d);
+    o.w1 = add_tensor(lm, p + "w1", F, d);
+    o.b1 = add_tensor(lm, p + "b1", 1, F);
+    o.w2 = add_tensor(lm, p + "w2", d, F);
+    o.b2 = add_tensor(lm, p + "b2", 1, d);
+  }
+  lm->off_final_norm = add_tensor(lm, "final_norm", 1, d);
+  lm->off_final_norm_b = add_tensor(lm, "final_norm_b", 1, d);
+  lm->off_embed = add_tensor(lm, "embed", lm->Vp, d);
+  lm->off_pos = add_tensor(lm, "pos_embed", lm->n_pos, d);
+  lm->off_head = cfg->tie_embeddings ? lm->off_embed : add_tensor(lm, "lm_head", lm->Vp, d);
+  // one gradient-norm group per HF parameter, weights and biases apart (torch clip_grad_norm_ over OPTForCausalLM)
+  std::vector<std::vector<std::pair<int64_t, int64_t>>> groups;
+  auto one = [&](int64_t off, int64_t n) { groups.push_back({{off, n}}); };
+  const int64_t dd = (int64_t)d * d;
+  one(lm->off_embed, (int64_t)lm->Vp * d);
+  one(lm->off_pos, (int64_t)lm->n_pos * d);
+  for (int l = 0; l < lm->L; ++l) {
+    const OptLayerOff& o = lm->olo[l];
+    for (int j = 0; j < 3; ++j) {   // q, k, v
+      one(o.wqkv + j * dd, dd);
+      one(o.bqkv + (int64_t)j * d, d);
+    }
+    one(o.wo, dd); one(o.bo, d);
+    one(o.ln1w, d); one(o.ln1b, d);
+    one(o.w1, (int64_t)F * d); one(o.b1, F);
+    one(o.w2, (int64_t)d * F); one(o.b2, d);
+    one(o.ln2w, d); one(o.ln2b, d);
+  }
+  one(lm->off_final_norm, d);
+  one(lm->off_final_norm_b, d);
+  if (!cfg->tie_embeddings) one(lm->off_head, (int64_t)lm->Vp * d);
+  const int rc = upload_norm_groups(lm, groups);
+  if (rc) {
+    sk_lm_destroy(lm);
+    return rc;
+  }
+  *out = lm;
+  return 0;
+}
+
 void sk_lm_destroy(SkLm* lm) {
   if (!lm) return;
   cudaFree(lm->d_chunk_start);
@@ -555,12 +904,13 @@ int sk_lm_tensor_info(const SkLm* lm, int idx, char* name_buf, int name_cap, int
 
 int64_t sk_lm_workspace_bytes(const SkLm* lm, int B, int T) {
   if (!lm || B <= 0 || T <= 0) return 0;
-  return make_layout(lm, B, T).total;
+  return layout_of(lm, B, T).total;
 }
 
 int sk_lm_bind(SkLm* lm, void* params, void* grads, const void* rope_cos, const void* rope_sin, void* workspace,
                int64_t workspace_bytes) {
-  SK_REQUIRE(lm && params && rope_cos && rope_sin && workspace, "sk_lm_bind: null argument");
+  SK_REQUIRE(lm && params && workspace, "sk_lm_bind: null argument");
+  SK_REQUIRE((rope_cos && rope_sin) || lm->arch == SK_ARCH_OPT, "sk_lm_bind: a Qwen2 handle needs the RoPE tables");
   SK_REQUIRE(((uintptr_t)params & 127) == 0 && (grads == nullptr || ((uintptr_t)grads & 127) == 0) &&
                  ((uintptr_t)workspace & 255) == 0,
              "sk_lm_bind: params/grads must be 128-byte and workspace 256-byte aligned");
@@ -572,7 +922,7 @@ int sk_lm_bind(SkLm* lm, void* params, void* grads, const void* rope_cos, const 
   lm->ws_bytes = workspace_bytes;
   // stream-K publish flags (last 4 KB of the GEMM scratch, which sits at a fixed offset) start out zero; the GEMM
   // re-arms them itself after every launch
-  const WsLayout w = make_layout(lm, 1, 1);
+  const WsLayout w = layout_of(lm, 1, 1);
   SK_REQUIRE(workspace_bytes >= w.splitk + w.splitk_bytes, "sk_lm_bind: workspace smaller than the GEMM scratch");
   SK_CUDA_CHECK(cudaMemset(lm->ws + w.splitk + w.splitk_bytes - 4096, 0, 4096));
   SK_CUDA_CHECK(cudaDeviceSynchronize());
@@ -583,8 +933,10 @@ int sk_lm_forward(SkLm* lm, const int64_t* ids, const int64_t* labels, const int
                   float num_items, float* stats, void* stream) {
   SK_REQUIRE(lm && ids, "sk_lm_forward: null argument");
   SK_REQUIRE(labels == nullptr || stats != nullptr, "sk_lm_forward: stats is required when labels are given");
-  const WsLayout w = make_layout(lm, B, T);
+  const WsLayout w = layout_of(lm, B, T);
   SK_TRY(check_bound(lm, B, T, w, pos_ids));
+  if (lm->arch == SK_ARCH_OPT)
+    return opt_forward(lm, ids, labels, pos_ids, B, T, num_items, 1.0f, false, stats, w, (cudaStream_t)stream);
   return forward_impl(lm, ids, labels, pos_ids, B, T, num_items, 1.0f, false, stats, w, (cudaStream_t)stream);
 }
 
@@ -592,8 +944,18 @@ int sk_lm_forward_backward(SkLm* lm, const int64_t* ids, const int64_t* labels, 
                            float num_items, float dloss, int accumulate, float* stats, void* stream) {
   SK_REQUIRE(lm && ids && labels && stats, "sk_lm_forward_backward: null argument");
   SK_REQUIRE(lm->grads, "sk_lm_forward_backward: no gradient buffer bound");
-  const WsLayout w = make_layout(lm, B, T);
+  const WsLayout w = layout_of(lm, B, T);
   SK_TRY(check_bound(lm, B, T, w, pos_ids));
+  if (lm->arch == SK_ARCH_OPT) {
+    cudaStream_t s = (cudaStream_t)stream;
+    if (lm->head_chunk > 0) {
+      SK_TRY(opt_forward(lm, ids, labels, pos_ids, B, T, num_items, dloss, true, stats, w, s, nullptr, false));
+      SK_TRY(head_chunked(lm, labels, B, T, num_items, dloss, accumulate, stats, w, s));
+      return opt_backward(lm, ids, pos_ids, B, T, accumulate, w, s, false);
+    }
+    SK_TRY(opt_forward(lm, ids, labels, pos_ids, B, T, num_items, dloss, true, stats, w, s));
+    return opt_backward(lm, ids, pos_ids, B, T, accumulate, w, s);
+  }
   if (lm->head_chunk > 0) {
     SK_TRY(forward_impl(lm, ids, labels, pos_ids, B, T, num_items, dloss, true, stats, w, (cudaStream_t)stream, nullptr, false));
     SK_TRY(head_chunked(lm, labels, B, T, num_items, dloss, accumulate, stats, w, (cudaStream_t)stream));
@@ -618,8 +980,10 @@ int sk_lm_set_backward_events(SkLm* lm, void* const* events, int n) {
 int sk_lm_forward_rows(SkLm* lm, const int64_t* ids, const int64_t* labels, const int32_t* pos_ids, int B, int T,
                        float* row_nll, float* stats, void* stream) {
   SK_REQUIRE(lm && ids && labels && row_nll && stats, "sk_lm_forward_rows: null argument");
-  const WsLayout w = make_layout(lm, B, T);
+  const WsLayout w = layout_of(lm, B, T);
   SK_TRY(check_bound(lm, B, T, w, pos_ids));
+  if (lm->arch == SK_ARCH_OPT)
+    return opt_forward(lm, ids, labels, pos_ids, B, T, 1.0f, 1.0f, false, stats, w, (cudaStream_t)stream, row_nll);
   return forward_impl(lm, ids, labels, pos_ids, B, T, 1.0f, 1.0f, false, stats, w, (cudaStream_t)stream, row_nll);
 }
 
@@ -628,19 +992,20 @@ int sk_lm_backward_weighted(SkLm* lm, const int64_t* ids, const int64_t* labels,
   SK_REQUIRE(lm && ids && labels && row_weight && stats, "sk_lm_backward_weighted: null argument");
   SK_REQUIRE(lm->grads, "sk_lm_backward_weighted: no gradient buffer bound");
   SK_REQUIRE(lm->last_B == B && lm->last_T == T, "sk_lm_backward_weighted: call sk_lm_forward_rows on the same batch first");
-  const WsLayout w = make_layout(lm, B, T);
+  const WsLayout w = layout_of(lm, B, T);
   SK_TRY(check_bound(lm, B, T, w, pos_ids));
   cudaStream_t s = (cudaStream_t)stream;
   // d loss / d logits[row] = row_weight[row] * (softmax - onehot): recomputed from the logits the forward pass left in
   // the workspace (num_items = 1, dloss = 1: the caller's weights carry every scale factor)
   SK_TRY(sk_ce_launch(wsp<bf16>(lm, w.logits), labels, wsp<bf16>(lm, w.dlogits), wsp<float>(lm, w.ce_partial), nullptr,
                       stats, B * T, T, lm->V, lm->Vp, 1.0f, 1.0f, s, row_weight));
+  if (lm->arch == SK_ARCH_OPT) return opt_backward(lm, ids, pos_ids, B, T, accumulate, w, s);
   return backward_impl(lm, ids, pos_ids, B, T, accumulate, w, s);
 }
 
 const void* sk_lm_logits(const SkLm* lm) {
   if (!lm || !lm->ws || lm->last_B == 0) return nullptr;
-  return lm->ws + make_layout(lm, lm->last_B, lm->last_T).logits;
+  return lm->ws + layout_of(lm, lm->last_B, lm->last_T).logits;
 }
 int sk_lm_logits_ld(const SkLm* lm) { return lm ? lm->Vp : 0; }
 

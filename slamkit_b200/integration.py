@@ -40,17 +40,32 @@ def hubert_b200_from_cfg(pretrained_model: str = "facebook/hubert-base-ls960",
 
 def tlm_b200_from_cfg(cfg, device: str = "cuda:0", max_batch: int = 8, max_seq: Optional[int] = None):
     """`cfg` is the reference's model config node (config/model/*.yaml): context_len, config_args{base_model_name,
-    vocab_size, twist_init, rope_theta, ...}.  Raises OSError when the base model cannot be reached (offline box) and
-    ValueError when its architecture has no kernels here (anything but Qwen2)."""
+    vocab_size, twist_init, rope_theta, torch_dtype, dropout, ...}.  The base config decides the decoder: Qwen2
+    (`LMConfig`) or pre-LayerNorm OPT (`OptLMConfig`, the default TWIST / GSLM base).  For OPT the reference's
+    `config_args` overrides are applied to the base config as `UnitLMConfig` does (pad / bos / eos ids, dropout,
+    attention_dropout, layerdrop), `rope_theta` is ignored, and `torch_dtype: bfloat16` is required: this path keeps bf16
+    parameters and bf16 AdamW moments, while the reference run with `torch_dtype: null` keeps fp32 master weights.
+    Raises OSError when the base model cannot be reached (offline box) and ValueError when its architecture or settings
+    have no kernels here."""
     from transformers import AutoConfig
-    from .lm import B200UnitLM, LMConfig
+    from .lm import B200UnitLM, OptLMConfig, lm_config_from_hf
 
     args = cfg["config_args"] if isinstance(cfg, dict) else cfg.config_args
     get = args.get if hasattr(args, "get") else (lambda k, d=None: getattr(args, k, d))
     base = AutoConfig.from_pretrained(get("base_model_name"))
     ctx = int(cfg["context_len"] if isinstance(cfg, dict) else cfg.context_len)
-    lm_cfg = LMConfig.from_hf(base, vocab_size=get("vocab_size", 502), max_positions=max(2048, ctx))
-    if get("rope_theta") is not None:
+    if getattr(base, "model_type", None) == "opt":
+        # slamkit/model/unit_lm.py:59-63 passes these to AutoConfig.from_pretrained; the yaml's dropout keys arrive as
+        # the same keyword arguments
+        for k in ("pad_token_id", "bos_token_id", "eos_token_id", "dropout", "attention_dropout", "layerdrop"):
+            if get(k) is not None:
+                setattr(base, k, get(k))
+        dt = get("torch_dtype")
+        if str(dt).replace("torch.", "") != "bfloat16":
+            raise ValueError(f"OPT on the GPU path trains bf16 parameters with bf16 AdamW moments; torch_dtype={dt} asks for "
+                             "fp32 master weights, which it does not implement (pass model.config_args.torch_dtype=bfloat16)")
+    lm_cfg = lm_config_from_hf(base, vocab_size=get("vocab_size", 502), max_positions=max(2048, ctx))
+    if get("rope_theta") is not None and not isinstance(lm_cfg, OptLMConfig):
         lm_cfg.rope_theta = float(get("rope_theta"))
     model = B200UnitLM(lm_cfg, device=device, max_batch=max_batch, max_seq=int(max_seq or ctx))
     if get("twist_init", True):

@@ -57,6 +57,75 @@ class LMConfig:
             pad_token_id=cfg.pad_token_id or 0)
 
 
+@dataclass
+class OptLMConfig:
+    """Shape of a pre-LayerNorm OPT decoder (defaults = facebook/opt-125m with the 502-entry unit vocabulary, the base of
+    config/model/twist.yaml and gslm.yaml).  `max_positions` is the checkpoint's `max_position_embeddings`: the learned
+    position table has max_positions + 2 rows (HF OPTLearnedPositionalEmbedding, offset 2)."""
+    vocab_size: int = 502
+    hidden: int = 768
+    n_layers: int = 12
+    n_heads: int = 12
+    ffn: int = 3072
+    max_positions: int = 2048
+    ln_eps: float = 1e-5
+    tie_embeddings: bool = True
+    pad_token_id: int = 0
+    bos_token_id: int = 1
+    eos_token_id: int = 1
+    init_std: float = 0.02
+    head_dim: int = 64
+
+    @staticmethod
+    def from_hf(cfg, vocab_size: Optional[int] = None) -> "OptLMConfig":
+        """From an HF `OPTConfig`.  Only what the sm_90a kernels implement is accepted; every other variant is refused by
+        name: post-LayerNorm OPT and the project_in / project_out pair (opt-350m), the legacy `_remove_final_layer_norm`,
+        bias-free linears, non-affine LayerNorms, activations other than ReLU, head_dim other than 64, and any dropout or
+        layerdrop (there are no dropout kernels: set them to 0.0 as config/model/default.yaml does)."""
+        if getattr(cfg, "model_type", None) != "opt":
+            raise ValueError(f"OptLMConfig.from_hf: model_type is '{getattr(cfg, 'model_type', None)}', not 'opt'")
+        if not getattr(cfg, "do_layer_norm_before", True):
+            raise ValueError("unsupported OPT variant: do_layer_norm_before=False (post-LayerNorm OPT, e.g. opt-350m)")
+        if getattr(cfg, "word_embed_proj_dim", cfg.hidden_size) != cfg.hidden_size:
+            raise ValueError(f"unsupported OPT variant: word_embed_proj_dim={cfg.word_embed_proj_dim} != hidden_size="
+                             f"{cfg.hidden_size} (project_in / project_out, e.g. opt-350m)")
+        if getattr(cfg, "_remove_final_layer_norm", False):
+            raise ValueError("unsupported OPT variant: _remove_final_layer_norm=True")
+        if not getattr(cfg, "enable_bias", True):
+            raise ValueError("unsupported OPT variant: enable_bias=False")
+        if not getattr(cfg, "layer_norm_elementwise_affine", True):
+            raise ValueError("unsupported OPT variant: layer_norm_elementwise_affine=False")
+        if getattr(cfg, "activation_function", "relu") != "relu":
+            raise ValueError(f"unsupported OPT variant: activation_function='{cfg.activation_function}' (only relu)")
+        if cfg.hidden_size % cfg.num_attention_heads or cfg.hidden_size // cfg.num_attention_heads != 64:
+            raise ValueError(f"unsupported attention geometry: hidden_size / num_attention_heads = "
+                             f"{cfg.hidden_size / cfg.num_attention_heads:g}; the sm_90a attention kernels need head_dim 64")
+        for k in ("dropout", "attention_dropout", "layerdrop"):
+            if float(getattr(cfg, k, 0.0) or 0.0) != 0.0:
+                raise ValueError(f"unsupported OPT setting: {k}={getattr(cfg, k)} (there are no dropout kernels; set it to 0.0)")
+        return OptLMConfig(
+            vocab_size=vocab_size or cfg.vocab_size, hidden=cfg.hidden_size, n_layers=cfg.num_hidden_layers,
+            n_heads=cfg.num_attention_heads, ffn=cfg.ffn_dim, max_positions=cfg.max_position_embeddings,
+            tie_embeddings=bool(getattr(cfg, "tie_word_embeddings", True)),
+            pad_token_id=cfg.pad_token_id if cfg.pad_token_id is not None else 0,
+            bos_token_id=cfg.bos_token_id if cfg.bos_token_id is not None else 1,
+            eos_token_id=cfg.eos_token_id if cfg.eos_token_id is not None else 1,
+            init_std=float(getattr(cfg, "init_std", 0.02)))
+
+
+def lm_config_from_hf(base, vocab_size: Optional[int] = None, max_positions: int = 2048):
+    """The decoder config for an HF base config, by `model_type`: `LMConfig` for qwen2 (RoPE tables of `max_positions`
+    rows), `OptLMConfig` for opt (its own learned position table; `max_positions` is ignored).  Anything else is
+    refused."""
+    mt = getattr(base, "model_type", None)
+    if mt == "opt":
+        return OptLMConfig.from_hf(base, vocab_size=vocab_size)
+    if mt == "qwen2":
+        return LMConfig.from_hf(base, vocab_size=vocab_size, max_positions=max_positions)
+    raise ValueError(f"unsupported base architecture '{mt}': the GPU path implements the Qwen2 and pre-LayerNorm OPT "
+                     "decoders")
+
+
 def rope_tables(theta: float, head_dim: int, max_positions: int) -> Tuple[torch.Tensor, torch.Tensor]:
     """cos/sin tables exactly as HF computes them (HF:models/qwen2/modeling_qwen2.py Qwen2RotaryEmbedding.forward):
     fp32 inv_freq, fp32 outer product, cos()/sin(), then cast to the activation dtype (bf16). Shape [P, head_dim/2]."""
@@ -73,8 +142,19 @@ class LMOutput:
     stats: Optional[torch.Tensor] = None   # device fp32[3]: loss, n_valid_targets, nll_sum
 
 
-def write_unit_lm_checkpoint(save_directory: str, state_dict_hf: Dict[str, torch.Tensor], config: "LMConfig",
-                             base_model_name: str = "Qwen/Qwen2.5-0.5B") -> None:
+def _opt_base_config(c: "OptLMConfig") -> dict:
+    """The HF `OPTConfig` fields of a pre-LayerNorm OPT decoder of this shape (opt-125m layout)."""
+    return {"model_type": "opt", "architectures": ["OPTForCausalLM"], "hidden_size": c.hidden, "ffn_dim": c.ffn,
+            "num_hidden_layers": c.n_layers, "num_attention_heads": c.n_heads, "vocab_size": c.vocab_size,
+            "max_position_embeddings": c.max_positions, "do_layer_norm_before": True, "word_embed_proj_dim": c.hidden,
+            "activation_function": "relu", "enable_bias": True, "layer_norm_elementwise_affine": True,
+            "_remove_final_layer_norm": False, "dropout": 0.0, "attention_dropout": 0.0, "layerdrop": 0.0,
+            "init_std": c.init_std, "tie_word_embeddings": c.tie_embeddings, "pad_token_id": c.pad_token_id,
+            "bos_token_id": c.bos_token_id, "eos_token_id": c.eos_token_id, "torch_dtype": "bfloat16"}
+
+
+def write_unit_lm_checkpoint(save_directory: str, state_dict_hf: Dict[str, torch.Tensor], config,
+                             base_model_name: Optional[str] = None) -> None:
     """Writes `model.safetensors` with the `lm.`-prefixed names of `UnitLM.state_dict()` (base_model_prefix = "lm",
     slamkit/model/unit_lm.py:87) and a `config.json` in the `UnitLMConfig` layout (unit_lm.py:32-79), so that the
     reference's `UnitLM.from_pretrained(dir)` / cli/eval.py consume a model trained with this package.  Pure host code (no CUDA):
@@ -84,10 +164,13 @@ def write_unit_lm_checkpoint(save_directory: str, state_dict_hf: Dict[str, torch
     from safetensors.torch import save_file
     os.makedirs(save_directory, exist_ok=True)
     c = config
+    is_opt = isinstance(c, OptLMConfig)
+    if base_model_name is None:
+        base_model_name = "facebook/opt-125m" if is_opt else "Qwen/Qwen2.5-0.5B"
     sd = {k: v.detach().contiguous().cpu() for k, v in state_dict_hf.items()
           if k != "lm.lm_head.weight" or not c.tie_embeddings}
     save_file(sd, os.path.join(save_directory, "model.safetensors"), metadata={"format": "pt"})
-    base = {"model_type": "qwen2", "architectures": ["Qwen2ForCausalLM"], "hidden_size": c.hidden,
+    base = _opt_base_config(c) if is_opt else {"model_type": "qwen2", "architectures": ["Qwen2ForCausalLM"], "hidden_size": c.hidden,
             "intermediate_size": c.ffn, "num_hidden_layers": c.n_layers, "num_attention_heads": c.n_heads,
             "num_key_value_heads": c.n_kv_heads, "vocab_size": c.vocab_size, "rms_norm_eps": c.rms_eps,
             "max_position_embeddings": c.max_positions, "tie_word_embeddings": c.tie_embeddings, "hidden_act": "silu",
@@ -120,17 +203,24 @@ def check_right_padded(attention_mask: Optional[torch.Tensor]) -> None:
 class B200UnitLM:
     """Causal unit LM whose forward/backward/optimiser run in libslamkit_b200.so."""
 
-    def __init__(self, config: LMConfig, device: str = "cuda:0", max_batch: int = 8, max_seq: int = 1024,
+    def __init__(self, config, device: str = "cuda:0", max_batch: int = 8, max_seq: int = 1024,
                  trainable: bool = True, seed: Optional[int] = None):
+        """`config`: `LMConfig` (Qwen2 decoder) or `OptLMConfig` (pre-LayerNorm OPT decoder)."""
         self.lib = L.require_cuda()
         self.config = config
+        self.is_opt = isinstance(config, OptLMConfig)
         self.device = torch.device(device)
         torch.cuda.set_device(self.device)
-        c = L.SkLmConfig(config.vocab_size, config.hidden, config.n_layers, config.n_heads, config.n_kv_heads,
-                         config.head_dim, config.ffn, config.max_positions, config.rms_eps,
-                         int(config.tie_embeddings), int(config.qkv_bias))
         self._h = C.c_void_p()
-        L.check(self.lib.sk_lm_create(C.byref(c), C.byref(self._h)))
+        if self.is_opt:
+            c = L.SkOptConfig(config.vocab_size, config.hidden, config.n_layers, config.n_heads, config.ffn,
+                              config.max_positions, config.ln_eps, int(config.tie_embeddings))
+            L.check(self.lib.sk_lm_create_opt(C.byref(c), C.byref(self._h)))
+        else:
+            c = L.SkLmConfig(config.vocab_size, config.hidden, config.n_layers, config.n_heads, config.n_kv_heads,
+                             config.head_dim, config.ffn, config.max_positions, config.rms_eps,
+                             int(config.tie_embeddings), int(config.qkv_bias))
+            L.check(self.lib.sk_lm_create(C.byref(c), C.byref(self._h)))
         self.n_params = int(self.lib.sk_lm_param_count(self._h))
         self.tensors: Dict[str, Tuple[int, int, int]] = {}
         n = self.lib.sk_lm_tensor_info(self._h, -1, None, 0, None, None, None)
@@ -142,8 +232,10 @@ class B200UnitLM:
         self.vocab_padded = self.tensors["embed"][1]
         self.params = torch.zeros(self.n_params, device=self.device, dtype=torch.bfloat16)
         self.grads = torch.zeros(self.n_params, device=self.device, dtype=torch.bfloat16) if trainable else None
-        cos, sin = rope_tables(config.rope_theta, config.head_dim, config.max_positions)
-        self.rope_cos, self.rope_sin = cos.to(self.device), sin.to(self.device)
+        self.rope_cos = self.rope_sin = None          # OPT: learned positions, no RoPE tables
+        if not self.is_opt:
+            cos, sin = rope_tables(config.rope_theta, config.head_dim, config.max_positions)
+            self.rope_cos, self.rope_sin = cos.to(self.device), sin.to(self.device)
         self.max_batch, self.max_seq = max_batch, max_seq
         self.workspace = None
         self._bind(max_batch, max_seq)
@@ -181,6 +273,8 @@ class B200UnitLM:
     def init_weights(self, seed: int = 0, std: float = 0.02) -> None:
         """HF `_init_weights` equivalent: normal(0, std) for linear/embedding weights, zeros for biases, ones for
         norms (HF:modeling_utils.py PreTrainedModel._init_weights)."""
+        if self.is_opt:
+            return self._init_weights_opt(seed)
         g = torch.Generator(device="cpu").manual_seed(seed)
         V = self.config.vocab_size
         for name, (off, r, c) in self.tensors.items():
@@ -196,12 +290,63 @@ class B200UnitLM:
             else:
                 t.copy_((torch.randn((r, c), generator=g) * std).to(torch.bfloat16))
 
+    def _init_weights_opt(self, seed: int) -> None:
+        """HF OPT init (PreTrainedModel._init_weights with config.init_std): normal(0, init_std) for the linear weights
+        and both embedding tables, zero for the token table's pad_token_id row (nn.Embedding(padding_idx)), LayerNorm
+        weights 1 and biases 0, linear biases 0."""
+        g = torch.Generator(device="cpu").manual_seed(seed)
+        cfg = self.config
+        std = cfg.init_std
+        for name, (off, r, c) in self.tensors.items():
+            t = self.params[off:off + r * c].view(r, c)
+            base = name.split(".")[-1]
+            if base in ("ln1", "ln2", "final_norm"):
+                t.fill_(1.0)
+            elif r == 1:                                   # LayerNorm and linear biases
+                t.zero_()
+            elif base in ("embed", "lm_head"):
+                t.zero_()
+                t[:cfg.vocab_size].copy_((torch.randn((cfg.vocab_size, c), generator=g) * std).to(torch.bfloat16))
+                if base == "embed" and 0 <= cfg.pad_token_id < cfg.vocab_size:
+                    t[cfg.pad_token_id].zero_()
+            else:
+                t.copy_((torch.randn((r, c), generator=g) * std).to(torch.bfloat16))
+
+    def _hf_map_opt(self) -> Iterator[Tuple[str, str, List[Tuple[int, int, int]]]]:
+        """OPT names of `UnitLM.state_dict()` over OPTForCausalLM: q/k/v are row ranges of the fused `wqkv` / `bqkv`."""
+        cfg = self.config
+        d = cfg.hidden
+        for l in range(cfg.n_layers):
+            p, h = f"layers.{l}.", f"lm.model.decoder.layers.{l}."
+            yield p + "ln1", h + "self_attn_layer_norm.weight", [(0, 0, 1)]
+            yield p + "ln1_b", h + "self_attn_layer_norm.bias", [(0, 0, 1)]
+            for j, n in enumerate("qkv"):
+                yield p + "wqkv", h + f"self_attn.{n}_proj.weight", [(j * d, 0, d)]
+                yield p + "bqkv", h + f"self_attn.{n}_proj.bias", [(j * d, 0, d)]
+            yield p + "wo", h + "self_attn.out_proj.weight", [(0, 0, d)]
+            yield p + "bo", h + "self_attn.out_proj.bias", [(0, 0, 1)]
+            yield p + "ln2", h + "final_layer_norm.weight", [(0, 0, 1)]
+            yield p + "ln2_b", h + "final_layer_norm.bias", [(0, 0, 1)]
+            yield p + "w1", h + "fc1.weight", [(0, 0, cfg.ffn)]
+            yield p + "b1", h + "fc1.bias", [(0, 0, 1)]
+            yield p + "w2", h + "fc2.weight", [(0, 0, d)]
+            yield p + "b2", h + "fc2.bias", [(0, 0, 1)]
+        yield "final_norm", "lm.model.decoder.final_layer_norm.weight", [(0, 0, 1)]
+        yield "final_norm_b", "lm.model.decoder.final_layer_norm.bias", [(0, 0, 1)]
+        yield "embed", "lm.model.decoder.embed_tokens.weight", [(0, 0, cfg.vocab_size)]
+        yield "pos_embed", "lm.model.decoder.embed_positions.weight", [(0, 0, cfg.max_positions + 2)]
+        if not cfg.tie_embeddings:
+            yield "lm_head", "lm.lm_head.weight", [(0, 0, cfg.vocab_size)]
+
     def _hf_map(self) -> Iterator[Tuple[str, str, List[Tuple[int, int, int]]]]:
         """(flat tensor name, HF parameter name, [(row in the flat tensor, row in the HF tensor, n rows), ...]).
 
         q/k/v are row ranges of the fused `wqkv` / `bqkv`.  gate_proj and up_proj share `wgu` in 128-row blocks --
         flat rows [256b, 256b+128) = gate rows [128b, 128b+128), flat rows [256b+128, 256b+256) = the same up rows -- so
         that one 256-column GEMM tile holds gate AND up of the same hidden units and SwiGLU runs in the GEMM epilogue."""
+        if self.is_opt:
+            yield from self._hf_map_opt()
+            return
         cfg = self.config
         q, kv = cfg.n_heads * cfg.head_dim, cfg.n_kv_heads * cfg.head_dim
         nb = cfg.ffn // 128
@@ -255,11 +400,12 @@ class B200UnitLM:
             v = torch.cat(parts, dim=0) if len(parts) > 1 else parts[0].clone()
             out[hf] = v.view(-1) if flat.endswith("bqkv") else v
         if self.config.tie_embeddings:
-            out["lm.lm_head.weight"] = out["lm.model.embed_tokens.weight"]
+            out["lm.lm_head.weight"] = out["lm.model.decoder.embed_tokens.weight" if self.is_opt else
+                                           "lm.model.embed_tokens.weight"]
         return out
 
     # ---- checkpoints (HF layout, SURVEY.md §5 / §8 f-4) ------------------------------------------------------------
-    def save_pretrained(self, save_directory: str, base_model_name: str = "Qwen/Qwen2.5-0.5B") -> None:
+    def save_pretrained(self, save_directory: str, base_model_name: Optional[str] = None) -> None:
         write_unit_lm_checkpoint(save_directory, self.state_dict_hf(), self.config, base_model_name)
 
     @classmethod
@@ -270,6 +416,15 @@ class B200UnitLM:
         from safetensors.torch import load_file
         cfg = json.load(open(os.path.join(directory, "config.json")))
         b = cfg["base_config"]
+        if b.get("model_type") == "opt":
+            from transformers import OPTConfig
+            b = {k: v for k, v in b.items() if k not in ("model_type", "architectures")}
+            if not trainable:                              # dropout is inactive in eval mode
+                b.update(dropout=0.0, attention_dropout=0.0, layerdrop=0.0)
+            lm_cfg = OptLMConfig.from_hf(OPTConfig(**b), vocab_size=cfg["vocab_size"])
+            m = cls(lm_cfg, device=device, max_batch=max_batch, max_seq=max_seq, trainable=trainable)
+            m.load_hf_state_dict(load_file(os.path.join(directory, "model.safetensors")))
+            return m
         theta = (b.get("rope_parameters") or {}).get("rope_theta", b.get("rope_theta", 10000.0))
         lm_cfg = LMConfig(vocab_size=cfg["vocab_size"], hidden=b["hidden_size"], n_layers=b["num_hidden_layers"],
                           n_heads=b["num_attention_heads"], n_kv_heads=b["num_key_value_heads"],
@@ -473,6 +628,9 @@ class B200UnitLM:
         Lmax = int(lens.max())
         if Lmax > P:
             raise L.SkError(f"generate: a prompt of {Lmax} tokens is longer than max_positions = {P}")
+        if self.is_opt and Lmax + max_new_tokens > P:
+            raise ValueError(f"generate: prompt ({Lmax}) + max_new_tokens ({max_new_tokens}) exceeds the {P} learned positions "
+                             "of the OPT position table")
         T_cache = min(Lmax + max_new_tokens, P)
         # left-padded [B, T] -> right-padded [B, Lmax]: row b's real tokens at positions 0..lens[b]-1
         cols = torch.arange(Lmax)[None, :]

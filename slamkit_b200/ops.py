@@ -131,6 +131,32 @@ def rmsnorm_bwd(dy, x, w, rstd, dres: Optional[torch.Tensor], dw: torch.Tensor, 
     return dx
 
 
+def layernorm_fwd(x: torch.Tensor, w: torch.Tensor, b: torch.Tensor, eps: float):
+    """-> (y bf16 [M, D], mean fp32 [M], rstd fp32 [M])"""
+    lib = L.load()
+    M, D = x.shape
+    y = torch.empty_like(x)
+    mean = torch.empty(M, device=x.device, dtype=torch.float32)
+    rstd = torch.empty(M, device=x.device, dtype=torch.float32)
+    L.check(lib.sk_layernorm_fwd(L.ptr(x), L.ptr(w), L.ptr(b), L.ptr(y), L.ptr(mean), L.ptr(rstd), M, D, L.f32(eps),
+                                 L.stream_ptr()))
+    return y, mean, rstd
+
+
+def layernorm_bwd(dy, x, w, mean, rstd, dres: Optional[torch.Tensor], dw: torch.Tensor, db: torch.Tensor,
+                  accumulate: bool) -> torch.Tensor:
+    """-> dx; dw / db written (or added to)"""
+    lib = L.load()
+    M, D = x.shape
+    dx = torch.empty_like(x)
+    n = lib.sk_layernorm_bwd_blocks() * D
+    pw = torch.empty(n, device=x.device, dtype=torch.float32)
+    pb = torch.empty(n, device=x.device, dtype=torch.float32)
+    L.check(lib.sk_layernorm_bwd(L.ptr(dy), L.ptr(x), L.ptr(w), L.ptr(mean), L.ptr(rstd), L.ptr(dres), L.ptr(dx), L.ptr(dw),
+                                 L.ptr(db), L.ptr(pw), L.ptr(pb), M, D, int(accumulate), L.stream_ptr()))
+    return dx
+
+
 def colsum(x: torch.Tensor, out: torch.Tensor, accumulate: bool) -> torch.Tensor:
     lib = L.require_cuda()
     M, N = x.shape
