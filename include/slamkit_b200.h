@@ -33,7 +33,7 @@ int sk_device_cc(void);                     /* 10*major + minor of the current d
  *   a_mn = 0: A is [M,K] row-major (lda = row pitch);  a_mn = 1: A is stored transposed as [K,M] (lda = its pitch).
  *   b_mn = 0: B is [N,K] row-major (a torch Linear weight);  b_mn = 1: B is stored as [K,N].
  *   act: 0 none, 1 GELU(erf), 2 ReLU on (acc+bias).  round_before_res: round (acc+bias) to bf16 before adding the residual
- *   (bit-matches an unfused bf16 linear followed by a bf16 add).  force_bn: 0 auto, else 64/128/256.
+ *   (bit-matches an unfused bf16 linear followed by a bf16 add).  force_bn: 0 auto, else 64/128/192/224/256.
  * Replaces every torch.nn.Linear / F.linear on both hot paths (HF:models/qwen2/modeling_qwen2.py:35-48,187-246;
  * HF:models/hubert/modeling_hubert.py:216-231,262-405) and their autograd dgrad/wgrad GEMMs. */
 int sk_gemm_bf16(int M, int N, int K, const void* A, int lda, int a_mn, const void* B, int ldb, int b_mn, void* C,
@@ -59,13 +59,13 @@ int64_t sk_gemm_ws_bytes(void);
  * after the same argument checks.  Nothing is launched and no pointer is dereferenced: only the shapes, the flags,
  * ws_bytes, which of bias / residual / ws are NULL and whether residual == C matter. */
 typedef struct SkGemmPlan {
-  int32_t bn;                /* tile width: 64, 128 or 256 (tiles are 128 rows) */
+  int32_t bn;                /* tile width: 64, 128, 192, 224 or 256 (tiles are 128 rows) */
   int32_t epi_warps;         /* 4, or 8 (two per 32-row quadrant) */
   int32_t splits;            /* > 1: split-K into this many K ranges, fp32 slabs summed by a second kernel */
   int32_t sk_units;          /* > 0: stream-K over the last sk_units units (rows of tiles, or columns: sk_colunits) */
   int32_t sk_groups;         /* CTA groups that share the stream-K iteration space (cut into equal K ranges) */
   int32_t sk_G;              /* tiles per unit = CTAs per group */
-  int32_t sk_colunits;       /* 1: a stream-K unit is a column of tiles (selected by SK_STREAMK=2) */
+  int32_t sk_colunits;       /* 1: a stream-K unit is a column of tiles (<= 8 tile rows, > 8 tile columns) */
   int32_t tma_store;         /* 1: bf16 output through TMA stores; 0: direct stores (fp32 output, split-K slabs) */
   int32_t grid;              /* CTAs of the GEMM kernel */
 } SkGemmPlan;

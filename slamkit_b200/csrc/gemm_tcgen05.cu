@@ -21,6 +21,7 @@
 #include <cudaTypedefs.h>
 #include <stdio.h>
 #include <mutex>
+#include <type_traits>
 #include <string.h>
 #include <stdlib.h>
 #include "kernels.h"
@@ -60,6 +61,7 @@ struct GemmParams {
   int sk_groups;        // CTA groups that share the stream-K iteration space (each unit is cut into <= ~4 ranges)
   int sk_G;             // tiles per unit = CTAs per group (they run the same k-blocks in lockstep)
   int sk_colunits;      // 0: a unit is one row of tiles (same A rows);  1: one column of tiles (same B rows)
+  int sk_carry;         // 1: carry-in stream-K (see WorkIter): a split tile's second range starts from the first's accumulator
   int units, n_groups;  // total units, CTA groups in the grid
   float* sk_ws;         // stream-K partial tiles, one 128 x 256 fp32 slot per CTA
   uint32_t* sk_flags;   // [grid][4] publish flags (per epilogue warp), zero between launches
@@ -87,6 +89,7 @@ struct GemmCfg {
   static constexpr int STAGING_BYTES = 4 * 2 * 4096;  // (32 rows x 128 B) TMA-store buffers: 2 per warp (EW = 4) or 1 (EW = 8)
   static constexpr int BAR_BYTES = 256;
   static constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + STAGING_BYTES + BAR_BYTES + 1024;  // +1024: manual alignment
+  static_assert(BN % 64 == 0 || (BN == 224 && EW == 4), "a 32-column tail chunk only on the 224-wide tile");
   static_assert(STAGES * STAGE_BYTES >= BM * BN * 4, "the parked fp32 accumulator must fit in the stage ring");
   static_assert(SMEM_BYTES <= 227 * 1024, "sm_90 allows 227 KB of shared memory per block");
 };
@@ -123,6 +126,14 @@ SK_DEVINL void acc_ld_32x32(uint32_t base, uint32_t ta, uint32_t (&r)[32]) {
                  : "r"(acc_chunk_addr<BN>(base, row, c0 + i)) : "memory");
 }
 
+// TMA-store staging address of 16-byte piece j of this lane's row.  A 64-column chunk has 128-byte rows in the 128B
+// swizzle (map tmC); the 32-column tail chunk of a 224-wide tile has 64-byte rows in the 64B swizzle and leaves through
+// a 32-column box (map tmAux), so a tile never writes its neighbour's columns.
+SK_DEVINL uint32_t staging_addr(uint32_t sbuf, int lane, int j, bool tail) {
+  return tail ? sbuf + (uint32_t)lane * 64u + (uint32_t)((j ^ ((lane >> 1) & 3)) << 4)
+              : sbuf + (uint32_t)lane * 128u + (uint32_t)((j ^ (lane & 7)) << 4);
+}
+
 // GELU(erf) for the fused epilogue (HuBERT conv layers and FFN): branch-free Abramowitz-Stegun 7.1.26 erf, folded as
 //   gelu(y) = relu(y) - |y| * (P(t)/2) * exp(-y^2/2),  t = 1/(1 + p|y|/sqrt2)
 // |error| <= 1.5e-7 * |y|/2 absolute -- below the 2^-17 relative grid of the hi/lo bf16 outputs it feeds -- at a third of
@@ -152,11 +163,17 @@ SK_DEVINL float gelu_erf(float y) {
 // role 2 = the range holds the unit's first k-block but not its last: this CTA finishes the tile and adds the partials
 // of the same member of the following groups in a fixed order (deterministic); role 0 = whole tile.  The remaining
 // units are processed whole, after the stream-K ranges, so the fix-up of a tile overlaps the next tile's MMAs.
+//
+// Carry-in mode (p.sk_carry, every range at least one unit long): a unit is cut into at most two ranges, and each group
+// runs its range's pieces last unit first.  role 1 = the unit's first k-blocks: the fp32 accumulator goes to the CTA's
+// scratch slot (published before this CTA's later pieces start); role 3 = the unit's remaining k-blocks: this CTA loads
+// that accumulator from the same member of the previous group into its registers and continues the K loop, so every
+// element sees the same MMAs in the same order as a whole tile (results bit-identical to whole-tile scheduling).
 template <bool SK>
 struct WorkIter {
   int num_kb, splits, kb_per_split, total_items, tiles_n;
   // stream-K
-  int G, colunits, units, n_groups, sk_groups, grp, mem;
+  int G, colunits, carry, units, n_groups, sk_groups, grp, mem;
   long sk_total, sk_cur, sk_end;
   int next_unit, next_item;
   // current item
@@ -170,6 +187,7 @@ struct WorkIter {
     tiles_n = p.tiles_n;
     G = p.sk_G;
     colunits = p.sk_colunits;
+    carry = p.sk_carry;
     units = p.units;
     n_groups = p.n_groups;
     sk_groups = p.sk_groups;
@@ -193,6 +211,19 @@ struct WorkIter {
   }
   SK_DEVINL int tile_of(int unit) const { return colunits ? mem * tiles_n + unit : unit * G + mem; }
   SK_DEVINL bool next() {
+    if (SK && sk_cur < sk_end && carry) {   // last piece of the range first
+      const int unit = (int)((sk_end - 1) / num_kb);
+      const long ustart = (long)unit * num_kb;
+      const long b = sk_cur > ustart ? sk_cur : ustart;
+      kb_begin = (int)(b - ustart);
+      kb_end = (int)(sk_end - ustart);
+      unit_end_it = ustart + num_kb;
+      tile = tile_of(unit);
+      split = 0;
+      role = kb_begin != 0 ? 3 : (kb_end < num_kb ? 1 : 0);
+      sk_end = b;
+      return true;
+    }
     if (SK && sk_cur < sk_end) {
       const int unit = (int)(sk_cur / num_kb);
       kb_begin = (int)(sk_cur - (long)unit * num_kb);
@@ -331,6 +362,8 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
   using Cfg = GemmCfg<BN, EW>;
   static_assert(EW == 4 || (EW == 8 && BN == 256 && !SK), "8 epilogue warps: plain 256-wide tiles only");
   constexpr int CS = EW / 4;          // column split: epilogue warps per 32-row quadrant
+  constexpr int NC64 = BN / 64;       // whole 64-column chunks of a tile
+  constexpr bool TAIL = BN % 64 != 0; // BN = 224: a last 32-column chunk, stored through tmAux
   griddep_launch();                 // the next kernel on the stream may start its own prologue now
   extern __shared__ uint8_t smem_raw[];
   const uint32_t smem_base = (smem_u32(smem_raw) + 1023u) & ~1023u;
@@ -444,6 +477,35 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
         float acc[BN / 2];
 #pragma unroll
         for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
+        if (SK && w.role == 3) {
+          // carry-in: continue from the fp32 accumulator of the tile's first k-blocks (same member, previous group)
+          const int src = (int)blockIdx.x - w.G;
+          if (threadIdx.x == 0) {
+            for (int qq = 0; qq < 4; ++qq) {
+              const uint32_t* f = p.sk_flags + src * 4 + qq;
+              const uint64_t t0 = globaltimer_ns();
+              while (ld_acquire_u32(f) == 0u) {
+                __nanosleep(64);
+                if (globaltimer_ns() - t0 > 8000000000ull) __trap();
+              }
+            }
+            for (int qq = 0; qq < 4; ++qq) p.sk_flags[src * 4 + qq] = 0u;   // re-armed for the next launch
+          }
+          named_bar_sync(1, 256);
+          const float* slot = p.sk_ws + (size_t)src * SK_SLOT_FLOATS;
+          const int r0 = 64 * wg + 16 * (warp & 3) + (lane >> 2);
+#pragma unroll
+          for (int j = 0; j < BN / 8; ++j) {
+            const int col = 8 * j + 2 * (lane & 3);
+#pragma unroll
+            for (int h = 0; h < 2; ++h) {
+              const float2 v = __ldcg(reinterpret_cast<const float2*>(slot + sk_slot_off(col >> 5, (col & 31) >> 2, r0 + 8 * h) +
+                                                                      (col & 3)));
+              acc[4 * j + 2 * h] = v.x;
+              acc[4 * j + 2 * h + 1] = v.y;
+            }
+          }
+        }
         const int k_iters = max(0, w.kb_end - w.kb_begin);
         int prev = -1;
         for (int kb = 0; kb < k_iters; ++kb) {
@@ -619,27 +681,35 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
           }
           __syncwarp();
         }
-        // one 64-column x 32-row bf16 chunk: registers -> this warp's swizzled staging buffer -> TMA store at (col, rows)
-        auto stage_store = [&](const CUtensorMap* map, const uint32_t (&pk)[32], int col) {
+        // one 64-column x 32-row bf16 chunk (tail: 32 columns, pk[0..15]): registers -> this warp's swizzled staging
+        // buffer -> TMA store at (col, rows)
+        auto stage_store = [&](const CUtensorMap* map, const uint32_t (&pk)[32], int col, auto tail_c) {
+          constexpr bool tail = decltype(tail_c)::value;
           const uint32_t sbuf = staging_base + (EW == 4 ? (uint32_t)warp * 8192u + (store_cnt & 1u) * 4096u : (uint32_t)warp * 4096u);
           if (lane == 0) {
             if constexpr (EW == 4) tma_store_wait_read<1>(); else tma_store_wait_read<0>();
           }
           __syncwarp();
 #pragma unroll
-          for (int j = 0; j < 8; ++j) {
-            const uint32_t dst = sbuf + (uint32_t)lane * 128u + (uint32_t)((j ^ (lane & 7)) << 4);
-            asm volatile("st.shared.v4.b32 [%0], {%1, %2, %3, %4};" ::"r"(dst), "r"(pk[4 * j]), "r"(pk[4 * j + 1]),
-                         "r"(pk[4 * j + 2]), "r"(pk[4 * j + 3])
+          for (int j = 0; j < (tail ? 4 : 8); ++j) {
+            asm volatile("st.shared.v4.b32 [%0], {%1, %2, %3, %4};" ::"r"(staging_addr(sbuf, lane, j, tail)), "r"(pk[4 * j]),
+                         "r"(pk[4 * j + 1]), "r"(pk[4 * j + 2]), "r"(pk[4 * j + 3])
                          : "memory");
           }
           fence_proxy_async();
           __syncwarp();
           if (lane == 0) {
-            tma_store_2d(map, sbuf, col, m0 + q * 32);
+            tma_store_2d(tail ? &tmAux : map, sbuf, col, m0 + q * 32);
             tma_store_commit();
           }
           ++store_cnt;
+        };
+        // the epilogues below run the whole 64-column chunks of this warp with tail = false and, for BN = 224, the
+        // 32-column tail chunk with tail = true (compile-time constants: one body, no run-time branches in it)
+        auto for_chunks = [&](auto&& body) {
+#pragma unroll 1
+          for (int c2 = chalf * (NC64 / CS); c2 < (chalf + 1) * (NC64 / CS); ++c2) body(std::false_type{}, c2);
+          if constexpr (TAIL) body(std::true_type{}, NC64);
         };
         if (!SK && p.tma_store && p.epi == 1) {
           // ---- SwiGLU forward: tile columns [0,128) = gate, [128,256) = up of the same 128 hidden units ----
@@ -658,7 +728,7 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
                   gpk[16 + t] = pack_bf16(__uint_as_float(r1[2 * t]), __uint_as_float(r1[2 * t + 1]));
                 }
               }
-              stage_store(&tmC, gpk, n0 + i * 64);
+              stage_store(&tmC, gpk, n0 + i * 64, std::false_type{});
               {
                 uint32_t r0[32], r1[32];
                 acc_ld(taddr + 128 + i * 64, r0);
@@ -669,14 +739,14 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
                   upk[16 + t] = pack_bf16(__uint_as_float(r1[2 * t]), __uint_as_float(r1[2 * t + 1]));
                 }
               }
-              stage_store(&tmC, upk, n0 + 128 + i * 64);
+              stage_store(&tmC, upk, n0 + 128 + i * 64, std::false_type{});
 #pragma unroll
               for (int t = 0; t < 32; ++t) {
                 const float2 gf = unpack_bf16(gpk[t]), uf = unpack_bf16(upk[t]);
                 const float2 sb = unpack_bf16(pack_bf16(silu_f(gf.x), silu_f(gf.y)));   // bf16(silu(g))
                 gpk[t] = pack_bf16(sb.x * uf.x, sb.y * uf.y);
               }
-              stage_store(&tmAux, gpk, (n0 >> 1) + i * 64);
+              stage_store(&tmAux, gpk, (n0 >> 1) + i * 64, std::false_type{});
             }
           }
         } else if (!SK && p.tma_store && p.epi == 3) {
@@ -737,52 +807,52 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
                 pk[16 + g * 4 + e] = pack_bf16(v1[2 * e], v1[2 * e + 1]);
               }
             }
-            stage_store(&tmC, pk, col64);
+            stage_store(&tmC, pk, col64, std::false_type{});
           }
         } else if (p.tma_store && !p.bias && !p.residual && !p.act) {
           // plain convert-and-store (dgrads, wgrads, gate/up ...): a straight-line instance without the per-column-group
           // bias / activation / residual tests of the general path below
-#pragma unroll 1
-          for (int c2 = chalf * (BN / 64 / CS); c2 < (chalf + 1) * (BN / 64 / CS); ++c2) {
+          for_chunks([&](auto tail_c, int c2) {
+            constexpr bool tail = decltype(tail_c)::value;
             uint32_t r0[32], r1[32], pk[32];
             acc_ld(taddr + c2 * 64, r0);
-            acc_ld(taddr + c2 * 64 + 32, r1);
-            if (SK && n_contrib > 0) {
-              sk_fixup_add(r0, p.sk_ws, c2 * 2, row_in_tile, first_contrib, w.G, n_contrib);
-              sk_fixup_add(r1, p.sk_ws, c2 * 2 + 1, row_in_tile, first_contrib, w.G, n_contrib);
-            }
+            if (SK && n_contrib > 0) sk_fixup_add(r0, p.sk_ws, c2 * 2, row_in_tile, first_contrib, w.G, n_contrib);
 #pragma unroll
-            for (int t = 0; t < 16; ++t) {
-              pk[t] = pack_bf16(__uint_as_float(r0[2 * t]), __uint_as_float(r0[2 * t + 1]));
-              pk[16 + t] = pack_bf16(__uint_as_float(r1[2 * t]), __uint_as_float(r1[2 * t + 1]));
+            for (int t = 0; t < 16; ++t) pk[t] = pack_bf16(__uint_as_float(r0[2 * t]), __uint_as_float(r0[2 * t + 1]));
+            if constexpr (!tail) {
+              acc_ld(taddr + c2 * 64 + 32, r1);
+              if (SK && n_contrib > 0) sk_fixup_add(r1, p.sk_ws, c2 * 2 + 1, row_in_tile, first_contrib, w.G, n_contrib);
+#pragma unroll
+              for (int t = 0; t < 16; ++t) pk[16 + t] = pack_bf16(__uint_as_float(r1[2 * t]), __uint_as_float(r1[2 * t + 1]));
             }
-            stage_store(&tmC, pk, n0 + c2 * 64);
-          }
+            stage_store(&tmC, pk, n0 + c2 * 64, tail_c);
+          });
         } else if (p.tma_store && !p.bias && !p.act && p.residual && !p.residual_lo) {
           // residual add only (o-proj and down-proj forward: x + linear(..), rounded like the unfused bf16 graph): the
           // row's 128 residual bytes are requested before the accumulator is read; straight-line
-#pragma unroll 1
-          for (int c2 = chalf * (BN / 64 / CS); c2 < (chalf + 1) * (BN / 64 / CS); ++c2) {
+          for_chunks([&](auto tail_c, int c2) {
+            constexpr bool tail = decltype(tail_c)::value;
+            constexpr int nj = tail ? 4 : 8;     // 16-byte pieces of the chunk
             const int col64 = n0 + c2 * 64;
-            if (col64 >= p.N) break;
+            if (col64 >= p.N) return;
             uint4 rv[8];
             if (row_ok) {
               const bf16* rp = p.residual + row * p.ldr + col64;
 #pragma unroll
-              for (int j = 0; j < 8; ++j) rv[j] = (col64 + 8 * j < p.N) ? ldg128(rp + 8 * j) : make_uint4(0u, 0u, 0u, 0u);
+              for (int j = 0; j < 8; ++j) rv[j] = (j < nj && col64 + 8 * j < p.N) ? ldg128(rp + 8 * j) : make_uint4(0u, 0u, 0u, 0u);
             } else {
 #pragma unroll
               for (int j = 0; j < 8; ++j) rv[j] = make_uint4(0u, 0u, 0u, 0u);
             }
             uint32_t r0[32], r1[32], pk[32];
             acc_ld(taddr + c2 * 64, r0);
-            acc_ld(taddr + c2 * 64 + 32, r1);
-            if (SK && n_contrib > 0) {
-              sk_fixup_add(r0, p.sk_ws, c2 * 2, row_in_tile, first_contrib, w.G, n_contrib);
-              sk_fixup_add(r1, p.sk_ws, c2 * 2 + 1, row_in_tile, first_contrib, w.G, n_contrib);
+            if (SK && n_contrib > 0) sk_fixup_add(r0, p.sk_ws, c2 * 2, row_in_tile, first_contrib, w.G, n_contrib);
+            if constexpr (!tail) {
+              acc_ld(taddr + c2 * 64 + 32, r1);
+              if (SK && n_contrib > 0) sk_fixup_add(r1, p.sk_ws, c2 * 2 + 1, row_in_tile, first_contrib, w.G, n_contrib);
             }
 #pragma unroll
-            for (int j = 0; j < 8; ++j) {
+            for (int j = 0; j < nj; ++j) {
               const uint32_t* r = j < 4 ? r0 + 8 * j : r1 + 8 * (j - 4);
               const uint32_t rw[4] = {rv[j].x, rv[j].y, rv[j].z, rv[j].w};
 #pragma unroll
@@ -796,19 +866,19 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
                 pk[4 * j + e] = pack_bf16(a0 + f.x, a1 + f.y);
               }
             }
-            stage_store(&tmC, pk, col64);
-          }
+            stage_store(&tmC, pk, col64, tail_c);
+          });
         } else if (p.tma_store) {
           // coalesced path: parked accumulator -> registers -> 128B-swizzled smem (this warp's private 32-row buffer) -> TMA store
-#pragma unroll 1
-          for (int c2 = chalf * (BN / 64 / CS); c2 < (chalf + 1) * (BN / 64 / CS); ++c2) {
+          for_chunks([&](auto tail_c, int c2) {
+            constexpr bool tail = decltype(tail_c)::value;
             const uint32_t sbuf = staging_base + (EW == 4 ? (uint32_t)warp * 8192u + (store_cnt & 1u) * 4096u : (uint32_t)warp * 4096u);
             if (lane == 0) {
               if constexpr (EW == 4) tma_store_wait_read<1>(); else tma_store_wait_read<0>();
             }
             __syncwarp();
 #pragma unroll
-            for (int half = 0; half < 2; ++half) {
+            for (int half = 0; half < (tail ? 1 : 2); ++half) {
               uint32_t r[32];
               acc_ld(taddr + c2 * 64 + half * 32, r);
               if (SK && n_contrib > 0) sk_fixup_add(r, p.sk_ws, c2 * 2 + half, row_in_tile, first_contrib, w.G, n_contrib);
@@ -822,21 +892,20 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
                   epi_bias_act(v, p, col);
                   if (row_ok) epi_residual(v, p, row, col);
                 }
-                const int j = half * 4 + g;
-                const uint32_t dst = sbuf + (uint32_t)lane * 128u + (uint32_t)((j ^ (lane & 7)) << 4);
-                asm volatile("st.shared.v4.b32 [%0], {%1, %2, %3, %4};" ::"r"(dst), "r"(pack_bf16(v[0], v[1])),
-                             "r"(pack_bf16(v[2], v[3])), "r"(pack_bf16(v[4], v[5])), "r"(pack_bf16(v[6], v[7]))
+                asm volatile("st.shared.v4.b32 [%0], {%1, %2, %3, %4};" ::"r"(staging_addr(sbuf, lane, half * 4 + g, tail)),
+                             "r"(pack_bf16(v[0], v[1])), "r"(pack_bf16(v[2], v[3])), "r"(pack_bf16(v[4], v[5])),
+                             "r"(pack_bf16(v[6], v[7]))
                              : "memory");
               }
             }
             fence_proxy_async();
             __syncwarp();
             if (lane == 0) {
-              tma_store_2d(&tmC, sbuf, n0 + c2 * 64, m0 + q * 32);
+              tma_store_2d(tail ? &tmAux : &tmC, sbuf, n0 + c2 * 64, m0 + q * 32);
               tma_store_commit();
             }
             ++store_cnt;
-          }
+          });
         }
         else
 #pragma unroll 1
@@ -954,7 +1023,7 @@ void load_encode() {
 }  // namespace
 
 // Build a 2-D bf16 (elem_bytes=2) / fp32 (elem_bytes=4) tensor map: `inner` contiguous elements, `outer` rows of pitch
-// ld elements, box (box_inner x box_outer), 128B swizzle.
+// ld elements, box (box_inner x box_outer), 128B swizzle (64B swizzle for a 64-byte box row).
 int sk_make_tmap_2d(CUtensorMap* out, const void* ptr, int elem_bytes, uint64_t inner, uint64_t outer, uint64_t ld,
                     uint32_t box_inner, uint32_t box_outer) {
   std::call_once(g_encode_once, load_encode);
@@ -962,14 +1031,15 @@ int sk_make_tmap_2d(CUtensorMap* out, const void* ptr, int elem_bytes, uint64_t 
   SK_REQUIRE((reinterpret_cast<uintptr_t>(ptr) & 15) == 0, "TMA base pointer must be 16-byte aligned");
   SK_REQUIRE((ld * elem_bytes) % 16 == 0, "TMA row pitch must be a multiple of 16 bytes (ld=%llu)",
              (unsigned long long)ld);
-  SK_REQUIRE(box_inner * elem_bytes == 128, "SW128 box inner extent must be 128 bytes");
+  SK_REQUIRE(box_inner * elem_bytes == 128 || box_inner * elem_bytes == 64, "box inner extent must be 128 (or 64) bytes");
   cuuint64_t dims[2] = {inner, outer};
   cuuint64_t strides[1] = {ld * (uint64_t)elem_bytes};
   cuuint32_t box[2] = {box_inner, box_outer};
   cuuint32_t estr[2] = {1, 1};
   CUtensorMapDataType dt = elem_bytes == 2 ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16 : CU_TENSOR_MAP_DATA_TYPE_FLOAT32;
   CUresult r = g_encode(out, dt, 2, const_cast<void*>(ptr), dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
-                        CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
+                        box_inner * elem_bytes == 64 ? CU_TENSOR_MAP_SWIZZLE_64B : CU_TENSOR_MAP_SWIZZLE_128B,
+                        CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
                         CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
   SK_REQUIRE(r == CUDA_SUCCESS, "cuTensorMapEncodeTiled failed with CUresult %d (inner=%llu outer=%llu ld=%llu)", (int)r,
              (unsigned long long)inner, (unsigned long long)outer, (unsigned long long)ld);
@@ -1023,8 +1093,9 @@ int dispatch_major(bool a_mn, bool b_mn, const CUtensorMap* tm, const GemmParams
 }
 
 // Relative cost of one 128 x BN tile (BN=256 == 100), a heuristic: narrow tiles pay the per-tile pipeline fill /
-// epilogue overhead and re-read the A tile from shared memory more often per FLOP.
-inline int tile_cost(int bn) { return bn >= 256 ? 100 : (bn >= 128 ? 61 : 54); }
+// epilogue overhead and re-read the A tile from shared memory more often per FLOP.  192 and 224 are put on the line
+// through 128 and 256 (80 and 90).
+inline int tile_cost(int bn) { return bn >= 256 ? 100 : (bn > 128 ? 61 + (bn - 128) * 39 / 128 : (bn == 128 ? 61 : 54)); }
 
 constexpr size_t SK_FLAG_BYTES = 4096;   // tail of the scratch buffer: stream-K publish flags ([CTA][32-row quadrant])
 
@@ -1032,21 +1103,36 @@ constexpr size_t SK_FLAG_BYTES = 4096;   // tail of the scratch buffer: stream-K
 
 size_t sk_gemm_ws_min_bytes(void) { return (size_t)sk_num_sms() * SK_SLOT_FLOATS * sizeof(float) + SK_FLAG_BYTES; }
 
-int sk_pick_bn(int M, int N, int force_bn) {
+// Tile width.  The persistent kernel runs a GEMM in about ceil(tiles / SMs) tile times, and every tile pays for its
+// whole BN columns (a half-empty last tile column costs a full one), so a width costs
+// waves(tiles, sk_num_sms()) x tile_cost(bn).  256 is the default; 128 or 64 displaces it only when clearly cheaper
+// (>= 25 %: near-ties favour the wide tile).  With `fit`, a 256 pick whose last tile column would be partly empty is
+// then replaced by 224 or 192 when that costs >= 5 % less: the empty columns of 256 are often what pushes the GEMM into
+// another wave (the LM's d = 896 = 4 x 224 and QKV = 1152 = 6 x 192).  Sizes that 256 divides keep it.  whole_heads
+// keeps the widths to whole 64-column heads (the RoPE epilogue).  A forced width is taken as it is (192 / 224 when
+// fit_forced).
+int sk_pick_bn(int M, int N, int force_bn, bool fit_forced, bool fit, bool whole_heads) {
   if (force_bn == 64 || force_bn == 128 || force_bn == 256) return force_bn;
+  if (fit_forced && (force_bn == 192 || (force_bn == 224 && !whole_heads))) return force_bn;
   const int nsm = sk_num_sms();
-  const int cands[3] = {256, 128, 64};
-  int best = 256;
-  long best_cost = -1;
-  for (int i = 0; i < 3; ++i) {
-    const int bn = cands[i];
+  auto cost = [&](int bn) {
     const long tiles = (long)((M + BM - 1) / BM) * ((N + bn - 1) / bn);
-    const long waves = (tiles + nsm - 1) / nsm;
-    const long cost = waves * tile_cost(bn);
-    // a narrower tile has to be clearly better (>= 25 %) to displace a wider one (near-ties favour BN = 256)
-    if (best_cost < 0 || cost * 100 < best_cost * 75) {
-      best_cost = cost;
+    return ((tiles + nsm - 1) / nsm) * tile_cost(bn);
+  };
+  int best = 256;
+  long best_cost = cost(256);
+  for (const int bn : {128, 64}) {
+    if (cost(bn) * 100 < best_cost * 75) {
+      best_cost = cost(bn);
       best = bn;
+    }
+  }
+  if (best == 256 && fit && N % 256 != 0) {
+    for (const int bn : {224, 192}) {
+      if (!(whole_heads && bn % 64 != 0) && cost(bn) * 100 < best_cost * 95) {
+        best_cost = cost(bn);
+        best = bn;
+      }
     }
   }
   return best;
@@ -1091,8 +1177,15 @@ int plan_gemm(const SkGemmEx& g, GemmParams& p, int& BN, int& ew, int& grid) {
   const bool sk_ok = sk_env != 0 && g.batch == 1 && !use3d && g.passes == 1 && g.a_mode == 0 && g.splitk_ws != nullptr &&
                      g.splitk_ws_bytes >= sk_gemm_ws_min_bytes();
   const size_t ws_data_bytes = g.splitk_ws_bytes > SK_FLAG_BYTES ? g.splitk_ws_bytes - SK_FLAG_BYTES : 0;
-  // the SwiGLU epilogues need both halves of a [128 gate | 128 up] block in one tile
-  BN = (g.a_mode == 1) ? 64 : sk_pick_bn(g.M * g.batch, g.N, (g.epi == 1 || g.epi == 2) ? 256 : g.force_bn);
+  // the SwiGLU epilogues need both halves of a [128 gate | 128 up] block in one tile.  The 192 / 224 widths are for
+  // plain one-pass 2-D problems; the auto planner leaves them to GEMMs without stream-K scratch (forward and dgrad):
+  // with scratch, split-K / stream-K balance the last wave at the widths they were tuned for
+  const bool fit = g.passes == 1 && g.batch == 1 && !use3d && g.a_mode == 0 && g.epi != 1 && g.epi != 2;
+  SK_REQUIRE((g.force_bn != 192 && g.force_bn != 224) || (fit && !(g.force_bn == 224 && g.epi == 3)),
+             "gemm: force_bn=%d needs a one-pass 2-D problem (and whole 64-column heads for RoPE)", g.force_bn);
+  BN = (g.a_mode == 1) ? 64
+                       : sk_pick_bn(g.M * g.batch, g.N, (g.epi == 1 || g.epi == 2) ? 256 : g.force_bn, fit,
+                                    fit && !sk_ok, g.epi == 3);
   memset(&p, 0, sizeof(p));
   p.M = g.M; p.N = g.N; p.K = g.K;
   p.batch = g.batch;
@@ -1159,18 +1252,31 @@ int plan_gemm(const SkGemmEx& g, GemmParams& p, int& BN, int& ew, int& grid) {
       SK_REQUIRE(false, "gemm: unknown fused epilogue %d", g.epi);
     }
   }
-  // stream-K over the units (rows or columns of tiles) of the last, partial wave -- see WorkIter
+  // stream-K over the units (rows or columns of tiles) of the last, partial wave -- see WorkIter.  Row units (a tile
+  // row of <= 8 tiles) cut the leftover units into at most ~4 ranges each.  Column units (<= 8 tile rows, more than 8
+  // tile columns: the down-projection weight gradient, 7 x 19 tiles) balance the last of several waves by default: the
+  // leftover units and the last full wave are laid end to end over every group, so each group runs 1 + rem / n_groups
+  // units and a unit is cut into at most two ranges, the second continuing from the first's accumulator (carry-in: the
+  // weight gradient comes out bit-identical to whole tiles).  SK_STREAMK=2 also takes single-wave shapes.
   p.sk_G = 1;
-  if (sk_ok && BN == 256 && p.splits == 1 && num_kb >= sk_min_kb && (p.tiles_n <= 8 || (sk_env >= 2 && p.tiles_m <= 8))) {
+  if (sk_ok && BN == 256 && p.splits == 1 && num_kb >= sk_min_kb && (p.tiles_n <= 8 || p.tiles_m <= 8)) {
     const int colunits = p.tiles_n <= 8 ? 0 : 1;
     const int G = colunits ? p.tiles_m : p.tiles_n;
     const int units = colunits ? p.tiles_n : p.tiles_m;
     const int n_groups = nsm / G;
     const int rem = units % n_groups;
     const long slots = ((long)(units + n_groups - 1) / n_groups) * n_groups;
-    if (n_groups >= 1 && rem != 0 && (slots - units) * 100 >= slots * sk_min_idle) {   // enough SM-time would idle
-      p.sk_units = rem;
-      p.sk_groups = n_groups < rem * sk_ranges ? n_groups : rem * sk_ranges;            // a unit is cut into at most ~4 ranges
+    const bool multiwave = units > n_groups;
+    if (n_groups >= 1 && rem != 0 && (slots - units) * 100 >= slots * sk_min_idle &&   // enough SM-time would idle
+        (!colunits || multiwave || sk_env >= 2)) {
+      if (colunits && multiwave) {
+        p.sk_units = rem + n_groups;
+        p.sk_groups = n_groups;
+        p.sk_carry = 1;
+      } else {
+        p.sk_units = rem;
+        p.sk_groups = n_groups < rem * sk_ranges ? n_groups : rem * sk_ranges;          // a unit is cut into at most ~4 ranges
+      }
       p.sk_G = G;
       p.sk_colunits = colunits;
       p.units = units;
@@ -1244,6 +1350,9 @@ int sk_gemm_ex_launch(const SkGemmEx& g, cudaStream_t stream) {
   if (g.epi == 1) {
     const int rc3 = sk_make_tmap_2d(&tm[5], g.aux_out, 2, (uint64_t)g.N / 2, (uint64_t)g.M, (uint64_t)g.ld_aux_out, 64, 32);
     if (rc3) return rc3;
+  } else if (p.tma_store && BN % 64 != 0) {   // the 32-column tail chunk of a 224-wide tile
+    const int rc3 = sk_make_tmap_2d(&tm[5], g.C, 2, (uint64_t)g.N, (uint64_t)g.M, (uint64_t)g.ldc, 32, 32);
+    if (rc3) return rc3;
   }
   int rc;
   if (p.sk_units > 0) {
@@ -1253,6 +1362,8 @@ int sk_gemm_ex_launch(const SkGemmEx& g, cudaStream_t stream) {
   } else {
     switch (BN) {
       case 256: rc = dispatch_major<256, false>(g.a_mn, g.b_mn, tm, p, grid, stream); break;
+      case 224: rc = dispatch_major<224, false>(g.a_mn, g.b_mn, tm, p, grid, stream); break;
+      case 192: rc = dispatch_major<192, false>(g.a_mn, g.b_mn, tm, p, grid, stream); break;
       case 128: rc = dispatch_major<128, false>(g.a_mn, g.b_mn, tm, p, grid, stream); break;
       default:  rc = dispatch_major<64, false>(g.a_mn, g.b_mn, tm, p, grid, stream); break;
     }

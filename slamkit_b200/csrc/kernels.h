@@ -8,7 +8,7 @@ int sk_make_tmap_2d(CUtensorMap* out, const void* ptr, int elem_bytes, uint64_t 
                     uint32_t box_inner, uint32_t box_outer);
 int sk_make_tmap_3d(CUtensorMap* out, const void* ptr, uint64_t inner, uint64_t rows, uint64_t batch, uint64_t row_stride,
                     uint64_t batch_stride, uint32_t box_rows);
-int sk_pick_bn(int M, int N, int force_bn);
+int sk_pick_bn(int M, int N, int force_bn, bool fit_forced, bool fit, bool whole_heads);
 size_t sk_gemm_ws_min_bytes(void);   // scratch size that enables stream-K (last 4 KB = flag words, zero on first use)
 // Extended GEMM description (HuBERT path): batched / strided-window A operands (convolutions as GEMMs without an
 // im2col copy), split-bf16 3-pass accumulation, fp32 bias, hi/lo residual and outputs, grouped column compaction.

@@ -1,5 +1,6 @@
 """Micro-benchmark of the wgmma GEMM on the LM shapes (CUDA events, L2 flushed between iterations).
-Prints one line per shape: our TFLOP/s per tile width, and torch.matmul (cuBLAS) for context."""
+Prints one line per shape: our TFLOP/s per tile width (bn0 = the planner's choice), with the scratch buffer (sk: split-K /
+stream-K where the planner takes them), torch.matmul (cuBLAS) for context, and the schedule the planner picks with scratch."""
 import sys, os
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import torch
@@ -41,13 +42,17 @@ for name, m, n, k, a_mn, b_mn in shapes:
     out = torch.empty((m, n), device=dev, dtype=torch.bfloat16)
     flops = 2.0 * m * n * k
     res = []
-    for bn in (0, 128, 256):
+    for bn in (0, 128, 192, 224, 256):
         t = timeit(lambda: ops.gemm(a, b, a_mn=bool(a_mn), b_mn=bool(b_mn), out=out, force_bn=bn))
         res.append(f"bn{bn}: {flops / t / 1e9:7.1f} TF/s ({t * 1e3:7.1f} us)")
-    for bn in (0, 256):   # with the scratch buffer: stream-K balancing
+    for bn in (0, 224, 256):   # with the scratch buffer: split-K / stream-K balancing
         t = timeit(lambda: ops.gemm(a, b, a_mn=bool(a_mn), b_mn=bool(b_mn), out=out, force_bn=bn, streamk=True))
         res.append(f"sk{bn}: {flops / t / 1e9:7.1f} TF/s ({t * 1e3:7.1f} us)")
     A = a.t() if a_mn else a
     Bt = b if b_mn else b.t()
     t = timeit(lambda: torch.matmul(A, Bt, out=out))
-    print(f"{name:11s} M{m} N{n} K{k} | " + " | ".join(res) + f" | cublas {flops / t / 1e9:7.1f} TF/s ({t*1e3:7.1f} us)", flush=True)
+    pl = ops.gemm_plan(a, b, a_mn=bool(a_mn), b_mn=bool(b_mn), out=out, streamk=True)
+    sched = (f"splitk{pl['splits']}" if pl["splits"] > 1 else
+             (f"streamk-{'cols' if pl['sk_colunits'] else 'rows'} {pl['sk_units']}u/{pl['sk_groups']}g" if pl["sk_units"] else "tiles"))
+    print(f"{name:11s} M{m} N{n} K{k} | " + " | ".join(res) + f" | cublas {flops / t / 1e9:7.1f} TF/s ({t*1e3:7.1f} us)"
+          f" | plan bn{pl['bn']} {sched}", flush=True)
