@@ -154,6 +154,12 @@ int sk_attn_tc_bwd(const void* qkv, const void* o, const void* d_o, const float*
 int sk_attn_bwd(const void* q, const void* k, const void* v, const void* o, const void* d_o, const float* lse,
                 float* delta, void* dq, void* dk, void* dv, int B, int T, int H, int KVH, int ld, int ldo, int ldg,
                 int causal, float scale, void* stream);
+/* Split-bf16 bidirectional forward of the HuBERT encoder: each value is an fp32-grade (hi, lo) bf16 pair.  qkv_hi /
+ * qkv_lo point at [B*T, ld] projections with H q-heads, then H k-heads, then H v-heads (64 columns each); o_hi / o_lo are
+ * [B*T, ldo].  S = Qh Kh^T + Qh Kl^T + Ql Kh^T and O = Ph Vh + Ph Vl + Pl Vh in fp32; the output pair is
+ * hi = bf16(o), lo = bf16(o - hi). */
+int sk_attn_tc_fwd_split(const void* qkv_hi, const void* qkv_lo, void* o_hi, void* o_lo, int B, int T, int H, int ld,
+                         int ldo, float scale, void* stream);
 
 /* ---- optimiser ----------------------------------------------------------------------------------------------------
  * Gradient clipping + AdamW as HF Trainer runs them (HF:trainer.py clip_grad_norm_ then torch.optim.AdamW(fused)):

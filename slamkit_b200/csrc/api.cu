@@ -205,6 +205,11 @@ int sk_attn_tc_bwd(const void* qkv, const void* o, const void* d_o, const float*
   return sk_attn_tc_bwd_launch(CBF(qkv), CBF(o), CBF(d_o), lse, delta, partial, BF(dqkv), B, T, H, KVH, ld, ldo, ldg, causal,
                                scale, S(stream), seg_start, seg_end);
 }
+int sk_attn_tc_fwd_split(const void* qkv_hi, const void* qkv_lo, void* o_hi, void* o_lo, int B, int T, int H, int ld,
+                         int ldo, float scale, void* stream) {
+  SK_REQUIRE(qkv_hi && qkv_lo && o_hi && o_lo, "sk_attn_tc_fwd_split: null argument");
+  return sk_attn_tc_fwd_split_launch(CBF(qkv_hi), CBF(qkv_lo), BF(o_hi), BF(o_lo), B, T, H, ld, ldo, scale, S(stream));
+}
 int sk_attn_bwd(const void* q, const void* k, const void* v, const void* o, const void* d_o, const float* lse,
                 float* delta, void* dq, void* dk, void* dv, int B, int T, int H, int KVH, int ld, int ldo, int ldg,
                 int causal, float scale, void* stream) {

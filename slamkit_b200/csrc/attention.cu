@@ -657,6 +657,7 @@ int set_smem(K kernel, int bytes) {
 int sk_attn_fwd_launch(const bf16* q, const bf16* k, const bf16* v, bf16* o, float* lse, int B, int T, int H, int KVH,
                        int ld, int ldo, int causal, float scale, cudaStream_t s, const int* seg_start) {
   SK_REQUIRE(seg_start == nullptr || causal, "attention: document segments need the causal kernel");
+  SK_REQUIRE(B > 0 && T > 0 && H > 0 && KVH > 0, "attention: bad shape B=%d T=%d H=%d KVH=%d", B, T, H, KVH);
   SK_REQUIRE(H % KVH == 0, "attention: H must be a multiple of KVH");
   SK_REQUIRE(ld % 8 == 0 && ldo % 8 == 0, "attention: leading dims must be multiples of 8");
   static bool init = false;
@@ -679,7 +680,10 @@ int sk_attn_bwd_launch(const bf16* q, const bf16* k, const bf16* v, const bf16* 
                        float* delta, bf16* dq, bf16* dk, bf16* dv, int B, int T, int H, int KVH, int ld, int ldo,
                        int ldg, int causal, float scale, cudaStream_t s, const int* seg_start) {
   SK_REQUIRE(seg_start == nullptr || causal, "attention: document segments need the causal kernels");
+  SK_REQUIRE(B > 0 && T > 0 && H > 0 && KVH > 0, "attention: bad shape B=%d T=%d H=%d KVH=%d", B, T, H, KVH);
   SK_REQUIRE(H % KVH == 0, "attention: H must be a multiple of KVH");
+  // q/k/v/o/d_o are read 16 bytes at a time (cp.async, ldg128); dq/dk/dv are written as bf16 pairs
+  SK_REQUIRE(ld % 8 == 0 && ldo % 8 == 0 && ldg % 2 == 0, "attention: ld and ldo must be multiples of 8 and ldg even");
   static bool init = false;
   if (!init) {
     if (set_smem(attn_bwd_dkdv_kernel<true>, DKDV_SMEM)) return -2;
@@ -714,6 +718,7 @@ int sk_attn_bwd_launch(const bf16* q, const bf16* k, const bf16* v, const bf16* 
 int sk_attn_fwd_split_launch(const bf16* q_hi, const bf16* q_lo, const bf16* k_hi, const bf16* k_lo, const bf16* v_hi,
                              const bf16* v_lo, bf16* o_hi, bf16* o_lo, int B, int T, int H, int ld, int ldo, float scale,
                              cudaStream_t s) {
+  SK_REQUIRE(B > 0 && T > 0 && H > 0, "attention: bad shape B=%d T=%d H=%d", B, T, H);
   SK_REQUIRE(ld % 8 == 0 && ldo % 8 == 0, "attention: leading dims must be multiples of 8");
   static bool init = false;
   if (!init) {

@@ -293,6 +293,18 @@ def attn_tc_bwd(qkv, o, d_o, lse, B, T, H, KVH, causal: bool, scale: float, seg_
     return dqkv
 
 
+def attn_tc_fwd_split(qkv_hi: torch.Tensor, qkv_lo: torch.Tensor, B: int, T: int, H: int, scale: float):
+    """Split-bf16 bidirectional forward of the HuBERT encoder (sk_attn_tc_fwd_split).  qkv_hi / qkv_lo: [B*T, 3*H*64]
+    (H q-, k- and v-heads) with the same row pitch.  Returns (o_hi, o_lo) [B*T, H*64]."""
+    lib = L.require_cuda()
+    assert qkv_hi.stride(0) == qkv_lo.stride(0)
+    o_hi = torch.empty((B * T, H * 64), device=qkv_hi.device, dtype=torch.bfloat16)
+    o_lo = torch.empty_like(o_hi)
+    L.check(lib.sk_attn_tc_fwd_split(L.ptr(qkv_hi), L.ptr(qkv_lo), L.ptr(o_hi), L.ptr(o_lo), B, T, H, qkv_hi.stride(0),
+                                     o_hi.stride(0), L.f32(scale), L.stream_ptr()))
+    return o_hi, o_lo
+
+
 def attn_bwd(qkv, o, d_o, lse, B, T, H, KVH, causal: bool, scale: float) -> torch.Tensor:
     lib = L.require_cuda()
     hd = 64
