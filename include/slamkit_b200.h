@@ -72,6 +72,39 @@ typedef struct SkGemmPlan {
 int sk_gemm_plan(int M, int N, int K, const void* A, int lda, int a_mn, const void* B, int ldb, int b_mn, const void* C,
                  int ldc, int out_f32, const void* bias, const void* residual, int ldr, int round_before_res, int act,
                  int force_bn, const void* ws, int64_t ws_bytes, SkGemmPlan* plan);
+/* Test hooks: the batched / split-bf16 form of the GEMM that the HuBERT path runs (sk_hubert_*), so that its features
+ * can be checked on their own.  C[b*M + m, n] = act(sum over the passes + bias) (+ residual), with
+ *   passes 1: A*B^T;  passes 3: A*B^T + A*B_lo^T + A_lo*B^T (split-bf16, fp32-grade products);
+ *   a_rows > 0: A is the 3-D K-major view (a_inner elements per row, a_rows rows a_row_stride apart, batch items
+ *     a_batch_stride apart): row m of batch item b is A[b*a_batch_stride + m*a_row_stride, + K) (strided-window conv);
+ *   a_mode 1 (needs the 3-D view; 64-column tiles): k-block kb of row m, column tile n reads A[b][m + kb][64n, 64n + 64)
+ *     (grouped positional conv on a [B, T + halo, G*64] staging buffer);
+ *   col_gin > 0: accumulator column c goes to output column (c / col_gin) * col_gout + c % col_gin and is dropped when
+ *     c % col_gin >= col_gout (bias is read at c, residual at the output column);
+ *   out_f32: C is fp32; else C (and C_lo when non-NULL: lo = bf16(v - bf16(v))) are bf16;
+ *   bias_f32: bias is fp32; residual_lo (optional) is added after residual.
+ * All elements counts and pitches are in elements.  sk_gemm_split_plan reports the schedule after the same argument
+ * checks, without launching or dereferencing anything. */
+typedef struct SkGemmSplitDesc {
+  int32_t M, N, K, batch, a_mode, passes;
+  const void* A;
+  const void* A_lo;
+  int32_t lda, a_mn;
+  int64_t a_inner, a_rows, a_row_stride, a_batch_stride;
+  const void* B;
+  const void* B_lo;
+  int32_t ldb;
+  void* C;
+  void* C_lo;
+  int32_t ldc, out_f32;
+  const void* bias;
+  int32_t bias_f32;
+  const void* residual;
+  const void* residual_lo;
+  int32_t ldr, act, col_gin, col_gout, force_bn;
+} SkGemmSplitDesc;
+int sk_gemm_split(const SkGemmSplitDesc* desc, void* stream);
+int sk_gemm_split_plan(const SkGemmSplitDesc* desc, SkGemmPlan* plan);
 
 /* Linears of the LM step with the following element-wise op fused into the GEMM epilogue (no extra pass over HBM).
  * sk_linear_swiglu_fwd: gu[M,2F] = x[M,K] * w_gu[2F,K]^T and act[M,F] = bf16(bf16(silu(gate)) * up)  (Qwen2MLP,
@@ -385,7 +418,9 @@ int sk_hubert_units(SkHubert* h, const float* wav, const int64_t* lens, int B, i
 /* the fp32 layer-`n_layers` features [B*T, hidden] (parity checks against hidden_states[layer]) */
 int sk_hubert_features(SkHubert* h, const float* wav, int B, int S, float* feat, void* stream);
 /* Test hook: run the pass up to one stage and return that stage as fp32. stage 100+i = conv layer i output
- * [B*T_i, conv_dim]; 200 = projection [B*T, hidden]; 201 = positional conv; 0..n_layers = hidden_states[stage]. */
+ * [B*T_i, conv_dim]; 200 = projection [B*T, hidden]; 201 = positional conv; 0..n_layers = hidden_states[stage];
+ * 300 + 10 l + j = inside encoder layer l: j = 0 qkv projection [B*T, 3 hidden], 1 attention, 2 o-proj + residual,
+ * 3 first LayerNorm, 4 GELU(ff1) [B*T, ffn], 5 ff2 + residual (each [B*T, hidden] unless given). */
 int sk_hubert_debug_stage(SkHubert* h, const float* wav, int B, int S, int stage, float* out, void* stream);
 /* Run-length dedup of each row's first n_frames[b] labels (UnitTokeniser.audio_represent,
  * slamkit/tokeniser/unit_tokeniser.py:57): units/durations int32 [B,T], counts int32 [B]. */

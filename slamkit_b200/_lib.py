@@ -110,6 +110,21 @@ class SkGemmPlan(C.Structure):
     ]
 
 
+class SkGemmSplitDesc(C.Structure):
+    """sk_gemm_split / sk_gemm_split_plan: the batched, split-bf16 GEMM of the HuBERT path (see the header)."""
+    _fields_ = [
+        ("M", C.c_int32), ("N", C.c_int32), ("K", C.c_int32), ("batch", C.c_int32), ("a_mode", C.c_int32),
+        ("passes", C.c_int32),
+        ("A", C.c_void_p), ("A_lo", C.c_void_p), ("lda", C.c_int32), ("a_mn", C.c_int32),
+        ("a_inner", C.c_int64), ("a_rows", C.c_int64), ("a_row_stride", C.c_int64), ("a_batch_stride", C.c_int64),
+        ("B", C.c_void_p), ("B_lo", C.c_void_p), ("ldb", C.c_int32),
+        ("C", C.c_void_p), ("C_lo", C.c_void_p), ("ldc", C.c_int32), ("out_f32", C.c_int32),
+        ("bias", C.c_void_p), ("bias_f32", C.c_int32),
+        ("residual", C.c_void_p), ("residual_lo", C.c_void_p), ("ldr", C.c_int32), ("act", C.c_int32),
+        ("col_gin", C.c_int32), ("col_gout", C.c_int32), ("force_bn", C.c_int32),
+    ]
+
+
 def declared_symbols() -> List[str]:
     """Names of all functions declared in include/slamkit_b200.h (used by the CPU symbol-export test)."""
     text = open(HEADER_PATH).read()

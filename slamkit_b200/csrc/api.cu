@@ -6,6 +6,7 @@
 #include <atomic>
 #include <stdarg.h>
 #include <stdio.h>
+#include <string.h>
 #include <vector>
 
 namespace {
@@ -141,6 +142,37 @@ int sk_gemm_plan(int M, int N, int K, const void* A, int lda, int a_mn, const vo
   return sk_gemm_plan_ex(sk_gemm_desc(M, N, K, A, lda, a_mn, B, ldb, b_mn, const_cast<void*>(C), ldc, out_f32, bias, residual,
                                       ldr, round_before_res, act, force_bn, const_cast<void*>(ws), (size_t)ws_bytes),
                          plan);
+}
+}  // extern "C"
+
+namespace {
+SkGemmEx split_desc_to_ex(const SkGemmSplitDesc& d) {
+  SkGemmEx g;
+  memset(&g, 0, sizeof(g));
+  g.M = d.M; g.N = d.N; g.K = d.K; g.batch = d.batch; g.a_mode = d.a_mode; g.passes = d.passes;
+  g.A = d.A; g.A_lo = d.A_lo; g.lda = d.lda; g.a_mn = d.a_mn;
+  g.a_inner = (long)d.a_inner; g.a_rows = (long)d.a_rows; g.a_row_stride = (long)d.a_row_stride;
+  g.a_batch_stride = (long)d.a_batch_stride;
+  g.B = d.B; g.B_lo = d.B_lo; g.ldb = d.ldb;
+  g.C = d.C; g.C_lo = d.C_lo; g.ldc = d.ldc; g.out_f32 = d.out_f32;
+  g.bias = d.bias; g.bias_f32 = d.bias_f32;
+  g.residual = d.residual; g.residual_lo = d.residual_lo; g.ldr = d.ldr;
+  g.act = d.act;
+  g.col_gin = d.col_gin; g.col_gout = d.col_gout;
+  g.force_bn = d.force_bn;
+  return g;
+}
+}  // namespace
+
+extern "C" {
+
+int sk_gemm_split(const SkGemmSplitDesc* desc, void* stream) {
+  SK_REQUIRE(desc && desc->A && desc->B && desc->C, "sk_gemm_split: null argument");
+  return sk_gemm_ex_launch(split_desc_to_ex(*desc), S(stream));
+}
+int sk_gemm_split_plan(const SkGemmSplitDesc* desc, SkGemmPlan* plan) {
+  SK_REQUIRE(desc && plan, "sk_gemm_split_plan: null argument");
+  return sk_gemm_plan_ex(split_desc_to_ex(*desc), plan);
 }
 int sk_embed_fwd(const int64_t* ids, const void* table, void* out, int M, int D, int V, void* stream) {
   return sk_embed_fwd_launch(ids, CBF(table), BF(out), M, D, V, S(stream));

@@ -85,10 +85,16 @@ __global__ void split_f32_kernel(const float* __restrict__ x, bf16* __restrict__
 // bilinear forms in the KW window sums  S[j] = sum_t x[ST t + j]  and  R[j][j'] = sum_t x[ST t + j] x[ST t + j']:
 //   sum_t y_c = sum_j w_cj S_j ,  sum_t y_c^2 = sum_jj' w_cj w_cj' R_jj'.
 // So the statistics pass reads the waveform once and never touches the C x T output.  Accumulated in fp64.
+// Each stats block writes its partial sums to its own slot and the affine kernel adds the slots in block order, so the
+// GroupNorm affine -- and every feature after it -- is bit-reproducible.  The block partition depends on T0 only (not on
+// B or on the launch), so a clip gets the same statistics alone and inside any batch.
 // The (pad,pad) zero padding of the reference (F.pad(wav,(40,40))) is applied by index arithmetic.
 // ------------------------------------------------------------------------------------------------
 constexpr int KW_MAX = 10;
 constexpr int NSTAT = KW_MAX + KW_MAX * (KW_MAX + 1) / 2;  // 65
+constexpr int STAT_BLOCKS_MAX = 64;                         // stats blocks (partial slots) per clip
+
+inline int conv0_stat_blocks(int T0) { return std::max(1, std::min(STAT_BLOCKS_MAX, (T0 + 255) / 256)); }
 
 SK_DEVINL float wav_at(const float* __restrict__ w, long i, int S, int pad) {
   const long j = i - pad;
@@ -96,8 +102,8 @@ SK_DEVINL float wav_at(const float* __restrict__ w, long i, int S, int pad) {
 }
 
 __global__ void __launch_bounds__(256)
-conv0_stats_kernel(const float* __restrict__ wav, double* __restrict__ stats /*[B][NSTAT]*/, int S, int pad, int T0,
-                   int KW, int ST) {
+conv0_stats_kernel(const float* __restrict__ wav, double* __restrict__ stats /*[B][STAT_BLOCKS_MAX][NSTAT]*/, int S,
+                   int pad, int T0, int KW, int ST) {
   __shared__ double sred[8][NSTAT];
   const int b = blockIdx.y;
   const float* w = wav + (size_t)b * S;
@@ -127,18 +133,26 @@ conv0_stats_kernel(const float* __restrict__ wav, double* __restrict__ stats /*[
   for (int i = threadIdx.x; i < NSTAT; i += blockDim.x) {
     double v = 0.0;
     for (int wi = 0; wi < 8; ++wi) v += sred[wi][i];
-    atomicAdd(stats + (size_t)b * NSTAT + i, v);
+    stats[((size_t)b * STAT_BLOCKS_MAX + blockIdx.x) * NSTAT + i] = v;
   }
 }
 
-// per (clip, channel): scale = gamma * rstd, shift = beta - mean * gamma * rstd
+// per (clip, channel): scale = gamma * rstd, shift = beta - mean * gamma * rstd.  The block first adds the n_blk
+// partial slots of its clip in slot order (fixed order: deterministic), then each thread forms its channel's affine.
 __global__ void conv0_affine_kernel(const double* __restrict__ stats, const float* __restrict__ w /*[C][KW]*/,
                                     const float* __restrict__ gamma, const float* __restrict__ beta,
-                                    float2* __restrict__ affine /*[B][C]*/, int C, int KW, int T0, float eps) {
+                                    float2* __restrict__ affine /*[B][C]*/, int C, int KW, int T0, int n_blk, float eps) {
+  __shared__ double st[NSTAT];
   const int b = blockIdx.y;
+  for (int i = threadIdx.x; i < NSTAT; i += blockDim.x) {
+    const double* sp = stats + (size_t)b * STAT_BLOCKS_MAX * NSTAT + i;
+    double v = 0.0;
+    for (int k = 0; k < n_blk; ++k) v += sp[(size_t)k * NSTAT];
+    st[i] = v;
+  }
+  __syncthreads();
   const int c = blockIdx.x * blockDim.x + threadIdx.x;
   if (c >= C) return;
-  const double* st = stats + (size_t)b * NSTAT;
   double m = 0.0, e2 = 0.0;
   int q = KW_MAX;
   for (int j = 0; j < KW_MAX; ++j) {
@@ -524,7 +538,8 @@ __global__ void regroup_pad_kernel(const bf16* __restrict__ in_hi, const bf16* _
 
 // ------------------------------------------------------------------------------------------------
 // k-means labels: label[m] = argmin_j (csq[j] - 2 * dot[m][j]), first minimum wins (SK:_k_means_lloyd.pyx:198-213).
-// dot: fp32 [M, ld] from the split GEMM; one warp per row.
+// dot: fp32 [M, ld] from the split GEMM; one warp per row.  Every lane starts at label 0, as sklearn's loop does: a row
+// with no distance below +inf (NaN features from non-finite audio) gets label 0, never an id outside [0, U).
 // ------------------------------------------------------------------------------------------------
 __global__ void __launch_bounds__(256)
 kmeans_argmin_kernel(const float* __restrict__ dot, const float* __restrict__ csq, int32_t* __restrict__ labels, int M,
@@ -533,7 +548,7 @@ kmeans_argmin_kernel(const float* __restrict__ dot, const float* __restrict__ cs
   const int row = blockIdx.x * 8 + warp;
   if (row >= M) return;
   float best = INFINITY;
-  int bi = 0x7fffffff;
+  int bi = 0;
   for (int j = lane; j < U; j += 32) {
     const float d = csq[j] + (-2.0f) * dot[(size_t)row * ld + j];
     if (d < best) { best = d; bi = j; }   // ascending j per lane: strict '<' keeps the first minimum
@@ -627,18 +642,17 @@ int sk_split_f32_launch(const float* x, bf16* hi, bf16* lo, long n, cudaStream_t
   SK_LAUNCH_CHECK();
   return 0;
 }
-extern "C" int sk_conv0_nstat(void) { return NSTAT; }
+extern "C" int sk_conv0_nstat(void) { return STAT_BLOCKS_MAX * NSTAT; }
 int sk_conv0_launch(const float* wav, const float* w, const float* gamma, const float* beta, double* stats,
                     float2* affine, bf16* out_hi, bf16* out_lo, int B, int S, int pad, int T0, int C, int KW, int ST,
                     float eps, cudaStream_t s) {
   SK_REQUIRE(KW <= KW_MAX, "conv0: kernel width %d > %d", KW, KW_MAX);
   SK_REQUIRE(C % 8 == 0 && C / 4 <= 256, "conv0: channel count must be a multiple of 8 and <= 1024");
-  SK_CUDA_CHECK(cudaMemsetAsync(stats, 0, (size_t)B * NSTAT * sizeof(double), s));
-  dim3 g1(std::min(64, (T0 + 255) / 256), B);
-  conv0_stats_kernel<<<g1, 256, 0, s>>>(wav, stats, S, pad, T0, KW, ST);
+  const int n_blk = conv0_stat_blocks(T0);
+  conv0_stats_kernel<<<dim3(n_blk, B), 256, 0, s>>>(wav, stats, S, pad, T0, KW, ST);
   SK_LAUNCH_CHECK();
   dim3 g2((C + 127) / 128, B);
-  conv0_affine_kernel<<<g2, 128, 0, s>>>(stats, w, gamma, beta, affine, C, KW, T0, eps);
+  conv0_affine_kernel<<<g2, 128, 0, s>>>(stats, w, gamma, beta, affine, C, KW, T0, n_blk, eps);
   SK_LAUNCH_CHECK();
   static const int mode = [] { const char* e = getenv("SK_CONV0_MODE"); return e ? atoi(e) : 2; }();
   // CUDA-core paths: HuBERT's kernel 10 / stride 5 front with 4 channels x 2 frames per thread; generic kernel otherwise

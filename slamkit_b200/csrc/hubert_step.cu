@@ -132,7 +132,8 @@ int linear_split(const SkHubert* h, int M, int N, int K, HiLo x, int64_t w_off, 
 }
 
 // dbg_stage (tests only): 100+i = output of conv layer i, 200 = projection, 201 = positional conv (post-GELU),
-// 0..n_layers = hidden_states[stage]; the fp32 stage tensor is written to feat_out and the pass stops there.
+// 0..n_layers = hidden_states[stage], 300 + 10 l + j = intermediate j of encoder layer l (see the layer loop); the fp32
+// stage tensor is written to feat_out and the pass stops there.
 int forward_impl(SkHubert* h, const float* wav, const int64_t* lens, int B, int S, int32_t* ids, int32_t* n_frames,
                  float* feat_out, cudaStream_t s, int dbg_stage = -1) {
   SK_REQUIRE(h->w_hi && h->ws, "sk_hubert: sk_hubert_bind has not been called");
@@ -207,20 +208,37 @@ int forward_impl(SkHubert* h, const float* wav, const int64_t* lens, int B, int 
   HiLo qkv = hl(h, w.qkv, (int64_t)M * 3 * H), ao = hl(h, w.ao, (int64_t)M * H), t1 = hl(h, w.t1, (int64_t)M * H),
        ff = hl(h, w.ff, (int64_t)M * F);
   const float scale = 1.0f / sqrtf((float)(H / h->cfg.n_heads));
+  // dbg_stage 300 + 10 l + j: intermediate j of layer l (0 qkv, 1 attention, 2 o-proj + residual, 3 LN1, 4 ff1 GELU,
+  // 5 ff2 + residual)
+  auto tap = [&](int l, int j, HiLo t, int cols) {
+    return dbg_stage == 300 + 10 * l + j ? sk_hilo_to_f32_launch(t.hi, t.lo, feat_out, (long)M * cols, s) : -1;
+  };
+#define SK_TAP(l, j, t, cols)                  \
+  do {                                         \
+    const int _rc = tap(l, j, t, cols);        \
+    if (_rc >= 0) return _rc;                  \
+  } while (0)
   for (int l = 0; l < h->cfg.n_layers; ++l) {
     const LayerOff& o = h->lo[l];
     const bool last = (l == h->cfg.n_layers - 1) || (dbg_stage == l + 1);
     SK_TRY(linear_split(h, M, 3 * H, H, hb[0], o.wqkv, o.bqkv, 0, nullptr, qkv, nullptr, 3 * H, s));
+    SK_TAP(l, 0, qkv, 3 * H);
     SK_TRY(sk_attn_tc_fwd_split_launch(qkv.hi, qkv.lo, ao.hi, ao.lo, B, Tf, h->cfg.n_heads, 3 * H, H, scale, s));
+    SK_TAP(l, 1, ao, H);
     SK_TRY(linear_split(h, M, H, H, ao, o.wo, o.bo, 0, &hb[0], t1, nullptr, H, s));
+    SK_TAP(l, 2, t1, H);
     SK_TRY(sk_layernorm_hilo_launch(t1.hi, t1.lo, nullptr, nullptr, h->w32 + o.ln1g, h->w32 + o.ln1b, hb[1].hi, hb[1].lo,
                                     nullptr, M, H, eps, s));
+    SK_TAP(l, 3, hb[1], H);
     SK_TRY(linear_split(h, M, F, H, hb[1], o.w1, o.b1, 1, nullptr, ff, nullptr, F, s));
+    SK_TAP(l, 4, ff, F);
     SK_TRY(linear_split(h, M, H, F, ff, o.w2, o.b2, 0, &hb[1], t1, nullptr, H, s));
+    SK_TAP(l, 5, t1, H);
     SK_TRY(sk_layernorm_hilo_launch(t1.hi, t1.lo, nullptr, nullptr, h->w32 + o.ln2g, h->w32 + o.ln2b, hb[0].hi, hb[0].lo,
                                     last ? feat_out : nullptr, M, H, eps, s));
     if (dbg_stage == l + 1) return 0;
   }
+#undef SK_TAP
   if (ids) {
     float* dot = reinterpret_cast<float*>(h->ws + w.dot);
     SK_TRY(linear_split(h, M, h->Upad, H, hb[0], h->km_c, -1, 0, nullptr, HiLo{nullptr, nullptr}, dot, h->Upad, s));

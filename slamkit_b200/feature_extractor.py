@@ -218,9 +218,14 @@ class HubertB200FeatureExtractor(torch.nn.Module):
 
     @torch.inference_mode()
     def extract(self, wav: torch.Tensor, lens: Optional[torch.Tensor] = None) -> List[np.ndarray]:
-        """hubert_feature_extractor.py:40-50: list of per-clip unit-id arrays, trimmed to ceil(len/S*T) frames."""
+        """hubert_feature_extractor.py:40-50: list of per-clip unit-id arrays, trimmed to ceil(len/S*T) frames.
+        Raises ValueError when the audio holds NaN or Inf, as the reference's k-means input validation does (the
+        device labels of such clips are in range but meaningless)."""
         ids, nf = self.units_device(wav, lens)
+        finite = bool(torch.isfinite(wav).all())
         ids_h, nf_h = ids.cpu().numpy(), nf.cpu().numpy()
+        if not finite:
+            raise ValueError("HuBERT features are not finite: the input audio holds NaN or Inf samples")
         return [ids_h[b, :nf_h[b]] for b in range(ids_h.shape[0])]
 
     @torch.inference_mode()
