@@ -53,9 +53,9 @@ def load_model(cfg, device: str, max_seq: int = 256):
     if not path:
         raise ValueError("no pretrained model: pass model.pretrained_model=<dir>")
     base = json.load(open(os.path.join(path, "config.json"))).get("base_config", {})
-    if base.get("model_type") not in ("qwen2", "opt"):
+    if base.get("model_type") not in ("qwen2", "opt", "gpt_neox"):
         raise ValueError(f"unsupported base architecture '{base.get('model_type')}' in {path}: the GPU scoring path "
-                         "implements the Qwen2 and OPT decoders")
+                         "implements the Qwen2, OPT and GPT-NeoX decoders")
     return B200UnitLM.from_pretrained(path, device=device, max_batch=cfg.batch_size, max_seq=max_seq, trainable=False)
 
 

@@ -118,6 +118,23 @@ int sk_linear_swiglu_fwd(int M, int F, int K, const void* x, const void* w_gu, v
 int sk_linear_swiglu_bwd(int M, int N, int F, const void* dy, const void* w_down, const void* gu, void* dgu, void* stream);
 int sk_linear_rope(int M, int N, int K, const void* x, const void* w, const void* bias, void* out, const void* cos_t,
                    const void* sin_t, const int32_t* pos_ids, int T, int rope_cols, int max_positions, void* stream);
+/* GPT-NeoX epilogues (HF:models/gpt_neox/modeling_gpt_neox.py):
+ * sk_linear_rope_partial: sk_linear_rope where only the first rot_dims (16, 32 or 64) columns of each rotated head turn,
+ *   element i with i + rot_dims/2, with bf16 tables [max_positions, rot_dims/2]; rot_dims = 64 is sk_linear_rope.
+ * sk_linear_gelu_fwd: pre[M,F] = bf16(x[M,K] * w1[F,K]^T + b1) and act[M,F] = bf16(gelu_erf(pre)); F % 64 == 0.
+ * sk_linear_gelu_bwd: dpre[M,F] = bf16(bf16(dy[M,N] * w2[N,F]) * gelu'(pre)); d_act is never written.
+ * sk_linear_res2: out[M,N] = bf16(bf16(bf16(x * w^T + bias) + res2) + res) (mlp + attn + x in HF's order; out may be res).
+ *   ws / ws_bytes: optional stream-K scratch as for sk_gemm_bf16_ws. */
+int sk_linear_rope_partial(int M, int N, int K, const void* x, const void* w, const void* bias, void* out, const void* cos_t,
+                           const void* sin_t, const int32_t* pos_ids, int T, int rope_cols, int max_positions, int rot_dims,
+                           void* stream);
+int sk_linear_gelu_fwd(int M, int F, int K, const void* x, const void* w1, const void* b1, void* pre, void* act, void* stream);
+int sk_linear_gelu_bwd(int M, int N, int F, const void* dy, const void* w2, const void* pre, void* dpre, void* stream);
+int sk_linear_res2(int M, int N, int K, const void* x, const void* w, const void* bias, const void* res2, const void* res,
+                   void* out, void* ws, int64_t ws_bytes, void* stream);
+/* Test hook: the schedule of the four launches above (kind 0 rope_partial, 1 gelu_fwd, 2 gelu_bwd, 3 res2 with the
+ * scratch of sk_gemm_ws_bytes() when with_ws), for an M x N x K problem; nothing is launched. */
+int sk_neox_gemm_plan(int kind, int M, int N, int K, int with_ws, SkGemmPlan* plan);
 
 /* ---- causal-LM element-wise / reduction kernels (path (ii)) --------------------------------------------------- */
 /* Embedding lookup, HF:models/qwen2/modeling_qwen2.py:332-415 (embed_tokens). ids int64 [M]. */
@@ -142,6 +159,15 @@ int sk_layernorm_bwd_blocks(void);
 int sk_layernorm_bwd(const void* dy, const void* x, const void* w, const float* mean, const float* rstd, const void* dres,
                      void* dx, void* dw, void* db, float* dw_partial, float* db_partial, int M, int D, int accumulate,
                      void* stream);
+/* GPT-NeoX parallel residual: y1 = LN(x; w1, b1) and y2 = LN(x; w2, b2) from one read of x, each bit-identical to
+ * sk_layernorm_fwd; mean / rstd (fp32 [M], may be NULL) are shared.  The backward forms, in fp32,
+ * dx = dres + LN'(w1 * dy1 + w2 * dy2) and dw1 / db1 / dw2 / db2 (+)= their row sums through fixed-order per-block
+ * partials (deterministic).  partial: fp32 [4 * sk_layernorm_bwd_blocks() * D].  D <= 2048. */
+int sk_layernorm2_fwd(const void* x, const void* w1, const void* b1, const void* w2, const void* b2, void* y1, void* y2,
+                      float* mean, float* rstd, int M, int D, float eps, void* stream);
+int sk_layernorm2_bwd(const void* dy1, const void* dy2, const void* x, const void* w1, const void* w2, const float* mean,
+                      const float* rstd, const void* dres, void* dx, void* dw1, void* db1, void* dw2, void* db2,
+                      float* partial, int M, int D, int accumulate, void* stream);
 /* Column sums of a bf16 matrix (bias gradient). partial: fp32 [sk_colsum_splits()*N]. */
 int sk_colsum_splits(void);
 int sk_colsum(const void* x, void* out, float* partial, int M, int N, int ld, int accumulate, void* stream);
@@ -151,6 +177,10 @@ int sk_colsum(const void* x, void* out, float* partial, int M, int N, int ld, in
  * inverse=1 applies the transposed rotation (backward). */
 int sk_rope(void* qkv, const void* cos_t, const void* sin_t, const int32_t* pos_ids, int M, int T, int ld,
             int n_rot_heads, int head_dim, int inverse, int max_positions, void* stream);
+/* sk_rope with GPT-NeoX partial rotary: the first rot_dims (16, 32 or head_dim = 64) columns of each head turn, tables
+ * bf16 [max_positions, rot_dims/2]; the other columns are left as they are. */
+int sk_rope_partial(void* qkv, const void* cos_t, const void* sin_t, const int32_t* pos_ids, int M, int T, int ld,
+                    int n_rot_heads, int head_dim, int rot_dims, int inverse, int max_positions, void* stream);
 /* Qwen2MLP activation down(silu(gate)*up), HF:models/qwen2/modeling_qwen2.py:35-48. gu = [gate | up], each F wide. */
 int sk_swiglu_fwd(const void* gu, void* act, int M, int F, void* stream);
 int sk_swiglu_bwd(const void* gu, const void* dact, void* dgu, int M, int F, void* stream);
@@ -253,6 +283,29 @@ typedef struct SkOptConfig {
   int32_t tie_embeddings;    /* 1: lm_head shares the token embedding table */
 } SkOptConfig;
 int sk_lm_create_opt(const SkOptConfig* cfg, SkLm** out);
+/* GPT-NeoX decoder with the parallel residual (HF GPTNeoXForCausalLM, use_parallel_residual = True, e.g. the Pythia
+ * models with head_dim 64: pythia-70m / -160m / -410m; HF:models/gpt_neox/modeling_gpt_neox.py):
+ *   x0 = embed_in[id];  per layer  h1 = LN1(x), h2 = LN2(x);  q|k|v = h1 W + b;  RoPE on the first rot_dims columns of
+ *   each q / k head;  causal MHA with scale 1/8;  attn = o W_o + b_o;  mlp = gelu(h2 W_1 + b_1) W_2 + b_2;
+ *   x = bf16(bf16(mlp + attn) + x);  final LN, untied embed_out without bias.
+ * Differences from a Qwen2 handle:
+ *   - the flat layout lists per layer ln1, ln1_b, ln2, ln2_b, wqkv [3*hidden, hidden] in [Q;K;V] row order (HF stores
+ *     per-head [q|k|v] blocks: the caller permutes), bqkv, wo, bo, w1 [ffn, hidden], b1, w2 [hidden, ffn], b2; then
+ *     final_norm, final_norm_b, embed [Vpad, hidden], lm_head [Vpad, hidden];
+ *   - sk_lm_bind takes RoPE tables of bf16 [max_positions, rot_dims/2];
+ *   - the gradient-norm groups are GPTNeoXForCausalLM's parameters (query_key_value weight and bias are one tensor each);
+ *   - the KV cache holds n_heads K/V heads per layer. */
+typedef struct SkNeoxConfig {
+  int32_t vocab_size;        /* 502 for unit_hubert_25 */
+  int32_t hidden;            /* 768 for pythia-160m; n_heads * 64, <= 2048 */
+  int32_t n_layers;
+  int32_t n_heads;
+  int32_t ffn;               /* intermediate_size (4 * hidden); a multiple of 64 */
+  int32_t max_positions;     /* rows of the RoPE tables */
+  int32_t rot_dims;          /* head_dim * partial_rotary_factor: 16, 32 or 64 */
+  float ln_eps;              /* layer_norm_eps, 1e-5 */
+} SkNeoxConfig;
+int sk_lm_create_neox(const SkNeoxConfig* cfg, SkLm** out);
 void sk_lm_destroy(SkLm* lm);
 /* Flat parameter layout (bf16 elements). Tensors are enumerated in a fixed order; name_buf receives e.g.
  * "layers.3.wqkv". Returns the number of tensors when idx < 0. */

@@ -51,6 +51,19 @@ class SkOptConfig(C.Structure):
     ]
 
 
+class SkNeoxConfig(C.Structure):
+    _fields_ = [
+        ("vocab_size", C.c_int32),
+        ("hidden", C.c_int32),
+        ("n_layers", C.c_int32),
+        ("n_heads", C.c_int32),
+        ("ffn", C.c_int32),
+        ("max_positions", C.c_int32),
+        ("rot_dims", C.c_int32),
+        ("ln_eps", C.c_float),
+    ]
+
+
 class SkHubertConfig(C.Structure):
     _fields_ = [
         ("n_conv", C.c_int32),

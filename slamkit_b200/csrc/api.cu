@@ -120,6 +120,48 @@ int sk_linear_rope(int M, int N, int K, const void* x, const void* w, const void
   SK_REQUIRE(x && w && out && cos_t && sin_t, "sk_linear_rope: null operand");
   return sk_linear_rope_launch(M, N, K, x, w, bias, out, cos_t, sin_t, pos_ids, T, rope_cols, max_positions, S(stream));
 }
+int sk_linear_rope_partial(int M, int N, int K, const void* x, const void* w, const void* bias, void* out, const void* cos_t,
+                           const void* sin_t, const int32_t* pos_ids, int T, int rope_cols, int max_positions, int rot_dims,
+                           void* stream) {
+  SK_REQUIRE(x && w && out && cos_t && sin_t, "sk_linear_rope_partial: null operand");
+  SK_REQUIRE(rot_dims == 16 || rot_dims == 32 || rot_dims == 64,
+             "sk_linear_rope_partial: rot_dims=%d is not supported (16, 32 or 64)", rot_dims);
+  return sk_linear_rope_launch(M, N, K, x, w, bias, out, cos_t, sin_t, pos_ids, T, rope_cols, max_positions, S(stream), rot_dims);
+}
+int sk_linear_gelu_fwd(int M, int F, int K, const void* x, const void* w1, const void* b1, void* pre, void* act, void* stream) {
+  SK_REQUIRE(x && w1 && pre && act, "sk_linear_gelu_fwd: null operand");
+  return sk_linear_gelu_fwd_launch(M, F, K, x, w1, b1, pre, act, S(stream));
+}
+int sk_linear_gelu_bwd(int M, int N, int F, const void* dy, const void* w2, const void* pre, void* dpre, void* stream) {
+  SK_REQUIRE(dy && w2 && pre && dpre, "sk_linear_gelu_bwd: null operand");
+  return sk_linear_gelu_bwd_launch(M, N, F, dy, w2, pre, dpre, S(stream));
+}
+int sk_linear_res2(int M, int N, int K, const void* x, const void* w, const void* bias, const void* res2, const void* res,
+                   void* out, void* ws, int64_t ws_bytes, void* stream) {
+  SK_REQUIRE(x && w && res2 && res && out, "sk_linear_res2: null operand");
+  return sk_linear_res2_launch(M, N, K, x, w, bias, res2, res, out, S(stream), ws, (size_t)ws_bytes);
+}
+int sk_neox_gemm_plan(int kind, int M, int N, int K, int with_ws, SkGemmPlan* plan) {
+  SK_REQUIRE(plan && kind >= 0 && kind <= 3, "sk_neox_gemm_plan: kind must be 0..3");
+  // stand-in operands: 256-byte aligned, never dereferenced by the planner
+  void* p = reinterpret_cast<void*>((uintptr_t)1 << 20);
+  SkGemmEx g;
+  memset(&g, 0, sizeof(g));
+  g.M = M; g.N = N; g.K = K; g.batch = 1; g.passes = 1; g.pdl = 1;
+  g.A = p; g.lda = K; g.B = p; g.ldb = K; g.C = p; g.ldc = N;
+  if (kind == 0) {
+    // the fused q|k|v projection: q and k heads rotate
+    g.bias = p; g.epi = 3; g.rope_cos = p; g.rope_sin = p; g.rope_T = 1; g.rope_cols = N / 3 * 2; g.rope_maxpos = 1; g.rope_rot = 16;
+  } else if (kind == 1) {
+    g.bias = p; g.epi = 4; g.aux_out = p; g.ld_aux_out = N;
+  } else if (kind == 2) {
+    g.ldb = N; g.b_mn = 1; g.epi = 5; g.aux = p; g.ld_aux = N;
+  } else {
+    g.bias = p; g.residual = p; g.ldr = N; g.round_before_res = 1; g.epi = 6; g.aux = p; g.ld_aux = N;
+    if (with_ws) { g.splitk_ws = p; g.splitk_ws_bytes = sk_gemm_ws_min_bytes(); }
+  }
+  return sk_gemm_plan_ex(g, plan);
+}
 int sk_gemm_bf16_splitk(int M, int N, int K, const void* A, int lda, int a_mn, const void* B, int ldb, int b_mn, void* C,
                         int ldc, int accumulate, void* splitk_ws, int64_t splitk_ws_bytes, void* stream) {
   SK_REQUIRE(A && B && C, "sk_gemm_bf16_splitk: null operand");
@@ -198,6 +240,25 @@ int sk_layernorm_bwd(const void* dy, const void* x, const void* w, const float* 
                      void* stream) {
   return sk_layernorm_bwd_launch(CBF(dy), CBF(x), CBF(w), mean, rstd, CBF(dres), BF(dx), BF(dw), BF(db), dw_partial, db_partial,
                                  M, D, accumulate, S(stream));
+}
+int sk_layernorm2_fwd(const void* x, const void* w1, const void* b1, const void* w2, const void* b2, void* y1, void* y2,
+                      float* mean, float* rstd, int M, int D, float eps, void* stream) {
+  SK_REQUIRE(x && w1 && b1 && w2 && b2 && y1 && y2, "sk_layernorm2_fwd: null argument");
+  return sk_layernorm2_fwd_launch(CBF(x), CBF(w1), CBF(b1), CBF(w2), CBF(b2), BF(y1), BF(y2), mean, rstd, M, D, eps, S(stream));
+}
+int sk_layernorm2_bwd(const void* dy1, const void* dy2, const void* x, const void* w1, const void* w2, const float* mean,
+                      const float* rstd, const void* dres, void* dx, void* dw1, void* db1, void* dw2, void* db2,
+                      float* partial, int M, int D, int accumulate, void* stream) {
+  SK_REQUIRE(dy1 && dy2 && x && w1 && w2 && mean && rstd && dx && dw1 && db1 && dw2 && db2 && partial,
+             "sk_layernorm2_bwd: null argument");
+  return sk_layernorm2_bwd_launch(CBF(dy1), CBF(dy2), CBF(x), CBF(w1), CBF(w2), mean, rstd, CBF(dres), BF(dx), BF(dw1), BF(db1),
+                                  BF(dw2), BF(db2), partial, M, D, accumulate, S(stream));
+}
+int sk_rope_partial(void* qkv, const void* cos_t, const void* sin_t, const int32_t* pos_ids, int M, int T, int ld,
+                    int n_rot_heads, int head_dim, int rot_dims, int inverse, int max_positions, void* stream) {
+  SK_REQUIRE(rot_dims > 0, "sk_rope_partial: rot_dims must be positive");
+  return sk_rope_launch(BF(qkv), CBF(cos_t), CBF(sin_t), pos_ids, M, T, ld, n_rot_heads, head_dim, inverse, max_positions,
+                        S(stream), rot_dims);
 }
 int sk_colsum(const void* x, void* out, float* partial, int M, int N, int ld, int accumulate, void* stream) {
   return sk_colsum_launch(CBF(x), BF(out), partial, M, N, ld, accumulate, S(stream));

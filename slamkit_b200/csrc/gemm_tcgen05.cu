@@ -69,14 +69,18 @@ struct GemmParams {
   //   1 SwiGLU forward : N = 2F laid out in [128 gate | 128 up] column blocks; writes gu through tmC AND act[M,F] =
   //                      bf16(bf16(silu(gate)) * up) through tmAux -- the unfused swiglu_fwd_kernel's rounding points
   //   2 SwiGLU backward: the accumulator is d_act[M,F]; reads gu (same block layout) and writes d_gu[M,2F] through tmC
-  //   3 RoPE           : after bias + bf16 rounding, every 64-column head below rope_cols is rotated (rotate_half form)
+  //   3 RoPE           : after bias + bf16 rounding, every 64-column head below rope_cols is rotated (rotate_half form);
+  //                      rope_rot < 64: only its first rope_rot columns (GPT-NeoX partial rotary)
+  //   4 GELU forward   : C = pre = bf16(acc + bias) through tmC and bf16(gelu(pre)) through tmAux
+  //   5 GELU backward  : the accumulator is d_act; reads the saved pre (aux) and writes bf16(bf16(d_act) * gelu'(pre))
+  //   6 two residuals  : bf16(bf16(bf16(acc + bias) + aux) + residual), in epi_residual (every output path)
   int epi;
-  const bf16* aux;      // epi 2: gu
+  const bf16* aux;      // epi 2: gu; epi 5: pre; epi 6: the residual added first
   int ld_aux;
-  const bf16* rope_cos; // epi 3: bf16 [rope_maxpos, 32]
+  const bf16* rope_cos; // epi 3: bf16 [rope_maxpos, rope_rot / 2]
   const bf16* rope_sin;
   const int* rope_pos;  // int32 [M] or null (position = row % rope_T)
-  int rope_T, rope_cols, rope_maxpos;
+  int rope_T, rope_cols, rope_maxpos, rope_rot;
 };
 
 template <int BN, int EW = 4>
@@ -148,6 +152,15 @@ SK_DEVINL float gelu_erf(float y) {
   s = fmaf(s, t, 0.5f * 0.254829592f);
   const float e = ex2_approx((y * y) * -0.72134752044448170368f);
   return fmaf(-a, (s * t) * e, fmaxf(y, 0.0f));
+}
+
+// GELU(erf) of the GPT-NeoX MLP (epi 4 / 5): the expressions of torch's CUDA gelu / gelu_backward kernels in fp32 with
+// the accurate erff / expf, so that the bf16 results track torch.nn.functional.gelu and its autograd to the ulp
+SK_DEVINL float gelu_exact(float x) { return x * 0.5f * (1.0f + erff(x * 0.70710678118654752440f)); }
+SK_DEVINL float gelu_exact_grad(float x) {
+  const float cdf = 0.5f * (1.0f + erff(x * 0.70710678118654752440f));
+  const float pdf = expf(-0.5f * x * x) * 0.39894228040143267794f;   // M_2_SQRTPI * M_SQRT1_2 * 0.5
+  return cdf + x * pdf;
 }
 
 // Work scheduler shared by the three warp roles.
@@ -304,6 +317,16 @@ SK_DEVINL void epi_bias_act(float (&v)[8], const GemmParams& p, int col) {
 
 // residual (hi, and lo when present) read at output column `ocol` of row `row`
 SK_DEVINL void epi_residual(float (&v)[8], const GemmParams& p, size_t row, int ocol) {
+  if (p.epi == 6) {   // mlp + attn first, rounded (then + x below with round_before_res)
+    const uint4 av = *reinterpret_cast<const uint4*>(p.aux + row * p.ld_aux + ocol);
+    const uint32_t aw[4] = {av.x, av.y, av.z, av.w};
+#pragma unroll
+    for (int i = 0; i < 4; ++i) {
+      const float2 f = unpack_bf16(aw[i]);
+      v[2 * i] = bf16_round(bf16_round(v[2 * i]) + f.x);
+      v[2 * i + 1] = bf16_round(bf16_round(v[2 * i + 1]) + f.y);
+    }
+  }
   if (!p.residual) return;
   const uint4 rv = *reinterpret_cast<const uint4*>(p.residual + row * p.ldr + ocol);
   const uint32_t rw[4] = {rv.x, rv.y, rv.z, rv.w};
@@ -749,6 +772,131 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
               stage_store(&tmAux, gpk, (n0 >> 1) + i * 64, std::false_type{});
             }
           }
+        } else if (!SK && p.tma_store && p.epi == 3 && p.rope_rot < 64) {
+          // ---- bias + partial RoPE (GPT-NeoX): in each head, element i < rope_rot/2 pairs with i + rope_rot/2; the
+          // columns from rope_rot on get the bias only.  Same rounding points as the whole-head form below ----
+          const int half = p.rope_rot >> 1;   // 8 or 16
+          float cf[16], sf[16];
+          {
+            int pos = 0;
+            if (row_ok) pos = p.rope_pos ? p.rope_pos[row] : (int)(row % (size_t)p.rope_T);
+            pos = max(0, min(pos, p.rope_maxpos - 1));
+#pragma unroll
+            for (int j = 0; j < 2; ++j) {
+              uint4 c = make_uint4(0u, 0u, 0u, 0u), sn = make_uint4(0u, 0u, 0u, 0u);
+              if (8 * j < half) {
+                c = ldg128(p.rope_cos + (size_t)pos * half + 8 * j);
+                sn = ldg128(p.rope_sin + (size_t)pos * half + 8 * j);
+              }
+              const uint32_t cw[4] = {c.x, c.y, c.z, c.w}, sw[4] = {sn.x, sn.y, sn.z, sn.w};
+#pragma unroll
+              for (int e = 0; e < 4; ++e) {
+                const float2 cc = unpack_bf16(cw[e]), ss = unpack_bf16(sw[e]);
+                cf[8 * j + 2 * e] = cc.x; cf[8 * j + 2 * e + 1] = cc.y;
+                sf[8 * j + 2 * e] = ss.x; sf[8 * j + 2 * e + 1] = ss.y;
+              }
+            }
+          }
+          auto rotate = [&](float (&a)[32], auto h_c) {
+            constexpr int H = decltype(h_c)::value;
+#pragma unroll
+            for (int i = 0; i < H; ++i) {
+              const float x1 = bf16_round(a[i]), x2 = bf16_round(a[i + H]);   // bf16 projection output
+              a[i] = bf16_round(x1 * cf[i]) + bf16_round(-x2 * sf[i]);
+              a[i + H] = bf16_round(x2 * cf[i]) + bf16_round(x1 * sf[i]);
+            }
+          };
+#pragma unroll 1
+          for (int c2 = chalf * (BN / 64 / CS); c2 < (chalf + 1) * (BN / 64 / CS); ++c2) {
+            const int col64 = n0 + c2 * 64;
+            if (col64 >= p.N) break;
+            uint32_t r0[32], r1[32], pk[32];
+            acc_ld(taddr + c2 * 64, r0);
+            acc_ld(taddr + c2 * 64 + 32, r1);
+            float a[32], b[32];
+#pragma unroll
+            for (int i = 0; i < 32; ++i) {
+              a[i] = __uint_as_float(r0[i]);
+              b[i] = __uint_as_float(r1[i]);
+            }
+            if (p.bias) {
+#pragma unroll
+              for (int g = 0; g < 4; ++g) {
+                const uint4 b0 = ldg128(reinterpret_cast<const bf16*>(p.bias) + col64 + g * 8);
+                const uint4 b1 = ldg128(reinterpret_cast<const bf16*>(p.bias) + col64 + 32 + g * 8);
+                const uint32_t w0[4] = {b0.x, b0.y, b0.z, b0.w}, w1[4] = {b1.x, b1.y, b1.z, b1.w};
+#pragma unroll
+                for (int e = 0; e < 4; ++e) {
+                  const float2 f0 = unpack_bf16(w0[e]), f1 = unpack_bf16(w1[e]);
+                  a[g * 8 + 2 * e] += f0.x; a[g * 8 + 2 * e + 1] += f0.y;
+                  b[g * 8 + 2 * e] += f1.x; b[g * 8 + 2 * e + 1] += f1.y;
+                }
+              }
+            }
+            if (col64 < p.rope_cols) {
+              if (half == 16) rotate(a, std::integral_constant<int, 16>{});
+              else            rotate(a, std::integral_constant<int, 8>{});
+            }
+#pragma unroll
+            for (int t = 0; t < 16; ++t) {
+              pk[t] = pack_bf16(a[2 * t], a[2 * t + 1]);
+              pk[16 + t] = pack_bf16(b[2 * t], b[2 * t + 1]);
+            }
+            stage_store(&tmC, pk, col64, std::false_type{});
+          }
+        } else if (!SK && p.tma_store && p.epi == 4) {
+          // ---- GELU forward (GPT-NeoX dense_h_to_4h): pre = bf16(acc + bias) -> C, bf16(gelu(pre)) -> aux_out ----
+#pragma unroll 1
+          for (int c2 = chalf * (BN / 64 / CS); c2 < (chalf + 1) * (BN / 64 / CS); ++c2) {
+            const int col64 = n0 + c2 * 64;
+            if (col64 >= p.N) break;
+            uint32_t r0[32], r1[32], pk[32];
+            acc_ld(taddr + c2 * 64, r0);
+            acc_ld(taddr + c2 * 64 + 32, r1);
+#pragma unroll
+            for (int g = 0; g < 8; ++g) {
+              const uint32_t* r = g < 4 ? r0 + 8 * g : r1 + 8 * (g - 4);
+              float v[8];
+#pragma unroll
+              for (int i = 0; i < 8; ++i) v[i] = __uint_as_float(r[i]);
+              epi_bias_act(v, p, col64 + 8 * g);
+#pragma unroll
+              for (int e = 0; e < 4; ++e) pk[4 * g + e] = pack_bf16(v[2 * e], v[2 * e + 1]);
+            }
+            stage_store(&tmC, pk, col64, std::false_type{});
+#pragma unroll
+            for (int t = 0; t < 32; ++t) {
+              const float2 f = unpack_bf16(pk[t]);
+              pk[t] = pack_bf16(gelu_exact(f.x), gelu_exact(f.y));
+            }
+            stage_store(&tmAux, pk, col64, std::false_type{});
+          }
+        } else if (!SK && p.tma_store && p.epi == 5) {
+          // ---- GELU backward (input gradient of dense_4h_to_h): d_pre = bf16(bf16(d_act) * gelu'(pre)) ----
+#pragma unroll 1
+          for (int c2 = chalf * (BN / 64 / CS); c2 < (chalf + 1) * (BN / 64 / CS); ++c2) {
+            const int col64 = n0 + c2 * 64;
+            if (col64 >= p.N) break;
+            uint4 pv[8];
+#pragma unroll
+            for (int j = 0; j < 8; ++j)
+              pv[j] = row_ok ? ldg128(p.aux + row * p.ld_aux + col64 + 8 * j) : make_uint4(0u, 0u, 0u, 0u);
+            uint32_t r0[32], r1[32], pk[32];
+            acc_ld(taddr + c2 * 64, r0);
+            acc_ld(taddr + c2 * 64 + 32, r1);
+#pragma unroll
+            for (int j = 0; j < 8; ++j) {
+              const uint32_t* r = j < 4 ? r0 + 8 * j : r1 + 8 * (j - 4);
+              const uint32_t pw[4] = {pv[j].x, pv[j].y, pv[j].z, pv[j].w};
+#pragma unroll
+              for (int e = 0; e < 4; ++e) {
+                const float2 x = unpack_bf16(pw[e]);
+                const float2 d = unpack_bf16(pack_bf16(__uint_as_float(r[2 * e]), __uint_as_float(r[2 * e + 1])));
+                pk[4 * j + e] = pack_bf16(d.x * gelu_exact_grad(x.x), d.y * gelu_exact_grad(x.y));
+              }
+            }
+            stage_store(&tmC, pk, col64, std::false_type{});
+          }
         } else if (!SK && p.tma_store && p.epi == 3) {
           // ---- bias + RoPE: a 64-column chunk is one attention head; element i pairs with element i + 32 ----
           uint32_t cw[16], sw[16];
@@ -827,7 +975,7 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
             }
             stage_store(&tmC, pk, n0 + c2 * 64, tail_c);
           });
-        } else if (p.tma_store && !p.bias && !p.act && p.residual && !p.residual_lo) {
+        } else if (p.tma_store && !p.bias && !p.act && p.residual && !p.residual_lo && p.epi == 0) {
           // residual add only (o-proj and down-proj forward: x + linear(..), rounded like the unfused bf16 graph): the
           // row's 128 residual bytes are requested before the accumulator is read; straight-line
           for_chunks([&](auto tail_c, int c2) {
@@ -1180,7 +1328,9 @@ int plan_gemm(const SkGemmEx& g, GemmParams& p, int& BN, int& ew, int& grid) {
   // the SwiGLU epilogues need both halves of a [128 gate | 128 up] block in one tile.  The 192 / 224 widths are for
   // plain one-pass 2-D problems; the auto planner leaves them to GEMMs without stream-K scratch (forward and dgrad):
   // with scratch, split-K / stream-K balance the last wave at the widths they were tuned for
-  const bool fit = g.passes == 1 && g.batch == 1 && !use3d && g.a_mode == 0 && g.epi != 1 && g.epi != 2;
+  // (the GELU epilogues 4 / 5 also stay on whole 64-column chunks: epi 4's second output leaves through tmAux)
+  const bool fit = g.passes == 1 && g.batch == 1 && !use3d && g.a_mode == 0 && g.epi != 1 && g.epi != 2 && g.epi != 4 &&
+                   g.epi != 5;
   SK_REQUIRE((g.force_bn != 192 && g.force_bn != 224) || (fit && !(g.force_bn == 224 && g.epi == 3)),
              "gemm: force_bn=%d needs a one-pass 2-D problem (and whole 64-column heads for RoPE)", g.force_bn);
   BN = (g.a_mode == 1) ? 64
@@ -1211,6 +1361,7 @@ int plan_gemm(const SkGemmEx& g, GemmParams& p, int& BN, int& ew, int& grid) {
   static const int splitk_env = [] { const char* e = getenv("SK_SPLITK"); return e ? atoi(e) : 1; }();
   static const int sk_ranges = [] { const char* e = getenv("SK_STREAMK_RANGES"); return e ? atoi(e) : 4; }();
   if (splitk_env && g.splitk_ws && g.batch == 1 && g.passes == 1 && !g.out_f32 && !g.bias && !g.act && !g.C_lo && g.col_gin == 0 &&
+      g.epi == 0 &&
       (g.residual == nullptr || g.residual == g.C) && tiles * 2 <= nsm && num_kb >= 16) {
     int sp = (int)(nsm / tiles);
     if (sp > 8) sp = 8;
@@ -1235,7 +1386,15 @@ int plan_gemm(const SkGemmEx& g, GemmParams& p, int& BN, int& ew, int& grid) {
   p.rope_sin = reinterpret_cast<const bf16*>(g.rope_sin);
   p.rope_pos = g.rope_pos;
   p.rope_T = g.rope_T; p.rope_cols = g.rope_cols; p.rope_maxpos = g.rope_maxpos;
-  if (g.epi != 0) {
+  p.rope_rot = g.rope_rot == 0 ? 64 : g.rope_rot;
+  if (g.epi == 6) {
+    // two residuals: runs on every output path (epi_residual), stream-K included; split-K is not planned for it
+    SK_REQUIRE(g.passes == 1 && g.batch == 1 && !use3d && g.residual && g.aux && !g.residual_lo && !g.act && !g.out_f32 &&
+                   !g.C_lo && g.col_gin == 0 && g.round_before_res && g.ld_aux >= g.N && g.ld_aux % 8 == 0 &&
+                   (reinterpret_cast<uintptr_t>(g.aux) & 15) == 0,
+               "gemm: two-residual epilogue needs a plain one-pass bf16 GEMM, both residuals (16-byte aligned, pitch >= N) and "
+               "round_before_res");
+  } else if (g.epi != 0) {
     SK_REQUIRE(p.tma_store && g.passes == 1 && !g.residual && !g.act && g.splitk_ws == nullptr,
                "gemm: fused epilogue %d needs the plain bf16 TMA-store path (no residual / activation / scratch)", g.epi);
     if (g.epi == 1) {
@@ -1248,6 +1407,16 @@ int plan_gemm(const SkGemmEx& g, GemmParams& p, int& BN, int& ew, int& grid) {
       SK_REQUIRE(g.rope_cos && g.rope_sin && g.rope_T > 0 && g.rope_maxpos > 0 && g.rope_cols % 64 == 0 && g.N % 64 == 0 &&
                      !g.bias_f32,
                  "gemm: RoPE epilogue needs cos/sin tables, 64-column heads and a bf16 bias");
+      SK_REQUIRE(p.rope_rot == 16 || p.rope_rot == 32 || p.rope_rot == 64,
+                 "gemm: RoPE epilogue rotary width rope_rot=%d is not supported (16, 32 or 64)", g.rope_rot);
+    } else if (g.epi == 4) {
+      SK_REQUIRE(BN % 64 == 0 && g.N % 64 == 0 && g.aux_out && g.ld_aux_out >= g.N && g.ld_aux_out % 8 == 0 && !g.bias_f32 &&
+                     (reinterpret_cast<uintptr_t>(g.aux_out) & 15) == 0,
+                 "gemm: GELU-forward epilogue needs N %% 64 == 0, an act output (pitch >= N) and a bf16 bias");
+    } else if (g.epi == 5) {
+      SK_REQUIRE(BN % 64 == 0 && g.N % 64 == 0 && g.aux && g.ld_aux >= g.N && g.ld_aux % 8 == 0 && !g.bias &&
+                     (reinterpret_cast<uintptr_t>(g.aux) & 15) == 0,
+                 "gemm: GELU-backward epilogue needs N %% 64 == 0, the saved pre-activation (pitch >= N) and no bias");
     } else {
       SK_REQUIRE(false, "gemm: unknown fused epilogue %d", g.epi);
     }
@@ -1290,7 +1459,7 @@ int plan_gemm(const SkGemmEx& g, GemmParams& p, int& BN, int& ew, int& grid) {
   // 8 epilogue warps (two per 32-row quadrant) where the epilogue does real work per element; the plain
   // convert-and-store epilogue is faster with 4 (fewer warps contending with the TMA / MMA issue threads)
   static const int ew_env = [] { const char* e = getenv("SK_GEMM_EW"); return e ? atoi(e) : 0; }();
-  ew = (p.sk_units == 0 && BN == 256 && p.tma_store && (ew_env == 8 || (ew_env == 0 && (g.epi == 2 || g.epi == 3)))) ? 8 : 4;
+  ew = (p.sk_units == 0 && BN == 256 && p.tma_store && (ew_env == 8 || (ew_env == 0 && (g.epi == 2 || g.epi == 3 || g.epi == 4 || g.epi == 5)))) ? 8 : 4;
   return 0;
 }
 
@@ -1349,6 +1518,9 @@ int sk_gemm_ex_launch(const SkGemmEx& g, cudaStream_t stream) {
   tm[5] = tm[4];
   if (g.epi == 1) {
     const int rc3 = sk_make_tmap_2d(&tm[5], g.aux_out, 2, (uint64_t)g.N / 2, (uint64_t)g.M, (uint64_t)g.ld_aux_out, 64, 32);
+    if (rc3) return rc3;
+  } else if (g.epi == 4) {   // the GELU output, same shape as C
+    const int rc3 = sk_make_tmap_2d(&tm[5], g.aux_out, 2, (uint64_t)g.N, (uint64_t)g.M, (uint64_t)g.ld_aux_out, 64, 32);
     if (rc3) return rc3;
   } else if (p.tma_store && BN % 64 != 0) {   // the 32-column tail chunk of a 224-wide tile
     const int rc3 = sk_make_tmap_2d(&tm[5], g.C, 2, (uint64_t)g.N, (uint64_t)g.M, (uint64_t)g.ldc, 32, 32);
@@ -1438,7 +1610,8 @@ int sk_linear_swiglu_bwd_launch(int M, int N, int F, const void* dy, const void*
 // out[M,N] = x[M,K] * W[N,K]^T + bias, 64-column heads below rope_cols rotated in the epilogue (HF apply_rotary_pos_emb,
 // HF:models/qwen2/modeling_qwen2.py:102-146)
 int sk_linear_rope_launch(int M, int N, int K, const void* x, const void* W, const void* bias, void* out, const void* cos_t,
-                          const void* sin_t, const int32_t* pos_ids, int T, int rope_cols, int max_positions, cudaStream_t s) {
+                          const void* sin_t, const int32_t* pos_ids, int T, int rope_cols, int max_positions, cudaStream_t s,
+                          int rope_rot) {
   SkGemmEx g;
   memset(&g, 0, sizeof(g));
   g.M = M; g.N = N; g.K = K; g.batch = 1; g.passes = 1;
@@ -1446,7 +1619,39 @@ int sk_linear_rope_launch(int M, int N, int K, const void* x, const void* W, con
   g.C = out; g.ldc = N;
   g.bias = bias;
   g.epi = 3; g.rope_cos = cos_t; g.rope_sin = sin_t; g.rope_pos = pos_ids; g.rope_T = T;
-  g.rope_cols = rope_cols; g.rope_maxpos = max_positions;
+  g.rope_cols = rope_cols; g.rope_maxpos = max_positions; g.rope_rot = rope_rot;
   g.pdl = 1;
+  return sk_gemm_ex_launch(g, s);
+}
+// GPT-NeoX MLP (HF GPTNeoXMLP): pre[M,F] = bf16(x W1^T + b1) and act = bf16(gelu(pre)) from one epilogue
+int sk_linear_gelu_fwd_launch(int M, int F, int K, const void* x, const void* W1, const void* b1, void* pre, void* act,
+                              cudaStream_t s) {
+  SkGemmEx g;
+  memset(&g, 0, sizeof(g));
+  g.M = M; g.N = F; g.K = K; g.batch = 1; g.passes = 1;
+  g.A = x; g.lda = K; g.B = W1; g.ldb = K;
+  g.C = pre; g.ldc = F;
+  g.bias = b1;
+  g.epi = 4; g.aux_out = act; g.ld_aux_out = F;
+  g.pdl = 1;
+  return sk_gemm_ex_launch(g, s);
+}
+// d_pre[M,F] = bf16(bf16(dy W2) * gelu'(pre)): d_act never reaches memory
+int sk_linear_gelu_bwd_launch(int M, int N, int F, const void* dy, const void* W2, const void* pre, void* dpre, cudaStream_t s) {
+  SkGemmEx g;
+  memset(&g, 0, sizeof(g));
+  g.M = M; g.N = F; g.K = N; g.batch = 1; g.passes = 1;
+  g.A = dy; g.lda = N; g.B = W2; g.ldb = F; g.b_mn = 1;
+  g.C = dpre; g.ldc = F;
+  g.epi = 5; g.aux = pre; g.ld_aux = F;
+  g.pdl = 1;
+  return sk_gemm_ex_launch(g, s);
+}
+// out[M,N] = bf16(bf16(bf16(x W^T + bias) + res2) + res): GPT-NeoX's `mlp_output + attn_output + hidden_states`, rounded
+// at each add in that order.  out may alias res (each element reads its residuals before it is stored).
+int sk_linear_res2_launch(int M, int N, int K, const void* x, const void* W, const void* bias, const void* res2, const void* res,
+                          void* out, cudaStream_t s, void* splitk_ws, size_t splitk_ws_bytes) {
+  SkGemmEx g = sk_gemm_desc(M, N, K, x, K, 0, W, K, 0, out, N, 0, bias, res, N, 1, 0, 0, splitk_ws, splitk_ws_bytes);
+  g.epi = 6; g.aux = res2; g.ld_aux = N;
   return sk_gemm_ex_launch(g, s);
 }

@@ -38,7 +38,11 @@ struct SkGemmEx {
   //                      layout) and aux_out = act [M,F] = bf16(bf16(silu(gate)) * up)
   //   2 SwiGLU backward: N = F, acc = d_act; aux = gu [M,2F]; C = d_gu [M,2F] (ldc = its pitch)
   //   3 bias + RoPE    : 64-column heads with column < rope_cols are rotated with cos/sin[pos] (pos = rope_pos[row] or
-  //                      row % rope_T, clamped to [0, rope_maxpos))
+  //                      row % rope_T, clamped to [0, rope_maxpos)); the first rope_rot columns of each head rotate
+  //                      (0 or 64: the whole head, tables [maxpos, 32]; 16 / 32: partial rotary, tables [maxpos, rope_rot/2])
+  //   4 GELU forward   : C = pre = bf16(acc + bias) and aux_out = bf16(gelu_erf(pre)) (same shape, ld_aux_out)
+  //   5 GELU backward  : acc = d_act; aux = the saved pre; C = bf16(bf16(acc) * gelu'(pre))
+  //   6 two residuals  : C = bf16(bf16(bf16(acc + bias) + aux) + residual) (GPT-NeoX parallel residual: mlp + attn + x)
   int epi;
   const void* aux;
   int ld_aux;
@@ -47,6 +51,7 @@ struct SkGemmEx {
   const void *rope_cos, *rope_sin;
   const int* rope_pos;
   int rope_T, rope_cols, rope_maxpos;
+  int rope_rot;
 };
 int sk_gemm_ex_launch(const SkGemmEx& g, cudaStream_t stream);
 struct SkGemmPlan;
@@ -61,7 +66,15 @@ SkGemmEx sk_gemm_desc(int M, int N, int K, const void* A, int lda, int a_mn, con
 int sk_linear_swiglu_fwd_launch(int M, int F, int K, const void* x, const void* Wgu, void* gu, void* act, cudaStream_t s);
 int sk_linear_swiglu_bwd_launch(int M, int N, int F, const void* dy, const void* Wd, const void* gu, void* dgu, cudaStream_t s);
 int sk_linear_rope_launch(int M, int N, int K, const void* x, const void* W, const void* bias, void* out, const void* cos_t,
-                          const void* sin_t, const int32_t* pos_ids, int T, int rope_cols, int max_positions, cudaStream_t s);
+                          const void* sin_t, const int32_t* pos_ids, int T, int rope_cols, int max_positions, cudaStream_t s,
+                          int rope_rot = 0);
+// GPT-NeoX MLP: pre[M,F] = x * W1^T + b1 and act = bf16(gelu(pre)) in one epilogue; d_pre[M,F] from d_act = dy * W2
+// without materialising d_act; out = bf16(bf16(bf16(x * W^T + b) + res2) + res) (mlp + attn + x)
+int sk_linear_gelu_fwd_launch(int M, int F, int K, const void* x, const void* W1, const void* b1, void* pre, void* act,
+                              cudaStream_t s);
+int sk_linear_gelu_bwd_launch(int M, int N, int F, const void* dy, const void* W2, const void* pre, void* dpre, cudaStream_t s);
+int sk_linear_res2_launch(int M, int N, int K, const void* x, const void* W, const void* bias, const void* res2, const void* res,
+                          void* out, cudaStream_t s, void* splitk_ws = nullptr, size_t splitk_ws_bytes = 0);
 
 // lm_kernels.cu
 int sk_embed_fwd_launch(const int64_t* ids, const bf16* E, bf16* out, int M, int D, int V, cudaStream_t s);
@@ -73,8 +86,9 @@ int sk_rmsnorm_bwd_launch(const bf16* dy, const bf16* x, const bf16* w, const fl
                           bf16* dw, float* dw_partial, int M, int D, int accumulate_dw, cudaStream_t s);
 extern "C" int sk_colsum_splits(void);
 int sk_colsum_launch(const bf16* x, bf16* out, float* partial, int M, int N, int ld, int accumulate, cudaStream_t s);
+// rot_dims: rotated columns per head (0 = head_dim; 16 / 32 for head_dim 64: partial rotary, tables [max_pos, rot_dims/2])
 int sk_rope_launch(bf16* qkv, const bf16* cos_t, const bf16* sin_t, const int* pos_ids, int M, int T, int ld,
-                   int n_rot_heads, int head_dim, int inverse, int max_positions, cudaStream_t s);
+                   int n_rot_heads, int head_dim, int inverse, int max_positions, cudaStream_t s, int rot_dims = 0);
 int sk_swiglu_fwd_launch(const bf16* gu, bf16* act, int M, int F, cudaStream_t s);
 int sk_swiglu_bwd_launch(const bf16* gu, const bf16* dact, bf16* dgu, int M, int F, cudaStream_t s);
 extern "C" int sk_ce_blocks(int M);
@@ -104,6 +118,14 @@ int sk_opt_embed_fwd_launch(const int64_t* ids, const int32_t* pos_ids, const bf
 int sk_opt_pos_bwd_launch(const int32_t* pos_ids, const bf16* dx, float* scratch, bf16* dP, int M, int T, int D, int n_pos,
                           int accumulate, cudaStream_t s);
 int sk_relu_bwd_launch(bf16* g, const bf16* a, long n, cudaStream_t s);
+// GPT-NeoX parallel residual: ln1(x) and ln2(x) from one read of x (shared fp32 mean / rstd), and the fused backward
+// dx = dres + LN'(w1 * dy1 + w2 * dy2) with the four deterministic parameter gradients (partial: 4 x
+// sk_layernorm_bwd_blocks() x D floats)
+int sk_layernorm2_fwd_launch(const bf16* x, const bf16* w1, const bf16* b1, const bf16* w2, const bf16* b2, bf16* y1, bf16* y2,
+                             float* mean, float* rstd, int M, int D, float eps, cudaStream_t s);
+int sk_layernorm2_bwd_launch(const bf16* dy1, const bf16* dy2, const bf16* x, const bf16* w1, const bf16* w2, const float* mean,
+                             const float* rstd, const bf16* dres, bf16* dx, bf16* dw1, bf16* db1, bf16* dw2, bf16* db2,
+                             float* partial, int M, int D, int accumulate, cudaStream_t s);
 
 // attention.cu
 int sk_attn_fwd_launch(const bf16* q, const bf16* k, const bf16* v, bf16* o, float* lse, int B, int T, int H, int KVH,

@@ -286,15 +286,16 @@ __global__ void colsum_partial_kernel(const bf16* __restrict__ x, float* __restr
 // RoPE (rotate_half form), in place on the q and k head slices of the fused qkv activation [M, ld].
 //   out[i]      = bf16(bf16(x[i]*c) + bf16(-x[i+hd/2]*s))
 //   out[i+hd/2] = bf16(bf16(x[i+hd/2]*c) + bf16(x[i]*s))          c,s: bf16 tables [maxpos, hd/2]
-// inverse=1 applies the transposed rotation (backward).
+// inverse=1 applies the transposed rotation (backward).  rot < head_dim (GPT-NeoX partial rotary): only the first rot
+// columns of each head rotate, pairing i with i + rot/2, with [maxpos, rot/2] tables; the other columns are untouched.
 // ------------------------------------------------------------------------------------------------
 __global__ void rope_kernel(bf16* __restrict__ qkv, const bf16* __restrict__ cos_t, const bf16* __restrict__ sin_t,
                             const int* __restrict__ pos_ids, int M, int T, int ld, int n_rot_heads, int head_dim,
-                            int inverse, int max_pos) {
+                            int inverse, int max_pos, int rot) {
   griddep_launch();
   griddep_wait();
-  const int half = head_dim / 2;          // 32
-  const int vec_per_head = half / 8;      // 4 threads per (token, head)
+  const int half = rot / 2;               // 32 (full rotary) / 16 / 8
+  const int vec_per_head = half / 8;      // 4 / 2 / 1 threads per (token, head)
   const long total = (long)M * n_rot_heads * vec_per_head;
   for (long i = blockIdx.x * (long)blockDim.x + threadIdx.x; i < total; i += (long)gridDim.x * blockDim.x) {
     const int v = (int)(i % vec_per_head);
@@ -844,11 +845,14 @@ int sk_colsum_launch(const bf16* x, bf16* out, float* partial, int M, int N, int
   return 0;
 }
 int sk_rope_launch(bf16* qkv, const bf16* cos_t, const bf16* sin_t, const int* pos_ids, int M, int T, int ld,
-                   int n_rot_heads, int head_dim, int inverse, int max_positions, cudaStream_t s) {
+                   int n_rot_heads, int head_dim, int inverse, int max_positions, cudaStream_t s, int rot_dims) {
   SK_REQUIRE(head_dim % 16 == 0 && ld % 8 == 0, "rope: head_dim must be a multiple of 16");
   SK_REQUIRE(max_positions > 0 && (pos_ids != nullptr || T <= max_positions), "rope: table rows (%d) do not cover T=%d", max_positions, T);
-  SK_CUDA_CHECK(sk_launch_pdl(rope_kernel, dim3(grid_for((long)M * n_rot_heads * (head_dim / 16), 256)), dim3(256), (size_t)(0), s, qkv, cos_t, sin_t, pos_ids, M, T, ld,
-                                                                                   n_rot_heads, head_dim, inverse, max_positions));
+  const int rot = rot_dims > 0 ? rot_dims : head_dim;
+  SK_REQUIRE(rot == head_dim || (head_dim == 64 && (rot == 16 || rot == 32)),
+             "rope: rotary width %d not supported (16, 32 or the head_dim %d)", rot, head_dim);
+  SK_CUDA_CHECK(sk_launch_pdl(rope_kernel, dim3(grid_for((long)M * n_rot_heads * (rot / 16), 256)), dim3(256), (size_t)(0), s, qkv, cos_t, sin_t, pos_ids, M, T, ld,
+                                                                                   n_rot_heads, head_dim, inverse, max_positions, rot));
   SK_LAUNCH_CHECK();
   return 0;
 }
@@ -947,10 +951,13 @@ constexpr int LN_BWD_WARPS = 4;
 
 // LayerNorm forward, one warp per row: y = bf16((x - mean) * rstd * g + b) in fp32 (nn.LayerNorm on a bf16 input, and
 // its autocast form that runs in fp32 and feeds the next linear a bf16 copy, both round once).  The row stays in
-// registers between the mean pass, the variance pass and the output pass.
-template <int MAXV>
+// registers between the mean pass, the variance pass and the output pass.  NOUT = 2 (GPT-NeoX's parallel residual,
+// HF:models/gpt_neox/modeling_gpt_neox.py use_parallel_residual) also writes y2 = LN(x; w2, b2) from the same registers
+// and statistics: each output is the NOUT = 1 value by construction.
+template <int MAXV, int NOUT = 1>
 __global__ void __launch_bounds__(WARPS_PER_BLOCK * 32)
 layernorm_fwd_kernel(const bf16* __restrict__ x, const bf16* __restrict__ w, const bf16* __restrict__ b, bf16* __restrict__ y,
+                     const bf16* __restrict__ w2, const bf16* __restrict__ b2, bf16* __restrict__ y2,
                      float* __restrict__ mean_out, float* __restrict__ rstd_out, int M, int D, float eps) {
   griddep_launch();
   griddep_wait();
@@ -996,16 +1003,19 @@ layernorm_fwd_kernel(const bf16* __restrict__ x, const bf16* __restrict__ w, con
   for (int j = 0; j < MAXV; ++j) {
     const int c = lane + 32 * j;
     if (c < nvec) {
-      const uint4 wv = ldg128(w + c * 8), bv = ldg128(b + c * 8);
       const uint32_t u[4] = {xv[j].x, xv[j].y, xv[j].z, xv[j].w};
-      const uint32_t wu[4] = {wv.x, wv.y, wv.z, wv.w}, bu[4] = {bv.x, bv.y, bv.z, bv.w};
-      uint32_t o[4];
 #pragma unroll
-      for (int k = 0; k < 4; ++k) {
-        const float2 f = unpack_bf16(u[k]), g = unpack_bf16(wu[k]), bb = unpack_bf16(bu[k]);
-        o[k] = pack_bf16(fmaf((f.x - mean) * rstd, g.x, bb.x), fmaf((f.y - mean) * rstd, g.y, bb.y));
+      for (int t = 0; t < NOUT; ++t) {
+        const uint4 wv = ldg128((t ? w2 : w) + c * 8), bv = ldg128((t ? b2 : b) + c * 8);
+        const uint32_t wu[4] = {wv.x, wv.y, wv.z, wv.w}, bu[4] = {bv.x, bv.y, bv.z, bv.w};
+        uint32_t o[4];
+#pragma unroll
+        for (int k = 0; k < 4; ++k) {
+          const float2 f = unpack_bf16(u[k]), g = unpack_bf16(wu[k]), bb = unpack_bf16(bu[k]);
+          o[k] = pack_bf16(fmaf((f.x - mean) * rstd, g.x, bb.x), fmaf((f.y - mean) * rstd, g.y, bb.y));
+        }
+        stg128((t ? y2 : y) + (size_t)row * D + c * 8, make_uint4(o[0], o[1], o[2], o[3]));
       }
-      stg128(y + (size_t)row * D + c * 8, make_uint4(o[0], o[1], o[2], o[3]));
     }
   }
 }
@@ -1015,53 +1025,80 @@ layernorm_fwd_kernel(const bf16* __restrict__ x, const bf16* __restrict__ w, con
 //   dw (+)= sum_rows dy * xhat ; db (+)= sum_rows dy
 // Each warp adds its rows' dw / db terms into its own shared-memory slab (a lane owns its columns: no conflicts); the
 // block writes one partial row per block, and colsum_reduce_kernel sums the partials in a fixed order (deterministic).
-template <int MAXV>
+// NIN = 2 is the backward of the two LayerNorms of one x (GPT-NeoX's parallel residual): the input gradient is linear in
+// g, so one pass takes g = dy * w + dy2 * w2 in fp32, and dw2 / db2 get their own slabs and partial rows.
+template <int MAXV, int NIN = 1>
 __global__ void __launch_bounds__(LN_BWD_WARPS * 32)
-layernorm_bwd_kernel(const bf16* __restrict__ dy, const bf16* __restrict__ x, const bf16* __restrict__ w,
-                     const float* __restrict__ mean_in, const float* __restrict__ rstd_in, const bf16* __restrict__ dres,
-                     bf16* __restrict__ dx, float* __restrict__ dw_partial, float* __restrict__ db_partial, int M, int D) {
+layernorm_bwd_kernel(const bf16* __restrict__ dy, const bf16* __restrict__ dy2, const bf16* __restrict__ x,
+                     const bf16* __restrict__ w, const bf16* __restrict__ w2, const float* __restrict__ mean_in,
+                     const float* __restrict__ rstd_in, const bf16* __restrict__ dres, bf16* __restrict__ dx,
+                     float* __restrict__ dw_partial, float* __restrict__ db_partial, float* __restrict__ dw2_partial,
+                     float* __restrict__ db2_partial, int M, int D) {
   griddep_launch();
   griddep_wait();
-  extern __shared__ float sacc[];   // [2][LN_BWD_WARPS][D]: dw then db
+  extern __shared__ float sacc[];   // [2 * NIN][LN_BWD_WARPS][D]: dw, db (then dw2, db2)
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int nvec = D / 8;
-  float* sdw = sacc + (size_t)warp * D;
-  float* sdb = sacc + (size_t)(LN_BWD_WARPS + warp) * D;
+  float* sl[2 * NIN];
+#pragma unroll
+  for (int t = 0; t < 2 * NIN; ++t) sl[t] = sacc + ((size_t)t * LN_BWD_WARPS + warp) * D;
   for (int c = lane; c < nvec; c += 32)
 #pragma unroll
-    for (int k = 0; k < 8; ++k) { sdw[c * 8 + k] = 0.f; sdb[c * 8 + k] = 0.f; }
+    for (int k = 0; k < 8; ++k)
+#pragma unroll
+      for (int t = 0; t < 2 * NIN; ++t) sl[t][c * 8 + k] = 0.f;
   for (int row = blockIdx.x * LN_BWD_WARPS + warp; row < M; row += gridDim.x * LN_BWD_WARPS) {
-    uint4 xq[MAXV], dq[MAXV];
+    uint4 xq[MAXV], dq[MAXV], dq2[MAXV];
 #pragma unroll
     for (int j = 0; j < MAXV; ++j) {
       const int c = lane + 32 * j;
       if (c < nvec) {
         xq[j] = ldg128_stream(x + (size_t)row * D + c * 8);
         dq[j] = ldg128_stream(dy + (size_t)row * D + c * 8);
+        if constexpr (NIN == 2) dq2[j] = ldg128_stream(dy2 + (size_t)row * D + c * 8);
       }
     }
     const float mean = mean_in[row], rstd = rstd_in[row];
+    // g of element pair k of vector j (the only place the two forms differ)
+    auto gpair = [&](int j, int k, const uint4& wv, const uint4& wv2) {
+      const uint32_t du[4] = {dq[j].x, dq[j].y, dq[j].z, dq[j].w}, wu[4] = {wv.x, wv.y, wv.z, wv.w};
+      const float2 df = unpack_bf16(du[k]), wf = unpack_bf16(wu[k]);
+      if constexpr (NIN == 2) {
+        const uint32_t eu[4] = {dq2[j].x, dq2[j].y, dq2[j].z, dq2[j].w}, vu[4] = {wv2.x, wv2.y, wv2.z, wv2.w};
+        const float2 ef = unpack_bf16(eu[k]), vf = unpack_bf16(vu[k]);
+        return make_float2(fmaf(df.x, wf.x, ef.x * vf.x), fmaf(df.y, wf.y, ef.y * vf.y));
+      } else {
+        return make_float2(df.x * wf.x, df.y * wf.y);
+      }
+    };
     float s1 = 0.f, s2 = 0.f;
 #pragma unroll
     for (int j = 0; j < MAXV; ++j) {
       const int c = lane + 32 * j;
       if (c < nvec) {
         const uint4 wv = ldg128(w + c * 8);
+        const uint4 wv2 = NIN == 2 ? ldg128(w2 + c * 8) : wv;
         const uint32_t xu[4] = {xq[j].x, xq[j].y, xq[j].z, xq[j].w}, du[4] = {dq[j].x, dq[j].y, dq[j].z, dq[j].w};
-        const uint32_t wu[4] = {wv.x, wv.y, wv.z, wv.w};
 #pragma unroll
         for (int k = 0; k < 4; ++k) {
-          const float2 xf = unpack_bf16(xu[k]), df = unpack_bf16(du[k]), wf = unpack_bf16(wu[k]);
+          const float2 xf = unpack_bf16(xu[k]), df = unpack_bf16(du[k]);
           const float xh0 = (xf.x - mean) * rstd, xh1 = (xf.y - mean) * rstd;
-          const float g0 = df.x * wf.x, g1 = df.y * wf.y;
-          s1 += g0 + g1;
-          s2 = fmaf(g0, xh0, fmaf(g1, xh1, s2));
-          float* pw = sdw + c * 8 + 2 * k;
-          float* pb = sdb + c * 8 + 2 * k;
-          pw[0] = fmaf(df.x, xh0, pw[0]);
-          pw[1] = fmaf(df.y, xh1, pw[1]);
-          pb[0] += df.x;
-          pb[1] += df.y;
+          const float2 g = gpair(j, k, wv, wv2);
+          s1 += g.x + g.y;
+          s2 = fmaf(g.x, xh0, fmaf(g.y, xh1, s2));
+          const int e = c * 8 + 2 * k;
+          sl[0][e] = fmaf(df.x, xh0, sl[0][e]);
+          sl[0][e + 1] = fmaf(df.y, xh1, sl[0][e + 1]);
+          sl[1][e] += df.x;
+          sl[1][e + 1] += df.y;
+          if constexpr (NIN == 2) {
+            const uint32_t eu[4] = {dq2[j].x, dq2[j].y, dq2[j].z, dq2[j].w};
+            const float2 ef = unpack_bf16(eu[k]);
+            sl[2][e] = fmaf(ef.x, xh0, sl[2][e]);
+            sl[2][e + 1] = fmaf(ef.y, xh1, sl[2][e + 1]);
+            sl[3][e] += ef.x;
+            sl[3][e + 1] += ef.y;
+          }
         }
       }
     }
@@ -1071,15 +1108,16 @@ layernorm_bwd_kernel(const bf16* __restrict__ dy, const bf16* __restrict__ x, co
       const int c = lane + 32 * j;
       if (c < nvec) {
         const uint4 wv = ldg128(w + c * 8);
+        const uint4 wv2 = NIN == 2 ? ldg128(w2 + c * 8) : wv;
         const uint4 rv = dres ? ldg128_stream(dres + (size_t)row * D + c * 8) : make_uint4(0, 0, 0, 0);
-        const uint32_t xu[4] = {xq[j].x, xq[j].y, xq[j].z, xq[j].w}, du[4] = {dq[j].x, dq[j].y, dq[j].z, dq[j].w};
-        const uint32_t wu[4] = {wv.x, wv.y, wv.z, wv.w}, ru[4] = {rv.x, rv.y, rv.z, rv.w};
+        const uint32_t xu[4] = {xq[j].x, xq[j].y, xq[j].z, xq[j].w}, ru[4] = {rv.x, rv.y, rv.z, rv.w};
         uint32_t o[4];
 #pragma unroll
         for (int k = 0; k < 4; ++k) {
-          const float2 xf = unpack_bf16(xu[k]), df = unpack_bf16(du[k]), wf = unpack_bf16(wu[k]), rf = unpack_bf16(ru[k]);
+          const float2 xf = unpack_bf16(xu[k]), rf = unpack_bf16(ru[k]);
           const float xh0 = (xf.x - mean) * rstd, xh1 = (xf.y - mean) * rstd;
-          const float d0 = rstd * (df.x * wf.x - m1 - xh0 * m2), d1 = rstd * (df.y * wf.y - m1 - xh1 * m2);
+          const float2 g = gpair(j, k, wv, wv2);
+          const float d0 = rstd * (g.x - m1 - xh0 * m2), d1 = rstd * (g.y - m1 - xh1 * m2);
           o[k] = pack_bf16(d0 + rf.x, d1 + rf.y);
         }
         stg128(dx + (size_t)row * D + c * 8, make_uint4(o[0], o[1], o[2], o[3]));
@@ -1087,15 +1125,15 @@ layernorm_bwd_kernel(const bf16* __restrict__ dy, const bf16* __restrict__ x, co
     }
   }
   __syncthreads();
+  float* outs[4] = {dw_partial, db_partial, dw2_partial, db2_partial};
   for (int i = threadIdx.x; i < D; i += blockDim.x) {
-    float a = 0.f, bsum = 0.f;
 #pragma unroll
-    for (int wi = 0; wi < LN_BWD_WARPS; ++wi) {
-      a += sacc[(size_t)wi * D + i];
-      bsum += sacc[(size_t)(LN_BWD_WARPS + wi) * D + i];
+    for (int t = 0; t < 2 * NIN; ++t) {
+      float a = 0.f;
+#pragma unroll
+      for (int wi = 0; wi < LN_BWD_WARPS; ++wi) a += sacc[((size_t)t * LN_BWD_WARPS + wi) * D + i];
+      outs[t][(size_t)blockIdx.x * D + i] = a;
     }
-    dw_partial[(size_t)blockIdx.x * D + i] = a;
-    db_partial[(size_t)blockIdx.x * D + i] = bsum;
   }
 }
 
@@ -1173,8 +1211,10 @@ int sk_layernorm_fwd_launch(const bf16* x, const bf16* w, const bf16* b, bf16* y
                             float eps, cudaStream_t s) {
   SK_REQUIRE(D % 8 == 0 && D <= 2048, "layernorm: D must be a multiple of 8 and <= 2048 (D=%d)", D);
   const dim3 grid((M + WARPS_PER_BLOCK - 1) / WARPS_PER_BLOCK), block(WARPS_PER_BLOCK * 32);
-  if (D <= 1024) SK_CUDA_CHECK(sk_launch_pdl(layernorm_fwd_kernel<4>, grid, block, (size_t)0, s, x, w, b, y, mean, rstd, M, D, eps));
-  else           SK_CUDA_CHECK(sk_launch_pdl(layernorm_fwd_kernel<8>, grid, block, (size_t)0, s, x, w, b, y, mean, rstd, M, D, eps));
+  const bf16* none = nullptr;
+  bf16* no_out = nullptr;
+  if (D <= 1024) SK_CUDA_CHECK(sk_launch_pdl(layernorm_fwd_kernel<4>, grid, block, (size_t)0, s, x, w, b, y, none, none, no_out, mean, rstd, M, D, eps));
+  else           SK_CUDA_CHECK(sk_launch_pdl(layernorm_fwd_kernel<8>, grid, block, (size_t)0, s, x, w, b, y, none, none, no_out, mean, rstd, M, D, eps));
   SK_LAUNCH_CHECK();
   return 0;
 }
@@ -1190,12 +1230,14 @@ int sk_layernorm_bwd_launch(const bf16* dy, const bf16* x, const bf16* w, const 
   const size_t smem = (size_t)2 * LN_BWD_WARPS * D * sizeof(float);
   if (smem > 48 * 1024)   // D > 1536
     SK_CUDA_CHECK(cudaFuncSetAttribute(layernorm_bwd_kernel<8>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+  const bf16* none = nullptr;
+  float* no_partial = nullptr;
   if (D <= 1024)
-    SK_CUDA_CHECK(sk_launch_pdl(layernorm_bwd_kernel<4>, dim3(blocks), dim3(LN_BWD_WARPS * 32), smem, s, dy, x, w, mean, rstd, dres, dx,
-                                dw_partial, db_partial, M, D));
+    SK_CUDA_CHECK(sk_launch_pdl(layernorm_bwd_kernel<4>, dim3(blocks), dim3(LN_BWD_WARPS * 32), smem, s, dy, none, x, w, none, mean, rstd,
+                                dres, dx, dw_partial, db_partial, no_partial, no_partial, M, D));
   else
-    SK_CUDA_CHECK(sk_launch_pdl(layernorm_bwd_kernel<8>, dim3(blocks), dim3(LN_BWD_WARPS * 32), smem, s, dy, x, w, mean, rstd, dres, dx,
-                                dw_partial, db_partial, M, D));
+    SK_CUDA_CHECK(sk_launch_pdl(layernorm_bwd_kernel<8>, dim3(blocks), dim3(LN_BWD_WARPS * 32), smem, s, dy, none, x, w, none, mean, rstd,
+                                dres, dx, dw_partial, db_partial, no_partial, no_partial, M, D));
   SK_LAUNCH_CHECK();
   SK_CUDA_CHECK(sk_launch_pdl(colsum_reduce_kernel, dim3((D + 31) / 32), dim3(1024), (size_t)0, s, (const float*)dw_partial, dw, blocks, D, accumulate));
   SK_LAUNCH_CHECK();
@@ -1221,6 +1263,46 @@ int sk_opt_pos_bwd_launch(const int32_t* pos_ids, const bf16* dx, float* scratch
   SK_REQUIRE(n % 8 == 0, "opt positions: table size must be a multiple of 8");
   add_fix_into_bf16_kernel<<<grid_for(n / 8, 256), 256, 0, s>>>(dP, fix, n, accumulate);
   SK_LAUNCH_CHECK();
+  return 0;
+}
+int sk_layernorm2_fwd_launch(const bf16* x, const bf16* w1, const bf16* b1, const bf16* w2, const bf16* b2, bf16* y1, bf16* y2,
+                             float* mean, float* rstd, int M, int D, float eps, cudaStream_t s) {
+  SK_REQUIRE(D % 8 == 0 && D <= 2048, "layernorm2: D must be a multiple of 8 and <= 2048 (D=%d)", D);
+  const dim3 grid((M + WARPS_PER_BLOCK - 1) / WARPS_PER_BLOCK), block(WARPS_PER_BLOCK * 32);
+  if (D <= 1024) SK_CUDA_CHECK(sk_launch_pdl(layernorm_fwd_kernel<4, 2>, grid, block, (size_t)0, s, x, w1, b1, y1, w2, b2, y2, mean, rstd, M, D, eps));
+  else           SK_CUDA_CHECK(sk_launch_pdl(layernorm_fwd_kernel<8, 2>, grid, block, (size_t)0, s, x, w1, b1, y1, w2, b2, y2, mean, rstd, M, D, eps));
+  SK_LAUNCH_CHECK();
+  return 0;
+}
+// partial must hold 4 * sk_layernorm_bwd_blocks() * D floats
+int sk_layernorm2_bwd_launch(const bf16* dy1, const bf16* dy2, const bf16* x, const bf16* w1, const bf16* w2, const float* mean,
+                             const float* rstd, const bf16* dres, bf16* dx, bf16* dw1, bf16* db1, bf16* dw2, bf16* db2,
+                             float* partial, int M, int D, int accumulate, cudaStream_t s) {
+  SK_REQUIRE(D % 8 == 0 && D <= 2048, "layernorm2: D must be a multiple of 8 and <= 2048 (D=%d)", D);
+  SK_REQUIRE(M > 0, "layernorm2: M must be positive");
+  int blocks = sk_layernorm_bwd_blocks();
+  const int need = (M + LN_BWD_WARPS - 1) / LN_BWD_WARPS;
+  if (blocks > need) blocks = need;
+  const size_t smem = (size_t)4 * LN_BWD_WARPS * D * sizeof(float);
+  float* pt[4];
+  for (int t = 0; t < 4; ++t) pt[t] = partial + (size_t)t * blocks * D;
+  if (D <= 1024) {
+    if (smem > 48 * 1024)
+      SK_CUDA_CHECK(cudaFuncSetAttribute(layernorm_bwd_kernel<4, 2>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    SK_CUDA_CHECK(sk_launch_pdl(layernorm_bwd_kernel<4, 2>, dim3(blocks), dim3(LN_BWD_WARPS * 32), smem, s, dy1, dy2, x, w1, w2, mean,
+                                rstd, dres, dx, pt[0], pt[1], pt[2], pt[3], M, D));
+  } else {
+    SK_CUDA_CHECK(cudaFuncSetAttribute(layernorm_bwd_kernel<8, 2>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    SK_CUDA_CHECK(sk_launch_pdl(layernorm_bwd_kernel<8, 2>, dim3(blocks), dim3(LN_BWD_WARPS * 32), smem, s, dy1, dy2, x, w1, w2, mean,
+                                rstd, dres, dx, pt[0], pt[1], pt[2], pt[3], M, D));
+  }
+  SK_LAUNCH_CHECK();
+  bf16* outs[4] = {dw1, db1, dw2, db2};
+  for (int t = 0; t < 4; ++t) {
+    SK_CUDA_CHECK(sk_launch_pdl(colsum_reduce_kernel, dim3((D + 31) / 32), dim3(1024), (size_t)0, s, (const float*)pt[t], outs[t],
+                                blocks, D, accumulate));
+    SK_LAUNCH_CHECK();
+  }
   return 0;
 }
 int sk_relu_bwd_launch(bf16* g, const bf16* a, long n, cudaStream_t s) {

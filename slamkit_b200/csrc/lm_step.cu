@@ -28,7 +28,11 @@ struct LayerOff {
 struct OptLayerOff {
   int64_t ln1w, ln1b, wqkv, bqkv, wo, bo, ln2w, ln2b, w1, b1, w2, b2;
 };
-enum { SK_ARCH_QWEN2 = 0, SK_ARCH_OPT = 1 };
+// GPT-NeoX layer (HF GPTNeoXLayer, use_parallel_residual = True): two LayerNorms of the same input, biased linears
+struct NeoxLayerOff {
+  int64_t ln1w, ln1b, ln2w, ln2b, wqkv, bqkv, wo, bo, w1, b1, w2, b2;
+};
+enum { SK_ARCH_QWEN2 = 0, SK_ARCH_OPT = 1, SK_ARCH_NEOX = 2 };
 // byte offsets into the workspace for one (B,T)
 struct WsLayout {
   int64_t X, h1, rstd1, qkv, ao, lse, xmid, h2, rstd2, gu, act;  // per-layer strides below
@@ -45,6 +49,8 @@ struct SkLm {
   std::vector<TensorDesc> tensors;
   std::vector<LayerOff> lo;
   std::vector<OptLayerOff> olo;   // OPT layers
+  std::vector<NeoxLayerOff> nlo;  // GPT-NeoX layers
+  int rot = 64;                   // GPT-NeoX: rotated columns per q / k head (rotary_ndims)
   int64_t off_final_norm_b = 0, off_pos = 0;
   int n_pos = 0;                  // OPT: rows of the learned position table (max_positions + 2)
   int64_t off_final_norm = 0, off_embed = 0, off_head = 0, n_params = 0;
@@ -345,7 +351,8 @@ DecLayout make_dec_layout(const SkLm* lm, int B, int T_cache) {
   w.h = take((int64_t)B * lm->d * 2);
   w.qkv = take((int64_t)B * lm->qkv_dim * 2);
   w.ao = take((int64_t)B * lm->d * 2);
-  w.gu = take((int64_t)B * 2 * lm->F * 2);
+  // Qwen2: gate|up [B, 2F]; GPT-NeoX: pre-activation [B, F] followed by ln2's output [B, d]
+  w.gu = take((int64_t)B * std::max(2 * lm->F, lm->F + lm->d) * 2);
   w.act = take((int64_t)B * lm->F * 2);
   w.lens = take((int64_t)B * 4);
   w.partial = take(sk_attn_decode_partial_bytes(B, lm->H, T_cache));
@@ -425,8 +432,232 @@ WsLayout make_opt_layout(const SkLm* lm, int B, int T) {
   return w;
 }
 
+// GPT-NeoX: rstd1 slabs hold the shared mean then rstd of the two LayerNorms (fp32 [2][M]), h1 / h2 their outputs,
+// `gu` the pre-activation of dense_h_to_4h [M, F] and `act` its GELU; `xmid` is one [M, d] slab for the attention
+// branch's output (read once, by the same layer's dense_4h_to_h epilogue); rstd2 is unused.
+WsLayout make_neox_layout(const SkLm* lm, int B, int T) {
+  WsLayout w;
+  const int64_t M = (int64_t)B * T;
+  int64_t cur = 0;
+  auto take = [&](int64_t bytes) {
+    const int64_t o = cur;
+    cur = align_up(cur + bytes, 256);
+    return o;
+  };
+  const int L = lm->L;
+  w.sX = align_up(M * lm->d * 2, 256);
+  w.sh = w.sX;
+  w.srstd = align_up(M * 8, 256);
+  w.sqkv = align_up(M * lm->qkv_dim * 2, 256);
+  w.slse = align_up((int64_t)B * lm->H * T * 4, 256);
+  w.sgu = align_up(M * lm->F * 2, 256);
+  w.sact = w.sgu;
+  // GEMM scratch first, at the same fixed offset as in make_layout (sk_lm_bind clears its flag words once)
+  w.splitk_bytes = align_up(std::max<int64_t>((int64_t)8 * lm->qkv_dim * lm->d * 4, (int64_t)sk_gemm_ws_min_bytes()) + 4096, 256);
+  w.splitk = take(w.splitk_bytes);
+  w.X = take(w.sX * (L + 1));
+  w.h1 = take(w.sh * L);
+  w.rstd1 = take(w.srstd * L);
+  w.qkv = take(w.sqkv * L);
+  w.ao = take(w.sX * L);
+  w.lse = take(w.slse * L);
+  w.xmid = take(w.sX);
+  w.h2 = take(w.sh * L);
+  w.rstd2 = 0;
+  w.gu = take(w.sgu * L);
+  w.act = take(w.sact * L);
+  w.hf = take(w.sX);
+  w.rstdf = take(w.srstd);
+  w.logits = take(M * lm->Vp * 2);
+  w.dlogits = lm->head_chunk > 0 ? w.logits : take(M * lm->Vp * 2);
+  w.dxA = take(w.sX);
+  w.dxB = take(w.sX);
+  w.dh = take(w.sX);
+  w.dao = take(w.sX);
+  w.dqkv = take(w.sqkv);
+  w.dgu = take(w.sgu);
+  w.delta = take(w.slse);
+  w.dw_partial = take((int64_t)4 * sk_layernorm_bwd_blocks() * lm->d * 4);   // the dual LayerNorm's four partials
+  w.colsum_partial = take((int64_t)sk_colsum_splits() * std::max(lm->qkv_dim, lm->F) * 4);
+  w.ce_partial = take((int64_t)sk_ce_blocks((int)M) * 2 * 4);
+  w.embed_scratch = take((int64_t)lm->Vp * lm->d * 8);
+  w.seg_start = take(M * 4);
+  w.seg_end = take(M * 4);
+  w.total = cur;
+  return w;
+}
+
 WsLayout layout_of(const SkLm* lm, int B, int T) {
+  if (lm->arch == SK_ARCH_NEOX) return make_neox_layout(lm, B, T);
   return lm->arch == SK_ARCH_OPT ? make_opt_layout(lm, B, T) : make_layout(lm, B, T);
+}
+
+// ---- GPT-NeoX decoder (HF:models/gpt_neox/modeling_gpt_neox.py: GPTNeoXAttention, GPTNeoXMLP, GPTNeoXLayer with
+// use_parallel_residual = True, GPTNeoXModel, GPTNeoXForCausalLM).  Separate functions, picked by lm->arch.
+//   h1 = LN1(x), h2 = LN2(x)              one dual-LayerNorm launch, shared mean / rstd
+//   qkv = h1 Wqkv + b, partial RoPE       the RoPE epilogue with rot columns per head (weights in [Q;K;V] row order)
+//   attn = attention(qkv) Wo + bo
+//   pre = h2 W1 + b1, act = gelu(pre)     one epilogue, two outputs
+//   x' = bf16(bf16(act W2 + b2 + attn) + x)   the two-residual epilogue, HF's order `mlp + attn + hidden_states`
+int neox_forward(SkLm* lm, const int64_t* ids, const int64_t* labels, const int32_t* pos_ids, int B, int T, float num_items,
+                 float dloss, bool want_dlogits, float* stats, const WsLayout& w, cudaStream_t s, float* row_nll = nullptr,
+                 bool with_head = true) {
+  const int M = B * T, d = lm->d, F = lm->F, L = lm->L, Q = lm->qkv_dim;
+  const float eps = lm->cfg.rms_eps;
+  const bf16* P = lm->params;
+  SK_TRY(sk_embed_fwd_launch(ids, P + lm->off_embed, wsp<bf16>(lm, w.X), M, d, lm->V, s));
+  const float scale = 1.0f / sqrtf((float)lm->hd);
+  const int* seg_start = nullptr;
+  if (pos_ids) {
+    SK_TRY(sk_seg_bounds_launch(pos_ids, wsp<int32_t>(lm, w.seg_start), wsp<int32_t>(lm, w.seg_end), B, T, s));
+    seg_start = wsp<int32_t>(lm, w.seg_start);
+  }
+  bf16* attn = wsp<bf16>(lm, w.xmid);
+  for (int l = 0; l < L; ++l) {
+    const NeoxLayerOff& o = lm->nlo[l];
+    bf16* x = wsp<bf16>(lm, w.X + w.sX * l);
+    bf16* xn = wsp<bf16>(lm, w.X + w.sX * (l + 1));
+    bf16* h1 = wsp<bf16>(lm, w.h1 + w.sh * l);
+    bf16* h2 = wsp<bf16>(lm, w.h2 + w.sh * l);
+    float* st = wsp<float>(lm, w.rstd1 + w.srstd * l);
+    bf16* qkv = wsp<bf16>(lm, w.qkv + w.sqkv * l);
+    bf16* ao = wsp<bf16>(lm, w.ao + w.sX * l);
+    float* lse = wsp<float>(lm, w.lse + w.slse * l);
+    bf16* pre = wsp<bf16>(lm, w.gu + w.sgu * l);
+    bf16* act = wsp<bf16>(lm, w.act + w.sact * l);
+
+    SK_TRY(sk_layernorm2_fwd_launch(x, P + o.ln1w, P + o.ln1b, P + o.ln2w, P + o.ln2b, h1, h2, st, st + M, M, d, eps, s));
+    SK_TRY(sk_linear_rope_launch(M, Q, d, h1, P + o.wqkv, P + o.bqkv, qkv, lm->rope_cos, lm->rope_sin, pos_ids, T, 2 * d,
+                                 lm->cfg.max_positions, s, lm->rot));
+    SK_TRY(sk_attn_tc_fwd_launch(qkv, ao, lse, B, T, lm->H, lm->H, Q, d, 1, scale, s, seg_start));
+    SK_TRY(linear_fwd(M, d, d, ao, P + o.wo, attn, P + o.bo, nullptr, s));
+    SK_TRY(sk_linear_gelu_fwd_launch(M, F, d, h2, P + o.w1, P + o.b1, pre, act, s));
+    SK_TRY(sk_linear_res2_launch(M, d, F, act, P + o.w2, P + o.b2, attn, x, xn, s));
+  }
+  float* stf = wsp<float>(lm, w.rstdf);
+  SK_TRY(sk_layernorm_fwd_launch(wsp<bf16>(lm, w.X + w.sX * L), P + lm->off_final_norm, P + lm->off_final_norm_b,
+                                 wsp<bf16>(lm, w.hf), stf, stf + M, M, d, eps, s));
+  lm->last_B = B;
+  lm->last_T = T;
+  if (!with_head) return 0;
+  bf16* logits = wsp<bf16>(lm, w.logits);
+  SK_TRY(linear_fwd(M, lm->Vp, d, wsp<bf16>(lm, w.hf), P + lm->off_head, logits, nullptr, nullptr, s));
+  if (labels) {
+    SK_TRY(sk_ce_launch(logits, labels, want_dlogits ? wsp<bf16>(lm, w.dlogits) : nullptr, wsp<float>(lm, w.ce_partial),
+                        row_nll, stats, M, T, lm->V, lm->Vp, num_items, dloss, s));
+  }
+  return 0;
+}
+
+// The layer output's gradient dy reaches the MLP, the attention branch and the residual unchanged.  dense and
+// dense_4h_to_h both take dy; their bias gradients are the same column sums, formed once per bias as HF does.  The input
+// gradient dx = dy + LN1'(dh1) + LN2'(dh2) is summed in fp32 inside the dual-LayerNorm backward.
+int neox_backward(SkLm* lm, const int64_t* ids, const int32_t* pos_ids, int B, int T, int accumulate, const WsLayout& w,
+                  cudaStream_t s, bool with_head = true) {
+  const int M = B * T, d = lm->d, F = lm->F, L = lm->L, Q = lm->qkv_dim;
+  const bf16* P = lm->params;
+  bf16* G = lm->grads;
+  float* lnp = wsp<float>(lm, w.dw_partial);
+  float* csp = wsp<float>(lm, w.colsum_partial);
+  bf16* dy = wsp<bf16>(lm, w.dxA);
+  bf16* dnext = wsp<bf16>(lm, w.dxB);
+  bf16* dh = wsp<bf16>(lm, w.dh);
+  bf16* dao = wsp<bf16>(lm, w.dao);
+  bf16* dqkv = wsp<bf16>(lm, w.dqkv);
+  bf16* dpre = wsp<bf16>(lm, w.dgu);
+  bf16* hf = wsp<bf16>(lm, w.hf);
+  void* sws = lm->ws + w.splitk;
+  const size_t swb = (size_t)w.splitk_bytes;
+  const float scale = 1.0f / sqrtf((float)lm->hd);
+  const int* seg_start = pos_ids ? wsp<int32_t>(lm, w.seg_start) : nullptr;
+  const int* seg_end = pos_ids ? wsp<int32_t>(lm, w.seg_end) : nullptr;
+
+  if (with_head) {
+    bf16* dlogits = wsp<bf16>(lm, w.dlogits);
+    SK_TRY(linear_dgrad(M, lm->Vp, d, dlogits, P + lm->off_head, dh, s));
+    SK_TRY(linear_wgrad(M, lm->Vp, d, dlogits, hf, G + lm->off_head, accumulate, s, sws, swb));
+  }
+  const float* stf = wsp<float>(lm, w.rstdf);
+  SK_TRY(sk_layernorm_bwd_launch(dh, wsp<bf16>(lm, w.X + w.sX * L), P + lm->off_final_norm, stf, stf + M, nullptr, dy,
+                                 G + lm->off_final_norm, G + lm->off_final_norm_b, lnp,
+                                 lnp + (size_t)sk_layernorm_bwd_blocks() * d, M, d, accumulate, s));
+  if (!lm->bwd_events.empty()) SK_CUDA_CHECK(cudaEventRecord(lm->bwd_events[L], s));
+  for (int l = L - 1; l >= 0; --l) {
+    const NeoxLayerOff& o = lm->nlo[l];
+    const bf16* x = wsp<bf16>(lm, w.X + w.sX * l);
+    const bf16* h1 = wsp<bf16>(lm, w.h1 + w.sh * l);
+    const bf16* h2 = wsp<bf16>(lm, w.h2 + w.sh * l);
+    const float* st = wsp<float>(lm, w.rstd1 + w.srstd * l);
+    const bf16* qkv = wsp<bf16>(lm, w.qkv + w.sqkv * l);
+    const bf16* ao = wsp<bf16>(lm, w.ao + w.sX * l);
+    const float* lse = wsp<float>(lm, w.lse + w.slse * l);
+    const bf16* pre = wsp<bf16>(lm, w.gu + w.sgu * l);
+    const bf16* act = wsp<bf16>(lm, w.act + w.sact * l);
+
+    // MLP: d_pre = bf16(bf16(dy W2) * gelu'(pre)) from the GEMM epilogue; dh2 -> dh
+    SK_TRY(sk_linear_gelu_bwd_launch(M, d, F, dy, P + o.w2, pre, dpre, s));
+    SK_TRY(linear_wgrad(M, d, F, dy, act, G + o.w2, accumulate, s, sws, swb));
+    SK_TRY(sk_colsum_launch(dy, G + o.b2, csp, M, d, d, accumulate, s));
+    SK_TRY(linear_dgrad(M, F, d, dpre, P + o.w1, dh, s));
+    SK_TRY(linear_wgrad(M, F, d, dpre, h2, G + o.w1, accumulate, s, sws, swb));
+    SK_TRY(sk_colsum_launch(dpre, G + o.b1, csp, M, F, F, accumulate, s));
+    // attention: the same dy; inverse partial RoPE on dq / dk after the attention backward; dh1 -> dao
+    SK_TRY(linear_dgrad(M, d, d, dy, P + o.wo, dao, s));
+    SK_TRY(linear_wgrad(M, d, d, dy, ao, G + o.wo, accumulate, s, sws, swb));
+    SK_TRY(sk_colsum_launch(dy, G + o.bo, csp, M, d, d, accumulate, s));
+    SK_TRY(sk_attn_tc_bwd_launch(qkv, ao, dao, lse, wsp<float>(lm, w.delta), nullptr, dqkv, B, T, lm->H, lm->H, Q, d, Q, 1,
+                                 scale, s, seg_start, seg_end));
+    SK_TRY(sk_rope_launch(dqkv, lm->rope_cos, lm->rope_sin, pos_ids, M, T, Q, 2 * lm->H, lm->hd, 1, lm->cfg.max_positions, s,
+                          lm->rot));
+    SK_TRY(sk_colsum_launch(dqkv, G + o.bqkv, csp, M, Q, Q, accumulate, s));
+    SK_TRY(linear_dgrad(M, Q, d, dqkv, P + o.wqkv, dao, s));
+    SK_TRY(linear_wgrad(M, Q, d, dqkv, h1, G + o.wqkv, accumulate, s, sws, swb));
+    SK_TRY(sk_layernorm2_bwd_launch(dao, dh, x, P + o.ln1w, P + o.ln2w, st, st + M, dy, dnext, G + o.ln1w, G + o.ln1b,
+                                    G + o.ln2w, G + o.ln2b, lnp, M, d, accumulate, s));
+    std::swap(dy, dnext);
+    if (!lm->bwd_events.empty()) SK_CUDA_CHECK(cudaEventRecord(lm->bwd_events[l], s));
+  }
+  return sk_embed_bwd_launch(ids, dy, wsp<float>(lm, w.embed_scratch), G + lm->off_embed, M, d, lm->V, lm->Vp, accumulate, s);
+}
+
+// One token per row at position pos[b] (read on the device: the step is graph-capturable).  Decode workspace: h = ln1,
+// `gu` = [pre (B x F) | ln2 (B x d)], `act` = the GELU, x1 = the attention branch's output; the layer output is written
+// over x in place by the two-residual epilogue.
+int neox_decode_step(SkLm* lm, const int64_t* tokens, const int32_t* pos, int B, void* kv_cache, int T_cache, void* logits,
+                     int ldl, uint8_t* dws, const DecLayout& dl, cudaStream_t s) {
+  const int d = lm->d, F = lm->F, Q = lm->qkv_dim;
+  const float eps = lm->cfg.rms_eps;
+  const bf16* P = lm->params;
+  bf16* x = reinterpret_cast<bf16*>(dws + dl.x0);
+  bf16* attn = reinterpret_cast<bf16*>(dws + dl.x1);
+  bf16* h = reinterpret_cast<bf16*>(dws + dl.h);
+  bf16* qkv = reinterpret_cast<bf16*>(dws + dl.qkv);
+  bf16* ao = reinterpret_cast<bf16*>(dws + dl.ao);
+  bf16* pre = reinterpret_cast<bf16*>(dws + dl.gu);
+  bf16* h2 = pre + (size_t)B * F;
+  bf16* act = reinterpret_cast<bf16*>(dws + dl.act);
+  int32_t* lens = reinterpret_cast<int32_t*>(dws + dl.lens);
+  float* partial = reinterpret_cast<float*>(dws + dl.partial);
+  void* gemm_ws = dws + dl.gemm;
+  const size_t plane = (size_t)B * lm->H * T_cache * lm->hd;
+  const float scale = 1.0f / sqrtf((float)lm->hd);
+  SK_TRY(sk_embed_fwd_launch(tokens, P + lm->off_embed, x, B, d, lm->V, s));
+  for (int l = 0; l < lm->L; ++l) {
+    const NeoxLayerOff& o = lm->nlo[l];
+    bf16* kc = reinterpret_cast<bf16*>(kv_cache) + (size_t)l * 2 * plane;
+    bf16* vc = kc + plane;
+    SK_TRY(sk_layernorm2_fwd_launch(x, P + o.ln1w, P + o.ln1b, P + o.ln2w, P + o.ln2b, h, h2, nullptr, nullptr, B, d, eps, s));
+    SK_TRY(sk_linear_rope_launch(B, Q, d, h, P + o.wqkv, P + o.bqkv, qkv, lm->rope_cos, lm->rope_sin, pos, 1, 2 * d,
+                                 lm->cfg.max_positions, s, lm->rot));
+    SK_TRY(sk_kv_append_launch(qkv, Q, kc, vc, pos, lens, B, lm->H, lm->H, T_cache, s));
+    SK_TRY(sk_attn_decode_launch(qkv, Q, kc, vc, lens, ao, d, partial, B, lm->H, lm->H, T_cache, scale, s));
+    SK_TRY(linear_fwd(B, d, d, ao, P + o.wo, attn, P + o.bo, nullptr, s));
+    SK_TRY(sk_linear_gelu_fwd_launch(B, F, d, h2, P + o.w1, P + o.b1, pre, act, s));
+    // with M = B the scratch lets stream-K spread dense_4h_to_h's long K loop over idle SMs
+    SK_TRY(sk_linear_res2_launch(B, d, F, act, P + o.w2, P + o.b2, attn, x, x, s, gemm_ws, (size_t)dl.gemm_bytes));
+  }
+  SK_TRY(sk_layernorm_fwd_launch(x, P + lm->off_final_norm, P + lm->off_final_norm_b, h, nullptr, nullptr, B, d, eps, s));
+  return sk_gemm_launch(B, lm->Vp, d, h, d, 0, P + lm->off_head, d, 0, logits, ldl, 0, nullptr, nullptr, 0, 0, 0, 0, s);
 }
 
 int opt_forward(SkLm* lm, const int64_t* ids, const int64_t* labels, const int32_t* pos_ids, int B, int T, float num_items,
@@ -644,8 +875,9 @@ int sk_lm_prefill(SkLm* lm, const int64_t* ids, const int32_t* lens, int B, int 
   cudaStream_t s = (cudaStream_t)stream;
   uint8_t* dws = reinterpret_cast<uint8_t*>(decode_ws);
   SK_CUDA_CHECK(cudaMemsetAsync(dws + dl.gemm + dl.gemm_bytes - 4096, 0, 4096, s));
-  if (lm->arch == SK_ARCH_OPT) SK_TRY(opt_forward(lm, ids, nullptr, nullptr, B, T, 0.f, 1.f, false, nullptr, w, s, nullptr, false));
-  else                         SK_TRY(forward_impl(lm, ids, nullptr, nullptr, B, T, 0.f, 1.f, false, nullptr, w, s, nullptr, false));
+  if (lm->arch == SK_ARCH_OPT)       SK_TRY(opt_forward(lm, ids, nullptr, nullptr, B, T, 0.f, 1.f, false, nullptr, w, s, nullptr, false));
+  else if (lm->arch == SK_ARCH_NEOX) SK_TRY(neox_forward(lm, ids, nullptr, nullptr, B, T, 0.f, 1.f, false, nullptr, w, s, nullptr, false));
+  else                               SK_TRY(forward_impl(lm, ids, nullptr, nullptr, B, T, 0.f, 1.f, false, nullptr, w, s, nullptr, false));
   SK_TRY(sk_kv_prefill_launch(wsp<bf16>(lm, w.qkv), w.sqkv / 2, lm->qkv_dim, reinterpret_cast<bf16*>(kv_cache), lens, lm->L, B,
                               T, lm->H, lm->KVH, T_cache, s));
   bf16* hl = reinterpret_cast<bf16*>(dws + dl.h);
@@ -662,6 +894,8 @@ int sk_lm_decode_step(SkLm* lm, const int64_t* tokens, const int32_t* pos, int B
   cudaStream_t s = (cudaStream_t)stream;
   if (lm->arch == SK_ARCH_OPT)
     return opt_decode_step(lm, tokens, pos, B, kv_cache, T_cache, logits, ldl, reinterpret_cast<uint8_t*>(decode_ws), dl, s);
+  if (lm->arch == SK_ARCH_NEOX)
+    return neox_decode_step(lm, tokens, pos, B, kv_cache, T_cache, logits, ldl, reinterpret_cast<uint8_t*>(decode_ws), dl, s);
   const int d = lm->d, F = lm->F, Q = lm->qkv_dim;
   const bf16* P = lm->params;
   uint8_t* dws = reinterpret_cast<uint8_t*>(decode_ws);
@@ -875,6 +1109,88 @@ int sk_lm_create_opt(const SkOptConfig* cfg, SkLm** out) {
   return 0;
 }
 
+int sk_lm_create_neox(const SkNeoxConfig* cfg, SkLm** out) {
+  SK_REQUIRE(cfg && out, "sk_lm_create_neox: null argument");
+  SK_REQUIRE(cfg->n_heads > 0 && cfg->hidden == 64 * cfg->n_heads,
+             "sk_lm_create_neox: only head_dim 64 is supported (hidden %d, %d heads)", cfg->hidden, cfg->n_heads);
+  SK_REQUIRE(cfg->hidden <= 2048, "sk_lm_create_neox: hidden must be <= 2048 (got %d)", cfg->hidden);
+  SK_REQUIRE(cfg->ffn > 0 && cfg->ffn % 64 == 0, "sk_lm_create_neox: ffn must be a positive multiple of 64 (got %d)", cfg->ffn);
+  SK_REQUIRE(cfg->rot_dims == 16 || cfg->rot_dims == 32 || cfg->rot_dims == 64,
+             "sk_lm_create_neox: rot_dims (rotary_ndims) must be 16, 32 or 64 (got %d)", cfg->rot_dims);
+  SK_REQUIRE(cfg->n_layers > 0 && cfg->max_positions > 0, "sk_lm_create_neox: n_layers and max_positions must be positive");
+  SK_REQUIRE(cfg->vocab_size > 0 && cfg->vocab_size <= (1 << 20), "sk_lm_create_neox: vocab_size must be in [1, 2^20]");
+  SkLm* lm = new SkLm();
+  lm->arch = SK_ARCH_NEOX;
+  lm->cfg.vocab_size = cfg->vocab_size;
+  lm->cfg.hidden = cfg->hidden;
+  lm->cfg.n_layers = cfg->n_layers;
+  lm->cfg.n_heads = cfg->n_heads;
+  lm->cfg.n_kv_heads = cfg->n_heads;
+  lm->cfg.head_dim = 64;
+  lm->cfg.ffn = cfg->ffn;
+  lm->cfg.max_positions = cfg->max_positions;
+  lm->cfg.rms_eps = cfg->ln_eps;
+  lm->cfg.tie_embeddings = 0;
+  lm->cfg.qkv_bias = 1;
+  lm->d = cfg->hidden;
+  lm->F = cfg->ffn;
+  lm->H = lm->KVH = cfg->n_heads;
+  lm->hd = 64;
+  lm->rot = cfg->rot_dims;
+  lm->L = cfg->n_layers;
+  lm->V = cfg->vocab_size;
+  lm->Vp = (cfg->vocab_size + 63) / 64 * 64;
+  lm->qkv_dim = 3 * lm->d;
+  lm->head_chunk = lm->Vp > 8192 ? 2048 : 0;
+  if (const char* e = getenv("SK_HEAD_CHUNK")) lm->head_chunk = (atoi(e) / 128) * 128;
+  const int d = lm->d, F = lm->F;
+  lm->nlo.resize(lm->L);
+  for (int l = 0; l < lm->L; ++l) {
+    const std::string p = "layers." + std::to_string(l) + ".";
+    NeoxLayerOff& o = lm->nlo[l];
+    o.ln1w = add_tensor(lm, p + "ln1", 1, d);
+    o.ln1b = add_tensor(lm, p + "ln1_b", 1, d);
+    o.ln2w = add_tensor(lm, p + "ln2", 1, d);
+    o.ln2b = add_tensor(lm, p + "ln2_b", 1, d);
+    o.wqkv = add_tensor(lm, p + "wqkv", 3 * d, d);
+    o.bqkv = add_tensor(lm, p + "bqkv", 1, 3 * d);
+    o.wo = add_tensor(lm, p + "wo", d, d);
+    o.bo = add_tensor(lm, p + "bo", 1, d);
+    o.w1 = add_tensor(lm, p + "w1", F, d);
+    o.b1 = add_tensor(lm, p + "b1", 1, F);
+    o.w2 = add_tensor(lm, p + "w2", d, F);
+    o.b2 = add_tensor(lm, p + "b2", 1, d);
+  }
+  lm->off_final_norm = add_tensor(lm, "final_norm", 1, d);
+  lm->off_final_norm_b = add_tensor(lm, "final_norm_b", 1, d);
+  lm->off_embed = add_tensor(lm, "embed", lm->Vp, d);
+  lm->off_head = add_tensor(lm, "lm_head", lm->Vp, d);
+  // one gradient-norm group per HF parameter, in GPTNeoXForCausalLM.parameters() order (query_key_value is one tensor)
+  std::vector<std::vector<std::pair<int64_t, int64_t>>> groups;
+  auto one = [&](int64_t off, int64_t n) { groups.push_back({{off, n}}); };
+  const int64_t dd = (int64_t)d * d;
+  one(lm->off_embed, (int64_t)lm->Vp * d);
+  for (int l = 0; l < lm->L; ++l) {
+    const NeoxLayerOff& o = lm->nlo[l];
+    one(o.ln1w, d); one(o.ln1b, d);
+    one(o.ln2w, d); one(o.ln2b, d);
+    one(o.wqkv, 3 * dd); one(o.bqkv, 3 * d);
+    one(o.wo, dd); one(o.bo, d);
+    one(o.w1, (int64_t)F * d); one(o.b1, F);
+    one(o.w2, (int64_t)d * F); one(o.b2, d);
+  }
+  one(lm->off_final_norm, d);
+  one(lm->off_final_norm_b, d);
+  one(lm->off_head, (int64_t)lm->Vp * d);
+  const int rc = upload_norm_groups(lm, groups);
+  if (rc) {
+    sk_lm_destroy(lm);
+    return rc;
+  }
+  *out = lm;
+  return 0;
+}
+
 void sk_lm_destroy(SkLm* lm) {
   if (!lm) return;
   cudaFree(lm->d_chunk_start);
@@ -910,7 +1226,7 @@ int64_t sk_lm_workspace_bytes(const SkLm* lm, int B, int T) {
 int sk_lm_bind(SkLm* lm, void* params, void* grads, const void* rope_cos, const void* rope_sin, void* workspace,
                int64_t workspace_bytes) {
   SK_REQUIRE(lm && params && workspace, "sk_lm_bind: null argument");
-  SK_REQUIRE((rope_cos && rope_sin) || lm->arch == SK_ARCH_OPT, "sk_lm_bind: a Qwen2 handle needs the RoPE tables");
+  SK_REQUIRE((rope_cos && rope_sin) || lm->arch == SK_ARCH_OPT, "sk_lm_bind: a Qwen2 or GPT-NeoX handle needs the RoPE tables");
   SK_REQUIRE(((uintptr_t)params & 127) == 0 && (grads == nullptr || ((uintptr_t)grads & 127) == 0) &&
                  ((uintptr_t)workspace & 255) == 0,
              "sk_lm_bind: params/grads must be 128-byte and workspace 256-byte aligned");
@@ -937,6 +1253,8 @@ int sk_lm_forward(SkLm* lm, const int64_t* ids, const int64_t* labels, const int
   SK_TRY(check_bound(lm, B, T, w, pos_ids));
   if (lm->arch == SK_ARCH_OPT)
     return opt_forward(lm, ids, labels, pos_ids, B, T, num_items, 1.0f, false, stats, w, (cudaStream_t)stream);
+  if (lm->arch == SK_ARCH_NEOX)
+    return neox_forward(lm, ids, labels, pos_ids, B, T, num_items, 1.0f, false, stats, w, (cudaStream_t)stream);
   return forward_impl(lm, ids, labels, pos_ids, B, T, num_items, 1.0f, false, stats, w, (cudaStream_t)stream);
 }
 
@@ -955,6 +1273,16 @@ int sk_lm_forward_backward(SkLm* lm, const int64_t* ids, const int64_t* labels, 
     }
     SK_TRY(opt_forward(lm, ids, labels, pos_ids, B, T, num_items, dloss, true, stats, w, s));
     return opt_backward(lm, ids, pos_ids, B, T, accumulate, w, s);
+  }
+  if (lm->arch == SK_ARCH_NEOX) {
+    cudaStream_t s = (cudaStream_t)stream;
+    if (lm->head_chunk > 0) {
+      SK_TRY(neox_forward(lm, ids, labels, pos_ids, B, T, num_items, dloss, true, stats, w, s, nullptr, false));
+      SK_TRY(head_chunked(lm, labels, B, T, num_items, dloss, accumulate, stats, w, s));
+      return neox_backward(lm, ids, pos_ids, B, T, accumulate, w, s, false);
+    }
+    SK_TRY(neox_forward(lm, ids, labels, pos_ids, B, T, num_items, dloss, true, stats, w, s));
+    return neox_backward(lm, ids, pos_ids, B, T, accumulate, w, s);
   }
   if (lm->head_chunk > 0) {
     SK_TRY(forward_impl(lm, ids, labels, pos_ids, B, T, num_items, dloss, true, stats, w, (cudaStream_t)stream, nullptr, false));
@@ -984,6 +1312,8 @@ int sk_lm_forward_rows(SkLm* lm, const int64_t* ids, const int64_t* labels, cons
   SK_TRY(check_bound(lm, B, T, w, pos_ids));
   if (lm->arch == SK_ARCH_OPT)
     return opt_forward(lm, ids, labels, pos_ids, B, T, 1.0f, 1.0f, false, stats, w, (cudaStream_t)stream, row_nll);
+  if (lm->arch == SK_ARCH_NEOX)
+    return neox_forward(lm, ids, labels, pos_ids, B, T, 1.0f, 1.0f, false, stats, w, (cudaStream_t)stream, row_nll);
   return forward_impl(lm, ids, labels, pos_ids, B, T, 1.0f, 1.0f, false, stats, w, (cudaStream_t)stream, row_nll);
 }
 
@@ -1000,6 +1330,7 @@ int sk_lm_backward_weighted(SkLm* lm, const int64_t* ids, const int64_t* labels,
   SK_TRY(sk_ce_launch(wsp<bf16>(lm, w.logits), labels, wsp<bf16>(lm, w.dlogits), wsp<float>(lm, w.ce_partial), nullptr,
                       stats, B * T, T, lm->V, lm->Vp, 1.0f, 1.0f, s, row_weight));
   if (lm->arch == SK_ARCH_OPT) return opt_backward(lm, ids, pos_ids, B, T, accumulate, w, s);
+  if (lm->arch == SK_ARCH_NEOX) return neox_backward(lm, ids, pos_ids, B, T, accumulate, w, s);
   return backward_impl(lm, ids, pos_ids, B, T, accumulate, w, s);
 }
 

@@ -41,7 +41,9 @@ def hubert_b200_from_cfg(pretrained_model: str = "facebook/hubert-base-ls960",
 def tlm_b200_from_cfg(cfg, device: str = "cuda:0", max_batch: int = 8, max_seq: Optional[int] = None):
     """`cfg` is the reference's model config node (config/model/*.yaml): context_len, config_args{base_model_name,
     vocab_size, twist_init, rope_theta, torch_dtype, dropout, ...}.  The base config decides the decoder: Qwen2
-    (`LMConfig`) or pre-LayerNorm OPT (`OptLMConfig`, the default TWIST / GSLM base).  For OPT the reference's
+    (`LMConfig`), pre-LayerNorm OPT (`OptLMConfig`, the default TWIST / GSLM base) or parallel-residual GPT-NeoX
+    (`NeoxLMConfig`, the Pythia bases of config/train_inter_scale.yaml; the same overrides and dtype rule as OPT, and
+    `twist_init` loads the Pythia weights from a local directory or cache).  For OPT the reference's
     `config_args` overrides are applied to the base config as `UnitLMConfig` does (pad / bos / eos ids, dropout,
     attention_dropout, layerdrop), `rope_theta` is ignored, and `torch_dtype: bfloat16` is required: this path keeps bf16
     parameters and bf16 AdamW moments, while the reference run with `torch_dtype: null` keeps fp32 master weights.
@@ -64,6 +66,18 @@ def tlm_b200_from_cfg(cfg, device: str = "cuda:0", max_batch: int = 8, max_seq: 
         if str(dt).replace("torch.", "") != "bfloat16":
             raise ValueError(f"OPT on the GPU path trains bf16 parameters with bf16 AdamW moments; torch_dtype={dt} asks for "
                              "fp32 master weights, which it does not implement (pass model.config_args.torch_dtype=bfloat16)")
+    elif getattr(base, "model_type", None) == "gpt_neox":
+        # UnitLMConfig (slamkit/model/unit_lm.py:59-63) hands pad / bos / eos (defaults 0 / 1 / 1) and the yaml's
+        # remaining config_args to AutoConfig.from_pretrained
+        for k, dflt in (("pad_token_id", 0), ("bos_token_id", 1), ("eos_token_id", 1)):
+            setattr(base, k, get(k) if get(k) is not None else dflt)
+        for k in ("attention_dropout", "hidden_dropout", "use_parallel_residual", "hidden_act", "tie_word_embeddings"):
+            if get(k) is not None:
+                setattr(base, k, get(k))
+        dt = get("torch_dtype")
+        if str(dt).replace("torch.", "") != "bfloat16":
+            raise ValueError(f"GPT-NeoX on the GPU path trains bf16 parameters with bf16 AdamW moments; torch_dtype={dt} asks "
+                             "for fp32 master weights, which it does not implement (pass model.config_args.torch_dtype=bfloat16)")
     lm_cfg = lm_config_from_hf(base, vocab_size=get("vocab_size", 502), max_positions=max(2048, ctx))
     if get("rope_theta") is not None and not isinstance(lm_cfg, OptLMConfig):
         lm_cfg.rope_theta = float(get("rope_theta"))

@@ -113,17 +113,94 @@ class OptLMConfig:
             init_std=float(getattr(cfg, "init_std", 0.02)))
 
 
+@dataclass
+class NeoxLMConfig:
+    """Shape of a GPT-NeoX decoder with the parallel residual (defaults = EleutherAI/pythia-160m with the 502-entry unit
+    vocabulary; the base family of config/train_inter_scale.yaml).  `rot_dims` = head_dim * partial_rotary_factor
+    columns of each q / k head are rotated; `max_positions` is the number of RoPE table rows."""
+    vocab_size: int = 502
+    hidden: int = 768
+    n_layers: int = 12
+    n_heads: int = 12
+    ffn: int = 3072
+    max_positions: int = 2048
+    rot_dims: int = 16
+    rope_theta: float = 10000.0
+    ln_eps: float = 1e-5
+    init_std: float = 0.02
+    pad_token_id: int = 0
+    bos_token_id: int = 0
+    eos_token_id: int = 0
+    head_dim: int = 64
+    tie_embeddings: bool = False          # embed_out is always a separate matrix here (tied heads are refused)
+
+    @staticmethod
+    def from_hf(cfg, vocab_size: Optional[int] = None, max_positions: Optional[int] = None) -> "NeoxLMConfig":
+        """From an HF `GPTNeoXConfig`.  Only what the sm_90a kernels implement is accepted; every other variant is refused
+        by name: the sequential residual (use_parallel_residual=False), head_dim other than 64 (pythia-14m / -31m have 32,
+        pythia-1b and up 128 or 256), a rotary width other than 16, 32 or 64 columns, rope types other than default,
+        activations other than exact gelu, bias-free attention, tied input / output embeddings and any dropout."""
+        if getattr(cfg, "model_type", None) != "gpt_neox":
+            raise ValueError(f"NeoxLMConfig.from_hf: model_type is '{getattr(cfg, 'model_type', None)}', not 'gpt_neox'")
+        if not getattr(cfg, "use_parallel_residual", True):
+            raise ValueError("unsupported GPT-NeoX variant: use_parallel_residual=False (sequential residual)")
+        hd = getattr(cfg, "head_dim", None) or cfg.hidden_size // cfg.num_attention_heads
+        if cfg.hidden_size % cfg.num_attention_heads or hd != 64:
+            raise ValueError(f"unsupported attention geometry: head_dim = hidden_size / num_attention_heads = "
+                             f"{cfg.hidden_size / cfg.num_attention_heads:g}; the sm_90a attention kernels need head_dim 64")
+        rp = dict(getattr(cfg, "rope_parameters", None) or {})
+        rope_type = rp.get("rope_type", rp.get("type", "default"))
+        if rope_type != "default":
+            raise ValueError(f"unsupported GPT-NeoX setting: rope_type='{rope_type}' (only default RoPE)")
+        factor = rp.get("partial_rotary_factor", getattr(cfg, "partial_rotary_factor", getattr(cfg, "rotary_pct", 1.0)))
+        rot = int(hd * float(factor))
+        if rot not in (16, 32, 64):
+            raise ValueError(f"unsupported GPT-NeoX setting: partial_rotary_factor={factor} gives rotary_ndims={rot}; "
+                             "the RoPE epilogue rotates 16, 32 or 64 columns per head")
+        theta = rp.get("rope_theta", getattr(cfg, "rope_theta", getattr(cfg, "rotary_emb_base", 10000.0)))
+        act = getattr(cfg, "hidden_act", "gelu")
+        if act != "gelu":
+            raise ValueError(f"unsupported GPT-NeoX setting: hidden_act='{act}' (only the exact erf gelu)")
+        if not getattr(cfg, "attention_bias", True):
+            raise ValueError("unsupported GPT-NeoX setting: attention_bias=False")
+        if getattr(cfg, "tie_word_embeddings", False):
+            raise ValueError("unsupported GPT-NeoX setting: tie_word_embeddings=True (embed_out must be untied)")
+        for k in ("attention_dropout", "hidden_dropout"):
+            if float(getattr(cfg, k, 0.0) or 0.0) != 0.0:
+                raise ValueError(f"unsupported GPT-NeoX setting: {k}={getattr(cfg, k)} (there are no dropout kernels; "
+                                 "set it to 0.0)")
+        bos = getattr(cfg, "bos_token_id", None)
+        eos = getattr(cfg, "eos_token_id", None)
+        return NeoxLMConfig(
+            vocab_size=vocab_size or cfg.vocab_size, hidden=cfg.hidden_size, n_layers=cfg.num_hidden_layers,
+            n_heads=cfg.num_attention_heads, ffn=cfg.intermediate_size,
+            max_positions=max_positions or cfg.max_position_embeddings, rot_dims=rot, rope_theta=float(theta),
+            ln_eps=float(cfg.layer_norm_eps), init_std=float(getattr(cfg, "initializer_range", 0.02)),
+            pad_token_id=getattr(cfg, "pad_token_id", None) or 0, bos_token_id=bos if bos is not None else 0,
+            eos_token_id=eos if isinstance(eos, int) else 0)
+
+
 def lm_config_from_hf(base, vocab_size: Optional[int] = None, max_positions: int = 2048):
     """The decoder config for an HF base config, by `model_type`: `LMConfig` for qwen2 (RoPE tables of `max_positions`
-    rows), `OptLMConfig` for opt (its own learned position table; `max_positions` is ignored).  Anything else is
-    refused."""
+    rows), `OptLMConfig` for opt (its own learned position table; `max_positions` is ignored), `NeoxLMConfig` for
+    gpt_neox (RoPE tables of max(max_positions, max_position_embeddings) rows).  Anything else is refused."""
     mt = getattr(base, "model_type", None)
     if mt == "opt":
         return OptLMConfig.from_hf(base, vocab_size=vocab_size)
     if mt == "qwen2":
         return LMConfig.from_hf(base, vocab_size=vocab_size, max_positions=max_positions)
-    raise ValueError(f"unsupported base architecture '{mt}': the GPU path implements the Qwen2 and pre-LayerNorm OPT "
-                     "decoders")
+    if mt == "gpt_neox":
+        return NeoxLMConfig.from_hf(base, vocab_size=vocab_size,
+                                    max_positions=max(max_positions, int(getattr(base, "max_position_embeddings", 0) or 0)))
+    raise ValueError(f"unsupported base architecture '{mt}': the GPU path implements the Qwen2, pre-LayerNorm OPT and "
+                     "GPT-NeoX (parallel residual) decoders")
+
+
+def neox_qkv_segments(n_heads: int, head_dim: int = 64) -> List[Tuple[int, int, int]]:
+    """(row in the kernels' [Q; K; V] layout, row in HF's per-head [q | k | v] query_key_value, n rows) for every head's
+    q, k and v block, in HF row order: the permutation applied to the fused weight and bias on load and undone on save."""
+    d = n_heads * head_dim
+    return [(j * d + h * head_dim, h * 3 * head_dim + j * head_dim, head_dim) for h in range(n_heads) for j in range(3)]
 
 
 def rope_tables(theta: float, head_dim: int, max_positions: int) -> Tuple[torch.Tensor, torch.Tensor]:
@@ -153,6 +230,19 @@ def _opt_base_config(c: "OptLMConfig") -> dict:
             "bos_token_id": c.bos_token_id, "eos_token_id": c.eos_token_id, "torch_dtype": "bfloat16"}
 
 
+def _neox_base_config(c: "NeoxLMConfig") -> dict:
+    """The HF `GPTNeoXConfig` fields of a parallel-residual GPT-NeoX decoder of this shape (Pythia layout)."""
+    return {"model_type": "gpt_neox", "architectures": ["GPTNeoXForCausalLM"], "hidden_size": c.hidden,
+            "intermediate_size": c.ffn, "num_hidden_layers": c.n_layers, "num_attention_heads": c.n_heads,
+            "vocab_size": c.vocab_size, "max_position_embeddings": c.max_positions, "layer_norm_eps": c.ln_eps,
+            "use_parallel_residual": True, "hidden_act": "gelu", "attention_bias": True, "attention_dropout": 0.0,
+            "hidden_dropout": 0.0, "initializer_range": c.init_std, "tie_word_embeddings": False,
+            "rope_parameters": {"rope_theta": c.rope_theta, "partial_rotary_factor": c.rot_dims / c.head_dim,
+                                "rope_type": "default"},
+            "pad_token_id": c.pad_token_id, "bos_token_id": c.bos_token_id, "eos_token_id": c.eos_token_id,
+            "torch_dtype": "bfloat16"}
+
+
 def write_unit_lm_checkpoint(save_directory: str, state_dict_hf: Dict[str, torch.Tensor], config,
                              base_model_name: Optional[str] = None) -> None:
     """Writes `model.safetensors` with the `lm.`-prefixed names of `UnitLM.state_dict()` (base_model_prefix = "lm",
@@ -165,12 +255,13 @@ def write_unit_lm_checkpoint(save_directory: str, state_dict_hf: Dict[str, torch
     os.makedirs(save_directory, exist_ok=True)
     c = config
     is_opt = isinstance(c, OptLMConfig)
+    is_neox = isinstance(c, NeoxLMConfig)
     if base_model_name is None:
-        base_model_name = "facebook/opt-125m" if is_opt else "Qwen/Qwen2.5-0.5B"
+        base_model_name = "facebook/opt-125m" if is_opt else ("EleutherAI/pythia-160m" if is_neox else "Qwen/Qwen2.5-0.5B")
     sd = {k: v.detach().contiguous().cpu() for k, v in state_dict_hf.items()
           if k != "lm.lm_head.weight" or not c.tie_embeddings}
     save_file(sd, os.path.join(save_directory, "model.safetensors"), metadata={"format": "pt"})
-    base = _opt_base_config(c) if is_opt else {"model_type": "qwen2", "architectures": ["Qwen2ForCausalLM"], "hidden_size": c.hidden,
+    base = _opt_base_config(c) if is_opt else _neox_base_config(c) if is_neox else {"model_type": "qwen2", "architectures": ["Qwen2ForCausalLM"], "hidden_size": c.hidden,
             "intermediate_size": c.ffn, "num_hidden_layers": c.n_layers, "num_attention_heads": c.n_heads,
             "num_key_value_heads": c.n_kv_heads, "vocab_size": c.vocab_size, "rms_norm_eps": c.rms_eps,
             "max_position_embeddings": c.max_positions, "tie_word_embeddings": c.tie_embeddings, "hidden_act": "silu",
@@ -209,10 +300,15 @@ class B200UnitLM:
         self.lib = L.require_cuda()
         self.config = config
         self.is_opt = isinstance(config, OptLMConfig)
+        self.is_neox = isinstance(config, NeoxLMConfig)
         self.device = torch.device(device)
         torch.cuda.set_device(self.device)
         self._h = C.c_void_p()
-        if self.is_opt:
+        if self.is_neox:
+            c = L.SkNeoxConfig(config.vocab_size, config.hidden, config.n_layers, config.n_heads, config.ffn,
+                               config.max_positions, config.rot_dims, config.ln_eps)
+            L.check(self.lib.sk_lm_create_neox(C.byref(c), C.byref(self._h)))
+        elif self.is_opt:
             c = L.SkOptConfig(config.vocab_size, config.hidden, config.n_layers, config.n_heads, config.ffn,
                               config.max_positions, config.ln_eps, int(config.tie_embeddings))
             L.check(self.lib.sk_lm_create_opt(C.byref(c), C.byref(self._h)))
@@ -233,8 +329,9 @@ class B200UnitLM:
         self.params = torch.zeros(self.n_params, device=self.device, dtype=torch.bfloat16)
         self.grads = torch.zeros(self.n_params, device=self.device, dtype=torch.bfloat16) if trainable else None
         self.rope_cos = self.rope_sin = None          # OPT: learned positions, no RoPE tables
-        if not self.is_opt:
-            cos, sin = rope_tables(config.rope_theta, config.head_dim, config.max_positions)
+        if not self.is_opt:          # GPT-NeoX: tables over the rotated columns only (partial rotary)
+            cos, sin = rope_tables(config.rope_theta, config.rot_dims if self.is_neox else config.head_dim,
+                                   config.max_positions)
             self.rope_cos, self.rope_sin = cos.to(self.device), sin.to(self.device)
         self.max_batch, self.max_seq = max_batch, max_seq
         self.workspace = None
@@ -273,7 +370,7 @@ class B200UnitLM:
     def init_weights(self, seed: int = 0, std: float = 0.02) -> None:
         """HF `_init_weights` equivalent: normal(0, std) for linear/embedding weights, zeros for biases, ones for
         norms (HF:modeling_utils.py PreTrainedModel._init_weights)."""
-        if self.is_opt:
+        if self.is_opt or self.is_neox:
             return self._init_weights_opt(seed)
         g = torch.Generator(device="cpu").manual_seed(seed)
         V = self.config.vocab_size
@@ -293,7 +390,8 @@ class B200UnitLM:
     def _init_weights_opt(self, seed: int) -> None:
         """HF OPT init (PreTrainedModel._init_weights with config.init_std): normal(0, init_std) for the linear weights
         and both embedding tables, zero for the token table's pad_token_id row (nn.Embedding(padding_idx)), LayerNorm
-        weights 1 and biases 0, linear biases 0."""
+        weights 1 and biases 0, linear biases 0.  GPT-NeoX's init is the same with initializer_range as the std and no
+        padding row (embed_in has no padding_idx)."""
         g = torch.Generator(device="cpu").manual_seed(seed)
         cfg = self.config
         std = cfg.init_std
@@ -307,7 +405,7 @@ class B200UnitLM:
             elif base in ("embed", "lm_head"):
                 t.zero_()
                 t[:cfg.vocab_size].copy_((torch.randn((cfg.vocab_size, c), generator=g) * std).to(torch.bfloat16))
-                if base == "embed" and 0 <= cfg.pad_token_id < cfg.vocab_size:
+                if base == "embed" and self.is_opt and 0 <= cfg.pad_token_id < cfg.vocab_size:
                     t[cfg.pad_token_id].zero_()
             else:
                 t.copy_((torch.randn((r, c), generator=g) * std).to(torch.bfloat16))
@@ -338,6 +436,32 @@ class B200UnitLM:
         if not cfg.tie_embeddings:
             yield "lm_head", "lm.lm_head.weight", [(0, 0, cfg.vocab_size)]
 
+    def _hf_map_neox(self) -> Iterator[Tuple[str, str, List[Tuple[int, int, int]]]]:
+        """GPT-NeoX names of `UnitLM.state_dict()` over GPTNeoXForCausalLM.  HF's fused query_key_value holds per-head
+        [q | k | v] blocks of 3 x 64 rows; the flat `wqkv` / `bqkv` hold [Q; K; V] (what the attention kernels read), so
+        each head's three 64-row blocks are segments, listed in HF row order."""
+        cfg = self.config
+        d = cfg.hidden
+        qkv = neox_qkv_segments(cfg.n_heads, cfg.head_dim)
+        for l in range(cfg.n_layers):
+            p, h = f"layers.{l}.", f"lm.gpt_neox.layers.{l}."
+            yield p + "ln1", h + "input_layernorm.weight", [(0, 0, 1)]
+            yield p + "ln1_b", h + "input_layernorm.bias", [(0, 0, 1)]
+            yield p + "ln2", h + "post_attention_layernorm.weight", [(0, 0, 1)]
+            yield p + "ln2_b", h + "post_attention_layernorm.bias", [(0, 0, 1)]
+            yield p + "wqkv", h + "attention.query_key_value.weight", qkv
+            yield p + "bqkv", h + "attention.query_key_value.bias", qkv
+            yield p + "wo", h + "attention.dense.weight", [(0, 0, d)]
+            yield p + "bo", h + "attention.dense.bias", [(0, 0, 1)]
+            yield p + "w1", h + "mlp.dense_h_to_4h.weight", [(0, 0, cfg.ffn)]
+            yield p + "b1", h + "mlp.dense_h_to_4h.bias", [(0, 0, 1)]
+            yield p + "w2", h + "mlp.dense_4h_to_h.weight", [(0, 0, d)]
+            yield p + "b2", h + "mlp.dense_4h_to_h.bias", [(0, 0, 1)]
+        yield "final_norm", "lm.gpt_neox.final_layer_norm.weight", [(0, 0, 1)]
+        yield "final_norm_b", "lm.gpt_neox.final_layer_norm.bias", [(0, 0, 1)]
+        yield "embed", "lm.gpt_neox.embed_in.weight", [(0, 0, cfg.vocab_size)]
+        yield "lm_head", "lm.embed_out.weight", [(0, 0, cfg.vocab_size)]
+
     def _hf_map(self) -> Iterator[Tuple[str, str, List[Tuple[int, int, int]]]]:
         """(flat tensor name, HF parameter name, [(row in the flat tensor, row in the HF tensor, n rows), ...]).
 
@@ -346,6 +470,9 @@ class B200UnitLM:
         that one 256-column GEMM tile holds gate AND up of the same hidden units and SwiGLU runs in the GEMM epilogue."""
         if self.is_opt:
             yield from self._hf_map_opt()
+            return
+        if self.is_neox:
+            yield from self._hf_map_neox()
             return
         cfg = self.config
         q, kv = cfg.n_heads * cfg.head_dim, cfg.n_kv_heads * cfg.head_dim
@@ -416,6 +543,14 @@ class B200UnitLM:
         from safetensors.torch import load_file
         cfg = json.load(open(os.path.join(directory, "config.json")))
         b = cfg["base_config"]
+        if b.get("model_type") == "gpt_neox":
+            from transformers import GPTNeoXConfig
+            b = {k: v for k, v in b.items() if k not in ("model_type", "architectures")}
+            lm_cfg = NeoxLMConfig.from_hf(GPTNeoXConfig(**b), vocab_size=cfg["vocab_size"],
+                                          max_positions=max(max_seq, int(b.get("max_position_embeddings", 2048))))
+            m = cls(lm_cfg, device=device, max_batch=max_batch, max_seq=max_seq, trainable=trainable)
+            m.load_hf_state_dict(load_file(os.path.join(directory, "model.safetensors")))
+            return m
         if b.get("model_type") == "opt":
             from transformers import OPTConfig
             b = {k: v for k, v in b.items() if k not in ("model_type", "architectures")}
