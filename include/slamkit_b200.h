@@ -60,7 +60,9 @@ int64_t sk_gemm_ws_bytes(void);
  * ws_bytes, which of bias / residual / ws are NULL and whether residual == C matter. */
 typedef struct SkGemmPlan {
   int32_t bn;                /* tile width: 64, 128, 192, 224 or 256 (tiles are 128 rows) */
-  int32_t epi_warps;         /* 4, or 8 (two per 32-row quadrant) */
+  int32_t epi_warps;         /* 4, or 8 (two per 32-row quadrant): warps of the parked epilogue.  One-pass TMA-store
+                                plans with epi_warps == 4 and the plain convert or SwiGLU-forward epilogue finish each
+                                tile from the wgmma registers on all 8 consumer warps instead */
   int32_t splits;            /* > 1: split-K into this many K ranges, fp32 slabs summed by a second kernel */
   int32_t sk_units;          /* > 0: stream-K over the last sk_units units (rows of tiles, or columns: sk_colunits) */
   int32_t sk_groups;         /* CTA groups that share the stream-K iteration space (cut into equal K ranges) */

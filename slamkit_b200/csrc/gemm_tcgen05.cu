@@ -8,8 +8,11 @@
 //               as a [128][BN] row-major tile, and the epilogue warps read it back one ROW per thread (32 columns at a
 //               time): bias / residual / fused element-wise op -> swizzled smem -> TMA store.  EW = 4 epilogue
 //               warps (one per 32-row quadrant) or EW = 8 (two per quadrant, each owning half of the columns).
+//               Register epilogue (GemmParams::reg_epi: one-pass TMA-store tiles with the plain convert or SwiGLU-forward
+//               epilogue, 4-epilogue-warp kernels): the accumulator is not parked; each of the 8 consumer warps packs its
+//               16 rows from the wgmma fragments, stmatrix -> swizzled 16-row staging box -> TMA store.
 //   warp 8      TMA producer (cp.async.bulk.tensor -> 128B-swizzled smem ring, mbarrier complete_tx); it starts the
-//               next tile's loads once the parked accumulator has been consumed.
+//               next tile's loads once the parked accumulator has been consumed, or at once under the register epilogue.
 //
 // Operand majors.  "K-major" = the contraction index is contiguous in memory (A row-major [M,K], B row-major [N,K]).
 // "MN-major" = the M (or N) index is contiguous (A stored as [K,M], B stored as [K,N]).  MN-major operands let the
@@ -56,6 +59,7 @@ struct GemmParams {
   int splits;           // > 1: split-K; work item = (tile, split), fp32 partial tiles go to splitk_ws[split][M][N]
   float* splitk_ws;
   int tma_store;        // 1: bf16 output leaves through swizzled smem staging + cp.async.bulk.tensor stores (tmC)
+  int reg_epi;          // 1: register epilogue (one-pass TMA-store tiles, plain convert or SwiGLU forward; see the kernel)
   int pdl;              // host-only: launch attribute
   int sk_units;         // > 0: stream-K over the first sk_units tile groups ("units", see WorkIter)
   int sk_groups;        // CTA groups that share the stream-K iteration space (each unit is cut into <= ~4 ranges)
@@ -90,7 +94,9 @@ struct GemmCfg {
   static constexpr int B_BYTES = B_ATOMS * 64 * BK * 2;
   static constexpr int STAGE_BYTES = A_BYTES + B_BYTES;
   static constexpr int STAGES = (BN > 128) ? 4 : (BN > 64 ? 6 : 8);
-  static constexpr int STAGING_BYTES = 4 * 2 * 4096;  // (32 rows x 128 B) TMA-store buffers: 2 per warp (EW = 4) or 1 (EW = 8)
+  // TMA-store buffers: parked epilogue 2 x (32 rows x 128 B) per epilogue warp (EW = 4) or 1 (EW = 8); register epilogue
+  // 2 x (16 rows x 128 B) per consumer warp
+  static constexpr int STAGING_BYTES = 4 * 2 * 4096;
   static constexpr int BAR_BYTES = 256;
   static constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + STAGING_BYTES + BAR_BYTES + 1024;  // +1024: manual alignment
   static_assert(BN % 64 == 0 || (BN == 224 && EW == 4), "a 32-column tail chunk only on the 224-wide tile");
@@ -161,6 +167,11 @@ SK_DEVINL float gelu_exact_grad(float x) {
   const float cdf = 0.5f * (1.0f + erff(x * 0.70710678118654752440f));
   const float pdf = expf(-0.5f * x * x) * 0.39894228040143267794f;   // M_2_SQRTPI * M_SQRT1_2 * 0.5
   return cdf + x * pdf;
+}
+
+SK_DEVINL void stmatrix_x4(uint32_t addr, uint32_t a, uint32_t b, uint32_t c, uint32_t d) {
+  asm volatile("stmatrix.sync.aligned.m8n8.x4.shared.b16 [%0], {%1, %2, %3, %4};" ::"r"(addr), "r"(a), "r"(b), "r"(c),
+               "r"(d) : "memory");
 }
 
 // Work scheduler shared by the three warp roles.
@@ -433,7 +444,7 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
       bool first = true;
       WorkIter<SK> w(p, num_kb_total, kb_per_split, total_items);
       while (w.next()) {
-        if (!first) {   // the previous tile's accumulator is parked in the ring until its epilogue is done
+        if (!first && !p.reg_epi) {   // the previous tile's accumulator is parked in the ring until its epilogue is done
           mbar_wait_nocall(acc_free, acc_phase);
           acc_phase ^= 1u;
         }
@@ -497,10 +508,118 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
     while (w.next()) {
       {
         // ---- K loop: this warpgroup's 64 rows x BN columns accumulate in registers ----
-        float acc[BN / 2];
+        // A tile that continues from a carried-in accumulator and one that starts from zero run separate copies of the
+        // K loop: with one copy the two definitions merge ahead of the loop and ptxas serialises its wgmma pipeline.
+        // Register epilogue (p.reg_epi): each consumer warp converts its 16 rows of the tile straight from the wgmma
+        // fragments -- thread (lane) holds rows r and r + 8 (r = 16 * warp + lane / 4 of the tile), columns 8j + 2(lane % 4)
+        // + {0, 1} as acc[4j + 2h], acc[4j + 2h + 1] -- packs a 64-column chunk to bf16 pairs pk[2jj + h], writes them to
+        // one of the warp's two 16 x 64 staging boxes with stmatrix (128B swizzle; the 32-column tail chunk of a 224-wide
+        // tile: 64B swizzle) and stores the box by TMA.  The ring never holds the accumulator, so the producer loads the
+        // next tile's k-blocks while this runs, and a staging box is waited on only before it is rewritten.
+        auto reg_epilogue = [&](const float (&acc)[BN / 2]) {
+          const int rr = w.tile;   // (batch == 1 on this path)
+          const int m0 = (rr / p.tiles_n) * BM, n0 = (rr % p.tiles_n) * BN;
+          const int row0 = m0 + 16 * warp;   // this warp's first output row
+          const uint32_t stg = staging_base + (uint32_t)warp * 4096u;
+          auto emit = [&](const uint32_t (&pk)[16], const CUtensorMap* map, int col, bool tail) {
+            const uint32_t sbuf = stg + (store_cnt & 1u) * 2048u;
+            if (lane == 0) tma_store_wait_read<1>();
+            __syncwarp();
+            const int srow = (lane & 7) + (lane & 8);   // stmatrix: lanes 8i..8i+7 address the rows of matrix i
 #pragma unroll
-        for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
+            for (int jj = 0; jj < (tail ? 4 : 8); jj += 2) {
+              const int ch = jj + (lane >> 4);
+              const uint32_t addr = tail ? sbuf + (uint32_t)srow * 64u + (uint32_t)((ch ^ ((srow >> 1) & 3)) << 4)
+                                         : sbuf + (uint32_t)srow * 128u + (uint32_t)((ch ^ (srow & 7)) << 4);
+              stmatrix_x4(addr, pk[2 * jj], pk[2 * jj + 1], pk[2 * jj + 2], pk[2 * jj + 3]);
+            }
+            fence_proxy_async();
+            __syncwarp();
+            if (lane == 0) {
+              tma_store_2d(map, sbuf, col, row0);
+              tma_store_commit();
+            }
+            ++store_cnt;
+          };
+          auto pair_bf16 = [&](int j, int h) { return pack_bf16(acc[4 * j + 2 * h], acc[4 * j + 2 * h + 1]); };
+          if (p.epi == 1) {
+            // SwiGLU forward: tile columns [0,128) = gate, [128,256) = up of the same 128 hidden units; gate, up and
+            // act = bf16(bf16(silu(gate)) * up) -- the unfused swiglu_fwd_kernel's rounding points
+            if constexpr (BN == 256) {
+#pragma unroll
+              for (int i = 0; i < 2; ++i) {
+                uint32_t pk[16];
+#pragma unroll
+                for (int t = 0; t < 16; ++t) pk[t] = pair_bf16(8 * i + (t >> 1), t & 1);
+                emit(pk, &tmC, n0 + 64 * i, false);
+#pragma unroll
+                for (int t = 0; t < 16; ++t) pk[t] = pair_bf16(16 + 8 * i + (t >> 1), t & 1);
+                emit(pk, &tmC, n0 + 128 + 64 * i, false);
+#pragma unroll
+                for (int t = 0; t < 16; ++t) {
+                  const float2 gf = unpack_bf16(pair_bf16(8 * i + (t >> 1), t & 1));
+                  const float2 uf = unpack_bf16(pair_bf16(16 + 8 * i + (t >> 1), t & 1));
+                  const float2 sb = unpack_bf16(pack_bf16(silu_f(gf.x), silu_f(gf.y)));   // bf16(silu(g))
+                  pk[t] = pack_bf16(sb.x * uf.x, sb.y * uf.y);
+                }
+                emit(pk, &tmAux, (n0 >> 1) + 64 * i, false);
+              }
+            }
+          } else {
+            // plain convert; the 32-column tail chunk of a 224-wide tile leaves through tmAux
+#pragma unroll
+            for (int c2 = 0; c2 < (BN + 63) / 64; ++c2) {
+              const bool tail = BN % 64 != 0 && c2 == BN / 64;
+              if (n0 + 64 * c2 >= p.N) continue;
+              uint32_t pk[16];
+#pragma unroll
+              for (int t = 0; t < (tail ? 8 : 16); ++t) pk[t] = pair_bf16(8 * c2 + (t >> 1), t & 1);
+              emit(pk, tail ? &tmAux : &tmC, n0 + 64 * c2, tail);
+            }
+          }
+        };
+        auto mainloop_park = [&](float (&acc)[BN / 2]) {
+          const int k_iters = max(0, w.kb_end - w.kb_begin);
+          int prev = -1;
+          for (int kb = 0; kb < k_iters; ++kb) {
+            mbar_wait_nocall(full_bar(stage), phase);
+            wgmma_fence();
+            const uint32_t s_hi = smem_base + stage * stage_bytes;
+            // products per k-block: hi*hi, then (split mode) hi*lo and lo*hi
+            for (int g = 0; g < (split ? 3 : 1); ++g) {
+              // this warpgroup's rows: 64 K-major rows of 128 B, or the g-th 64-row MN atom -- 8 KB in both layouts
+              const uint32_t sA = s_hi + (g == 2 ? Cfg::STAGE_BYTES : 0) + (uint32_t)wg * 8192u;
+              const uint32_t sB = s_hi + Cfg::A_BYTES + (g == 1 ? Cfg::STAGE_BYTES : 0);
+#pragma unroll
+              for (int k = 0; k < BK / MMA_K; ++k) {
+                const uint64_t adesc = A_MN ? gmma_desc_sw128(sA + k * (MMA_K * 128), BK * 128, 1024)
+                                            : gmma_desc_sw128(sA + k * (MMA_K * 2), 16, 1024);
+                const uint64_t bdesc = B_MN ? gmma_desc_sw128(sB + k * (MMA_K * 128), BK * 128, 1024)
+                                            : gmma_desc_sw128(sB + k * (MMA_K * 2), 16, 1024);
+                wgmma_bf16<BN, A_MN ? 1 : 0, B_MN ? 1 : 0>(acc, adesc, bdesc);
+              }
+            }
+            wgmma_commit();
+            wgmma_wait<1>();            // the previous k-block's MMAs have retired: its slot can be refilled
+            if (prev >= 0 && lane == 0) mbar_arrive(empty_bar(prev));
+            prev = stage;
+            if (++stage == n_stage) { stage = 0; phase ^= 1u; }
+          }
+          wgmma_wait<0>();
+          if (prev >= 0 && lane == 0) mbar_arrive(empty_bar(prev));
+          if constexpr (!SK && EW == 4) {
+            if (p.reg_epi) {
+              reg_epilogue(acc);
+              return;
+            }
+          }
+          // every k-block of this tile has been consumed and the producer waits for acc_free: the ring is idle
+          named_bar_sync(1, 256);
+          acc_park<BN>(smem_base, acc, wg, warp & 3, lane);
+          named_bar_sync(1, 256);
+        };
         if (SK && w.role == 3) {
+          float acc[BN / 2];
           // carry-in: continue from the fp32 accumulator of the tile's first k-blocks (same member, previous group)
           const int src = (int)blockIdx.x - w.G;
           if (threadIdx.x == 0) {
@@ -528,40 +647,15 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
               acc[4 * j + 2 * h + 1] = v.y;
             }
           }
-        }
-        const int k_iters = max(0, w.kb_end - w.kb_begin);
-        int prev = -1;
-        for (int kb = 0; kb < k_iters; ++kb) {
-          mbar_wait_nocall(full_bar(stage), phase);
-          wgmma_fence();
-          const uint32_t s_hi = smem_base + stage * stage_bytes;
-          // products per k-block: hi*hi, then (split mode) hi*lo and lo*hi
-          for (int g = 0; g < (split ? 3 : 1); ++g) {
-            // this warpgroup's rows: 64 K-major rows of 128 B, or the g-th 64-row MN atom -- 8 KB in both layouts
-            const uint32_t sA = s_hi + (g == 2 ? Cfg::STAGE_BYTES : 0) + (uint32_t)wg * 8192u;
-            const uint32_t sB = s_hi + Cfg::A_BYTES + (g == 1 ? Cfg::STAGE_BYTES : 0);
+          mainloop_park(acc);
+        } else {
+          float acc[BN / 2];
 #pragma unroll
-            for (int k = 0; k < BK / MMA_K; ++k) {
-              const uint64_t adesc = A_MN ? gmma_desc_sw128(sA + k * (MMA_K * 128), BK * 128, 1024)
-                                          : gmma_desc_sw128(sA + k * (MMA_K * 2), 16, 1024);
-              const uint64_t bdesc = B_MN ? gmma_desc_sw128(sB + k * (MMA_K * 128), BK * 128, 1024)
-                                          : gmma_desc_sw128(sB + k * (MMA_K * 2), 16, 1024);
-              wgmma_bf16<BN, A_MN ? 1 : 0, B_MN ? 1 : 0>(acc, adesc, bdesc);
-            }
-          }
-          wgmma_commit();
-          wgmma_wait<1>();            // the previous k-block's MMAs have retired: its slot can be refilled
-          if (prev >= 0 && lane == 0) mbar_arrive(empty_bar(prev));
-          prev = stage;
-          if (++stage == n_stage) { stage = 0; phase ^= 1u; }
+          for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
+          mainloop_park(acc);
         }
-        wgmma_wait<0>();
-        if (prev >= 0 && lane == 0) mbar_arrive(empty_bar(prev));
-        // every k-block of this tile has been consumed and the producer waits for acc_free: the ring is idle
-        named_bar_sync(1, 256);
-        acc_park<BN>(smem_base, acc, wg, warp & 3, lane);
-        named_bar_sync(1, 256);
       }
+      if (!SK && p.reg_epi) continue;
       if (!epi_warp) {
         release_acc();
         continue;
@@ -1118,7 +1212,7 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
       }
       release_acc();
     }
-    if (epi_warp && p.tma_store && lane == 0) tma_store_wait<0>();   // all bulk stores retired before the CTA exits
+    if ((epi_warp || p.reg_epi) && p.tma_store && lane == 0) tma_store_wait<0>();   // all bulk stores retired before the CTA exits
   }
 }
 
@@ -1460,6 +1554,9 @@ int plan_gemm(const SkGemmEx& g, GemmParams& p, int& BN, int& ew, int& grid) {
   // convert-and-store epilogue is faster with 4 (fewer warps contending with the TMA / MMA issue threads)
   static const int ew_env = [] { const char* e = getenv("SK_GEMM_EW"); return e ? atoi(e) : 0; }();
   ew = (p.sk_units == 0 && BN == 256 && p.tma_store && (ew_env == 8 || (ew_env == 0 && (g.epi == 2 || g.epi == 3 || g.epi == 4 || g.epi == 5)))) ? 8 : 4;
+  // the register epilogue takes the one-pass TMA-store tiles whose epilogue reads no operand (plain convert and SwiGLU
+  // forward) on the 4-epilogue-warp kernels; the others keep the parked accumulator
+  p.reg_epi = (p.tma_store && p.sk_units == 0 && ew == 4 && !g.bias && !g.act && !g.residual && (g.epi == 0 || g.epi == 1)) ? 1 : 0;
   return 0;
 }
 
@@ -1510,20 +1607,23 @@ int sk_gemm_ex_launch(const SkGemmEx& g, cudaStream_t stream) {
     if (rc) return rc;
   }
   tm[4] = tm[0];
+  // store boxes: 16 rows (one warp's rows of the wgmma fragment) for the register epilogue, 32 rows (one parked-epilogue
+  // warp's quadrant) otherwise
+  const uint32_t box_rows = p.reg_epi ? 16 : 32;
   if (p.tma_store) {
     // epi 2 writes d_gu [M, 2N] (the accumulator tile is d_act [M, N])
-    const int rc2 = sk_make_tmap_2d(&tm[4], g.C, 2, (uint64_t)(g.epi == 2 ? 2 * g.N : g.N), (uint64_t)g.M, (uint64_t)g.ldc, 64, 32);
+    const int rc2 = sk_make_tmap_2d(&tm[4], g.C, 2, (uint64_t)(g.epi == 2 ? 2 * g.N : g.N), (uint64_t)g.M, (uint64_t)g.ldc, 64, box_rows);
     if (rc2) return rc2;
   }
   tm[5] = tm[4];
   if (g.epi == 1) {
-    const int rc3 = sk_make_tmap_2d(&tm[5], g.aux_out, 2, (uint64_t)g.N / 2, (uint64_t)g.M, (uint64_t)g.ld_aux_out, 64, 32);
+    const int rc3 = sk_make_tmap_2d(&tm[5], g.aux_out, 2, (uint64_t)g.N / 2, (uint64_t)g.M, (uint64_t)g.ld_aux_out, 64, box_rows);
     if (rc3) return rc3;
   } else if (g.epi == 4) {   // the GELU output, same shape as C
     const int rc3 = sk_make_tmap_2d(&tm[5], g.aux_out, 2, (uint64_t)g.N, (uint64_t)g.M, (uint64_t)g.ld_aux_out, 64, 32);
     if (rc3) return rc3;
   } else if (p.tma_store && BN % 64 != 0) {   // the 32-column tail chunk of a 224-wide tile
-    const int rc3 = sk_make_tmap_2d(&tm[5], g.C, 2, (uint64_t)g.N, (uint64_t)g.M, (uint64_t)g.ldc, 32, 32);
+    const int rc3 = sk_make_tmap_2d(&tm[5], g.C, 2, (uint64_t)g.N, (uint64_t)g.M, (uint64_t)g.ldc, 32, box_rows);
     if (rc3) return rc3;
   }
   int rc;
