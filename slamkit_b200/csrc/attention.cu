@@ -5,8 +5,8 @@
 // with P / dS is one wgmma.mma_async chain (m64n64k16 bf16, fp32 accumulate).  Operand tiles are staged by cp.async
 // (double-buffered) into 1024-byte-aligned [rows][64] bf16 tiles in the 128B-swizzled layout wgmma reads directly;
 // P and dS stay in registers and feed the next product as the register A operand.  S/P never touch HBM; the backward
-// is split in two deterministic kernels (dK/dV per key tile looping over the GQA group, dQ per query tile) so no atomics
-// are needed.
+// has two deterministic parts (dK/dV per key tile looping over the GQA group, dQ per query tile) so no atomics are
+// needed; they share one launch, so dQ tiles fill the SMs while the long dK/dV tiles run.
 //
 // Packed batches: with seg_start (int32 [B*T], in-row index of the first token of each token's document) the causal
 // kernels mask keys before the query's document start -- block-diagonal causal attention.
@@ -82,6 +82,34 @@ SK_DEVINL void wg_p_b(float (&acc)[8][4], const uint32_t (&p)[4][4], uint32_t sB
   wgmma_fence();
 #pragma unroll
   for (int kk = 0; kk < 4; ++kk) wgmma_m64n64_rs(d, p[kk], gmma_desc_sw128(sB + kk * 2048, 8192, 1024));
+  wgmma_commit();
+  wgmma_wait<0>();
+}
+
+// Two independent products issued back to back and waited on once; each accumulator sees its MMAs in the order two
+// separate calls would issue them, so the results are those of wg_a_bT / wg_p_b.
+SK_DEVINL void wg_a_bT2(float (&acc1)[8][4], uint32_t sA1, uint32_t sB1, float (&acc2)[8][4], uint32_t sA2, uint32_t sB2) {
+  float(&d1)[32] = reinterpret_cast<float(&)[32]>(acc1);
+  float(&d2)[32] = reinterpret_cast<float(&)[32]>(acc2);
+  wgmma_fence();
+#pragma unroll
+  for (int ks = 0; ks < 4; ++ks)
+    wgmma_m64n64<0, 0>(d1, gmma_desc_sw128(sA1 + ks * 32, 16, 1024), gmma_desc_sw128(sB1 + ks * 32, 16, 1024));
+#pragma unroll
+  for (int ks = 0; ks < 4; ++ks)
+    wgmma_m64n64<0, 0>(d2, gmma_desc_sw128(sA2 + ks * 32, 16, 1024), gmma_desc_sw128(sB2 + ks * 32, 16, 1024));
+  wgmma_commit();
+  wgmma_wait<0>();
+}
+SK_DEVINL void wg_p_b2(float (&acc1)[8][4], const uint32_t (&p1)[4][4], uint32_t sB1, float (&acc2)[8][4],
+                       const uint32_t (&p2)[4][4], uint32_t sB2) {
+  float(&d1)[32] = reinterpret_cast<float(&)[32]>(acc1);
+  float(&d2)[32] = reinterpret_cast<float(&)[32]>(acc2);
+  wgmma_fence();
+#pragma unroll
+  for (int kk = 0; kk < 4; ++kk) wgmma_m64n64_rs(d1, p1[kk], gmma_desc_sw128(sB1 + kk * 2048, 8192, 1024));
+#pragma unroll
+  for (int kk = 0; kk < 4; ++kk) wgmma_m64n64_rs(d2, p2[kk], gmma_desc_sw128(sB2 + kk * 2048, 8192, 1024));
   wgmma_commit();
   wgmma_wait<0>();
 }
@@ -419,23 +447,21 @@ __global__ void attn_delta_kernel(const bf16* __restrict__ o, const bf16* __rest
 }
 
 // ------------------------------------------------------------------------------------------------
-// backward dK/dV: one CTA per (64-key tile, kv head, batch); 4 warps x 16 keys; loops over the GQA group's query
+// backward dK/dV: one CTA per (64-key tile kt, kv head g, batch b); 4 warps x 16 keys; loops over the GQA group's query
 // heads and their query tiles.  Works on transposed score tiles S^T = K Q^T so P^T/dS^T are directly A operands.
 // ------------------------------------------------------------------------------------------------
 template <bool CAUSAL>
-__global__ void __launch_bounds__(128, 3)
-attn_bwd_dkdv_kernel(const bf16* __restrict__ q, const bf16* __restrict__ k, const bf16* __restrict__ v,
-                     const bf16* __restrict__ d_o, const float* __restrict__ lse, const float* __restrict__ delta,
-                     bf16* __restrict__ dk, bf16* __restrict__ dv, int T, int ld, int ldo, int ldg, int H, int group,
-                     float scale, const int* __restrict__ seg_start) {
+SK_DEVINL void attn_bwd_dkdv_tile(const bf16* __restrict__ q, const bf16* __restrict__ k, const bf16* __restrict__ v,
+                                  const bf16* __restrict__ d_o, const float* __restrict__ lse,
+                                  const float* __restrict__ delta, bf16* __restrict__ dk, bf16* __restrict__ dv, int T,
+                                  int ld, int ldo, int ldg, int H, int group, float scale,
+                                  const int* __restrict__ seg_start, int kt, int g, int b) {
   extern __shared__ __align__(128) uint8_t smem_attn[];
   const uint32_t sKV = smem_base_1k(smem_attn);        // K tile then V tile (each 8 KB)
   const uint32_t sQ = sKV + 2 * 8192;                  // 2 stages
   const uint32_t sdO = sQ + 2 * 8192;                  // 2 stages
   float* sStat = reinterpret_cast<float*>(smem_attn + (sKV - smem_u32(smem_attn)) + 6 * 8192);  // [2 stages][2 (lse, delta)][64]
   int* sSeg = reinterpret_cast<int*>(sStat + 2 * 2 * 64);          // [2 stages][64] document start of each query row
-  const int b = blockIdx.z, g = blockIdx.y;
-  const int kt = blockIdx.x;  // tile 0 has the most work under the causal mask and is scheduled first
   const int k0 = kt * 64;
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const float sl2 = scale * 1.4426950408889634f;
@@ -489,8 +515,10 @@ attn_bwd_dkdv_kernel(const bf16* __restrict__ q, const bf16* __restrict__ k, con
     const float* s_del = sStat + (st * 2 + 1) * 64;
 
     float st_acc[8][4];  // S^T tile: rows = keys (this warp's 16), cols = 64 query rows
+    float dp[8][4];      // dP^T = V dO^T
     zero_acc(st_acc);
-    wg_a_bT(st_acc, sKV, sQ + st * 8192);
+    zero_acc(dp);
+    wg_a_bT2(st_acc, sKV, sQ + st * 8192, dp, sKV + 8192, sdO + st * 8192);
     const int* s_seg = sSeg + st * 64;
     const bool need_mask = (CAUSAL && (q0 < k0 + 64)) || (q0 + 64 > T) || (k0 + 64 > T) || seg_start;
 #pragma unroll
@@ -505,25 +533,13 @@ attn_bwd_dkdv_kernel(const bf16* __restrict__ q, const bf16* __restrict__ k, con
           if (qrow >= T || key >= T || (CAUSAL && key > qrow) || key < s_seg[qi]) pv = 0.f;
         }
         st_acc[nt][e] = pv;
+        dp[nt][e] = pv * (dp[nt][e] - s_del[qi]) * scale;  // dS^T
       }
     }
-    uint32_t pa[4][4];
+    uint32_t pa[4][4], dsa[4][4];
     acc_to_a(st_acc, pa);
-    wg_p_b(dvacc, pa, sdO + st * 8192);  // dV += P^T dO
-
-    float dp[8][4];
-    zero_acc(dp);
-    wg_a_bT(dp, sKV + 8192, sdO + st * 8192);  // dP^T = V dO^T
-#pragma unroll
-    for (int nt = 0; nt < 8; ++nt) {
-#pragma unroll
-      for (int e = 0; e < 4; ++e) {
-        const int qi = nt * 8 + (lane & 3) * 2 + (e & 1);
-        dp[nt][e] = st_acc[nt][e] * (dp[nt][e] - s_del[qi]) * scale;  // dS^T
-      }
-    }
-    acc_to_a(dp, pa);
-    wg_p_b(dkacc, pa, sQ + st * 8192);  // dK += dS^T Q
+    acc_to_a(dp, dsa);
+    wg_p_b2(dvacc, pa, sdO + st * 8192, dkacc, dsa, sQ + st * 8192);  // dV += P^T dO, dK += dS^T Q
     __syncthreads();
   }
 #pragma unroll
@@ -542,20 +558,17 @@ attn_bwd_dkdv_kernel(const bf16* __restrict__ q, const bf16* __restrict__ k, con
 }
 
 // ------------------------------------------------------------------------------------------------
-// backward dQ: one CTA per (64-row query tile, head, batch); loops over key tiles up to the diagonal
+// backward dQ: one CTA per (64-row query tile qt, head h, batch b); loops over key tiles up to the diagonal
 // ------------------------------------------------------------------------------------------------
 template <bool CAUSAL>
-__global__ void __launch_bounds__(128)
-attn_bwd_dq_kernel(const bf16* __restrict__ q, const bf16* __restrict__ k, const bf16* __restrict__ v,
-                   const bf16* __restrict__ d_o, const float* __restrict__ lse, const float* __restrict__ delta,
-                   bf16* __restrict__ dq, int T, int ld, int ldo, int ldg, int H, int group, float scale,
-                   const int* __restrict__ seg_start) {
+SK_DEVINL void attn_bwd_dq_tile(const bf16* __restrict__ q, const bf16* __restrict__ k, const bf16* __restrict__ v,
+                                const bf16* __restrict__ d_o, const float* __restrict__ lse,
+                                const float* __restrict__ delta, bf16* __restrict__ dq, int T, int ld, int ldo, int ldg,
+                                int H, int group, float scale, const int* __restrict__ seg_start, int qt, int h, int b) {
   extern __shared__ __align__(128) uint8_t smem_attn[];
   const uint32_t sQdO = smem_base_1k(smem_attn);  // Q tile, dO tile
   const uint32_t sK = sQdO + 2 * 8192;        // 2 stages
   const uint32_t sV = sK + 2 * 8192;          // 2 stages
-  const int b = blockIdx.z, h = blockIdx.y;
-  const int qt = gridDim.x - 1 - blockIdx.x;
   const int q0 = qt * 64;
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const float sl2 = scale * 1.4426950408889634f;
@@ -640,10 +653,37 @@ attn_bwd_dq_kernel(const bf16* __restrict__ q, const bf16* __restrict__ k, const
   }
 }
 
+// ------------------------------------------------------------------------------------------------
+// backward: the dK/dV tiles (blocks [0, n_dkdv)) and the dQ tiles (the rest) in one grid.  Under the causal mask key
+// tile 0 loops over every query tile of the group, a chain far longer than the others; in one launch the dQ tiles run
+// beside it instead of after it.  Both parts go heaviest first: key tiles ascending, then query tiles descending.
+// Each output element is computed exactly as by two separate kernels.
+// ------------------------------------------------------------------------------------------------
+template <bool CAUSAL>
+__global__ void __launch_bounds__(128, 3)
+attn_bwd_kernel(const bf16* __restrict__ q, const bf16* __restrict__ k, const bf16* __restrict__ v,
+                const bf16* __restrict__ d_o, const float* __restrict__ lse, const float* __restrict__ delta,
+                bf16* __restrict__ dq, bf16* __restrict__ dk, bf16* __restrict__ dv, int B, int T, int ld, int ldo,
+                int ldg, int H, int KVH, float scale, const int* __restrict__ seg_start) {
+  const int group = H / KVH;
+  const int n_dkdv = (T + 63) / 64 * KVH * B;
+  int i = blockIdx.x;
+  if (i < n_dkdv) {
+    attn_bwd_dkdv_tile<CAUSAL>(q, k, v, d_o, lse, delta, dk, dv, T, ld, ldo, ldg, H, group, scale, seg_start,
+                               i / (KVH * B), i % KVH, i / KVH % B);
+  } else {
+    i -= n_dkdv;
+    const int n_qt = (T + 63) / 64;
+    attn_bwd_dq_tile<CAUSAL>(q, k, v, d_o, lse, delta, dq, T, ld, ldo, ldg, H, group, scale, seg_start,
+                             n_qt - 1 - i / (H * B), i % H, i / H % B);
+  }
+}
+
 // +1024: the tiles start at the first 1024-byte boundary of the dynamic shared memory
 constexpr int FWD_SMEM = 128 * 128 + 4 * 8192 + 1024;        // 48 KB
 constexpr int DKDV_SMEM = 6 * 8192 + 2 * 2 * 64 * 4 + 2 * 64 * 4 + 1024;  // 48 KB + stats + document starts
 constexpr int DQ_SMEM = 6 * 8192 + 1024;
+constexpr int BWD_SMEM = DKDV_SMEM > DQ_SMEM ? DKDV_SMEM : DQ_SMEM;
 constexpr int FWD_SPLIT_SMEM = 2 * 128 * 128 + 8 * 8192 + 1024;  // 96 KB
 
 template <typename K>
@@ -686,29 +726,22 @@ int sk_attn_bwd_launch(const bf16* q, const bf16* k, const bf16* v, const bf16* 
   SK_REQUIRE(ld % 8 == 0 && ldo % 8 == 0 && ldg % 2 == 0, "attention: ld and ldo must be multiples of 8 and ldg even");
   static bool init = false;
   if (!init) {
-    if (set_smem(attn_bwd_dkdv_kernel<true>, DKDV_SMEM)) return -2;
-    if (set_smem(attn_bwd_dkdv_kernel<false>, DKDV_SMEM)) return -2;
-    if (set_smem(attn_bwd_dq_kernel<true>, DQ_SMEM)) return -2;
-    if (set_smem(attn_bwd_dq_kernel<false>, DQ_SMEM)) return -2;
+    if (set_smem(attn_bwd_kernel<true>, BWD_SMEM)) return -2;
+    if (set_smem(attn_bwd_kernel<false>, BWD_SMEM)) return -2;
     init = true;
   }
+  const long n_blocks = (long)(T + 63) / 64 * (KVH + H) * B;   // dK/dV tiles, then dQ tiles
+  SK_REQUIRE(n_blocks <= 0x7fffffffL, "attention: grid of %ld blocks too large", n_blocks);
   const long total = (long)B * T * H * 8;
   sk_prof_begin(1, s);
   SK_CUDA_CHECK(sk_launch_pdl(attn_delta_kernel, dim3((int)((total + 255) / 256)), dim3(256), (size_t)(0), s, o, d_o, delta, B, T, H, ldo));
   SK_LAUNCH_CHECK();
-  const int group = H / KVH;
-  dim3 g1((T + 63) / 64, KVH, B), g2((T + 63) / 64, H, B);
-  if (causal) {
-    attn_bwd_dkdv_kernel<true><<<g1, 128, DKDV_SMEM, s>>>(q, k, v, d_o, lse, delta, dk, dv, T, ld, ldo, ldg, H, group, scale,
-                                                          seg_start);
-    SK_LAUNCH_CHECK();
-    attn_bwd_dq_kernel<true><<<g2, 128, DQ_SMEM, s>>>(q, k, v, d_o, lse, delta, dq, T, ld, ldo, ldg, H, group, scale, seg_start);
-  } else {
-    attn_bwd_dkdv_kernel<false><<<g1, 128, DKDV_SMEM, s>>>(q, k, v, d_o, lse, delta, dk, dv, T, ld, ldo, ldg, H, group, scale,
-                                                           nullptr);
-    SK_LAUNCH_CHECK();
-    attn_bwd_dq_kernel<false><<<g2, 128, DQ_SMEM, s>>>(q, k, v, d_o, lse, delta, dq, T, ld, ldo, ldg, H, group, scale, nullptr);
-  }
+  if (causal)
+    attn_bwd_kernel<true><<<(unsigned)n_blocks, 128, BWD_SMEM, s>>>(q, k, v, d_o, lse, delta, dq, dk, dv, B, T, ld, ldo, ldg,
+                                                                    H, KVH, scale, seg_start);
+  else
+    attn_bwd_kernel<false><<<(unsigned)n_blocks, 128, BWD_SMEM, s>>>(q, k, v, d_o, lse, delta, dq, dk, dv, B, T, ld, ldo,
+                                                                     ldg, H, KVH, scale, nullptr);
   sk_prof_end(s);
   SK_LAUNCH_CHECK();
   return 0;
