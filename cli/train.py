@@ -135,7 +135,8 @@ def build_model(cfg, device: str, max_batch: int, max_seq: int):
     args = cfg.model.config_args
     try:
         from slamkit_b200.integration import tlm_b200_from_cfg
-        return tlm_b200_from_cfg(to_container(cfg.model), device=device, max_batch=max_batch, max_seq=max_seq)
+        return tlm_b200_from_cfg(to_container(cfg.model), device=device, max_batch=max_batch, max_seq=max_seq,
+                                 autocast_bf16=cfg.training_args.get("bf16"))
     except OSError as e:       # HF hub / local path lookup failures are OSErrors; anything else is a real error
         if args.get("twist_init", True):
             raise RuntimeError(f"base model '{args.base_model_name}' is unreachable and twist_init=true needs its weights "

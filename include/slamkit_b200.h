@@ -239,6 +239,24 @@ int sk_grad_norm(const void* grads, const int64_t* chunk_start, const int32_t* c
 /* One fused pass over the flat parameter buffer (14 B/param). clip_stats: the stats buffer of sk_grad_norm or NULL. */
 int sk_adamw_step(void* params, const void* grads, void* exp_avg, void* exp_avg_sq, int64_t n, float lr, float beta1,
                   float beta2, float eps, float weight_decay, int step, const float* clip_stats, void* stream);
+/* fp32 master weights (see sk_lm_set_master).  sk_grad_norm_f32: sk_grad_norm over fp32 gradients, fp32 throughout (no
+ * bf16 rounding).  sk_adamw_master_step: AdamW on fp32 params / grads / moments (n a multiple of 8, 16-byte aligned)
+ * with torch's fp32 element arithmetic, each operation rounded once; 1 - beta, lr * weight_decay, lr / (1 - beta1^step)
+ * and sqrt(1 - beta2^step) are formed in double from the fp32 arguments; also writes shadow = bf16(params) [n]. */
+int sk_grad_norm_f32(const float* grads, const int64_t* chunk_start, const int32_t* chunk_len, int n_chunks,
+                     const int32_t* tensor_chunk_begin, int n_tensors, float* partial, float max_norm, float* stats, void* stream);
+int sk_adamw_master_step(float* params, void* shadow, const float* grads, float* exp_avg, float* exp_avg_sq, int64_t n, float lr,
+                         float beta1, float beta2, float eps, float weight_decay, int step, const float* clip_stats, void* stream);
+/* OPT master weights: residual add + LayerNorm on fp32 rows, one warp per row (D a multiple of 8, <= 2048):
+ * xo = x + float(y) (y bf16 [M, D] or NULL: no add, xo unused), h = bf16(LN(xo) * w + b) with fp32 w, b; mean / rstd
+ * fp32 [M] (may be NULL).  Backward: dres_out = dres_in + LN'(float(dy) * w) in fp32 (dres_in NULL reads zeros; may
+ * alias dres_out), dres16 = bf16(dres_out), dw / db fp32 [D] (+)= (accumulate) through partial fp32
+ * [2 * sk_layernorm_bwd_blocks() * D] in a fixed order. */
+int sk_add_layernorm_f32(const float* x, const void* y, const float* w, const float* b, float* xo, void* h, float* mean, float* rstd,
+                         int M, int D, float eps, void* stream);
+int sk_layernorm_bwd_f32(const void* dy, const float* x, const float* w, const float* mean, const float* rstd, const float* dres_in,
+                         float* dres_out, void* dres16, float* dw, float* db, float* partial, int M, int D, int accumulate,
+                         void* stream);
 
 /* ---- causal-LM train step (path (ii)) ---------------------------------------------------------------------------
  * One object per model replica; replaces UnitLM.forward + compute_loss + autograd backward
@@ -319,6 +337,21 @@ int64_t sk_lm_workspace_bytes(const SkLm* lm, int B, int T);
  * workspace >= sk_lm_workspace_bytes(B,T) for the largest (B,T) used. */
 int sk_lm_bind(SkLm* lm, void* params, void* grads, const void* rope_cos, const void* rope_sin, void* workspace,
                int64_t workspace_bytes);
+/* OPT handles only, after sk_lm_bind: train fp32 master weights, as HF OPTForCausalLM with fp32 parameters runs under
+ * torch.autocast(bfloat16) (the reference's default recipe, torch_dtype null and bf16: true).  params32 / grads32 are
+ * caller-owned flat fp32 [param_count] buffers in the bf16 layout (grads32 may be NULL for a forward-only handle); the
+ * bound bf16 `params` become the shadow bf16(params32) that the GEMMs read (the caller fills it once; the optimiser step
+ * rewrites it), the bound bf16 `grads` the per-micro-batch scratch of the linear gradients.  From then on:
+ *   - the residual stream is fp32: x0 = E[id] + P[pos + 2] from the fp32 tables, x += float(bf16 branch output), every
+ *     LayerNorm reads fp32 x, gamma, beta and rounds its output once to bf16 for the next linear;
+ *   - sk_lm_forward_backward accumulates into grads32: linear weight / bias gradients are computed in bf16 and widened,
+ *     LayerNorm and table gradients are fp32, the residual gradient is fp32 (its bf16 copy feeds the GEMMs);
+ *   - sk_lm_optimizer_step takes fp32 exp_avg / exp_avg_sq, clips over the fp32 grads32 (emulate_bf16_norm is ignored)
+ *     and writes params32, the moments and the bf16 shadow;
+ *   - sk_lm_workspace_bytes reports the larger fp32-residual workspace: bind it again before the next forward pass;
+ *   - sk_lm_prefill / sk_lm_decode_step refuse the handle (generation runs on the saved checkpoint).
+ * Qwen2 and GPT-NeoX handles are refused. */
+int sk_lm_set_master(SkLm* lm, float* params32, float* grads32);
 /* Forward only (eval / log-likelihood): logits stay in the workspace, see sk_lm_logits. labels may be NULL.
  * pos_ids: int32 [B*T] or NULL (positions 0..T-1 per row).  When given they drive RoPE AND mark packed documents: a
  * document starts wherever pos_ids == 0, and tokens attend only within their document (the reference's varlen

@@ -315,6 +315,28 @@ int sk_grad_norm(const void* grads, const int64_t* chunk_start, const int32_t* c
   return sk_gradnorm_launch(CBF(grads), reinterpret_cast<const long*>(chunk_start), chunk_len, n_chunks,
                             tensor_chunk_begin, n_tensors, partial, max_norm, emulate_bf16, stats, S(stream));
 }
+int sk_add_layernorm_f32(const float* x, const void* y, const float* w, const float* b, float* xo, void* h, float* mean, float* rstd,
+                        int M, int D, float eps, void* stream) {
+  SK_REQUIRE(x && w && b && h, "sk_add_layernorm_f32: null argument");
+  return sk_add_layernorm_f32_launch(x, CBF(y), w, b, xo, BF(h), mean, rstd, M, D, eps, S(stream));
+}
+int sk_layernorm_bwd_f32(const void* dy, const float* x, const float* w, const float* mean, const float* rstd, const float* dres_in,
+                         float* dres_out, void* dres16, float* dw, float* db, float* partial, int M, int D, int accumulate,
+                         void* stream) {
+  SK_REQUIRE(dy && x && w && mean && rstd && dres_out && dres16 && dw && db && partial, "sk_layernorm_bwd_f32: null argument");
+  return sk_layernorm_bwd_f32_launch(CBF(dy), x, w, mean, rstd, dres_in, dres_out, BF(dres16), dw, db, partial, M, D, accumulate,
+                                     S(stream));
+}
+int sk_grad_norm_f32(const float* grads, const int64_t* chunk_start, const int32_t* chunk_len, int n_chunks,
+                     const int32_t* tensor_chunk_begin, int n_tensors, float* partial, float max_norm, float* stats, void* stream) {
+  return sk_gradnorm_f32_launch(grads, reinterpret_cast<const long*>(chunk_start), chunk_len, n_chunks, tensor_chunk_begin,
+                                n_tensors, partial, max_norm, stats, S(stream));
+}
+int sk_adamw_master_step(float* params, void* shadow, const float* grads, float* exp_avg, float* exp_avg_sq, int64_t n, float lr,
+                         float beta1, float beta2, float eps, float weight_decay, int step, const float* clip_stats, void* stream) {
+  return sk_adamw_master_launch(params, BF(shadow), grads, exp_avg, exp_avg_sq, (long)n, lr, beta1, beta2, eps, weight_decay, step,
+                                clip_stats, S(stream));
+}
 int sk_adamw_step(void* params, const void* grads, void* exp_avg, void* exp_avg_sq, int64_t n, float lr, float beta1,
                   float beta2, float eps, float weight_decay, int step, const float* clip_stats, void* stream) {
   return sk_adamw_launch(BF(params), CBF(grads), BF(exp_avg), BF(exp_avg_sq), (long)n, lr, beta1, beta2, eps,

@@ -118,6 +118,26 @@ int sk_opt_embed_fwd_launch(const int64_t* ids, const int32_t* pos_ids, const bf
 int sk_opt_pos_bwd_launch(const int32_t* pos_ids, const bf16* dx, float* scratch, bf16* dP, int M, int T, int D, int n_pos,
                           int accumulate, cudaStream_t s);
 int sk_relu_bwd_launch(bf16* g, const bf16* a, long n, cudaStream_t s);
+// OPT with fp32 master weights (autocast numerics): the fp32 embedding sum, the fused residual add + LayerNorm of the
+// fp32 residual stream, its backward into an fp32 residual gradient (plus a bf16 copy) with fp32 dw / db (partial:
+// 2 x sk_layernorm_bwd_blocks() x D floats), table gradients from fp32 rows into fp32, the widening of bf16 linear
+// gradients into the fp32 gradient buffer, the fp32 gradient norm and AdamW on the fp32 masters
+int sk_opt_embed_fwd_f32_launch(const int64_t* ids, const int32_t* pos_ids, const float* E, const float* P, float* out, int M,
+                                int T, int D, int V, int n_pos, cudaStream_t s);
+int sk_add_layernorm_f32_launch(const float* x, const bf16* y, const float* w, const float* b, float* xo, bf16* h, float* mean,
+                                float* rstd, int M, int D, float eps, cudaStream_t s);
+int sk_layernorm_bwd_f32_launch(const bf16* dy, const float* x, const float* w, const float* mean, const float* rstd,
+                                const float* dres_in, float* dres_out, bf16* dres16, float* dw, float* db, float* partial, int M,
+                                int D, int accumulate, cudaStream_t s);
+int sk_table_bwd_f32_launch(const int64_t* ids, const int32_t* pos_ids, const float* dx, float* scratch, float* dtable,
+                            const bf16* head, int M, int T, int D, int n_rows, int n_rows_padded, int keep, cudaStream_t s);
+int sk_widen_grads_launch(const bf16* g16, float* g32, const long* chunk_start, const int* chunk_len, int n_chunks, int keep,
+                          cudaStream_t s);
+int sk_gradnorm_f32_launch(const float* g, const long* chunk_start, const int* chunk_len, int n_chunks,
+                           const int* tensor_chunk_begin, int n_tensors, float* partial, float max_norm, float* stats_out,
+                           cudaStream_t s);
+int sk_adamw_master_launch(float* p, bf16* shadow, const float* g, float* m, float* v, long n, float lr, float beta1, float beta2,
+                           float eps, float wd, int step, const float* clip_stats, cudaStream_t s);
 // GPT-NeoX parallel residual: ln1(x) and ln2(x) from one read of x (shared fp32 mean / rstd), and the fused backward
 // dx = dres + LN'(w1 * dy1 + w2 * dy2) with the four deterministic parameter gradients (partial: 4 x
 // sk_layernorm_bwd_blocks() x D floats)

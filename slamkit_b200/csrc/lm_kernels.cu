@@ -232,10 +232,16 @@ rmsnorm_bwd_kernel(const bf16* __restrict__ dy, const bf16* __restrict__ x, cons
   }
 }
 
-// out[j] = bf16( (accumulate ? out[j] : 0) + sum_b partial[b][j] ).  Block = 32 columns x 32 row groups (1024 threads);
+SK_DEVINL float to_f32(bf16 v) { return __bfloat162float(v); }
+SK_DEVINL float to_f32(float v) { return v; }
+SK_DEVINL void store_f32(bf16* p, float v) { *p = __float2bfloat16_rn(v); }
+SK_DEVINL void store_f32(float* p, float v) { *p = v; }
+
+// out[j] = OutT( (accumulate ? out[j] : 0) + sum_b partial[b][j] ).  Block = 32 columns x 32 row groups (1024 threads);
 // every thread sums a fixed strided subset of rows, then a fixed-order tree over the 32 groups (deterministic).
+template <typename OutT>
 __global__ void __launch_bounds__(1024)
-colsum_reduce_kernel(const float* __restrict__ partial, bf16* __restrict__ out, int nblocks, int D, int accumulate) {
+colsum_reduce_kernel(const float* __restrict__ partial, OutT* __restrict__ out, int nblocks, int D, int accumulate) {
   griddep_launch();
   griddep_wait();
   __shared__ float sred[32][33];
@@ -253,8 +259,8 @@ colsum_reduce_kernel(const float* __restrict__ partial, bf16* __restrict__ out, 
   }
   if (rg == 0 && j < D) {
     float t = sred[0][c];
-    if (accumulate) t += __bfloat162float(out[j]);
-    out[j] = __float2bfloat16_rn(t);
+    if (accumulate) t += to_f32(out[j]);
+    store_f32(out + j, t);
   }
 }
 
@@ -620,25 +626,34 @@ __global__ void scale_by_inv_count_kernel(bf16* __restrict__ x, long n, const fl
 // ------------------------------------------------------------------------------------------------
 // gradient norm (torch.nn.utils.clip_grad_norm_ semantics on bf16 grads) + fused AdamW
 // ------------------------------------------------------------------------------------------------
+// acc += the squares of one 16-byte vector of gradients (pairwise for bf16, as the bf16 path has always summed them)
+SK_DEVINL void add_sq16(float& acc, const uint4 v, const bf16*) {
+  const uint32_t u[4] = {v.x, v.y, v.z, v.w};
+#pragma unroll
+  for (int k = 0; k < 4; ++k) {
+    const float2 f = unpack_bf16(u[k]);
+    acc += f.x * f.x + f.y * f.y;
+  }
+}
+SK_DEVINL void add_sq16(float& acc, const uint4 v, const float*) {
+  const float f[4] = {__uint_as_float(v.x), __uint_as_float(v.y), __uint_as_float(v.z), __uint_as_float(v.w)};
+#pragma unroll
+  for (int k = 0; k < 4; ++k) acc += f[k] * f[k];
+}
+
 // chunk c covers grads[chunk_start[c] .. +chunk_len[c]) and never straddles a tensor; partial[c] = sum of squares
-__global__ void sumsq_chunks_kernel(const bf16* __restrict__ g, const long* __restrict__ chunk_start,
+template <typename T>
+__global__ void sumsq_chunks_kernel(const T* __restrict__ g, const long* __restrict__ chunk_start,
                                     const int* __restrict__ chunk_len, float* __restrict__ partial) {
   __shared__ float sred[32];
+  constexpr int VEC = 16 / sizeof(T);
   const long s = chunk_start[blockIdx.x];
   const int n = chunk_len[blockIdx.x];
   float acc = 0.f;
-  const int nvec = n / 8;
-  for (int i = threadIdx.x; i < nvec; i += blockDim.x) {
-    const uint4 v = ldg128_stream(g + s + (long)i * 8);
-    const uint32_t u[4] = {v.x, v.y, v.z, v.w};
-#pragma unroll
-    for (int k = 0; k < 4; ++k) {
-      const float2 f = unpack_bf16(u[k]);
-      acc += f.x * f.x + f.y * f.y;
-    }
-  }
-  for (int i = nvec * 8 + threadIdx.x; i < n; i += blockDim.x) {
-    const float f = __bfloat162float(g[s + i]);
+  const int nvec = n / VEC;
+  for (int i = threadIdx.x; i < nvec; i += blockDim.x) add_sq16(acc, ldg128_stream(g + s + (long)i * VEC), g);
+  for (int i = nvec * VEC + threadIdx.x; i < n; i += blockDim.x) {
+    const float f = to_f32(g[s + i]);
     acc += f * f;
   }
   acc = warp_sum(acc);
@@ -829,7 +844,7 @@ int sk_rmsnorm_bwd_launch(const bf16* dy, const bf16* x, const bf16* w, const fl
   const size_t smem = (size_t)WARPS_PER_BLOCK * D * sizeof(float);
   SK_CUDA_CHECK(sk_launch_pdl(rmsnorm_bwd_kernel, dim3(blocks), dim3(WARPS_PER_BLOCK * 32), (size_t)(smem), s, dy, x, w, rstd, dres, dx, dw_partial, M, D));
   SK_LAUNCH_CHECK();
-  SK_CUDA_CHECK(sk_launch_pdl(colsum_reduce_kernel, dim3((D + 31) / 32), dim3(1024), (size_t)(0), s, dw_partial, dw, blocks, D, accumulate_dw));
+  SK_CUDA_CHECK(sk_launch_pdl(colsum_reduce_kernel<bf16>, dim3((D + 31) / 32), dim3(1024), (size_t)(0), s, dw_partial, dw, blocks, D, accumulate_dw));
   SK_LAUNCH_CHECK();
   return 0;
 }
@@ -840,7 +855,7 @@ int sk_colsum_launch(const bf16* x, bf16* out, float* partial, int M, int N, int
   dim3 grid((N / 8 + 127) / 128, COLSUM_SPLITS);
   SK_CUDA_CHECK(sk_launch_pdl(colsum_partial_kernel, dim3(grid), dim3(128), (size_t)(0), s, x, partial, M, N, ld));
   SK_LAUNCH_CHECK();
-  SK_CUDA_CHECK(sk_launch_pdl(colsum_reduce_kernel, dim3((N + 31) / 32), dim3(1024), (size_t)(0), s, partial, out, COLSUM_SPLITS, N, accumulate));
+  SK_CUDA_CHECK(sk_launch_pdl(colsum_reduce_kernel<bf16>, dim3((N + 31) / 32), dim3(1024), (size_t)(0), s, partial, out, COLSUM_SPLITS, N, accumulate));
   SK_LAUNCH_CHECK();
   return 0;
 }
@@ -916,6 +931,16 @@ int sk_gradnorm_launch(const bf16* g, const long* chunk_start, const int* chunk_
   sumsq_chunks_kernel<<<n_chunks, 256, 0, s>>>(g, chunk_start, chunk_len, partial);
   SK_LAUNCH_CHECK();
   gradnorm_finalize_kernel<<<1, 256, 0, s>>>(partial, tensor_chunk_begin, n_tensors, max_norm, emulate_bf16, stats_out);
+  SK_LAUNCH_CHECK();
+  return 0;
+}
+// fp32 gradients: per-tensor fp32 norms and their fp32 norm, no bf16 rounding anywhere (clip_grad_norm_ on fp32 .grad)
+int sk_gradnorm_f32_launch(const float* g, const long* chunk_start, const int* chunk_len, int n_chunks,
+                           const int* tensor_chunk_begin, int n_tensors, float* partial, float max_norm, float* stats_out,
+                           cudaStream_t s) {
+  sumsq_chunks_kernel<<<n_chunks, 256, 0, s>>>(g, chunk_start, chunk_len, partial);
+  SK_LAUNCH_CHECK();
+  gradnorm_finalize_kernel<<<1, 256, 0, s>>>(partial, tensor_chunk_begin, n_tensors, max_norm, 0, stats_out);
   SK_LAUNCH_CHECK();
   return 0;
 }
@@ -1239,9 +1264,9 @@ int sk_layernorm_bwd_launch(const bf16* dy, const bf16* x, const bf16* w, const 
     SK_CUDA_CHECK(sk_launch_pdl(layernorm_bwd_kernel<8>, dim3(blocks), dim3(LN_BWD_WARPS * 32), smem, s, dy, none, x, w, none, mean, rstd,
                                 dres, dx, dw_partial, db_partial, no_partial, no_partial, M, D));
   SK_LAUNCH_CHECK();
-  SK_CUDA_CHECK(sk_launch_pdl(colsum_reduce_kernel, dim3((D + 31) / 32), dim3(1024), (size_t)0, s, (const float*)dw_partial, dw, blocks, D, accumulate));
+  SK_CUDA_CHECK(sk_launch_pdl(colsum_reduce_kernel<bf16>, dim3((D + 31) / 32), dim3(1024), (size_t)0, s, (const float*)dw_partial, dw, blocks, D, accumulate));
   SK_LAUNCH_CHECK();
-  SK_CUDA_CHECK(sk_launch_pdl(colsum_reduce_kernel, dim3((D + 31) / 32), dim3(1024), (size_t)0, s, (const float*)db_partial, db, blocks, D, accumulate));
+  SK_CUDA_CHECK(sk_launch_pdl(colsum_reduce_kernel<bf16>, dim3((D + 31) / 32), dim3(1024), (size_t)0, s, (const float*)db_partial, db, blocks, D, accumulate));
   SK_LAUNCH_CHECK();
   return 0;
 }
@@ -1299,7 +1324,7 @@ int sk_layernorm2_bwd_launch(const bf16* dy1, const bf16* dy2, const bf16* x, co
   SK_LAUNCH_CHECK();
   bf16* outs[4] = {dw1, db1, dw2, db2};
   for (int t = 0; t < 4; ++t) {
-    SK_CUDA_CHECK(sk_launch_pdl(colsum_reduce_kernel, dim3((D + 31) / 32), dim3(1024), (size_t)0, s, (const float*)pt[t], outs[t],
+    SK_CUDA_CHECK(sk_launch_pdl(colsum_reduce_kernel<bf16>, dim3((D + 31) / 32), dim3(1024), (size_t)0, s, (const float*)pt[t], outs[t],
                                 blocks, D, accumulate));
     SK_LAUNCH_CHECK();
   }
@@ -1308,6 +1333,374 @@ int sk_layernorm2_bwd_launch(const bf16* dy1, const bf16* dy2, const bf16* x, co
 int sk_relu_bwd_launch(bf16* g, const bf16* a, long n, cudaStream_t s) {
   SK_REQUIRE(n % 8 == 0, "relu backward: size must be a multiple of 8");
   SK_CUDA_CHECK(sk_launch_pdl(relu_bwd_kernel, dim3(grid_for(n / 8, 256)), dim3(256), (size_t)0, s, g, a, n));
+  SK_LAUNCH_CHECK();
+  return 0;
+}
+
+// ------------------------------------------------------------------------------------------------
+// OPT with fp32 master weights: HF OPTForCausalLM with fp32 parameters under torch.autocast(bfloat16), the precision of
+// the reference's default recipe (torch_dtype null, bf16: true).  The residual stream, the embedding tables, the
+// LayerNorm parameters and every gradient are fp32; each linear reads bf16 operands (the bf16 shadow of the masters)
+// and writes a bf16 output, so the GEMMs are the bf16 path's own.
+// ------------------------------------------------------------------------------------------------
+namespace {
+
+constexpr int VEC4_PER_WARP = 32 * 4;   // fp32 row elements per warp pass (one float4 per lane)
+
+SK_DEVINL float4 ldg4(const float* p) { return __ldg(reinterpret_cast<const float4*>(p)); }
+SK_DEVINL float4 ldg4_stream(const float* p) {
+  const uint4 u = ldg128_stream(p);
+  return make_float4(__uint_as_float(u.x), __uint_as_float(u.y), __uint_as_float(u.z), __uint_as_float(u.w));
+}
+SK_DEVINL float4 ld_bf16x4(const bf16* p) {
+  const uint2 u = *reinterpret_cast<const uint2*>(p);
+  const float2 a = unpack_bf16(u.x), b = unpack_bf16(u.y);
+  return make_float4(a.x, a.y, b.x, b.y);
+}
+SK_DEVINL void st_bf16x4(bf16* p, float4 v) {
+  *reinterpret_cast<uint2*>(p) = make_uint2(pack_bf16(v.x, v.y), pack_bf16(v.z, v.w));
+}
+
+// x0 = E[id] + P[pos + 2] in fp32 (embed_tokens + embed_positions of the fp32 tables: the residual stream starts fp32)
+__global__ void opt_embed_fwd_f32_kernel(const int64_t* __restrict__ ids, const int32_t* __restrict__ pos_ids,
+                                         const float* __restrict__ E, const float* __restrict__ P, float* __restrict__ out,
+                                         int M, int T, int D, int V, int n_pos) {
+  const int vec_per_row = D / 4;
+  const long total = (long)M * vec_per_row;
+  for (long i = blockIdx.x * (long)blockDim.x + threadIdx.x; i < total; i += (long)gridDim.x * blockDim.x) {
+    const int m = (int)(i / vec_per_row);
+    const int c = (int)(i % vec_per_row);
+    long id = ids[m];
+    if (id < 0 || id >= V) id = 0;
+    const int pr = opt_pos_row(pos_ids, m, T, n_pos);
+    const float4 a = ldg4(E + (size_t)id * D + c * 4), b = ldg4(P + (size_t)pr * D + c * 4);
+    *reinterpret_cast<float4*>(out + (size_t)m * D + c * 4) = make_float4(a.x + b.x, a.y + b.y, a.z + b.z, a.w + b.w);
+  }
+}
+
+// Residual add + LayerNorm, one warp per row, the row in registers:
+//   x' = x + float(y)  (fp32 + bf16 promotes to fp32: the residual is never rounded to bf16; y == nullptr: x' = x)
+//   h  = bf16((x' - mean) * rstd * g + b)   (fp32 LayerNorm of fp32 parameters; the next linear's autocast rounds once)
+// x' is written to xo when y is given (the backward pass reads it), mean / rstd when their pointers are.
+template <int MAXV>
+__global__ void __launch_bounds__(WARPS_PER_BLOCK * 32)
+add_layernorm_f32_kernel(const float* __restrict__ x, const bf16* __restrict__ y, const float* __restrict__ w,
+                         const float* __restrict__ b, float* __restrict__ xo, bf16* __restrict__ h,
+                         float* __restrict__ mean_out, float* __restrict__ rstd_out, int M, int D, float eps) {
+  griddep_launch();
+  griddep_wait();
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int row = blockIdx.x * WARPS_PER_BLOCK + warp;
+  if (row >= M) return;
+  const int nvec = D / 4;
+  float4 xv[MAXV];
+  float s = 0.f;
+#pragma unroll
+  for (int j = 0; j < MAXV; ++j) {
+    const int c = lane + 32 * j;
+    if (c < nvec) {
+      xv[j] = ldg4_stream(x + (size_t)row * D + c * 4);
+      if (y) {
+        const float4 yv = ld_bf16x4(y + (size_t)row * D + c * 4);
+        xv[j] = make_float4(xv[j].x + yv.x, xv[j].y + yv.y, xv[j].z + yv.z, xv[j].w + yv.w);
+        *reinterpret_cast<float4*>(xo + (size_t)row * D + c * 4) = xv[j];
+      }
+      s += (xv[j].x + xv[j].y) + (xv[j].z + xv[j].w);
+    }
+  }
+  const float mean = warp_sum(s) / (float)D;
+  float ss = 0.f;
+#pragma unroll
+  for (int j = 0; j < MAXV; ++j) {
+    const int c = lane + 32 * j;
+    if (c < nvec) {
+      const float a0 = xv[j].x - mean, a1 = xv[j].y - mean, a2 = xv[j].z - mean, a3 = xv[j].w - mean;
+      ss += (a0 * a0 + a1 * a1) + (a2 * a2 + a3 * a3);
+    }
+  }
+  const float rstd = rsqrtf(warp_sum(ss) / (float)D + eps);
+  if (lane == 0) {
+    if (mean_out) mean_out[row] = mean;
+    if (rstd_out) rstd_out[row] = rstd;
+  }
+#pragma unroll
+  for (int j = 0; j < MAXV; ++j) {
+    const int c = lane + 32 * j;
+    if (c < nvec) {
+      const float4 g = ldg4(w + c * 4), bb = ldg4(b + c * 4);
+      st_bf16x4(h + (size_t)row * D + c * 4,
+                make_float4(fmaf((xv[j].x - mean) * rstd, g.x, bb.x), fmaf((xv[j].y - mean) * rstd, g.y, bb.y),
+                            fmaf((xv[j].z - mean) * rstd, g.z, bb.z), fmaf((xv[j].w - mean) * rstd, g.w, bb.w)));
+    }
+  }
+}
+
+// LayerNorm backward on the fp32 residual, one warp per row, grid-stride over rows with a fixed grid:
+//   xhat = (x - mean) * rstd ; g = float(dy) * w ; dres' = dres + rstd * (g - mean(g) - xhat * mean(g * xhat))
+// dres' is written in fp32 (dres_out may alias dres_in: each element is read, then written, by the same lane) and as a
+// bf16 copy for the next branch's GEMMs; dres_in == nullptr reads zeros.  dw / db partial rows as in
+// layernorm_bwd_kernel (per-warp shared slabs, one partial row per block, fixed-order reduction afterwards).
+template <int MAXV>
+__global__ void __launch_bounds__(LN_BWD_WARPS * 32)
+layernorm_bwd_f32_kernel(const bf16* __restrict__ dy, const float* __restrict__ x, const float* __restrict__ w,
+                         const float* __restrict__ mean_in, const float* __restrict__ rstd_in, const float* dres_in,
+                         float* dres_out, bf16* __restrict__ dres16, float* __restrict__ dw_partial,
+                         float* __restrict__ db_partial, int M, int D) {
+  griddep_launch();
+  griddep_wait();
+  extern __shared__ float sacc[];   // [2][LN_BWD_WARPS][D]: dw, db
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int nvec = D / 4;
+  float* sw = sacc + (size_t)warp * D;
+  float* sb = sacc + ((size_t)LN_BWD_WARPS + warp) * D;
+  for (int e = lane; e < D; e += 32) sw[e] = sb[e] = 0.f;
+  for (int row = blockIdx.x * LN_BWD_WARPS + warp; row < M; row += gridDim.x * LN_BWD_WARPS) {
+    float4 xh[MAXV], gv[MAXV];
+    const float mean = mean_in[row], rstd = rstd_in[row];
+    float s1 = 0.f, s2 = 0.f;
+#pragma unroll
+    for (int j = 0; j < MAXV; ++j) {
+      const int c = lane + 32 * j;
+      if (c < nvec) {
+        const float4 xv = ldg4_stream(x + (size_t)row * D + c * 4);
+        const float4 dv = ld_bf16x4(dy + (size_t)row * D + c * 4);
+        const float4 wv = ldg4(w + c * 4);
+        xh[j] = make_float4((xv.x - mean) * rstd, (xv.y - mean) * rstd, (xv.z - mean) * rstd, (xv.w - mean) * rstd);
+        gv[j] = make_float4(dv.x * wv.x, dv.y * wv.y, dv.z * wv.z, dv.w * wv.w);
+        s1 += (gv[j].x + gv[j].y) + (gv[j].z + gv[j].w);
+        s2 += (gv[j].x * xh[j].x + gv[j].y * xh[j].y) + (gv[j].z * xh[j].z + gv[j].w * xh[j].w);
+        const int e = c * 4;
+        sw[e] = fmaf(dv.x, xh[j].x, sw[e]);
+        sw[e + 1] = fmaf(dv.y, xh[j].y, sw[e + 1]);
+        sw[e + 2] = fmaf(dv.z, xh[j].z, sw[e + 2]);
+        sw[e + 3] = fmaf(dv.w, xh[j].w, sw[e + 3]);
+        sb[e] += dv.x;
+        sb[e + 1] += dv.y;
+        sb[e + 2] += dv.z;
+        sb[e + 3] += dv.w;
+      }
+    }
+    const float m1 = warp_sum(s1) / (float)D, m2 = warp_sum(s2) / (float)D;
+#pragma unroll
+    for (int j = 0; j < MAXV; ++j) {
+      const int c = lane + 32 * j;
+      if (c < nvec) {
+        const size_t o = (size_t)row * D + c * 4;
+        const float4 r = dres_in ? *reinterpret_cast<const float4*>(dres_in + o) : make_float4(0.f, 0.f, 0.f, 0.f);
+        const float4 d = make_float4(r.x + rstd * (gv[j].x - m1 - xh[j].x * m2), r.y + rstd * (gv[j].y - m1 - xh[j].y * m2),
+                                     r.z + rstd * (gv[j].z - m1 - xh[j].z * m2), r.w + rstd * (gv[j].w - m1 - xh[j].w * m2));
+        *reinterpret_cast<float4*>(dres_out + o) = d;
+        st_bf16x4(dres16 + o, d);
+      }
+    }
+  }
+  __syncthreads();
+  for (int i = threadIdx.x; i < D; i += blockDim.x) {
+    float a = 0.f, bsum = 0.f;
+#pragma unroll
+    for (int wi = 0; wi < LN_BWD_WARPS; ++wi) {
+      a += sacc[(size_t)wi * D + i];
+      bsum += sacc[((size_t)LN_BWD_WARPS + wi) * D + i];
+    }
+    dw_partial[(size_t)blockIdx.x * D + i] = a;
+    db_partial[(size_t)blockIdx.x * D + i] = bsum;
+  }
+}
+
+// table_fix[row(m)] += dx[m] for fp32 rows, in the 64-bit fixed point of embed_bwd_scatter_kernel (2^-40 units,
+// order-independent).  row(m) = ids[m] (ids given; out-of-range ids are skipped) or the position-table row of m.
+__global__ void scatter_rows_fix_f32_kernel(const int64_t* __restrict__ ids, const int32_t* __restrict__ pos_ids,
+                                            const float* __restrict__ dx, unsigned long long* __restrict__ scratch, int M,
+                                            int T, int D, int n_rows) {
+  const int vec_per_row = D / 4;
+  const long total = (long)M * vec_per_row;
+  for (long i = blockIdx.x * (long)blockDim.x + threadIdx.x; i < total; i += (long)gridDim.x * blockDim.x) {
+    const int m = (int)(i / vec_per_row);
+    const int c = (int)(i % vec_per_row);
+    long r;
+    if (ids) {
+      r = ids[m];
+      if (r < 0 || r >= n_rows) continue;
+    } else {
+      r = opt_pos_row(pos_ids, m, T, n_rows);
+    }
+    const float4 v = ldg4_stream(dx + (size_t)m * D + c * 4);
+    const float f[4] = {v.x, v.y, v.z, v.w};
+    unsigned long long* dst = scratch + (size_t)r * D + c * 4;
+#pragma unroll
+    for (int k = 0; k < 4; ++k)
+      if (f[k] != 0.f) atomicAdd(dst + k, (unsigned long long)__float2ll_rn(f[k] * EMBED_FIX_SCALE));
+  }
+}
+
+// grad = (keep ? grad : 0) + (float(head) + fix * 2^-40): the tied lm_head's bf16 gradient widened (head may be null)
+// plus the embedding's own fp32 gradient, added to the fp32 .grad as autograd accumulates a leaf used twice
+__global__ void add_fix_into_f32_kernel(float* __restrict__ grad, const unsigned long long* __restrict__ scratch,
+                                        const bf16* __restrict__ head, long n, int keep) {
+  for (long i = (blockIdx.x * (long)blockDim.x + threadIdx.x) * 4; i < n; i += (long)gridDim.x * blockDim.x * 4) {
+    const ulonglong2 a = *reinterpret_cast<const ulonglong2*>(scratch + i);
+    const ulonglong2 b = *reinterpret_cast<const ulonglong2*>(scratch + i + 2);
+    float t[4] = {(float)((double)(long long)a.x * (1.0 / 1099511627776.0)), (float)((double)(long long)a.y * (1.0 / 1099511627776.0)),
+                  (float)((double)(long long)b.x * (1.0 / 1099511627776.0)), (float)((double)(long long)b.y * (1.0 / 1099511627776.0))};
+    if (head) {
+      const float4 hv = ld_bf16x4(head + i);
+      t[0] = hv.x + t[0]; t[1] = hv.y + t[1]; t[2] = hv.z + t[2]; t[3] = hv.w + t[3];
+    }
+    float4* g = reinterpret_cast<float4*>(grad + i);
+    if (keep) {
+      const float4 o = *g;
+      t[0] = o.x + t[0]; t[1] = o.y + t[1]; t[2] = o.z + t[2]; t[3] = o.w + t[3];
+    }
+    *g = make_float4(t[0], t[1], t[2], t[3]);
+  }
+}
+
+// g32 = (keep ? g32 : 0) + float(g16) over the listed chunks (the linear weights and biases, whose bf16 gradients the
+// wgrad GEMMs and column sums write): the widening of autocast's bf16 dW into the fp32 .grad, one pass per micro-batch
+__global__ void widen_grads_kernel(const bf16* __restrict__ g16, float* __restrict__ g32, const long* __restrict__ chunk_start,
+                                   const int* __restrict__ chunk_len, int keep) {
+  const long s = chunk_start[blockIdx.x];
+  const int n = chunk_len[blockIdx.x];
+  for (int i = threadIdx.x * 8; i < n; i += blockDim.x * 8) {
+    const uint4 v = ldg128_stream(g16 + s + i);
+    const float2 a = unpack_bf16(v.x), b = unpack_bf16(v.y), c = unpack_bf16(v.z), d = unpack_bf16(v.w);
+    float4* o = reinterpret_cast<float4*>(g32 + s + i);
+    float4 lo = make_float4(a.x, a.y, b.x, b.y), hi = make_float4(c.x, c.y, d.x, d.y);
+    if (keep) {
+      const float4 p = o[0], q = o[1];
+      lo = make_float4(p.x + lo.x, p.y + lo.y, p.z + lo.z, p.w + lo.w);
+      hi = make_float4(q.x + hi.x, q.y + hi.y, q.z + hi.z, q.w + hi.w);
+    }
+    o[0] = lo;
+    o[1] = hi;
+  }
+}
+
+// AdamW on fp32 master weights, element for element the arithmetic of torch's AdamW (fused=True) on fp32 tensors as
+// written out in ATen's adam_math: every product, sum and quotient rounded on its own (no contraction), the clip
+// coefficient applied to the gradient first.  Writes the master, both moments and the bf16 shadow the kernels read.
+__global__ void adamw_master_kernel(float* __restrict__ p, bf16* __restrict__ shadow, const float* __restrict__ g,
+                                    float* __restrict__ m, float* __restrict__ v, long n, float lr_wd, float one_m_b1,
+                                    float beta2, float one_m_b2, float eps, float step_size, float bc2_sqrt,
+                                    const float* __restrict__ clip_stats) {
+  const float coef = clip_stats ? clip_stats[1] : 1.0f;
+  for (long i = (blockIdx.x * (long)blockDim.x + threadIdx.x) * 4; i < n; i += (long)gridDim.x * blockDim.x * 4) {
+    float4 pv = *reinterpret_cast<const float4*>(p + i), mv = *reinterpret_cast<const float4*>(m + i);
+    float4 vv = *reinterpret_cast<const float4*>(v + i);
+    const float4 gv = ldg4_stream(g + i);
+    float* pp = &pv.x;
+    float* mm = &mv.x;
+    float* ss = &vv.x;
+    const float gg[4] = {gv.x, gv.y, gv.z, gv.w};
+#pragma unroll
+    for (int e = 0; e < 4; ++e) {
+      const float grad = __fmul_rn(gg[e], coef);
+      float param = __fsub_rn(pp[e], __fmul_rn(lr_wd, pp[e]));
+      const float ea = __fadd_rn(mm[e], __fmul_rn(one_m_b1, __fsub_rn(grad, mm[e])));
+      const float es = __fadd_rn(__fmul_rn(beta2, ss[e]), __fmul_rn(__fmul_rn(one_m_b2, grad), grad));
+      const float denom = __fadd_rn(__fdiv_rn(__fsqrt_rn(es), bc2_sqrt), eps);
+      param = __fsub_rn(param, __fdiv_rn(__fmul_rn(step_size, ea), denom));
+      pp[e] = param;
+      mm[e] = ea;
+      ss[e] = es;
+    }
+    *reinterpret_cast<float4*>(p + i) = pv;
+    *reinterpret_cast<float4*>(m + i) = mv;
+    *reinterpret_cast<float4*>(v + i) = vv;
+    st_bf16x4(shadow + i, pv);
+  }
+}
+
+}  // namespace
+
+int sk_opt_embed_fwd_f32_launch(const int64_t* ids, const int32_t* pos_ids, const float* E, const float* P, float* out, int M,
+                                int T, int D, int V, int n_pos, cudaStream_t s) {
+  SK_REQUIRE(D % 8 == 0 && n_pos > 0 && T > 0, "opt embed (fp32): D must be a multiple of 8");
+  opt_embed_fwd_f32_kernel<<<grid_for((long)M * D / 4, 256), 256, 0, s>>>(ids, pos_ids, E, P, out, M, T, D, V, n_pos);
+  SK_LAUNCH_CHECK();
+  return 0;
+}
+int sk_add_layernorm_f32_launch(const float* x, const bf16* y, const float* w, const float* b, float* xo, bf16* h, float* mean,
+                                float* rstd, int M, int D, float eps, cudaStream_t s) {
+  SK_REQUIRE(D % 8 == 0 && D <= 2048, "add+layernorm (fp32): D must be a multiple of 8 and <= 2048 (D=%d)", D);
+  SK_REQUIRE(y == nullptr || xo != nullptr, "add+layernorm (fp32): the sum x + y needs an output");
+  const dim3 grid((M + WARPS_PER_BLOCK - 1) / WARPS_PER_BLOCK), block(WARPS_PER_BLOCK * 32);
+  if (D <= 4 * VEC4_PER_WARP)
+    SK_CUDA_CHECK(sk_launch_pdl(add_layernorm_f32_kernel<4>, grid, block, (size_t)0, s, x, y, w, b, xo, h, mean, rstd, M, D, eps));
+  else if (D <= 8 * VEC4_PER_WARP)
+    SK_CUDA_CHECK(sk_launch_pdl(add_layernorm_f32_kernel<8>, grid, block, (size_t)0, s, x, y, w, b, xo, h, mean, rstd, M, D, eps));
+  else
+    SK_CUDA_CHECK(sk_launch_pdl(add_layernorm_f32_kernel<16>, grid, block, (size_t)0, s, x, y, w, b, xo, h, mean, rstd, M, D, eps));
+  SK_LAUNCH_CHECK();
+  return 0;
+}
+// partial must hold 2 * sk_layernorm_bwd_blocks() * D floats
+int sk_layernorm_bwd_f32_launch(const bf16* dy, const float* x, const float* w, const float* mean, const float* rstd,
+                                const float* dres_in, float* dres_out, bf16* dres16, float* dw, float* db, float* partial, int M,
+                                int D, int accumulate, cudaStream_t s) {
+  SK_REQUIRE(D % 8 == 0 && D <= 2048, "layernorm backward (fp32): D must be a multiple of 8 and <= 2048 (D=%d)", D);
+  SK_REQUIRE(M > 0, "layernorm backward (fp32): M must be positive");
+  int blocks = sk_layernorm_bwd_blocks();
+  const int need = (M + LN_BWD_WARPS - 1) / LN_BWD_WARPS;
+  if (blocks > need) blocks = need;
+  const size_t smem = (size_t)2 * LN_BWD_WARPS * D * sizeof(float);
+  float* dwp = partial;
+  float* dbp = partial + (size_t)blocks * D;
+  const dim3 grid(blocks), block(LN_BWD_WARPS * 32);
+  if (D <= 4 * VEC4_PER_WARP) {
+    SK_CUDA_CHECK(sk_launch_pdl(layernorm_bwd_f32_kernel<4>, grid, block, smem, s, dy, x, w, mean, rstd, dres_in, dres_out, dres16,
+                                dwp, dbp, M, D));
+  } else if (D <= 8 * VEC4_PER_WARP) {
+    SK_CUDA_CHECK(sk_launch_pdl(layernorm_bwd_f32_kernel<8>, grid, block, smem, s, dy, x, w, mean, rstd, dres_in, dres_out, dres16,
+                                dwp, dbp, M, D));
+  } else {
+    SK_CUDA_CHECK(cudaFuncSetAttribute(layernorm_bwd_f32_kernel<16>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    SK_CUDA_CHECK(sk_launch_pdl(layernorm_bwd_f32_kernel<16>, grid, block, smem, s, dy, x, w, mean, rstd, dres_in, dres_out, dres16,
+                                dwp, dbp, M, D));
+  }
+  SK_LAUNCH_CHECK();
+  SK_CUDA_CHECK(sk_launch_pdl(colsum_reduce_kernel<float>, dim3((D + 31) / 32), dim3(1024), (size_t)0, s, (const float*)dwp, dw, blocks,
+                              D, accumulate));
+  SK_LAUNCH_CHECK();
+  SK_CUDA_CHECK(sk_launch_pdl(colsum_reduce_kernel<float>, dim3((D + 31) / 32), dim3(1024), (size_t)0, s, (const float*)dbp, db, blocks,
+                              D, accumulate));
+  SK_LAUNCH_CHECK();
+  return 0;
+}
+// Gradient of a table from fp32 rows: the 64-bit fixed point (2^-40 units; exact integer sums, so bit-identical run to
+// run) resolves 9.1e-13 absolute per term -- fp32's own resolution for terms near 1e-5, finer above -- and holds sums
+// below 2^23.  ids given: token table (n_rows = vocabulary), head = the tied lm_head's bf16 gradient or null; ids null:
+// position table (n_rows = max_positions + 2).  keep: add to the fp32 gradient instead of overwriting it.
+int sk_table_bwd_f32_launch(const int64_t* ids, const int32_t* pos_ids, const float* dx, float* scratch, float* dtable,
+                            const bf16* head, int M, int T, int D, int n_rows, int n_rows_padded, int keep, cudaStream_t s) {
+  SK_REQUIRE(D % 8 == 0 && n_rows > 0 && T > 0, "table backward (fp32): D must be a multiple of 8");
+  unsigned long long* fix = reinterpret_cast<unsigned long long*>(scratch);
+  const long n = (long)n_rows_padded * D;
+  SK_CUDA_CHECK(cudaMemsetAsync(fix, 0, (size_t)n * sizeof(unsigned long long), s));
+  scatter_rows_fix_f32_kernel<<<grid_for((long)M * D / 4, 256), 256, 0, s>>>(ids, pos_ids, dx, fix, M, T, D, n_rows);
+  SK_LAUNCH_CHECK();
+  add_fix_into_f32_kernel<<<grid_for(n / 4, 256), 256, 0, s>>>(dtable, fix, head, n, keep);
+  SK_LAUNCH_CHECK();
+  return 0;
+}
+int sk_widen_grads_launch(const bf16* g16, float* g32, const long* chunk_start, const int* chunk_len, int n_chunks, int keep,
+                          cudaStream_t s) {
+  if (n_chunks == 0) return 0;
+  widen_grads_kernel<<<n_chunks, 256, 0, s>>>(g16, g32, chunk_start, chunk_len, keep);
+  SK_LAUNCH_CHECK();
+  return 0;
+}
+// The fp32 hyperparameters are combined on the host in double, as Python does before torch sees them: 1 - beta,
+// lr * weight_decay, lr / (1 - beta1^step) and sqrt(1 - beta2^step), each rounded to fp32 once.
+int sk_adamw_master_launch(float* p, bf16* shadow, const float* g, float* m, float* v, long n, float lr, float beta1, float beta2,
+                           float eps, float wd, int step, const float* clip_stats, cudaStream_t s) {
+  SK_REQUIRE(n % 8 == 0, "adamw (fp32): flat parameter count must be a multiple of 8 (n=%ld)", n);
+  SK_REQUIRE(step >= 1, "adamw (fp32): step counts from 1");
+  const double bc1 = 1.0 - pow((double)beta1, (double)step);
+  const float bc2_sqrt = (float)sqrt(1.0 - pow((double)beta2, (double)step));
+  adamw_master_kernel<<<grid_for(n / 4, 256, 8), 256, 0, s>>>(p, shadow, g, m, v, n, (float)((double)lr * (double)wd),
+                                                              (float)(1.0 - (double)beta1), beta2, (float)(1.0 - (double)beta2),
+                                                              eps, (float)((double)lr / bc1), bc2_sqrt, clip_stats);
   SK_LAUNCH_CHECK();
   return 0;
 }

@@ -39,6 +39,7 @@ struct WsLayout {
   int64_t sX, sh, srstd, sqkv, slse, sgu, sact;
   int64_t hf, rstdf, logits, dlogits, dxA, dxB, dh, dao, dqkv, dgu, delta;
   int64_t dw_partial, colsum_partial, ce_partial, embed_scratch, splitk, splitk_bytes, seg_start, seg_end, total;
+  int64_t sR = 0, dres32 = 0;   // OPT: residual-stream slab stride (X, xmid); fp32 residual gradient (master weights)
 };
 }  // namespace
 
@@ -68,6 +69,14 @@ struct SkLm {
   int n_chunks = 0, n_norm_groups = 0;
   int last_B = 0, last_T = 0;
   int head_chunk = 0;   // > 0: rows per chunk of the chunked lm_head + CE (large vocabularies), 0: one pass
+  // OPT with fp32 master weights (sk_lm_set_master): `params` is then the bf16 shadow of params32 that the GEMMs read,
+  // `grads` the bf16 scratch of the linear gradients, widened into grads32 over the widen_* chunks once per micro-batch
+  bool master = false;
+  float* params32 = nullptr;
+  float* grads32 = nullptr;
+  long* d_widen_start = nullptr;
+  int* d_widen_len = nullptr;
+  int n_widen = 0;
   // optional: events recorded on the compute stream as soon as a layer's gradients are final (index = layer; index
   // n_layers = lm_head / final-norm part), so the host can start that bucket's all-reduce while backward continues
   std::vector<cudaEvent_t> bwd_events;
@@ -396,16 +405,17 @@ WsLayout make_opt_layout(const SkLm* lm, int B, int T) {
   w.slse = align_up((int64_t)B * lm->H * T * 4, 256);
   w.sgu = align_up(M * lm->F * 2, 256);
   w.sact = 0;
+  w.sR = lm->master ? align_up(M * lm->d * 4, 256) : w.sX;   // master weights: the residual stream is fp32
   // GEMM scratch first, at the same fixed offset as in make_layout (sk_lm_bind clears its flag words once)
   w.splitk_bytes = align_up(std::max<int64_t>((int64_t)8 * lm->qkv_dim * lm->d * 4, (int64_t)sk_gemm_ws_min_bytes()) + 4096, 256);
   w.splitk = take(w.splitk_bytes);
-  w.X = take(w.sX * (L + 1));
+  w.X = take(w.sR * (L + 1));
   w.h1 = take(w.sh * L);
   w.rstd1 = take(w.srstd * L);
   w.qkv = take(w.sqkv * L);
   w.ao = take(w.sX * L);
   w.lse = take(w.slse * L);
-  w.xmid = take(w.sX * L);
+  w.xmid = take(w.sR * L);
   w.h2 = take(w.sh * L);
   w.rstd2 = take(w.srstd * L);
   w.gu = take(w.sgu * L);
@@ -428,6 +438,7 @@ WsLayout make_opt_layout(const SkLm* lm, int B, int T) {
   w.embed_scratch = take((int64_t)std::max(lm->Vp, lm->n_pos) * lm->d * 8);
   w.seg_start = take(M * 4);
   w.seg_end = take(M * 4);
+  if (lm->master) w.dres32 = take(w.sR);
   w.total = cur;
   return w;
 }
@@ -660,9 +671,150 @@ int neox_decode_step(SkLm* lm, const int64_t* tokens, const int32_t* pos, int B,
   return sk_gemm_launch(B, lm->Vp, d, h, d, 0, P + lm->off_head, d, 0, logits, ldl, 0, nullptr, nullptr, 0, 0, 0, 0, s);
 }
 
+// ---- OPT with fp32 master weights (sk_lm_set_master): HF OPTForCausalLM with fp32 parameters under
+// torch.autocast(bfloat16).  The residual stream X / xmid is fp32 and never rounded; every LayerNorm reads it with fp32
+// gamma / beta and hands the next linear one bf16 rounding; every linear is the bf16 path's GEMM on the bf16 shadow
+// weights with a bf16 output, which is autocast's linear.  Each branch output's residual add is fused into the next
+// LayerNorm (the last fc2's into the final norm); the bf16 branch output waits in the dxB slab, unused until backward.
+int opt_forward_master(SkLm* lm, const int64_t* ids, const int64_t* labels, const int32_t* pos_ids, int B, int T, float num_items,
+                       float dloss, bool want_dlogits, float* stats, const WsLayout& w, cudaStream_t s, float* row_nll,
+                       bool with_head) {
+  const int M = B * T, d = lm->d, F = lm->F, L = lm->L, Q = lm->qkv_dim;
+  const float eps = lm->cfg.rms_eps;
+  const bf16* P = lm->params;
+  const float* P32 = lm->params32;
+  bf16* y = wsp<bf16>(lm, w.dxB);
+  SK_TRY(sk_opt_embed_fwd_f32_launch(ids, pos_ids, P32 + lm->off_embed, P32 + lm->off_pos, wsp<float>(lm, w.X), M, T, d, lm->V,
+                                     lm->n_pos, s));
+  const float scale = 1.0f / sqrtf((float)lm->hd);
+  const int* seg_start = nullptr;
+  if (pos_ids) {
+    SK_TRY(sk_seg_bounds_launch(pos_ids, wsp<int32_t>(lm, w.seg_start), wsp<int32_t>(lm, w.seg_end), B, T, s));
+    seg_start = wsp<int32_t>(lm, w.seg_start);
+  }
+  for (int l = 0; l < L; ++l) {
+    const OptLayerOff& o = lm->olo[l];
+    float* x = wsp<float>(lm, w.X + w.sR * l);
+    float* xmid = wsp<float>(lm, w.xmid + w.sR * l);
+    bf16* h1 = wsp<bf16>(lm, w.h1 + w.sh * l);
+    float* st1 = wsp<float>(lm, w.rstd1 + w.srstd * l);
+    bf16* qkv = wsp<bf16>(lm, w.qkv + w.sqkv * l);
+    bf16* ao = wsp<bf16>(lm, w.ao + w.sX * l);
+    float* lse = wsp<float>(lm, w.lse + w.slse * l);
+    bf16* h2 = wsp<bf16>(lm, w.h2 + w.sh * l);
+    float* st2 = wsp<float>(lm, w.rstd2 + w.srstd * l);
+    bf16* a = wsp<bf16>(lm, w.gu + w.sgu * l);
+
+    // x = xmid[l-1] + fc2 output of layer l-1 (layer 0: the embedding sum as it is)
+    const float* xin = l == 0 ? x : wsp<float>(lm, w.xmid + w.sR * (l - 1));
+    SK_TRY(sk_add_layernorm_f32_launch(xin, l == 0 ? nullptr : y, P32 + o.ln1w, P32 + o.ln1b, l == 0 ? nullptr : x, h1, st1,
+                                       st1 + M, M, d, eps, s));
+    SK_TRY(linear_fwd(M, Q, d, h1, P + o.wqkv, qkv, P + o.bqkv, nullptr, s));
+    SK_TRY(sk_attn_tc_fwd_launch(qkv, ao, lse, B, T, lm->H, lm->H, Q, d, 1, scale, s, seg_start));
+    SK_TRY(linear_fwd(M, d, d, ao, P + o.wo, y, P + o.bo, nullptr, s));
+    SK_TRY(sk_add_layernorm_f32_launch(x, y, P32 + o.ln2w, P32 + o.ln2b, xmid, h2, st2, st2 + M, M, d, eps, s));
+    SK_TRY(sk_gemm_launch(M, F, d, h2, d, 0, P + o.w1, d, 0, a, F, 0, P + o.b1, nullptr, 0, 0, 2, 0, s));   // relu(fc1)
+    SK_TRY(linear_fwd(M, d, F, a, P + o.w2, y, P + o.b2, nullptr, s));
+  }
+  float* stf = wsp<float>(lm, w.rstdf);
+  SK_TRY(sk_add_layernorm_f32_launch(wsp<float>(lm, w.xmid + w.sR * (L - 1)), y, P32 + lm->off_final_norm,
+                                     P32 + lm->off_final_norm_b, wsp<float>(lm, w.X + w.sR * L), wsp<bf16>(lm, w.hf), stf,
+                                     stf + M, M, d, eps, s));
+  lm->last_B = B;
+  lm->last_T = T;
+  if (!with_head) return 0;
+  bf16* logits = wsp<bf16>(lm, w.logits);
+  SK_TRY(linear_fwd(M, lm->Vp, d, wsp<bf16>(lm, w.hf), P + lm->off_head, logits, nullptr, nullptr, s));
+  if (labels) {
+    SK_TRY(sk_ce_launch(logits, labels, want_dlogits ? wsp<bf16>(lm, w.dlogits) : nullptr, wsp<float>(lm, w.ce_partial),
+                        row_nll, stats, M, T, lm->V, lm->Vp, num_items, dloss, s));
+  }
+  return 0;
+}
+
+// The residual gradient dres is fp32 (dres32); each branch's GEMMs and bias column sums read its bf16 copy (dxA), and
+// each LayerNorm backward adds its input gradient to dres in fp32.  Linear weight and bias gradients land in the bf16
+// buffer (never accumulated there) and are widened into grads32 at the end; LayerNorm and table gradients go straight
+// into grads32.  `accumulate` = a later micro-batch: add to grads32 instead of overwriting it.
+int opt_backward_master(SkLm* lm, const int64_t* ids, const int32_t* pos_ids, int B, int T, int accumulate, const WsLayout& w,
+                        cudaStream_t s, bool with_head) {
+  const int M = B * T, d = lm->d, F = lm->F, L = lm->L, Q = lm->qkv_dim;
+  const bf16* P = lm->params;
+  const float* P32 = lm->params32;
+  bf16* G = lm->grads;
+  float* G32 = lm->grads32;
+  float* lnp = wsp<float>(lm, w.dw_partial);
+  float* csp = wsp<float>(lm, w.colsum_partial);
+  float* dres = wsp<float>(lm, w.dres32);
+  bf16* dr16 = wsp<bf16>(lm, w.dxA);
+  bf16* dh = wsp<bf16>(lm, w.dh);
+  bf16* dao = wsp<bf16>(lm, w.dao);
+  bf16* dqkv = wsp<bf16>(lm, w.dqkv);
+  bf16* da = wsp<bf16>(lm, w.dgu);
+  void* sws = lm->ws + w.splitk;
+  const size_t swb = (size_t)w.splitk_bytes;
+  const float scale = 1.0f / sqrtf((float)lm->hd);
+  const int* seg_start = pos_ids ? wsp<int32_t>(lm, w.seg_start) : nullptr;
+  const int* seg_end = pos_ids ? wsp<int32_t>(lm, w.seg_end) : nullptr;
+
+  if (with_head) {
+    bf16* dlogits = wsp<bf16>(lm, w.dlogits);
+    SK_TRY(linear_dgrad(M, lm->Vp, d, dlogits, P + lm->off_head, dh, s));
+    SK_TRY(linear_wgrad(M, lm->Vp, d, dlogits, wsp<bf16>(lm, w.hf), G + lm->off_head, 0, s, sws, swb));
+  }
+  const float* stf = wsp<float>(lm, w.rstdf);
+  SK_TRY(sk_layernorm_bwd_f32_launch(dh, wsp<float>(lm, w.X + w.sR * L), P32 + lm->off_final_norm, stf, stf + M, nullptr, dres,
+                                     dr16, G32 + lm->off_final_norm, G32 + lm->off_final_norm_b, lnp, M, d, accumulate, s));
+  if (!lm->bwd_events.empty()) SK_CUDA_CHECK(cudaEventRecord(lm->bwd_events[L], s));
+  for (int l = L - 1; l >= 0; --l) {
+    const OptLayerOff& o = lm->olo[l];
+    const float* x = wsp<float>(lm, w.X + w.sR * l);
+    const float* xmid = wsp<float>(lm, w.xmid + w.sR * l);
+    const bf16* h1 = wsp<bf16>(lm, w.h1 + w.sh * l);
+    const float* st1 = wsp<float>(lm, w.rstd1 + w.srstd * l);
+    const bf16* qkv = wsp<bf16>(lm, w.qkv + w.sqkv * l);
+    const bf16* ao = wsp<bf16>(lm, w.ao + w.sX * l);
+    const float* lse = wsp<float>(lm, w.lse + w.slse * l);
+    const bf16* h2 = wsp<bf16>(lm, w.h2 + w.sh * l);
+    const float* st2 = wsp<float>(lm, w.rstd2 + w.srstd * l);
+    const bf16* a = wsp<bf16>(lm, w.gu + w.sgu * l);
+
+    // MLP on bf16(dres)
+    SK_TRY(linear_dgrad(M, d, F, dr16, P + o.w2, da, s));
+    SK_TRY(sk_relu_bwd_launch(da, a, (long)M * F, s));
+    SK_TRY(linear_wgrad(M, d, F, dr16, a, G + o.w2, 0, s, sws, swb));
+    SK_TRY(sk_colsum_launch(dr16, G + o.b2, csp, M, d, d, 0, s));
+    SK_TRY(linear_dgrad(M, F, d, da, P + o.w1, dh, s));
+    SK_TRY(linear_wgrad(M, F, d, da, h2, G + o.w1, 0, s, sws, swb));
+    SK_TRY(sk_colsum_launch(da, G + o.b1, csp, M, F, F, 0, s));
+    SK_TRY(sk_layernorm_bwd_f32_launch(dh, xmid, P32 + o.ln2w, st2, st2 + M, dres, dres, dr16, G32 + o.ln2w, G32 + o.ln2b, lnp, M,
+                                       d, accumulate, s));
+    // attention on bf16(dres)
+    SK_TRY(linear_dgrad(M, d, d, dr16, P + o.wo, dao, s));
+    SK_TRY(linear_wgrad(M, d, d, dr16, ao, G + o.wo, 0, s, sws, swb));
+    SK_TRY(sk_colsum_launch(dr16, G + o.bo, csp, M, d, d, 0, s));
+    SK_TRY(sk_attn_tc_bwd_launch(qkv, ao, dao, lse, wsp<float>(lm, w.delta), nullptr, dqkv, B, T, lm->H, lm->H, Q, d, Q, 1,
+                                 scale, s, seg_start, seg_end));
+    SK_TRY(sk_colsum_launch(dqkv, G + o.bqkv, csp, M, Q, Q, 0, s));
+    SK_TRY(linear_dgrad(M, Q, d, dqkv, P + o.wqkv, dh, s));
+    SK_TRY(linear_wgrad(M, Q, d, dqkv, h1, G + o.wqkv, 0, s, sws, swb));
+    SK_TRY(sk_layernorm_bwd_f32_launch(dh, x, P32 + o.ln1w, st1, st1 + M, dres, dres, dr16, G32 + o.ln1w, G32 + o.ln1b, lnp, M, d,
+                                       accumulate, s));
+    if (!lm->bwd_events.empty()) SK_CUDA_CHECK(cudaEventRecord(lm->bwd_events[l], s));
+  }
+  float* scratch = wsp<float>(lm, w.embed_scratch);
+  SK_TRY(sk_table_bwd_f32_launch(ids, nullptr, dres, scratch, G32 + lm->off_embed,
+                                 lm->cfg.tie_embeddings ? G + lm->off_head : nullptr, M, T, d, lm->V, lm->Vp, accumulate, s));
+  SK_TRY(sk_table_bwd_f32_launch(nullptr, pos_ids, dres, scratch, G32 + lm->off_pos, nullptr, M, T, d, lm->n_pos, lm->n_pos,
+                                 accumulate, s));
+  return sk_widen_grads_launch(G, G32, lm->d_widen_start, lm->d_widen_len, lm->n_widen, accumulate, s);
+}
+
 int opt_forward(SkLm* lm, const int64_t* ids, const int64_t* labels, const int32_t* pos_ids, int B, int T, float num_items,
                 float dloss, bool want_dlogits, float* stats, const WsLayout& w, cudaStream_t s, float* row_nll = nullptr,
                 bool with_head = true) {
+  if (lm->master)
+    return opt_forward_master(lm, ids, labels, pos_ids, B, T, num_items, dloss, want_dlogits, stats, w, s, row_nll, with_head);
   const int M = B * T, d = lm->d, F = lm->F, L = lm->L, Q = lm->qkv_dim;
   const float eps = lm->cfg.rms_eps;
   const bf16* P = lm->params;
@@ -717,6 +869,7 @@ int opt_forward(SkLm* lm, const int64_t* ids, const int64_t* labels, const int32
 // reaching a pad position is zero (pad targets carry no loss and only later pad positions attend to a pad key).
 int opt_backward(SkLm* lm, const int64_t* ids, const int32_t* pos_ids, int B, int T, int accumulate, const WsLayout& w,
                  cudaStream_t s, bool with_head = true) {
+  if (lm->master) return opt_backward_master(lm, ids, pos_ids, B, T, accumulate, w, s, with_head);
   const int M = B * T, d = lm->d, F = lm->F, L = lm->L, Q = lm->qkv_dim;
   const bf16* P = lm->params;
   bf16* G = lm->grads;
@@ -867,6 +1020,8 @@ int64_t sk_lm_decode_workspace_bytes(const SkLm* lm, int B, int T_cache) {
 int sk_lm_prefill(SkLm* lm, const int64_t* ids, const int32_t* lens, int B, int T, void* kv_cache, int T_cache,
                   void* logits, int ldl, void* decode_ws, int64_t decode_ws_bytes, void* stream) {
   SK_REQUIRE(lm && ids && lens, "sk_lm_prefill: null argument");
+  SK_REQUIRE(!lm->master, "sk_lm_prefill: this handle trains fp32 master weights (sk_lm_set_master); generate from its saved "
+                          "checkpoint with a handle that has no master weights");
   const DecLayout dl = make_dec_layout(lm, B, T_cache);
   SK_TRY(check_decode(lm, B, T_cache, ldl, kv_cache, logits, decode_ws, decode_ws_bytes, dl));
   SK_REQUIRE(T > 0 && T <= T_cache, "sk_lm_prefill: prompt width T=%d must be in [1, T_cache=%d]", T, T_cache);
@@ -889,6 +1044,8 @@ int sk_lm_prefill(SkLm* lm, const int64_t* ids, const int32_t* lens, int B, int 
 int sk_lm_decode_step(SkLm* lm, const int64_t* tokens, const int32_t* pos, int B, void* kv_cache, int T_cache,
                       void* logits, int ldl, void* decode_ws, int64_t decode_ws_bytes, void* stream) {
   SK_REQUIRE(lm && tokens && pos, "sk_lm_decode_step: null argument");
+  SK_REQUIRE(!lm->master, "sk_lm_decode_step: this handle trains fp32 master weights (sk_lm_set_master); generate from its "
+                          "saved checkpoint with a handle that has no master weights");
   const DecLayout dl = make_dec_layout(lm, B, T_cache);
   SK_TRY(check_decode(lm, B, T_cache, ldl, kv_cache, logits, decode_ws, decode_ws_bytes, dl));
   cudaStream_t s = (cudaStream_t)stream;
@@ -1197,6 +1354,8 @@ void sk_lm_destroy(SkLm* lm) {
   cudaFree(lm->d_chunk_len);
   cudaFree(lm->d_tensor_chunk_begin);
   cudaFree(lm->d_chunk_partial);
+  cudaFree(lm->d_widen_start);
+  cudaFree(lm->d_widen_len);
   delete lm;
 }
 
@@ -1245,6 +1404,43 @@ int sk_lm_bind(SkLm* lm, void* params, void* grads, const void* rope_cos, const 
   return 0;
 }
 
+int sk_lm_set_master(SkLm* lm, float* params32, float* grads32) {
+  SK_REQUIRE(lm && params32, "sk_lm_set_master: null argument");
+  SK_REQUIRE(lm->arch == SK_ARCH_OPT, "sk_lm_set_master: fp32 master weights are implemented for the OPT decoder only (the "
+                                      "Qwen2 and GPT-NeoX recipes train bf16 parameters)");
+  SK_REQUIRE(lm->params && lm->ws, "sk_lm_set_master: call sk_lm_bind first");
+  SK_REQUIRE(((uintptr_t)params32 & 127) == 0 && ((uintptr_t)grads32 & 127) == 0,
+             "sk_lm_set_master: params32 / grads32 must be 128-byte aligned");
+  if (!lm->d_widen_start) {
+    // linear weights and biases, whose bf16 gradients are widened: per layer [wqkv .. bo] and [w1 .. b2] (contiguous in
+    // the layout), plus an untied lm_head; the tied lm_head's gradient is folded into the embedding's
+    std::vector<std::pair<int64_t, int64_t>> ranges;
+    for (int l = 0; l < lm->L; ++l) {
+      const OptLayerOff& o = lm->olo[l];
+      ranges.push_back({o.wqkv, o.ln2w - o.wqkv});
+      const int64_t end = l + 1 < lm->L ? lm->olo[l + 1].ln1w : lm->off_final_norm;
+      ranges.push_back({o.w1, end - o.w1});
+    }
+    if (!lm->cfg.tie_embeddings) ranges.push_back({lm->off_head, lm->n_params - lm->off_head});
+    std::vector<long> cs;
+    std::vector<int> cl;
+    for (const auto& r : ranges)
+      for (int64_t o = 0; o < r.second; o += GN_CHUNK) {
+        cs.push_back((long)(r.first + o));
+        cl.push_back((int)std::min<int64_t>(GN_CHUNK, r.second - o));
+      }
+    SK_CUDA_CHECK(cudaMalloc(&lm->d_widen_start, cs.size() * sizeof(long)));
+    SK_CUDA_CHECK(cudaMalloc(&lm->d_widen_len, cl.size() * sizeof(int)));
+    SK_CUDA_CHECK(cudaMemcpy(lm->d_widen_start, cs.data(), cs.size() * sizeof(long), cudaMemcpyHostToDevice));
+    SK_CUDA_CHECK(cudaMemcpy(lm->d_widen_len, cl.data(), cl.size() * sizeof(int), cudaMemcpyHostToDevice));
+    lm->n_widen = (int)cs.size();
+  }
+  lm->params32 = params32;
+  lm->grads32 = grads32;
+  lm->master = true;
+  return 0;
+}
+
 int sk_lm_forward(SkLm* lm, const int64_t* ids, const int64_t* labels, const int32_t* pos_ids, int B, int T,
                   float num_items, float* stats, void* stream) {
   SK_REQUIRE(lm && ids, "sk_lm_forward: null argument");
@@ -1262,13 +1458,15 @@ int sk_lm_forward_backward(SkLm* lm, const int64_t* ids, const int64_t* labels, 
                            float num_items, float dloss, int accumulate, float* stats, void* stream) {
   SK_REQUIRE(lm && ids && labels && stats, "sk_lm_forward_backward: null argument");
   SK_REQUIRE(lm->grads, "sk_lm_forward_backward: no gradient buffer bound");
+  SK_REQUIRE(!lm->master || lm->grads32, "sk_lm_forward_backward: no fp32 gradient buffer given to sk_lm_set_master");
   const WsLayout w = layout_of(lm, B, T);
   SK_TRY(check_bound(lm, B, T, w, pos_ids));
   if (lm->arch == SK_ARCH_OPT) {
     cudaStream_t s = (cudaStream_t)stream;
     if (lm->head_chunk > 0) {
       SK_TRY(opt_forward(lm, ids, labels, pos_ids, B, T, num_items, dloss, true, stats, w, s, nullptr, false));
-      SK_TRY(head_chunked(lm, labels, B, T, num_items, dloss, accumulate, stats, w, s));
+      // master weights: the bf16 gradient buffer holds one micro-batch (grads32 accumulates)
+      SK_TRY(head_chunked(lm, labels, B, T, num_items, dloss, lm->master ? 0 : accumulate, stats, w, s));
       return opt_backward(lm, ids, pos_ids, B, T, accumulate, w, s, false);
     }
     SK_TRY(opt_forward(lm, ids, labels, pos_ids, B, T, num_items, dloss, true, stats, w, s));
@@ -1321,6 +1519,7 @@ int sk_lm_backward_weighted(SkLm* lm, const int64_t* ids, const int64_t* labels,
                             const float* row_weight, int accumulate, float* stats, void* stream) {
   SK_REQUIRE(lm && ids && labels && row_weight && stats, "sk_lm_backward_weighted: null argument");
   SK_REQUIRE(lm->grads, "sk_lm_backward_weighted: no gradient buffer bound");
+  SK_REQUIRE(!lm->master || lm->grads32, "sk_lm_backward_weighted: no fp32 gradient buffer given to sk_lm_set_master");
   SK_REQUIRE(lm->last_B == B && lm->last_T == T, "sk_lm_backward_weighted: call sk_lm_forward_rows on the same batch first");
   const WsLayout w = layout_of(lm, B, T);
   SK_TRY(check_bound(lm, B, T, w, pos_ids));
@@ -1346,6 +1545,30 @@ int sk_lm_optimizer_step(SkLm* lm, void* exp_avg, void* exp_avg_sq, float lr, fl
   SK_REQUIRE(lm && exp_avg && exp_avg_sq && stats, "sk_lm_optimizer_step: null argument");
   SK_REQUIRE(lm->params && lm->grads, "sk_lm_optimizer_step: params/grads not bound");
   cudaStream_t s = (cudaStream_t)stream;
+  if (lm->master) {
+    // fp32 master weights: exp_avg / exp_avg_sq are fp32; clip_grad_norm_ and AdamW over the fp32 gradients, the bf16
+    // shadow rewritten from the new masters (emulate_bf16_norm does not apply to fp32 gradients)
+    SK_REQUIRE(lm->grads32, "sk_lm_optimizer_step: no fp32 gradient buffer given to sk_lm_set_master");
+    float* m = reinterpret_cast<float*>(exp_avg);
+    float* v = reinterpret_cast<float*>(exp_avg_sq);
+    sk_prof_begin(2, s);
+    SK_TRY(sk_gradnorm_f32_launch(lm->grads32, lm->d_chunk_start, lm->d_chunk_len, lm->n_chunks, lm->d_tensor_chunk_begin,
+                                  lm->n_norm_groups, lm->d_chunk_partial, max_grad_norm, stats, s));
+    int rc = 0;
+    if (weight_decay == 0.0f) {
+      rc = sk_adamw_master_launch(lm->params32, lm->params, lm->grads32, m, v, lm->n_params, lr, beta1, beta2, eps, 0.0f, step,
+                                  stats, s);
+    } else {
+      for (const TensorDesc& t : lm->tensors) {   // decay groups as below
+        const int64_t n = (((int64_t)t.rows * t.cols + ALIGN_ELEMS - 1) / ALIGN_ELEMS) * ALIGN_ELEMS;
+        rc = sk_adamw_master_launch(lm->params32 + t.off, lm->params + t.off, lm->grads32 + t.off, m + t.off, v + t.off, n, lr,
+                                    beta1, beta2, eps, t.rows == 1 ? 0.0f : weight_decay, step, stats, s);
+        if (rc) break;
+      }
+    }
+    sk_prof_end(s);
+    return rc;
+  }
   sk_prof_begin(2, s);
   SK_TRY(sk_gradnorm_launch(lm->grads, lm->d_chunk_start, lm->d_chunk_len, lm->n_chunks, lm->d_tensor_chunk_begin,
                             lm->n_norm_groups, lm->d_chunk_partial, max_grad_norm, emulate_bf16_norm, stats, s));

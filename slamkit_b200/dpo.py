@@ -62,6 +62,8 @@ class B200DPOTrainer:
     def __init__(self, policy: B200UnitLM, reference: B200UnitLM, beta: float = 0.1, lr: float = 5e-5,
                  max_grad_norm: float = 0.5, weight_decay: float = 0.0, grad_accum: int = 1, overlap_comm: bool = True):
         from .trainer import GradSync
+        if getattr(policy, "master", False) or getattr(reference, "master", False):
+            raise NotImplementedError("B200DPOTrainer does not take models with fp32 master weights")
         self.policy, self.reference, self.beta = policy, reference, beta
         self.opt = B200AdamW(policy, lr=lr, max_grad_norm=max_grad_norm, weight_decay=weight_decay)
         self.sync = GradSync(policy, overlap=overlap_comm)

@@ -41,6 +41,9 @@ class B200UnitLMModule(torch.nn.Module):
         super().__init__()
         if core.grads is None:
             raise ValueError("B200UnitLMModule needs a trainable B200UnitLM (trainable=True)")
+        if getattr(core, "master", False):
+            raise NotImplementedError("B200UnitLMModule does not take a model with fp32 master weights (train it with "
+                                      "slamkit_b200.trainer.B200Trainer / cli/train.py)")
         self.core = core
         self.flat = torch.nn.Parameter(core.params, requires_grad=True)      # shares storage with the bound buffer
         self.config = core.config

@@ -38,34 +38,48 @@ def hubert_b200_from_cfg(pretrained_model: str = "facebook/hubert-base-ls960",
     return HubertB200FeatureExtractor(cfg, params, device=device, max_batch=max_batch, max_samples=max_samples)
 
 
-def tlm_b200_from_cfg(cfg, device: str = "cuda:0", max_batch: int = 8, max_seq: Optional[int] = None):
-    """`cfg` is the reference's model config node (config/model/*.yaml): context_len, config_args{base_model_name,
-    vocab_size, twist_init, rope_theta, torch_dtype, dropout, ...}.  The base config decides the decoder: Qwen2
-    (`LMConfig`), pre-LayerNorm OPT (`OptLMConfig`, the default TWIST / GSLM base) or parallel-residual GPT-NeoX
-    (`NeoxLMConfig`, the Pythia bases of config/train_inter_scale.yaml; the same overrides and dtype rule as OPT, and
-    `twist_init` loads the Pythia weights from a local directory or cache).  For OPT the reference's
-    `config_args` overrides are applied to the base config as `UnitLMConfig` does (pad / bos / eos ids, dropout,
-    attention_dropout, layerdrop), `rope_theta` is ignored, and `torch_dtype: bfloat16` is required: this path keeps bf16
-    parameters and bf16 AdamW moments, while the reference run with `torch_dtype: null` keeps fp32 master weights.
-    Raises OSError when the base model cannot be reached (offline box) and ValueError when its architecture or settings
-    have no kernels here."""
+def tlm_b200_config(cfg, autocast_bf16: Optional[bool] = None):
+    """The decoder config and precision for the reference's model config node (config/model/*.yaml): context_len,
+    config_args{base_model_name, vocab_size, twist_init, rope_theta, torch_dtype, dropout, ...}.  Host code only (reads the
+    base config, builds nothing on the GPU).  Returns (lm_cfg, master_weights).
+
+    The base config decides the decoder: Qwen2 (`LMConfig`), pre-LayerNorm OPT (`OptLMConfig`, the default TWIST / GSLM
+    base) or parallel-residual GPT-NeoX (`NeoxLMConfig`, the Pythia bases of config/train_inter_scale.yaml).  For OPT the
+    reference's `config_args` overrides are applied to the base config as `UnitLMConfig` does (pad / bos / eos ids,
+    dropout, attention_dropout, layerdrop), `rope_theta` is ignored, and `torch_dtype` picks the precision:
+      - bfloat16: bf16 parameters with bf16 AdamW moments;
+      - float32: fp32 master weights, fp32 gradients and fp32 AdamW moments with bf16 autocast numerics -- the
+        reference's default recipe, whose `torch_dtype: null` loads the model in fp32 and whose `bf16: true` trains under
+        autocast.  `autocast_bf16` is `training_args.bf16` where the caller has it: False asks for pure fp32 training,
+        which is refused.
+    `torch_dtype: null` is refused by name (pass bfloat16 or float32 explicitly).  GPT-NeoX takes the same overrides and
+    requires bfloat16.  Raises OSError when the base model cannot be reached (offline box) and ValueError when its
+    architecture or settings have no kernels here."""
     from transformers import AutoConfig
-    from .lm import B200UnitLM, OptLMConfig, lm_config_from_hf
+    from .lm import OptLMConfig, lm_config_from_hf
 
     args = cfg["config_args"] if isinstance(cfg, dict) else cfg.config_args
     get = args.get if hasattr(args, "get") else (lambda k, d=None: getattr(args, k, d))
     base = AutoConfig.from_pretrained(get("base_model_name"))
     ctx = int(cfg["context_len"] if isinstance(cfg, dict) else cfg.context_len)
+    master = False
     if getattr(base, "model_type", None) == "opt":
         # slamkit/model/unit_lm.py:59-63 passes these to AutoConfig.from_pretrained; the yaml's dropout keys arrive as
         # the same keyword arguments
         for k in ("pad_token_id", "bos_token_id", "eos_token_id", "dropout", "attention_dropout", "layerdrop"):
             if get(k) is not None:
                 setattr(base, k, get(k))
-        dt = get("torch_dtype")
-        if str(dt).replace("torch.", "") != "bfloat16":
-            raise ValueError(f"OPT on the GPU path trains bf16 parameters with bf16 AdamW moments; torch_dtype={dt} asks for "
-                             "fp32 master weights, which it does not implement (pass model.config_args.torch_dtype=bfloat16)")
+        dt = str(get("torch_dtype")).replace("torch.", "")
+        if dt == "float32":
+            if autocast_bf16 is False:
+                raise ValueError("OPT with model.config_args.torch_dtype=float32 trains fp32 master weights under bf16 autocast; "
+                                 "training_args.bf16=false asks for pure fp32 training, which the GPU path does not implement "
+                                 "(set training_args.bf16=true)")
+            master = True
+        elif dt != "bfloat16":
+            raise ValueError(f"OPT on the GPU path trains bf16 parameters with bf16 AdamW moments (torch_dtype=bfloat16) or "
+                             f"fp32 master weights under bf16 autocast (torch_dtype=float32); torch_dtype={get('torch_dtype')} "
+                             "names neither (pass model.config_args.torch_dtype=bfloat16 or model.config_args.torch_dtype=float32)")
     elif getattr(base, "model_type", None) == "gpt_neox":
         # UnitLMConfig (slamkit/model/unit_lm.py:59-63) hands pad / bos / eos (defaults 0 / 1 / 1) and the yaml's
         # remaining config_args to AutoConfig.from_pretrained
@@ -81,11 +95,26 @@ def tlm_b200_from_cfg(cfg, device: str = "cuda:0", max_batch: int = 8, max_seq: 
     lm_cfg = lm_config_from_hf(base, vocab_size=get("vocab_size", 502), max_positions=max(2048, ctx))
     if get("rope_theta") is not None and not isinstance(lm_cfg, OptLMConfig):
         lm_cfg.rope_theta = float(get("rope_theta"))
-    model = B200UnitLM(lm_cfg, device=device, max_batch=max_batch, max_seq=int(max_seq or ctx))
+    return lm_cfg, master
+
+
+def tlm_b200_from_cfg(cfg, device: str = "cuda:0", max_batch: int = 8, max_seq: Optional[int] = None,
+                      autocast_bf16: Optional[bool] = None):
+    """The `B200UnitLM` of the reference's model config node, with the decoder and precision `tlm_b200_config` picks
+    (OPT with `torch_dtype: float32` trains fp32 master weights, `master_weights=True`).  `twist_init` loads the base
+    model's HF weights (opt-125m ships fp16: with master weights they are widened to fp32, as the reference loads them;
+    the Pythia weights come from a local directory or cache), else the HF init is seeded."""
+    from .lm import B200UnitLM
+
+    args = cfg["config_args"] if isinstance(cfg, dict) else cfg.config_args
+    get = args.get if hasattr(args, "get") else (lambda k, d=None: getattr(args, k, d))
+    lm_cfg, master = tlm_b200_config(cfg, autocast_bf16)
+    ctx = int(cfg["context_len"] if isinstance(cfg, dict) else cfg.context_len)
+    model = B200UnitLM(lm_cfg, device=device, max_batch=max_batch, max_seq=int(max_seq or ctx), master_weights=master)
     if get("twist_init", True):
         from transformers import AutoModelForCausalLM
         import torch
-        hf = AutoModelForCausalLM.from_pretrained(get("base_model_name"), dtype=torch.bfloat16)
+        hf = AutoModelForCausalLM.from_pretrained(get("base_model_name"), dtype=torch.float32 if master else torch.bfloat16)
         hf.resize_token_embeddings(lm_cfg.vocab_size)
         model.load_hf_state_dict({"lm." + k: v for k, v in hf.state_dict().items()})
     else:

@@ -219,7 +219,7 @@ class LMOutput:
     stats: Optional[torch.Tensor] = None   # device fp32[3]: loss, n_valid_targets, nll_sum
 
 
-def _opt_base_config(c: "OptLMConfig") -> dict:
+def _opt_base_config(c: "OptLMConfig", torch_dtype: str = "bfloat16") -> dict:
     """The HF `OPTConfig` fields of a pre-LayerNorm OPT decoder of this shape (opt-125m layout)."""
     return {"model_type": "opt", "architectures": ["OPTForCausalLM"], "hidden_size": c.hidden, "ffn_dim": c.ffn,
             "num_hidden_layers": c.n_layers, "num_attention_heads": c.n_heads, "vocab_size": c.vocab_size,
@@ -227,7 +227,7 @@ def _opt_base_config(c: "OptLMConfig") -> dict:
             "activation_function": "relu", "enable_bias": True, "layer_norm_elementwise_affine": True,
             "_remove_final_layer_norm": False, "dropout": 0.0, "attention_dropout": 0.0, "layerdrop": 0.0,
             "init_std": c.init_std, "tie_word_embeddings": c.tie_embeddings, "pad_token_id": c.pad_token_id,
-            "bos_token_id": c.bos_token_id, "eos_token_id": c.eos_token_id, "torch_dtype": "bfloat16"}
+            "bos_token_id": c.bos_token_id, "eos_token_id": c.eos_token_id, "torch_dtype": torch_dtype}
 
 
 def _neox_base_config(c: "NeoxLMConfig") -> dict:
@@ -244,11 +244,12 @@ def _neox_base_config(c: "NeoxLMConfig") -> dict:
 
 
 def write_unit_lm_checkpoint(save_directory: str, state_dict_hf: Dict[str, torch.Tensor], config,
-                             base_model_name: Optional[str] = None) -> None:
+                             base_model_name: Optional[str] = None, torch_dtype: str = "bfloat16") -> None:
     """Writes `model.safetensors` with the `lm.`-prefixed names of `UnitLM.state_dict()` (base_model_prefix = "lm",
     slamkit/model/unit_lm.py:87) and a `config.json` in the `UnitLMConfig` layout (unit_lm.py:32-79), so that the
     reference's `UnitLM.from_pretrained(dir)` / cli/eval.py consume a model trained with this package.  Pure host code (no CUDA):
-    tests/test_host_cpu.py loads such a directory with the reference's own class."""
+    tests/test_host_cpu.py loads such a directory with the reference's own class.  `torch_dtype` names the tensors' dtype
+    ("float32" for an OPT model trained with fp32 master weights, as the reference's own run saves it)."""
     import json
     import os
     from safetensors.torch import save_file
@@ -261,7 +262,7 @@ def write_unit_lm_checkpoint(save_directory: str, state_dict_hf: Dict[str, torch
     sd = {k: v.detach().contiguous().cpu() for k, v in state_dict_hf.items()
           if k != "lm.lm_head.weight" or not c.tie_embeddings}
     save_file(sd, os.path.join(save_directory, "model.safetensors"), metadata={"format": "pt"})
-    base = _opt_base_config(c) if is_opt else _neox_base_config(c) if is_neox else {"model_type": "qwen2", "architectures": ["Qwen2ForCausalLM"], "hidden_size": c.hidden,
+    base = _opt_base_config(c, torch_dtype) if is_opt else _neox_base_config(c) if is_neox else {"model_type": "qwen2", "architectures": ["Qwen2ForCausalLM"], "hidden_size": c.hidden,
             "intermediate_size": c.ffn, "num_hidden_layers": c.n_layers, "num_attention_heads": c.n_heads,
             "num_key_value_heads": c.n_kv_heads, "vocab_size": c.vocab_size, "rms_norm_eps": c.rms_eps,
             "max_position_embeddings": c.max_positions, "tie_word_embeddings": c.tie_embeddings, "hidden_act": "silu",
@@ -269,7 +270,7 @@ def write_unit_lm_checkpoint(save_directory: str, state_dict_hf: Dict[str, torch
             "pad_token_id": c.pad_token_id, "bos_token_id": 1, "eos_token_id": 1, "torch_dtype": "bfloat16"}
     cfg = {"model_type": "speech_language_model", "architectures": ["UnitLM"], "base_model_name": base_model_name,
            "base_config": base, "vocab_size": c.vocab_size, "twist_init": False, "use_cache": False,
-           "tie_word_embeddings": c.tie_embeddings, "torch_dtype": "bfloat16",
+           "tie_word_embeddings": c.tie_embeddings, "torch_dtype": torch_dtype,
            "max_position_embeddings": c.max_positions}
     with open(os.path.join(save_directory, "config.json"), "w") as f:
         json.dump(cfg, f, indent=2)
@@ -295,12 +296,21 @@ class B200UnitLM:
     """Causal unit LM whose forward/backward/optimiser run in libslamkit_b200.so."""
 
     def __init__(self, config, device: str = "cuda:0", max_batch: int = 8, max_seq: int = 1024,
-                 trainable: bool = True, seed: Optional[int] = None):
-        """`config`: `LMConfig` (Qwen2 decoder) or `OptLMConfig` (pre-LayerNorm OPT decoder)."""
+                 trainable: bool = True, seed: Optional[int] = None, master_weights: bool = False):
+        """`config`: `LMConfig` (Qwen2 decoder), `OptLMConfig` (pre-LayerNorm OPT decoder) or `NeoxLMConfig` (GPT-NeoX).
+
+        `master_weights` (OPT only): train fp32 parameters, fp32 gradients and fp32 AdamW moments under bf16 autocast
+        numerics -- the reference's default recipe (`torch_dtype: null`, `bf16: true`).  `params32` / `grads32` then hold
+        the model; `params` is their bf16 shadow that the GEMMs read and `grads` the per-micro-batch bf16 scratch of the
+        linear gradients.  Such a model trains and scores; `generate` refuses it (generate from its saved checkpoint)."""
         self.lib = L.require_cuda()
         self.config = config
         self.is_opt = isinstance(config, OptLMConfig)
         self.is_neox = isinstance(config, NeoxLMConfig)
+        self.master = bool(master_weights)
+        if self.master and not self.is_opt:
+            raise ValueError("master_weights=True is implemented for the OPT decoder only (the Qwen2 and GPT-NeoX recipes "
+                             "train bf16 parameters)")
         self.device = torch.device(device)
         torch.cuda.set_device(self.device)
         self._h = C.c_void_p()
@@ -335,7 +345,13 @@ class B200UnitLM:
             self.rope_cos, self.rope_sin = cos.to(self.device), sin.to(self.device)
         self.max_batch, self.max_seq = max_batch, max_seq
         self.workspace = None
+        self.params32 = self.grads32 = None
         self._bind(max_batch, max_seq)
+        if self.master:
+            self.params32 = torch.zeros(self.n_params, device=self.device, dtype=torch.float32)
+            self.grads32 = torch.zeros(self.n_params, device=self.device, dtype=torch.float32) if trainable else None
+            L.check(self.lib.sk_lm_set_master(self._h, L.ptr(self.params32), L.ptr(self.grads32)))
+            self._bind(max_batch, max_seq)                # the fp32 residual stream needs the larger workspace
         self.stats = torch.zeros(3, device=self.device, dtype=torch.float32)
         if seed is not None:
             self.init_weights(seed)
@@ -354,9 +370,19 @@ class B200UnitLM:
             self._bind(B, T)
 
     def tensor(self, name: str, grad: bool = False) -> torch.Tensor:
+        """A parameter (or its gradient) as a [rows, cols] view of the flat buffers: the fp32 masters with master
+        weights, else the bf16 ones."""
         off, r, c = self.tensors[name]
-        flat = self.grads if grad else self.params
+        if self.master:
+            flat = self.grads32 if grad else self.params32
+        else:
+            flat = self.grads if grad else self.params
         return flat[off:off + r * c].view(r, c)
+
+    def refresh_shadow(self) -> None:
+        """Master weights: rewrite the bf16 shadow from the fp32 masters (after they are loaded or changed by hand)."""
+        if self.master:
+            self.params.copy_(self.params32)
 
     def __del__(self):
         try:
@@ -395,8 +421,9 @@ class B200UnitLM:
         g = torch.Generator(device="cpu").manual_seed(seed)
         cfg = self.config
         std = cfg.init_std
+        dt = torch.float32 if self.master else torch.bfloat16
         for name, (off, r, c) in self.tensors.items():
-            t = self.params[off:off + r * c].view(r, c)
+            t = self.tensor(name)
             base = name.split(".")[-1]
             if base in ("ln1", "ln2", "final_norm"):
                 t.fill_(1.0)
@@ -404,11 +431,12 @@ class B200UnitLM:
                 t.zero_()
             elif base in ("embed", "lm_head"):
                 t.zero_()
-                t[:cfg.vocab_size].copy_((torch.randn((cfg.vocab_size, c), generator=g) * std).to(torch.bfloat16))
+                t[:cfg.vocab_size].copy_((torch.randn((cfg.vocab_size, c), generator=g) * std).to(dt))
                 if base == "embed" and self.is_opt and 0 <= cfg.pad_token_id < cfg.vocab_size:
                     t[cfg.pad_token_id].zero_()
             else:
-                t.copy_((torch.randn((r, c), generator=g) * std).to(torch.bfloat16))
+                t.copy_((torch.randn((r, c), generator=g) * std).to(dt))
+        self.refresh_shadow()
 
     def _hf_map_opt(self) -> Iterator[Tuple[str, str, List[Tuple[int, int, int]]]]:
         """OPT names of `UnitLM.state_dict()` over OPTForCausalLM: q/k/v are row ranges of the fused `wqkv` / `bqkv`."""
@@ -504,9 +532,11 @@ class B200UnitLM:
         return t.view(-1, 1) if t.shape[0] == 1 else t
 
     def load_hf_state_dict(self, sd: Dict[str, torch.Tensor], grads: bool = False) -> None:
-        """Load parameters named as in `UnitLM.state_dict()` (prefix `lm.`, slamkit/model/unit_lm.py:87)."""
+        """Load parameters named as in `UnitLM.state_dict()` (prefix `lm.`, slamkit/model/unit_lm.py:87).  With master
+        weights the fp32 masters take the values (fp16 / bf16 checkpoints are widened exactly) and the bf16 shadow is
+        refreshed from them."""
         for flat, hf, segs in self._hf_map():
-            src = sd[hf].to(torch.bfloat16)
+            src = sd[hf].to(torch.float32 if self.master else torch.bfloat16)
             dst = self._flat_rows(flat, grads)
             if src.dim() == 1:
                 src = src.view(-1, 1)
@@ -515,6 +545,8 @@ class B200UnitLM:
                 continue
             for f0, h0, n in segs:
                 dst[f0:f0 + n].copy_(src[h0:h0 + n])
+        if not grads:
+            self.refresh_shadow()
 
     def state_dict_hf(self, grads: bool = False) -> Dict[str, torch.Tensor]:
         out = {}
@@ -533,11 +565,13 @@ class B200UnitLM:
 
     # ---- checkpoints (HF layout, SURVEY.md §5 / §8 f-4) ------------------------------------------------------------
     def save_pretrained(self, save_directory: str, base_model_name: Optional[str] = None) -> None:
-        write_unit_lm_checkpoint(save_directory, self.state_dict_hf(), self.config, base_model_name)
+        """With master weights the checkpoint holds the fp32 masters and says `torch_dtype: float32`."""
+        write_unit_lm_checkpoint(save_directory, self.state_dict_hf(), self.config, base_model_name,
+                                 torch_dtype="float32" if self.master else "bfloat16")
 
     @classmethod
     def from_pretrained(cls, directory: str, device: str = "cuda:0", max_batch: int = 8, max_seq: int = 1024,
-                        trainable: bool = True) -> "B200UnitLM":
+                        trainable: bool = True, master_weights: bool = False) -> "B200UnitLM":
         import json
         import os
         from safetensors.torch import load_file
@@ -557,7 +591,8 @@ class B200UnitLM:
             if not trainable:                              # dropout is inactive in eval mode
                 b.update(dropout=0.0, attention_dropout=0.0, layerdrop=0.0)
             lm_cfg = OptLMConfig.from_hf(OPTConfig(**b), vocab_size=cfg["vocab_size"])
-            m = cls(lm_cfg, device=device, max_batch=max_batch, max_seq=max_seq, trainable=trainable)
+            m = cls(lm_cfg, device=device, max_batch=max_batch, max_seq=max_seq, trainable=trainable,
+                    master_weights=master_weights)
             m.load_hf_state_dict(load_file(os.path.join(directory, "model.safetensors")))
             return m
         theta = (b.get("rope_parameters") or {}).get("rope_theta", b.get("rope_theta", 10000.0))
@@ -698,6 +733,9 @@ class B200UnitLM:
         The host looks at the rows' `finished` flags every 16 steps only.  Sampling draws from a Philox stream whose seed
         comes from `generator` (or torch's default CPU generator), so `torch.manual_seed` makes runs reproducible.
         Prompt plus continuation is bounded by `max_positions`."""
+        if self.master:
+            raise NotImplementedError("generate: this model trains fp32 master weights; generate from its saved checkpoint "
+                                      "(B200UnitLM.from_pretrained without master_weights)")
         generator = kwargs.pop("generator", None)
         if inputs is None:
             inputs = kwargs.pop("input_ids", None)
@@ -884,8 +922,9 @@ class B200AdamW:
         self.lr, self.betas, self.eps, self.wd = lr, betas, eps, weight_decay
         self.max_grad_norm = max_grad_norm
         self.emulate = emulate_bf16_norm
-        self.exp_avg = torch.zeros_like(model.params)
-        self.exp_avg_sq = torch.zeros_like(model.params)
+        # fp32 moments with master weights (torch.optim.AdamW keeps its state in the parameters' dtype)
+        self.exp_avg = torch.zeros_like(model.params32 if model.master else model.params)
+        self.exp_avg_sq = torch.zeros_like(self.exp_avg)
         self.step_count = 0
         self.stats = torch.zeros(3, device=model.device, dtype=torch.float32)  # total_norm, clip_coef, exact norm
 

@@ -52,6 +52,9 @@ class GradSync:
         self.model = model
         self.group = group
         self.world = dist.get_world_size(group) if dist.is_initialized() else 1
+        if getattr(model, "master", False) and self.world > 1:
+            raise NotImplementedError("data-parallel training of a model with fp32 master weights is not implemented (the "
+                                      "gradient all-reduce sums bf16 buffers); train it on one GPU")
         nl = model.config.n_layers
         t = model.tensors
         self.layer_start = [t[f"layers.{l}.ln1"][0] for l in range(nl)] + [t["final_norm"][0]]

@@ -5,6 +5,11 @@ batches and card, and cached greedy generate at B = 1 and 64.  Prints one JSON l
 and power limit first.
 
     python tools/opt_bench.py [--steps 20] [--warmup 5] [--out results.jsonl]
+    python tools/opt_bench.py --master [--steps 20] [--warmup 5] [--rounds 3]
+
+--master times bf16 parameters against fp32 master weights (the reference's default recipe: fp32 parameters,
+gradients and AdamW moments under bf16 autocast) on the same batches, alternating the two in rounds, and reports each
+mode's median step; then each mode's kernel split with the master-weight element-wise kernels and the optimiser named.
 
 Shapes: [8, 512] is config/model/default.yaml's context_len with config/training_args/default.yaml's per-device batch;
 [8, 1024] doubles the context."""
@@ -61,7 +66,14 @@ def time_steps(step, steps, warmup):
     return a.elapsed_time(b) / steps
 
 
-def split(step):
+SPLIT = (("gemm", ("gemm", "splitk")), ("attention", ("attn",)), ("layernorm", ("layernorm",)), ("relu_bwd", ("relu_bwd",)))
+# the master-weight element-wise kernels and the optimiser by name (checked in this order, before SPLIT's classes)
+SPLIT_MASTER = (("add_layernorm_f32", ("add_layernorm_f32",)), ("layernorm_bwd_f32", ("layernorm_bwd_f32",)),
+                ("widen_grads", ("widen_grads",)), ("adamw", ("adamw",)), ("grad_norm", ("sumsq", "gradnorm")),
+                ("embedding_fwd_bwd", ("embed", "scatter", "add_fix"))) + SPLIT
+
+
+def split(step, classes=SPLIT):
     """Device time of one step by kernel class, from a profiled step.  Run in a process of its own with SK_PDL=0: with
     programmatic dependent launch a kernel starts while its predecessor drains and waits inside, so kernel spans
     overlap and would not add up to the step."""
@@ -71,7 +83,8 @@ def split(step):
     with profile(activities=[ProfilerActivity.CUDA]) as prof:
         step()
         torch.cuda.synchronize()
-    out = {"gemm": 0.0, "attention": 0.0, "layernorm": 0.0, "relu_bwd": 0.0, "other": 0.0}
+    out = {name: 0.0 for name, _ in classes}
+    out["other"] = 0.0
     for e in prof.key_averages():
         us = getattr(e, "self_device_time_total", None)
         if us is None:
@@ -79,8 +92,7 @@ def split(step):
         if us <= 0 or e.key.startswith("cuda") or e.key.startswith("Memset") or e.key.startswith("Memcpy"):
             continue
         k = e.key.lower()
-        cat = ("gemm" if "gemm" in k or "splitk" in k else "attention" if "attn" in k else
-               "layernorm" if "layernorm" in k else "relu_bwd" if "relu_bwd" in k else "other")
+        cat = next((name for name, keys in classes if any(x in k for x in keys)), "other")
         out[cat] += us / 1e3
     out["total"] = sum(out.values())
     return {k: round(v, 3) for k, v in out.items()}
@@ -108,6 +120,54 @@ def bench_train(B, T, steps, warmup, out):
     del m, opt
     torch.cuda.empty_cache()
     return rec
+
+
+def bench_master(B, T, steps, warmup, rounds, out, profile_only=False):
+    """bf16 parameters against fp32 master weights at opt-125m geometry: both models on the same batch, timed in
+    alternating rounds (each round: `warmup` untimed steps, then `steps` steps timed one by one with device events), the
+    median step of each mode over all rounds."""
+    import statistics
+    ids, labels = batch(B, T, T)
+    n = float(B * T)
+    models = {}
+    for mode in ("bf16", "master"):
+        m = B200UnitLM(OptLMConfig(), device=DEV, max_batch=B, max_seq=T, seed=0, master_weights=mode == "master")
+        models[mode] = (m, B200AdamW(m, lr=1e-4, max_grad_norm=0.5))
+
+    def stepper(mode):
+        m, opt = models[mode]
+
+        def step():
+            m.forward_backward(ids, labels, num_items_in_batch=n)
+            opt.step()
+        return step
+    if profile_only:
+        for mode in models:
+            emit({"what": "opt125m_train_step_split", "impl": f"sk_{mode}_no_pdl", "B": B, "T": T,
+                  "kernel_ms": split(stepper(mode), SPLIT_MASTER)}, out)
+    else:
+        times = {mode: [] for mode in models}
+        for _ in range(rounds):
+            for mode in models:
+                step = stepper(mode)
+                for _ in range(warmup):
+                    step()
+                ev = [torch.cuda.Event(enable_timing=True) for _ in range(steps + 1)]
+                ev[0].record()
+                for i in range(steps):
+                    step()
+                    ev[i + 1].record()
+                torch.cuda.synchronize()
+                times[mode] += [ev[i].elapsed_time(ev[i + 1]) for i in range(steps)]
+        med = {mode: statistics.median(t) for mode, t in times.items()}
+        for mode, t in times.items():
+            emit({"what": "opt125m_train_step", "impl": f"sk_{mode}", "B": B, "T": T, "median_ms": round(med[mode], 3),
+                  "min_ms": round(min(t), 3), "max_ms": round(max(t), 3), "steps_timed": len(t),
+                  "loss": float(models[mode][0].stats[0])}, out)
+        emit({"what": "opt125m_master_overhead", "B": B, "T": T,
+              "master_over_bf16": round(med["master"] / med["bf16"] - 1.0, 4)}, out)
+    del models
+    torch.cuda.empty_cache()
 
 
 def bench_hf(B, T, steps, warmup, out):
@@ -158,7 +218,22 @@ def main():
     ap.add_argument("--warmup", type=int, default=5)
     ap.add_argument("--out", default=None)
     ap.add_argument("--split-only", action="store_true", help=argparse.SUPPRESS)
+    ap.add_argument("--master", action="store_true", help="bf16 parameters vs fp32 master weights, alternating")
+    ap.add_argument("--rounds", type=int, default=3)
     a = ap.parse_args()
+    if a.master and a.split_only:
+        for T in (512, 1024):
+            bench_master(8, T, a.steps, a.warmup, 1, a.out, profile_only=True)
+        return
+    if a.master:
+        if not torch.cuda.is_available():
+            raise SystemExit("opt_bench needs a CUDA device: there is nothing to measure on the CPU")
+        emit({"what": "card", "name_power_limit_max_sm_clock": card()}, a.out)
+        for T in (512, 1024):
+            bench_master(8, T, a.steps, a.warmup, a.rounds, a.out)
+        subprocess.run([sys.executable, os.path.abspath(__file__), "--master", "--split-only"] + (["--out", a.out] if a.out else []),
+                       env={**os.environ, "SK_PDL": "0"}, check=True)
+        return
     if a.split_only:
         for T in (512, 1024):
             bench_train(8, T, a.steps, a.warmup, a.out)
