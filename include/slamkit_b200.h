@@ -571,6 +571,32 @@ int sk_vocoder_durations(SkVocoder* v, const int64_t* codes, int ld, const int32
  * rows that fit the workspace.  Codes must have passed sk_vocoder_durations with status {0, 0}. */
 int sk_vocoder_run(SkVocoder* v, const int64_t* codes, int ld, const int32_t* counts, int B, const int32_t* frames_host,
                    float* wave, int64_t ldw, void* stream);
+/* Test hook: one convolution layer run exactly as sk_vocoder_run runs it (the same weight preparation and launcher).
+ * x fp32 [T_in, Cin] is staged through leaky_relu(., slope) (slope 1: identity).  A conv (transposed 0: rate 1, odd k,
+ * padding (k - 1) * dilation / 2) gives T_out = T_in; a ConvTranspose1d (stride rate, padding (k - rate) / 2, k - rate
+ * even) gives T_out = T_in * rate.  weight is torch's layout (Conv1d [Cout, Cin, k], ConvTranspose1d [Cin, Cout, k]),
+ * bias fp32 [Cout].  Output position o is zero when valid[o / up] == 0 (uint8 [T_out / up]); else
+ *   v = acc + bias;  v += res[o] (when res);  mode 2: v = sum[o] + v;  divide > 0: v = v / divide,
+ * stored to y [T_out, Cout] in mode 0, or to sum [T_out, Cout] in modes 1 and 2 (y is not written).  prep: device scratch
+ * of 2 * 2 * k * round_up(Cout, 64) * round_up(Cin, 32) bytes for the split bf16 weights.  Cin and Cout are multiples of 4;
+ * every argument is checked before anything is launched. */
+typedef struct SkVocoderConvDesc {
+  int32_t T_in, Cin, Cout, k;
+  int32_t transposed, rate, dilation;
+  float slope;
+  const float* x;
+  const float* weight;
+  const float* bias;
+  const uint8_t* valid;
+  int32_t up, mode;
+  float* y;
+  const float* res;
+  float* sum;
+  int32_t divide;
+  void* prep;
+  int64_t prep_bytes;
+} SkVocoderConvDesc;
+int sk_vocoder_conv(const SkVocoderConvDesc* desc, void* stream);
 
 /* ---- host-side FLAC decoding (no audio decoder exists in the image) ------------------------------------------------
  * Replaces torchaudio.info / torchaudio.load in cli/extract_features.py:45-57.  Host pointers. md5_16 receives the

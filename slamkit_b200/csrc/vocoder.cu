@@ -33,6 +33,8 @@ constexpr int KC = 32;       // input channels per staged chunk
 constexpr int LDS = KC + 8;  // smem row pitch in bf16 (80 bytes: 16-byte aligned rows, conflict-free ldmatrix)
 constexpr int CPAD = 64;     // prepared weights: output channels padded to a multiple of this
 constexpr int MAX_TAPS = 32;
+constexpr size_t CONV_SMEM_MAX = 96 * 1024;   // dynamic shared memory a convolution may request
+constexpr size_t DUR_SMEM_MAX = 48 * 1024;    // dur_kernel runs without raising the default limit
 
 inline int64_t align_up(int64_t x, int64_t a) { return (x + a - 1) / a * a; }
 inline int round_up(int x, int a) { return (x + a - 1) / a * a; }
@@ -412,6 +414,38 @@ struct Tensor {
   int64_t off, numel;
 };
 
+// One convolution layer: offsets of its fp32 weight and bias in the flat buffer and of its prepared split weights.
+struct ConvLayer { int64_t w, b, prep; int Cout, Cin, k, transposed, u, dil, Cout_pad, Cin_pad; };
+
+ConvLayer conv_layer(int Cout, int Cin, int k, int transposed, int u, int dil) {
+  ConvLayer L;
+  L.w = L.b = L.prep = 0;
+  L.Cout = Cout; L.Cin = Cin; L.k = k; L.transposed = transposed; L.u = u; L.dil = dil;
+  L.Cout_pad = round_up(Cout, CPAD);
+  L.Cin_pad = round_up(Cin, KC);
+  return L;
+}
+
+int64_t prep_elems(const ConvLayer& L) { return (int64_t)L.k * L.Cout_pad * L.Cin_pad; }
+
+// tile width (n8 tiles per warp) the launcher picks from the output channels
+int conv_nt(int Cout) { return Cout >= 64 ? 4 : Cout >= 32 ? 2 : 1; }
+
+// dynamic shared memory of a conv CTA: the activation tile plus a halo of `span` rows (hi and lo), and one tap's weights
+size_t conv_smem_bytes(int span, int NT) { return ((size_t)2 * (BM + span) * LDS + 2 * 16 * NT * LDS) * sizeof(bf16); }
+
+// widest halo of the layer's phases, in rows
+int halo_span(const ConvLayer& L) { return L.transposed ? (L.k + L.u - 1) / L.u - 1 : (L.k - 1) * L.dil; }
+
+size_t dur_smem_bytes(int E, int H) { return (5 * (size_t)E + 3 * (size_t)H + 32) * sizeof(float); }
+
+int prepare_layer(const ConvLayer& L, const float* w, bf16* hi, bf16* lo, cudaStream_t s) {
+  const int blocks = (int)std::min<int64_t>((prep_elems(L) + 255) / 256, 4096);
+  prepare_kernel<<<blocks, 256, 0, s>>>(w, L.Cout, L.Cin, L.k, L.transposed, L.u, L.Cout_pad, L.Cin_pad, hi, lo);
+  SK_LAUNCH_CHECK();
+  return 0;
+}
+
 }  // namespace
 
 struct SkVocoder {
@@ -420,8 +454,7 @@ struct SkVocoder {
   std::vector<Tensor> tensors;
   int64_t n_params = 0;
   // prepared conv layers (order: conv_pre, per stage: ups, resblocks' convs1/convs2 interleaved)
-  struct Layer { int64_t w, b, prep; int Cout, Cin, k, transposed, u, dil, Cout_pad, Cin_pad; };
-  std::vector<Layer> layers;
+  std::vector<ConvLayer> layers;
   int64_t prep_elems = 0;
   int64_t t_dict = -1, t_spk = -1, t_sty = -1, t_dur = -1, t_post_w = -1, t_post_b = -1;
   int64_t T0_cap = 0, act_elems = 0;
@@ -448,16 +481,13 @@ int64_t add_tensor(SkVocoder* v, const char* name, int64_t numel) {
 
 void add_conv(SkVocoder* v, const char* base, int Cout, int Cin, int k, int transposed, int u, int dil) {
   char nm[64];
-  SkVocoder::Layer L;
+  ConvLayer L = conv_layer(Cout, Cin, k, transposed, u, dil);
   snprintf(nm, sizeof nm, "%s.weight", base);
   L.w = add_tensor(v, nm, (int64_t)Cout * Cin * k);
   snprintf(nm, sizeof nm, "%s.bias", base);
   L.b = add_tensor(v, nm, Cout);
-  L.Cout = Cout; L.Cin = Cin; L.k = k; L.transposed = transposed; L.u = u; L.dil = dil;
-  L.Cout_pad = round_up(Cout, CPAD);
-  L.Cin_pad = round_up(Cin, KC);
   L.prep = v->prep_elems;
-  v->prep_elems += align_up((int64_t)k * L.Cout_pad * L.Cin_pad, 128);
+  v->prep_elems += align_up(prep_elems(L), 128);
   v->layers.push_back(L);
 }
 
@@ -466,8 +496,8 @@ int launch_conv_nt(const ConvParams& p, int n_tiles_m, cudaStream_t s) {
   constexpr int BN = 16 * NT;
   int maxspan = 0;
   for (int r = 0; r < p.n_phase; ++r) maxspan = std::max(maxspan, (p.ntaps[r] - 1) * abs(p.in_step));
-  const size_t smem = ((size_t)2 * (BM + maxspan) * LDS + 2 * BN * LDS) * sizeof(bf16);
-  SK_REQUIRE(smem <= 96 * 1024, "sk_vocoder: convolution halo too wide (%zu bytes of shared memory)", smem);
+  const size_t smem = conv_smem_bytes(maxspan, NT);
+  SK_REQUIRE(smem <= CONV_SMEM_MAX, "sk_vocoder: convolution halo too wide (%zu bytes of shared memory)", smem);
   SK_CUDA_CHECK(cudaFuncSetAttribute(vocoder_conv_kernel<NT>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
   dim3 grid(n_tiles_m, (p.Cout + BN - 1) / BN, p.n_phase);
   vocoder_conv_kernel<NT><<<grid, 256, smem, s>>>(p);
@@ -477,18 +507,22 @@ int launch_conv_nt(const ConvParams& p, int n_tiles_m, cudaStream_t s) {
 
 int launch_conv(const ConvParams& p, cudaStream_t s) {
   const int tiles = (p.Q + BM - 1) / BM;
-  if (p.Cout >= 64) return launch_conv_nt<4>(p, tiles, s);
-  if (p.Cout >= 32) return launch_conv_nt<2>(p, tiles, s);
-  return launch_conv_nt<1>(p, tiles, s);
+  switch (conv_nt(p.Cout)) {
+    case 4: return launch_conv_nt<4>(p, tiles, s);
+    case 2: return launch_conv_nt<2>(p, tiles, s);
+    default: return launch_conv_nt<1>(p, tiles, s);
+  }
 }
 
-// One convolution layer over the packed timeline at `up` positions per frame.
-int run_layer(const SkVocoder* v, const SkVocoder::Layer& L, const float* x, int T_in, int T_out, float slope, float* y,
-              const float* res, float* sum, int mode, int divide, int up, cudaStream_t s) {
+// One convolution layer over the packed timeline at `up` positions per frame, from its prepared (split) weights.
+// The network and the sk_vocoder_conv test hook both run every layer through here.
+int run_layer(const ConvLayer& L, const bf16* w_hi, const bf16* w_lo, const float* bias, const uint8_t* valid,
+              const float* x, int T_in, int T_out, float slope, float* y, const float* res, float* sum, int mode, int divide,
+              int up, cudaStream_t s) {
   ConvParams p;
   memset(&p, 0, sizeof p);
   p.x = x; p.T_in = T_in; p.Cin = L.Cin; p.Cin_pad = L.Cin_pad;
-  p.w_hi = v->hi + L.prep; p.w_lo = v->lo + L.prep;
+  p.w_hi = w_hi; p.w_lo = w_lo;
   p.Cout = L.Cout; p.Cout_pad = L.Cout_pad;
   if (!L.transposed) {
     const int pad = (L.k * L.dil - L.dil) / 2;
@@ -504,8 +538,8 @@ int run_layer(const SkVocoder* v, const SkVocoder::Layer& L, const float* x, int
     p.out_mul = u; p.out_off = -pad; p.Q = T_in + (pad + u - 1) / u;
   }
   p.T_out = T_out; p.slope = slope;
-  p.bias = v->w + L.b; p.y = y; p.res = res; p.sum = sum; p.mode = mode; p.divide = divide;
-  p.valid = v->valid; p.up = up;
+  p.bias = bias; p.y = y; p.res = res; p.sum = sum; p.mode = mode; p.divide = divide;
+  p.valid = valid; p.up = up;
   return launch_conv(p, s);
 }
 
@@ -522,7 +556,7 @@ int enqueue_durations(SkVocoder* v, const int64_t* codes, int ld, const int32_t*
     const int64_t d = v->t_dur;
     const float* W = v->w;
     const int threads = round_up(H, 32);
-    const size_t smem = (size_t)(5 * E + 3 * H + 32) * sizeof(float);
+    const size_t smem = dur_smem_bytes(E, H);
     dim3 grid(std::min(ld, MU), B);
     // tensor order: conv1.w, conv1.b, ln1.w, ln1.b, conv2.w, conv2.b, ln2.w, ln2.b, proj.w, proj.b
     const int64_t o_c1w = d, o_c1b = o_c1w + align_up((int64_t)H * E * 3, 4), o_l1w = o_c1b + align_up(H, 4),
@@ -551,24 +585,29 @@ int enqueue_network(SkVocoder* v, int B, int T0, float* wave, int ldw, cudaStrea
   const int nk = c.n_resblocks;
   size_t li = 0;
   float *X = v->buf[0], *Y = v->buf[1], *Tm = v->buf[2], *S = v->buf[3];
-  VOC_TRY(run_layer(v, v->layers[li++], v->x0, T0, T0, 1.f, S, nullptr, nullptr, 0, 0, 1, s));   // conv_pre
+  auto run = [&](const ConvLayer& L, const float* x, int T_in, int T_out, float slope, float* y, const float* res, float* sum,
+                 int mode, int divide, int up) {
+    return run_layer(L, v->hi + L.prep, v->lo + L.prep, W + L.b, v->valid, x, T_in, T_out, slope, y, res, sum, mode, divide,
+                     up, s);
+  };
+  VOC_TRY(run(v->layers[li++], v->x0, T0, T0, 1.f, S, nullptr, nullptr, 0, 0, 1));   // conv_pre
   int U = 1;
   for (int i = 0; i < c.n_upsamples; ++i) {
     const int T_in = T0 * U, u = c.upsample_rates[i];
     U *= u;
     const int T = T0 * U;
-    VOC_TRY(run_layer(v, v->layers[li++], S, T_in, T, 0.1f, X, nullptr, nullptr, 0, 0, U, s));     // ups[i]
+    VOC_TRY(run(v->layers[li++], S, T_in, T, 0.1f, X, nullptr, nullptr, 0, 0, U));     // ups[i]
     for (int j = 0; j < nk; ++j) {
       const float* cur = X;
       for (int a = 0; a < 3; ++a) {
-        const SkVocoder::Layer& c1 = v->layers[li++];
-        const SkVocoder::Layer& c2 = v->layers[li++];
-        VOC_TRY(run_layer(v, c1, cur, T, T, 0.1f, Tm, nullptr, nullptr, 0, 0, U, s));
+        const ConvLayer& c1 = v->layers[li++];
+        const ConvLayer& c2 = v->layers[li++];
+        VOC_TRY(run(c1, cur, T, T, 0.1f, Tm, nullptr, nullptr, 0, 0, U));
         if (a < 2) {
-          VOC_TRY(run_layer(v, c2, Tm, T, T, 0.1f, Y, cur, nullptr, 0, 0, U, s));
+          VOC_TRY(run(c2, Tm, T, T, 0.1f, Y, cur, nullptr, 0, 0, U));
           cur = Y;
         } else {   // last conv of the ResBlock: add the residual, then into the running sum (and the mean at the end)
-          VOC_TRY(run_layer(v, c2, Tm, T, T, 0.1f, nullptr, cur, S, j == 0 ? 1 : 2, j == nk - 1 ? nk : 0, U, s));
+          VOC_TRY(run(c2, Tm, T, T, 0.1f, nullptr, cur, S, j == 0 ? 1 : 2, j == nk - 1 ? nk : 0, U));
         }
       }
     }
@@ -607,13 +646,18 @@ int sk_vocoder_create(const SkVocoderConfig* cfg, SkVocoder** out) {
                "rate samples)", i);
     G0 = std::max(G0, ((k + u - 1) / u + 1 + U - 1) / U);   // transposed-conv input reach at the stage's input resolution
     U *= u;
+    const int ch = c.upsample_initial_channel >> (i + 1);
     int reach = 0;
     for (int j = 0; j < c.n_resblocks; ++j) {
       const int rk = c.resblock_kernel_sizes[j];
       SK_REQUIRE(rk % 2 == 1 && rk <= MAX_TAPS, "sk_vocoder_create: ResBlock kernels must be odd, <= %d", MAX_TAPS);
       for (int a = 0; a < 3; ++a) {
-        SK_REQUIRE(c.resblock_dilations[j][a] >= 1, "sk_vocoder_create: dilations must be positive");
-        reach = std::max(reach, (rk - 1) * c.resblock_dilations[j][a] / 2);
+        const int dil = c.resblock_dilations[j][a];
+        SK_REQUIRE(dil >= 1 && dil <= 1024, "sk_vocoder_create: dilations must be in [1, 1024]");
+        const size_t smem = conv_smem_bytes((rk - 1) * dil, conv_nt(ch));
+        SK_REQUIRE(smem <= CONV_SMEM_MAX, "sk_vocoder_create: stage %d: ResBlock kernel %d at dilation %d (%d channels) "
+                   "needs %zu bytes of shared memory for its halo, more than %zu", i, rk, dil, ch, smem, CONV_SMEM_MAX);
+        reach = std::max(reach, (rk - 1) * dil / 2);
       }
     }
     G0 = std::max(G0, (reach + U - 1) / U);
@@ -622,6 +666,10 @@ int sk_vocoder_create(const SkVocoderConfig* cfg, SkVocoder** out) {
   SK_REQUIRE(!c.dur_predictor || (c.dur_kernel == 3 && c.dur_hidden >= 1 && c.dur_hidden <= 1024),
              "sk_vocoder_create: the duration predictor needs var_pred_kernel_size 3 (its second conv has padding 1) and "
              "var_pred_hidden_dim <= 1024");
+  SK_REQUIRE(!c.dur_predictor || dur_smem_bytes(c.embedding_dim, c.dur_hidden) <= DUR_SMEM_MAX,
+             "sk_vocoder_create: the duration predictor needs (5 x embedding_dim + 3 x var_pred_hidden_dim + 32) x 4 = %zu "
+             "bytes of shared memory (embedding_dim %d, var_pred_hidden_dim %d), more than %zu",
+             dur_smem_bytes(c.embedding_dim, c.dur_hidden), c.embedding_dim, c.dur_hidden, DUR_SMEM_MAX);
   SkVocoder* v = new (std::nothrow) SkVocoder();
   SK_REQUIRE(v, "sk_vocoder_create: out of host memory");
   v->cfg = c;
@@ -716,13 +764,7 @@ int sk_vocoder_bind(SkVocoder* v, const float* weights, void* prepared, int64_t 
   v->w = weights;
   v->hi = (bf16*)prepared;
   v->lo = v->hi + v->prep_elems;
-  for (const auto& L : v->layers) {
-    const int64_t n = (int64_t)L.k * L.Cout_pad * L.Cin_pad;
-    const int blocks = (int)std::min<int64_t>((n + 255) / 256, 4096);
-    prepare_kernel<<<blocks, 256, 0, s>>>(weights + L.w, L.Cout, L.Cin, L.k, L.transposed, L.u, L.Cout_pad, L.Cin_pad,
-                                          v->hi + L.prep, v->lo + L.prep);
-    SK_LAUNCH_CHECK();
-  }
+  for (const auto& L : v->layers) VOC_TRY(prepare_layer(L, weights + L.w, v->hi + L.prep, v->lo + L.prep, s));
   const int64_t R = v->cfg.max_rows, MU = v->cfg.max_frames;
   unsigned char* p = (unsigned char*)workspace;
   auto take = [&](int64_t bytes) { unsigned char* r = p; p += align_up(bytes, 256); return r; };
@@ -789,6 +831,46 @@ int sk_vocoder_run(SkVocoder* v, const int64_t* codes, int ld, const int32_t* co
     b0 = b1;
   }
   return 0;
+}
+
+int sk_vocoder_conv(const SkVocoderConvDesc* desc, void* stream) {
+  SK_REQUIRE(desc, "sk_vocoder_conv: null descriptor");
+  const SkVocoderConvDesc& d = *desc;
+  SK_REQUIRE(d.x && d.weight && d.bias && d.valid && d.prep, "sk_vocoder_conv: null x, weight, bias, valid or prep");
+  SK_REQUIRE(d.T_in >= 1, "sk_vocoder_conv: T_in = %d must be positive", d.T_in);
+  SK_REQUIRE(d.Cin > 0 && d.Cin % 4 == 0 && d.Cout > 0 && d.Cout % 4 == 0,
+             "sk_vocoder_conv: Cin = %d and Cout = %d must be positive multiples of 4", d.Cin, d.Cout);
+  SK_REQUIRE(d.k >= 1 && d.k <= MAX_TAPS, "sk_vocoder_conv: kernel %d outside [1, %d]", d.k, MAX_TAPS);
+  if (d.transposed)
+    SK_REQUIRE(d.rate >= 1 && d.rate <= d.k && (d.k - d.rate) % 2 == 0 && d.dilation == 1,
+               "sk_vocoder_conv: a transposed conv needs 1 <= rate <= kernel, kernel - rate even and dilation 1 "
+               "(rate %d, kernel %d, dilation %d)", d.rate, d.k, d.dilation);
+  else
+    SK_REQUIRE(d.rate == 1 && d.k % 2 == 1 && d.dilation >= 1 && d.dilation <= 1024,
+               "sk_vocoder_conv: a conv needs rate 1, an odd kernel and a dilation in [1, 1024] (rate %d, kernel %d, "
+               "dilation %d)", d.rate, d.k, d.dilation);
+  const int64_t T_out = d.transposed ? (int64_t)d.T_in * d.rate : d.T_in;
+  SK_REQUIRE(T_out <= INT32_MAX / 4, "sk_vocoder_conv: %lld output positions are too many", (long long)T_out);
+  SK_REQUIRE(d.up >= 1 && T_out % d.up == 0, "sk_vocoder_conv: up = %d must divide T_out = %lld", d.up, (long long)T_out);
+  SK_REQUIRE(d.mode >= 0 && d.mode <= 2 && d.divide >= 0, "sk_vocoder_conv: mode %d must be 0..2 and divide %d >= 0",
+             d.mode, d.divide);
+  SK_REQUIRE(d.mode == 0 ? (d.y && !d.divide) : d.sum != nullptr,
+             "sk_vocoder_conv: mode 0 writes y (and does not divide); modes 1 and 2 write sum");
+  SK_REQUIRE((uintptr_t)d.x % 16 == 0 && (uintptr_t)d.prep % 16 == 0 &&
+                 ((uintptr_t)d.y | (uintptr_t)d.res | (uintptr_t)d.sum) % 8 == 0,
+             "sk_vocoder_conv: x and prep must be 16-byte aligned, y, res and sum 8-byte aligned");
+  const ConvLayer L = conv_layer(d.Cout, d.Cin, d.k, d.transposed, d.transposed ? d.rate : 1, d.dilation);
+  const int64_t need = 2 * prep_elems(L) * (int64_t)sizeof(bf16);
+  SK_REQUIRE(d.prep_bytes >= need, "sk_vocoder_conv: prep holds %lld bytes, the split weights need %lld",
+             (long long)d.prep_bytes, (long long)need);
+  const size_t smem = conv_smem_bytes(halo_span(L), conv_nt(d.Cout));
+  SK_REQUIRE(smem <= CONV_SMEM_MAX, "sk_vocoder_conv: kernel %d at dilation %d needs %zu bytes of shared memory for its "
+             "halo, more than %zu", d.k, d.dilation, smem, CONV_SMEM_MAX);
+  cudaStream_t s = (cudaStream_t)stream;
+  bf16* hi = (bf16*)d.prep;
+  bf16* lo = hi + prep_elems(L);
+  VOC_TRY(prepare_layer(L, d.weight, hi, lo, s));
+  return run_layer(L, hi, lo, d.bias, d.valid, d.x, d.T_in, (int)T_out, d.slope, d.y, d.res, d.sum, d.mode, d.divide, d.up, s);
 }
 
 }  // extern "C"

@@ -41,6 +41,19 @@ class SkVocoderConfig(C.Structure):
     ]
 
 
+class SkVocoderConvDesc(C.Structure):
+    """sk_vocoder_conv: one convolution layer of the network, run as sk_vocoder_run runs it (see the header)."""
+    _fields_ = [
+        ("T_in", C.c_int32), ("Cin", C.c_int32), ("Cout", C.c_int32), ("k", C.c_int32),
+        ("transposed", C.c_int32), ("rate", C.c_int32), ("dilation", C.c_int32), ("slope", C.c_float),
+        ("x", C.c_void_p), ("weight", C.c_void_p), ("bias", C.c_void_p), ("valid", C.c_void_p),
+        ("up", C.c_int32), ("mode", C.c_int32),
+        ("y", C.c_void_p), ("res", C.c_void_p), ("sum", C.c_void_p),
+        ("divide", C.c_int32),
+        ("prep", C.c_void_p), ("prep_bytes", C.c_int64),
+    ]
+
+
 def parse_config(cfg: Dict) -> Dict:
     """The geometry of a `CodeGenerator` JSON config (generator.py:24-125), or ValueError for what the reference's
     `vocode()` cannot run either (f0 conditioning, `embedder_params`) and for what these kernels do not implement."""
