@@ -56,7 +56,10 @@ def load_model(cfg, device: str, max_seq: int = 256):
     if base.get("model_type") not in ("qwen2", "opt", "gpt_neox"):
         raise ValueError(f"unsupported base architecture '{base.get('model_type')}' in {path}: the GPU scoring path "
                          "implements the Qwen2, OPT and GPT-NeoX decoders")
-    return B200UnitLM.from_pretrained(path, device=device, max_batch=cfg.batch_size, max_seq=max_seq, trainable=False)
+    m = B200UnitLM.from_pretrained(path, device=device, max_batch=cfg.batch_size, max_seq=max_seq, trainable=False)
+    logger.info("%s: %s", path, "float32 checkpoint, fp32 inference (split-bf16 GEMMs, fp32 logits and scores)" if m.fp32
+                else "bf16 inference")
+    return m
 
 
 def build_tokeniser(cfg, device: str):

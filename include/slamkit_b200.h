@@ -225,6 +225,10 @@ int sk_attn_bwd(const void* q, const void* k, const void* v, const void* o, cons
  * hi = bf16(o), lo = bf16(o - hi). */
 int sk_attn_tc_fwd_split(const void* qkv_hi, const void* qkv_lo, void* o_hi, void* o_lo, int B, int T, int H, int ld,
                          int ldo, float scale, void* stream);
+/* The causal instance of the same kernel (fp32 OPT inference): row t attends to keys 0..t of its batch row.  No key tile
+ * past a query tile's diagonal is read. */
+int sk_attn_tc_fwd_split_causal(const void* qkv_hi, const void* qkv_lo, void* o_hi, void* o_lo, int B, int T, int H, int ld,
+                                int ldo, float scale, void* stream);
 
 /* ---- optimiser ----------------------------------------------------------------------------------------------------
  * Gradient clipping + AdamW as HF Trainer runs them (HF:trainer.py clip_grad_norm_ then torch.optim.AdamW(fused)):
@@ -352,6 +356,19 @@ int sk_lm_bind(SkLm* lm, void* params, void* grads, const void* rope_cos, const 
  *   - sk_lm_prefill / sk_lm_decode_step refuse the handle (generation runs on the saved checkpoint).
  * Qwen2 and GPT-NeoX handles are refused. */
 int sk_lm_set_master(SkLm* lm, float* params32, float* grads32);
+/* OPT handles only, after sk_lm_bind: fp32 inference, as the reference scores and generates a float32 checkpoint (HF
+ * OPTForCausalLM in fp32, no autocast).  params32 is a caller-owned flat fp32 [param_count] buffer in the bf16 layout
+ * (it stays referenced); `prepared` (>= sk_lm_fp32_prepared_bytes, 256-byte aligned) receives its split-bf16 (hi, lo)
+ * copy, written on `stream`.  Call again after params32 changes.  From then on the handle is forward only:
+ *   - every linear is the split-bf16 three-product GEMM with fp32 bias; activations and the residual stream are (hi, lo)
+ *     pairs; LayerNorms use fp32 gamma / beta; attention is the causal split-bf16 kernel; fp32-grade throughout;
+ *   - sk_lm_forward (labels and pos_ids NULL) writes fp32 logits, read through sk_lm_logits_f32 (sk_lm_logits is NULL);
+ *   - sk_lm_prefill / sk_lm_decode_step write fp32 logits [B, ldl]; the KV cache is fp32 (sk_lm_kv_cache_bytes);
+ *   - sk_lm_workspace_bytes and sk_lm_decode_workspace_bytes report the fp32-grade sizes: bind the workspace again;
+ *   - sk_lm_forward_backward, sk_lm_forward_rows, sk_lm_backward_weighted and sk_lm_optimizer_step are refused.
+ * Mutually exclusive with sk_lm_set_master.  Qwen2 and GPT-NeoX handles are refused; hidden <= 1024. */
+int64_t sk_lm_fp32_prepared_bytes(const SkLm* lm);
+int sk_lm_set_fp32(SkLm* lm, const float* params32, void* prepared, int64_t prepared_bytes, void* stream);
 /* Forward only (eval / log-likelihood): logits stay in the workspace, see sk_lm_logits. labels may be NULL.
  * pos_ids: int32 [B*T] or NULL (positions 0..T-1 per row).  When given they drive RoPE AND mark packed documents: a
  * document starts wherever pos_ids == 0, and tokens attend only within their document (the reference's varlen
@@ -381,6 +398,8 @@ int sk_lm_backward_weighted(SkLm* lm, const int64_t* ids, const int64_t* labels,
 /* bf16 [B*T, sk_lm_logits_ld()] logits of the last forward (valid columns: vocab_size). */
 const void* sk_lm_logits(const SkLm* lm);
 int sk_lm_logits_ld(const SkLm* lm);
+/* fp32 [B*T, sk_lm_logits_ld()] logits of the last forward of an fp32 inference handle (NULL on other handles). */
+const float* sk_lm_logits_f32(const SkLm* lm);
 /* Clip (max_norm <= 0 disables) + AdamW over the bound params/grads; moments are caller-owned flat bf16 buffers.
  * stats fp32[3] as sk_grad_norm. */
 int sk_lm_optimizer_step(SkLm* lm, void* exp_avg, void* exp_avg_sq, float lr, float beta1, float beta2, float eps,
@@ -414,6 +433,11 @@ int sk_lm_decode_step(SkLm* lm, const int64_t* tokens, const int32_t* pos, int B
 int64_t sk_attn_decode_partial_bytes(int B, int H, int T_cache);
 int sk_attn_decode(const void* q, int ldq, const void* k_cache, const void* v_cache, const int32_t* lens, void* o, int ldo,
                    float* partial, int B, int H, int KVH, int T_cache, float scale, void* stream);
+/* The same over an fp32 cache (fp32 inference): q = q_hi + q_lo (bf16 pairs, pitch ldq), k_cache / v_cache
+ * [B][H][T_cache][64] fp32, the fp32 result written as the pair o_hi = bf16(o), o_lo = bf16(o - o_hi) (pitch ldo). */
+int sk_attn_decode_split(const void* q_hi, const void* q_lo, int ldq, const float* k_cache, const float* v_cache,
+                         const int32_t* lens, void* o_hi, void* o_lo, int ldo, float* partial, int B, int H, int T_cache,
+                         float scale, void* stream);
 /* Token selection settings (HF GenerationConfig fields). */
 typedef struct SkSampling {
   uint64_t seed;             /* Philox key of the draws */
@@ -445,6 +469,9 @@ typedef struct SkDecodeState {
  * n_gen[b], tokens[b], pos[b] (+1) and finished[b] (eos) are updated; the step index advances by one per call. */
 int sk_select_next(const void* logits, int ldl, int V, int B, const uint32_t* ban_bits, const SkSampling* cfg,
                    const float* uniforms, const SkDecodeState* state, void* stream);
+/* sk_select_next on fp32 logits [B, ldl] (fp32 inference handles); logits 16-byte aligned. */
+int sk_select_next_f32(const float* logits, int ldl, int V, int B, const uint32_t* ban_bits, const SkSampling* cfg,
+                       const float* uniforms, const SkDecodeState* state, void* stream);
 
 /* ---- sequence scoring (modelling metrics of cli/eval.py) ---------------------------------------------------------------
  * The tail of UnitLM.log_likelihood (slamkit/model/unit_lm.py:184-194 -> calc_nll, slamkit/utils/calculation_utils.py:5-29)
@@ -460,6 +487,10 @@ int sk_select_next(const void* logits, int ldl, int V, int B, const uint32_t* ba
  * ldl % 8 == 0, logits 16-byte aligned. */
 int sk_seq_loglik(const void* logits, int ldl, int V, const int64_t* ids, int B, int T, int pad_id, const uint32_t* ban_bits,
                   int mean_nll, float* token_nll, void* ll_out, void* stream);
+/* The same contract on fp32 logits of an fp32 model, as calc_nll runs on them: no bf16 rounding anywhere,
+ *   token_nll[b, t] = -((z_y - max) - log(sum exp(z - max))),  ll_out[b] (fp32) = -sum_t, or -(sum / count). */
+int sk_seq_loglik_f32(const float* logits, int ldl, int V, const int64_t* ids, int B, int T, int pad_id,
+                      const uint32_t* ban_bits, int mean_nll, float* token_nll, float* ll_out, void* stream);
 /* UnitTokeniser.tokenise on the device (slamkit/tokeniser/unit_tokeniser.py:40-73 with its `<S> $0 <S>` template): sk_rle's
  * units int32 [B, T_units] and counts int32 [B] -> right-padded ids int64 [B, T_out] = [bos, units + offset..., eos, pad...].
  * T_out = max(counts) + 2 gives the batch tokenise() builds. */

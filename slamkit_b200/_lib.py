@@ -160,10 +160,10 @@ def load() -> C.CDLL:
     for name in ("sk_lm_param_count", "sk_lm_workspace_bytes", "sk_launch_count", "sk_hubert_param_count", "sk_hubert_prepared_bytes",
                  "sk_hubert_workspace_bytes", "sk_gemm_ws_bytes", "sk_lm_kv_cache_bytes", "sk_lm_decode_workspace_bytes",
                  "sk_attn_decode_partial_bytes", "sk_vocoder_param_count", "sk_vocoder_prepared_bytes",
-                 "sk_vocoder_workspace_bytes"):
+                 "sk_vocoder_workspace_bytes", "sk_lm_fp32_prepared_bytes"):
         if hasattr(lib, name):
             getattr(lib, name).restype = C.c_int64
-    for name in ("sk_lm_logits",):
+    for name in ("sk_lm_logits", "sk_lm_logits_f32"):
         getattr(lib, name).restype = C.c_void_p
     lib.sk_lm_destroy.restype = None
     if hasattr(lib, "sk_hubert_destroy"):

@@ -303,6 +303,11 @@ int sk_attn_tc_fwd_split(const void* qkv_hi, const void* qkv_lo, void* o_hi, voi
   SK_REQUIRE(qkv_hi && qkv_lo && o_hi && o_lo, "sk_attn_tc_fwd_split: null argument");
   return sk_attn_tc_fwd_split_launch(CBF(qkv_hi), CBF(qkv_lo), BF(o_hi), BF(o_lo), B, T, H, ld, ldo, scale, S(stream));
 }
+int sk_attn_tc_fwd_split_causal(const void* qkv_hi, const void* qkv_lo, void* o_hi, void* o_lo, int B, int T, int H, int ld,
+                                int ldo, float scale, void* stream) {
+  SK_REQUIRE(qkv_hi && qkv_lo && o_hi && o_lo, "sk_attn_tc_fwd_split_causal: null argument");
+  return sk_attn_tc_fwd_split_launch(CBF(qkv_hi), CBF(qkv_lo), BF(o_hi), BF(o_lo), B, T, H, ld, ldo, scale, S(stream), 1);
+}
 int sk_attn_bwd(const void* q, const void* k, const void* v, const void* o, const void* d_o, const float* lse,
                 float* delta, void* dq, void* dk, void* dv, int B, int T, int H, int KVH, int ld, int ldo, int ldg,
                 int causal, float scale, void* stream) {

@@ -268,9 +268,10 @@ attn_fwd_kernel(const bf16* __restrict__ q, const bf16* __restrict__ k, const bf
 }
 
 // ------------------------------------------------------------------------------------------------
-// forward, split-bf16 precision (HuBERT path): q/k/v/o are (hi, lo) bf16 pairs representing fp32-grade values;
-// S = Qh Kh^T + Qh Kl^T + Ql Kh^T and O = Ph Vh + Ph Vl + Pl Vh, all accumulated in fp32.  Bidirectional (the
-// reference passes no mask to HuBERT, hubert_feature_extractor.py:42), forward only.
+// forward, split-bf16 precision (HuBERT encoder, fp32 OPT inference): q/k/v/o are (hi, lo) bf16 pairs representing
+// fp32-grade values; S = Qh Kh^T + Qh Kl^T + Ql Kh^T and O = Ph Vh + Ph Vl + Pl Vh, all accumulated in fp32.  Forward
+// only.  Bidirectional for HuBERT (the reference passes no mask, hubert_feature_extractor.py:42); the causal instance
+// (OPT) reads no key tile past the diagonal and masks keys > query inside it, heaviest query tiles first.
 // ------------------------------------------------------------------------------------------------
 SK_DEVINL void acc_to_a_split(const float (&s)[8][4], uint32_t (&ph)[4][4], uint32_t (&pl)[4][4]) {
 #pragma unroll
@@ -287,6 +288,7 @@ SK_DEVINL void acc_to_a_split(const float (&s)[8][4], uint32_t (&ph)[4][4], uint
   }
 }
 
+template <bool CAUSAL>
 __global__ void __launch_bounds__(256)
 attn_fwd_split_kernel(const bf16* __restrict__ q_hi, const bf16* __restrict__ q_lo, const bf16* __restrict__ k_hi,
                       const bf16* __restrict__ k_lo, const bf16* __restrict__ v_hi, const bf16* __restrict__ v_lo,
@@ -296,11 +298,11 @@ attn_fwd_split_kernel(const bf16* __restrict__ q_hi, const bf16* __restrict__ q_
   const uint32_t sQl = sQh + 128 * 128;
   const uint32_t sKV = sQl + 128 * 128;  // per stage: Kh, Kl, Vh, Vl (4 x 8 KB)
   const int b = blockIdx.z, h = blockIdx.y;
-  const int q0 = blockIdx.x * 128;
+  const int q0 = (CAUSAL ? gridDim.x - 1 - blockIdx.x : blockIdx.x) * 128;
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const size_t base = (size_t)b * T * ld + h * HD;
   const float sl2 = scale * 1.4426950408889634f;
-  const int n_kv = (T + 63) / 64;
+  const int n_kv = CAUSAL ? min(T - 1, q0 + 127) / 64 + 1 : (T + 63) / 64;
 
   auto load_kv = [&](int j, int st) {
     const uint32_t sb = sKV + st * 4 * 8192;
@@ -337,12 +339,14 @@ attn_fwd_split_kernel(const bf16* __restrict__ q_hi, const bf16* __restrict__ q_
     wg_a_bT(s, qh, sb + 8192);   // Qh Kl^T
     wg_a_bT(s, qh, sb);          // Qh Kh^T
     const int k0 = j * 64;
-    if (k0 + 64 > T) {
+    if (k0 + 64 > T || (CAUSAL && k0 + 63 > q0 + warp * 16)) {
 #pragma unroll
       for (int nt = 0; nt < 8; ++nt)
 #pragma unroll
-        for (int e = 0; e < 4; ++e)
-          if (k0 + nt * 8 + (lane & 3) * 2 + (e & 1) >= T) s[nt][e] = -INFINITY;
+        for (int e = 0; e < 4; ++e) {
+          const int key = k0 + nt * 8 + (lane & 3) * 2 + (e & 1);
+          if (key >= T || (CAUSAL && key > row_a + ((e >> 1) << 3))) s[nt][e] = -INFINITY;
+        }
     }
     float mx[2] = {m_i[0], m_i[1]};
 #pragma unroll
@@ -747,20 +751,26 @@ int sk_attn_bwd_launch(const bf16* q, const bf16* k, const bf16* v, const bf16* 
   return 0;
 }
 
-// split-bf16 (hi, lo) bidirectional forward for the HuBERT encoder; all six inputs share the row pitch ld
+// split-bf16 (hi, lo) forward: bidirectional for the HuBERT encoder, causal for fp32 OPT inference; all six inputs share
+// the row pitch ld
 int sk_attn_fwd_split_launch(const bf16* q_hi, const bf16* q_lo, const bf16* k_hi, const bf16* k_lo, const bf16* v_hi,
                              const bf16* v_lo, bf16* o_hi, bf16* o_lo, int B, int T, int H, int ld, int ldo, float scale,
-                             cudaStream_t s) {
+                             cudaStream_t s, int causal) {
   SK_REQUIRE(B > 0 && T > 0 && H > 0, "attention: bad shape B=%d T=%d H=%d", B, T, H);
   SK_REQUIRE(ld % 8 == 0 && ldo % 8 == 0, "attention: leading dims must be multiples of 8");
-  static bool init = false;
-  if (!init) {
-    if (set_smem(attn_fwd_split_kernel, FWD_SPLIT_SMEM)) return -2;
-    init = true;
+  static bool init[2] = {false, false};
+  if (!init[causal ? 1 : 0]) {
+    if (set_smem(causal ? attn_fwd_split_kernel<true> : attn_fwd_split_kernel<false>, FWD_SPLIT_SMEM)) return -2;
+    init[causal ? 1 : 0] = true;
   }
   dim3 grid((T + 127) / 128, H, B);
   sk_prof_begin(1, s);
-  attn_fwd_split_kernel<<<grid, 256, FWD_SPLIT_SMEM, s>>>(q_hi, q_lo, k_hi, k_lo, v_hi, v_lo, o_hi, o_lo, T, ld, ldo, scale);
+  if (causal)
+    attn_fwd_split_kernel<true><<<grid, 256, FWD_SPLIT_SMEM, s>>>(q_hi, q_lo, k_hi, k_lo, v_hi, v_lo, o_hi, o_lo, T, ld, ldo,
+                                                                  scale);
+  else
+    attn_fwd_split_kernel<false><<<grid, 256, FWD_SPLIT_SMEM, s>>>(q_hi, q_lo, k_hi, k_lo, v_hi, v_lo, o_hi, o_lo, T, ld, ldo,
+                                                                   scale);
   sk_prof_end(s);
   SK_LAUNCH_CHECK();
   return 0;
@@ -802,7 +812,7 @@ int sk_attn_tc_bwd_launch(const bf16* qkv, const bf16* o, const bf16* d_o, const
 
 // qkv_hi / qkv_lo: [B*T, ld] with H q-heads, H k-heads, H v-heads (64 columns each); o_hi / o_lo: [B*T, ldo]
 int sk_attn_tc_fwd_split_launch(const bf16* qkv_hi, const bf16* qkv_lo, bf16* o_hi, bf16* o_lo, int B, int T, int H, int ld,
-                                int ldo, float scale, cudaStream_t s) {
+                                int ldo, float scale, cudaStream_t s, int causal) {
   return sk_attn_fwd_split_launch(qkv_hi, qkv_lo, qkv_hi + H * HD, qkv_lo + H * HD, qkv_hi + 2 * H * HD, qkv_lo + 2 * H * HD,
-                                  o_hi, o_lo, B, T, H, ld, ldo, scale, s);
+                                  o_hi, o_lo, B, T, H, ld, ldo, scale, s, causal);
 }

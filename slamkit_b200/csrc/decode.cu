@@ -12,41 +12,66 @@ namespace {
 
 constexpr int DEC_CH = 64;        // keys per attention split (one CTA); the split count is ceil(T_cache / DEC_CH)
 constexpr int DEC_THREADS = 128;
-constexpr int DEC_KPAD = 72;      // smem row pitch of the K / V tiles (144 B: conflict-free 16-byte row reads)
 constexpr int DEC_MAX_G = 16;     // query heads per kv head served by one CTA
+// smem row pitch of the K / V tiles: 144 B (bf16 cache) or 272 B (fp32 cache), conflict-free 16-byte row reads
+template <typename KV> constexpr int dec_kpad() { return sizeof(KV) == 2 ? 72 : 68; }
 
 // ---- KV cache ---------------------------------------------------------------------------------------------------
-// cache layout per layer: [K|V][B][KVH][T_cache][64] bf16, K after RoPE
+// cache layout per layer: [K|V][B][KVH][T_cache][64] of KV = bf16 (K after RoPE) or, for fp32 OPT inference, fp32
+// (the value hi + lo of the split-bf16 projections: fp32-grade K / V).  `lo` (fp32 cache only) is the lo half of the
+// projections, at the same offsets as their hi half.
+
+// eight cache elements from the projections at src (+ lo)
+SK_DEVINL void put8(bf16* dst, const bf16* src, const bf16*) { stg128(dst, ldg128(src)); }
+SK_DEVINL void put8(float* dst, const bf16* src, const bf16* lo) {
+  const uint4 h = ldg128(src), l = ldg128(lo);
+  const uint32_t hw[4] = {h.x, h.y, h.z, h.w}, lw[4] = {l.x, l.y, l.z, l.w};
+  float v[8];
+#pragma unroll
+  for (int k = 0; k < 4; ++k) {
+    const float2 a = unpack_bf16(hw[k]), b = unpack_bf16(lw[k]);
+    v[2 * k] = a.x + b.x;
+    v[2 * k + 1] = a.y + b.y;
+  }
+  reinterpret_cast<float4*>(dst)[0] = make_float4(v[0], v[1], v[2], v[3]);
+  reinterpret_cast<float4*>(dst)[1] = make_float4(v[4], v[5], v[6], v[7]);
+}
 
 // prefill: copy K/V of positions t < lens[b] of every layer out of the fused projections [B*T, ldq] (layer stride
 // `layer_stride` elements) into the cache.  grid (B*T, L)
-__global__ void kv_prefill_kernel(const bf16* __restrict__ qkv, long layer_stride, int ldq, bf16* __restrict__ cache,
-                                  const int32_t* __restrict__ lens, int B, int T, int H, int KVH, int T_cache) {
+template <typename KV>
+__global__ void kv_prefill_kernel(const bf16* __restrict__ qkv, const bf16* __restrict__ qkv_lo, long layer_stride, int ldq,
+                                  KV* __restrict__ cache, const int32_t* __restrict__ lens, int B, int T, int H, int KVH,
+                                  int T_cache) {
   griddep_wait();
   const int row = blockIdx.x, l = blockIdx.y;
   const int b = row / T, t = row % T;
   if (t >= lens[b] || t >= T_cache) return;
-  const bf16* src = qkv + l * layer_stride + (size_t)row * ldq + (size_t)H * 64;
+  const size_t so = l * layer_stride + (size_t)row * ldq + (size_t)H * 64;
   const size_t plane = (size_t)B * KVH * T_cache * 64;
-  bf16* kc = cache + (size_t)l * 2 * plane;
+  KV* kc = cache + (size_t)l * 2 * plane;
   for (int i = threadIdx.x; i < 2 * KVH * 8; i += blockDim.x) {
     const int which = i / (KVH * 8), r = i % (KVH * 8), kvh = r / 8, c = r % 8;
-    bf16* dst = kc + which * plane + (((size_t)b * KVH + kvh) * T_cache + t) * 64 + c * 8;
-    stg128(dst, ldg128(src + (size_t)(which * KVH + kvh) * 64 + c * 8));
+    KV* dst = kc + which * plane + (((size_t)b * KVH + kvh) * T_cache + t) * 64 + c * 8;
+    const size_t o = so + (size_t)(which * KVH + kvh) * 64 + c * 8;
+    put8(dst, qkv + o, qkv_lo + o);
   }
 }
 
 // decode: append the K/V of the one new token of every row at pos[b] and publish lens[b] = pos[b] + 1.  grid B
-__global__ void kv_append_kernel(const bf16* __restrict__ qkv, int ldq, bf16* __restrict__ kc, bf16* __restrict__ vc,
-                                 const int32_t* __restrict__ pos, int32_t* __restrict__ lens, int H, int KVH, int T_cache) {
+template <typename KV>
+__global__ void kv_append_kernel(const bf16* __restrict__ qkv, const bf16* __restrict__ qkv_lo, int ldq, KV* __restrict__ kc,
+                                 KV* __restrict__ vc, const int32_t* __restrict__ pos, int32_t* __restrict__ lens, int H,
+                                 int KVH, int T_cache) {
   griddep_wait();
   const int b = blockIdx.x;
   const int p = min(max(pos[b], 0), T_cache - 1);
-  const bf16* src = qkv + (size_t)b * ldq + (size_t)H * 64;
+  const size_t so = (size_t)b * ldq + (size_t)H * 64;
   for (int i = threadIdx.x; i < 2 * KVH * 8; i += blockDim.x) {
     const int which = i / (KVH * 8), r = i % (KVH * 8), kvh = r / 8, c = r % 8;
-    bf16* dst = (which ? vc : kc) + (((size_t)b * KVH + kvh) * T_cache + p) * 64 + c * 8;
-    stg128(dst, ldg128(src + (size_t)(which * KVH + kvh) * 64 + c * 8));
+    KV* dst = (which ? vc : kc) + (((size_t)b * KVH + kvh) * T_cache + p) * 64 + c * 8;
+    const size_t o = so + (size_t)(which * KVH + kvh) * 64 + c * 8;
+    put8(dst, qkv + o, qkv_lo + o);
   }
   if (threadIdx.x == 0 && lens) lens[b] = p + 1;
 }
@@ -65,15 +90,25 @@ __global__ void gather_last_kernel(const bf16* __restrict__ x, const int32_t* __
 // Flash-decoding: CTA (split s, kv head, row b) serves all G = H/KVH query heads of its group over keys
 // [64 s, min(64 s + 64, lens[b])), so every K/V byte is read once.  Scores and the (unnormalised) P.V sum are fp32;
 // the partial (o, m, l) per (row, head, split) goes to `partial` and sk_attn_decode's combine pass merges the splits in
-// split order.  CTAs whose range starts at or past lens[b] exit before touching the cache.
+// split order.  CTAs whose range starts at or past lens[b] exit before touching the cache.  An fp32 cache (KV = float)
+// goes with a split-bf16 query: q = q_hi + q_lo.
+
+// 16 bytes of a cache row (8 bf16 / 4 fp32 elements) at element i, and two elements as fp32
+template <typename KV> SK_DEVINL uint4 cache16(const KV* p) { return ldg128_stream(reinterpret_cast<const bf16*>(p)); }
+SK_DEVINL float2 two(const bf16* p) { return __bfloat1622float2(*reinterpret_cast<const bf162*>(p)); }
+SK_DEVINL float2 two(const float* p) { return *reinterpret_cast<const float2*>(p); }
+
+template <typename KV>
 __global__ void __launch_bounds__(DEC_THREADS) attn_decode_split_kernel(
-    const bf16* __restrict__ q, int ldq, const bf16* __restrict__ kc, const bf16* __restrict__ vc,
+    const bf16* __restrict__ q, const bf16* __restrict__ q_lo, int ldq, const KV* __restrict__ kc, const KV* __restrict__ vc,
     const int32_t* __restrict__ lens, float* __restrict__ part_o, float2* __restrict__ part_ml, int H, int KVH,
     int T_cache, int S, float scale_log2) {
+  constexpr int KPAD = dec_kpad<KV>();
+  constexpr int EPV = 16 / sizeof(KV);   // cache elements per 16-byte vector
   extern __shared__ __align__(16) uint8_t dec_smem[];
-  bf16* sK = reinterpret_cast<bf16*>(dec_smem);
-  bf16* sV = sK + DEC_CH * DEC_KPAD;
-  float* sQ = reinterpret_cast<float*>(sV + DEC_CH * DEC_KPAD);   // [G][64], pre-scaled by scale * log2(e)
+  KV* sK = reinterpret_cast<KV*>(dec_smem);
+  KV* sV = sK + DEC_CH * KPAD;
+  float* sQ = reinterpret_cast<float*>(sV + DEC_CH * KPAD);   // [G][64], pre-scaled by scale * log2(e)
   float* sP = sQ + DEC_MAX_G * 64;                                  // [G][64] scores, then exp2(score - max)
   const int s = blockIdx.x, kvh = blockIdx.y, b = blockIdx.z;
   const int G = H / KVH;
@@ -84,18 +119,29 @@ __global__ void __launch_bounds__(DEC_THREADS) attn_decode_split_kernel(
   if (k0 >= len) return;
   const int n = min(DEC_CH, len - k0);
   const size_t base = (((size_t)b * KVH + kvh) * T_cache + k0) * 64;
-  for (int i = tid; i < n * 8; i += DEC_THREADS) {
-    const int r = i >> 3, c = i & 7;
-    *reinterpret_cast<uint4*>(sK + r * DEC_KPAD + c * 8) = ldg128_stream(kc + base + (size_t)r * 64 + c * 8);
-    *reinterpret_cast<uint4*>(sV + r * DEC_KPAD + c * 8) = ldg128_stream(vc + base + (size_t)r * 64 + c * 8);
+  for (int i = tid; i < n * (64 / EPV); i += DEC_THREADS) {
+    const int r = i / (64 / EPV), c = i % (64 / EPV);
+    *reinterpret_cast<uint4*>(sK + r * KPAD + c * EPV) = cache16(kc + base + (size_t)r * 64 + c * EPV);
+    *reinterpret_cast<uint4*>(sV + r * KPAD + c * EPV) = cache16(vc + base + (size_t)r * 64 + c * EPV);
   }
   for (int i = tid; i < G * 8; i += DEC_THREADS) {
     const int g = i >> 3, c = i & 7;
-    const uint4 v = ldg128(q + (size_t)b * ldq + (size_t)(kvh * G + g) * 64 + c * 8);
+    const size_t qo = (size_t)b * ldq + (size_t)(kvh * G + g) * 64 + c * 8;
+    const uint4 v = ldg128(q + qo);
     const uint32_t u[4] = {v.x, v.y, v.z, v.w};
+    uint32_t ul[4] = {0u, 0u, 0u, 0u};
+    if constexpr (sizeof(KV) == 4) {
+      const uint4 vl = ldg128(q_lo + qo);
+      ul[0] = vl.x; ul[1] = vl.y; ul[2] = vl.z; ul[3] = vl.w;
+    }
 #pragma unroll
     for (int k = 0; k < 4; ++k) {
-      const float2 f = unpack_bf16(u[k]);
+      float2 f = unpack_bf16(u[k]);
+      if constexpr (sizeof(KV) == 4) {
+        const float2 fl = unpack_bf16(ul[k]);
+        f.x += fl.x;
+        f.y += fl.y;
+      }
       sQ[g * 64 + c * 8 + 2 * k] = f.x * scale_log2;
       sQ[g * 64 + c * 8 + 2 * k + 1] = f.y * scale_log2;
     }
@@ -106,15 +152,26 @@ __global__ void __launch_bounds__(DEC_THREADS) attn_decode_split_kernel(
     const int j = tid & 63;
     if (j < n) {
       float kf[64];
+      if constexpr (sizeof(KV) == 2) {
 #pragma unroll
-      for (int c = 0; c < 8; ++c) {
-        const uint4 v = *reinterpret_cast<const uint4*>(sK + j * DEC_KPAD + c * 8);
-        const uint32_t u[4] = {v.x, v.y, v.z, v.w};
+        for (int c = 0; c < 8; ++c) {
+          const uint4 v = *reinterpret_cast<const uint4*>(sK + j * KPAD + c * 8);
+          const uint32_t u[4] = {v.x, v.y, v.z, v.w};
 #pragma unroll
-        for (int k = 0; k < 4; ++k) {
-          const float2 f = unpack_bf16(u[k]);
-          kf[c * 8 + 2 * k] = f.x;
-          kf[c * 8 + 2 * k + 1] = f.y;
+          for (int k = 0; k < 4; ++k) {
+            const float2 f = unpack_bf16(u[k]);
+            kf[c * 8 + 2 * k] = f.x;
+            kf[c * 8 + 2 * k + 1] = f.y;
+          }
+        }
+      } else {
+#pragma unroll
+        for (int c = 0; c < 16; ++c) {
+          const float4 v = *reinterpret_cast<const float4*>(sK + j * KPAD + c * 4);
+          kf[4 * c] = v.x;
+          kf[4 * c + 1] = v.y;
+          kf[4 * c + 2] = v.z;
+          kf[4 * c + 3] = v.w;
         }
       }
       for (int g = tid >> 6; g < G; g += DEC_THREADS / 64) {
@@ -151,7 +208,7 @@ __global__ void __launch_bounds__(DEC_THREADS) attn_decode_split_kernel(
 #pragma unroll
   for (int i = 0; i < DEC_MAX_G / 4; ++i) acc[i] = make_float2(0.f, 0.f);
   for (int j = 0; j < n; ++j) {
-    const float2 v = __bfloat1622float2(*reinterpret_cast<const bf162*>(sV + j * DEC_KPAD + 2 * lane));
+    const float2 v = two(sV + j * KPAD + 2 * lane);
 #pragma unroll
     for (int i = 0; i < DEC_MAX_G / 4; ++i) {
       const int g = warp + 4 * i;
@@ -170,11 +227,13 @@ __global__ void __launch_bounds__(DEC_THREADS) attn_decode_split_kernel(
   }
 }
 
-// one warp per (row, head): merge the ceil(lens[b] / 64) valid splits in split order
+// one warp per (row, head): merge the ceil(lens[b] / 64) valid splits in split order.  SPLIT_OUT: write the (hi, lo)
+// pair of the fp32 result (o_lo) instead of its bf16 rounding
+template <bool SPLIT_OUT>
 __global__ void __launch_bounds__(128) attn_decode_combine_kernel(const float* __restrict__ part_o,
                                                                   const float2* __restrict__ part_ml,
                                                                   const int32_t* __restrict__ lens, bf16* __restrict__ o,
-                                                                  int ldo, int B, int H, int S) {
+                                                                  bf16* __restrict__ o_lo, int ldo, int B, int H, int S) {
   griddep_wait();
   const int w = blockIdx.x * 4 + (threadIdx.x >> 5), lane = threadIdx.x & 31;
   if (w >= B * H) return;
@@ -194,7 +253,14 @@ __global__ void __launch_bounds__(128) attn_decode_combine_kernel(const float* _
     acc.y = fmaf(f, v.y, acc.y);
   }
   const float inv = ns > 0 ? 1.0f / L : 0.f;
-  *reinterpret_cast<bf162*>(o + (size_t)b * ldo + h * 64 + 2 * lane) = __floats2bfloat162_rn(acc.x * inv, acc.y * inv);
+  const size_t oo = (size_t)b * ldo + h * 64 + 2 * lane;
+  if (SPLIT_OUT) {
+    const float v0 = acc.x * inv, v1 = acc.y * inv, h0 = bf16_round(v0), h1 = bf16_round(v1);
+    *reinterpret_cast<uint32_t*>(o + oo) = pack_bf16(h0, h1);
+    *reinterpret_cast<uint32_t*>(o_lo + oo) = pack_bf16(v0 - h0, v1 - h1);
+  } else {
+    *reinterpret_cast<bf162*>(o + oo) = __floats2bfloat162_rn(acc.x * inv, acc.y * inv);
+  }
 }
 
 // ---- token selection -------------------------------------------------------------------------------------------
@@ -255,14 +321,18 @@ SK_DEVINL T block_exclusive_scan(T v, T* red, T& total) {
   return before + inc - v;
 }
 
+SK_DEVINL float logit_at(const bf16* row, int i) { return __bfloat162float(row[i]); }
+SK_DEVINL float logit_at(const float* row, int i) { return row[i]; }
+
+template <typename LT>
 struct SelRow {
-  const bf16* row;
+  const LT* row;
   const uint32_t* ban;
   float temp;
   bool use_temp;
   SK_DEVINL float score(int i) const {
     if (ban && ((ban[i >> 5] >> (i & 31)) & 1u)) return -INFINITY;
-    const float x = __bfloat162float(row[i]);
+    const float x = logit_at(row, i);
     return use_temp ? __fdiv_rn(x, temp) : x;
   }
 };
@@ -270,7 +340,9 @@ struct SelRow {
 // One CTA per row.  Order of HF's processors: bans -> (sampling only) temperature -> top-k -> top-p -> softmax -> draw;
 // greedy = argmax of the banned scores, lowest id on ties.  Each thread owns the contiguous id range
 // [tid * chunk, (tid + 1) * chunk), so per-thread partial sums are in token order and every sum is taken in a fixed order.
-__global__ void __launch_bounds__(SEL_THREADS) select_next_kernel(const bf16* __restrict__ logits, int ldl, int V,
+// LT: bf16 logits, or fp32 ones (fp32 OPT inference).
+template <typename LT>
+__global__ void __launch_bounds__(SEL_THREADS) select_next_kernel(const LT* __restrict__ logits, int ldl, int V,
                                                                   const uint32_t* __restrict__ ban, SkSampling cfg,
                                                                   const float* __restrict__ uniforms, SkDecodeState st) {
   __shared__ float red_f[SEL_WARPS];
@@ -303,7 +375,7 @@ __global__ void __launch_bounds__(SEL_THREADS) select_next_kernel(const bf16* __
   }
   const int chunk = (V + SEL_THREADS - 1) / SEL_THREADS;
   const int i0 = min(tid * chunk, V), i1 = min(i0 + chunk, V);
-  SelRow R{logits + (size_t)b * ldl, ban, cfg.temperature, cfg.do_sample != 0 && cfg.temperature != 1.0f};
+  SelRow<LT> R{logits + (size_t)b * ldl, ban, cfg.temperature, cfg.do_sample != 0 && cfg.temperature != 1.0f};
   int tok = 0;
   if (!cfg.do_sample) {
     // argmax, lowest id among equal maxima
@@ -470,15 +542,31 @@ __global__ void __launch_bounds__(SEL_THREADS) select_next_kernel(const bf16* __
 int sk_kv_prefill_launch(const bf16* qkv, long layer_stride, int ldq, bf16* cache, const int32_t* lens, int L, int B, int T,
                          int H, int KVH, int T_cache, cudaStream_t s) {
   SK_REQUIRE(ldq % 8 == 0, "kv_prefill: ldq must be a multiple of 8");
-  SK_CUDA_CHECK(sk_launch_pdl(kv_prefill_kernel, dim3(B * T, L), dim3(64), (size_t)0, s, qkv, layer_stride, ldq, cache, lens,
-                              B, T, H, KVH, T_cache));
+  SK_CUDA_CHECK(sk_launch_pdl(kv_prefill_kernel<bf16>, dim3(B * T, L), dim3(64), (size_t)0, s, qkv, (const bf16*)nullptr,
+                              layer_stride, ldq, cache, lens, B, T, H, KVH, T_cache));
+  SK_LAUNCH_CHECK();
+  return 0;
+}
+int sk_kv_prefill_f32_launch(const bf16* qkv_hi, const bf16* qkv_lo, int ldq, float* cache, const int32_t* lens, int B, int T,
+                             int H, int T_cache, cudaStream_t s) {
+  SK_REQUIRE(ldq % 8 == 0, "kv_prefill: ldq must be a multiple of 8");
+  SK_CUDA_CHECK(sk_launch_pdl(kv_prefill_kernel<float>, dim3(B * T, 1), dim3(64), (size_t)0, s, qkv_hi, qkv_lo, 0L, ldq, cache,
+                              lens, B, T, H, H, T_cache));
   SK_LAUNCH_CHECK();
   return 0;
 }
 
 int sk_kv_append_launch(const bf16* qkv, int ldq, bf16* kc, bf16* vc, const int32_t* pos, int32_t* lens, int B, int H,
                         int KVH, int T_cache, cudaStream_t s) {
-  SK_CUDA_CHECK(sk_launch_pdl(kv_append_kernel, dim3(B), dim3(64), (size_t)0, s, qkv, ldq, kc, vc, pos, lens, H, KVH, T_cache));
+  SK_CUDA_CHECK(sk_launch_pdl(kv_append_kernel<bf16>, dim3(B), dim3(64), (size_t)0, s, qkv, (const bf16*)nullptr, ldq, kc, vc,
+                              pos, lens, H, KVH, T_cache));
+  SK_LAUNCH_CHECK();
+  return 0;
+}
+int sk_kv_append_f32_launch(const bf16* qkv_hi, const bf16* qkv_lo, int ldq, float* kc, float* vc, const int32_t* pos,
+                            int32_t* lens, int B, int H, int T_cache, cudaStream_t s) {
+  SK_CUDA_CHECK(sk_launch_pdl(kv_append_kernel<float>, dim3(B), dim3(64), (size_t)0, s, qkv_hi, qkv_lo, ldq, kc, vc, pos, lens,
+                              H, H, T_cache));
   SK_LAUNCH_CHECK();
   return 0;
 }
@@ -492,38 +580,56 @@ int sk_gather_last_launch(const bf16* x, const int32_t* lens, bf16* out, int B, 
 
 int sk_attn_decode_splits(int T_cache) { return (T_cache + DEC_CH - 1) / DEC_CH; }
 
-int sk_attn_decode_launch(const bf16* q, int ldq, const bf16* kc, const bf16* vc, const int32_t* lens, bf16* o, int ldo,
-                          float* partial, int B, int H, int KVH, int T_cache, float scale, cudaStream_t s) {
+// KV = bf16: q, o bf16 (q_lo, o_lo unused); KV = float: q and o are (hi, lo) pairs
+template <typename KV>
+int attn_decode(const bf16* q, const bf16* q_lo, int ldq, const KV* kc, const KV* vc, const int32_t* lens, bf16* o, bf16* o_lo,
+                int ldo, float* partial, int B, int H, int KVH, int T_cache, float scale, cudaStream_t s) {
   SK_REQUIRE(B > 0 && H > 0 && KVH > 0 && T_cache > 0 && H % KVH == 0 && H / KVH <= DEC_MAX_G,
              "attn_decode: bad shape B=%d H=%d KVH=%d T_cache=%d (H/KVH <= %d)", B, H, KVH, T_cache, DEC_MAX_G);
   SK_REQUIRE(ldq % 8 == 0 && ldo % 2 == 0, "attn_decode: ldq must be a multiple of 8 and ldo even");
   const int S = sk_attn_decode_splits(T_cache);
   float* part_o = partial;
   float2* part_ml = reinterpret_cast<float2*>(partial + (size_t)B * H * S * 64);
-  const size_t smem = (size_t)2 * DEC_CH * DEC_KPAD * sizeof(bf16) + (size_t)2 * DEC_MAX_G * 64 * sizeof(float);
+  const size_t smem = (size_t)2 * DEC_CH * dec_kpad<KV>() * sizeof(KV) + (size_t)2 * DEC_MAX_G * 64 * sizeof(float);
+  constexpr bool split = sizeof(KV) == 4;
   sk_prof_begin(1, s);
-  cudaError_t e = sk_launch_pdl(attn_decode_split_kernel, dim3(S, KVH, B), dim3(DEC_THREADS), smem, s, q, ldq, kc, vc, lens,
-                                part_o, part_ml, H, KVH, T_cache, S, scale * 1.4426950408889634f);
+  cudaError_t e = sk_launch_pdl(attn_decode_split_kernel<KV>, dim3(S, KVH, B), dim3(DEC_THREADS), smem, s, q, q_lo, ldq, kc, vc,
+                                lens, part_o, part_ml, H, KVH, T_cache, S, scale * 1.4426950408889634f);
   if (e == cudaSuccess)
-    e = sk_launch_pdl(attn_decode_combine_kernel, dim3((B * H + 3) / 4), dim3(128), (size_t)0, s,
-                      (const float*)part_o, (const float2*)part_ml, lens, o, ldo, B, H, S);
+    e = sk_launch_pdl(attn_decode_combine_kernel<split>, dim3((B * H + 3) / 4), dim3(128), (size_t)0, s,
+                      (const float*)part_o, (const float2*)part_ml, lens, o, o_lo, ldo, B, H, S);
   sk_prof_end(s);
   SK_CUDA_CHECK(e);
   SK_LAUNCH_CHECK();
   return 0;
 }
 
-int sk_select_next_launch(const bf16* logits, int ldl, int V, int B, const uint32_t* ban, const SkSampling& cfg,
-                          const float* uniforms, const SkDecodeState& st, cudaStream_t s) {
+int sk_attn_decode_launch(const bf16* q, int ldq, const bf16* kc, const bf16* vc, const int32_t* lens, bf16* o, int ldo,
+                          float* partial, int B, int H, int KVH, int T_cache, float scale, cudaStream_t s) {
+  return attn_decode<bf16>(q, nullptr, ldq, kc, vc, lens, o, nullptr, ldo, partial, B, H, KVH, T_cache, scale, s);
+}
+int sk_attn_decode_f32_launch(const bf16* q_hi, const bf16* q_lo, int ldq, const float* kc, const float* vc, const int32_t* lens,
+                              bf16* o_hi, bf16* o_lo, int ldo, float* partial, int B, int H, int T_cache, float scale,
+                              cudaStream_t s) {
+  return attn_decode<float>(q_hi, q_lo, ldq, kc, vc, lens, o_hi, o_lo, ldo, partial, B, H, H, T_cache, scale, s);
+}
+
+template <typename LT>
+int select_next(const LT* logits, int ldl, int V, int B, const uint32_t* ban, const SkSampling& cfg, const float* uniforms,
+                const SkDecodeState& st, cudaStream_t s) {
   SK_REQUIRE(B > 0 && V > 0 && ldl >= V, "select_next: bad shape B=%d V=%d ldl=%d", B, V, ldl);
   SK_REQUIRE(cfg.n_eos >= 0 && cfg.n_eos <= 8, "select_next: at most 8 eos ids");
   SK_REQUIRE(!cfg.do_sample || cfg.temperature > 0.f, "select_next: temperature must be > 0");
   SK_REQUIRE(st.tokens && st.pos && st.finished && st.n_gen && st.out && st.step && st.max_new > 0,
              "select_next: incomplete decode state");
-  SK_CUDA_CHECK(sk_launch_pdl(select_next_kernel, dim3(B), dim3(SEL_THREADS), (size_t)0, s, logits, ldl, V, ban, cfg,
+  SK_CUDA_CHECK(sk_launch_pdl(select_next_kernel<LT>, dim3(B), dim3(SEL_THREADS), (size_t)0, s, logits, ldl, V, ban, cfg,
                               uniforms, st));
   SK_LAUNCH_CHECK();
   return 0;
+}
+int sk_select_next_launch(const bf16* logits, int ldl, int V, int B, const uint32_t* ban, const SkSampling& cfg,
+                          const float* uniforms, const SkDecodeState& st, cudaStream_t s) {
+  return select_next<bf16>(logits, ldl, V, B, ban, cfg, uniforms, st, s);
 }
 
 extern "C" {
@@ -546,6 +652,22 @@ int sk_select_next(const void* logits, int ldl, int V, int B, const uint32_t* ba
   SK_REQUIRE(logits && cfg && state, "sk_select_next: null argument");
   return sk_select_next_launch(reinterpret_cast<const bf16*>(logits), ldl, V, B, ban_bits, *cfg, uniforms, *state,
                                (cudaStream_t)stream);
+}
+
+int sk_select_next_f32(const float* logits, int ldl, int V, int B, const uint32_t* ban_bits, const SkSampling* cfg,
+                       const float* uniforms, const SkDecodeState* state, void* stream) {
+  SK_REQUIRE(logits && cfg && state, "sk_select_next_f32: null argument");
+  SK_REQUIRE(((uintptr_t)logits & 15) == 0, "sk_select_next_f32: logits must be 16-byte aligned");
+  return select_next<float>(logits, ldl, V, B, ban_bits, *cfg, uniforms, *state, (cudaStream_t)stream);
+}
+
+int sk_attn_decode_split(const void* q_hi, const void* q_lo, int ldq, const float* k_cache, const float* v_cache,
+                         const int32_t* lens, void* o_hi, void* o_lo, int ldo, float* partial, int B, int H, int T_cache,
+                         float scale, void* stream) {
+  SK_REQUIRE(q_hi && q_lo && k_cache && v_cache && lens && o_hi && o_lo && partial, "sk_attn_decode_split: null argument");
+  return sk_attn_decode_f32_launch(reinterpret_cast<const bf16*>(q_hi), reinterpret_cast<const bf16*>(q_lo), ldq, k_cache,
+                                   v_cache, lens, reinterpret_cast<bf16*>(o_hi), reinterpret_cast<bf16*>(o_lo), ldo, partial,
+                                   B, H, T_cache, scale, (cudaStream_t)stream);
 }
 
 }  // extern "C"

@@ -118,17 +118,8 @@ HiLo hl(const SkHubert* h, int64_t off, int64_t elems) {
 // y(hi,lo)[M,N] = act(x(hi,lo)[M,K] * W(hi,lo)[N,K]^T + bias) (+ residual(hi,lo)), split-bf16 3-pass
 int linear_split(const SkHubert* h, int M, int N, int K, HiLo x, int64_t w_off, int64_t b_off, int act, const HiLo* res,
                  HiLo y, float* y_f32, int ldy, cudaStream_t s) {
-  SkGemmEx g;
-  memset(&g, 0, sizeof(g));
-  g.M = M; g.N = N; g.K = K; g.batch = 1; g.passes = 3;
-  g.A = x.hi; g.A_lo = x.lo; g.lda = K;
-  g.B = h->w_hi + w_off; g.B_lo = h->w_lo + w_off; g.ldb = K;
-  if (y_f32) { g.C = y_f32; g.out_f32 = 1; } else { g.C = y.hi; g.C_lo = y.lo; }
-  g.ldc = ldy;
-  if (b_off >= 0) { g.bias = h->w32 + b_off; g.bias_f32 = 1; }
-  if (res) { g.residual = res->hi; g.residual_lo = res->lo; g.ldr = N; }
-  g.act = act;
-  return sk_gemm_ex_launch(g, s);
+  return sk_linear_split_launch(M, N, K, x.hi, x.lo, h->w_hi + w_off, h->w_lo + w_off, b_off >= 0 ? h->w32 + b_off : nullptr,
+                                act, res ? res->hi : nullptr, res ? res->lo : nullptr, y.hi, y.lo, y_f32, ldy, s);
 }
 
 // dbg_stage (tests only): 100+i = output of conv layer i, 200 = projection, 201 = positional conv (post-GELU),

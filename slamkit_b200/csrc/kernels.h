@@ -2,6 +2,7 @@
 // (The public, C-ABI surface is include/slamkit_b200.h.)
 #pragma once
 #include "common.cuh"
+#include <string.h>
 
 // gemm_tcgen05.cu
 int sk_make_tmap_2d(CUtensorMap* out, const void* ptr, int elem_bytes, uint64_t inner, uint64_t outer, uint64_t ld,
@@ -54,6 +55,24 @@ struct SkGemmEx {
   int rope_rot;
 };
 int sk_gemm_ex_launch(const SkGemmEx& g, cudaStream_t stream);
+// The fp32-grade linear of the HuBERT encoder and of fp32 OPT inference: y[M,N] = act(x[M,K] W[N,K]^T + bias) (+ res),
+// split-bf16 3-pass on (hi, lo) pairs of x and W, fp32 bias (or none), optional (hi, lo) residual [M, N]; the result as a
+// (hi, lo) pair y_hi / y_lo, or fp32 into y32 when y32 is given; output pitch ldy.
+inline int sk_linear_split_launch(int M, int N, int K, const bf16* x_hi, const bf16* x_lo, const bf16* w_hi, const bf16* w_lo,
+                                  const float* bias, int act, const bf16* res_hi, const bf16* res_lo, bf16* y_hi, bf16* y_lo,
+                                  float* y32, int ldy, cudaStream_t s) {
+  SkGemmEx g;
+  memset(&g, 0, sizeof(g));
+  g.M = M; g.N = N; g.K = K; g.batch = 1; g.passes = 3;
+  g.A = x_hi; g.A_lo = x_lo; g.lda = K;
+  g.B = w_hi; g.B_lo = w_lo; g.ldb = K;
+  if (y32) { g.C = y32; g.out_f32 = 1; } else { g.C = y_hi; g.C_lo = y_lo; }
+  g.ldc = ldy;
+  if (bias) { g.bias = bias; g.bias_f32 = 1; }
+  if (res_hi) { g.residual = res_hi; g.residual_lo = res_lo; g.ldr = N; }
+  g.act = act;
+  return sk_gemm_ex_launch(g, s);
+}
 struct SkGemmPlan;
 int sk_gemm_plan_ex(const SkGemmEx& g, SkGemmPlan* out);   // the decisions sk_gemm_ex_launch makes for g, nothing launched
 int sk_gemm_launch(int M, int N, int K, const void* A, int lda, int a_mn, const void* B, int ldb, int b_mn, void* C,
@@ -155,11 +174,11 @@ int sk_attn_bwd_launch(const bf16* q, const bf16* k, const bf16* v, const bf16* 
                        int ldg, int causal, float scale, cudaStream_t s, const int* seg_start = nullptr);
 int sk_attn_fwd_split_launch(const bf16* q_hi, const bf16* q_lo, const bf16* k_hi, const bf16* k_lo, const bf16* v_hi,
                              const bf16* v_lo, bf16* o_hi, bf16* o_lo, int B, int T, int H, int ld, int ldo, float scale,
-                             cudaStream_t s);
+                             cudaStream_t s, int causal = 0);
 
 // attention.cu: entry points on the fused q|k|v projection (LM step, HuBERT encoder)
 int sk_attn_tc_fwd_split_launch(const bf16* qkv_hi, const bf16* qkv_lo, bf16* o_hi, bf16* o_lo, int B, int T, int H, int ld,
-                                int ldo, float scale, cudaStream_t s);
+                                int ldo, float scale, cudaStream_t s, int causal = 0);
 // seg_start / seg_end (optional, int32 [B*T]): in-row index of the first token of each token's document and one past
 // its last -- block-diagonal causal attention for packed batches (sk_seg_bounds_launch builds them from position_ids)
 int sk_attn_tc_bwd_launch(const bf16* qkv, const bf16* o, const bf16* d_o, const float* lse, float* delta, float* partial,
@@ -178,6 +197,15 @@ int sk_kv_prefill_launch(const bf16* qkv, long layer_stride, int ldq, bf16* cach
 int sk_kv_append_launch(const bf16* qkv, int ldq, bf16* kc, bf16* vc, const int32_t* pos, int32_t* lens, int B, int H,
                         int KVH, int T_cache, cudaStream_t s);
 int sk_gather_last_launch(const bf16* x, const int32_t* lens, bf16* out, int B, int T, int D, cudaStream_t s);
+// fp32 OPT inference: an fp32 cache ([K|V][B][H][T_cache][64] per layer) filled from the (hi, lo) projections of one layer,
+// decode attention with a (hi, lo) query and output
+int sk_kv_prefill_f32_launch(const bf16* qkv_hi, const bf16* qkv_lo, int ldq, float* cache, const int32_t* lens, int B, int T,
+                             int H, int T_cache, cudaStream_t s);
+int sk_kv_append_f32_launch(const bf16* qkv_hi, const bf16* qkv_lo, int ldq, float* kc, float* vc, const int32_t* pos,
+                            int32_t* lens, int B, int H, int T_cache, cudaStream_t s);
+int sk_attn_decode_f32_launch(const bf16* q_hi, const bf16* q_lo, int ldq, const float* kc, const float* vc, const int32_t* lens,
+                              bf16* o_hi, bf16* o_lo, int ldo, float* partial, int B, int H, int T_cache, float scale,
+                              cudaStream_t s);
 int sk_attn_decode_splits(int T_cache);
 int sk_attn_decode_launch(const bf16* q, int ldq, const bf16* kc, const bf16* vc, const int32_t* lens, bf16* o, int ldo,
                           float* partial, int B, int H, int KVH, int T_cache, float scale, cudaStream_t s);

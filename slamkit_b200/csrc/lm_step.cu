@@ -77,6 +77,11 @@ struct SkLm {
   long* d_widen_start = nullptr;
   int* d_widen_len = nullptr;
   int n_widen = 0;
+  // OPT fp32 inference (sk_lm_set_fp32): params32 holds the model, w_hi / w_lo its split-bf16 (hi, lo) copy that the
+  // GEMMs read; forward only
+  bool fp32 = false;
+  bf16* w_hi = nullptr;
+  bf16* w_lo = nullptr;
   // optional: events recorded on the compute stream as soon as a layer's gradients are final (index = layer; index
   // n_layers = lm_head / final-norm part), so the host can start that bucket's all-reduce while backward continues
   std::vector<cudaEvent_t> bwd_events;
@@ -342,6 +347,7 @@ int backward_impl(SkLm* lm, const int64_t* ids, const int32_t* pos_ids, int B, i
 // byte offsets into the decode workspace for (B, T_cache): one token per row
 struct DecLayout {
   int64_t gemm, gemm_bytes, x0, x1, h, qkv, ao, gu, act, lens, partial, total;
+  int64_t e32 = 0;   // fp32 inference: the fp32 embedding sum [B, d]
 };
 
 DecLayout make_dec_layout(const SkLm* lm, int B, int T_cache) {
@@ -353,18 +359,21 @@ DecLayout make_dec_layout(const SkLm* lm, int B, int T_cache) {
     return o;
   };
   // GEMM scratch: split-K slabs of the down projection and stream-K partial tiles, flag words in its last 4 KB
+  // fp32 inference: the activations are (hi, lo) pairs, lo right after hi
+  const int64_t pf = lm->fp32 ? 2 : 1;
   w.gemm_bytes = align_up((int64_t)sk_gemm_ws_min_bytes(), 256);
   w.gemm = take(w.gemm_bytes);
-  w.x0 = take((int64_t)B * lm->d * 2);
-  w.x1 = take((int64_t)B * lm->d * 2);
-  w.h = take((int64_t)B * lm->d * 2);
-  w.qkv = take((int64_t)B * lm->qkv_dim * 2);
-  w.ao = take((int64_t)B * lm->d * 2);
+  w.x0 = take((int64_t)B * lm->d * 2 * pf);
+  w.x1 = take((int64_t)B * lm->d * 2 * pf);
+  w.h = take((int64_t)B * lm->d * 2 * pf);
+  w.qkv = take((int64_t)B * lm->qkv_dim * 2 * pf);
+  w.ao = take((int64_t)B * lm->d * 2 * pf);
   // Qwen2: gate|up [B, 2F]; GPT-NeoX: pre-activation [B, F] followed by ln2's output [B, d]
-  w.gu = take((int64_t)B * std::max(2 * lm->F, lm->F + lm->d) * 2);
+  w.gu = take((int64_t)B * std::max(2 * lm->F, lm->F + lm->d) * 2 * pf);
   w.act = take((int64_t)B * lm->F * 2);
   w.lens = take((int64_t)B * 4);
   w.partial = take(sk_attn_decode_partial_bytes(B, lm->H, T_cache));
+  if (lm->fp32) w.e32 = take((int64_t)B * lm->d * 4);
   w.total = cur;
   return w;
 }
@@ -498,7 +507,38 @@ WsLayout make_neox_layout(const SkLm* lm, int B, int T) {
   return w;
 }
 
+// OPT fp32 inference (forward only): every activation is a (hi, lo) bf16 pair [M, cols], lo at hi + the slab stride
+// (sX, sqkv, sgu); no per-layer copies.  X / xmid are the residual stream before / after the attention branch, h1 the
+// LayerNorm outputs (the final one included), gu relu(fc1); embed_scratch the fp32 embedding sum; logits fp32 [M, Vp].
+WsLayout make_opt_fp32_layout(const SkLm* lm, int B, int T) {
+  WsLayout w{};
+  const int64_t M = (int64_t)B * T;
+  int64_t cur = 0;
+  auto take = [&](int64_t bytes) {
+    const int64_t o = cur;
+    cur = align_up(cur + bytes, 256);
+    return o;
+  };
+  w.sX = w.sh = align_up(M * lm->d * 2, 256);
+  w.sqkv = align_up(M * lm->qkv_dim * 2, 256);
+  w.sgu = align_up(M * lm->F * 2, 256);
+  // the split GEMMs take no scratch: only the 4 KB of flag words that sk_lm_bind clears at the fixed offset
+  w.splitk_bytes = 4096;
+  w.splitk = take(w.splitk_bytes);
+  w.X = take(2 * w.sX);
+  w.xmid = take(2 * w.sX);
+  w.h1 = take(2 * w.sX);
+  w.qkv = take(2 * w.sqkv);
+  w.ao = take(2 * w.sX);
+  w.gu = take(2 * w.sgu);
+  w.embed_scratch = take(M * lm->d * 4);
+  w.logits = take(M * lm->Vp * 4);
+  w.total = cur;
+  return w;
+}
+
 WsLayout layout_of(const SkLm* lm, int B, int T) {
+  if (lm->fp32) return make_opt_fp32_layout(lm, B, T);
   if (lm->arch == SK_ARCH_NEOX) return make_neox_layout(lm, B, T);
   return lm->arch == SK_ARCH_OPT ? make_opt_layout(lm, B, T) : make_layout(lm, B, T);
 }
@@ -978,6 +1018,100 @@ int opt_decode_step(SkLm* lm, const int64_t* tokens, const int32_t* pos, int B, 
   return sk_gemm_launch(B, lm->Vp, d, h, d, 0, P + lm->off_head, d, 0, logits, ldl, 0, nullptr, nullptr, 0, 0, 0, 0, s);
 }
 
+// ---- OPT fp32 inference (sk_lm_set_fp32): HF OPTForCausalLM in fp32, as the reference scores and generates a float32
+// checkpoint.  Every linear is the split-bf16 three-product GEMM (hi*hi + hi*lo + lo*hi, fp32 accumulation) on the
+// (hi, lo) weight copy with the fp32 bias; activations and the residual stream are (hi, lo) pairs; LayerNorms read the
+// pair (plus an optional second one) with fp32 gamma / beta; attention is the causal split-bf16 kernel; the lm_head
+// writes fp32 logits.
+struct Pair {
+  bf16* hi;
+  bf16* lo;
+};
+
+// sk_linear_split_launch on the split weights at w_off (bias fp32 at b_off >= 0)
+int linear_split(const SkLm* lm, int M, int N, int K, Pair x, int64_t w_off, int64_t b_off, int act, const Pair* res, Pair y,
+                 float* y32, int ldy, cudaStream_t s) {
+  return sk_linear_split_launch(M, N, K, x.hi, x.lo, lm->w_hi + w_off, lm->w_lo + w_off,
+                                b_off >= 0 ? lm->params32 + b_off : nullptr, act, res ? res->hi : nullptr,
+                                res ? res->lo : nullptr, y.hi, y.lo, y32, ldy, s);
+}
+
+// kv (optional, prefill): the fp32 cache of T_cache positions that receives the K / V of positions < lens[b]
+int opt_forward_fp32(SkLm* lm, const int64_t* ids, int B, int T, const WsLayout& w, cudaStream_t s, bool with_head,
+                     float* kv = nullptr, const int32_t* lens = nullptr, int T_cache = 0) {
+  const int M = B * T, d = lm->d, F = lm->F, L = lm->L, Q = lm->qkv_dim;
+  const float eps = lm->cfg.rms_eps;
+  const float* P32 = lm->params32;
+  auto pair = [&](int64_t off, int64_t stride) { return Pair{wsp<bf16>(lm, off), wsp<bf16>(lm, off + stride)}; };
+  const Pair x = pair(w.X, w.sX), xm = pair(w.xmid, w.sX), h = pair(w.h1, w.sX), qkv = pair(w.qkv, w.sqkv),
+             ao = pair(w.ao, w.sX), a = pair(w.gu, w.sgu);
+  float* e32 = wsp<float>(lm, w.embed_scratch);
+  SK_TRY(sk_opt_embed_fwd_f32_launch(ids, nullptr, P32 + lm->off_embed, P32 + lm->off_pos, e32, M, T, d, lm->V, lm->n_pos, s));
+  SK_TRY(sk_split_f32_launch(e32, x.hi, x.lo, (long)M * d, s));
+  // q * head_dim^-0.5 = q / 8 (HF:modeling_opt.py:146): a power of two, folded into the softmax scale exactly
+  const float scale = 1.0f / sqrtf((float)lm->hd);
+  const size_t plane = (size_t)B * lm->H * T_cache * lm->hd;
+  for (int l = 0; l < L; ++l) {
+    const OptLayerOff& o = lm->olo[l];
+    SK_TRY(sk_layernorm_hilo_launch(x.hi, x.lo, nullptr, nullptr, P32 + o.ln1w, P32 + o.ln1b, h.hi, h.lo, nullptr, M, d, eps, s));
+    SK_TRY(linear_split(lm, M, Q, d, h, o.wqkv, o.bqkv, 0, nullptr, qkv, nullptr, Q, s));
+    if (kv) SK_TRY(sk_kv_prefill_f32_launch(qkv.hi, qkv.lo, Q, kv + (size_t)l * 2 * plane, lens, B, T, lm->H, T_cache, s));
+    SK_TRY(sk_attn_tc_fwd_split_launch(qkv.hi, qkv.lo, ao.hi, ao.lo, B, T, lm->H, Q, d, scale, s, 1));
+    SK_TRY(linear_split(lm, M, d, d, ao, o.wo, o.bo, 0, &x, xm, nullptr, d, s));
+    SK_TRY(sk_layernorm_hilo_launch(xm.hi, xm.lo, nullptr, nullptr, P32 + o.ln2w, P32 + o.ln2b, h.hi, h.lo, nullptr, M, d, eps, s));
+    SK_TRY(linear_split(lm, M, F, d, h, o.w1, o.b1, 2, nullptr, a, nullptr, F, s));   // relu(fc1)
+    SK_TRY(linear_split(lm, M, d, F, a, o.w2, o.b2, 0, &xm, x, nullptr, d, s));
+  }
+  SK_TRY(sk_layernorm_hilo_launch(x.hi, x.lo, nullptr, nullptr, P32 + lm->off_final_norm, P32 + lm->off_final_norm_b, h.hi,
+                                  h.lo, nullptr, M, d, eps, s));
+  lm->last_B = B;
+  lm->last_T = T;
+  if (!with_head) return 0;
+  return linear_split(lm, M, lm->Vp, d, h, lm->off_head, -1, 0, nullptr, Pair{nullptr, nullptr}, wsp<float>(lm, w.logits),
+                      lm->Vp, s);
+}
+
+// One token per row at position pos[b] on the fp32 cache ([K|V][B][H][T_cache][64] fp32 per layer); fp32 logits [B, ldl]
+int opt_decode_step_fp32(SkLm* lm, const int64_t* tokens, const int32_t* pos, int B, float* kv, int T_cache, float* logits,
+                         int ldl, uint8_t* dws, const DecLayout& dl, cudaStream_t s) {
+  const int d = lm->d, F = lm->F, Q = lm->qkv_dim;
+  const float eps = lm->cfg.rms_eps;
+  const float* P32 = lm->params32;
+  auto pair = [&](int64_t off, int64_t n) {
+    bf16* hi = reinterpret_cast<bf16*>(dws + off);
+    return Pair{hi, hi + n};
+  };
+  const Pair x = pair(dl.x0, (int64_t)B * d), xm = pair(dl.x1, (int64_t)B * d), h = pair(dl.h, (int64_t)B * d),
+             qkv = pair(dl.qkv, (int64_t)B * Q), ao = pair(dl.ao, (int64_t)B * d), a = pair(dl.gu, (int64_t)B * F);
+  int32_t* lens = reinterpret_cast<int32_t*>(dws + dl.lens);
+  float* partial = reinterpret_cast<float*>(dws + dl.partial);
+  float* e32 = reinterpret_cast<float*>(dws + dl.e32);
+  const size_t plane = (size_t)B * lm->H * T_cache * lm->hd;
+  const float scale = 1.0f / sqrtf((float)lm->hd);
+  SK_TRY(sk_opt_embed_fwd_f32_launch(tokens, pos, P32 + lm->off_embed, P32 + lm->off_pos, e32, B, 1, d, lm->V, lm->n_pos, s));
+  SK_TRY(sk_split_f32_launch(e32, x.hi, x.lo, (long)B * d, s));
+  for (int l = 0; l < lm->L; ++l) {
+    const OptLayerOff& o = lm->olo[l];
+    float* kc = kv + (size_t)l * 2 * plane;
+    float* vc = kc + plane;
+    SK_TRY(sk_layernorm_hilo_launch(x.hi, x.lo, nullptr, nullptr, P32 + o.ln1w, P32 + o.ln1b, h.hi, h.lo, nullptr, B, d, eps, s));
+    SK_TRY(linear_split(lm, B, Q, d, h, o.wqkv, o.bqkv, 0, nullptr, qkv, nullptr, Q, s));
+    SK_TRY(sk_kv_append_f32_launch(qkv.hi, qkv.lo, Q, kc, vc, pos, lens, B, lm->H, T_cache, s));
+    SK_TRY(sk_attn_decode_f32_launch(qkv.hi, qkv.lo, Q, kc, vc, lens, ao.hi, ao.lo, d, partial, B, lm->H, T_cache, scale, s));
+    SK_TRY(linear_split(lm, B, d, d, ao, o.wo, o.bo, 0, &x, xm, nullptr, d, s));
+    SK_TRY(sk_layernorm_hilo_launch(xm.hi, xm.lo, nullptr, nullptr, P32 + o.ln2w, P32 + o.ln2b, h.hi, h.lo, nullptr, B, d, eps, s));
+    SK_TRY(linear_split(lm, B, F, d, h, o.w1, o.b1, 2, nullptr, a, nullptr, F, s));
+    SK_TRY(linear_split(lm, B, d, F, a, o.w2, o.b2, 0, &xm, x, nullptr, d, s));
+  }
+  SK_TRY(sk_layernorm_hilo_launch(x.hi, x.lo, nullptr, nullptr, P32 + lm->off_final_norm, P32 + lm->off_final_norm_b, h.hi,
+                                  h.lo, nullptr, B, d, eps, s));
+  return linear_split(lm, B, lm->Vp, d, h, lm->off_head, -1, 0, nullptr, Pair{nullptr, nullptr}, logits, ldl, s);
+}
+
+#define SK_REFUSE_FP32(lm, who)                                                                                          \
+  SK_REQUIRE(!(lm)->fp32, who ": this handle runs fp32 inference (sk_lm_set_fp32), which is forward only; train with a " \
+                          "bf16 or master-weights handle")
+
 // gradient-norm groups (one per HF parameter) and their device chunk tables; `groups` lists (offset, n) ranges
 int upload_norm_groups(SkLm* lm, const std::vector<std::vector<std::pair<int64_t, int64_t>>>& groups) {
   std::vector<long> cs;
@@ -1009,7 +1143,7 @@ extern "C" {
 
 int64_t sk_lm_kv_cache_bytes(const SkLm* lm, int B, int T_cache) {
   if (!lm || B <= 0 || T_cache <= 0) return 0;
-  return (int64_t)lm->L * 2 * B * lm->KVH * T_cache * lm->hd * 2;
+  return (int64_t)lm->L * 2 * B * lm->KVH * T_cache * lm->hd * (lm->fp32 ? 4 : 2);
 }
 
 int64_t sk_lm_decode_workspace_bytes(const SkLm* lm, int B, int T_cache) {
@@ -1030,6 +1164,16 @@ int sk_lm_prefill(SkLm* lm, const int64_t* ids, const int32_t* lens, int B, int 
   cudaStream_t s = (cudaStream_t)stream;
   uint8_t* dws = reinterpret_cast<uint8_t*>(decode_ws);
   SK_CUDA_CHECK(cudaMemsetAsync(dws + dl.gemm + dl.gemm_bytes - 4096, 0, 4096, s));
+  if (lm->fp32) {
+    SK_TRY(opt_forward_fp32(lm, ids, B, T, w, s, false, reinterpret_cast<float*>(kv_cache), lens, T_cache));
+    const int64_t n = (int64_t)B * lm->d;
+    const Pair hf{wsp<bf16>(lm, w.h1), wsp<bf16>(lm, w.h1 + w.sX)};
+    const Pair hl{reinterpret_cast<bf16*>(dws + dl.h), reinterpret_cast<bf16*>(dws + dl.h) + n};
+    SK_TRY(sk_gather_last_launch(hf.hi, lens, hl.hi, B, T, lm->d, s));
+    SK_TRY(sk_gather_last_launch(hf.lo, lens, hl.lo, B, T, lm->d, s));
+    return linear_split(lm, B, lm->Vp, lm->d, hl, lm->off_head, -1, 0, nullptr, Pair{nullptr, nullptr},
+                        reinterpret_cast<float*>(logits), ldl, s);
+  }
   if (lm->arch == SK_ARCH_OPT)       SK_TRY(opt_forward(lm, ids, nullptr, nullptr, B, T, 0.f, 1.f, false, nullptr, w, s, nullptr, false));
   else if (lm->arch == SK_ARCH_NEOX) SK_TRY(neox_forward(lm, ids, nullptr, nullptr, B, T, 0.f, 1.f, false, nullptr, w, s, nullptr, false));
   else                               SK_TRY(forward_impl(lm, ids, nullptr, nullptr, B, T, 0.f, 1.f, false, nullptr, w, s, nullptr, false));
@@ -1049,6 +1193,9 @@ int sk_lm_decode_step(SkLm* lm, const int64_t* tokens, const int32_t* pos, int B
   const DecLayout dl = make_dec_layout(lm, B, T_cache);
   SK_TRY(check_decode(lm, B, T_cache, ldl, kv_cache, logits, decode_ws, decode_ws_bytes, dl));
   cudaStream_t s = (cudaStream_t)stream;
+  if (lm->fp32)
+    return opt_decode_step_fp32(lm, tokens, pos, B, reinterpret_cast<float*>(kv_cache), T_cache, reinterpret_cast<float*>(logits),
+                                ldl, reinterpret_cast<uint8_t*>(decode_ws), dl, s);
   if (lm->arch == SK_ARCH_OPT)
     return opt_decode_step(lm, tokens, pos, B, kv_cache, T_cache, logits, ldl, reinterpret_cast<uint8_t*>(decode_ws), dl, s);
   if (lm->arch == SK_ARCH_NEOX)
@@ -1409,6 +1556,8 @@ int sk_lm_set_master(SkLm* lm, float* params32, float* grads32) {
   SK_REQUIRE(lm->arch == SK_ARCH_OPT, "sk_lm_set_master: fp32 master weights are implemented for the OPT decoder only (the "
                                       "Qwen2 and GPT-NeoX recipes train bf16 parameters)");
   SK_REQUIRE(lm->params && lm->ws, "sk_lm_set_master: call sk_lm_bind first");
+  SK_REQUIRE(!lm->fp32, "sk_lm_set_master: this handle runs fp32 inference (sk_lm_set_fp32); master weights are a training "
+                        "mode, create a separate handle");
   SK_REQUIRE(((uintptr_t)params32 & 127) == 0 && ((uintptr_t)grads32 & 127) == 0,
              "sk_lm_set_master: params32 / grads32 must be 128-byte aligned");
   if (!lm->d_widen_start) {
@@ -1441,10 +1590,40 @@ int sk_lm_set_master(SkLm* lm, float* params32, float* grads32) {
   return 0;
 }
 
+int64_t sk_lm_fp32_prepared_bytes(const SkLm* lm) { return lm ? 2 * align_up(lm->n_params * 2, 256) : 0; }
+
+int sk_lm_set_fp32(SkLm* lm, const float* params32, void* prepared, int64_t prepared_bytes, void* stream) {
+  SK_REQUIRE(lm && params32 && prepared, "sk_lm_set_fp32: null argument");
+  SK_REQUIRE(lm->arch == SK_ARCH_OPT, "sk_lm_set_fp32: fp32 inference is implemented for the OPT decoder only (the Qwen2 and "
+                                      "GPT-NeoX recipes are bf16)");
+  SK_REQUIRE(lm->params && lm->ws, "sk_lm_set_fp32: call sk_lm_bind first");
+  SK_REQUIRE(!lm->master, "sk_lm_set_fp32: this handle trains fp32 master weights (sk_lm_set_master); score its saved "
+                          "checkpoint with a separate handle");
+  SK_REQUIRE(lm->d <= 1024, "sk_lm_set_fp32: hidden must be <= 1024 (got %d)", lm->d);
+  SK_REQUIRE(prepared_bytes >= sk_lm_fp32_prepared_bytes(lm), "sk_lm_set_fp32: prepared buffer too small: need %lld bytes",
+             (long long)sk_lm_fp32_prepared_bytes(lm));
+  SK_REQUIRE(((uintptr_t)params32 & 127) == 0 && ((uintptr_t)prepared & 255) == 0,
+             "sk_lm_set_fp32: params32 must be 128-byte and prepared 256-byte aligned");
+  uint8_t* p = reinterpret_cast<uint8_t*>(prepared);
+  lm->params32 = const_cast<float*>(params32);
+  lm->w_hi = reinterpret_cast<bf16*>(p);
+  lm->w_lo = reinterpret_cast<bf16*>(p + align_up(lm->n_params * 2, 256));
+  SK_TRY(sk_split_f32_launch(params32, lm->w_hi, lm->w_lo, (long)lm->n_params, (cudaStream_t)stream));
+  lm->fp32 = true;
+  return 0;
+}
+
 int sk_lm_forward(SkLm* lm, const int64_t* ids, const int64_t* labels, const int32_t* pos_ids, int B, int T,
                   float num_items, float* stats, void* stream) {
   SK_REQUIRE(lm && ids, "sk_lm_forward: null argument");
   SK_REQUIRE(labels == nullptr || stats != nullptr, "sk_lm_forward: stats is required when labels are given");
+  if (lm->fp32) {
+    SK_REQUIRE(labels == nullptr && pos_ids == nullptr, "sk_lm_forward: an fp32 inference handle (sk_lm_set_fp32) takes "
+                                                        "neither labels (score with sk_seq_loglik_f32) nor position_ids");
+    const WsLayout w = layout_of(lm, B, T);
+    SK_TRY(check_bound(lm, B, T, w, nullptr));
+    return opt_forward_fp32(lm, ids, B, T, w, (cudaStream_t)stream, true);
+  }
   const WsLayout w = layout_of(lm, B, T);
   SK_TRY(check_bound(lm, B, T, w, pos_ids));
   if (lm->arch == SK_ARCH_OPT)
@@ -1457,6 +1636,7 @@ int sk_lm_forward(SkLm* lm, const int64_t* ids, const int64_t* labels, const int
 int sk_lm_forward_backward(SkLm* lm, const int64_t* ids, const int64_t* labels, const int32_t* pos_ids, int B, int T,
                            float num_items, float dloss, int accumulate, float* stats, void* stream) {
   SK_REQUIRE(lm && ids && labels && stats, "sk_lm_forward_backward: null argument");
+  SK_REFUSE_FP32(lm, "sk_lm_forward_backward");
   SK_REQUIRE(lm->grads, "sk_lm_forward_backward: no gradient buffer bound");
   SK_REQUIRE(!lm->master || lm->grads32, "sk_lm_forward_backward: no fp32 gradient buffer given to sk_lm_set_master");
   const WsLayout w = layout_of(lm, B, T);
@@ -1506,6 +1686,7 @@ int sk_lm_set_backward_events(SkLm* lm, void* const* events, int n) {
 int sk_lm_forward_rows(SkLm* lm, const int64_t* ids, const int64_t* labels, const int32_t* pos_ids, int B, int T,
                        float* row_nll, float* stats, void* stream) {
   SK_REQUIRE(lm && ids && labels && row_nll && stats, "sk_lm_forward_rows: null argument");
+  SK_REFUSE_FP32(lm, "sk_lm_forward_rows");
   const WsLayout w = layout_of(lm, B, T);
   SK_TRY(check_bound(lm, B, T, w, pos_ids));
   if (lm->arch == SK_ARCH_OPT)
@@ -1518,6 +1699,7 @@ int sk_lm_forward_rows(SkLm* lm, const int64_t* ids, const int64_t* labels, cons
 int sk_lm_backward_weighted(SkLm* lm, const int64_t* ids, const int64_t* labels, const int32_t* pos_ids, int B, int T,
                             const float* row_weight, int accumulate, float* stats, void* stream) {
   SK_REQUIRE(lm && ids && labels && row_weight && stats, "sk_lm_backward_weighted: null argument");
+  SK_REFUSE_FP32(lm, "sk_lm_backward_weighted");
   SK_REQUIRE(lm->grads, "sk_lm_backward_weighted: no gradient buffer bound");
   SK_REQUIRE(!lm->master || lm->grads32, "sk_lm_backward_weighted: no fp32 gradient buffer given to sk_lm_set_master");
   SK_REQUIRE(lm->last_B == B && lm->last_T == T, "sk_lm_backward_weighted: call sk_lm_forward_rows on the same batch first");
@@ -1534,8 +1716,12 @@ int sk_lm_backward_weighted(SkLm* lm, const int64_t* ids, const int64_t* labels,
 }
 
 const void* sk_lm_logits(const SkLm* lm) {
-  if (!lm || !lm->ws || lm->last_B == 0) return nullptr;
+  if (!lm || !lm->ws || lm->last_B == 0 || lm->fp32) return nullptr;
   return lm->ws + layout_of(lm, lm->last_B, lm->last_T).logits;
+}
+const float* sk_lm_logits_f32(const SkLm* lm) {
+  if (!lm || !lm->ws || lm->last_B == 0 || !lm->fp32) return nullptr;
+  return reinterpret_cast<const float*>(lm->ws + layout_of(lm, lm->last_B, lm->last_T).logits);
 }
 int sk_lm_logits_ld(const SkLm* lm) { return lm ? lm->Vp : 0; }
 
@@ -1543,6 +1729,7 @@ int sk_lm_optimizer_step(SkLm* lm, void* exp_avg, void* exp_avg_sq, float lr, fl
                          float weight_decay, int step, float max_grad_norm, int emulate_bf16_norm, float* stats,
                          void* stream) {
   SK_REQUIRE(lm && exp_avg && exp_avg_sq && stats, "sk_lm_optimizer_step: null argument");
+  SK_REFUSE_FP32(lm, "sk_lm_optimizer_step");
   SK_REQUIRE(lm->params && lm->grads, "sk_lm_optimizer_step: params/grads not bound");
   cudaStream_t s = (cudaStream_t)stream;
   if (lm->master) {

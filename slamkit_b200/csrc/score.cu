@@ -8,6 +8,8 @@
 //   seq   = bf16(sum_t nll_t)                                fp32 accumulation of the bf16 values, one rounding
 //   mean  = bf16(seq / count)                                bf16 / int64 -> float division, one rounding
 // Banned columns are -inf before the softmax; a target equal to the model's pad id is masked (0, not counted).
+// An fp32 model (sk_seq_loglik_f32: fp32 OPT inference) is scored in fp32 throughout, as calc_nll does on fp32 logits:
+// the same kernels on fp32 logits with every bf16 rounding above left out.
 #include "kernels.h"
 #include "../../include/slamkit_b200.h"
 
@@ -16,7 +18,24 @@ namespace {
 constexpr float kLog2e = 1.4426950408889634f;
 constexpr int kWarpRowMaxV = 8192;   // up to this many columns a warp scores a row; beyond it a 256-thread CTA does
 
+SK_DEVINL float logit_at(const bf16* row, long i) { return __bfloat162float(row[i]); }
+SK_DEVINL float logit_at(const float* row, long i) { return row[i]; }
+
 // eight columns [c0, c0 + 8) of a logits row as fp32, -inf where banned or at/after V (those columns are not read)
+SK_DEVINL void load8(const float* __restrict__ row, int c0, int V, const uint32_t* __restrict__ ban, float (&v)[8]) {
+  const uint32_t bits = ban ? (__ldg(ban + (c0 >> 5)) >> (c0 & 31)) & 0xffu : 0u;
+  if (c0 + 8 <= V) {
+    const float4 a = __ldcs(reinterpret_cast<const float4*>(row + c0)), b = __ldcs(reinterpret_cast<const float4*>(row + c0 + 4));
+    v[0] = a.x; v[1] = a.y; v[2] = a.z; v[3] = a.w;
+    v[4] = b.x; v[5] = b.y; v[6] = b.z; v[7] = b.w;
+  } else {
+#pragma unroll
+    for (int k = 0; k < 8; ++k) v[k] = (c0 + k < V) ? row[c0 + k] : -INFINITY;
+  }
+#pragma unroll
+  for (int k = 0; k < 8; ++k)
+    if ((bits >> k) & 1u) v[k] = -INFINITY;
+}
 SK_DEVINL void load8(const bf16* __restrict__ row, int c0, int V, const uint32_t* __restrict__ ban, float (&v)[8]) {
   const uint32_t bits = ban ? (__ldg(ban + (c0 >> 5)) >> (c0 & 31)) & 0xffu : 0u;
   if (c0 + 8 <= V) {
@@ -66,13 +85,18 @@ SK_DEVINL void ms_warp(float& m, float& s) {
 }
 
 // target logit of a row (-inf when banned): the same value the softmax saw
-SK_DEVINL float target_logit(const bf16* __restrict__ row, long y, const uint32_t* __restrict__ ban) {
+template <typename LT>
+SK_DEVINL float target_logit(const LT* __restrict__ row, long y, const uint32_t* __restrict__ ban) {
   if (ban && ((__ldg(ban + (y >> 5)) >> (y & 31)) & 1u)) return -INFINITY;
-  return __bfloat162float(row[y]);
+  return logit_at(row, y);
 }
 
-// torch's log_softmax epilogue ((x - max) - log(sum)) in fp32, rounded to bf16, negated by nll_loss
-SK_DEVINL float token_value(float zy, float m, float s) { return -bf16_round((zy - m) - logf(s)); }
+// torch's log_softmax epilogue ((x - max) - log(sum)) in fp32, rounded to bf16 on a bf16 model, negated by nll_loss
+template <bool ROUND>
+SK_DEVINL float token_value(float zy, float m, float s) {
+  const float lp = (zy - m) - logf(s);
+  return -(ROUND ? bf16_round(lp) : lp);
+}
 
 // Scoring row r = b * (T - 1) + t: logits row b * T + t against target ids[b, t + 1].  A pad target is masked: its
 // logits row is not read and its value is 0.  A target outside [0, V) gives NaN.
@@ -86,8 +110,9 @@ SK_DEVINL RowTarget row_target(const int64_t* __restrict__ ids, int r, int T, in
   return {y, y == pad ? 1 : (y < 0 || y >= V) ? 2 : 0};
 }
 
+template <typename LT, bool ROUND>
 __global__ void __launch_bounds__(256)
-seqll_warp_kernel(const bf16* __restrict__ logits, int ldl, int V, const int64_t* __restrict__ ids, int R, int T, int pad,
+seqll_warp_kernel(const LT* __restrict__ logits, int ldl, int V, const int64_t* __restrict__ ids, int R, int T, int pad,
                   const uint32_t* __restrict__ ban, float* __restrict__ token_nll) {
   const int r = blockIdx.x * 8 + (threadIdx.x >> 5), lane = threadIdx.x & 31;
   if (r >= R) return;
@@ -97,7 +122,7 @@ seqll_warp_kernel(const bf16* __restrict__ logits, int ldl, int V, const int64_t
     return;
   }
   const int b = r / (T - 1), t = r % (T - 1);
-  const bf16* row = logits + ((size_t)b * T + t) * ldl;
+  const LT* row = logits + ((size_t)b * T + t) * ldl;
   float m = -INFINITY, s = 0.f;
   for (int c0 = lane * 8; c0 < V; c0 += 32 * 8) {
     float v[8];
@@ -105,11 +130,12 @@ seqll_warp_kernel(const bf16* __restrict__ logits, int ldl, int V, const int64_t
     ms_update(v, m, s);
   }
   ms_warp(m, s);
-  if (lane == 0) token_nll[r] = token_value(target_logit(row, tg.y, ban), m, s);
+  if (lane == 0) token_nll[r] = token_value<ROUND>(target_logit(row, tg.y, ban), m, s);
 }
 
+template <typename LT, bool ROUND>
 __global__ void __launch_bounds__(256)
-seqll_cta_kernel(const bf16* __restrict__ logits, int ldl, int V, const int64_t* __restrict__ ids, int T, int pad,
+seqll_cta_kernel(const LT* __restrict__ logits, int ldl, int V, const int64_t* __restrict__ ids, int T, int pad,
                  const uint32_t* __restrict__ ban, float* __restrict__ token_nll) {
   __shared__ float s_m[8], s_s[8];
   const int r = blockIdx.x;
@@ -119,7 +145,7 @@ seqll_cta_kernel(const bf16* __restrict__ logits, int ldl, int V, const int64_t*
     return;
   }
   const int b = r / (T - 1), t = r % (T - 1);
-  const bf16* row = logits + ((size_t)b * T + t) * ldl;
+  const LT* row = logits + ((size_t)b * T + t) * ldl;
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   float m = -INFINITY, s = 0.f;
   // four 16-byte loads in flight per thread before any of them is used
@@ -143,14 +169,17 @@ seqll_cta_kernel(const bf16* __restrict__ logits, int ldl, int V, const int64_t*
     s = s_s[0];
 #pragma unroll
     for (int i = 1; i < 8; ++i) ms_combine(m, s, s_m[i], s_s[i]);
-    token_nll[r] = token_value(target_logit(row, tg.y, ban), m, s);
+    token_nll[r] = token_value<ROUND>(target_logit(row, tg.y, ban), m, s);
   }
 }
 
-// one warp per sequence: fixed-order fp32 sum of the bf16 token values (lane-strided partial sums, then a butterfly)
+// one warp per sequence: fixed-order fp32 sum of the token values (lane-strided partial sums, then a butterfly)
+SK_DEVINL void store_ll(bf16* out, float v) { *out = __float2bfloat16_rn(v); }
+SK_DEVINL void store_ll(float* out, float v) { *out = v; }
+template <typename OT, bool ROUND>
 __global__ void __launch_bounds__(256)
 seqll_reduce_kernel(const int64_t* __restrict__ ids, const float* __restrict__ token_nll, int B, int T, int pad, int mean_nll,
-                    bf16* __restrict__ ll_out) {
+                    OT* __restrict__ ll_out) {
   const int b = blockIdx.x * 8 + (threadIdx.x >> 5), lane = threadIdx.x & 31;
   if (b >= B) return;
   float acc = 0.f;
@@ -167,9 +196,13 @@ seqll_reduce_kernel(const int64_t* __restrict__ ids, const float* __restrict__ t
     cnt += __shfl_xor_sync(0xffffffffu, cnt, o);
   }
   if (lane == 0) {
-    const float sum = bf16_round(acc);
-    const float v = mean_nll ? bf16_round(__fdiv_rn(sum, (float)cnt)) : sum;   // count 0: 0 / 0 = NaN, as the reference
-    ll_out[b] = __float2bfloat16_rn(-v);
+    const float sum = ROUND ? bf16_round(acc) : acc;
+    float v = sum;
+    if (mean_nll) {   // count 0: 0 / 0 = NaN, as the reference
+      v = __fdiv_rn(sum, (float)cnt);
+      if (ROUND) v = bf16_round(v);
+    }
+    store_ll(ll_out + b, -v);
   }
 }
 
@@ -188,33 +221,47 @@ __global__ void units_to_tokens_kernel(const int32_t* __restrict__ units, const 
   ids[i] = v;
 }
 
+// LT: logits element type; OT: ll_out element type; ROUND: the bf16 model's roundings
+template <typename LT, typename OT, bool ROUND>
+int seq_loglik(const char* who, const void* logits, int ldl, int V, const int64_t* ids, int B, int T, int pad_id,
+               const uint32_t* ban_bits, int mean_nll, float* token_nll, void* ll_out, cudaStream_t s) {
+  SK_REQUIRE(logits && ids && token_nll && ll_out, "%s: null argument", who);
+  SK_REQUIRE(B > 0 && T >= 1, "%s: bad shape B=%d T=%d", who, B, T);
+  SK_REQUIRE(V >= 2 && V <= (1 << 20), "%s: V=%d outside [2, 2^20]", who, V);
+  SK_REQUIRE(ldl >= V && ldl % 8 == 0, "%s: ldl must be >= V and a multiple of 8 (ldl=%d V=%d)", who, ldl, V);
+  SK_REQUIRE(((uintptr_t)logits & 15) == 0, "%s: logits must be 16-byte aligned", who);
+  SK_REQUIRE(((uintptr_t)ban_bits & 3) == 0, "%s: ban_bits must be 4-byte aligned", who);
+  SK_REQUIRE(mean_nll == 0 || mean_nll == 1, "%s: mean_nll must be 0 or 1", who);
+  SK_REQUIRE((long)B * T < (1L << 31), "%s: B*T=%ld too large", who, (long)B * T);
+  const LT* lg = reinterpret_cast<const LT*>(logits);
+  const int R = B * (T - 1);
+  if (R > 0) {
+    if (V <= kWarpRowMaxV)
+      seqll_warp_kernel<LT, ROUND><<<(R + 7) / 8, 256, 0, s>>>(lg, ldl, V, ids, R, T, pad_id, ban_bits, token_nll);
+    else
+      seqll_cta_kernel<LT, ROUND><<<R, 256, 0, s>>>(lg, ldl, V, ids, T, pad_id, ban_bits, token_nll);
+    SK_LAUNCH_CHECK();
+  }
+  seqll_reduce_kernel<OT, ROUND><<<(B + 7) / 8, 256, 0, s>>>(ids, token_nll, B, T, pad_id, mean_nll,
+                                                            reinterpret_cast<OT*>(ll_out));
+  SK_LAUNCH_CHECK();
+  return 0;
+}
+
 }  // namespace
 
 extern "C" {
 
 int sk_seq_loglik(const void* logits, int ldl, int V, const int64_t* ids, int B, int T, int pad_id,
                   const uint32_t* ban_bits, int mean_nll, float* token_nll, void* ll_out, void* stream) {
-  SK_REQUIRE(logits && ids && token_nll && ll_out, "sk_seq_loglik: null argument");
-  SK_REQUIRE(B > 0 && T >= 1, "sk_seq_loglik: bad shape B=%d T=%d", B, T);
-  SK_REQUIRE(V >= 2 && V <= (1 << 20), "sk_seq_loglik: V=%d outside [2, 2^20]", V);
-  SK_REQUIRE(ldl >= V && ldl % 8 == 0, "sk_seq_loglik: ldl must be >= V and a multiple of 8 (ldl=%d V=%d)", ldl, V);
-  SK_REQUIRE(((uintptr_t)logits & 15) == 0, "sk_seq_loglik: logits must be 16-byte aligned");
-  SK_REQUIRE(((uintptr_t)ban_bits & 3) == 0, "sk_seq_loglik: ban_bits must be 4-byte aligned");
-  SK_REQUIRE(mean_nll == 0 || mean_nll == 1, "sk_seq_loglik: mean_nll must be 0 or 1");
-  SK_REQUIRE((long)B * T < (1L << 31), "sk_seq_loglik: B*T=%ld too large", (long)B * T);
-  cudaStream_t s = (cudaStream_t)stream;
-  const bf16* lg = reinterpret_cast<const bf16*>(logits);
-  const int R = B * (T - 1);
-  if (R > 0) {
-    if (V <= kWarpRowMaxV)
-      seqll_warp_kernel<<<(R + 7) / 8, 256, 0, s>>>(lg, ldl, V, ids, R, T, pad_id, ban_bits, token_nll);
-    else
-      seqll_cta_kernel<<<R, 256, 0, s>>>(lg, ldl, V, ids, T, pad_id, ban_bits, token_nll);
-    SK_LAUNCH_CHECK();
-  }
-  seqll_reduce_kernel<<<(B + 7) / 8, 256, 0, s>>>(ids, token_nll, B, T, pad_id, mean_nll, reinterpret_cast<bf16*>(ll_out));
-  SK_LAUNCH_CHECK();
-  return 0;
+  return seq_loglik<bf16, bf16, true>("sk_seq_loglik", logits, ldl, V, ids, B, T, pad_id, ban_bits, mean_nll, token_nll,
+                                      ll_out, (cudaStream_t)stream);
+}
+
+int sk_seq_loglik_f32(const float* logits, int ldl, int V, const int64_t* ids, int B, int T, int pad_id,
+                      const uint32_t* ban_bits, int mean_nll, float* token_nll, float* ll_out, void* stream) {
+  return seq_loglik<float, float, false>("sk_seq_loglik_f32", logits, ldl, V, ids, B, T, pad_id, ban_bits, mean_nll,
+                                         token_nll, ll_out, (cudaStream_t)stream);
 }
 
 int sk_units_to_tokens(const int32_t* units, const int32_t* counts, int B, int T_units, int offset, int bos, int eos,

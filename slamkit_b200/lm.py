@@ -276,6 +276,17 @@ def write_unit_lm_checkpoint(save_directory: str, state_dict_hf: Dict[str, torch
         json.dump(cfg, f, indent=2)
 
 
+def checkpoint_is_fp32(config: dict) -> bool:
+    """Whether a `save_pretrained` config.json (top level, else its base_config) names float32 as its dtype, under
+    `torch_dtype` or under `dtype` (the key transformers writes since 4.56)."""
+    def dtype_of(c: dict):
+        return c.get("dtype", c.get("torch_dtype"))
+    dt = dtype_of(config)
+    if dt is None:
+        dt = dtype_of(config.get("base_config") or {})
+    return str(dt).replace("torch.", "") == "float32"
+
+
 def check_right_padded(attention_mask: Optional[torch.Tensor]) -> None:
     """The kernels apply the causal mask only (plus document boundaries from position_ids).  That is exact for the
     reference's batches -- right-padded by DataCollatorForLanguageModeling / `padding_side = "right"`
@@ -296,13 +307,22 @@ class B200UnitLM:
     """Causal unit LM whose forward/backward/optimiser run in libslamkit_b200.so."""
 
     def __init__(self, config, device: str = "cuda:0", max_batch: int = 8, max_seq: int = 1024,
-                 trainable: bool = True, seed: Optional[int] = None, master_weights: bool = False):
+                 trainable: bool = True, seed: Optional[int] = None, master_weights: bool = False,
+                 fp32_inference: bool = False):
         """`config`: `LMConfig` (Qwen2 decoder), `OptLMConfig` (pre-LayerNorm OPT decoder) or `NeoxLMConfig` (GPT-NeoX).
 
         `master_weights` (OPT only): train fp32 parameters, fp32 gradients and fp32 AdamW moments under bf16 autocast
         numerics -- the reference's default recipe (`torch_dtype: null`, `bf16: true`).  `params32` / `grads32` then hold
         the model; `params` is their bf16 shadow that the GEMMs read and `grads` the per-micro-batch bf16 scratch of the
-        linear gradients.  Such a model trains and scores; `generate` refuses it (generate from its saved checkpoint)."""
+        linear gradients.  Such a model trains and scores; `generate` refuses it (generate from its saved checkpoint).
+
+        `fp32_inference` (OPT, `trainable=False`): score and generate in fp32, as the reference runs a float32 checkpoint
+        (`from_pretrained` picks it for one).  `params32` holds the model; the linears run as split-bf16 three-product
+        GEMMs on its (hi, lo) copy, and logits, log-likelihoods and the sampled distribution are fp32-grade."""
+        self.fp32 = bool(fp32_inference)
+        if self.fp32 and (not isinstance(config, OptLMConfig) or trainable or master_weights):
+            raise ValueError("fp32_inference=True is a forward-only mode of the OPT decoder: it needs an OPT config and "
+                             "trainable=False, without master_weights (the Qwen2 and GPT-NeoX recipes are bf16)")
         self.lib = L.require_cuda()
         self.config = config
         self.is_opt = isinstance(config, OptLMConfig)
@@ -336,7 +356,8 @@ class B200UnitLM:
             L.check(self.lib.sk_lm_tensor_info(self._h, i, buf, 64, C.byref(off), C.byref(r), C.byref(cc)))
             self.tensors[buf.value.decode()] = (off.value, r.value, cc.value)
         self.vocab_padded = self.tensors["embed"][1]
-        self.params = torch.zeros(self.n_params, device=self.device, dtype=torch.bfloat16)
+        # fp32 inference reads params32 and its split copy only: the bf16 buffer that sk_lm_bind requires is a placeholder
+        self.params = torch.zeros(64 if self.fp32 else self.n_params, device=self.device, dtype=torch.bfloat16)
         self.grads = torch.zeros(self.n_params, device=self.device, dtype=torch.bfloat16) if trainable else None
         self.rope_cos = self.rope_sin = None          # OPT: learned positions, no RoPE tables
         if not self.is_opt:          # GPT-NeoX: tables over the rotated columns only (partial rotary)
@@ -352,6 +373,12 @@ class B200UnitLM:
             self.grads32 = torch.zeros(self.n_params, device=self.device, dtype=torch.float32) if trainable else None
             L.check(self.lib.sk_lm_set_master(self._h, L.ptr(self.params32), L.ptr(self.grads32)))
             self._bind(max_batch, max_seq)                # the fp32 residual stream needs the larger workspace
+        if self.fp32:
+            self.params32 = torch.zeros(self.n_params, device=self.device, dtype=torch.float32)
+            self.prepared = torch.empty(int(self.lib.sk_lm_fp32_prepared_bytes(self._h)), device=self.device,
+                                        dtype=torch.uint8)
+            self.refresh_shadow()
+            self._bind(max_batch, max_seq)                # (hi, lo) activations and fp32 logits: a larger workspace
         self.stats = torch.zeros(3, device=self.device, dtype=torch.float32)
         if seed is not None:
             self.init_weights(seed)
@@ -370,19 +397,23 @@ class B200UnitLM:
             self._bind(B, T)
 
     def tensor(self, name: str, grad: bool = False) -> torch.Tensor:
-        """A parameter (or its gradient) as a [rows, cols] view of the flat buffers: the fp32 masters with master
-        weights, else the bf16 ones."""
+        """A parameter (or its gradient) as a [rows, cols] view of the flat buffers: the fp32 ones with master weights
+        or fp32 inference, else the bf16 ones."""
         off, r, c = self.tensors[name]
-        if self.master:
+        if self.master or self.fp32:
             flat = self.grads32 if grad else self.params32
         else:
             flat = self.grads if grad else self.params
         return flat[off:off + r * c].view(r, c)
 
     def refresh_shadow(self) -> None:
-        """Master weights: rewrite the bf16 shadow from the fp32 masters (after they are loaded or changed by hand)."""
+        """Master weights: rewrite the bf16 shadow from the fp32 masters; fp32 inference: rewrite the split (hi, lo) copy
+        of params32 (after they are loaded or changed by hand)."""
         if self.master:
             self.params.copy_(self.params32)
+        if self.fp32:
+            L.check(self.lib.sk_lm_set_fp32(self._h, L.ptr(self.params32), L.ptr(self.prepared),
+                                            C.c_int64(self.prepared.numel()), L.stream_ptr()))
 
     def __del__(self):
         try:
@@ -421,7 +452,7 @@ class B200UnitLM:
         g = torch.Generator(device="cpu").manual_seed(seed)
         cfg = self.config
         std = cfg.init_std
-        dt = torch.float32 if self.master else torch.bfloat16
+        dt = torch.float32 if self.master or self.fp32 else torch.bfloat16
         for name, (off, r, c) in self.tensors.items():
             t = self.tensor(name)
             base = name.split(".")[-1]
@@ -533,10 +564,10 @@ class B200UnitLM:
 
     def load_hf_state_dict(self, sd: Dict[str, torch.Tensor], grads: bool = False) -> None:
         """Load parameters named as in `UnitLM.state_dict()` (prefix `lm.`, slamkit/model/unit_lm.py:87).  With master
-        weights the fp32 masters take the values (fp16 / bf16 checkpoints are widened exactly) and the bf16 shadow is
-        refreshed from them."""
+        weights or fp32 inference the fp32 buffer takes the values exactly (fp16 / bf16 checkpoints are widened) and the
+        bf16 shadow or the split copy is refreshed from them."""
         for flat, hf, segs in self._hf_map():
-            src = sd[hf].to(torch.float32 if self.master else torch.bfloat16)
+            src = sd[hf].to(torch.float32 if self.master or self.fp32 else torch.bfloat16)
             dst = self._flat_rows(flat, grads)
             if src.dim() == 1:
                 src = src.view(-1, 1)
@@ -565,13 +596,16 @@ class B200UnitLM:
 
     # ---- checkpoints (HF layout, SURVEY.md §5 / §8 f-4) ------------------------------------------------------------
     def save_pretrained(self, save_directory: str, base_model_name: Optional[str] = None) -> None:
-        """With master weights the checkpoint holds the fp32 masters and says `torch_dtype: float32`."""
+        """With master weights or fp32 inference the checkpoint holds the fp32 values and says `torch_dtype: float32`."""
         write_unit_lm_checkpoint(save_directory, self.state_dict_hf(), self.config, base_model_name,
-                                 torch_dtype="float32" if self.master else "bfloat16")
+                                 torch_dtype="float32" if self.master or self.fp32 else "bfloat16")
 
     @classmethod
     def from_pretrained(cls, directory: str, device: str = "cuda:0", max_batch: int = 8, max_seq: int = 1024,
                         trainable: bool = True, master_weights: bool = False) -> "B200UnitLM":
+        """An OPT checkpoint whose config says `torch_dtype: float32`, loaded for inference (`trainable=False`, no
+        `master_weights`), runs in fp32 (`fp32_inference`): the checkpoint's dtype decides the precision, as for the
+        reference's `UnitLM`.  Every other checkpoint runs in bf16."""
         import json
         import os
         from safetensors.torch import load_file
@@ -592,7 +626,8 @@ class B200UnitLM:
                 b.update(dropout=0.0, attention_dropout=0.0, layerdrop=0.0)
             lm_cfg = OptLMConfig.from_hf(OPTConfig(**b), vocab_size=cfg["vocab_size"])
             m = cls(lm_cfg, device=device, max_batch=max_batch, max_seq=max_seq, trainable=trainable,
-                    master_weights=master_weights)
+                    master_weights=master_weights,
+                    fp32_inference=checkpoint_is_fp32(cfg) and not trainable and not master_weights)
             m.load_hf_state_dict(load_file(os.path.join(directory, "model.safetensors")))
             return m
         theta = (b.get("rope_parameters") or {}).get("rope_theta", b.get("rope_theta", 10000.0))
@@ -617,12 +652,17 @@ class B200UnitLM:
             pos = position_ids.to(self.device, non_blocking=True).to(torch.int32).contiguous().view(-1)
         return B, T, ids, pos
 
+    def _logits_ptr(self) -> int:
+        return self.lib.sk_lm_logits_f32(self._h) if self.fp32 else self.lib.sk_lm_logits(self._h)
+
     def logits_view(self, B: int, T: int) -> torch.Tensor:
-        """Zero-copy view of the bf16 logits of the last forward: [B, T, vocab_size]."""
-        p = self.lib.sk_lm_logits(self._h)
+        """Zero-copy view of the logits of the last forward: [B, T, vocab_size], bf16 (fp32 with fp32 inference)."""
+        p = self._logits_ptr()
         ld = self.lib.sk_lm_logits_ld(self._h)
         off = p - self.workspace.data_ptr()
-        flat = self.workspace[off:off + B * T * ld * 2].view(torch.bfloat16).view(B, T, ld)
+        dt = torch.float32 if self.fp32 else torch.bfloat16
+        es = 4 if self.fp32 else 2
+        flat = self.workspace[off:off + B * T * ld * es].view(dt).view(B, T, ld)
         return flat[:, :, :self.config.vocab_size]
 
     def forward(self, input_ids: torch.Tensor, attention_mask: Optional[torch.Tensor] = None,
@@ -692,11 +732,12 @@ class B200UnitLM:
     def sequence_log_likelihood(self, tokens: torch.Tensor, mean_nll: bool, ignore_tokens=None,
                                 attention_mask: Optional[torch.Tensor] = None,
                                 return_token_nll: bool = False):
-        """`UnitLM.log_likelihood` of the bf16 reference model (slamkit/model/unit_lm.py:184-194): bf16 [B] per-sequence
-        (mean or summed) log-likelihood on the device, with the reference's bf16 rounding of each token's log-prob, of the
-        sum and of the mean (the metric's 0.5 tie rule sees those roundings).  One forward pass, then `sk_seq_loglik` reads
-        the bf16 logits once; no fp32 copy of the logits is made.  Targets equal to the model's pad id are masked;
-        `ignore_tokens` are -inf columns.  With `return_token_nll`, also returns the fp32 [B, T-1] per-token values."""
+        """`UnitLM.log_likelihood` of the reference model (slamkit/model/unit_lm.py:184-194): [B] per-sequence (mean or
+        summed) log-likelihood on the device.  A bf16 model gives bf16 scores with the reference's bf16 rounding of each
+        token's log-prob, of the sum and of the mean (the metric's 0.5 tie rule sees those roundings); an fp32 inference
+        model gives fp32 scores with no rounding, as calc_nll on fp32 logits.  One forward pass, then `sk_seq_loglik` /
+        `sk_seq_loglik_f32` reads the logits once.  Targets equal to the model's pad id are masked; `ignore_tokens` are
+        -inf columns.  With `return_token_nll`, also returns the fp32 [B, T-1] per-token values."""
         check_right_padded(attention_mask)
         if tokens.dim() != 2:
             raise ValueError("tokens must be [batch, seq]")
@@ -705,22 +746,23 @@ class B200UnitLM:
             raise ValueError(f"sequence_log_likelihood: a row of {T} tokens is longer than max_positions = "
                              f"{self.config.max_positions} (rows are not truncated)")
         if B == 0:
-            ll = torch.empty((0,), device=self.device, dtype=torch.bfloat16)
+            ll = torch.empty((0,), device=self.device, dtype=torch.float32 if self.fp32 else torch.bfloat16)
             return (ll, torch.empty((0, max(T - 1, 0)), device=self.device)) if return_token_nll else ll
         ids = tokens.to(self.device, dtype=torch.int64).contiguous()
         self.forward(ids)
         return self.score_last_forward(ids, mean_nll, ignore_tokens, return_token_nll)
 
     def score_last_forward(self, ids: torch.Tensor, mean_nll: bool, ignore_tokens=None, return_token_nll: bool = False):
-        """The scoring half of `sequence_log_likelihood`: `sk_seq_loglik` on the logits of the last `forward(ids)`
-        (ids: device int64 [B, T], B >= 1)."""
+        """The scoring half of `sequence_log_likelihood`: `sk_seq_loglik` (`sk_seq_loglik_f32` with fp32 inference) on the
+        logits of the last `forward(ids)` (ids: device int64 [B, T], B >= 1)."""
         B, T = ids.shape
-        ll = torch.empty((B,), device=self.device, dtype=torch.bfloat16)
+        ll = torch.empty((B,), device=self.device, dtype=torch.float32 if self.fp32 else torch.bfloat16)
         token_nll = torch.empty((B * max(T - 1, 1),), device=self.device, dtype=torch.float32)
         ban = self._ban_bits(ignore_tokens)
-        L.check(self.lib.sk_seq_loglik(C.c_void_p(self.lib.sk_lm_logits(self._h)), self.lib.sk_lm_logits_ld(self._h),
-                                       self.config.vocab_size, L.ptr(ids), B, T, int(self.config.pad_token_id), L.ptr(ban),
-                                       int(bool(mean_nll)), L.ptr(token_nll), L.ptr(ll), L.stream_ptr()))
+        fn = self.lib.sk_seq_loglik_f32 if self.fp32 else self.lib.sk_seq_loglik
+        L.check(fn(C.c_void_p(self._logits_ptr()), self.lib.sk_lm_logits_ld(self._h), self.config.vocab_size, L.ptr(ids), B,
+                   T, int(self.config.pad_token_id), L.ptr(ban), int(bool(mean_nll)), L.ptr(token_nll), L.ptr(ll),
+                   L.stream_ptr()))
         return (ll, token_nll[:B * (T - 1)].view(B, T - 1)) if return_token_nll else ll
 
     @torch.inference_mode()
@@ -866,7 +908,7 @@ class DecodeSession:
         self.ldl = model.vocab_padded
         self.kv = torch.empty(int(lib.sk_lm_kv_cache_bytes(h, B, T_cache)), device=dev, dtype=torch.uint8)
         self.ws = torch.empty(int(lib.sk_lm_decode_workspace_bytes(h, B, T_cache)), device=dev, dtype=torch.uint8)
-        self.logits_buf = torch.empty(B, self.ldl, device=dev, dtype=torch.bfloat16)
+        self.logits_buf = torch.empty(B, self.ldl, device=dev, dtype=torch.float32 if model.fp32 else torch.bfloat16)
         self.tokens = torch.zeros(B, device=dev, dtype=torch.long)
         self.pos = torch.zeros(B, device=dev, dtype=torch.int32)
         self.finished = torch.zeros(B, device=dev, dtype=torch.int32)
@@ -878,7 +920,7 @@ class DecodeSession:
 
     @property
     def logits(self) -> torch.Tensor:
-        """[B, vocab_size] bf16 logits of the last prefill / decode step."""
+        """[B, vocab_size] logits of the last prefill / decode step (bf16; fp32 with fp32 inference)."""
         return self.logits_buf[:, :self.m.config.vocab_size]
 
     def prefill(self, ids: torch.Tensor, lens: torch.Tensor) -> torch.Tensor:
@@ -908,8 +950,9 @@ class DecodeSession:
 
     def select(self, cfg: "L.SkSampling", ban: Optional[torch.Tensor] = None, uniforms: Optional[torch.Tensor] = None) -> None:
         m = self.m
-        L.check(m.lib.sk_select_next(L.ptr(self.logits_buf), self.ldl, m.config.vocab_size, self.B, L.ptr(ban),
-                                     C.byref(cfg), L.ptr(uniforms), C.byref(self.state), L.stream_ptr()))
+        fn = m.lib.sk_select_next_f32 if m.fp32 else m.lib.sk_select_next
+        L.check(fn(L.ptr(self.logits_buf), self.ldl, m.config.vocab_size, self.B, L.ptr(ban), C.byref(cfg), L.ptr(uniforms),
+                   C.byref(self.state), L.stream_ptr()))
 
 
 class B200AdamW:

@@ -2,8 +2,9 @@
 SALMon.  Each metric is a list of (positive, negative) clip pairs; a pair scores 1 when the model gives the positive clip
 the higher log-likelihood, 0.5 on a tie and 0 otherwise (also when a score is NaN), and the metric is the mean.
 
-Scores are the bf16 values of `B200SpeechLM.log_likelihood`, as the bf16 reference model returns them, so ties happen
-where the reference has them.  Batching follows the reference exactly: `batch_size` positives form one batch and the
+Scores are the values of `B200SpeechLM.log_likelihood` in the model's own precision, as the reference model returns them:
+bf16 for a bf16 checkpoint, fp32 for a float32 OPT checkpoint (fp32 inference), so ties happen where the reference has
+them.  Batching follows the reference exactly: `batch_size` positives form one batch and the
 same pairs' negatives another, each zero-padded to its own longest clip, in dataset order.  HuBERT sees the padding
 (no attention mask, GroupNorm over time), so the batch composition is part of what decides a clip's units."""
 from __future__ import annotations
@@ -85,9 +86,9 @@ def score_pairs(pos: torch.Tensor, neg: torch.Tensor) -> torch.Tensor:
 
 def pair_scores(model, dataset, used_token_modality: Optional[str], mean_nll: bool = True, batch_size: int = 1,
                 num_workers: int = 8, pin_memory: bool = True) -> torch.Tensor:
-    """Per-pair results (the dtype of the scores, bf16) in dataset order.  Audio is decoded by `num_workers` threads
-    ahead of the GPU into pinned buffers (cli/extract_features.BatchPrefetcher; it always pins, so `pin_memory` is
-    accepted for the reference's signature only)."""
+    """Per-pair results (the dtype of the scores: bf16, or fp32 for an fp32 inference model) in dataset order.  Audio
+    is decoded by `num_workers` threads ahead of the GPU into pinned buffers (cli/extract_features.BatchPrefetcher; it
+    always pins, so `pin_memory` is accepted for the reference's signature only)."""
     from cli.extract_features import BatchPrefetcher
     n = len(dataset)
     batches = []

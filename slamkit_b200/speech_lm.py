@@ -29,7 +29,8 @@ class B200SpeechLM:
     @torch.inference_mode()
     def log_likelihood(self, wavs: torch.Tensor, lens: Optional[torch.Tensor] = None, mean_nll: bool = True,
                        used_token_modality: Optional[str] = None) -> torch.Tensor:
-        """speech_lm.py:22-36: bf16 [B] log-likelihood of each zero-padded clip (mean over tokens with `mean_nll`)."""
+        """speech_lm.py:22-36: [B] log-likelihood of each zero-padded clip (mean over tokens with `mean_nll`), in the model's
+        precision (bf16, or fp32 for an fp32 inference model)."""
         ids, mask = self.tokenise(wavs, lens)
         ignore = self.tokeniser.get_ignore_tokens(used_token_modality)
         return self.model.sequence_log_likelihood(ids, mean_nll, ignore, attention_mask=mask)
