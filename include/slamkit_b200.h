@@ -295,7 +295,16 @@ int sk_lm_create(const SkLmConfig* cfg, SkLm** out);
  *   - positions (row % T, pos_ids, or the decode step's pos[b]) select table row position + 2, clamped to the table;
  *   - the gradient-norm groups are OPTForCausalLM's parameters: q, k, v, out_proj, fc1, fc2 weights and biases and the
  *     LayerNorm weights and biases each count as one tensor;
- *   - the KV cache holds n_heads K/V heads per layer (same layout as above with n_kv_heads = n_heads). */
+ *   - the KV cache holds n_heads K/V heads per layer (same layout as above with n_kv_heads = n_heads).
+ * post_ln = 1 selects the post-LayerNorm OPT (do_layer_norm_before = False, e.g. facebook/opt-350m), optionally with the
+ * bias-free project_in / project_out pair (proj_dim = word_embed_proj_dim, 0 or hidden: none):
+ *   e = embed_tokens[id] [proj_dim];  x0 = bf16(bf16(e W_in^T) + embed_positions[pos + 2]);  per layer
+ *   s1 = bf16(bf16(attn(x) W_o + b_o) + x), y1 = LN1(s1);  s2 = bf16(bf16(relu(y1 W_1 + b_1) W_2 + b_2) + y1), x' = LN2(s2);
+ *   h = bf16(x_L W_out^T);  logits = h E^T (tied: K = proj_dim).  There is no decoder-level final LayerNorm.
+ * Its flat layout has embed [Vpad, proj_dim], proj_in [hidden, proj_dim] and proj_out [proj_dim, hidden] (when
+ * projecting) and no final_norm / final_norm_b; its gradient-norm groups add project_out and project_in.  It trains in
+ * bf16 and runs fp32 inference (sk_lm_set_fp32); sk_lm_set_master refuses it.  Zero in both fields (what an 8-field
+ * initialiser leaves) is the pre-LayerNorm decoder above; pre-LN with proj_dim != hidden is refused. */
 typedef struct SkOptConfig {
   int32_t vocab_size;        /* 502 for unit_hubert_25 */
   int32_t hidden;            /* 768 for opt-125m; n_heads * 64, <= 2048 */
@@ -305,6 +314,8 @@ typedef struct SkOptConfig {
   int32_t max_positions;     /* max_position_embeddings (2048): the position table has max_positions + 2 rows */
   float ln_eps;              /* 1e-5 */
   int32_t tie_embeddings;    /* 1: lm_head shares the token embedding table */
+  int32_t post_ln;           /* 0: pre-LayerNorm (opt-125m); 1: post-LayerNorm (opt-350m) */
+  int32_t proj_dim;          /* word_embed_proj_dim: 0 or hidden = no projections; else a multiple of 64, < hidden */
 } SkOptConfig;
 int sk_lm_create_opt(const SkOptConfig* cfg, SkLm** out);
 /* GPT-NeoX decoder with the parallel residual (HF GPTNeoXForCausalLM, use_parallel_residual = True, e.g. the Pythia

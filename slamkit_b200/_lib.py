@@ -48,6 +48,8 @@ class SkOptConfig(C.Structure):
         ("max_positions", C.c_int32),
         ("ln_eps", C.c_float),
         ("tie_embeddings", C.c_int32),
+        ("post_ln", C.c_int32),
+        ("proj_dim", C.c_int32),
     ]
 
 

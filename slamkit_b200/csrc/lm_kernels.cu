@@ -1176,10 +1176,14 @@ __global__ void opt_embed_fwd_kernel(const int64_t* __restrict__ ids, const int3
   for (long i = blockIdx.x * (long)blockDim.x + threadIdx.x; i < total; i += (long)gridDim.x * blockDim.x) {
     const int m = (int)(i / vec_per_row);
     const int c = (int)(i % vec_per_row);
-    long id = ids[m];
-    if (id < 0 || id >= V) id = 0;
     const int pr = opt_pos_row(pos_ids, m, T, n_pos);
-    const uint4 a = ldg128(E + (size_t)id * D + c * 8), b = ldg128(P + (size_t)pr * D + c * 8);
+    uint4 a = make_uint4(0u, 0u, 0u, 0u);   // E == nullptr: the position rows alone (post-LN OPT with project_in)
+    if (E) {
+      long id = ids[m];
+      if (id < 0 || id >= V) id = 0;
+      a = ldg128(E + (size_t)id * D + c * 8);
+    }
+    const uint4 b = ldg128(P + (size_t)pr * D + c * 8);
     const uint32_t au[4] = {a.x, a.y, a.z, a.w}, bu[4] = {b.x, b.y, b.z, b.w};
     uint32_t o[4];
 #pragma unroll
@@ -1370,10 +1374,15 @@ __global__ void opt_embed_fwd_f32_kernel(const int64_t* __restrict__ ids, const 
   for (long i = blockIdx.x * (long)blockDim.x + threadIdx.x; i < total; i += (long)gridDim.x * blockDim.x) {
     const int m = (int)(i / vec_per_row);
     const int c = (int)(i % vec_per_row);
-    long id = ids[m];
-    if (id < 0 || id >= V) id = 0;
-    const int pr = opt_pos_row(pos_ids, m, T, n_pos);
-    const float4 a = ldg4(E + (size_t)id * D + c * 4), b = ldg4(P + (size_t)pr * D + c * 4);
+    // E == nullptr: the position rows alone; P == nullptr: the token rows alone (post-LN OPT with project_in, whose
+    // token rows are proj_dim wide)
+    float4 a = make_float4(0.f, 0.f, 0.f, 0.f), b = a;
+    if (E) {
+      long id = ids[m];
+      if (id < 0 || id >= V) id = 0;
+      a = ldg4(E + (size_t)id * D + c * 4);
+    }
+    if (P) b = ldg4(P + (size_t)opt_pos_row(pos_ids, m, T, n_pos) * D + c * 4);
     *reinterpret_cast<float4*>(out + (size_t)m * D + c * 4) = make_float4(a.x + b.x, a.y + b.y, a.z + b.z, a.w + b.w);
   }
 }

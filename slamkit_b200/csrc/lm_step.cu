@@ -40,6 +40,7 @@ struct WsLayout {
   int64_t hf, rstdf, logits, dlogits, dxA, dxB, dh, dao, dqkv, dgu, delta;
   int64_t dw_partial, colsum_partial, ce_partial, embed_scratch, splitk, splitk_bytes, seg_start, seg_end, total;
   int64_t sR = 0, dres32 = 0;   // OPT: residual-stream slab stride (X, xmid); fp32 residual gradient (master weights)
+  int64_t pe = 0;               // post-LN OPT with projections: the token rows e [M, proj_dim] that project_in reads
 };
 }  // namespace
 
@@ -54,6 +55,11 @@ struct SkLm {
   int rot = 64;                   // GPT-NeoX: rotated columns per q / k head (rotary_ndims)
   int64_t off_final_norm_b = 0, off_pos = 0;
   int n_pos = 0;                  // OPT: rows of the learned position table (max_positions + 2)
+  // post-LayerNorm OPT (opt-350m): no final LayerNorm; with `proj`, the token table and the tied head are pw = proj_dim
+  // wide and proj_in [d, pw] / proj_out [pw, d] map between them and the residual stream.  pw = d otherwise.
+  bool post_ln = false, proj = false;
+  int pw = 0;
+  int64_t off_pin = 0, off_pout = 0;
   int64_t off_final_norm = 0, off_embed = 0, off_head = 0, n_params = 0;
   bf16* params = nullptr;
   bf16* grads = nullptr;
@@ -164,6 +170,15 @@ T* wsp(const SkLm* lm, int64_t off) {
     if (_rc) return _rc;    \
   } while (0)
 
+// width of the lm_head's input: proj_dim for a post-LN OPT with project_out, else hidden
+int head_k(const SkLm* lm) { return lm->proj ? lm->pw : lm->d; }
+// the lm_head's input rows [M, head_k]: the final LayerNorm's output, or for post-LN OPT (no final LayerNorm) the last
+// layer's output or its project_out image
+bf16* head_in(const SkLm* lm, const WsLayout& w) {
+  if (lm->post_ln && !lm->proj) return wsp<bf16>(lm, w.X + w.sX * lm->L);
+  return wsp<bf16>(lm, w.hf);
+}
+
 // y[M,N] = x[M,K] * W[N,K]^T (+bias) (+residual)
 // (forward and dgrad GEMMs get no scratch: whole-tile scheduling keeps every output row's fp32 summation order
 //  independent of the batch it sits in -- logits of a sequence are bit-identical alone or inside a batch)
@@ -259,13 +274,14 @@ int forward_impl(SkLm* lm, const int64_t* ids, const int64_t* labels, const int3
 // of logits traffic it removes.)  The sums per row meet in `ce_partial`, finalised once.
 int head_chunked(SkLm* lm, const int64_t* labels, int B, int T, float num_items, float dloss, int accumulate, float* stats,
                  const WsLayout& w, cudaStream_t s) {
-  const int M = B * T, d = lm->d;
+  const int M = B * T, d = head_k(lm);
   SK_REQUIRE(num_items > 0.f, "sk_lm: training with a large vocabulary needs num_items_in_batch (the 'sum / num_items' loss of "
                               "slamkit/model/unit_lm.py:26-28): the gradient scale must be known before the first chunk");
   const bf16* P = lm->params;
   bf16* G = lm->grads;
-  bf16* hf = wsp<bf16>(lm, w.hf);
-  bf16* dh = wsp<bf16>(lm, w.dh);
+  bf16* hf = head_in(lm, w);
+  // post-LN OPT without projections: the head's input gradient is the residual-stream gradient that the layers read
+  bf16* dh = wsp<bf16>(lm, lm->post_ln && !lm->proj ? w.dxA : w.dh);
   bf16* chunk = wsp<bf16>(lm, w.logits);
   float* partial = wsp<float>(lm, w.ce_partial);
   const float gs = dloss / num_items;
@@ -448,6 +464,7 @@ WsLayout make_opt_layout(const SkLm* lm, int B, int T) {
   w.seg_start = take(M * 4);
   w.seg_end = take(M * 4);
   if (lm->master) w.dres32 = take(w.sR);
+  if (lm->proj) w.pe = take(M * lm->pw * 2);
   w.total = cur;
   return w;
 }
@@ -850,9 +867,163 @@ int opt_backward_master(SkLm* lm, const int64_t* ids, const int32_t* pos_ids, in
   return sk_widen_grads_launch(G, G32, lm->d_widen_start, lm->d_widen_len, lm->n_widen, accumulate, s);
 }
 
+// ---- post-LayerNorm OPT (HF OPTDecoderLayer with do_layer_norm_before = False, and OPTDecoder's bias-free
+// project_in / project_out; facebook/opt-350m).  No new per-layer memory: X[l] holds the layer input, xmid
+// s1 = bf16(bf16(attn W_o + b_o) + x), h1 y1 = LN1(s1), h2 s2 = bf16(bf16(relu(y1 W_1 + b_1) W_2 + b_2) + y1),
+// X[l+1] = LN2(s2); rstd1 / rstd2 the two LayerNorms' mean / rstd, gu relu(fc1).  With projections, `pe` holds the token
+// rows e [M, proj_dim] and hf the head input h = bf16(x_L W_out^T) [M, proj_dim].
+int opt_postln_forward(SkLm* lm, const int64_t* ids, const int64_t* labels, const int32_t* pos_ids, int B, int T,
+                       float num_items, float dloss, bool want_dlogits, float* stats, const WsLayout& w, cudaStream_t s,
+                       float* row_nll, bool with_head) {
+  const int M = B * T, d = lm->d, F = lm->F, L = lm->L, Q = lm->qkv_dim, K = head_k(lm);
+  const float eps = lm->cfg.rms_eps;
+  const bf16* P = lm->params;
+  bf16* X0 = wsp<bf16>(lm, w.X);
+  if (lm->proj) {
+    // x0 = bf16(bf16(e W_in^T) + pos[p + 2]): the position rows, gathered into dxB (unused until the backward pass), are
+    // the GEMM's residual, added after the projection is rounded
+    bf16* e = wsp<bf16>(lm, w.pe);
+    bf16* prow = wsp<bf16>(lm, w.dxB);
+    SK_TRY(sk_embed_fwd_launch(ids, P + lm->off_embed, e, M, K, lm->V, s));
+    SK_TRY(sk_opt_embed_fwd_launch(ids, pos_ids, nullptr, P + lm->off_pos, prow, M, T, d, lm->V, lm->n_pos, s));
+    SK_TRY(linear_fwd(M, d, K, e, P + lm->off_pin, X0, nullptr, prow, s));
+  } else {
+    SK_TRY(sk_opt_embed_fwd_launch(ids, pos_ids, P + lm->off_embed, P + lm->off_pos, X0, M, T, d, lm->V, lm->n_pos, s));
+  }
+  const float scale = 1.0f / sqrtf((float)lm->hd);
+  const int* seg_start = nullptr;
+  if (pos_ids) {
+    SK_TRY(sk_seg_bounds_launch(pos_ids, wsp<int32_t>(lm, w.seg_start), wsp<int32_t>(lm, w.seg_end), B, T, s));
+    seg_start = wsp<int32_t>(lm, w.seg_start);
+  }
+  for (int l = 0; l < L; ++l) {
+    const OptLayerOff& o = lm->olo[l];
+    bf16* x = wsp<bf16>(lm, w.X + w.sX * l);
+    bf16* xn = wsp<bf16>(lm, w.X + w.sX * (l + 1));
+    bf16* y1 = wsp<bf16>(lm, w.h1 + w.sh * l);
+    float* st1 = wsp<float>(lm, w.rstd1 + w.srstd * l);
+    bf16* qkv = wsp<bf16>(lm, w.qkv + w.sqkv * l);
+    bf16* ao = wsp<bf16>(lm, w.ao + w.sX * l);
+    float* lse = wsp<float>(lm, w.lse + w.slse * l);
+    bf16* s1 = wsp<bf16>(lm, w.xmid + w.sX * l);
+    bf16* s2 = wsp<bf16>(lm, w.h2 + w.sh * l);
+    float* st2 = wsp<float>(lm, w.rstd2 + w.srstd * l);
+    bf16* a = wsp<bf16>(lm, w.gu + w.sgu * l);
+
+    SK_TRY(linear_fwd(M, Q, d, x, P + o.wqkv, qkv, P + o.bqkv, nullptr, s));
+    SK_TRY(sk_attn_tc_fwd_launch(qkv, ao, lse, B, T, lm->H, lm->H, Q, d, 1, scale, s, seg_start));
+    SK_TRY(linear_fwd(M, d, d, ao, P + o.wo, s1, P + o.bo, x, s));
+    SK_TRY(sk_layernorm_fwd_launch(s1, P + o.ln1w, P + o.ln1b, y1, st1, st1 + M, M, d, eps, s));
+    SK_TRY(sk_gemm_launch(M, F, d, y1, d, 0, P + o.w1, d, 0, a, F, 0, P + o.b1, nullptr, 0, 0, 2, 0, s));   // relu(fc1)
+    SK_TRY(linear_fwd(M, d, F, a, P + o.w2, s2, P + o.b2, y1, s));
+    SK_TRY(sk_layernorm_fwd_launch(s2, P + o.ln2w, P + o.ln2b, xn, st2, st2 + M, M, d, eps, s));
+  }
+  if (lm->proj)
+    SK_TRY(linear_fwd(M, K, d, wsp<bf16>(lm, w.X + w.sX * L), P + lm->off_pout, wsp<bf16>(lm, w.hf), nullptr, nullptr, s));
+  lm->last_B = B;
+  lm->last_T = T;
+  if (!with_head) return 0;
+  bf16* logits = wsp<bf16>(lm, w.logits);
+  SK_TRY(linear_fwd(M, lm->Vp, K, head_in(lm, w), P + lm->off_head, logits, nullptr, nullptr, s));
+  if (labels) {
+    SK_TRY(sk_ce_launch(logits, labels, want_dlogits ? wsp<bf16>(lm, w.dlogits) : nullptr, wsp<float>(lm, w.ce_partial),
+                        row_nll, stats, M, T, lm->V, lm->Vp, num_items, dloss, s));
+  }
+  return 0;
+}
+
+// The residual stream is the LayerNorm output, so each LayerNorm backward reads the sum of its output's two gradients:
+// the fc1 and q|k|v dgrad GEMMs add the skip path's gradient in their epilogue, bf16(ds + bf16(dgrad)) as autograd
+// rounds it.  Every reduction is the deterministic one of the pre-LN path.
+int opt_postln_backward(SkLm* lm, const int64_t* ids, const int32_t* pos_ids, int B, int T, int accumulate, const WsLayout& w,
+                        cudaStream_t s, bool with_head) {
+  const int M = B * T, d = lm->d, F = lm->F, L = lm->L, Q = lm->qkv_dim, K = head_k(lm);
+  const bf16* P = lm->params;
+  bf16* G = lm->grads;
+  float* dwp = wsp<float>(lm, w.dw_partial);
+  float* dbp = dwp + (size_t)sk_layernorm_bwd_blocks() * d;
+  float* csp = wsp<float>(lm, w.colsum_partial);
+  bf16* dxA = wsp<bf16>(lm, w.dxA);
+  bf16* dxB = wsp<bf16>(lm, w.dxB);
+  bf16* dh = wsp<bf16>(lm, w.dh);   // [M, proj_dim]: the gradient of h, later of e
+  bf16* dao = wsp<bf16>(lm, w.dao);
+  bf16* dqkv = wsp<bf16>(lm, w.dqkv);
+  bf16* da = wsp<bf16>(lm, w.dgu);
+  bf16* xL = wsp<bf16>(lm, w.X + w.sX * L);
+  void* sws = lm->ws + w.splitk;
+  const size_t swb = (size_t)w.splitk_bytes;
+  const float scale = 1.0f / sqrtf((float)lm->hd);
+  const int* seg_start = pos_ids ? wsp<int32_t>(lm, w.seg_start) : nullptr;
+  const int* seg_end = pos_ids ? wsp<int32_t>(lm, w.seg_end) : nullptr;
+
+  if (with_head) {   // tied head at K = proj_dim (already done chunk by chunk for large vocabularies)
+    bf16* dlogits = wsp<bf16>(lm, w.dlogits);
+    SK_TRY(linear_dgrad(M, lm->Vp, K, dlogits, P + lm->off_head, lm->proj ? dh : dxA, s));
+    SK_TRY(linear_wgrad(M, lm->Vp, K, dlogits, head_in(lm, w), G + lm->off_head, accumulate, s, sws, swb));
+  }
+  if (lm->proj) {
+    SK_TRY(linear_dgrad(M, K, d, dh, P + lm->off_pout, dxA, s));
+    SK_TRY(linear_wgrad(M, K, d, dh, xL, G + lm->off_pout, accumulate, s, sws, swb));
+  }
+  if (!lm->bwd_events.empty()) SK_CUDA_CHECK(cudaEventRecord(lm->bwd_events[L], s));
+  for (int l = L - 1; l >= 0; --l) {   // dxA: the gradient of the layer's output LN2(s2)
+    const OptLayerOff& o = lm->olo[l];
+    const bf16* x = wsp<bf16>(lm, w.X + w.sX * l);
+    const bf16* y1 = wsp<bf16>(lm, w.h1 + w.sh * l);
+    const float* st1 = wsp<float>(lm, w.rstd1 + w.srstd * l);
+    const bf16* qkv = wsp<bf16>(lm, w.qkv + w.sqkv * l);
+    const bf16* ao = wsp<bf16>(lm, w.ao + w.sX * l);
+    const float* lse = wsp<float>(lm, w.lse + w.slse * l);
+    const bf16* s1 = wsp<bf16>(lm, w.xmid + w.sX * l);
+    const bf16* s2 = wsp<bf16>(lm, w.h2 + w.sh * l);
+    const float* st2 = wsp<float>(lm, w.rstd2 + w.srstd * l);
+    const bf16* a = wsp<bf16>(lm, w.gu + w.sgu * l);
+
+    // LN2 backward from s2: ds2 -> dxB
+    SK_TRY(sk_layernorm_bwd_launch(dxA, s2, P + o.ln2w, st2, st2 + M, nullptr, dxB, G + o.ln2w, G + o.ln2b, dwp, dbp, M, d,
+                                   accumulate, s));
+    // MLP: dy = ds2; ReLU backward masked by the saved a = relu(fc1) > 0
+    SK_TRY(linear_dgrad(M, d, F, dxB, P + o.w2, da, s));
+    SK_TRY(sk_relu_bwd_launch(da, a, (long)M * F, s));
+    SK_TRY(linear_wgrad(M, d, F, dxB, a, G + o.w2, accumulate, s, sws, swb));
+    SK_TRY(sk_colsum_launch(dxB, G + o.b2, csp, M, d, d, accumulate, s));
+    // dy1 = bf16(ds2 + bf16(da W_1)) -> dxA: fc1's dgrad with the skip path's gradient as its residual
+    SK_TRY(sk_gemm_launch(M, d, F, da, F, 0, P + o.w1, d, 1, dxA, d, 0, nullptr, dxB, d, 1, 0, 0, s));
+    SK_TRY(linear_wgrad(M, F, d, da, y1, G + o.w1, accumulate, s, sws, swb));
+    SK_TRY(sk_colsum_launch(da, G + o.b1, csp, M, F, F, accumulate, s));
+    // LN1 backward from s1: ds1 -> dxB
+    SK_TRY(sk_layernorm_bwd_launch(dxA, s1, P + o.ln1w, st1, st1 + M, nullptr, dxB, G + o.ln1w, G + o.ln1b, dwp, dbp, M, d,
+                                   accumulate, s));
+    // attention: dy = ds1
+    SK_TRY(linear_dgrad(M, d, d, dxB, P + o.wo, dao, s));
+    SK_TRY(linear_wgrad(M, d, d, dxB, ao, G + o.wo, accumulate, s, sws, swb));
+    SK_TRY(sk_colsum_launch(dxB, G + o.bo, csp, M, d, d, accumulate, s));
+    SK_TRY(sk_attn_tc_bwd_launch(qkv, ao, dao, lse, wsp<float>(lm, w.delta), nullptr, dqkv, B, T, lm->H, lm->H, Q, d, Q, 1,
+                                 scale, s, seg_start, seg_end));
+    SK_TRY(sk_colsum_launch(dqkv, G + o.bqkv, csp, M, Q, Q, accumulate, s));
+    // dx = bf16(ds1 + bf16(dqkv W_qkv)) -> dxA
+    SK_TRY(sk_gemm_launch(M, d, Q, dqkv, Q, 0, P + o.wqkv, d, 1, dxA, d, 0, nullptr, dxB, d, 1, 0, 0, s));
+    SK_TRY(linear_wgrad(M, Q, d, dqkv, x, G + o.wqkv, accumulate, s, sws, swb));
+    if (!lm->bwd_events.empty()) SK_CUDA_CHECK(cudaEventRecord(lm->bwd_events[l], s));
+  }
+  // dxA = the gradient of x0: the position table, then project_in, then the (tied) token table
+  float* scratch = wsp<float>(lm, w.embed_scratch);
+  SK_TRY(sk_opt_pos_bwd_launch(pos_ids, dxA, scratch, G + lm->off_pos, M, T, d, lm->n_pos, accumulate, s));
+  const bf16* de = dxA;
+  if (lm->proj) {
+    SK_TRY(linear_wgrad(M, d, K, dxA, wsp<bf16>(lm, w.pe), G + lm->off_pin, accumulate, s, sws, swb));
+    SK_TRY(linear_dgrad(M, d, K, dxA, P + lm->off_pin, dh, s));
+    de = dh;
+  }
+  return sk_embed_bwd_launch(ids, de, scratch, G + lm->off_embed, M, K, lm->V, lm->Vp, lm->cfg.tie_embeddings ? 1 : accumulate,
+                             s);
+}
+
 int opt_forward(SkLm* lm, const int64_t* ids, const int64_t* labels, const int32_t* pos_ids, int B, int T, float num_items,
                 float dloss, bool want_dlogits, float* stats, const WsLayout& w, cudaStream_t s, float* row_nll = nullptr,
                 bool with_head = true) {
+  if (lm->post_ln)
+    return opt_postln_forward(lm, ids, labels, pos_ids, B, T, num_items, dloss, want_dlogits, stats, w, s, row_nll, with_head);
   if (lm->master)
     return opt_forward_master(lm, ids, labels, pos_ids, B, T, num_items, dloss, want_dlogits, stats, w, s, row_nll, with_head);
   const int M = B * T, d = lm->d, F = lm->F, L = lm->L, Q = lm->qkv_dim;
@@ -910,6 +1081,7 @@ int opt_forward(SkLm* lm, const int64_t* ids, const int64_t* labels, const int32
 int opt_backward(SkLm* lm, const int64_t* ids, const int32_t* pos_ids, int B, int T, int accumulate, const WsLayout& w,
                  cudaStream_t s, bool with_head = true) {
   if (lm->master) return opt_backward_master(lm, ids, pos_ids, B, T, accumulate, w, s, with_head);
+  if (lm->post_ln) return opt_postln_backward(lm, ids, pos_ids, B, T, accumulate, w, s, with_head);
   const int M = B * T, d = lm->d, F = lm->F, L = lm->L, Q = lm->qkv_dim;
   const bf16* P = lm->params;
   bf16* G = lm->grads;
@@ -979,10 +1151,58 @@ int opt_backward(SkLm* lm, const int64_t* ids, const int32_t* pos_ids, int B, in
   return sk_opt_pos_bwd_launch(pos_ids, dxA, wsp<float>(lm, w.embed_scratch), G + lm->off_pos, M, T, d, lm->n_pos, accumulate, s);
 }
 
+// Post-LN decode step (the formulas of opt_postln_forward at M = B).  With projections the h slot holds e [B, proj_dim]
+// at the start and the head input bf16(x_L W_out^T) at the end; x1 the position rows, then s1 and s2.
+int opt_postln_decode_step(SkLm* lm, const int64_t* tokens, const int32_t* pos, int B, void* kv_cache, int T_cache,
+                           void* logits, int ldl, uint8_t* dws, const DecLayout& dl, cudaStream_t s) {
+  const int d = lm->d, F = lm->F, Q = lm->qkv_dim, K = head_k(lm);
+  const float eps = lm->cfg.rms_eps;
+  const bf16* P = lm->params;
+  bf16* x = reinterpret_cast<bf16*>(dws + dl.x0);
+  bf16* xm = reinterpret_cast<bf16*>(dws + dl.x1);
+  bf16* h = reinterpret_cast<bf16*>(dws + dl.h);
+  bf16* qkv = reinterpret_cast<bf16*>(dws + dl.qkv);
+  bf16* ao = reinterpret_cast<bf16*>(dws + dl.ao);
+  bf16* a = reinterpret_cast<bf16*>(dws + dl.gu);
+  int32_t* lens = reinterpret_cast<int32_t*>(dws + dl.lens);
+  float* partial = reinterpret_cast<float*>(dws + dl.partial);
+  void* gemm_ws = dws + dl.gemm;
+  const size_t plane = (size_t)B * lm->H * T_cache * lm->hd;
+  const float scale = 1.0f / sqrtf((float)lm->hd);
+  if (lm->proj) {
+    SK_TRY(sk_embed_fwd_launch(tokens, P + lm->off_embed, h, B, K, lm->V, s));
+    SK_TRY(sk_opt_embed_fwd_launch(tokens, pos, nullptr, P + lm->off_pos, xm, B, 1, d, lm->V, lm->n_pos, s));
+    SK_TRY(linear_fwd(B, d, K, h, P + lm->off_pin, x, nullptr, xm, s));
+  } else {
+    SK_TRY(sk_opt_embed_fwd_launch(tokens, pos, P + lm->off_embed, P + lm->off_pos, x, B, 1, d, lm->V, lm->n_pos, s));
+  }
+  for (int l = 0; l < lm->L; ++l) {
+    const OptLayerOff& o = lm->olo[l];
+    bf16* kc = reinterpret_cast<bf16*>(kv_cache) + (size_t)l * 2 * plane;
+    bf16* vc = kc + plane;
+    SK_TRY(linear_fwd(B, Q, d, x, P + o.wqkv, qkv, P + o.bqkv, nullptr, s));
+    SK_TRY(sk_kv_append_launch(qkv, Q, kc, vc, pos, lens, B, lm->H, lm->H, T_cache, s));
+    SK_TRY(sk_attn_decode_launch(qkv, Q, kc, vc, lens, ao, d, partial, B, lm->H, lm->H, T_cache, scale, s));
+    SK_TRY(linear_fwd(B, d, d, ao, P + o.wo, xm, P + o.bo, x, s));
+    SK_TRY(sk_layernorm_fwd_launch(xm, P + o.ln1w, P + o.ln1b, h, nullptr, nullptr, B, d, eps, s));
+    SK_TRY(sk_gemm_launch(B, F, d, h, d, 0, P + o.w1, d, 0, a, F, 0, P + o.b1, nullptr, 0, 0, 2, 0, s));
+    SK_TRY(sk_gemm_launch(B, d, F, a, F, 0, P + o.w2, F, 0, xm, d, 0, P + o.b2, h, d, 1, 0, 0, s, gemm_ws,
+                          (size_t)dl.gemm_bytes));
+    SK_TRY(sk_layernorm_fwd_launch(xm, P + o.ln2w, P + o.ln2b, x, nullptr, nullptr, B, d, eps, s));
+  }
+  const bf16* hin = x;
+  if (lm->proj) {
+    SK_TRY(linear_fwd(B, K, d, x, P + lm->off_pout, h, nullptr, nullptr, s));
+    hin = h;
+  }
+  return sk_gemm_launch(B, lm->Vp, K, hin, K, 0, P + lm->off_head, K, 0, logits, ldl, 0, nullptr, nullptr, 0, 0, 0, 0, s);
+}
+
 // One token per row at position pos[b] (read on the device: the step is graph-capturable).  The KV cache layout is the
 // Qwen2 one with KVH = H.
 int opt_decode_step(SkLm* lm, const int64_t* tokens, const int32_t* pos, int B, void* kv_cache, int T_cache, void* logits,
                     int ldl, uint8_t* dws, const DecLayout& dl, cudaStream_t s) {
+  if (lm->post_ln) return opt_postln_decode_step(lm, tokens, pos, B, kv_cache, T_cache, logits, ldl, dws, dl, s);
   const int d = lm->d, F = lm->F, Q = lm->qkv_dim;
   const float eps = lm->cfg.rms_eps;
   const bf16* P = lm->params;
@@ -1036,9 +1256,106 @@ int linear_split(const SkLm* lm, int M, int N, int K, Pair x, int64_t w_off, int
                                 res ? res->lo : nullptr, y.hi, y.lo, y32, ldy, s);
 }
 
+// Post-LN fp32 inference.  The slabs: X the layer input x, xmid s1 then s2, h1 y1 (and, with projections, e at the start
+// and the head input h = x_L W_out^T at the end); embed_scratch the fp32 rows before they are split.  The head input pair
+// is returned in *hin.
+int opt_postln_forward_fp32(SkLm* lm, const int64_t* ids, int B, int T, const WsLayout& w, cudaStream_t s, bool with_head,
+                            float* kv, const int32_t* lens, int T_cache, Pair* hin_out) {
+  const int M = B * T, d = lm->d, F = lm->F, L = lm->L, Q = lm->qkv_dim, K = head_k(lm);
+  const float eps = lm->cfg.rms_eps;
+  const float* P32 = lm->params32;
+  auto pair = [&](int64_t off, int64_t stride) { return Pair{wsp<bf16>(lm, off), wsp<bf16>(lm, off + stride)}; };
+  const Pair x = pair(w.X, w.sX), xm = pair(w.xmid, w.sX), h = pair(w.h1, w.sX), qkv = pair(w.qkv, w.sqkv),
+             ao = pair(w.ao, w.sX), a = pair(w.gu, w.sgu);
+  float* e32 = wsp<float>(lm, w.embed_scratch);
+  if (lm->proj) {   // x0 = e W_in^T + pos[p + 2], the position rows as the split GEMM's residual
+    SK_TRY(sk_opt_embed_fwd_f32_launch(ids, nullptr, nullptr, P32 + lm->off_pos, e32, M, T, d, lm->V, lm->n_pos, s));
+    SK_TRY(sk_split_f32_launch(e32, xm.hi, xm.lo, (long)M * d, s));
+    SK_TRY(sk_opt_embed_fwd_f32_launch(ids, nullptr, P32 + lm->off_embed, nullptr, e32, M, T, K, lm->V, lm->n_pos, s));
+    SK_TRY(sk_split_f32_launch(e32, h.hi, h.lo, (long)M * K, s));
+    SK_TRY(linear_split(lm, M, d, K, h, lm->off_pin, -1, 0, &xm, x, nullptr, d, s));
+  } else {
+    SK_TRY(sk_opt_embed_fwd_f32_launch(ids, nullptr, P32 + lm->off_embed, P32 + lm->off_pos, e32, M, T, d, lm->V, lm->n_pos, s));
+    SK_TRY(sk_split_f32_launch(e32, x.hi, x.lo, (long)M * d, s));
+  }
+  const float scale = 1.0f / sqrtf((float)lm->hd);
+  const size_t plane = (size_t)B * lm->H * T_cache * lm->hd;
+  for (int l = 0; l < L; ++l) {
+    const OptLayerOff& o = lm->olo[l];
+    SK_TRY(linear_split(lm, M, Q, d, x, o.wqkv, o.bqkv, 0, nullptr, qkv, nullptr, Q, s));
+    if (kv) SK_TRY(sk_kv_prefill_f32_launch(qkv.hi, qkv.lo, Q, kv + (size_t)l * 2 * plane, lens, B, T, lm->H, T_cache, s));
+    SK_TRY(sk_attn_tc_fwd_split_launch(qkv.hi, qkv.lo, ao.hi, ao.lo, B, T, lm->H, Q, d, scale, s, 1));
+    SK_TRY(linear_split(lm, M, d, d, ao, o.wo, o.bo, 0, &x, xm, nullptr, d, s));
+    SK_TRY(sk_layernorm_hilo_launch(xm.hi, xm.lo, nullptr, nullptr, P32 + o.ln1w, P32 + o.ln1b, h.hi, h.lo, nullptr, M, d, eps, s));
+    SK_TRY(linear_split(lm, M, F, d, h, o.w1, o.b1, 2, nullptr, a, nullptr, F, s));   // relu(fc1)
+    SK_TRY(linear_split(lm, M, d, F, a, o.w2, o.b2, 0, &h, xm, nullptr, d, s));
+    SK_TRY(sk_layernorm_hilo_launch(xm.hi, xm.lo, nullptr, nullptr, P32 + o.ln2w, P32 + o.ln2b, x.hi, x.lo, nullptr, M, d, eps, s));
+  }
+  Pair hin = x;
+  if (lm->proj) {
+    SK_TRY(linear_split(lm, M, K, d, x, lm->off_pout, -1, 0, nullptr, h, nullptr, K, s));
+    hin = h;
+  }
+  if (hin_out) *hin_out = hin;
+  lm->last_B = B;
+  lm->last_T = T;
+  if (!with_head) return 0;
+  return linear_split(lm, M, lm->Vp, K, hin, lm->off_head, -1, 0, nullptr, Pair{nullptr, nullptr}, wsp<float>(lm, w.logits),
+                      lm->Vp, s);
+}
+
+// Post-LN fp32 decode step: the slots of opt_decode_step_fp32, with h holding e at the start and the head input at the end
+int opt_postln_decode_step_fp32(SkLm* lm, const int64_t* tokens, const int32_t* pos, int B, float* kv, int T_cache,
+                                float* logits, int ldl, uint8_t* dws, const DecLayout& dl, cudaStream_t s) {
+  const int d = lm->d, F = lm->F, Q = lm->qkv_dim, K = head_k(lm);
+  const float eps = lm->cfg.rms_eps;
+  const float* P32 = lm->params32;
+  auto pair = [&](int64_t off, int64_t n) {
+    bf16* hi = reinterpret_cast<bf16*>(dws + off);
+    return Pair{hi, hi + n};
+  };
+  const Pair x = pair(dl.x0, (int64_t)B * d), xm = pair(dl.x1, (int64_t)B * d), h = pair(dl.h, (int64_t)B * d),
+             qkv = pair(dl.qkv, (int64_t)B * Q), ao = pair(dl.ao, (int64_t)B * d), a = pair(dl.gu, (int64_t)B * F);
+  int32_t* lens = reinterpret_cast<int32_t*>(dws + dl.lens);
+  float* partial = reinterpret_cast<float*>(dws + dl.partial);
+  float* e32 = reinterpret_cast<float*>(dws + dl.e32);
+  const size_t plane = (size_t)B * lm->H * T_cache * lm->hd;
+  const float scale = 1.0f / sqrtf((float)lm->hd);
+  if (lm->proj) {
+    SK_TRY(sk_opt_embed_fwd_f32_launch(tokens, pos, nullptr, P32 + lm->off_pos, e32, B, 1, d, lm->V, lm->n_pos, s));
+    SK_TRY(sk_split_f32_launch(e32, xm.hi, xm.lo, (long)B * d, s));
+    SK_TRY(sk_opt_embed_fwd_f32_launch(tokens, pos, P32 + lm->off_embed, nullptr, e32, B, 1, K, lm->V, lm->n_pos, s));
+    SK_TRY(sk_split_f32_launch(e32, h.hi, h.lo, (long)B * K, s));
+    SK_TRY(linear_split(lm, B, d, K, h, lm->off_pin, -1, 0, &xm, x, nullptr, d, s));
+  } else {
+    SK_TRY(sk_opt_embed_fwd_f32_launch(tokens, pos, P32 + lm->off_embed, P32 + lm->off_pos, e32, B, 1, d, lm->V, lm->n_pos, s));
+    SK_TRY(sk_split_f32_launch(e32, x.hi, x.lo, (long)B * d, s));
+  }
+  for (int l = 0; l < lm->L; ++l) {
+    const OptLayerOff& o = lm->olo[l];
+    float* kc = kv + (size_t)l * 2 * plane;
+    float* vc = kc + plane;
+    SK_TRY(linear_split(lm, B, Q, d, x, o.wqkv, o.bqkv, 0, nullptr, qkv, nullptr, Q, s));
+    SK_TRY(sk_kv_append_f32_launch(qkv.hi, qkv.lo, Q, kc, vc, pos, lens, B, lm->H, T_cache, s));
+    SK_TRY(sk_attn_decode_f32_launch(qkv.hi, qkv.lo, Q, kc, vc, lens, ao.hi, ao.lo, d, partial, B, lm->H, T_cache, scale, s));
+    SK_TRY(linear_split(lm, B, d, d, ao, o.wo, o.bo, 0, &x, xm, nullptr, d, s));
+    SK_TRY(sk_layernorm_hilo_launch(xm.hi, xm.lo, nullptr, nullptr, P32 + o.ln1w, P32 + o.ln1b, h.hi, h.lo, nullptr, B, d, eps, s));
+    SK_TRY(linear_split(lm, B, F, d, h, o.w1, o.b1, 2, nullptr, a, nullptr, F, s));
+    SK_TRY(linear_split(lm, B, d, F, a, o.w2, o.b2, 0, &h, xm, nullptr, d, s));
+    SK_TRY(sk_layernorm_hilo_launch(xm.hi, xm.lo, nullptr, nullptr, P32 + o.ln2w, P32 + o.ln2b, x.hi, x.lo, nullptr, B, d, eps, s));
+  }
+  Pair hin = x;
+  if (lm->proj) {
+    SK_TRY(linear_split(lm, B, K, d, x, lm->off_pout, -1, 0, nullptr, h, nullptr, K, s));
+    hin = h;
+  }
+  return linear_split(lm, B, lm->Vp, K, hin, lm->off_head, -1, 0, nullptr, Pair{nullptr, nullptr}, logits, ldl, s);
+}
+
 // kv (optional, prefill): the fp32 cache of T_cache positions that receives the K / V of positions < lens[b]
 int opt_forward_fp32(SkLm* lm, const int64_t* ids, int B, int T, const WsLayout& w, cudaStream_t s, bool with_head,
-                     float* kv = nullptr, const int32_t* lens = nullptr, int T_cache = 0) {
+                     float* kv = nullptr, const int32_t* lens = nullptr, int T_cache = 0, Pair* hin_out = nullptr) {
+  if (lm->post_ln) return opt_postln_forward_fp32(lm, ids, B, T, w, s, with_head, kv, lens, T_cache, hin_out);
   const int M = B * T, d = lm->d, F = lm->F, L = lm->L, Q = lm->qkv_dim;
   const float eps = lm->cfg.rms_eps;
   const float* P32 = lm->params32;
@@ -1064,6 +1381,7 @@ int opt_forward_fp32(SkLm* lm, const int64_t* ids, int B, int T, const WsLayout&
   }
   SK_TRY(sk_layernorm_hilo_launch(x.hi, x.lo, nullptr, nullptr, P32 + lm->off_final_norm, P32 + lm->off_final_norm_b, h.hi,
                                   h.lo, nullptr, M, d, eps, s));
+  if (hin_out) *hin_out = h;
   lm->last_B = B;
   lm->last_T = T;
   if (!with_head) return 0;
@@ -1074,6 +1392,7 @@ int opt_forward_fp32(SkLm* lm, const int64_t* ids, int B, int T, const WsLayout&
 // One token per row at position pos[b] on the fp32 cache ([K|V][B][H][T_cache][64] fp32 per layer); fp32 logits [B, ldl]
 int opt_decode_step_fp32(SkLm* lm, const int64_t* tokens, const int32_t* pos, int B, float* kv, int T_cache, float* logits,
                          int ldl, uint8_t* dws, const DecLayout& dl, cudaStream_t s) {
+  if (lm->post_ln) return opt_postln_decode_step_fp32(lm, tokens, pos, B, kv, T_cache, logits, ldl, dws, dl, s);
   const int d = lm->d, F = lm->F, Q = lm->qkv_dim;
   const float eps = lm->cfg.rms_eps;
   const float* P32 = lm->params32;
@@ -1164,14 +1483,15 @@ int sk_lm_prefill(SkLm* lm, const int64_t* ids, const int32_t* lens, int B, int 
   cudaStream_t s = (cudaStream_t)stream;
   uint8_t* dws = reinterpret_cast<uint8_t*>(decode_ws);
   SK_CUDA_CHECK(cudaMemsetAsync(dws + dl.gemm + dl.gemm_bytes - 4096, 0, 4096, s));
+  const int K = head_k(lm);
   if (lm->fp32) {
-    SK_TRY(opt_forward_fp32(lm, ids, B, T, w, s, false, reinterpret_cast<float*>(kv_cache), lens, T_cache));
+    Pair hf{nullptr, nullptr};   // the head input rows
+    SK_TRY(opt_forward_fp32(lm, ids, B, T, w, s, false, reinterpret_cast<float*>(kv_cache), lens, T_cache, &hf));
     const int64_t n = (int64_t)B * lm->d;
-    const Pair hf{wsp<bf16>(lm, w.h1), wsp<bf16>(lm, w.h1 + w.sX)};
     const Pair hl{reinterpret_cast<bf16*>(dws + dl.h), reinterpret_cast<bf16*>(dws + dl.h) + n};
-    SK_TRY(sk_gather_last_launch(hf.hi, lens, hl.hi, B, T, lm->d, s));
-    SK_TRY(sk_gather_last_launch(hf.lo, lens, hl.lo, B, T, lm->d, s));
-    return linear_split(lm, B, lm->Vp, lm->d, hl, lm->off_head, -1, 0, nullptr, Pair{nullptr, nullptr},
+    SK_TRY(sk_gather_last_launch(hf.hi, lens, hl.hi, B, T, K, s));
+    SK_TRY(sk_gather_last_launch(hf.lo, lens, hl.lo, B, T, K, s));
+    return linear_split(lm, B, lm->Vp, K, hl, lm->off_head, -1, 0, nullptr, Pair{nullptr, nullptr},
                         reinterpret_cast<float*>(logits), ldl, s);
   }
   if (lm->arch == SK_ARCH_OPT)       SK_TRY(opt_forward(lm, ids, nullptr, nullptr, B, T, 0.f, 1.f, false, nullptr, w, s, nullptr, false));
@@ -1180,8 +1500,8 @@ int sk_lm_prefill(SkLm* lm, const int64_t* ids, const int32_t* lens, int B, int 
   SK_TRY(sk_kv_prefill_launch(wsp<bf16>(lm, w.qkv), w.sqkv / 2, lm->qkv_dim, reinterpret_cast<bf16*>(kv_cache), lens, lm->L, B,
                               T, lm->H, lm->KVH, T_cache, s));
   bf16* hl = reinterpret_cast<bf16*>(dws + dl.h);
-  SK_TRY(sk_gather_last_launch(wsp<bf16>(lm, w.hf), lens, hl, B, T, lm->d, s));
-  return sk_gemm_launch(B, lm->Vp, lm->d, hl, lm->d, 0, lm->params + lm->off_head, lm->d, 0, logits, ldl, 0, nullptr, nullptr,
+  SK_TRY(sk_gather_last_launch(head_in(lm, w), lens, hl, B, T, K, s));
+  return sk_gemm_launch(B, lm->Vp, K, hl, K, 0, lm->params + lm->off_head, K, 0, logits, ldl, 0, nullptr, nullptr,
                         0, 0, 0, 0, s);
 }
 
@@ -1336,8 +1656,17 @@ int sk_lm_create_opt(const SkOptConfig* cfg, SkLm** out) {
   SK_REQUIRE(cfg->ffn > 0 && cfg->ffn % 8 == 0, "sk_lm_create_opt: ffn must be a positive multiple of 8 (got %d)", cfg->ffn);
   SK_REQUIRE(cfg->n_layers > 0 && cfg->max_positions > 0, "sk_lm_create_opt: n_layers and max_positions must be positive");
   SK_REQUIRE(cfg->vocab_size > 0 && cfg->vocab_size <= (1 << 20), "sk_lm_create_opt: vocab_size must be in [1, 2^20]");
+  SK_REQUIRE(cfg->post_ln == 0 || cfg->post_ln == 1, "sk_lm_create_opt: post_ln must be 0 or 1 (got %d)", cfg->post_ln);
+  const bool proj = cfg->proj_dim != 0 && cfg->proj_dim != cfg->hidden;
+  SK_REQUIRE(!proj || cfg->post_ln, "sk_lm_create_opt: proj_dim=%d != hidden=%d (project_in / project_out) is implemented for "
+                                    "the post-LayerNorm decoder only (post_ln = 1)", cfg->proj_dim, cfg->hidden);
+  SK_REQUIRE(!proj || (cfg->proj_dim > 0 && cfg->proj_dim % 64 == 0 && cfg->proj_dim < cfg->hidden),
+             "sk_lm_create_opt: proj_dim must be a positive multiple of 64 below hidden (got %d)", cfg->proj_dim);
   SkLm* lm = new SkLm();
   lm->arch = SK_ARCH_OPT;
+  lm->post_ln = cfg->post_ln != 0;
+  lm->proj = proj;
+  lm->pw = proj ? cfg->proj_dim : cfg->hidden;
   lm->cfg.vocab_size = cfg->vocab_size;
   lm->cfg.hidden = cfg->hidden;
   lm->cfg.n_layers = cfg->n_layers;
@@ -1378,17 +1707,29 @@ int sk_lm_create_opt(const SkOptConfig* cfg, SkLm** out) {
     o.w2 = add_tensor(lm, p + "w2", d, F);
     o.b2 = add_tensor(lm, p + "b2", 1, d);
   }
-  lm->off_final_norm = add_tensor(lm, "final_norm", 1, d);
-  lm->off_final_norm_b = add_tensor(lm, "final_norm_b", 1, d);
-  lm->off_embed = add_tensor(lm, "embed", lm->Vp, d);
+  const int pw = lm->pw;
+  if (!lm->post_ln) {   // post-LN OPT has no decoder-level final LayerNorm
+    lm->off_final_norm = add_tensor(lm, "final_norm", 1, d);
+    lm->off_final_norm_b = add_tensor(lm, "final_norm_b", 1, d);
+  }
+  lm->off_embed = add_tensor(lm, "embed", lm->Vp, pw);
   lm->off_pos = add_tensor(lm, "pos_embed", lm->n_pos, d);
-  lm->off_head = cfg->tie_embeddings ? lm->off_embed : add_tensor(lm, "lm_head", lm->Vp, d);
-  // one gradient-norm group per HF parameter, weights and biases apart (torch clip_grad_norm_ over OPTForCausalLM)
+  if (proj) {
+    lm->off_pin = add_tensor(lm, "proj_in", d, pw);
+    lm->off_pout = add_tensor(lm, "proj_out", pw, d);
+  }
+  lm->off_head = cfg->tie_embeddings ? lm->off_embed : add_tensor(lm, "lm_head", lm->Vp, pw);
+  // one gradient-norm group per HF parameter, weights and biases apart (torch clip_grad_norm_ over OPTForCausalLM, whose
+  // decoder lists embed_tokens, embed_positions, project_out, project_in, then the layers)
   std::vector<std::vector<std::pair<int64_t, int64_t>>> groups;
   auto one = [&](int64_t off, int64_t n) { groups.push_back({{off, n}}); };
   const int64_t dd = (int64_t)d * d;
-  one(lm->off_embed, (int64_t)lm->Vp * d);
+  one(lm->off_embed, (int64_t)lm->Vp * pw);
   one(lm->off_pos, (int64_t)lm->n_pos * d);
+  if (proj) {
+    one(lm->off_pout, (int64_t)pw * d);
+    one(lm->off_pin, (int64_t)d * pw);
+  }
   for (int l = 0; l < lm->L; ++l) {
     const OptLayerOff& o = lm->olo[l];
     for (int j = 0; j < 3; ++j) {   // q, k, v
@@ -1401,9 +1742,11 @@ int sk_lm_create_opt(const SkOptConfig* cfg, SkLm** out) {
     one(o.w2, (int64_t)d * F); one(o.b2, d);
     one(o.ln2w, d); one(o.ln2b, d);
   }
-  one(lm->off_final_norm, d);
-  one(lm->off_final_norm_b, d);
-  if (!cfg->tie_embeddings) one(lm->off_head, (int64_t)lm->Vp * d);
+  if (!lm->post_ln) {
+    one(lm->off_final_norm, d);
+    one(lm->off_final_norm_b, d);
+  }
+  if (!cfg->tie_embeddings) one(lm->off_head, (int64_t)lm->Vp * pw);
   const int rc = upload_norm_groups(lm, groups);
   if (rc) {
     sk_lm_destroy(lm);
@@ -1555,6 +1898,8 @@ int sk_lm_set_master(SkLm* lm, float* params32, float* grads32) {
   SK_REQUIRE(lm && params32, "sk_lm_set_master: null argument");
   SK_REQUIRE(lm->arch == SK_ARCH_OPT, "sk_lm_set_master: fp32 master weights are implemented for the OPT decoder only (the "
                                       "Qwen2 and GPT-NeoX recipes train bf16 parameters)");
+  SK_REQUIRE(!lm->post_ln, "sk_lm_set_master: fp32 master weights are implemented for the pre-LayerNorm OPT decoder only; "
+                           "this handle is post-LayerNorm (post_ln = 1): train it with bf16 parameters");
   SK_REQUIRE(lm->params && lm->ws, "sk_lm_set_master: call sk_lm_bind first");
   SK_REQUIRE(!lm->fp32, "sk_lm_set_master: this handle runs fp32 inference (sk_lm_set_fp32); master weights are a training "
                         "mode, create a separate handle");

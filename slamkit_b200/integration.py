@@ -44,7 +44,7 @@ def tlm_b200_config(cfg, autocast_bf16: Optional[bool] = None):
     base config, builds nothing on the GPU).  Returns (lm_cfg, master_weights).
 
     The base config decides the decoder: Qwen2 (`LMConfig`), pre-LayerNorm OPT (`OptLMConfig`, the default TWIST / GSLM
-    base) or parallel-residual GPT-NeoX (`NeoxLMConfig`, the Pythia bases of config/train_inter_scale.yaml).  For OPT the
+    base), post-LayerNorm OPT (`OptPostLnLMConfig`, opt-350m, bfloat16 only) or parallel-residual GPT-NeoX (`NeoxLMConfig`, the Pythia bases of config/train_inter_scale.yaml).  For OPT the
     reference's `config_args` overrides are applied to the base config as `UnitLMConfig` does (pad / bos / eos ids,
     dropout, attention_dropout, layerdrop), `rope_theta` is ignored, and `torch_dtype` picks the precision:
       - bfloat16: bf16 parameters with bf16 AdamW moments;
@@ -70,6 +70,10 @@ def tlm_b200_config(cfg, autocast_bf16: Optional[bool] = None):
             if get(k) is not None:
                 setattr(base, k, get(k))
         dt = str(get("torch_dtype")).replace("torch.", "")
+        if dt == "float32" and not getattr(base, "do_layer_norm_before", True):
+            raise ValueError("a post-LayerNorm OPT base (do_layer_norm_before=False, e.g. opt-350m) trains bf16 parameters "
+                             "with bf16 AdamW moments on the GPU path; fp32 master weights (torch_dtype=float32) are "
+                             "implemented for the pre-LayerNorm OPT only (pass model.config_args.torch_dtype=bfloat16)")
         if dt == "float32":
             if autocast_bf16 is False:
                 raise ValueError("OPT with model.config_args.torch_dtype=float32 trains fp32 master weights under bf16 autocast; "

@@ -89,6 +89,12 @@ class OptLMConfig:
         if getattr(cfg, "word_embed_proj_dim", cfg.hidden_size) != cfg.hidden_size:
             raise ValueError(f"unsupported OPT variant: word_embed_proj_dim={cfg.word_embed_proj_dim} != hidden_size="
                              f"{cfg.hidden_size} (project_in / project_out, e.g. opt-350m)")
+        OptLMConfig._check_common(cfg)
+        return OptLMConfig(**OptLMConfig._fields_from_hf(cfg, vocab_size))
+
+    @staticmethod
+    def _check_common(cfg) -> None:
+        """The refusals that pre- and post-LayerNorm OPT share, each naming its field."""
         if getattr(cfg, "_remove_final_layer_norm", False):
             raise ValueError("unsupported OPT variant: _remove_final_layer_norm=True")
         if not getattr(cfg, "enable_bias", True):
@@ -103,7 +109,10 @@ class OptLMConfig:
         for k in ("dropout", "attention_dropout", "layerdrop"):
             if float(getattr(cfg, k, 0.0) or 0.0) != 0.0:
                 raise ValueError(f"unsupported OPT setting: {k}={getattr(cfg, k)} (there are no dropout kernels; set it to 0.0)")
-        return OptLMConfig(
+
+    @staticmethod
+    def _fields_from_hf(cfg, vocab_size: Optional[int]) -> dict:
+        return dict(
             vocab_size=vocab_size or cfg.vocab_size, hidden=cfg.hidden_size, n_layers=cfg.num_hidden_layers,
             n_heads=cfg.num_attention_heads, ffn=cfg.ffn_dim, max_positions=cfg.max_position_embeddings,
             tie_embeddings=bool(getattr(cfg, "tie_word_embeddings", True)),
@@ -111,6 +120,39 @@ class OptLMConfig:
             bos_token_id=cfg.bos_token_id if cfg.bos_token_id is not None else 1,
             eos_token_id=cfg.eos_token_id if cfg.eos_token_id is not None else 1,
             init_std=float(getattr(cfg, "init_std", 0.02)))
+
+
+@dataclass
+class OptPostLnLMConfig(OptLMConfig):
+    """Shape of a post-LayerNorm OPT decoder (HF `do_layer_norm_before=False`; defaults = facebook/opt-350m with the
+    502-entry unit vocabulary, TWIST-350M's base).  Each layer normalises after its residual add and there is no final
+    LayerNorm.  `proj_dim` is `word_embed_proj_dim`: when it is neither 0 nor `hidden`, the token table and the tied head
+    are `proj_dim` wide and the bias-free project_in / project_out map them to and from the residual stream.  It is an
+    `OptLMConfig`, so every OPT path (learned positions, checkpoints, generate, scoring) takes it."""
+    hidden: int = 1024
+    n_layers: int = 24
+    n_heads: int = 16
+    ffn: int = 4096
+    proj_dim: int = 512
+
+    @property
+    def has_proj(self) -> bool:
+        return self.proj_dim not in (0, self.hidden)
+
+    @staticmethod
+    def from_hf(cfg, vocab_size: Optional[int] = None) -> "OptPostLnLMConfig":
+        """From an HF `OPTConfig` with `do_layer_norm_before=False`, with or without `word_embed_proj_dim != hidden_size`.
+        Every other variant that `OptLMConfig.from_hf` refuses is refused here too, by the same field names."""
+        if getattr(cfg, "model_type", None) != "opt":
+            raise ValueError(f"OptPostLnLMConfig.from_hf: model_type is '{getattr(cfg, 'model_type', None)}', not 'opt'")
+        if getattr(cfg, "do_layer_norm_before", True):
+            raise ValueError("OptPostLnLMConfig.from_hf: do_layer_norm_before=True is the pre-LayerNorm OPT (OptLMConfig)")
+        OptLMConfig._check_common(cfg)
+        pd = int(getattr(cfg, "word_embed_proj_dim", None) or cfg.hidden_size)
+        if pd != cfg.hidden_size and (pd % 64 or pd > cfg.hidden_size):
+            raise ValueError(f"unsupported OPT variant: word_embed_proj_dim={pd} (project_in / project_out need a multiple "
+                             f"of 64 below hidden_size={cfg.hidden_size})")
+        return OptPostLnLMConfig(**OptLMConfig._fields_from_hf(cfg, vocab_size), proj_dim=pd)
 
 
 @dataclass
@@ -182,18 +224,21 @@ class NeoxLMConfig:
 
 def lm_config_from_hf(base, vocab_size: Optional[int] = None, max_positions: int = 2048):
     """The decoder config for an HF base config, by `model_type`: `LMConfig` for qwen2 (RoPE tables of `max_positions`
-    rows), `OptLMConfig` for opt (its own learned position table; `max_positions` is ignored), `NeoxLMConfig` for
+    rows), `OptLMConfig` for opt (`OptPostLnLMConfig` when `do_layer_norm_before` is False; both have their own learned
+    position table and ignore `max_positions`), `NeoxLMConfig` for
     gpt_neox (RoPE tables of max(max_positions, max_position_embeddings) rows).  Anything else is refused."""
     mt = getattr(base, "model_type", None)
     if mt == "opt":
+        if not getattr(base, "do_layer_norm_before", True):   # post-LayerNorm OPT (opt-350m)
+            return OptPostLnLMConfig.from_hf(base, vocab_size=vocab_size)
         return OptLMConfig.from_hf(base, vocab_size=vocab_size)
     if mt == "qwen2":
         return LMConfig.from_hf(base, vocab_size=vocab_size, max_positions=max_positions)
     if mt == "gpt_neox":
         return NeoxLMConfig.from_hf(base, vocab_size=vocab_size,
                                     max_positions=max(max_positions, int(getattr(base, "max_position_embeddings", 0) or 0)))
-    raise ValueError(f"unsupported base architecture '{mt}': the GPU path implements the Qwen2, pre-LayerNorm OPT and "
-                     "GPT-NeoX (parallel residual) decoders")
+    raise ValueError(f"unsupported base architecture '{mt}': the GPU path implements the Qwen2, OPT (pre- and "
+                     "post-LayerNorm) and GPT-NeoX (parallel residual) decoders")
 
 
 def neox_qkv_segments(n_heads: int, head_dim: int = 64) -> List[Tuple[int, int, int]]:
@@ -220,10 +265,13 @@ class LMOutput:
 
 
 def _opt_base_config(c: "OptLMConfig", torch_dtype: str = "bfloat16") -> dict:
-    """The HF `OPTConfig` fields of a pre-LayerNorm OPT decoder of this shape (opt-125m layout)."""
+    """The HF `OPTConfig` fields of an OPT decoder of this shape: the opt-125m layout, or for `OptPostLnLMConfig` the
+    opt-350m one (post-LayerNorm, `word_embed_proj_dim`)."""
+    post = isinstance(c, OptPostLnLMConfig)
     return {"model_type": "opt", "architectures": ["OPTForCausalLM"], "hidden_size": c.hidden, "ffn_dim": c.ffn,
             "num_hidden_layers": c.n_layers, "num_attention_heads": c.n_heads, "vocab_size": c.vocab_size,
-            "max_position_embeddings": c.max_positions, "do_layer_norm_before": True, "word_embed_proj_dim": c.hidden,
+            "max_position_embeddings": c.max_positions, "do_layer_norm_before": not post,
+            "word_embed_proj_dim": c.proj_dim if post and c.has_proj else c.hidden,
             "activation_function": "relu", "enable_bias": True, "layer_norm_elementwise_affine": True,
             "_remove_final_layer_norm": False, "dropout": 0.0, "attention_dropout": 0.0, "layerdrop": 0.0,
             "init_std": c.init_std, "tie_word_embeddings": c.tie_embeddings, "pad_token_id": c.pad_token_id,
@@ -258,7 +306,8 @@ def write_unit_lm_checkpoint(save_directory: str, state_dict_hf: Dict[str, torch
     is_opt = isinstance(c, OptLMConfig)
     is_neox = isinstance(c, NeoxLMConfig)
     if base_model_name is None:
-        base_model_name = "facebook/opt-125m" if is_opt else ("EleutherAI/pythia-160m" if is_neox else "Qwen/Qwen2.5-0.5B")
+        base_model_name = (("facebook/opt-350m" if isinstance(c, OptPostLnLMConfig) else "facebook/opt-125m") if is_opt
+                           else ("EleutherAI/pythia-160m" if is_neox else "Qwen/Qwen2.5-0.5B"))
     sd = {k: v.detach().contiguous().cpu() for k, v in state_dict_hf.items()
           if k != "lm.lm_head.weight" or not c.tie_embeddings}
     save_file(sd, os.path.join(save_directory, "model.safetensors"), metadata={"format": "pt"})
@@ -309,7 +358,9 @@ class B200UnitLM:
     def __init__(self, config, device: str = "cuda:0", max_batch: int = 8, max_seq: int = 1024,
                  trainable: bool = True, seed: Optional[int] = None, master_weights: bool = False,
                  fp32_inference: bool = False):
-        """`config`: `LMConfig` (Qwen2 decoder), `OptLMConfig` (pre-LayerNorm OPT decoder) or `NeoxLMConfig` (GPT-NeoX).
+        """`config`: `LMConfig` (Qwen2 decoder), `OptLMConfig` (pre-LayerNorm OPT decoder), `OptPostLnLMConfig`
+        (post-LayerNorm OPT, opt-350m; bf16 training and both inference modes, no master weights) or `NeoxLMConfig`
+        (GPT-NeoX).
 
         `master_weights` (OPT only): train fp32 parameters, fp32 gradients and fp32 AdamW moments under bf16 autocast
         numerics -- the reference's default recipe (`torch_dtype: null`, `bf16: true`).  `params32` / `grads32` then hold
@@ -328,9 +379,13 @@ class B200UnitLM:
         self.is_opt = isinstance(config, OptLMConfig)
         self.is_neox = isinstance(config, NeoxLMConfig)
         self.master = bool(master_weights)
+        self.post_ln = isinstance(config, OptPostLnLMConfig)
         if self.master and not self.is_opt:
             raise ValueError("master_weights=True is implemented for the OPT decoder only (the Qwen2 and GPT-NeoX recipes "
                              "train bf16 parameters)")
+        if self.master and self.post_ln:
+            raise ValueError("master_weights=True is implemented for the pre-LayerNorm OPT decoder only; a post-LayerNorm "
+                             "OPT (OptPostLnLMConfig, e.g. opt-350m) trains bf16 parameters (torch_dtype bfloat16)")
         self.device = torch.device(device)
         torch.cuda.set_device(self.device)
         self._h = C.c_void_p()
@@ -341,6 +396,8 @@ class B200UnitLM:
         elif self.is_opt:
             c = L.SkOptConfig(config.vocab_size, config.hidden, config.n_layers, config.n_heads, config.ffn,
                               config.max_positions, config.ln_eps, int(config.tie_embeddings))
+            if self.post_ln:
+                c.post_ln, c.proj_dim = 1, config.proj_dim
             L.check(self.lib.sk_lm_create_opt(C.byref(c), C.byref(self._h)))
         else:
             c = L.SkLmConfig(config.vocab_size, config.hidden, config.n_layers, config.n_heads, config.n_kv_heads,
@@ -488,10 +545,14 @@ class B200UnitLM:
             yield p + "b1", h + "fc1.bias", [(0, 0, 1)]
             yield p + "w2", h + "fc2.weight", [(0, 0, d)]
             yield p + "b2", h + "fc2.bias", [(0, 0, 1)]
-        yield "final_norm", "lm.model.decoder.final_layer_norm.weight", [(0, 0, 1)]
-        yield "final_norm_b", "lm.model.decoder.final_layer_norm.bias", [(0, 0, 1)]
+        if not self.post_ln:                              # post-LN OPT has no decoder-level final LayerNorm
+            yield "final_norm", "lm.model.decoder.final_layer_norm.weight", [(0, 0, 1)]
+            yield "final_norm_b", "lm.model.decoder.final_layer_norm.bias", [(0, 0, 1)]
         yield "embed", "lm.model.decoder.embed_tokens.weight", [(0, 0, cfg.vocab_size)]
         yield "pos_embed", "lm.model.decoder.embed_positions.weight", [(0, 0, cfg.max_positions + 2)]
+        if self.post_ln and cfg.has_proj:
+            yield "proj_in", "lm.model.decoder.project_in.weight", [(0, 0, d)]
+            yield "proj_out", "lm.model.decoder.project_out.weight", [(0, 0, cfg.proj_dim)]
         if not cfg.tie_embeddings:
             yield "lm_head", "lm.lm_head.weight", [(0, 0, cfg.vocab_size)]
 
@@ -624,7 +685,7 @@ class B200UnitLM:
             b = {k: v for k, v in b.items() if k not in ("model_type", "architectures")}
             if not trainable:                              # dropout is inactive in eval mode
                 b.update(dropout=0.0, attention_dropout=0.0, layerdrop=0.0)
-            lm_cfg = OptLMConfig.from_hf(OPTConfig(**b), vocab_size=cfg["vocab_size"])
+            lm_cfg = lm_config_from_hf(OPTConfig(**b), vocab_size=cfg["vocab_size"])
             m = cls(lm_cfg, device=device, max_batch=max_batch, max_seq=max_seq, trainable=trainable,
                     master_weights=master_weights,
                     fp32_inference=checkpoint_is_fp32(cfg) and not trainable and not master_weights)

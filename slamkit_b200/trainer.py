@@ -57,7 +57,8 @@ class GradSync:
                                       "gradient all-reduce sums bf16 buffers); train it on one GPU")
         nl = model.config.n_layers
         t = model.tensors
-        self.layer_start = [t[f"layers.{l}.ln1"][0] for l in range(nl)] + [t["final_norm"][0]]
+        # the last bucket (lm_head / tables) starts at the final norm, or at the token table of a post-LN OPT, which has none
+        self.layer_start = [t[f"layers.{l}.ln1"][0] for l in range(nl)] + [t["final_norm" if "final_norm" in t else "embed"][0]]
         # backend: "p2p" = own kernels over CUDA-IPC peer memory (ranks on one NVSwitch node; p2p.PeerAllReduce), "nccl" =
         # torch.distributed all_reduce.  All ranks must agree, so a rank that cannot map its peers makes everyone use NCCL.
         want = (comm or os.environ.get("SK_DP_COMM", "p2p")).lower()

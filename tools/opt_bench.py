@@ -6,6 +6,10 @@ and power limit first.
 
     python tools/opt_bench.py [--steps 20] [--warmup 5] [--out results.jsonl]
     python tools/opt_bench.py --master [--steps 20] [--warmup 5] [--rounds 3]
+    python tools/opt_bench.py --geometry opt-350m [--steps 20] [--warmup 5]
+
+--geometry opt-350m runs the same train / HF / split / generate measurements on the post-LayerNorm facebook/opt-350m
+geometry (hidden 1024, 24 layers, 16 heads, ffn 4096, project_in / project_out to a 512-wide tied head).
 
 --master times bf16 parameters against fp32 master weights (the reference's default recipe: fp32 parameters,
 gradients and AdamW moments under bf16 autocast) on the same batches, alternating the two in rounds, and reports each
@@ -25,11 +29,29 @@ import torch
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 
-from oracle.opt_oracle import OracleOptConfig, flops_per_token  # noqa: E402
-from slamkit_b200.lm import B200AdamW, B200UnitLM, OptLMConfig  # noqa: E402
+from oracle import opt_oracle, opt_postln_oracle  # noqa: E402
+from slamkit_b200.lm import B200AdamW, B200UnitLM, OptLMConfig, OptPostLnLMConfig  # noqa: E402
 
 PEAK_BF16 = 989e12
 DEV = "cuda:0"
+# per geometry: the model's config, the oracle config whose FLOPs are counted, the HF OPTConfig fields, the record prefix
+GEOMETRIES = {
+    "opt-125m": (OptLMConfig, opt_oracle.OracleOptConfig, opt_oracle.flops_per_token, {}, "opt125m"),
+    "opt-350m": (OptPostLnLMConfig, lambda: opt_postln_oracle.OraclePostLnConfig(hidden=1024, n_layers=24, n_heads=16,
+                                                                                  ffn=4096, proj_dim=512),
+                 opt_postln_oracle.flops_per_token,
+                 dict(hidden_size=1024, num_hidden_layers=24, num_attention_heads=16, ffn_dim=4096, word_embed_proj_dim=512,
+                      do_layer_norm_before=False), "opt350m"),
+}
+GEOM = GEOMETRIES["opt-125m"]
+
+
+def OptConfig():
+    return GEOM[0]()
+
+
+def flops_per_token(T):
+    return GEOM[2](GEOM[1](), T)
 
 
 def emit(rec, out):
@@ -99,7 +121,7 @@ def split(step, classes=SPLIT):
 
 
 def bench_train(B, T, steps, warmup, out):
-    cfg = OptLMConfig()
+    cfg = OptConfig()
     m = B200UnitLM(cfg, device=DEV, max_batch=B, max_seq=T, seed=0)
     opt = B200AdamW(m, lr=1e-4, max_grad_norm=0.5)
     ids, labels = batch(B, T, T)
@@ -110,11 +132,11 @@ def bench_train(B, T, steps, warmup, out):
         opt.step()
     ms = time_steps(step, steps, warmup)
     toks = B * T / (ms / 1e3)
-    fl = flops_per_token(OracleOptConfig(), T) * toks
-    rec = {"what": "opt125m_train_step", "impl": "sk", "B": B, "T": T, "ms": round(ms, 3), "tokens_per_s": round(toks),
+    fl = flops_per_token(T) * toks
+    rec = {"what": f"{GEOM[4]}_train_step", "impl": "sk", "B": B, "T": T, "ms": round(ms, 3), "tokens_per_s": round(toks),
            "model_tflops": round(fl / 1e12, 1), "mfu_vs_989": round(fl / PEAK_BF16, 4), "loss": float(m.stats[0])}
     if os.environ.get("SK_PDL") == "0":
-        rec = {"what": "opt125m_train_step_split", "impl": "sk_no_pdl", "B": B, "T": T, "ms": round(ms, 3),
+        rec = {"what": f"{GEOM[4]}_train_step_split", "impl": "sk_no_pdl", "B": B, "T": T, "ms": round(ms, 3),
                "kernel_ms": split(step)}
     emit(rec, out)
     del m, opt
@@ -174,7 +196,7 @@ def bench_hf(B, T, steps, warmup, out):
     from transformers import OPTConfig, OPTForCausalLM
     torch.manual_seed(0)
     hf = OPTForCausalLM(OPTConfig(vocab_size=502, dropout=0.0, attention_dropout=0.0, layerdrop=0.0, pad_token_id=0,
-                                  bos_token_id=1, eos_token_id=1, attn_implementation="sdpa")).to(DEV).train()
+                                  bos_token_id=1, eos_token_id=1, attn_implementation="sdpa", **GEOM[3])).to(DEV).train()
     opt = torch.optim.AdamW(hf.parameters(), lr=1e-4, fused=True)
     ids, labels = batch(B, T, T)
 
@@ -189,15 +211,15 @@ def bench_hf(B, T, steps, warmup, out):
         opt.zero_grad(set_to_none=True)
     ms = time_steps(step, steps, warmup)
     toks = B * T / (ms / 1e3)
-    fl = flops_per_token(OracleOptConfig(), T) * toks
-    emit({"what": "opt125m_train_step", "impl": "hf_sdpa_autocast_bf16", "B": B, "T": T, "ms": round(ms, 3),
+    fl = flops_per_token(T) * toks
+    emit({"what": f"{GEOM[4]}_train_step", "impl": "hf_sdpa_autocast_bf16", "B": B, "T": T, "ms": round(ms, 3),
           "tokens_per_s": round(toks), "model_tflops": round(fl / 1e12, 1), "mfu_vs_989": round(fl / PEAK_BF16, 4)}, out)
     del hf, opt
     torch.cuda.empty_cache()
 
 
 def bench_generate(B, prompt, new, out):
-    m = B200UnitLM(OptLMConfig(), device=DEV, max_batch=B, max_seq=prompt, trainable=False, seed=0)
+    m = B200UnitLM(OptConfig(), device=DEV, max_batch=B, max_seq=prompt, trainable=False, seed=0)
     ids = batch(B, prompt, 5)[0]
     kw = dict(max_new_tokens=new, do_sample=False, eos_token_id=None)
     m.generate(ids, **kw)
@@ -208,7 +230,7 @@ def bench_generate(B, prompt, new, out):
         m.generate(ids, **kw)
     torch.cuda.synchronize()
     s = (time.perf_counter() - t0) / reps
-    emit({"what": "opt125m_generate", "impl": "sk", "B": B, "prompt": prompt, "new_tokens": new, "s": round(s, 4),
+    emit({"what": f"{GEOM[4]}_generate", "impl": "sk", "B": B, "prompt": prompt, "new_tokens": new, "s": round(s, 4),
           "new_tokens_per_s": round(B * new / s), "ms_per_step": round(s / new * 1e3, 3)}, out)
 
 
@@ -220,7 +242,12 @@ def main():
     ap.add_argument("--split-only", action="store_true", help=argparse.SUPPRESS)
     ap.add_argument("--master", action="store_true", help="bf16 parameters vs fp32 master weights, alternating")
     ap.add_argument("--rounds", type=int, default=3)
+    ap.add_argument("--geometry", choices=sorted(GEOMETRIES), default="opt-125m")
     a = ap.parse_args()
+    global GEOM
+    GEOM = GEOMETRIES[a.geometry]
+    if a.master and a.geometry != "opt-125m":
+        raise SystemExit("--master measures the pre-LayerNorm opt-125m geometry only (post-LN OPT trains bf16 parameters)")
     if a.master and a.split_only:
         for T in (512, 1024):
             bench_master(8, T, a.steps, a.warmup, 1, a.out, profile_only=True)
@@ -244,7 +271,8 @@ def main():
     for T in (512, 1024):
         bench_train(8, T, a.steps, a.warmup, a.out)
         bench_hf(8, T, a.steps, a.warmup, a.out)
-    subprocess.run([sys.executable, os.path.abspath(__file__), "--split-only", "--steps", "3", "--warmup", "2"] +
+    subprocess.run([sys.executable, os.path.abspath(__file__), "--split-only", "--steps", "3", "--warmup", "2",
+                    "--geometry", a.geometry] +
                    (["--out", a.out] if a.out else []), env={**os.environ, "SK_PDL": "0"}, check=True)
     for B in (1, 64):
         bench_generate(B, 64, 256, a.out)
