@@ -267,8 +267,9 @@ __global__ void __launch_bounds__(128) attn_decode_combine_kernel(const float* _
 constexpr int SEL_THREADS = 512;
 constexpr int SEL_WARPS = SEL_THREADS / 32;
 
+// order-preserving key of a score; -0.0 and +0.0 share the key of +0.0, as they compare equal in HF's argmax and warpers
 SK_DEVINL uint32_t ordered_key(float f) {
-  const uint32_t u = __float_as_uint(f);
+  const uint32_t u = f == 0.f ? 0u : __float_as_uint(f);
   return (u & 0x80000000u) ? ~u : (u | 0x80000000u);
 }
 

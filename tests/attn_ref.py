@@ -29,6 +29,11 @@ known bit for bit.  They rely on the kernels evaluating p = exp2f(s * sl2 - m * 
 - Decode.  q is pre-multiplied by scale * log2(e) per element, so scores are not exact; the row max is the target's
   own computed score, so p(target) = exp2f(0) = 1, and the margin still zeroes every other key and split.
   decode_scores emulates the kernel's fp32 FMA chain to assert that margin.
+- Decode over an fp32 cache (sk_attn_decode_split).  The query arrives as a bf16 pair, q = fl(q_hi + q_lo) (the one-hot
+  query split as in split_onehot; the target stays the maximum whatever q_lo is, so only random mode sees a dropped
+  q_lo); K holds the one-hot digits plus fp32 values that are not bf16 values in columns where q is 0; V = Vh + Vl
+  with Vl on the 2^-6 grid, so O = V[target] exactly and the output pair is o_hi = bf16(O), o_lo = bf16(O - o_hi).
+  Uniform (q = 0): O = fl(sum V) * fl(1 / n), the sum exact (|sum| < 2^15 on the 2^-6 grid).
 
 Random mode (any finite data, any scale): fp64 reference and a per-element bound that any valid flash implementation
 meets, whatever its key-tile order: P (and dS) may be rounded to bf16 once, relative to any running max; scores and
@@ -50,6 +55,9 @@ exponent error
             |dQ - dQ*| <= sum (E + N 2^-23 (|dS| + E)) |k|, each plus half a bf16 ulp, N = terms in the sum.
   split     the same with 2^-16 in place of 2^-9 (P and V carried as pairs, Pl Vl dropped) and the dropped Ql Kl term
             added to the score error (2^-16 * Sd); the output is hi + lo, within 2^-17 |O*| of its pair rounding.
+  decode, fp32 cache (q = q_hi + q_lo exact in fp32, P and V fp32): the bf16-P term drops out,
+            |O - O*| <= (e^(2D) - 1 + (3n + 8) 2^-23) sum_j pi_j (|v_j| + |O*|) + 2^-17 |O*|
+            for the output o_hi + o_lo (2^-17 |O*|: the pair rounding of the fp32 result).
 
 Checker: every comparison reports the number of mismatches and the first few as (batch, head, row, column, 64-row
 tile, 16-row warp slice), for dK / dV with the key tile as the row tile.  Works on CPU and GPU tensors alike.
@@ -301,13 +309,14 @@ def split_uniform(B: int, T: int, H: int, seed: int):
 
 
 # ----------------------------------------------------------------------------------------------------- decode
-def decode_scores(q: torch.Tensor, k: torch.Tensor, scale: float) -> torch.Tensor:
-    """The decode kernel's scaled scores, emulated: a = fl(q * fl(scale * log2 e)) per element, then a sequential fp32
-    FMA chain over the 64 dims.  q [B, H, 64], k [B, KVH, Tc, 64] -> [B, H, Tc]."""
+def decode_scores(q: torch.Tensor, k: torch.Tensor, scale: float, q_lo: Optional[torch.Tensor] = None) -> torch.Tensor:
+    """The decode kernel's scaled scores, emulated: a = fl(q * fl(scale * log2 e)) per element (q = fl(q + q_lo) for a
+    split query), then a sequential fp32 FMA chain over the 64 dims.  q [B, H, 64], k [B, KVH, Tc, 64] -> [B, H, Tc]."""
     B, H, _ = q.shape
     KVH = k.shape[1]
     sl2 = torch.tensor(scale, dtype=torch.float32) * torch.tensor(LOG2E, dtype=torch.float32)
-    a = q.float() * sl2                                                   # fp32 product
+    qf = q.float() if q_lo is None else q.float() + q_lo.float()          # fp32 sum
+    a = qf * sl2                                                          # fp32 product
     kk = k.float().repeat_interleave(H // KVH, dim=1)                    # [B, H, Tc, 64]
     acc = torch.zeros(kk.shape[:3])
     for d in range(HD):
@@ -325,8 +334,16 @@ def decode_onehot(B: int, H: int, KVH: int, T_cache: int, lens: torch.Tensor, mo
     q = onehot_q(tgt, modes)
     k = onehot_k(B, T_cache, KVH).permute(0, 2, 1, 3).contiguous()
     v = int_values((B, KVH, T_cache, HD), 8, seed)
-    e = decode_scores(q, k, EXACT_SCALE)                                 # [B, H, Tc]
-    for b in range(B):
+    _check_decode_margin(decode_scores(q, k, EXACT_SCALE), tgt, lens)
+    kv = torch.arange(H) // (H // KVH)
+    o = v[torch.arange(B)[:, None], kv[None, :], tgt]
+    o[lens == 0] = 0.0
+    return q, k, v, o
+
+
+def _check_decode_margin(e: torch.Tensor, tgt: torch.Tensor, lens: torch.Tensor) -> None:
+    """e [B, H, Tc] emulated exponents: every allowed non-target key lies more than UNDERFLOW below the target."""
+    for b in range(e.shape[0]):
         n = int(lens[b])
         if n == 0:
             continue
@@ -334,11 +351,76 @@ def decode_onehot(B: int, H: int, KVH: int, T_cache: int, lens: torch.Tensor, mo
         st = eb.gather(1, tgt[b][:, None])
         gap = eb - st
         gap.scatter_(1, tgt[b][:, None], -math.inf)
-        assert float(gap.max()) < -UNDERFLOW, f"decode margin {float(gap.max())}"
-    kv = torch.arange(H) // (H // KVH)
-    o = v[torch.arange(B)[:, None], kv[None, :], tgt]
+        if n > 1:
+            assert float(gap.max()) < -UNDERFLOW, f"decode margin {float(gap.max())}"
+
+
+def _pair(x: torch.Tensor):
+    hi = bf16(x)
+    return hi, bf16(x - hi)
+
+
+def decode_split_onehot(B: int, H: int, T_cache: int, lens: torch.Tensor, modes: Sequence[str], seed: int):
+    """One-hot inputs of the fp32-cache decode (KVH = H): (q_hi, q_lo [B, H, 64], k, v fp32 [B, H, T_cache, 64]) and
+    the expected (o_hi, o_lo) [B, H, 64]; asserts the margin on the emulated scores.  k = k_hi + k_lo and
+    v = v_hi + v_lo exactly (bf16 pairs), so the same keys can be fed to the split-bf16 prefill kernel."""
+    lens = lens.long()
+    lo = torch.zeros(B, 1, dtype=torch.int64)
+    hi = (lens - 1).clamp_min(0)[:, None]
+    tgt = onehot_targets(lo, hi, modes)[:, 0]                          # [B, H]
+    q = onehot_q(tgt, modes)
+    sg = torch.tensor([1.0 if m == "latest" else -1.0 for m in modes])
+    p = torch.tensor([2.0 ** (10 + 4 * d) for d in range(4)])
+    q_lo = torch.zeros_like(q)
+    q_lo[..., 4:8] = sg[:, None] * p
+    q_hi = q - q_lo
+    assert is_bf16(q_hi) and is_bf16(q_lo) and torch.equal(q_hi + q_lo, q)
+    g = torch.Generator().manual_seed(seed)
+    k = onehot_k(B, T_cache, H).permute(0, 2, 1, 3).contiguous()
+    k[..., 8:16] = sum(_pair(torch.randn(B, H, T_cache, 8, generator=g)))   # fp32, never multiplied by a non-zero q
+    v = int_values((B, H, T_cache, HD), 8, seed) + int_values((B, H, T_cache, HD), 16, seed + 1) / 64.0
+    _check_decode_margin(decode_scores(q_hi, k, EXACT_SCALE, q_lo), tgt, lens)
+    o = v[torch.arange(B)[:, None], torch.arange(H)[None, :], tgt]
     o[lens == 0] = 0.0
-    return q, k, v, o
+    return (q_hi, q_lo, k, v), _pair(o)
+
+
+def decode_split_uniform(B: int, H: int, T_cache: int, lens: torch.Tensor, seed: int):
+    """q = 0 over an fp32 cache: (k, v [B, H, T_cache, 64]) and the expected (o_hi, o_lo) of
+    O = fl(sum_{j < lens} v) * fl(1 / lens), the sum exact; 0 for lens = 0."""
+    g = torch.Generator().manual_seed(seed)
+    k = sum(_pair(torch.randn(B, H, T_cache, HD, generator=g) * 4))
+    v = int_values((B, H, T_cache, HD), 8, seed) + int_values((B, H, T_cache, HD), 16, seed + 1) / 64.0
+    o = torch.zeros(B, H, HD)
+    for b in range(B):
+        n = int(lens[b])
+        if n:
+            s = v[b, :, :n].double().sum(1)
+            assert float(s.abs().max()) < 2 ** 15
+            o[b] = s.float() * (torch.ones(()) / torch.tensor(float(n)))
+    return (k, v), _pair(o)
+
+
+def decode_f32_reference(q: torch.Tensor, k: torch.Tensor, v: torch.Tensor, lens: torch.Tensor, scale: float):
+    """fp64 decode over an fp32 cache with the per-element bound of the module docstring: q [B, H, 64] (fp32 value of
+    the pair), k / v [B, H, Tc, 64] -> (O* [B, H, 64], bound)."""
+    B, H, _ = q.shape
+    O = torch.zeros(B, H, HD, dtype=torch.float64)
+    bo = torch.zeros_like(O)
+    for b in range(B):
+        n = int(lens[b])
+        if n == 0:
+            continue
+        qb, kb, vb = q[b].double(), k[b, :, :n].double(), v[b, :, :n].double()
+        s = torch.einsum("hd,hjd->hj", qb, kb) * scale
+        sd = torch.einsum("hd,hjd->hj", qb.abs(), kb.abs()) * scale
+        pi = torch.softmax(s, -1)
+        o = torch.einsum("hj,hjd->hd", pi, vb)
+        D = 64 * 2.0 ** -23 * sd.max(-1).values + 2.0 ** -20 * (s.abs().max(-1).values + 1)
+        spread = torch.einsum("hj,hjd->hd", pi, vb.abs()) + o.abs()
+        O[b] = o
+        bo[b] = (torch.expm1(2 * D)[:, None] + (3 * n + 8) * 2.0 ** -23) * spread + 2.0 ** -17 * o.abs()
+    return O, bo
 
 
 def expect_decode_uniform(v: torch.Tensor, lens: torch.Tensor, H: int):

@@ -67,7 +67,7 @@ def _tokens(V, kind, ban, B, T, g):
     return ids
 
 
-@pytest.mark.parametrize("V", [502, 152167])
+@pytest.mark.parametrize("V", [502, 8192, 8193, 152167])
 @pytest.mark.parametrize("kind", [None, "400", "speech"])
 def test_seq_loglik_matches_reference_formula(V, kind):
     if kind == "speech" and V != 152167:

@@ -1,6 +1,6 @@
 """Batched KV-cache decoding behind `B200UnitLM.generate`: decode attention against fp32 math, prefill + decode steps against
 the full forward and the fp32 oracle, cached greedy generation against the oracle's argmax, the device sampler against the
-CPU statement of HF's selection rules (slamkit_b200/generation.py), the Philox draw distribution, reproducibility and CUDA
+CPU statement of HF's selection rules (tests/decode_ref.py), the Philox draw distribution, reproducibility and CUDA
 graph replay, and the 152 k text+unit vocabulary."""
 import ctypes as C
 import math
@@ -8,6 +8,7 @@ import math
 import pytest
 import torch
 
+from decode_ref import expected_token
 from helpers import rel_err
 
 pytestmark = pytest.mark.gpu
@@ -208,28 +209,6 @@ def test_generate_eos_max_length_max_positions_and_bans():
 
 
 # ---------------------------------------------------------------------------------------------- 4. sampler vs CPU rules
-def _expected_token(logits, do_sample, temperature, top_k, top_p, banned, u):
-    """generation.process_logits (top-p restated with a stable sort), softmax, inverse CDF at u in token-id order.
-    Returns (token, distance of u to the nearest CDF boundary)."""
-    from slamkit_b200.generation import process_logits
-    if not do_sample:
-        s = logits.float().clone()
-        if banned:
-            s[banned] = float("-inf")
-        return int(torch.nonzero(s == s.max())[0]), 1.0
-    s = process_logits(logits, temperature, top_k, None, banned)
-    if top_p is not None and top_p < 1.0:
-        ss, idx = torch.sort(s, descending=False, stable=True)
-        cum = ss.softmax(-1).cumsum(-1)
-        remove = cum <= (1.0 - top_p)
-        remove[-1] = False
-        s = s.masked_fill(remove.scatter(0, idx, remove), float("-inf"))
-    cdf = torch.softmax(s.double(), -1).cumsum(-1)
-    tok = int(torch.searchsorted(cdf, torch.tensor([u], dtype=torch.float64), right=True)[0])
-    tok = min(tok, int(torch.nonzero(s > float("-inf"))[-1]))
-    return tok, float((cdf - u).abs().min())
-
-
 SAMPLER_CASES = {
     "greedy": dict(do_sample=False),
     "temp0.8-top_k25": dict(do_sample=True, temperature=0.8, top_k=25),
@@ -276,8 +255,8 @@ def test_sampler_matches_cpu_rules(V, case):
     assert int(step[0]) == 1 and tokens.cpu().tolist() == got and st["pos"].cpu().tolist() == [1] * B
     skipped = 0
     for b in range(B):
-        want, dist = _expected_token(logits[b], c["do_sample"], c.get("temperature", 1.0), c.get("top_k"), c.get("top_p"),
-                                     banned, float(u[b]))
+        want, dist = expected_token(logits[b], c["do_sample"], c.get("temperature", 1.0), c.get("top_k"), c.get("top_p"),
+                                    banned, float(u[b]))
         if dist < 1e-6:
             skipped += 1
             continue

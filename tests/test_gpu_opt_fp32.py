@@ -327,7 +327,7 @@ def _scoring_case(V, B, T, seed):
     return z, buf.to(DEV), ids, ban, ldl
 
 
-@pytest.mark.parametrize("V", [502, 9000])
+@pytest.mark.parametrize("V", [502, 8192, 8193, 9000])
 @pytest.mark.parametrize("mean_nll", [False, True])
 @pytest.mark.parametrize("banned", [False, True])
 def test_seq_loglik_f32_vs_fp64(V, mean_nll, banned):
@@ -434,7 +434,8 @@ def test_decode_graph_replay_and_batch_invariance():
 
 @pytest.mark.parametrize("case", ["greedy", "temp0.8-top_k25", "top_p0.9", "bans-greedy", "bans-temp1.3-top_k40"])
 def test_select_next_f32_matches_host_rules(case):
-    from test_gpu_generate import SAMPLER_CASES, _expected_token
+    from decode_ref import expected_token
+    from test_gpu_generate import SAMPLER_CASES
     from slamkit_b200.generation import ban_bitmask
     L, lib = _lib()
     c = dict(SAMPLER_CASES[case])
@@ -464,8 +465,8 @@ def test_select_next_f32_matches_host_rules(case):
     got = out[:, 0].cpu().tolist()
     skipped = 0
     for b in range(B):
-        want, dist = _expected_token(logits[b], c["do_sample"], c.get("temperature", 1.0), c.get("top_k"), c.get("top_p"),
-                                     banned, float(u[b]))
+        want, dist = expected_token(logits[b], c["do_sample"], c.get("temperature", 1.0), c.get("top_k"), c.get("top_p"),
+                                    banned, float(u[b]))
         if dist < 1e-6:
             skipped += 1
             continue
