@@ -134,7 +134,8 @@ def generate_max_seq(cfg, tokeniser, dataset) -> int:
 
 def run_generate(cfg, tokeniser, device: str) -> dict:
     """cli/eval.py's `metric=generate` branch: continue the prompts and write `<out_path>/generate_<i>.wav` (32-bit
-    float at the tokeniser's sample rate) for the first `num_log` non-empty continuations.  Prints no metric lines."""
+    float at the tokeniser's sample rate) for the first `num_log` non-empty continuations, numbered in the result list's
+    order (with `num_return_sequences = k`, the k continuations of a prompt are adjacent).  Prints no metric lines."""
     from slamkit_b200 import metrics as M
     from slamkit_b200.audio_io import write_wav_float
     from slamkit_b200.integration import vocoder_b200_from_cfg
@@ -145,7 +146,9 @@ def run_generate(cfg, tokeniser, device: str) -> dict:
                          num_files=m.num_files, min_file_length=m.get("min_file_length", None),
                          use_alignment=m.get("use_alignment", False), alignment_folder=m.get("alignment_folder", None))
     assert len(ds) > 0, f"no samples found for {path}"
-    vocoder = vocoder_b200_from_cfg(cfg.vocoder, device=device, max_rows=cfg.batch_size)
+    # every prompt yields num_return_sequences continuations, vocoded in one batch
+    n_ret = int(m.get("generate_kwargs", {}).get("num_return_sequences", None) or 1)
+    vocoder = vocoder_b200_from_cfg(cfg.vocoder, device=device, max_rows=cfg.batch_size * n_ret)
     model = B200SpeechLM(load_model(cfg, device, max_seq=generate_max_seq(cfg, tokeniser, ds)), tokeniser, vocoder=vocoder)
     res = M.generate(model, path, cfg.batch_size, m.get("used_token_modality", None), m.prompt_length,
                      m.get("min_file_length", None), m.get("alignment_folder", None), m.get("use_alignment", False),

@@ -437,6 +437,12 @@ int sk_lm_prefill(SkLm* lm, const int64_t* ids, const int32_t* lens, int B, int 
  * RMSNorm -> SwiGLU GEMM -> down-proj + residual; final norm, head -> logits [B, ldl]. */
 int sk_lm_decode_step(SkLm* lm, const int64_t* tokens, const int32_t* pos, int B, void* kv_cache, int T_cache,
                       void* logits, int ldl, void* decode_ws, int64_t decode_ws_bytes, void* stream);
+/* Prompt fan-out for num_return_sequences: copies positions t < lens[b] of every layer's K and V of row b of src_cache
+ * (B rows) into rows b*k .. b*k + k - 1 of dst_cache (B*k rows), both with the same T_cache and the handle's layout
+ * ([L][K|V][rows][KVH][T_cache][head_dim], bf16, or fp32 on fp32 inference handles).  Positions >= lens[b] of the
+ * destination are not written.  src and dst must not overlap; both 16-byte aligned. */
+int sk_lm_kv_fanout(const SkLm* lm, const void* src_cache, int B, int k, void* dst_cache, int T_cache, const int32_t* lens,
+                    void* stream);
 /* Stand-alone decode attention: o[b, h*64 .. h*64+63] (pitch ldo) = softmax(q k^T * scale) v over keys [0, lens[b]) of
  * row b; q [B, H*64] pitch ldq; k_cache / v_cache [B][KVH][T_cache][64] bf16.  Flash-decoding over fixed 64-key splits
  * (one CTA per row, kv head and split serves the H/KVH <= 16 query heads of its group) and a combine pass in split
@@ -483,6 +489,35 @@ int sk_select_next(const void* logits, int ldl, int V, int B, const uint32_t* ba
 /* sk_select_next on fp32 logits [B, ldl] (fp32 inference handles); logits 16-byte aligned. */
 int sk_select_next_f32(const float* logits, int ldl, int V, int B, const uint32_t* ban_bits, const SkSampling* cfg,
                        const float* uniforms, const SkDecodeState* state, void* stream);
+/* History-dependent logits processors (HF GenerationConfig repetition_penalty, no_repeat_ngram_size, min_new_tokens /
+ * min_length).  Row b's history is history[b, 0 .. prompt_len + step): the padded prompt exactly as the caller passed
+ * it (left pads included), then the tokens selected so far (pad_token_id for finished rows). */
+typedef struct SkLogitRules {
+  int64_t* history;          /* [B, hist_ld]; columns < prompt_len filled by the caller, the rest appended per step */
+  uint32_t* presence;        /* [B, ceil(V/32)] bit i: id i occurs in the history (sk_presence_init, then per step) */
+  uint32_t* scratch;         /* [B, ceil(V/32)] per-step bans; needed when ngram > 0 or min_step > 0 */
+  float penalty;             /* repetition_penalty; 1: off */
+  int32_t ngram;             /* no_repeat_ngram_size; <= 0: off */
+  int32_t min_step;          /* eos ids are -inf while step < min_step (needs n_eos > 0) */
+  int32_t prompt_len;        /* T, the padded prompt width */
+  int32_t hist_ld;           /* >= prompt_len + max_new */
+  int32_t reserved;
+} SkLogitRules;
+/* sk_select_next / sk_select_next_f32 with rules, applied on the fp32 scores in HF's order (penalty -> n-gram bans ->
+ * ban_bits -> min length), before temperature; greedy honours them too:
+ *   repetition penalty: every id whose presence bit is set: s = s < 0 ? s * penalty : s / penalty (rounded once);
+ *   n-gram bans (cur_len = prompt_len + step, when cur_len + 1 >= ngram): every id that followed an earlier occurrence of
+ *     the row's last ngram - 1 tokens, at any position of the history, pads included, is -inf;
+ *   min length: while step < min_step, every eos id is -inf.
+ * After the selection every row appends its token (pad_token_id once finished) at history[b, prompt_len + step] and
+ * sets its presence bit.  The step index is read from device memory: graph-capturable as sk_select_next.
+ * presence may be NULL when penalty == 1; scratch may be NULL when there are no n-gram or min-length bans. */
+int sk_select_next_ex(const void* logits, int ldl, int V, int B, const uint32_t* ban_bits, const SkSampling* cfg,
+                      const float* uniforms, const SkDecodeState* state, const SkLogitRules* rules, void* stream);
+int sk_select_next_ex_f32(const float* logits, int ldl, int V, int B, const uint32_t* ban_bits, const SkSampling* cfg,
+                          const float* uniforms, const SkDecodeState* state, const SkLogitRules* rules, void* stream);
+/* presence[b] = the bitmap of history[b, 0 .. prompt_len) (ids outside [0, V) are skipped); overwrites every word. */
+int sk_presence_init(const int64_t* history, int hist_ld, int prompt_len, int B, int V, uint32_t* presence, void* stream);
 
 /* ---- sequence scoring (modelling metrics of cli/eval.py) ---------------------------------------------------------------
  * The tail of UnitLM.log_likelihood (slamkit/model/unit_lm.py:184-194 -> calc_nll, slamkit/utils/calculation_utils.py:5-29)

@@ -111,6 +111,20 @@ class SkDecodeState(C.Structure):
     ]
 
 
+class SkLogitRules(C.Structure):
+    _fields_ = [
+        ("history", C.c_void_p),
+        ("presence", C.c_void_p),
+        ("scratch", C.c_void_p),
+        ("penalty", C.c_float),
+        ("ngram", C.c_int32),
+        ("min_step", C.c_int32),
+        ("prompt_len", C.c_int32),
+        ("hist_ld", C.c_int32),
+        ("reserved", C.c_int32),
+    ]
+
+
 class SkGemmPlan(C.Structure):
     _fields_ = [
         ("bn", C.c_int32),
@@ -168,6 +182,12 @@ def load() -> C.CDLL:
     for name in ("sk_lm_logits", "sk_lm_logits_f32"):
         getattr(lib, name).restype = C.c_void_p
     lib.sk_lm_destroy.restype = None
+    _p, _i = C.c_void_p, C.c_int
+    for name in ("sk_select_next_ex", "sk_select_next_ex_f32"):
+        getattr(lib, name).argtypes = [_p, _i, _i, _i, _p, C.POINTER(SkSampling), _p, C.POINTER(SkDecodeState),
+                                       C.POINTER(SkLogitRules), _p]
+    lib.sk_presence_init.argtypes = [_p, _i, _i, _i, _i, _p, _p]
+    lib.sk_lm_kv_fanout.argtypes = [_p, _p, _i, _i, _p, _i, _p, _p]
     if hasattr(lib, "sk_hubert_destroy"):
         lib.sk_hubert_destroy.restype = None
     if hasattr(lib, "sk_vocoder_destroy"):

@@ -325,27 +325,79 @@ SK_DEVINL T block_exclusive_scan(T v, T* red, T& total) {
 SK_DEVINL float logit_at(const bf16* row, int i) { return __bfloat162float(row[i]); }
 SK_DEVINL float logit_at(const float* row, int i) { return row[i]; }
 
-template <typename LT>
+SK_DEVINL bool bit_set(const uint32_t* bits, int i) { return (bits[i >> 5] >> (i & 31)) & 1u; }
+
+// RULES: the SkLogitRules processors of one row.  `dyn` holds this step's n-gram and min-length bans (NULL when there
+// are none), `pres` the presence bitmap when the repetition penalty is on.  The penalty is one rounded multiply or divide
+// and the temperature one rounded divide, as HF applies them one processor after the other.
+template <typename LT, bool RULES>
 struct SelRow {
   const LT* row;
   const uint32_t* ban;
   float temp;
   bool use_temp;
+  const uint32_t* dyn;
+  const uint32_t* pres;
+  float penalty;
   SK_DEVINL float score(int i) const {
     if (ban && ((ban[i >> 5] >> (i & 31)) & 1u)) return -INFINITY;
-    const float x = logit_at(row, i);
+    float x = logit_at(row, i);
+    if constexpr (RULES) {
+      if (dyn && bit_set(dyn, i)) return -INFINITY;
+      if (pres && bit_set(pres, i)) x = x < 0.f ? __fmul_rn(x, penalty) : __fdiv_rn(x, penalty);
+    }
     return use_temp ? __fdiv_rn(x, temp) : x;
   }
 };
 
+// appends the selected token (pad once finished) to the row's history and sets its presence bit
+SK_DEVINL void rules_append(const SkLogitRules& r, int b, int step, int tok, int V) {
+  const int c = r.prompt_len + step;
+  if (c < r.hist_ld) r.history[(size_t)b * r.hist_ld + c] = tok;
+  if (r.presence && tok >= 0 && tok < V) r.presence[(size_t)b * ((V + 31) >> 5) + (tok >> 5)] |= 1u << (tok & 31);
+}
+
+// this step's n-gram and min-length bans of row b into its scratch bitmap (all threads of the CTA); NULL if none apply
+SK_DEVINL const uint32_t* rules_bans(const SkLogitRules& r, const SkSampling& cfg, int b, int step, int V) {
+  const int cur = min(r.prompt_len + step, r.hist_ld), n = r.ngram;
+  const bool ngram = n > 0 && cur + 1 >= n;
+  const bool min_len = step < r.min_step && cfg.n_eos > 0;
+  if (!ngram && !min_len) return nullptr;
+  const int W = (V + 31) >> 5;
+  uint32_t* d = r.scratch + (size_t)b * W;
+  for (int w = threadIdx.x; w < W; w += blockDim.x) d[w] = 0u;
+  __syncthreads();
+  if (min_len && threadIdx.x == 0)
+    for (int e = 0; e < cfg.n_eos && e < 8; ++e)
+      if (cfg.eos[e] >= 0 && cfg.eos[e] < V) atomicOr(&d[cfg.eos[e] >> 5], 1u << (cfg.eos[e] & 31));
+  if (ngram) {
+    // HF's NoRepeatNGram: the n-grams h[j .. j+n-1], j <= cur - n, whose first n-1 tokens equal the last n-1 tokens
+    // h[cur-n+1 .. cur-1] ban their last token
+    const int64_t* h = r.history + (size_t)b * r.hist_ld;
+    const int tail = cur - n + 1;
+    for (int j = threadIdx.x; j <= cur - n; j += blockDim.x) {
+      int m = 0;
+      while (m < n - 1 && h[j + m] == h[tail + m]) ++m;
+      if (m == n - 1) {
+        const int64_t t = h[j + n - 1];
+        if (t >= 0 && t < V) atomicOr(&d[t >> 5], 1u << (t & 31));
+      }
+    }
+  }
+  __syncthreads();
+  return d;
+}
+
 // One CTA per row.  Order of HF's processors: bans -> (sampling only) temperature -> top-k -> top-p -> softmax -> draw;
 // greedy = argmax of the banned scores, lowest id on ties.  Each thread owns the contiguous id range
 // [tid * chunk, (tid + 1) * chunk), so per-thread partial sums are in token order and every sum is taken in a fixed order.
-// LT: bf16 logits, or fp32 ones (fp32 OPT inference).
-template <typename LT>
+// LT: bf16 logits, or fp32 ones (fp32 OPT inference).  RULES: apply `rules` (sk_select_next_ex) and append to the
+// history; without, `rules` is not read.
+template <typename LT, bool RULES>
 __global__ void __launch_bounds__(SEL_THREADS) select_next_kernel(const LT* __restrict__ logits, int ldl, int V,
                                                                   const uint32_t* __restrict__ ban, SkSampling cfg,
-                                                                  const float* __restrict__ uniforms, SkDecodeState st) {
+                                                                  const float* __restrict__ uniforms, SkDecodeState st,
+                                                                  SkLogitRules rules) {
   __shared__ float red_f[SEL_WARPS];
   __shared__ int red_i[SEL_WARPS];
   __shared__ unsigned long long red_u[SEL_WARPS];
@@ -371,12 +423,21 @@ __global__ void __launch_bounds__(SEL_THREADS) select_next_kernel(const LT* __re
     if (tid == 0) {
       st.finished[b] = 1;
       if (step < st.max_new) st.out[(size_t)b * st.max_new + step] = cfg.pad_token_id;
+      if constexpr (RULES) rules_append(rules, b, step, cfg.pad_token_id, V);
     }
     return;
   }
   const int chunk = (V + SEL_THREADS - 1) / SEL_THREADS;
   const int i0 = min(tid * chunk, V), i1 = min(i0 + chunk, V);
-  SelRow<LT> R{logits + (size_t)b * ldl, ban, cfg.temperature, cfg.do_sample != 0 && cfg.temperature != 1.0f};
+  SelRow<LT, RULES> R{logits + (size_t)b * ldl, ban, cfg.temperature, cfg.do_sample != 0 && cfg.temperature != 1.0f,
+                      nullptr, nullptr, 1.f};
+  if constexpr (RULES) {
+    R.dyn = rules_bans(rules, cfg, b, step, V);
+    if (rules.penalty != 1.f) {
+      R.pres = rules.presence + (size_t)b * ((V + 31) >> 5);
+      R.penalty = rules.penalty;
+    }
+  }
   int tok = 0;
   if (!cfg.do_sample) {
     // argmax, lowest id among equal maxima
@@ -535,6 +596,36 @@ __global__ void __launch_bounds__(SEL_THREADS) select_next_kernel(const LT* __re
     bool eos = false;
     for (int e = 0; e < cfg.n_eos && e < 8; ++e) eos |= (tok == cfg.eos[e]);
     if (eos) st.finished[b] = 1;
+    if constexpr (RULES) rules_append(rules, b, step, tok, V);
+  }
+}
+
+// presence[b] = bitmap of history[b, 0 .. T).  grid B
+__global__ void presence_init_kernel(const int64_t* __restrict__ history, int hist_ld, int T, int V,
+                                     uint32_t* __restrict__ presence) {
+  griddep_wait();
+  const int b = blockIdx.x, W = (V + 31) >> 5;
+  uint32_t* p = presence + (size_t)b * W;
+  for (int w = threadIdx.x; w < W; w += blockDim.x) p[w] = 0u;
+  __syncthreads();
+  for (int t = threadIdx.x; t < T; t += blockDim.x) {
+    const int64_t id = history[(size_t)b * hist_ld + t];
+    if (id >= 0 && id < V) atomicOr(&p[id >> 5], 1u << (id & 31));
+  }
+}
+
+// prompt fan-out: the first lens[b] rows of the [T_cache][row_bytes] plane of (layer | K/V, row b, kv head) go to rows
+// b*k .. b*k+k-1 of the destination.  grid (B * KVH, 2 L)
+__global__ void kv_fanout_kernel(const uint4* __restrict__ src, uint4* __restrict__ dst, const int32_t* __restrict__ lens,
+                                 int B, int k, int KVH, int T_cache, int row16) {
+  griddep_wait();
+  const int b = blockIdx.x / KVH, kvh = blockIdx.x % KVH, lw = blockIdx.y;
+  const int n = min(max(lens[b], 0), T_cache) * row16;
+  const size_t plane = (size_t)T_cache * row16;
+  const uint4* s = src + (((size_t)lw * B + b) * KVH + kvh) * plane;
+  for (int j = 0; j < k; ++j) {
+    uint4* d = dst + (((size_t)lw * B * k + (size_t)b * k + j) * KVH + kvh) * plane;
+    for (int i = threadIdx.x; i < n; i += blockDim.x) d[i] = s[i];
   }
 }
 
@@ -579,6 +670,18 @@ int sk_gather_last_launch(const bf16* x, const int32_t* lens, bf16* out, int B, 
   return 0;
 }
 
+int sk_kv_fanout_launch(const void* src, void* dst, const int32_t* lens, int L, int B, int k, int KVH, int T_cache,
+                        int row_bytes, cudaStream_t s) {
+  SK_REQUIRE(B > 0 && k > 0 && L > 0 && KVH > 0 && T_cache > 0 && row_bytes % 16 == 0, "kv_fanout: bad shape B=%d k=%d "
+             "T_cache=%d row_bytes=%d", B, k, T_cache, row_bytes);
+  SK_REQUIRE((((uintptr_t)src | (uintptr_t)dst) & 15) == 0, "kv_fanout: caches must be 16-byte aligned");
+  SK_CUDA_CHECK(sk_launch_pdl(kv_fanout_kernel, dim3(B * KVH, 2 * L), dim3(256), (size_t)0, s,
+                              reinterpret_cast<const uint4*>(src), reinterpret_cast<uint4*>(dst), lens, B, k, KVH, T_cache,
+                              row_bytes / 16));
+  SK_LAUNCH_CHECK();
+  return 0;
+}
+
 int sk_attn_decode_splits(int T_cache) { return (T_cache + DEC_CH - 1) / DEC_CH; }
 
 // KV = bf16: q, o bf16 (q_lo, o_lo unused); KV = float: q and o are (hi, lo) pairs
@@ -617,14 +720,27 @@ int sk_attn_decode_f32_launch(const bf16* q_hi, const bf16* q_lo, int ldq, const
 
 template <typename LT>
 int select_next(const LT* logits, int ldl, int V, int B, const uint32_t* ban, const SkSampling& cfg, const float* uniforms,
-                const SkDecodeState& st, cudaStream_t s) {
+                const SkDecodeState& st, cudaStream_t s, const SkLogitRules* rules = nullptr) {
   SK_REQUIRE(B > 0 && V > 0 && ldl >= V, "select_next: bad shape B=%d V=%d ldl=%d", B, V, ldl);
   SK_REQUIRE(cfg.n_eos >= 0 && cfg.n_eos <= 8, "select_next: at most 8 eos ids");
   SK_REQUIRE(!cfg.do_sample || cfg.temperature > 0.f, "select_next: temperature must be > 0");
   SK_REQUIRE(st.tokens && st.pos && st.finished && st.n_gen && st.out && st.step && st.max_new > 0,
              "select_next: incomplete decode state");
-  SK_CUDA_CHECK(sk_launch_pdl(select_next_kernel<LT>, dim3(B), dim3(SEL_THREADS), (size_t)0, s, logits, ldl, V, ban, cfg,
-                              uniforms, st));
+  if (rules) {
+    const SkLogitRules& r = *rules;
+    SK_REQUIRE(r.history && r.prompt_len >= 0 && r.hist_ld >= r.prompt_len + st.max_new,
+               "select_next_ex: history [B, hist_ld] with hist_ld >= prompt_len + max_new required (prompt_len=%d "
+               "hist_ld=%d max_new=%d)", r.prompt_len, r.hist_ld, st.max_new);
+    SK_REQUIRE(r.penalty > 0.f, "select_next_ex: repetition penalty must be > 0");
+    SK_REQUIRE(r.penalty == 1.f || r.presence, "select_next_ex: the repetition penalty needs the presence bitmap");
+    SK_REQUIRE(r.scratch || (r.ngram <= 0 && (r.min_step <= 0 || cfg.n_eos == 0)),
+               "select_next_ex: n-gram and min-length bans need the scratch bitmap");
+    SK_CUDA_CHECK(sk_launch_pdl(select_next_kernel<LT, true>, dim3(B), dim3(SEL_THREADS), (size_t)0, s, logits, ldl, V, ban,
+                                cfg, uniforms, st, r));
+  } else {
+    SK_CUDA_CHECK(sk_launch_pdl(select_next_kernel<LT, false>, dim3(B), dim3(SEL_THREADS), (size_t)0, s, logits, ldl, V, ban,
+                                cfg, uniforms, st, SkLogitRules{}));
+  }
   SK_LAUNCH_CHECK();
   return 0;
 }
@@ -660,6 +776,30 @@ int sk_select_next_f32(const float* logits, int ldl, int V, int B, const uint32_
   SK_REQUIRE(logits && cfg && state, "sk_select_next_f32: null argument");
   SK_REQUIRE(((uintptr_t)logits & 15) == 0, "sk_select_next_f32: logits must be 16-byte aligned");
   return select_next<float>(logits, ldl, V, B, ban_bits, *cfg, uniforms, *state, (cudaStream_t)stream);
+}
+
+int sk_select_next_ex(const void* logits, int ldl, int V, int B, const uint32_t* ban_bits, const SkSampling* cfg,
+                      const float* uniforms, const SkDecodeState* state, const SkLogitRules* rules, void* stream) {
+  SK_REQUIRE(logits && cfg && state && rules, "sk_select_next_ex: null argument");
+  return select_next<bf16>(reinterpret_cast<const bf16*>(logits), ldl, V, B, ban_bits, *cfg, uniforms, *state,
+                           (cudaStream_t)stream, rules);
+}
+
+int sk_select_next_ex_f32(const float* logits, int ldl, int V, int B, const uint32_t* ban_bits, const SkSampling* cfg,
+                          const float* uniforms, const SkDecodeState* state, const SkLogitRules* rules, void* stream) {
+  SK_REQUIRE(logits && cfg && state && rules, "sk_select_next_ex_f32: null argument");
+  SK_REQUIRE(((uintptr_t)logits & 15) == 0, "sk_select_next_ex_f32: logits must be 16-byte aligned");
+  return select_next<float>(logits, ldl, V, B, ban_bits, *cfg, uniforms, *state, (cudaStream_t)stream, rules);
+}
+
+int sk_presence_init(const int64_t* history, int hist_ld, int prompt_len, int B, int V, uint32_t* presence, void* stream) {
+  SK_REQUIRE(history && presence, "sk_presence_init: null argument");
+  SK_REQUIRE(B > 0 && V > 0 && prompt_len >= 0 && hist_ld >= prompt_len, "sk_presence_init: bad shape B=%d V=%d T=%d "
+             "hist_ld=%d", B, V, prompt_len, hist_ld);
+  SK_CUDA_CHECK(sk_launch_pdl(presence_init_kernel, dim3(B), dim3(256), (size_t)0, (cudaStream_t)stream, history, hist_ld,
+                              prompt_len, V, presence));
+  SK_LAUNCH_CHECK();
+  return 0;
 }
 
 int sk_attn_decode_split(const void* q_hi, const void* q_lo, int ldq, const float* k_cache, const float* v_cache,

@@ -209,6 +209,8 @@ int sk_attn_decode_f32_launch(const bf16* q_hi, const bf16* q_lo, int ldq, const
 int sk_attn_decode_splits(int T_cache);
 int sk_attn_decode_launch(const bf16* q, int ldq, const bf16* kc, const bf16* vc, const int32_t* lens, bf16* o, int ldo,
                           float* partial, int B, int H, int KVH, int T_cache, float scale, cudaStream_t s);
+int sk_kv_fanout_launch(const void* src, void* dst, const int32_t* lens, int L, int B, int k, int KVH, int T_cache,
+                        int row_bytes, cudaStream_t s);
 struct SkSampling;
 struct SkDecodeState;
 int sk_select_next_launch(const bf16* logits, int ldl, int V, int B, const uint32_t* ban, const SkSampling& cfg,

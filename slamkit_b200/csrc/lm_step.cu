@@ -1505,6 +1505,13 @@ int sk_lm_prefill(SkLm* lm, const int64_t* ids, const int32_t* lens, int B, int 
                         0, 0, 0, 0, s);
 }
 
+int sk_lm_kv_fanout(const SkLm* lm, const void* src_cache, int B, int k, void* dst_cache, int T_cache, const int32_t* lens,
+                    void* stream) {
+  SK_REQUIRE(lm && src_cache && dst_cache && lens, "sk_lm_kv_fanout: null argument");
+  return sk_kv_fanout_launch(src_cache, dst_cache, lens, lm->L, B, k, lm->KVH, T_cache, lm->hd * (lm->fp32 ? 4 : 2),
+                             (cudaStream_t)stream);
+}
+
 int sk_lm_decode_step(SkLm* lm, const int64_t* tokens, const int32_t* pos, int B, void* kv_cache, int T_cache,
                       void* logits, int ldl, void* decode_ws, int64_t decode_ws_bytes, void* stream) {
   SK_REQUIRE(lm && tokens && pos, "sk_lm_decode_step: null argument");

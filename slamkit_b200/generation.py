@@ -9,8 +9,11 @@ CPU statement of the rules that path implements, so that a model trained here ca
   * decoder-only conventions: prompts arrive LEFT-padded with an `attention_mask` (speech_lm.py:44-45); each row is decoded
     without the pads (positions start at 0 at the first real token, as HF derives them from the mask) and the result is
     the padded prompt followed by the continuation, right-padded with `pad_token_id` after `eos_token_id`;
-  * logits processing in HF's order: `bad_words_ids` (single-token entries) -> temperature -> top-k -> top-p -> softmax ->
-    multinomial (`do_sample=True`) or argmax.
+  * logits processing in HF's order: `repetition_penalty` -> `no_repeat_ngram_size` -> `bad_words_ids` (single-token
+    entries) -> `min_length` / `min_new_tokens` -> temperature -> top-k -> top-p -> softmax -> multinomial
+    (`do_sample=True`) or argmax; the first four also apply in greedy mode.  The history they read is the padded
+    prompt exactly as passed (left pads included) followed by the tokens generated so far;
+  * `num_return_sequences = k`: the prompts are `repeat_interleave(k)`-ed, rows in that order (sampling only).
 `select_next` and `generate_tokens` are pure torch functions of a `next_logits(ids[1,t]) -> [vocab]` callable (one row at
 a time, no cache), which is how the CPU tests check them against `transformers`' own `generate` and logits warpers and
 how the GPU tests check the device sampler.
@@ -22,11 +25,57 @@ from typing import Callable, List, Optional, Sequence
 import torch
 
 
-def process_logits(logits: torch.Tensor, temperature: float = 1.0, top_k: Optional[int] = None, top_p: Optional[float] = None,
-                   banned: Optional[Sequence[int]] = None) -> torch.Tensor:
-    """fp32 scores after HF's NoBadWords -> Temperature -> TopK -> TopP processors (filtered entries = -inf)."""
-    s = logits.float().clone()
+def min_step(prompt_len: int, min_length: Optional[int] = None, min_new_tokens: Optional[int] = None) -> int:
+    """Steps during which eos is masked.  HF turns a set `min_new_tokens` into `min_length = min_new_tokens + T` (the
+    given `min_length` is then ignored), and both processors count the padded prompt width T."""
+    if min_new_tokens is not None:
+        return max(int(min_new_tokens), 0)
+    return max(int(min_length or 0) - prompt_len, 0)
+
+
+def ngram_bans(history: Sequence[int], n: int) -> List[int]:
+    """HF NoRepeatNGramLogitsProcessor on one row: the tokens that followed an earlier occurrence of the row's last n-1
+    tokens (none while len(history) + 1 < n)."""
+    h, cur = list(history), len(history)
+    if n <= 0 or cur + 1 < n:
+        return []
+    key = h[cur - n + 1:]
+    return sorted({h[j + n - 1] for j in range(cur - n + 1) if h[j:j + n - 1] == key})
+
+
+def apply_rules(s: torch.Tensor, history: Optional[Sequence[int]] = None, prompt_len: int = 0,
+                repetition_penalty: Optional[float] = None, no_repeat_ngram_size: int = 0,
+                banned: Optional[Sequence[int]] = None, eos: Sequence[int] = (), min_length: Optional[int] = None,
+                min_new_tokens: Optional[int] = None) -> torch.Tensor:
+    """fp32 scores [V] of one row after HF's RepetitionPenalty -> NoRepeatNGram -> NoBadWords -> MinLength /
+    MinNewTokens processors (in place).  history: the row's padded prompt (prompt_len ids) + the tokens generated."""
+    history = [] if history is None else [int(t) for t in history]
+    if repetition_penalty is not None and repetition_penalty != 1.0:
+        if repetition_penalty <= 0:
+            raise ValueError("repetition_penalty must be a strictly positive float")
+        ids = torch.tensor(sorted(set(history)), dtype=torch.long)
+        g = s[ids]
+        s[ids] = torch.where(g < 0, g * repetition_penalty, g / repetition_penalty)
+    if no_repeat_ngram_size and no_repeat_ngram_size > 0:
+        b = ngram_bans(history, int(no_repeat_ngram_size))
+        if b:
+            s[b] = float("-inf")
     if banned is not None and len(banned):
+        s[list(banned)] = float("-inf")
+    if eos and len(history) - prompt_len < min_step(prompt_len, min_length, min_new_tokens):
+        s[list(eos)] = float("-inf")
+    return s
+
+
+def process_logits(logits: torch.Tensor, temperature: float = 1.0, top_k: Optional[int] = None, top_p: Optional[float] = None,
+                   banned: Optional[Sequence[int]] = None, **rules) -> torch.Tensor:
+    """fp32 scores after HF's [RepetitionPenalty -> NoRepeatNGram ->] NoBadWords [-> MinLength / MinNewTokens] ->
+    Temperature -> TopK -> TopP processors (filtered entries = -inf).  `rules`: the history keywords of `apply_rules`
+    (one row, logits [V])."""
+    s = logits.float().clone()
+    if rules:
+        s = apply_rules(s, banned=banned, **rules)
+    elif banned is not None and len(banned):
         s[..., list(banned)] = float("-inf")
     if temperature is not None and temperature != 1.0:
         if temperature <= 0:
@@ -49,13 +98,15 @@ def process_logits(logits: torch.Tensor, temperature: float = 1.0, top_k: Option
 
 def select_next(logits: torch.Tensor, do_sample: bool, temperature: float = 1.0, top_k: Optional[int] = None,
                 top_p: Optional[float] = None, banned: Optional[Sequence[int]] = None,
-                generator: Optional[torch.Generator] = None) -> int:
+                generator: Optional[torch.Generator] = None, **rules) -> int:
     if not do_sample:          # greedy: the warpers are not applied (HF only builds them when sampling)
         s = logits.float().clone()
-        if banned is not None and len(banned):
+        if rules:
+            s = apply_rules(s, banned=banned, **rules)
+        elif banned is not None and len(banned):
             s[..., list(banned)] = float("-inf")
         return int(torch.argmax(s, dim=-1))
-    s = process_logits(logits, temperature, top_k, top_p, banned)
+    s = process_logits(logits, temperature, top_k, top_p, banned, **rules)
     return int(torch.multinomial(torch.softmax(s, dim=-1), 1, generator=generator))
 
 
@@ -91,10 +142,23 @@ def generate_tokens(next_logits: Callable[[torch.Tensor], torch.Tensor], inputs:
                     max_length: Optional[int] = None, do_sample: bool = False, temperature: float = 1.0,
                     top_k: Optional[int] = None, top_p: Optional[float] = None, eos_token_id=None,
                     pad_token_id: Optional[int] = None, bad_words_ids=None, max_positions: Optional[int] = None,
-                    generator: Optional[torch.Generator] = None) -> torch.Tensor:
-    """inputs [B, T] (left-padded when attention_mask has leading zeros) -> [B, T + n_new] int64 on inputs' device."""
+                    generator: Optional[torch.Generator] = None, repetition_penalty: Optional[float] = None,
+                    no_repeat_ngram_size: Optional[int] = None, min_length: Optional[int] = None,
+                    min_new_tokens: Optional[int] = None, num_return_sequences: Optional[int] = None) -> torch.Tensor:
+    """inputs [B, T] (left-padded when attention_mask has leading zeros) -> [B*k, T + n_new] int64 on inputs' device
+    (k = num_return_sequences).  Rows advance together one step at a time, so sampling draws from `generator` in HF's
+    order (step by step, rows in order)."""
     if inputs.dim() != 2:
         raise ValueError("generate: inputs must be [batch, time]")
+    k = int(num_return_sequences or 1)
+    if k < 1:
+        raise ValueError("num_return_sequences must be >= 1")
+    if k > 1 and not do_sample:
+        raise ValueError("Greedy methods (do_sample != True) without beam search do not support `num_return_sequences` "
+                         f"different than 1 (got {k}).")
+    if k > 1:
+        inputs = inputs.repeat_interleave(k, dim=0)
+        attention_mask = attention_mask.repeat_interleave(k, dim=0) if attention_mask is not None else None
     B, T = inputs.shape
     if max_new_tokens is None:
         max_new_tokens = (max_length if max_length is not None else 20) - T          # HF's default: max_length = 20 in total
@@ -104,7 +168,12 @@ def generate_tokens(next_logits: Callable[[torch.Tensor], torch.Tensor], inputs:
     if eos and pad_token_id is None:
         pad_token_id = min(eos)                                  # HF: "Setting pad_token_id to eos_token_id"
     banned = _single_token_bans(bad_words_ids)
-    rows: List[List[int]] = []
+    rules = {}
+    if (repetition_penalty not in (None, 1.0) or (no_repeat_ngram_size or 0) > 0
+            or (eos and min_step(T, min_length, min_new_tokens) > 0)):
+        rules = dict(prompt_len=T, repetition_penalty=repetition_penalty, no_repeat_ngram_size=no_repeat_ngram_size or 0,
+                     eos=sorted(eos), min_length=min_length, min_new_tokens=min_new_tokens)
+    seqs: List[List[int]] = []
     for b in range(B):
         row = inputs[b]
         if attention_mask is not None:
@@ -113,19 +182,28 @@ def generate_tokens(next_logits: Callable[[torch.Tensor], torch.Tensor], inputs:
             if n_real == 0 or not bool(m[T - n_real:].all()):
                 raise ValueError("generate: attention_mask must be left-padding (zeros first, then ones) for every row")
             row = row[T - n_real:]
-        seq = row.tolist()
-        new: List[int] = []
-        for _ in range(max_new_tokens):
+        seqs.append(row.tolist())
+    padded = inputs.to("cpu").tolist()
+    fill = pad_token_id if pad_token_id is not None else 0
+    rows: List[List[int]] = [[] for _ in range(B)]
+    done = [False] * B
+    for step in range(max_new_tokens):
+        for b in range(B):
+            if done[b]:
+                continue
+            seq, new = seqs[b], rows[b]
             if max_positions is not None and len(seq) + len(new) >= max_positions:
-                break
+                done[b] = True
+                continue
             ids = torch.tensor([seq + new], dtype=torch.long)
-            tok = select_next(next_logits(ids), do_sample, temperature, top_k, top_p, banned, generator)
+            hist = dict(rules, history=padded[b] + new) if rules else {}
+            tok = select_next(next_logits(ids), do_sample, temperature, top_k, top_p, banned, generator, **hist)
             new.append(tok)
             if tok in eos:
-                break
-        rows.append(new)
+                done[b] = True
+        if all(done):
+            break
     n_new = max((len(r) for r in rows), default=0)
-    fill = pad_token_id if pad_token_id is not None else 0
     out = torch.full((B, T + n_new), fill, dtype=torch.long)
     out[:, :T] = inputs.to("cpu")
     for b, r in enumerate(rows):

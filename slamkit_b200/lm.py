@@ -835,7 +835,10 @@ class B200UnitLM:
         token is one batched decode step plus on-device token selection, captured once as a CUDA graph and replayed.
         The host looks at the rows' `finished` flags every 16 steps only.  Sampling draws from a Philox stream whose seed
         comes from `generator` (or torch's default CPU generator), so `torch.manual_seed` makes runs reproducible.
-        Prompt plus continuation is bounded by `max_positions`."""
+        Prompt plus continuation is bounded by `max_positions`.  `repetition_penalty`, `no_repeat_ngram_size` and
+        `min_length` / `min_new_tokens` run inside the selection kernel on a device copy of each row's history;
+        `num_return_sequences = k` prefills each prompt once and copies its KV cache to k rows (output [B*k, ...],
+        rows of one prompt adjacent, as HF orders them)."""
         if self.master:
             raise NotImplementedError("generate: this model trains fp32 master weights; generate from its saved checkpoint "
                                       "(B200UnitLM.from_pretrained without master_weights)")
@@ -845,7 +848,8 @@ class B200UnitLM:
         if inputs is None:
             raise ValueError("generate: no prompt (inputs / input_ids)")
         keys = ("max_new_tokens", "max_length", "do_sample", "temperature", "top_k", "top_p", "eos_token_id", "pad_token_id",
-                "bad_words_ids")
+                "bad_words_ids", "repetition_penalty", "no_repeat_ngram_size", "min_length", "min_new_tokens",
+                "num_return_sequences")
         opts = {}
         if generation_config is not None:
             for k in keys:
@@ -864,7 +868,9 @@ class B200UnitLM:
         unknown = sorted(k for k in kwargs if k not in keys and k not in ignored and kwargs[k] is not None)
         if unknown:
             raise NotImplementedError(f"generate: unsupported arguments {unknown} (greedy / sampling with temperature, top_k, "
-                                      "top_p, bad_words_ids, eos / pad ids and length limits are implemented)")
+                                      "top_p, bad_words_ids, repetition_penalty, no_repeat_ngram_size, min_length, "
+                                      "min_new_tokens, num_return_sequences, eos / pad ids and length limits are "
+                                      "implemented)")
         opts.setdefault("eos_token_id", getattr(self.config, "eos_token_id", 1))      # UnitTokeniser: bos = eos = 1
         opts.setdefault("pad_token_id", self.config.pad_token_id)
         if opts.get("do_sample") and "top_k" not in opts:
@@ -873,11 +879,23 @@ class B200UnitLM:
 
     def _generate_cached(self, inputs: torch.Tensor, attention_mask: Optional[torch.Tensor], max_new_tokens=None,
                          max_length=None, do_sample=False, temperature=None, top_k=None, top_p=None, eos_token_id=None,
-                         pad_token_id=None, bad_words_ids=None, generator=None) -> torch.Tensor:
-        from .generation import _single_token_bans, ban_bitmask
+                         pad_token_id=None, bad_words_ids=None, generator=None, repetition_penalty=None,
+                         no_repeat_ngram_size=None, min_length=None, min_new_tokens=None,
+                         num_return_sequences=None) -> torch.Tensor:
+        from .generation import _single_token_bans, ban_bitmask, min_step
         if inputs.dim() != 2:
             raise ValueError("generate: inputs must be [batch, time]")
         B, T = inputs.shape
+        k = int(num_return_sequences or 1)
+        if k < 1:
+            raise ValueError("num_return_sequences must be >= 1")
+        if k > 1 and not do_sample:
+            raise ValueError("Greedy methods (do_sample != True) without beam search do not support `num_return_sequences` "
+                             f"different than 1 (got {k}).")
+        penalty = float(repetition_penalty) if repetition_penalty is not None else 1.0
+        if penalty <= 0:
+            raise ValueError(f"repetition_penalty has to be a strictly positive float, but is {repetition_penalty}")
+        ngram = int(no_repeat_ngram_size or 0)
         if max_new_tokens is None:
             max_new_tokens = (max_length if max_length is not None else 20) - T      # HF's default: max_length = 20 in total
         if max_new_tokens < 0:
@@ -898,8 +916,14 @@ class B200UnitLM:
             left = torch.arange(T)[None, :] >= (T - lens)[:, None]
             if B and (bool((lens == 0).any()) or not torch.equal(m, left)):
                 raise ValueError("generate: attention_mask must be left-padding (zeros first, then ones) for every row")
+        bound = min_step(T, min_length, min_new_tokens) if eos else 0
+        rules = penalty != 1.0 or ngram > 0 or bound > 0
+        V = self.config.vocab_size
+        if rules and B and bool(((inputs < 0) | (inputs >= V)).any()):
+            raise ValueError(f"generate: repetition_penalty / no_repeat_ngram_size read every prompt id, pads included; "
+                             f"all must be in [0, {V})")
         if B == 0 or max_new_tokens == 0:
-            return inputs.clone()
+            return inputs.repeat_interleave(k, dim=0) if k > 1 else inputs.clone()
         P = self.config.max_positions
         Lmax = int(lens.max())
         if Lmax > P:
@@ -912,7 +936,6 @@ class B200UnitLM:
         cols = torch.arange(Lmax)[None, :]
         src = ((T - lens)[:, None] + cols).clamp(max=T - 1)
         ids = torch.where(cols < lens[:, None], inputs.to("cpu").gather(1, src), torch.zeros((), dtype=torch.long))
-        V = self.config.vocab_size
         seed = 0
         if do_sample:
             gen = generator if generator is not None else torch.default_generator
@@ -924,9 +947,11 @@ class B200UnitLM:
             cfg.eos[i] = e
         if do_sample and cfg.temperature <= 0:
             raise ValueError("temperature must be > 0")
-        sess = DecodeSession(self, B, T_cache, max_new_tokens, fill)
+        sess = DecodeSession(self, B * k, T_cache, max_new_tokens, fill)
+        if rules:
+            sess.set_rules(inputs.repeat_interleave(k, dim=0), penalty, ngram, bound)
         ban = ban_bitmask(banned, V).to(self.device) if banned else None
-        sess.prefill(ids, lens)
+        sess.prefill(ids, lens, k)
         sess.select(cfg, ban)
         n_steps = max_new_tokens - 1
         if n_steps > 0:
@@ -953,7 +978,8 @@ class B200UnitLM:
                     g.replay()
                     done += 1
         n_new = int(sess.n_gen.max())
-        out = torch.cat([inputs.to(self.device), sess.out[:, :n_new]], dim=1)
+        prompts = inputs.repeat_interleave(k, dim=0) if k > 1 else inputs
+        out = torch.cat([prompts.to(self.device), sess.out[:, :n_new]], dim=1)
         return out.to(inputs.device)
 
 
@@ -961,7 +987,8 @@ class DecodeSession:
     """Device buffers of one batched incremental decode of a `B200UnitLM`: the KV cache of all layers, the decode
     workspace, the [B, vocab] logits of the current step and the selection state (`SkDecodeState`).  PyTorch owns the
     memory; `prefill`, `step` and `select` enqueue `sk_lm_prefill`, `sk_lm_decode_step` and `sk_select_next` on the
-    current stream.  `step` and `select` take the same arguments every call, so they can be captured in a CUDA graph."""
+    current stream.  `step` and `select` take the same arguments every call, so they can be captured in a CUDA graph.
+    After `set_rules`, `select` runs `sk_select_next_ex` over the rows' device history instead."""
 
     def __init__(self, model: B200UnitLM, B: int, T_cache: int, max_new: int, pad_token_id: int = 0):
         self.m, self.B, self.T_cache = model, B, T_cache
@@ -978,25 +1005,56 @@ class DecodeSession:
         self.step_ctr = torch.zeros(2, device=dev, dtype=torch.int32)
         self.state = L.SkDecodeState(self.tokens.data_ptr(), self.pos.data_ptr(), self.finished.data_ptr(),
                                      self.n_gen.data_ptr(), self.out.data_ptr(), self.step_ctr.data_ptr(), self.out.shape[1], 0)
+        self.rules = None
+
+    def set_rules(self, prompts: torch.Tensor, penalty: float = 1.0, ngram: int = 0, min_step: int = 0) -> None:
+        """Turns on the history processors (SkLogitRules): prompts are the [B, T] padded prompts exactly as passed to
+        generate.  Allocates the history [B, T + max_new] and, as the rules need them, the presence and ban bitmaps;
+        call before `prefill`, which builds the presence bitmap."""
+        B, T = prompts.shape
+        if B != self.B:
+            raise ValueError(f"set_rules: {B} prompts for a session of {self.B} rows")
+        dev, W = self.m.device, (self.m.config.vocab_size + 31) // 32
+        self.history = torch.zeros(B, T + self.out.shape[1], device=dev, dtype=torch.long)
+        self.history[:, :T] = prompts.to(dev)
+        self.presence = torch.empty(B, W, device=dev, dtype=torch.int32) if penalty != 1.0 else None
+        self.scratch = torch.empty(B, W, device=dev, dtype=torch.int32) if ngram > 0 or min_step > 0 else None
+        self.rules = L.SkLogitRules(self.history.data_ptr(), L.ptr(self.presence).value, L.ptr(self.scratch).value,
+                                    float(penalty), int(ngram), int(min_step), T, self.history.shape[1], 0)
 
     @property
     def logits(self) -> torch.Tensor:
         """[B, vocab_size] logits of the last prefill / decode step (bf16; fp32 with fp32 inference)."""
         return self.logits_buf[:, :self.m.config.vocab_size]
 
-    def prefill(self, ids: torch.Tensor, lens: torch.Tensor) -> torch.Tensor:
+    def prefill(self, ids: torch.Tensor, lens: torch.Tensor, k: int = 1) -> torch.Tensor:
         """ids: right-padded [B, T] prompts, lens: real tokens per row.  Fills the cache; the next token of row b goes
-        to position lens[b] (its last prompt token, at lens[b] - 1, is the state's current token)."""
+        to position lens[b] (its last prompt token, at lens[b] - 1, is the state's current token).  k > 1
+        (num_return_sequences): the session has B*k rows; each prompt is prefilled once at [B, T] and its cache rows,
+        logits, token and position are copied to rows b*k .. b*k + k - 1 (`sk_lm_kv_fanout`)."""
         m = self.m
         B, T = ids.shape
+        if B * k != self.B:
+            raise ValueError(f"prefill: {B} prompts x {k} for a session of {self.B} rows")
         m._ensure(B, T)
         ids_d = ids.to(m.device, dtype=torch.long).contiguous()
         lens_d = lens.to(m.device, dtype=torch.int32).contiguous()
-        self.tokens.copy_(ids_d.gather(1, (lens_d.long() - 1).clamp(min=0)[:, None])[:, 0])
-        self.pos.copy_(lens_d - 1)
-        L.check(m.lib.sk_lm_prefill(m._h, L.ptr(ids_d), L.ptr(lens_d), B, T, L.ptr(self.kv), self.T_cache,
+        tok = ids_d.gather(1, (lens_d.long() - 1).clamp(min=0)[:, None])[:, 0]
+        kv = self.kv if k == 1 else torch.empty(int(m.lib.sk_lm_kv_cache_bytes(m._h, B, self.T_cache)), device=m.device,
+                                                dtype=torch.uint8)
+        L.check(m.lib.sk_lm_prefill(m._h, L.ptr(ids_d), L.ptr(lens_d), B, T, L.ptr(kv), self.T_cache,
                                     L.ptr(self.logits_buf), self.ldl, L.ptr(self.ws), C.c_int64(self.ws.numel()),
                                     L.stream_ptr()))
+        if k > 1:
+            L.check(m.lib.sk_lm_kv_fanout(m._h, L.ptr(kv), B, k, L.ptr(self.kv), self.T_cache, L.ptr(lens_d),
+                                          L.stream_ptr()))
+            self.logits_buf.copy_(self.logits_buf[:B].repeat_interleave(k, dim=0))
+            tok, lens_d = tok.repeat_interleave(k), lens_d.repeat_interleave(k)
+        self.tokens.copy_(tok)
+        self.pos.copy_(lens_d - 1)
+        if self.rules is not None and self.presence is not None:
+            L.check(m.lib.sk_presence_init(L.ptr(self.history), self.history.shape[1], self.rules.prompt_len, self.B,
+                                           m.config.vocab_size, L.ptr(self.presence), L.stream_ptr()))
         return self.logits
 
     def step(self, tokens: Optional[torch.Tensor] = None, pos: Optional[torch.Tensor] = None) -> torch.Tensor:
@@ -1011,9 +1069,14 @@ class DecodeSession:
 
     def select(self, cfg: "L.SkSampling", ban: Optional[torch.Tensor] = None, uniforms: Optional[torch.Tensor] = None) -> None:
         m = self.m
-        fn = m.lib.sk_select_next_f32 if m.fp32 else m.lib.sk_select_next
-        L.check(fn(L.ptr(self.logits_buf), self.ldl, m.config.vocab_size, self.B, L.ptr(ban), C.byref(cfg), L.ptr(uniforms),
-                   C.byref(self.state), L.stream_ptr()))
+        args = (L.ptr(self.logits_buf), self.ldl, m.config.vocab_size, self.B, L.ptr(ban), C.byref(cfg), L.ptr(uniforms),
+                C.byref(self.state))
+        if self.rules is None:
+            fn = m.lib.sk_select_next_f32 if m.fp32 else m.lib.sk_select_next
+            L.check(fn(*args, L.stream_ptr()))
+        else:
+            fn = m.lib.sk_select_next_ex_f32 if m.fp32 else m.lib.sk_select_next_ex
+            L.check(fn(*args, C.byref(self.rules), L.stream_ptr()))
 
 
 class B200AdamW:

@@ -39,7 +39,8 @@ class B200SpeechLM:
     def generate(self, wavs: torch.Tensor, lens: Optional[torch.Tensor] = None, output_modality: str = "SPEECH",
                  remove_prompt: bool = False, **kwargs) -> List[torch.Tensor]:
         """speech_lm.py:38-55: continue each zero-padded prompt clip; with a vocoder, one waveform per row (an empty
-        tensor for an empty continuation), otherwise the decoded unit ids."""
+        tensor for an empty continuation), otherwise the decoded unit ids.  With `num_return_sequences = k` there are
+        B*k rows, the k continuations of each prompt adjacent (HF's order)."""
         if not hasattr(self.tokeniser, "build_prompt"):
             raise NotImplementedError("generate needs the unit tokeniser: interleaved (speech + text) prompts are not "
                                       "supported")
