@@ -193,6 +193,22 @@ int sk_swiglu_bwd(const void* gu, const void* dact, void* dgu, int M, int F, voi
 int sk_ce_blocks(int M);
 int sk_ce_fwd_bwd(const void* logits, const int64_t* labels, void* dlogits, float* partial, float* row_nll,
                   float* stats, int M, int T, int V, int ldl, float num_items, float dloss, void* stream);
+/* Test hooks over the launchers the train step uses.  sk_ce_fwd_bwd_weighted: sk_ce_fwd_bwd with the gradient of row m
+ * scaled by row_weight[m] (fp32 [M], the DPO path's per-sequence weights).  sk_ce_chunk: the chunked lm_head's CE on rows
+ * [row0, row0 + rows) whose logits sit at logits_chunk ([rows, ldl]; dlogits_chunk may equal it), one (nll, valid) pair
+ * per global row in partial fp32 [2 * M]; grad_scale multiplies the gradient.  sk_ce_finalize sums the pairs into stats. */
+int sk_ce_fwd_bwd_weighted(const void* logits, const int64_t* labels, void* dlogits, float* partial, float* row_nll,
+                           const float* row_weight, float* stats, int M, int T, int V, int ldl, float num_items, float dloss,
+                           void* stream);
+int sk_ce_chunk(const void* logits_chunk, const int64_t* labels, void* dlogits_chunk, float* partial, int row0, int rows,
+                int M, int T, int V, int ldl, float grad_scale, void* stream);
+int sk_ce_finalize(const float* partial, int M, float num_items, float* stats, void* stream);
+/* OPT learned positions: dP[row(m)] (+)= dx[m] in the fixed point of sk_embed_bwd, row(m) = min(max(pos + 2, 0), n_pos - 1)
+ * with pos = pos_ids[m] (int32 [M]) or m % T when pos_ids is NULL.  scratch: n_pos * D 64-bit words. */
+int sk_opt_pos_bwd(const int32_t* pos_ids, const void* dx, float* scratch, void* dP, int M, int T, int D, int n_pos,
+                   int accumulate, void* stream);
+/* ReLU backward in place, torch threshold_backward(g, a, 0): g = a <= 0 ? 0 : g (bf16 [n], n a multiple of 8). */
+int sk_relu_bwd(void* g, const void* a, int64_t n, void* stream);
 
 /* ---- attention -------------------------------------------------------------------------------------------------
  * softmax(q k^T * scale [causal]) v with grouped-query heads, head_dim 64; q/k/v are column slices (pitch ld) of the
@@ -261,6 +277,16 @@ int sk_add_layernorm_f32(const float* x, const void* y, const float* w, const fl
 int sk_layernorm_bwd_f32(const void* dy, const float* x, const float* w, const float* mean, const float* rstd, const float* dres_in,
                          float* dres_out, void* dres16, float* dw, float* db, float* partial, int M, int D, int accumulate,
                          void* stream);
+/* Test hooks over the master step's table and widening launchers.  sk_table_bwd_f32: fp32 table gradient from fp32 rows
+ * dx [M, D] in the 64-bit fixed point of sk_embed_bwd: ids given, row(m) = ids[m] (ids outside [0, n_rows) skipped) and
+ * head (bf16 [n_rows_padded, D] or NULL) is added; ids NULL, row(m) is the OPT position row of sk_opt_pos_bwd.
+ * dtable = (keep ? dtable : 0) + (float(head) + sum); scratch: n_rows_padded * D 64-bit words.
+ * sk_widen_grads: g32 (+)= float(g16) over the chunks [chunk_start[c], + chunk_len[c]) (device tables as sk_grad_norm;
+ * starts and lengths multiples of 8). */
+int sk_table_bwd_f32(const int64_t* ids, const int32_t* pos_ids, const float* dx, float* scratch, float* dtable, const void* head,
+                     int M, int T, int D, int n_rows, int n_rows_padded, int keep, void* stream);
+int sk_widen_grads(const void* g16, float* g32, const int64_t* chunk_start, const int32_t* chunk_len, int n_chunks, int keep,
+                   void* stream);
 
 /* ---- causal-LM train step (path (ii)) ---------------------------------------------------------------------------
  * One object per model replica; replaces UnitLM.forward + compute_loss + autograd backward
@@ -367,6 +393,9 @@ int sk_lm_bind(SkLm* lm, void* params, void* grads, const void* rope_cos, const 
  *   - sk_lm_prefill / sk_lm_decode_step refuse the handle (generation runs on the saved checkpoint).
  * Qwen2 and GPT-NeoX handles are refused. */
 int sk_lm_set_master(SkLm* lm, float* params32, float* grads32);
+/* The chunks whose bf16 gradients the master step widens into grads32 (see sk_widen_grads), copied to host arrays of
+ * capacity cap; returns the number of chunks, or -1. */
+int sk_lm_widen_chunks(const SkLm* lm, int64_t* chunk_start, int32_t* chunk_len, int cap);
 /* OPT handles only, after sk_lm_bind: fp32 inference, as the reference scores and generates a float32 checkpoint (HF
  * OPTForCausalLM in fp32, no autocast).  params32 is a caller-owned flat fp32 [param_count] buffer in the bf16 layout
  * (it stays referenced); `prepared` (>= sk_lm_fp32_prepared_bytes, 256-byte aligned) receives its split-bf16 (hi, lo)

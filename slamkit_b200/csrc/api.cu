@@ -279,6 +279,32 @@ int sk_ce_fwd_bwd(const void* logits, const int64_t* labels, void* dlogits, floa
   return sk_ce_launch(CBF(logits), labels, BF(dlogits), partial, row_nll, stats, M, T, V, ldl, num_items, dloss,
                       S(stream));
 }
+int sk_ce_fwd_bwd_weighted(const void* logits, const int64_t* labels, void* dlogits, float* partial, float* row_nll,
+                           const float* row_weight, float* stats, int M, int T, int V, int ldl, float num_items, float dloss,
+                           void* stream) {
+  SK_REQUIRE(logits && labels && partial && row_weight && stats && M > 0 && T > 0, "sk_ce_fwd_bwd_weighted: bad arguments");
+  return sk_ce_launch(CBF(logits), labels, BF(dlogits), partial, row_nll, stats, M, T, V, ldl, num_items, dloss, S(stream),
+                      row_weight);
+}
+int sk_ce_chunk(const void* logits_chunk, const int64_t* labels, void* dlogits_chunk, float* partial, int row0, int rows,
+                int M, int T, int V, int ldl, float grad_scale, void* stream) {
+  SK_REQUIRE(logits_chunk && labels && partial && T > 0, "sk_ce_chunk: bad arguments");
+  return sk_ce_chunk_launch(CBF(logits_chunk), labels, BF(dlogits_chunk), partial, row0, rows, M, T, V, ldl, grad_scale,
+                            S(stream));
+}
+int sk_ce_finalize(const float* partial, int M, float num_items, float* stats, void* stream) {
+  SK_REQUIRE(partial && stats && M > 0, "sk_ce_finalize: bad arguments");
+  return sk_ce_finalize_launch(partial, M, num_items, stats, S(stream));
+}
+int sk_opt_pos_bwd(const int32_t* pos_ids, const void* dx, float* scratch, void* dP, int M, int T, int D, int n_pos,
+                   int accumulate, void* stream) {
+  SK_REQUIRE(dx && scratch && dP && M > 0, "sk_opt_pos_bwd: bad arguments");
+  return sk_opt_pos_bwd_launch(pos_ids, CBF(dx), scratch, BF(dP), M, T, D, n_pos, accumulate, S(stream));
+}
+int sk_relu_bwd(void* g, const void* a, int64_t n, void* stream) {
+  SK_REQUIRE(g && a && n > 0, "sk_relu_bwd: bad arguments");
+  return sk_relu_bwd_launch(BF(g), CBF(a), (long)n, S(stream));
+}
 int sk_attn_fwd(const void* q, const void* k, const void* v, void* o, float* lse, int B, int T, int H, int KVH, int ld,
                 int ldo, int causal, float scale, void* stream) {
   return sk_attn_fwd_launch(CBF(q), CBF(k), CBF(v), BF(o), lse, B, T, H, KVH, ld, ldo, causal, scale, S(stream));
@@ -336,6 +362,18 @@ int sk_grad_norm_f32(const float* grads, const int64_t* chunk_start, const int32
                      const int32_t* tensor_chunk_begin, int n_tensors, float* partial, float max_norm, float* stats, void* stream) {
   return sk_gradnorm_f32_launch(grads, reinterpret_cast<const long*>(chunk_start), chunk_len, n_chunks, tensor_chunk_begin,
                                 n_tensors, partial, max_norm, stats, S(stream));
+}
+int sk_table_bwd_f32(const int64_t* ids, const int32_t* pos_ids, const float* dx, float* scratch, float* dtable, const void* head,
+                     int M, int T, int D, int n_rows, int n_rows_padded, int keep, void* stream) {
+  SK_REQUIRE(dx && scratch && dtable && M > 0 && n_rows_padded >= n_rows && (n_rows_padded * (int64_t)D) % 4 == 0,
+             "sk_table_bwd_f32: bad arguments");
+  SK_REQUIRE(ids || !head, "sk_table_bwd_f32: the tied head gradient belongs to the token table (ids given)");
+  return sk_table_bwd_f32_launch(ids, pos_ids, dx, scratch, dtable, CBF(head), M, T, D, n_rows, n_rows_padded, keep, S(stream));
+}
+int sk_widen_grads(const void* g16, float* g32, const int64_t* chunk_start, const int32_t* chunk_len, int n_chunks, int keep,
+                   void* stream) {
+  SK_REQUIRE(g16 && g32 && chunk_start && chunk_len && n_chunks >= 0, "sk_widen_grads: bad arguments");
+  return sk_widen_grads_launch(CBF(g16), g32, reinterpret_cast<const long*>(chunk_start), chunk_len, n_chunks, keep, S(stream));
 }
 int sk_adamw_master_step(float* params, void* shadow, const float* grads, float* exp_avg, float* exp_avg_sq, int64_t n, float lr,
                          float beta1, float beta2, float eps, float weight_decay, int step, const float* clip_stats, void* stream) {

@@ -694,7 +694,8 @@ __global__ void gradnorm_finalize_kernel(const float* __restrict__ partial, cons
     if (max_norm > 0.f) {
       coef = max_norm / (total + 1e-6f);
       if (emulate_bf16) coef = bf16_round(coef);
-      coef = fminf(coef, 1.0f);
+      // torch.clamp(coef, max=1) keeps a NaN (a NaN gradient makes every gradient NaN); fminf would return 1
+      coef = coef > 1.0f ? 1.0f : coef;
     }
     out[0] = total;
     out[1] = coef;
@@ -1216,7 +1217,8 @@ __global__ void opt_pos_bwd_scatter_kernel(const int32_t* __restrict__ pos_ids, 
   }
 }
 
-// torch threshold_backward(grad, relu_out, 0): grad where the saved activation is > 0, else 0 (in place on grad)
+// torch threshold_backward(grad, relu_out, 0) = where(relu_out <= 0, 0, grad), in place on grad: a NaN activation passes
+// the gradient through, as autograd's ReLU backward does
 __global__ void relu_bwd_kernel(bf16* __restrict__ g, const bf16* __restrict__ a, long n) {
   griddep_launch();
   griddep_wait();
@@ -1228,7 +1230,7 @@ __global__ void relu_bwd_kernel(bf16* __restrict__ g, const bf16* __restrict__ a
 #pragma unroll
     for (int k = 0; k < 4; ++k) {
       const float2 fa = unpack_bf16(au[k]);
-      o[k] = (fa.x > 0.f ? (gu[k] & 0xffffu) : 0u) | (fa.y > 0.f ? (gu[k] & 0xffff0000u) : 0u);
+      o[k] = (fa.x <= 0.f ? 0u : (gu[k] & 0xffffu)) | (fa.y <= 0.f ? 0u : (gu[k] & 0xffff0000u));
     }
     stg128(g + i, make_uint4(o[0], o[1], o[2], o[3]));
   }

@@ -1942,6 +1942,17 @@ int sk_lm_set_master(SkLm* lm, float* params32, float* grads32) {
   return 0;
 }
 
+int sk_lm_widen_chunks(const SkLm* lm, int64_t* chunk_start, int32_t* chunk_len, int cap) {
+  SK_REQUIRE(lm && chunk_start && chunk_len, "sk_lm_widen_chunks: null argument");
+  SK_REQUIRE(lm->d_widen_start, "sk_lm_widen_chunks: the handle has no master weights (sk_lm_set_master)");
+  SK_REQUIRE(cap >= lm->n_widen, "sk_lm_widen_chunks: %d chunks do not fit in %d", lm->n_widen, cap);
+  std::vector<long> cs(lm->n_widen);
+  SK_CUDA_CHECK(cudaMemcpy(cs.data(), lm->d_widen_start, cs.size() * sizeof(long), cudaMemcpyDeviceToHost));
+  SK_CUDA_CHECK(cudaMemcpy(chunk_len, lm->d_widen_len, (size_t)lm->n_widen * sizeof(int), cudaMemcpyDeviceToHost));
+  for (int i = 0; i < lm->n_widen; ++i) chunk_start[i] = (int64_t)cs[i];
+  return lm->n_widen;
+}
+
 int64_t sk_lm_fp32_prepared_bytes(const SkLm* lm) { return lm ? 2 * align_up(lm->n_params * 2, 256) : 0; }
 
 int sk_lm_set_fp32(SkLm* lm, const float* params32, void* prepared, int64_t prepared_bytes, void* stream) {
