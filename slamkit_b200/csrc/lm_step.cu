@@ -24,12 +24,9 @@ struct TensorDesc {
 struct LayerOff {
   int64_t ln1, wqkv, bqkv, wo, ln2, wgu, wd;
 };
-// OPT decoder layer (HF OPTDecoderLayer, do_layer_norm_before = True): every linear has a bias, q|k|v fused as in Qwen2
-struct OptLayerOff {
-  int64_t ln1w, ln1b, wqkv, bqkv, wo, bo, ln2w, ln2b, w1, b1, w2, b2;
-};
-// GPT-NeoX layer (HF GPTNeoXLayer, use_parallel_residual = True): two LayerNorms of the same input, biased linears
-struct NeoxLayerOff {
+// LayerNorm decoder layer: OPT (HF OPTDecoderLayer) and GPT-NeoX (HF GPTNeoXLayer, use_parallel_residual = True).  Two
+// affine LayerNorms and biased linears, q|k|v fused as in Qwen2; each architecture registers them in its own order.
+struct LnLayerOff {
   int64_t ln1w, ln1b, ln2w, ln2b, wqkv, bqkv, wo, bo, w1, b1, w2, b2;
 };
 enum { SK_ARCH_QWEN2 = 0, SK_ARCH_OPT = 1, SK_ARCH_NEOX = 2 };
@@ -45,13 +42,14 @@ struct WsLayout {
 }  // namespace
 
 struct SkLm {
-  SkLmConfig cfg;      // OPT handles fill it too (n_kv_heads = n_heads, rms_eps = the LayerNorm eps): shape checks are shared
   int arch = SK_ARCH_QWEN2;
   int d, F, H, KVH, hd, L, V, Vp, qkv_dim;
+  int max_pos;                    // rows of the RoPE tables (Qwen2, GPT-NeoX) or OPT's max_position_embeddings
+  float eps;                      // RMSNorm (Qwen2) or LayerNorm eps
+  bool tie, qkv_bias;             // lm_head shares the token table; q|k|v projection has a bias
   std::vector<TensorDesc> tensors;
-  std::vector<LayerOff> lo;
-  std::vector<OptLayerOff> olo;   // OPT layers
-  std::vector<NeoxLayerOff> nlo;  // GPT-NeoX layers
+  std::vector<LayerOff> lo;       // Qwen2 layers
+  std::vector<LnLayerOff> lnl;    // OPT and GPT-NeoX layers
   int rot = 64;                   // GPT-NeoX: rotated columns per q / k head (rotary_ndims)
   int64_t off_final_norm_b = 0, off_pos = 0;
   int n_pos = 0;                  // OPT: rows of the learned position table (max_positions + 2)
@@ -104,6 +102,13 @@ int64_t add_tensor(SkLm* lm, const std::string& name, int rows, int cols) {
   return off;
 }
 
+// Workspace plan of the bf16 and master-weight paths, one set of per-layer slabs per saved activation.  Qwen2: rstd
+// slabs hold the RMSNorm rstd, `gu` gate|up [M, 2F] and `act` the SwiGLU output.  OPT: rstd slabs hold the LayerNorm
+// mean then rstd (fp32 [2][M]), `gu` the ReLU output a = relu(fc1) [M, F] that fc2 and the ReLU backward read, `dgu`
+// its gradient; `act` is unused.  GPT-NeoX: rstd1 slabs hold the shared mean then rstd of the two LayerNorms, h1 / h2
+// their outputs, `gu` the pre-activation of dense_h_to_4h [M, F] and `act` its GELU; `xmid` is one [M, d] slab for the
+// attention branch's output (read once, by the same layer's dense_4h_to_h epilogue); rstd2 is unused.  Unused slots
+// take 0 bytes.
 WsLayout make_layout(const SkLm* lm, int B, int T) {
   WsLayout w;
   const int64_t M = (int64_t)B * T;
@@ -114,26 +119,28 @@ WsLayout make_layout(const SkLm* lm, int B, int T) {
     return o;
   };
   const int L = lm->L;
+  const bool qwen2 = lm->arch == SK_ARCH_QWEN2, opt = lm->arch == SK_ARCH_OPT, neox = lm->arch == SK_ARCH_NEOX;
   w.sX = align_up(M * lm->d * 2, 256);
   w.sh = w.sX;
-  w.srstd = align_up(M * 4, 256);
+  w.srstd = align_up(M * (qwen2 ? 4 : 8), 256);
   w.sqkv = align_up(M * lm->qkv_dim * 2, 256);
   w.slse = align_up((int64_t)B * lm->H * T * 4, 256);
-  w.sgu = align_up(M * 2 * lm->F * 2, 256);
-  w.sact = align_up(M * lm->F * 2, 256);
+  w.sgu = align_up(M * (qwen2 ? 2 : 1) * lm->F * 2, 256);
+  w.sact = opt ? 0 : align_up(M * lm->F * 2, 256);
+  w.sR = lm->master ? align_up(M * lm->d * 4, 256) : w.sX;   // master weights: the residual stream is fp32
   // GEMM scratch first: its offset (and the stream-K flag words in its last 4 KB, zeroed by sk_lm_bind) must not move
   // with (B, T).  Sized for 8 fp32 slabs of the largest split-K wgrad and for the stream-K partial tiles.
   w.splitk_bytes = align_up(std::max<int64_t>((int64_t)8 * lm->qkv_dim * lm->d * 4, (int64_t)sk_gemm_ws_min_bytes()) + 4096, 256);
   w.splitk = take(w.splitk_bytes);
-  w.X = take(w.sX * (L + 1));
+  w.X = take(w.sR * (L + 1));
   w.h1 = take(w.sh * L);
   w.rstd1 = take(w.srstd * L);
   w.qkv = take(w.sqkv * L);
   w.ao = take(w.sX * L);
   w.lse = take(w.slse * L);
-  w.xmid = take(w.sX * L);
+  w.xmid = take(neox ? w.sX : w.sR * L);
   w.h2 = take(w.sh * L);
-  w.rstd2 = take(w.srstd * L);
+  w.rstd2 = take(neox ? 0 : w.srstd * L);
   w.gu = take(w.sgu * L);
   w.act = take(w.sact * L);
   w.hf = take(w.sX);
@@ -149,12 +156,18 @@ WsLayout make_layout(const SkLm* lm, int B, int T) {
   w.dqkv = take(w.sqkv);
   w.dgu = take(w.sgu);
   w.delta = take(w.slse);
-  w.dw_partial = take((int64_t)sk_rmsnorm_bwd_blocks() * lm->d * 4);
-  w.colsum_partial = take((int64_t)sk_colsum_splits() * lm->qkv_dim * 4);
+  // RMSNorm weight partials; LayerNorm weight and bias partials (OPT), the dual LayerNorm's four (GPT-NeoX)
+  w.dw_partial = take(qwen2 ? (int64_t)sk_rmsnorm_bwd_blocks() * lm->d * 4
+                            : (int64_t)(opt ? 2 : 4) * sk_layernorm_bwd_blocks() * lm->d * 4);
+  w.colsum_partial = take((int64_t)sk_colsum_splits() * (qwen2 ? lm->qkv_dim : std::max(lm->qkv_dim, lm->F)) * 4);
   w.ce_partial = take((int64_t)sk_ce_blocks((int)M) * 2 * 4);
-  w.embed_scratch = take((int64_t)lm->Vp * lm->d * 8);   // 64-bit fixed-point accumulators of the embedding gradient
+  // 64-bit fixed-point accumulators of the embedding gradient; OPT's token and position tables share them, their
+  // gradients are formed one after the other
+  w.embed_scratch = take((int64_t)std::max(lm->Vp, lm->n_pos) * lm->d * 8);
   w.seg_start = take(M * 4);   // document bounds of packed batches (position_ids given), int32 per token
   w.seg_end = take(M * 4);
+  if (lm->master) w.dres32 = take(w.sR);
+  if (lm->proj) w.pe = take(M * lm->pw * 2);
   w.total = cur;
   return w;
 }
@@ -200,34 +213,74 @@ int linear_wgrad(int M, int N, int K, const bf16* dy, const bf16* x, bf16* dW, i
 int linear_qkv_rope(const SkLm* lm, int M, int T, const bf16* x, const bf16* W, const bf16* bias, bf16* qkv,
                     const int32_t* pos_ids, cudaStream_t s) {
   return sk_linear_rope_launch(M, lm->qkv_dim, lm->d, x, W, bias, qkv, lm->rope_cos, lm->rope_sin, pos_ids, T,
-                               (lm->H + lm->KVH) * lm->hd, lm->cfg.max_positions, s);
+                               (lm->H + lm->KVH) * lm->hd, lm->max_pos, s);
 }
 
 int check_bound(const SkLm* lm, int B, int T, const WsLayout& w, const int32_t* pos_ids) {
   SK_REQUIRE(lm->params && lm->ws, "sk_lm: sk_lm_bind has not been called");
   // a packed row (position_ids given) may be longer than the RoPE tables: positions restart per document
-  SK_REQUIRE(B > 0 && T > 0 && (T <= lm->cfg.max_positions || pos_ids != nullptr),
-             "sk_lm: bad batch shape B=%d T=%d (max_positions=%d; longer rows need position_ids)", B, T, lm->cfg.max_positions);
+  SK_REQUIRE(B > 0 && T > 0 && (T <= lm->max_pos || pos_ids != nullptr),
+             "sk_lm: bad batch shape B=%d T=%d (max_positions=%d; longer rows need position_ids)", B, T, lm->max_pos);
   SK_REQUIRE(w.total <= lm->ws_bytes, "sk_lm: workspace too small: need %lld bytes, bound %lld", (long long)w.total,
              (long long)lm->ws_bytes);
   return 0;
 }
 
-int forward_impl(SkLm* lm, const int64_t* ids, const int64_t* labels, const int32_t* pos_ids, int B, int T,
-                 float num_items, float dloss, bool want_dlogits, float* stats, const WsLayout& w, cudaStream_t s,
-                 float* row_nll = nullptr, bool with_head = true) {
-  const int M = B * T, d = lm->d, F = lm->F, L = lm->L;
+// One pass over a batch: what the forward computes and, for the backward, which batch it differentiates
+struct FwdArgs {
+  const int64_t* ids;
+  const int64_t* labels;      // nullptr: logits only
+  const int32_t* pos_ids;     // packed batch, or nullptr
+  int B, T;
+  float num_items = 0.f, dloss = 1.f;
+  bool want_dlogits = false;  // the CE writes the logit gradient for the backward pass
+  float* stats = nullptr;
+  float* row_nll = nullptr;
+  bool with_head = true;      // false: stop at the lm_head's input (chunked head, prefill)
+  // fp32 prefill: the fp32 cache of T_cache positions that receives the K / V of positions < lens[b]
+  float* kv = nullptr;
+  const int32_t* lens = nullptr;
+  int T_cache = 0;
+};
+
+// packed batch (position_ids given): document bounds -> block-diagonal causal attention, as the reference's varlen
+// flash-attention path does (slamkit/data/hf_dataset.py:61-62 + HF prepare_fa_kwargs_from_position_ids)
+int seg_bounds(const SkLm* lm, const FwdArgs& a, const WsLayout& w, cudaStream_t s) {
+  if (!a.pos_ids) return 0;
+  return sk_seg_bounds_launch(a.pos_ids, wsp<int32_t>(lm, w.seg_start), wsp<int32_t>(lm, w.seg_end), a.B, a.T, s);
+}
+const int* seg_ptr(const SkLm* lm, const FwdArgs& a, int64_t off) { return a.pos_ids ? wsp<int32_t>(lm, off) : nullptr; }
+
+// lm_head on the rows hin [M, K] and, with labels, compute_loss; records the batch shape for the logits and backward
+int head_forward(SkLm* lm, const WsLayout& w, const FwdArgs& a, const bf16* hin, int K, cudaStream_t s) {
+  lm->last_B = a.B;
+  lm->last_T = a.T;
+  if (!a.with_head) return 0;
+  const int M = a.B * a.T;
+  bf16* logits = wsp<bf16>(lm, w.logits);
+  SK_TRY(linear_fwd(M, lm->Vp, K, hin, lm->params + lm->off_head, logits, nullptr, nullptr, s));
+  if (!a.labels) return 0;
+  return sk_ce_launch(logits, a.labels, a.want_dlogits ? wsp<bf16>(lm, w.dlogits) : nullptr, wsp<float>(lm, w.ce_partial),
+                      a.row_nll, a.stats, M, a.T, lm->V, lm->Vp, a.num_items, a.dloss, s);
+}
+
+// the lm_head's backward from dlogits: its input gradient into dst [M, K], its weight gradient (+)= into the head
+int head_backward(SkLm* lm, const WsLayout& w, int M, bf16* dst, const bf16* hin, int K, int accumulate, cudaStream_t s) {
+  const bf16* dlogits = wsp<bf16>(lm, w.dlogits);
+  SK_TRY(linear_dgrad(M, lm->Vp, K, dlogits, lm->params + lm->off_head, dst, s));
+  return linear_wgrad(M, lm->Vp, K, dlogits, hin, lm->grads + lm->off_head, accumulate, s, lm->ws + w.splitk,
+                      (size_t)w.splitk_bytes);
+}
+
+int qwen2_forward(SkLm* lm, const FwdArgs& a, const WsLayout& w, cudaStream_t s) {
+  const int B = a.B, T = a.T, M = B * T, d = lm->d, F = lm->F, L = lm->L;
+  const int32_t* pos_ids = a.pos_ids;
   const bf16* P = lm->params;
   bf16* X0 = wsp<bf16>(lm, w.X);
-  SK_TRY(sk_embed_fwd_launch(ids, P + lm->off_embed, X0, M, d, lm->V, s));
+  SK_TRY(sk_embed_fwd_launch(a.ids, P + lm->off_embed, X0, M, d, lm->V, s));
   const float scale = 1.0f / sqrtf((float)lm->hd);
-  // packed batch (position_ids given): document bounds -> block-diagonal causal attention, as the reference's varlen
-  // flash-attention path does (slamkit/data/hf_dataset.py:61-62 + HF prepare_fa_kwargs_from_position_ids)
-  const int* seg_start = nullptr;
-  if (pos_ids) {
-    SK_TRY(sk_seg_bounds_launch(pos_ids, wsp<int32_t>(lm, w.seg_start), wsp<int32_t>(lm, w.seg_end), B, T, s));
-    seg_start = wsp<int32_t>(lm, w.seg_start);
-  }
+  SK_TRY(seg_bounds(lm, a, w, s));
+  const int* seg_start = seg_ptr(lm, a, w.seg_start);
   for (int l = 0; l < L; ++l) {
     const LayerOff& o = lm->lo[l];
     bf16* x = wsp<bf16>(lm, w.X + w.sX * l);
@@ -243,27 +296,18 @@ int forward_impl(SkLm* lm, const int64_t* ids, const int64_t* labels, const int3
     bf16* gu = wsp<bf16>(lm, w.gu + w.sgu * l);
     bf16* act = wsp<bf16>(lm, w.act + w.sact * l);
 
-    SK_TRY(sk_rmsnorm_fwd_launch(x, P + o.ln1, h1, r1, M, d, lm->cfg.rms_eps, s));
-    SK_TRY(linear_qkv_rope(lm, M, T, h1, P + o.wqkv, lm->cfg.qkv_bias ? P + o.bqkv : nullptr, qkv, pos_ids, s));
+    SK_TRY(sk_rmsnorm_fwd_launch(x, P + o.ln1, h1, r1, M, d, lm->eps, s));
+    SK_TRY(linear_qkv_rope(lm, M, T, h1, P + o.wqkv, lm->qkv_bias ? P + o.bqkv : nullptr, qkv, pos_ids, s));
     SK_TRY(sk_attn_tc_fwd_launch(qkv, ao, lse, B, T, lm->H, lm->KVH, lm->qkv_dim, d, 1, scale, s, seg_start));
     SK_TRY(linear_fwd(M, d, d, ao, P + o.wo, xmid, nullptr, x, s));
-    SK_TRY(sk_rmsnorm_fwd_launch(xmid, P + o.ln2, h2, r2, M, d, lm->cfg.rms_eps, s));
+    SK_TRY(sk_rmsnorm_fwd_launch(xmid, P + o.ln2, h2, r2, M, d, lm->eps, s));
     SK_TRY(sk_linear_swiglu_fwd_launch(M, F, d, h2, P + o.wgu, gu, act, s));
     SK_TRY(linear_fwd(M, d, F, act, P + o.wd, xn, nullptr, xmid, s));
   }
   bf16* xL = wsp<bf16>(lm, w.X + w.sX * L);
   bf16* hf = wsp<bf16>(lm, w.hf);
-  SK_TRY(sk_rmsnorm_fwd_launch(xL, P + lm->off_final_norm, hf, wsp<float>(lm, w.rstdf), M, d, lm->cfg.rms_eps, s));
-  lm->last_B = B;
-  lm->last_T = T;
-  if (!with_head) return 0;
-  bf16* logits = wsp<bf16>(lm, w.logits);
-  SK_TRY(linear_fwd(M, lm->Vp, d, hf, P + lm->off_head, logits, nullptr, nullptr, s));
-  if (labels) {
-    SK_TRY(sk_ce_launch(logits, labels, want_dlogits ? wsp<bf16>(lm, w.dlogits) : nullptr, wsp<float>(lm, w.ce_partial),
-                        row_nll, stats, M, T, lm->V, lm->Vp, num_items, dloss, s));
-  }
-  return 0;
+  SK_TRY(sk_rmsnorm_fwd_launch(xL, P + lm->off_final_norm, hf, wsp<float>(lm, w.rstdf), M, d, lm->eps, s));
+  return head_forward(lm, w, a, hf, d, s);
 }
 
 // lm_head + compute_loss + their backward for text+unit vocabularies (~152 k columns; BASELINE cfg-4), in row chunks:
@@ -272,10 +316,9 @@ int forward_impl(SkLm* lm, const int64_t* ids, const int64_t* labels, const int3
 // moves through HBM as in the one-pass form; the price is one read-modify-write of dE per extra chunk.  (A fully fused
 // "flash" CE would recompute the logits GEMM in the backward pass -- 2.2 TFLOP at this shape, more time than the 7.5 GB
 // of logits traffic it removes.)  The sums per row meet in `ce_partial`, finalised once.
-int head_chunked(SkLm* lm, const int64_t* labels, int B, int T, float num_items, float dloss, int accumulate, float* stats,
-                 const WsLayout& w, cudaStream_t s) {
-  const int M = B * T, d = head_k(lm);
-  SK_REQUIRE(num_items > 0.f, "sk_lm: training with a large vocabulary needs num_items_in_batch (the 'sum / num_items' loss of "
+int head_chunked(SkLm* lm, const FwdArgs& a, int accumulate, const WsLayout& w, cudaStream_t s) {
+  const int M = a.B * a.T, d = head_k(lm);
+  SK_REQUIRE(a.num_items > 0.f, "sk_lm: training with a large vocabulary needs num_items_in_batch (the 'sum / num_items' loss of "
                               "slamkit/model/unit_lm.py:26-28): the gradient scale must be known before the first chunk");
   const bf16* P = lm->params;
   bf16* G = lm->grads;
@@ -284,21 +327,21 @@ int head_chunked(SkLm* lm, const int64_t* labels, int B, int T, float num_items,
   bf16* dh = wsp<bf16>(lm, lm->post_ln && !lm->proj ? w.dxA : w.dh);
   bf16* chunk = wsp<bf16>(lm, w.logits);
   float* partial = wsp<float>(lm, w.ce_partial);
-  const float gs = dloss / num_items;
+  const float gs = a.dloss / a.num_items;
   for (int r0 = 0; r0 < M; r0 += lm->head_chunk) {
     const int rows = std::min(lm->head_chunk, M - r0);
     SK_TRY(linear_fwd(rows, lm->Vp, d, hf + (size_t)r0 * d, P + lm->off_head, chunk, nullptr, nullptr, s));
-    SK_TRY(sk_ce_chunk_launch(chunk, labels, chunk, partial, r0, rows, M, T, lm->V, lm->Vp, gs, s));
+    SK_TRY(sk_ce_chunk_launch(chunk, a.labels, chunk, partial, r0, rows, M, a.T, lm->V, lm->Vp, gs, s));
     SK_TRY(linear_dgrad(rows, lm->Vp, d, chunk, P + lm->off_head, dh + (size_t)r0 * d, s));
     SK_TRY(linear_wgrad(rows, lm->Vp, d, chunk, hf + (size_t)r0 * d, G + lm->off_head, (accumulate || r0 > 0) ? 1 : 0, s,
                         lm->ws + w.splitk, (size_t)w.splitk_bytes));
   }
-  return sk_ce_finalize_launch(partial, M, num_items, stats, s);
+  return sk_ce_finalize_launch(partial, M, a.num_items, a.stats, s);
 }
 
-int backward_impl(SkLm* lm, const int64_t* ids, const int32_t* pos_ids, int B, int T, int accumulate,
-                  const WsLayout& w, cudaStream_t s, bool with_head = true) {
-  const int M = B * T, d = lm->d, F = lm->F, L = lm->L, Q = lm->qkv_dim;
+int qwen2_backward(SkLm* lm, const FwdArgs& a, int accumulate, const WsLayout& w, cudaStream_t s) {
+  const int B = a.B, T = a.T, M = B * T, d = lm->d, F = lm->F, L = lm->L, Q = lm->qkv_dim;
+  const int32_t* pos_ids = a.pos_ids;
   const bf16* P = lm->params;
   bf16* G = lm->grads;
   float* dwp = wsp<float>(lm, w.dw_partial);
@@ -308,15 +351,10 @@ int backward_impl(SkLm* lm, const int64_t* ids, const int32_t* pos_ids, int B, i
   bf16* dao = wsp<bf16>(lm, w.dao);
   bf16* dqkv = wsp<bf16>(lm, w.dqkv);
   bf16* dgu = wsp<bf16>(lm, w.dgu);
-  bf16* dlogits = wsp<bf16>(lm, w.dlogits);
-  bf16* hf = wsp<bf16>(lm, w.hf);
   const float scale = 1.0f / sqrtf((float)lm->hd);
 
   // lm_head (already done chunk by chunk for large vocabularies)
-  if (with_head) {
-    SK_TRY(linear_dgrad(M, lm->Vp, d, dlogits, P + lm->off_head, dh, s));
-    SK_TRY(linear_wgrad(M, lm->Vp, d, dlogits, hf, G + lm->off_head, accumulate, s, lm->ws + w.splitk, (size_t)w.splitk_bytes));
-  }
+  if (a.with_head) SK_TRY(head_backward(lm, w, M, dh, wsp<bf16>(lm, w.hf), d, accumulate, s));
   SK_TRY(sk_rmsnorm_bwd_launch(dh, wsp<bf16>(lm, w.X + w.sX * L), P + lm->off_final_norm, wsp<float>(lm, w.rstdf),
                                nullptr, dxA, G + lm->off_final_norm, dwp, M, d, accumulate, s));
   if (!lm->bwd_events.empty()) SK_CUDA_CHECK(cudaEventRecord(lm->bwd_events[L], s));
@@ -344,10 +382,10 @@ int backward_impl(SkLm* lm, const int64_t* ids, const int32_t* pos_ids, int B, i
     SK_TRY(linear_dgrad(M, d, d, dxB, P + o.wo, dao, s));
     SK_TRY(linear_wgrad(M, d, d, dxB, ao, G + o.wo, accumulate, s, lm->ws + w.splitk, (size_t)w.splitk_bytes));
     SK_TRY(sk_attn_tc_bwd_launch(qkv, ao, dao, lse, wsp<float>(lm, w.delta), nullptr, dqkv, B, T,
-                                 lm->H, lm->KVH, Q, d, Q, 1, scale, s, pos_ids ? wsp<int32_t>(lm, w.seg_start) : nullptr,
-                                 pos_ids ? wsp<int32_t>(lm, w.seg_end) : nullptr, lm->rope_cos, lm->rope_sin, pos_ids,
-                                 lm->cfg.max_positions));   // inverse RoPE on dq / dk applied after the attention backward
-    if (lm->cfg.qkv_bias)
+                                 lm->H, lm->KVH, Q, d, Q, 1, scale, s, seg_ptr(lm, a, w.seg_start), seg_ptr(lm, a, w.seg_end),
+                                 lm->rope_cos, lm->rope_sin, pos_ids,
+                                 lm->max_pos));   // inverse RoPE on dq / dk applied after the attention backward
+    if (lm->qkv_bias)
       SK_TRY(sk_colsum_launch(dqkv, G + o.bqkv, wsp<float>(lm, w.colsum_partial), M, Q, Q, accumulate, s));
     SK_TRY(linear_dgrad(M, Q, d, dqkv, P + o.wqkv, dh, s));
     SK_TRY(linear_wgrad(M, Q, d, dqkv, h1, G + o.wqkv, accumulate, s, lm->ws + w.splitk, (size_t)w.splitk_bytes));
@@ -355,9 +393,8 @@ int backward_impl(SkLm* lm, const int64_t* ids, const int32_t* pos_ids, int B, i
     if (!lm->bwd_events.empty()) SK_CUDA_CHECK(cudaEventRecord(lm->bwd_events[l], s));
   }
   // embedding: tied -> add on top of the lm_head gradient just written; untied -> honour `accumulate`
-  SK_TRY(sk_embed_bwd_launch(ids, dxA, wsp<float>(lm, w.embed_scratch), G + lm->off_embed, M, d, lm->V, lm->Vp,
-                             lm->cfg.tie_embeddings ? 1 : accumulate, s));
-  return 0;
+  return sk_embed_bwd_launch(a.ids, dxA, wsp<float>(lm, w.embed_scratch), G + lm->off_embed, M, d, lm->V, lm->Vp,
+                             lm->tie ? 1 : accumulate, s);
 }
 
 // byte offsets into the decode workspace for (B, T_cache): one token per row
@@ -398,8 +435,8 @@ int check_decode(const SkLm* lm, int B, int T_cache, int ldl, const void* kv_cac
                  int64_t ws_bytes, const DecLayout& w) {
   SK_REQUIRE(lm->params && lm->ws, "sk_lm: sk_lm_bind has not been called");
   SK_REQUIRE(kv_cache && logits && ws, "sk_lm decode: null argument");
-  SK_REQUIRE(B > 0 && T_cache > 0 && T_cache <= lm->cfg.max_positions, "sk_lm decode: bad shape B=%d T_cache=%d (max_positions=%d)",
-             B, T_cache, lm->cfg.max_positions);
+  SK_REQUIRE(B > 0 && T_cache > 0 && T_cache <= lm->max_pos, "sk_lm decode: bad shape B=%d T_cache=%d (max_positions=%d)",
+             B, T_cache, lm->max_pos);
   SK_REQUIRE(ldl >= lm->Vp && ldl % 8 == 0, "sk_lm decode: ldl must be >= %d and a multiple of 8 (got %d)", lm->Vp, ldl);
   SK_REQUIRE(((uintptr_t)ws & 255) == 0 && ((uintptr_t)kv_cache & 15) == 0 && ((uintptr_t)logits & 15) == 0,
              "sk_lm decode: decode workspace must be 256-byte, cache and logits 16-byte aligned");
@@ -408,121 +445,26 @@ int check_decode(const SkLm* lm, int B, int T_cache, int ldl, const void* kv_cac
   return 0;
 }
 
+// the decode workspace's slots as typed pointers (fp32 inference: each hi half, its lo half right after it)
+struct DecBufs {
+  bf16 *x0, *x1, *h, *qkv, *ao, *gu, *act;
+  int32_t* lens;
+  float* partial;
+  float* e32;
+  void* gemm;
+  size_t gemm_bytes;
+};
+
+DecBufs dec_bufs(void* ws, const DecLayout& dl) {
+  uint8_t* p = reinterpret_cast<uint8_t*>(ws);
+  auto b16 = [&](int64_t off) { return reinterpret_cast<bf16*>(p + off); };
+  return DecBufs{b16(dl.x0), b16(dl.x1), b16(dl.h), b16(dl.qkv), b16(dl.ao), b16(dl.gu), b16(dl.act),
+                 reinterpret_cast<int32_t*>(p + dl.lens), reinterpret_cast<float*>(p + dl.partial),
+                 reinterpret_cast<float*>(p + dl.e32), p + dl.gemm, (size_t)dl.gemm_bytes};
+}
+
 // ---- OPT decoder (HF:models/opt/modeling_opt.py:45-70 positions, :100-182 attention, :185-260 decoder layer,
-// :480-560 decoder).  Separate functions from the Qwen2 ones above; the entry points below pick one by lm->arch.
-
-// The Qwen2 workspace plan with OPT's tensors: rstd slabs hold the LayerNorm mean then rstd (fp32 [2][M]), `gu` holds
-// the ReLU output a = relu(fc1) [M, F] that fc2 and the ReLU backward read, `dgu` its gradient; `act` is unused.
-WsLayout make_opt_layout(const SkLm* lm, int B, int T) {
-  WsLayout w;
-  const int64_t M = (int64_t)B * T;
-  int64_t cur = 0;
-  auto take = [&](int64_t bytes) {
-    const int64_t o = cur;
-    cur = align_up(cur + bytes, 256);
-    return o;
-  };
-  const int L = lm->L;
-  w.sX = align_up(M * lm->d * 2, 256);
-  w.sh = w.sX;
-  w.srstd = align_up(M * 8, 256);
-  w.sqkv = align_up(M * lm->qkv_dim * 2, 256);
-  w.slse = align_up((int64_t)B * lm->H * T * 4, 256);
-  w.sgu = align_up(M * lm->F * 2, 256);
-  w.sact = 0;
-  w.sR = lm->master ? align_up(M * lm->d * 4, 256) : w.sX;   // master weights: the residual stream is fp32
-  // GEMM scratch first, at the same fixed offset as in make_layout (sk_lm_bind clears its flag words once)
-  w.splitk_bytes = align_up(std::max<int64_t>((int64_t)8 * lm->qkv_dim * lm->d * 4, (int64_t)sk_gemm_ws_min_bytes()) + 4096, 256);
-  w.splitk = take(w.splitk_bytes);
-  w.X = take(w.sR * (L + 1));
-  w.h1 = take(w.sh * L);
-  w.rstd1 = take(w.srstd * L);
-  w.qkv = take(w.sqkv * L);
-  w.ao = take(w.sX * L);
-  w.lse = take(w.slse * L);
-  w.xmid = take(w.sR * L);
-  w.h2 = take(w.sh * L);
-  w.rstd2 = take(w.srstd * L);
-  w.gu = take(w.sgu * L);
-  w.act = 0;
-  w.hf = take(w.sX);
-  w.rstdf = take(w.srstd);
-  w.logits = take(M * lm->Vp * 2);
-  w.dlogits = lm->head_chunk > 0 ? w.logits : take(M * lm->Vp * 2);
-  w.dxA = take(w.sX);
-  w.dxB = take(w.sX);
-  w.dh = take(w.sX);
-  w.dao = take(w.sX);
-  w.dqkv = take(w.sqkv);
-  w.dgu = take(w.sgu);
-  w.delta = take(w.slse);
-  w.dw_partial = take((int64_t)2 * sk_layernorm_bwd_blocks() * lm->d * 4);   // LayerNorm weight and bias partials
-  w.colsum_partial = take((int64_t)sk_colsum_splits() * std::max(lm->qkv_dim, lm->F) * 4);
-  w.ce_partial = take((int64_t)sk_ce_blocks((int)M) * 2 * 4);
-  // token and position tables share the fixed-point scratch: their gradients are formed one after the other
-  w.embed_scratch = take((int64_t)std::max(lm->Vp, lm->n_pos) * lm->d * 8);
-  w.seg_start = take(M * 4);
-  w.seg_end = take(M * 4);
-  if (lm->master) w.dres32 = take(w.sR);
-  if (lm->proj) w.pe = take(M * lm->pw * 2);
-  w.total = cur;
-  return w;
-}
-
-// GPT-NeoX: rstd1 slabs hold the shared mean then rstd of the two LayerNorms (fp32 [2][M]), h1 / h2 their outputs,
-// `gu` the pre-activation of dense_h_to_4h [M, F] and `act` its GELU; `xmid` is one [M, d] slab for the attention
-// branch's output (read once, by the same layer's dense_4h_to_h epilogue); rstd2 is unused.
-WsLayout make_neox_layout(const SkLm* lm, int B, int T) {
-  WsLayout w;
-  const int64_t M = (int64_t)B * T;
-  int64_t cur = 0;
-  auto take = [&](int64_t bytes) {
-    const int64_t o = cur;
-    cur = align_up(cur + bytes, 256);
-    return o;
-  };
-  const int L = lm->L;
-  w.sX = align_up(M * lm->d * 2, 256);
-  w.sh = w.sX;
-  w.srstd = align_up(M * 8, 256);
-  w.sqkv = align_up(M * lm->qkv_dim * 2, 256);
-  w.slse = align_up((int64_t)B * lm->H * T * 4, 256);
-  w.sgu = align_up(M * lm->F * 2, 256);
-  w.sact = w.sgu;
-  // GEMM scratch first, at the same fixed offset as in make_layout (sk_lm_bind clears its flag words once)
-  w.splitk_bytes = align_up(std::max<int64_t>((int64_t)8 * lm->qkv_dim * lm->d * 4, (int64_t)sk_gemm_ws_min_bytes()) + 4096, 256);
-  w.splitk = take(w.splitk_bytes);
-  w.X = take(w.sX * (L + 1));
-  w.h1 = take(w.sh * L);
-  w.rstd1 = take(w.srstd * L);
-  w.qkv = take(w.sqkv * L);
-  w.ao = take(w.sX * L);
-  w.lse = take(w.slse * L);
-  w.xmid = take(w.sX);
-  w.h2 = take(w.sh * L);
-  w.rstd2 = 0;
-  w.gu = take(w.sgu * L);
-  w.act = take(w.sact * L);
-  w.hf = take(w.sX);
-  w.rstdf = take(w.srstd);
-  w.logits = take(M * lm->Vp * 2);
-  w.dlogits = lm->head_chunk > 0 ? w.logits : take(M * lm->Vp * 2);
-  w.dxA = take(w.sX);
-  w.dxB = take(w.sX);
-  w.dh = take(w.sX);
-  w.dao = take(w.sX);
-  w.dqkv = take(w.sqkv);
-  w.dgu = take(w.sgu);
-  w.delta = take(w.slse);
-  w.dw_partial = take((int64_t)4 * sk_layernorm_bwd_blocks() * lm->d * 4);   // the dual LayerNorm's four partials
-  w.colsum_partial = take((int64_t)sk_colsum_splits() * std::max(lm->qkv_dim, lm->F) * 4);
-  w.ce_partial = take((int64_t)sk_ce_blocks((int)M) * 2 * 4);
-  w.embed_scratch = take((int64_t)lm->Vp * lm->d * 8);
-  w.seg_start = take(M * 4);
-  w.seg_end = take(M * 4);
-  w.total = cur;
-  return w;
-}
+// :480-560 decoder).  Separate functions from the Qwen2 ones above; forward / backward / decode_step pick one.
 
 // OPT fp32 inference (forward only): every activation is a (hi, lo) bf16 pair [M, cols], lo at hi + the slab stride
 // (sX, sqkv, sgu); no per-layer copies.  X / xmid are the residual stream before / after the attention branch, h1 the
@@ -555,34 +497,28 @@ WsLayout make_opt_fp32_layout(const SkLm* lm, int B, int T) {
 }
 
 WsLayout layout_of(const SkLm* lm, int B, int T) {
-  if (lm->fp32) return make_opt_fp32_layout(lm, B, T);
-  if (lm->arch == SK_ARCH_NEOX) return make_neox_layout(lm, B, T);
-  return lm->arch == SK_ARCH_OPT ? make_opt_layout(lm, B, T) : make_layout(lm, B, T);
+  return lm->fp32 ? make_opt_fp32_layout(lm, B, T) : make_layout(lm, B, T);
 }
 
 // ---- GPT-NeoX decoder (HF:models/gpt_neox/modeling_gpt_neox.py: GPTNeoXAttention, GPTNeoXMLP, GPTNeoXLayer with
-// use_parallel_residual = True, GPTNeoXModel, GPTNeoXForCausalLM).  Separate functions, picked by lm->arch.
+// use_parallel_residual = True, GPTNeoXModel, GPTNeoXForCausalLM).  Separate functions, picked as above.
 //   h1 = LN1(x), h2 = LN2(x)              one dual-LayerNorm launch, shared mean / rstd
 //   qkv = h1 Wqkv + b, partial RoPE       the RoPE epilogue with rot columns per head (weights in [Q;K;V] row order)
 //   attn = attention(qkv) Wo + bo
 //   pre = h2 W1 + b1, act = gelu(pre)     one epilogue, two outputs
 //   x' = bf16(bf16(act W2 + b2 + attn) + x)   the two-residual epilogue, HF's order `mlp + attn + hidden_states`
-int neox_forward(SkLm* lm, const int64_t* ids, const int64_t* labels, const int32_t* pos_ids, int B, int T, float num_items,
-                 float dloss, bool want_dlogits, float* stats, const WsLayout& w, cudaStream_t s, float* row_nll = nullptr,
-                 bool with_head = true) {
-  const int M = B * T, d = lm->d, F = lm->F, L = lm->L, Q = lm->qkv_dim;
-  const float eps = lm->cfg.rms_eps;
+int neox_forward(SkLm* lm, const FwdArgs& a, const WsLayout& w, cudaStream_t s) {
+  const int B = a.B, T = a.T, M = B * T, d = lm->d, F = lm->F, L = lm->L, Q = lm->qkv_dim;
+  const int32_t* pos_ids = a.pos_ids;
+  const float eps = lm->eps;
   const bf16* P = lm->params;
-  SK_TRY(sk_embed_fwd_launch(ids, P + lm->off_embed, wsp<bf16>(lm, w.X), M, d, lm->V, s));
+  SK_TRY(sk_embed_fwd_launch(a.ids, P + lm->off_embed, wsp<bf16>(lm, w.X), M, d, lm->V, s));
   const float scale = 1.0f / sqrtf((float)lm->hd);
-  const int* seg_start = nullptr;
-  if (pos_ids) {
-    SK_TRY(sk_seg_bounds_launch(pos_ids, wsp<int32_t>(lm, w.seg_start), wsp<int32_t>(lm, w.seg_end), B, T, s));
-    seg_start = wsp<int32_t>(lm, w.seg_start);
-  }
+  SK_TRY(seg_bounds(lm, a, w, s));
+  const int* seg_start = seg_ptr(lm, a, w.seg_start);
   bf16* attn = wsp<bf16>(lm, w.xmid);
   for (int l = 0; l < L; ++l) {
-    const NeoxLayerOff& o = lm->nlo[l];
+    const LnLayerOff& o = lm->lnl[l];
     bf16* x = wsp<bf16>(lm, w.X + w.sX * l);
     bf16* xn = wsp<bf16>(lm, w.X + w.sX * (l + 1));
     bf16* h1 = wsp<bf16>(lm, w.h1 + w.sh * l);
@@ -596,7 +532,7 @@ int neox_forward(SkLm* lm, const int64_t* ids, const int64_t* labels, const int3
 
     SK_TRY(sk_layernorm2_fwd_launch(x, P + o.ln1w, P + o.ln1b, P + o.ln2w, P + o.ln2b, h1, h2, st, st + M, M, d, eps, s));
     SK_TRY(sk_linear_rope_launch(M, Q, d, h1, P + o.wqkv, P + o.bqkv, qkv, lm->rope_cos, lm->rope_sin, pos_ids, T, 2 * d,
-                                 lm->cfg.max_positions, s, lm->rot));
+                                 lm->max_pos, s, lm->rot));
     SK_TRY(sk_attn_tc_fwd_launch(qkv, ao, lse, B, T, lm->H, lm->H, Q, d, 1, scale, s, seg_start));
     SK_TRY(linear_fwd(M, d, d, ao, P + o.wo, attn, P + o.bo, nullptr, s));
     SK_TRY(sk_linear_gelu_fwd_launch(M, F, d, h2, P + o.w1, P + o.b1, pre, act, s));
@@ -605,24 +541,15 @@ int neox_forward(SkLm* lm, const int64_t* ids, const int64_t* labels, const int3
   float* stf = wsp<float>(lm, w.rstdf);
   SK_TRY(sk_layernorm_fwd_launch(wsp<bf16>(lm, w.X + w.sX * L), P + lm->off_final_norm, P + lm->off_final_norm_b,
                                  wsp<bf16>(lm, w.hf), stf, stf + M, M, d, eps, s));
-  lm->last_B = B;
-  lm->last_T = T;
-  if (!with_head) return 0;
-  bf16* logits = wsp<bf16>(lm, w.logits);
-  SK_TRY(linear_fwd(M, lm->Vp, d, wsp<bf16>(lm, w.hf), P + lm->off_head, logits, nullptr, nullptr, s));
-  if (labels) {
-    SK_TRY(sk_ce_launch(logits, labels, want_dlogits ? wsp<bf16>(lm, w.dlogits) : nullptr, wsp<float>(lm, w.ce_partial),
-                        row_nll, stats, M, T, lm->V, lm->Vp, num_items, dloss, s));
-  }
-  return 0;
+  return head_forward(lm, w, a, wsp<bf16>(lm, w.hf), d, s);
 }
 
 // The layer output's gradient dy reaches the MLP, the attention branch and the residual unchanged.  dense and
 // dense_4h_to_h both take dy; their bias gradients are the same column sums, formed once per bias as HF does.  The input
 // gradient dx = dy + LN1'(dh1) + LN2'(dh2) is summed in fp32 inside the dual-LayerNorm backward.
-int neox_backward(SkLm* lm, const int64_t* ids, const int32_t* pos_ids, int B, int T, int accumulate, const WsLayout& w,
-                  cudaStream_t s, bool with_head = true) {
-  const int M = B * T, d = lm->d, F = lm->F, L = lm->L, Q = lm->qkv_dim;
+int neox_backward(SkLm* lm, const FwdArgs& a, int accumulate, const WsLayout& w, cudaStream_t s) {
+  const int B = a.B, T = a.T, M = B * T, d = lm->d, F = lm->F, L = lm->L, Q = lm->qkv_dim;
+  const int32_t* pos_ids = a.pos_ids;
   const bf16* P = lm->params;
   bf16* G = lm->grads;
   float* lnp = wsp<float>(lm, w.dw_partial);
@@ -633,25 +560,20 @@ int neox_backward(SkLm* lm, const int64_t* ids, const int32_t* pos_ids, int B, i
   bf16* dao = wsp<bf16>(lm, w.dao);
   bf16* dqkv = wsp<bf16>(lm, w.dqkv);
   bf16* dpre = wsp<bf16>(lm, w.dgu);
-  bf16* hf = wsp<bf16>(lm, w.hf);
   void* sws = lm->ws + w.splitk;
   const size_t swb = (size_t)w.splitk_bytes;
   const float scale = 1.0f / sqrtf((float)lm->hd);
-  const int* seg_start = pos_ids ? wsp<int32_t>(lm, w.seg_start) : nullptr;
-  const int* seg_end = pos_ids ? wsp<int32_t>(lm, w.seg_end) : nullptr;
+  const int* seg_start = seg_ptr(lm, a, w.seg_start);
+  const int* seg_end = seg_ptr(lm, a, w.seg_end);
 
-  if (with_head) {
-    bf16* dlogits = wsp<bf16>(lm, w.dlogits);
-    SK_TRY(linear_dgrad(M, lm->Vp, d, dlogits, P + lm->off_head, dh, s));
-    SK_TRY(linear_wgrad(M, lm->Vp, d, dlogits, hf, G + lm->off_head, accumulate, s, sws, swb));
-  }
+  if (a.with_head) SK_TRY(head_backward(lm, w, M, dh, wsp<bf16>(lm, w.hf), d, accumulate, s));
   const float* stf = wsp<float>(lm, w.rstdf);
   SK_TRY(sk_layernorm_bwd_launch(dh, wsp<bf16>(lm, w.X + w.sX * L), P + lm->off_final_norm, stf, stf + M, nullptr, dy,
                                  G + lm->off_final_norm, G + lm->off_final_norm_b, lnp,
                                  lnp + (size_t)sk_layernorm_bwd_blocks() * d, M, d, accumulate, s));
   if (!lm->bwd_events.empty()) SK_CUDA_CHECK(cudaEventRecord(lm->bwd_events[L], s));
   for (int l = L - 1; l >= 0; --l) {
-    const NeoxLayerOff& o = lm->nlo[l];
+    const LnLayerOff& o = lm->lnl[l];
     const bf16* x = wsp<bf16>(lm, w.X + w.sX * l);
     const bf16* h1 = wsp<bf16>(lm, w.h1 + w.sh * l);
     const bf16* h2 = wsp<bf16>(lm, w.h2 + w.sh * l);
@@ -675,7 +597,7 @@ int neox_backward(SkLm* lm, const int64_t* ids, const int32_t* pos_ids, int B, i
     SK_TRY(sk_colsum_launch(dy, G + o.bo, csp, M, d, d, accumulate, s));
     SK_TRY(sk_attn_tc_bwd_launch(qkv, ao, dao, lse, wsp<float>(lm, w.delta), nullptr, dqkv, B, T, lm->H, lm->H, Q, d, Q, 1,
                                  scale, s, seg_start, seg_end));
-    SK_TRY(sk_rope_launch(dqkv, lm->rope_cos, lm->rope_sin, pos_ids, M, T, Q, 2 * lm->H, lm->hd, 1, lm->cfg.max_positions, s,
+    SK_TRY(sk_rope_launch(dqkv, lm->rope_cos, lm->rope_sin, pos_ids, M, T, Q, 2 * lm->H, lm->hd, 1, lm->max_pos, s,
                           lm->rot));
     SK_TRY(sk_colsum_launch(dqkv, G + o.bqkv, csp, M, Q, Q, accumulate, s));
     SK_TRY(linear_dgrad(M, Q, d, dqkv, P + o.wqkv, dao, s));
@@ -685,44 +607,41 @@ int neox_backward(SkLm* lm, const int64_t* ids, const int32_t* pos_ids, int B, i
     std::swap(dy, dnext);
     if (!lm->bwd_events.empty()) SK_CUDA_CHECK(cudaEventRecord(lm->bwd_events[l], s));
   }
-  return sk_embed_bwd_launch(ids, dy, wsp<float>(lm, w.embed_scratch), G + lm->off_embed, M, d, lm->V, lm->Vp, accumulate, s);
+  return sk_embed_bwd_launch(a.ids, dy, wsp<float>(lm, w.embed_scratch), G + lm->off_embed, M, d, lm->V, lm->Vp, accumulate, s);
 }
 
 // One token per row at position pos[b] (read on the device: the step is graph-capturable).  Decode workspace: h = ln1,
 // `gu` = [pre (B x F) | ln2 (B x d)], `act` = the GELU, x1 = the attention branch's output; the layer output is written
 // over x in place by the two-residual epilogue.
 int neox_decode_step(SkLm* lm, const int64_t* tokens, const int32_t* pos, int B, void* kv_cache, int T_cache, void* logits,
-                     int ldl, uint8_t* dws, const DecLayout& dl, cudaStream_t s) {
+                     int ldl, const DecBufs& b, cudaStream_t s) {
   const int d = lm->d, F = lm->F, Q = lm->qkv_dim;
-  const float eps = lm->cfg.rms_eps;
+  const float eps = lm->eps;
   const bf16* P = lm->params;
-  bf16* x = reinterpret_cast<bf16*>(dws + dl.x0);
-  bf16* attn = reinterpret_cast<bf16*>(dws + dl.x1);
-  bf16* h = reinterpret_cast<bf16*>(dws + dl.h);
-  bf16* qkv = reinterpret_cast<bf16*>(dws + dl.qkv);
-  bf16* ao = reinterpret_cast<bf16*>(dws + dl.ao);
-  bf16* pre = reinterpret_cast<bf16*>(dws + dl.gu);
+  bf16* x = b.x0;
+  bf16* attn = b.x1;
+  bf16* h = b.h;
+  bf16* qkv = b.qkv;
+  bf16* ao = b.ao;
+  bf16* pre = b.gu;
   bf16* h2 = pre + (size_t)B * F;
-  bf16* act = reinterpret_cast<bf16*>(dws + dl.act);
-  int32_t* lens = reinterpret_cast<int32_t*>(dws + dl.lens);
-  float* partial = reinterpret_cast<float*>(dws + dl.partial);
-  void* gemm_ws = dws + dl.gemm;
+  bf16* act = b.act;
   const size_t plane = (size_t)B * lm->H * T_cache * lm->hd;
   const float scale = 1.0f / sqrtf((float)lm->hd);
   SK_TRY(sk_embed_fwd_launch(tokens, P + lm->off_embed, x, B, d, lm->V, s));
   for (int l = 0; l < lm->L; ++l) {
-    const NeoxLayerOff& o = lm->nlo[l];
+    const LnLayerOff& o = lm->lnl[l];
     bf16* kc = reinterpret_cast<bf16*>(kv_cache) + (size_t)l * 2 * plane;
     bf16* vc = kc + plane;
     SK_TRY(sk_layernorm2_fwd_launch(x, P + o.ln1w, P + o.ln1b, P + o.ln2w, P + o.ln2b, h, h2, nullptr, nullptr, B, d, eps, s));
     SK_TRY(sk_linear_rope_launch(B, Q, d, h, P + o.wqkv, P + o.bqkv, qkv, lm->rope_cos, lm->rope_sin, pos, 1, 2 * d,
-                                 lm->cfg.max_positions, s, lm->rot));
-    SK_TRY(sk_kv_append_launch(qkv, Q, kc, vc, pos, lens, B, lm->H, lm->H, T_cache, s));
-    SK_TRY(sk_attn_decode_launch(qkv, Q, kc, vc, lens, ao, d, partial, B, lm->H, lm->H, T_cache, scale, s));
+                                 lm->max_pos, s, lm->rot));
+    SK_TRY(sk_kv_append_launch(qkv, Q, kc, vc, pos, b.lens, B, lm->H, lm->H, T_cache, s));
+    SK_TRY(sk_attn_decode_launch(qkv, Q, kc, vc, b.lens, ao, d, b.partial, B, lm->H, lm->H, T_cache, scale, s));
     SK_TRY(linear_fwd(B, d, d, ao, P + o.wo, attn, P + o.bo, nullptr, s));
     SK_TRY(sk_linear_gelu_fwd_launch(B, F, d, h2, P + o.w1, P + o.b1, pre, act, s));
     // with M = B the scratch lets stream-K spread dense_4h_to_h's long K loop over idle SMs
-    SK_TRY(sk_linear_res2_launch(B, d, F, act, P + o.w2, P + o.b2, attn, x, x, s, gemm_ws, (size_t)dl.gemm_bytes));
+    SK_TRY(sk_linear_res2_launch(B, d, F, act, P + o.w2, P + o.b2, attn, x, x, s, b.gemm, b.gemm_bytes));
   }
   SK_TRY(sk_layernorm_fwd_launch(x, P + lm->off_final_norm, P + lm->off_final_norm_b, h, nullptr, nullptr, B, d, eps, s));
   return sk_gemm_launch(B, lm->Vp, d, h, d, 0, P + lm->off_head, d, 0, logits, ldl, 0, nullptr, nullptr, 0, 0, 0, 0, s);
@@ -733,24 +652,19 @@ int neox_decode_step(SkLm* lm, const int64_t* tokens, const int32_t* pos, int B,
 // gamma / beta and hands the next linear one bf16 rounding; every linear is the bf16 path's GEMM on the bf16 shadow
 // weights with a bf16 output, which is autocast's linear.  Each branch output's residual add is fused into the next
 // LayerNorm (the last fc2's into the final norm); the bf16 branch output waits in the dxB slab, unused until backward.
-int opt_forward_master(SkLm* lm, const int64_t* ids, const int64_t* labels, const int32_t* pos_ids, int B, int T, float num_items,
-                       float dloss, bool want_dlogits, float* stats, const WsLayout& w, cudaStream_t s, float* row_nll,
-                       bool with_head) {
-  const int M = B * T, d = lm->d, F = lm->F, L = lm->L, Q = lm->qkv_dim;
-  const float eps = lm->cfg.rms_eps;
+int opt_master_forward(SkLm* lm, const FwdArgs& a, const WsLayout& w, cudaStream_t s) {
+  const int B = a.B, T = a.T, M = B * T, d = lm->d, F = lm->F, L = lm->L, Q = lm->qkv_dim;
+  const float eps = lm->eps;
   const bf16* P = lm->params;
   const float* P32 = lm->params32;
   bf16* y = wsp<bf16>(lm, w.dxB);
-  SK_TRY(sk_opt_embed_fwd_f32_launch(ids, pos_ids, P32 + lm->off_embed, P32 + lm->off_pos, wsp<float>(lm, w.X), M, T, d, lm->V,
-                                     lm->n_pos, s));
+  SK_TRY(sk_opt_embed_fwd_f32_launch(a.ids, a.pos_ids, P32 + lm->off_embed, P32 + lm->off_pos, wsp<float>(lm, w.X), M, T, d,
+                                     lm->V, lm->n_pos, s));
   const float scale = 1.0f / sqrtf((float)lm->hd);
-  const int* seg_start = nullptr;
-  if (pos_ids) {
-    SK_TRY(sk_seg_bounds_launch(pos_ids, wsp<int32_t>(lm, w.seg_start), wsp<int32_t>(lm, w.seg_end), B, T, s));
-    seg_start = wsp<int32_t>(lm, w.seg_start);
-  }
+  SK_TRY(seg_bounds(lm, a, w, s));
+  const int* seg_start = seg_ptr(lm, a, w.seg_start);
   for (int l = 0; l < L; ++l) {
-    const OptLayerOff& o = lm->olo[l];
+    const LnLayerOff& o = lm->lnl[l];
     float* x = wsp<float>(lm, w.X + w.sR * l);
     float* xmid = wsp<float>(lm, w.xmid + w.sR * l);
     bf16* h1 = wsp<bf16>(lm, w.h1 + w.sh * l);
@@ -777,25 +691,15 @@ int opt_forward_master(SkLm* lm, const int64_t* ids, const int64_t* labels, cons
   SK_TRY(sk_add_layernorm_f32_launch(wsp<float>(lm, w.xmid + w.sR * (L - 1)), y, P32 + lm->off_final_norm,
                                      P32 + lm->off_final_norm_b, wsp<float>(lm, w.X + w.sR * L), wsp<bf16>(lm, w.hf), stf,
                                      stf + M, M, d, eps, s));
-  lm->last_B = B;
-  lm->last_T = T;
-  if (!with_head) return 0;
-  bf16* logits = wsp<bf16>(lm, w.logits);
-  SK_TRY(linear_fwd(M, lm->Vp, d, wsp<bf16>(lm, w.hf), P + lm->off_head, logits, nullptr, nullptr, s));
-  if (labels) {
-    SK_TRY(sk_ce_launch(logits, labels, want_dlogits ? wsp<bf16>(lm, w.dlogits) : nullptr, wsp<float>(lm, w.ce_partial),
-                        row_nll, stats, M, T, lm->V, lm->Vp, num_items, dloss, s));
-  }
-  return 0;
+  return head_forward(lm, w, a, wsp<bf16>(lm, w.hf), d, s);
 }
 
 // The residual gradient dres is fp32 (dres32); each branch's GEMMs and bias column sums read its bf16 copy (dxA), and
 // each LayerNorm backward adds its input gradient to dres in fp32.  Linear weight and bias gradients land in the bf16
 // buffer (never accumulated there) and are widened into grads32 at the end; LayerNorm and table gradients go straight
 // into grads32.  `accumulate` = a later micro-batch: add to grads32 instead of overwriting it.
-int opt_backward_master(SkLm* lm, const int64_t* ids, const int32_t* pos_ids, int B, int T, int accumulate, const WsLayout& w,
-                        cudaStream_t s, bool with_head) {
-  const int M = B * T, d = lm->d, F = lm->F, L = lm->L, Q = lm->qkv_dim;
+int opt_master_backward(SkLm* lm, const FwdArgs& a, int accumulate, const WsLayout& w, cudaStream_t s) {
+  const int B = a.B, T = a.T, M = B * T, d = lm->d, F = lm->F, L = lm->L, Q = lm->qkv_dim;
   const bf16* P = lm->params;
   const float* P32 = lm->params32;
   bf16* G = lm->grads;
@@ -811,20 +715,17 @@ int opt_backward_master(SkLm* lm, const int64_t* ids, const int32_t* pos_ids, in
   void* sws = lm->ws + w.splitk;
   const size_t swb = (size_t)w.splitk_bytes;
   const float scale = 1.0f / sqrtf((float)lm->hd);
-  const int* seg_start = pos_ids ? wsp<int32_t>(lm, w.seg_start) : nullptr;
-  const int* seg_end = pos_ids ? wsp<int32_t>(lm, w.seg_end) : nullptr;
+  const int* seg_start = seg_ptr(lm, a, w.seg_start);
+  const int* seg_end = seg_ptr(lm, a, w.seg_end);
 
-  if (with_head) {
-    bf16* dlogits = wsp<bf16>(lm, w.dlogits);
-    SK_TRY(linear_dgrad(M, lm->Vp, d, dlogits, P + lm->off_head, dh, s));
-    SK_TRY(linear_wgrad(M, lm->Vp, d, dlogits, wsp<bf16>(lm, w.hf), G + lm->off_head, 0, s, sws, swb));
-  }
+  // the bf16 gradient buffer holds one micro-batch (grads32 accumulates)
+  if (a.with_head) SK_TRY(head_backward(lm, w, M, dh, wsp<bf16>(lm, w.hf), d, 0, s));
   const float* stf = wsp<float>(lm, w.rstdf);
   SK_TRY(sk_layernorm_bwd_f32_launch(dh, wsp<float>(lm, w.X + w.sR * L), P32 + lm->off_final_norm, stf, stf + M, nullptr, dres,
                                      dr16, G32 + lm->off_final_norm, G32 + lm->off_final_norm_b, lnp, M, d, accumulate, s));
   if (!lm->bwd_events.empty()) SK_CUDA_CHECK(cudaEventRecord(lm->bwd_events[L], s));
   for (int l = L - 1; l >= 0; --l) {
-    const OptLayerOff& o = lm->olo[l];
+    const LnLayerOff& o = lm->lnl[l];
     const float* x = wsp<float>(lm, w.X + w.sR * l);
     const float* xmid = wsp<float>(lm, w.xmid + w.sR * l);
     const bf16* h1 = wsp<bf16>(lm, w.h1 + w.sh * l);
@@ -860,9 +761,9 @@ int opt_backward_master(SkLm* lm, const int64_t* ids, const int32_t* pos_ids, in
     if (!lm->bwd_events.empty()) SK_CUDA_CHECK(cudaEventRecord(lm->bwd_events[l], s));
   }
   float* scratch = wsp<float>(lm, w.embed_scratch);
-  SK_TRY(sk_table_bwd_f32_launch(ids, nullptr, dres, scratch, G32 + lm->off_embed,
-                                 lm->cfg.tie_embeddings ? G + lm->off_head : nullptr, M, T, d, lm->V, lm->Vp, accumulate, s));
-  SK_TRY(sk_table_bwd_f32_launch(nullptr, pos_ids, dres, scratch, G32 + lm->off_pos, nullptr, M, T, d, lm->n_pos, lm->n_pos,
+  SK_TRY(sk_table_bwd_f32_launch(a.ids, nullptr, dres, scratch, G32 + lm->off_embed,
+                                 lm->tie ? G + lm->off_head : nullptr, M, T, d, lm->V, lm->Vp, accumulate, s));
+  SK_TRY(sk_table_bwd_f32_launch(nullptr, a.pos_ids, dres, scratch, G32 + lm->off_pos, nullptr, M, T, d, lm->n_pos, lm->n_pos,
                                  accumulate, s));
   return sk_widen_grads_launch(G, G32, lm->d_widen_start, lm->d_widen_len, lm->n_widen, accumulate, s);
 }
@@ -872,11 +773,11 @@ int opt_backward_master(SkLm* lm, const int64_t* ids, const int32_t* pos_ids, in
 // s1 = bf16(bf16(attn W_o + b_o) + x), h1 y1 = LN1(s1), h2 s2 = bf16(bf16(relu(y1 W_1 + b_1) W_2 + b_2) + y1),
 // X[l+1] = LN2(s2); rstd1 / rstd2 the two LayerNorms' mean / rstd, gu relu(fc1).  With projections, `pe` holds the token
 // rows e [M, proj_dim] and hf the head input h = bf16(x_L W_out^T) [M, proj_dim].
-int opt_postln_forward(SkLm* lm, const int64_t* ids, const int64_t* labels, const int32_t* pos_ids, int B, int T,
-                       float num_items, float dloss, bool want_dlogits, float* stats, const WsLayout& w, cudaStream_t s,
-                       float* row_nll, bool with_head) {
-  const int M = B * T, d = lm->d, F = lm->F, L = lm->L, Q = lm->qkv_dim, K = head_k(lm);
-  const float eps = lm->cfg.rms_eps;
+int opt_postln_forward(SkLm* lm, const FwdArgs& a, const WsLayout& w, cudaStream_t s) {
+  const int B = a.B, T = a.T, M = B * T, d = lm->d, F = lm->F, L = lm->L, Q = lm->qkv_dim, K = head_k(lm);
+  const int64_t* ids = a.ids;
+  const int32_t* pos_ids = a.pos_ids;
+  const float eps = lm->eps;
   const bf16* P = lm->params;
   bf16* X0 = wsp<bf16>(lm, w.X);
   if (lm->proj) {
@@ -891,13 +792,10 @@ int opt_postln_forward(SkLm* lm, const int64_t* ids, const int64_t* labels, cons
     SK_TRY(sk_opt_embed_fwd_launch(ids, pos_ids, P + lm->off_embed, P + lm->off_pos, X0, M, T, d, lm->V, lm->n_pos, s));
   }
   const float scale = 1.0f / sqrtf((float)lm->hd);
-  const int* seg_start = nullptr;
-  if (pos_ids) {
-    SK_TRY(sk_seg_bounds_launch(pos_ids, wsp<int32_t>(lm, w.seg_start), wsp<int32_t>(lm, w.seg_end), B, T, s));
-    seg_start = wsp<int32_t>(lm, w.seg_start);
-  }
+  SK_TRY(seg_bounds(lm, a, w, s));
+  const int* seg_start = seg_ptr(lm, a, w.seg_start);
   for (int l = 0; l < L; ++l) {
-    const OptLayerOff& o = lm->olo[l];
+    const LnLayerOff& o = lm->lnl[l];
     bf16* x = wsp<bf16>(lm, w.X + w.sX * l);
     bf16* xn = wsp<bf16>(lm, w.X + w.sX * (l + 1));
     bf16* y1 = wsp<bf16>(lm, w.h1 + w.sh * l);
@@ -920,24 +818,14 @@ int opt_postln_forward(SkLm* lm, const int64_t* ids, const int64_t* labels, cons
   }
   if (lm->proj)
     SK_TRY(linear_fwd(M, K, d, wsp<bf16>(lm, w.X + w.sX * L), P + lm->off_pout, wsp<bf16>(lm, w.hf), nullptr, nullptr, s));
-  lm->last_B = B;
-  lm->last_T = T;
-  if (!with_head) return 0;
-  bf16* logits = wsp<bf16>(lm, w.logits);
-  SK_TRY(linear_fwd(M, lm->Vp, K, head_in(lm, w), P + lm->off_head, logits, nullptr, nullptr, s));
-  if (labels) {
-    SK_TRY(sk_ce_launch(logits, labels, want_dlogits ? wsp<bf16>(lm, w.dlogits) : nullptr, wsp<float>(lm, w.ce_partial),
-                        row_nll, stats, M, T, lm->V, lm->Vp, num_items, dloss, s));
-  }
-  return 0;
+  return head_forward(lm, w, a, head_in(lm, w), K, s);
 }
 
 // The residual stream is the LayerNorm output, so each LayerNorm backward reads the sum of its output's two gradients:
 // the fc1 and q|k|v dgrad GEMMs add the skip path's gradient in their epilogue, bf16(ds + bf16(dgrad)) as autograd
 // rounds it.  Every reduction is the deterministic one of the pre-LN path.
-int opt_postln_backward(SkLm* lm, const int64_t* ids, const int32_t* pos_ids, int B, int T, int accumulate, const WsLayout& w,
-                        cudaStream_t s, bool with_head) {
-  const int M = B * T, d = lm->d, F = lm->F, L = lm->L, Q = lm->qkv_dim, K = head_k(lm);
+int opt_postln_backward(SkLm* lm, const FwdArgs& a, int accumulate, const WsLayout& w, cudaStream_t s) {
+  const int B = a.B, T = a.T, M = B * T, d = lm->d, F = lm->F, L = lm->L, Q = lm->qkv_dim, K = head_k(lm);
   const bf16* P = lm->params;
   bf16* G = lm->grads;
   float* dwp = wsp<float>(lm, w.dw_partial);
@@ -953,21 +841,18 @@ int opt_postln_backward(SkLm* lm, const int64_t* ids, const int32_t* pos_ids, in
   void* sws = lm->ws + w.splitk;
   const size_t swb = (size_t)w.splitk_bytes;
   const float scale = 1.0f / sqrtf((float)lm->hd);
-  const int* seg_start = pos_ids ? wsp<int32_t>(lm, w.seg_start) : nullptr;
-  const int* seg_end = pos_ids ? wsp<int32_t>(lm, w.seg_end) : nullptr;
+  const int* seg_start = seg_ptr(lm, a, w.seg_start);
+  const int* seg_end = seg_ptr(lm, a, w.seg_end);
 
-  if (with_head) {   // tied head at K = proj_dim (already done chunk by chunk for large vocabularies)
-    bf16* dlogits = wsp<bf16>(lm, w.dlogits);
-    SK_TRY(linear_dgrad(M, lm->Vp, K, dlogits, P + lm->off_head, lm->proj ? dh : dxA, s));
-    SK_TRY(linear_wgrad(M, lm->Vp, K, dlogits, head_in(lm, w), G + lm->off_head, accumulate, s, sws, swb));
-  }
+  // tied head at K = proj_dim (already done chunk by chunk for large vocabularies)
+  if (a.with_head) SK_TRY(head_backward(lm, w, M, lm->proj ? dh : dxA, head_in(lm, w), K, accumulate, s));
   if (lm->proj) {
     SK_TRY(linear_dgrad(M, K, d, dh, P + lm->off_pout, dxA, s));
     SK_TRY(linear_wgrad(M, K, d, dh, xL, G + lm->off_pout, accumulate, s, sws, swb));
   }
   if (!lm->bwd_events.empty()) SK_CUDA_CHECK(cudaEventRecord(lm->bwd_events[L], s));
   for (int l = L - 1; l >= 0; --l) {   // dxA: the gradient of the layer's output LN2(s2)
-    const OptLayerOff& o = lm->olo[l];
+    const LnLayerOff& o = lm->lnl[l];
     const bf16* x = wsp<bf16>(lm, w.X + w.sX * l);
     const bf16* y1 = wsp<bf16>(lm, w.h1 + w.sh * l);
     const float* st1 = wsp<float>(lm, w.rstd1 + w.srstd * l);
@@ -1008,38 +893,29 @@ int opt_postln_backward(SkLm* lm, const int64_t* ids, const int32_t* pos_ids, in
   }
   // dxA = the gradient of x0: the position table, then project_in, then the (tied) token table
   float* scratch = wsp<float>(lm, w.embed_scratch);
-  SK_TRY(sk_opt_pos_bwd_launch(pos_ids, dxA, scratch, G + lm->off_pos, M, T, d, lm->n_pos, accumulate, s));
+  SK_TRY(sk_opt_pos_bwd_launch(a.pos_ids, dxA, scratch, G + lm->off_pos, M, T, d, lm->n_pos, accumulate, s));
   const bf16* de = dxA;
   if (lm->proj) {
     SK_TRY(linear_wgrad(M, d, K, dxA, wsp<bf16>(lm, w.pe), G + lm->off_pin, accumulate, s, sws, swb));
     SK_TRY(linear_dgrad(M, d, K, dxA, P + lm->off_pin, dh, s));
     de = dh;
   }
-  return sk_embed_bwd_launch(ids, de, scratch, G + lm->off_embed, M, K, lm->V, lm->Vp, lm->cfg.tie_embeddings ? 1 : accumulate,
-                             s);
+  return sk_embed_bwd_launch(a.ids, de, scratch, G + lm->off_embed, M, K, lm->V, lm->Vp, lm->tie ? 1 : accumulate, s);
 }
 
-int opt_forward(SkLm* lm, const int64_t* ids, const int64_t* labels, const int32_t* pos_ids, int B, int T, float num_items,
-                float dloss, bool want_dlogits, float* stats, const WsLayout& w, cudaStream_t s, float* row_nll = nullptr,
-                bool with_head = true) {
-  if (lm->post_ln)
-    return opt_postln_forward(lm, ids, labels, pos_ids, B, T, num_items, dloss, want_dlogits, stats, w, s, row_nll, with_head);
-  if (lm->master)
-    return opt_forward_master(lm, ids, labels, pos_ids, B, T, num_items, dloss, want_dlogits, stats, w, s, row_nll, with_head);
-  const int M = B * T, d = lm->d, F = lm->F, L = lm->L, Q = lm->qkv_dim;
-  const float eps = lm->cfg.rms_eps;
+int opt_forward(SkLm* lm, const FwdArgs& a, const WsLayout& w, cudaStream_t s) {
+  const int B = a.B, T = a.T, M = B * T, d = lm->d, F = lm->F, L = lm->L, Q = lm->qkv_dim;
+  const float eps = lm->eps;
   const bf16* P = lm->params;
-  SK_TRY(sk_opt_embed_fwd_launch(ids, pos_ids, P + lm->off_embed, P + lm->off_pos, wsp<bf16>(lm, w.X), M, T, d, lm->V, lm->n_pos, s));
+  SK_TRY(sk_opt_embed_fwd_launch(a.ids, a.pos_ids, P + lm->off_embed, P + lm->off_pos, wsp<bf16>(lm, w.X), M, T, d, lm->V,
+                                 lm->n_pos, s));
   // q is multiplied by head_dim^-0.5 = 1/8 after q_proj (HF:modeling_opt.py:146); a power of two, so the same value as
   // scaling the scores inside attention
   const float scale = 1.0f / sqrtf((float)lm->hd);
-  const int* seg_start = nullptr;
-  if (pos_ids) {
-    SK_TRY(sk_seg_bounds_launch(pos_ids, wsp<int32_t>(lm, w.seg_start), wsp<int32_t>(lm, w.seg_end), B, T, s));
-    seg_start = wsp<int32_t>(lm, w.seg_start);
-  }
+  SK_TRY(seg_bounds(lm, a, w, s));
+  const int* seg_start = seg_ptr(lm, a, w.seg_start);
   for (int l = 0; l < L; ++l) {
-    const OptLayerOff& o = lm->olo[l];
+    const LnLayerOff& o = lm->lnl[l];
     bf16* x = wsp<bf16>(lm, w.X + w.sX * l);
     bf16* xn = wsp<bf16>(lm, w.X + w.sX * (l + 1));
     bf16* h1 = wsp<bf16>(lm, w.h1 + w.sh * l);
@@ -1063,26 +939,14 @@ int opt_forward(SkLm* lm, const int64_t* ids, const int64_t* labels, const int32
   float* stf = wsp<float>(lm, w.rstdf);
   SK_TRY(sk_layernorm_fwd_launch(wsp<bf16>(lm, w.X + w.sX * L), P + lm->off_final_norm, P + lm->off_final_norm_b,
                                  wsp<bf16>(lm, w.hf), stf, stf + M, M, d, eps, s));
-  lm->last_B = B;
-  lm->last_T = T;
-  if (!with_head) return 0;
-  bf16* logits = wsp<bf16>(lm, w.logits);
-  SK_TRY(linear_fwd(M, lm->Vp, d, wsp<bf16>(lm, w.hf), P + lm->off_head, logits, nullptr, nullptr, s));
-  if (labels) {
-    SK_TRY(sk_ce_launch(logits, labels, want_dlogits ? wsp<bf16>(lm, w.dlogits) : nullptr, wsp<float>(lm, w.ce_partial),
-                        row_nll, stats, M, T, lm->V, lm->Vp, num_items, dloss, s));
-  }
-  return 0;
+  return head_forward(lm, w, a, wsp<bf16>(lm, w.hf), d, s);
 }
 
 // The embedding table's pad row gets the gradient of every token equal to pad_token_id.  HF's nn.Embedding(padding_idx)
 // drops that row's gradient instead; in right-padded and packed batches the two agree exactly, because the gradient
 // reaching a pad position is zero (pad targets carry no loss and only later pad positions attend to a pad key).
-int opt_backward(SkLm* lm, const int64_t* ids, const int32_t* pos_ids, int B, int T, int accumulate, const WsLayout& w,
-                 cudaStream_t s, bool with_head = true) {
-  if (lm->master) return opt_backward_master(lm, ids, pos_ids, B, T, accumulate, w, s, with_head);
-  if (lm->post_ln) return opt_postln_backward(lm, ids, pos_ids, B, T, accumulate, w, s, with_head);
-  const int M = B * T, d = lm->d, F = lm->F, L = lm->L, Q = lm->qkv_dim;
+int opt_backward(SkLm* lm, const FwdArgs& a, int accumulate, const WsLayout& w, cudaStream_t s) {
+  const int B = a.B, T = a.T, M = B * T, d = lm->d, F = lm->F, L = lm->L, Q = lm->qkv_dim;
   const bf16* P = lm->params;
   bf16* G = lm->grads;
   float* dwp = wsp<float>(lm, w.dw_partial);
@@ -1094,24 +958,19 @@ int opt_backward(SkLm* lm, const int64_t* ids, const int32_t* pos_ids, int B, in
   bf16* dao = wsp<bf16>(lm, w.dao);
   bf16* dqkv = wsp<bf16>(lm, w.dqkv);
   bf16* da = wsp<bf16>(lm, w.dgu);
-  bf16* hf = wsp<bf16>(lm, w.hf);
   void* sws = lm->ws + w.splitk;
   const size_t swb = (size_t)w.splitk_bytes;
   const float scale = 1.0f / sqrtf((float)lm->hd);
-  const int* seg_start = pos_ids ? wsp<int32_t>(lm, w.seg_start) : nullptr;
-  const int* seg_end = pos_ids ? wsp<int32_t>(lm, w.seg_end) : nullptr;
+  const int* seg_start = seg_ptr(lm, a, w.seg_start);
+  const int* seg_end = seg_ptr(lm, a, w.seg_end);
 
-  if (with_head) {
-    bf16* dlogits = wsp<bf16>(lm, w.dlogits);
-    SK_TRY(linear_dgrad(M, lm->Vp, d, dlogits, P + lm->off_head, dh, s));
-    SK_TRY(linear_wgrad(M, lm->Vp, d, dlogits, hf, G + lm->off_head, accumulate, s, sws, swb));
-  }
+  if (a.with_head) SK_TRY(head_backward(lm, w, M, dh, wsp<bf16>(lm, w.hf), d, accumulate, s));
   const float* stf = wsp<float>(lm, w.rstdf);
   SK_TRY(sk_layernorm_bwd_launch(dh, wsp<bf16>(lm, w.X + w.sX * L), P + lm->off_final_norm, stf, stf + M, nullptr, dxA,
                                  G + lm->off_final_norm, G + lm->off_final_norm_b, dwp, dbp, M, d, accumulate, s));
   if (!lm->bwd_events.empty()) SK_CUDA_CHECK(cudaEventRecord(lm->bwd_events[L], s));
   for (int l = L - 1; l >= 0; --l) {
-    const OptLayerOff& o = lm->olo[l];
+    const LnLayerOff& o = lm->lnl[l];
     const bf16* x = wsp<bf16>(lm, w.X + w.sX * l);
     const bf16* h1 = wsp<bf16>(lm, w.h1 + w.sh * l);
     const float* st1 = wsp<float>(lm, w.rstd1 + w.srstd * l);
@@ -1146,27 +1005,24 @@ int opt_backward(SkLm* lm, const int64_t* ids, const int32_t* pos_ids, int B, in
                                    accumulate, s));
     if (!lm->bwd_events.empty()) SK_CUDA_CHECK(cudaEventRecord(lm->bwd_events[l], s));
   }
-  SK_TRY(sk_embed_bwd_launch(ids, dxA, wsp<float>(lm, w.embed_scratch), G + lm->off_embed, M, d, lm->V, lm->Vp,
-                             lm->cfg.tie_embeddings ? 1 : accumulate, s));
-  return sk_opt_pos_bwd_launch(pos_ids, dxA, wsp<float>(lm, w.embed_scratch), G + lm->off_pos, M, T, d, lm->n_pos, accumulate, s);
+  SK_TRY(sk_embed_bwd_launch(a.ids, dxA, wsp<float>(lm, w.embed_scratch), G + lm->off_embed, M, d, lm->V, lm->Vp,
+                             lm->tie ? 1 : accumulate, s));
+  return sk_opt_pos_bwd_launch(a.pos_ids, dxA, wsp<float>(lm, w.embed_scratch), G + lm->off_pos, M, T, d, lm->n_pos, accumulate, s);
 }
 
 // Post-LN decode step (the formulas of opt_postln_forward at M = B).  With projections the h slot holds e [B, proj_dim]
 // at the start and the head input bf16(x_L W_out^T) at the end; x1 the position rows, then s1 and s2.
 int opt_postln_decode_step(SkLm* lm, const int64_t* tokens, const int32_t* pos, int B, void* kv_cache, int T_cache,
-                           void* logits, int ldl, uint8_t* dws, const DecLayout& dl, cudaStream_t s) {
+                           void* logits, int ldl, const DecBufs& b, cudaStream_t s) {
   const int d = lm->d, F = lm->F, Q = lm->qkv_dim, K = head_k(lm);
-  const float eps = lm->cfg.rms_eps;
+  const float eps = lm->eps;
   const bf16* P = lm->params;
-  bf16* x = reinterpret_cast<bf16*>(dws + dl.x0);
-  bf16* xm = reinterpret_cast<bf16*>(dws + dl.x1);
-  bf16* h = reinterpret_cast<bf16*>(dws + dl.h);
-  bf16* qkv = reinterpret_cast<bf16*>(dws + dl.qkv);
-  bf16* ao = reinterpret_cast<bf16*>(dws + dl.ao);
-  bf16* a = reinterpret_cast<bf16*>(dws + dl.gu);
-  int32_t* lens = reinterpret_cast<int32_t*>(dws + dl.lens);
-  float* partial = reinterpret_cast<float*>(dws + dl.partial);
-  void* gemm_ws = dws + dl.gemm;
+  bf16* x = b.x0;
+  bf16* xm = b.x1;
+  bf16* h = b.h;
+  bf16* qkv = b.qkv;
+  bf16* ao = b.ao;
+  bf16* a = b.gu;
   const size_t plane = (size_t)B * lm->H * T_cache * lm->hd;
   const float scale = 1.0f / sqrtf((float)lm->hd);
   if (lm->proj) {
@@ -1177,17 +1033,16 @@ int opt_postln_decode_step(SkLm* lm, const int64_t* tokens, const int32_t* pos, 
     SK_TRY(sk_opt_embed_fwd_launch(tokens, pos, P + lm->off_embed, P + lm->off_pos, x, B, 1, d, lm->V, lm->n_pos, s));
   }
   for (int l = 0; l < lm->L; ++l) {
-    const OptLayerOff& o = lm->olo[l];
+    const LnLayerOff& o = lm->lnl[l];
     bf16* kc = reinterpret_cast<bf16*>(kv_cache) + (size_t)l * 2 * plane;
     bf16* vc = kc + plane;
     SK_TRY(linear_fwd(B, Q, d, x, P + o.wqkv, qkv, P + o.bqkv, nullptr, s));
-    SK_TRY(sk_kv_append_launch(qkv, Q, kc, vc, pos, lens, B, lm->H, lm->H, T_cache, s));
-    SK_TRY(sk_attn_decode_launch(qkv, Q, kc, vc, lens, ao, d, partial, B, lm->H, lm->H, T_cache, scale, s));
+    SK_TRY(sk_kv_append_launch(qkv, Q, kc, vc, pos, b.lens, B, lm->H, lm->H, T_cache, s));
+    SK_TRY(sk_attn_decode_launch(qkv, Q, kc, vc, b.lens, ao, d, b.partial, B, lm->H, lm->H, T_cache, scale, s));
     SK_TRY(linear_fwd(B, d, d, ao, P + o.wo, xm, P + o.bo, x, s));
     SK_TRY(sk_layernorm_fwd_launch(xm, P + o.ln1w, P + o.ln1b, h, nullptr, nullptr, B, d, eps, s));
     SK_TRY(sk_gemm_launch(B, F, d, h, d, 0, P + o.w1, d, 0, a, F, 0, P + o.b1, nullptr, 0, 0, 2, 0, s));
-    SK_TRY(sk_gemm_launch(B, d, F, a, F, 0, P + o.w2, F, 0, xm, d, 0, P + o.b2, h, d, 1, 0, 0, s, gemm_ws,
-                          (size_t)dl.gemm_bytes));
+    SK_TRY(sk_gemm_launch(B, d, F, a, F, 0, P + o.w2, F, 0, xm, d, 0, P + o.b2, h, d, 1, 0, 0, s, b.gemm, b.gemm_bytes));
     SK_TRY(sk_layernorm_fwd_launch(xm, P + o.ln2w, P + o.ln2b, x, nullptr, nullptr, B, d, eps, s));
   }
   const bf16* hin = x;
@@ -1201,38 +1056,33 @@ int opt_postln_decode_step(SkLm* lm, const int64_t* tokens, const int32_t* pos, 
 // One token per row at position pos[b] (read on the device: the step is graph-capturable).  The KV cache layout is the
 // Qwen2 one with KVH = H.
 int opt_decode_step(SkLm* lm, const int64_t* tokens, const int32_t* pos, int B, void* kv_cache, int T_cache, void* logits,
-                    int ldl, uint8_t* dws, const DecLayout& dl, cudaStream_t s) {
-  if (lm->post_ln) return opt_postln_decode_step(lm, tokens, pos, B, kv_cache, T_cache, logits, ldl, dws, dl, s);
+                    int ldl, const DecBufs& b, cudaStream_t s) {
   const int d = lm->d, F = lm->F, Q = lm->qkv_dim;
-  const float eps = lm->cfg.rms_eps;
+  const float eps = lm->eps;
   const bf16* P = lm->params;
-  bf16* x = reinterpret_cast<bf16*>(dws + dl.x0);
-  bf16* xm = reinterpret_cast<bf16*>(dws + dl.x1);
-  bf16* h = reinterpret_cast<bf16*>(dws + dl.h);
-  bf16* qkv = reinterpret_cast<bf16*>(dws + dl.qkv);
-  bf16* ao = reinterpret_cast<bf16*>(dws + dl.ao);
-  bf16* a = reinterpret_cast<bf16*>(dws + dl.gu);
-  int32_t* lens = reinterpret_cast<int32_t*>(dws + dl.lens);
-  float* partial = reinterpret_cast<float*>(dws + dl.partial);
-  void* gemm_ws = dws + dl.gemm;
+  bf16* x = b.x0;
+  bf16* xm = b.x1;
+  bf16* h = b.h;
+  bf16* qkv = b.qkv;
+  bf16* ao = b.ao;
+  bf16* a = b.gu;
   const size_t plane = (size_t)B * lm->H * T_cache * lm->hd;
   const float scale = 1.0f / sqrtf((float)lm->hd);
   SK_TRY(sk_opt_embed_fwd_launch(tokens, pos, P + lm->off_embed, P + lm->off_pos, x, B, 1, d, lm->V, lm->n_pos, s));
   for (int l = 0; l < lm->L; ++l) {
-    const OptLayerOff& o = lm->olo[l];
+    const LnLayerOff& o = lm->lnl[l];
     bf16* kc = reinterpret_cast<bf16*>(kv_cache) + (size_t)l * 2 * plane;
     bf16* vc = kc + plane;
     SK_TRY(sk_layernorm_fwd_launch(x, P + o.ln1w, P + o.ln1b, h, nullptr, nullptr, B, d, eps, s));
     SK_TRY(linear_fwd(B, Q, d, h, P + o.wqkv, qkv, P + o.bqkv, nullptr, s));
-    SK_TRY(sk_kv_append_launch(qkv, Q, kc, vc, pos, lens, B, lm->H, lm->H, T_cache, s));
-    SK_TRY(sk_attn_decode_launch(qkv, Q, kc, vc, lens, ao, d, partial, B, lm->H, lm->H, T_cache, scale, s));
+    SK_TRY(sk_kv_append_launch(qkv, Q, kc, vc, pos, b.lens, B, lm->H, lm->H, T_cache, s));
+    SK_TRY(sk_attn_decode_launch(qkv, Q, kc, vc, b.lens, ao, d, b.partial, B, lm->H, lm->H, T_cache, scale, s));
     SK_TRY(linear_fwd(B, d, d, ao, P + o.wo, xm, P + o.bo, x, s));
     SK_TRY(sk_layernorm_fwd_launch(xm, P + o.ln2w, P + o.ln2b, h, nullptr, nullptr, B, d, eps, s));
     SK_TRY(sk_gemm_launch(B, F, d, h, d, 0, P + o.w1, d, 0, a, F, 0, P + o.b1, nullptr, 0, 0, 2, 0, s));
     // fc2 + bias + residual into x (not in place): with M = B the scratch lets stream-K spread the long K loop over idle
     // SMs; rounded before the residual add like the forward pass
-    SK_TRY(sk_gemm_launch(B, d, F, a, F, 0, P + o.w2, F, 0, x, d, 0, P + o.b2, xm, d, 1, 0, 0, s, gemm_ws,
-                          (size_t)dl.gemm_bytes));
+    SK_TRY(sk_gemm_launch(B, d, F, a, F, 0, P + o.w2, F, 0, x, d, 0, P + o.b2, xm, d, 1, 0, 0, s, b.gemm, b.gemm_bytes));
   }
   SK_TRY(sk_layernorm_fwd_launch(x, P + lm->off_final_norm, P + lm->off_final_norm_b, h, nullptr, nullptr, B, d, eps, s));
   return sk_gemm_launch(B, lm->Vp, d, h, d, 0, P + lm->off_head, d, 0, logits, ldl, 0, nullptr, nullptr, 0, 0, 0, 0, s);
@@ -1256,13 +1106,19 @@ int linear_split(const SkLm* lm, int M, int N, int K, Pair x, int64_t w_off, int
                                 res ? res->lo : nullptr, y.hi, y.lo, y32, ldy, s);
 }
 
+// the lm_head's input rows [M, head_k] of fp32 inference: the final LayerNorm's output in h1, or for post-LN OPT the last
+// layer's output in X or its project_out image in h1
+Pair head_in_fp32(const SkLm* lm, const WsLayout& w) {
+  const int64_t off = lm->post_ln && !lm->proj ? w.X : w.h1;
+  return Pair{wsp<bf16>(lm, off), wsp<bf16>(lm, off + w.sX)};
+}
+
 // Post-LN fp32 inference.  The slabs: X the layer input x, xmid s1 then s2, h1 y1 (and, with projections, e at the start
-// and the head input h = x_L W_out^T at the end); embed_scratch the fp32 rows before they are split.  The head input pair
-// is returned in *hin.
-int opt_postln_forward_fp32(SkLm* lm, const int64_t* ids, int B, int T, const WsLayout& w, cudaStream_t s, bool with_head,
-                            float* kv, const int32_t* lens, int T_cache, Pair* hin_out) {
-  const int M = B * T, d = lm->d, F = lm->F, L = lm->L, Q = lm->qkv_dim, K = head_k(lm);
-  const float eps = lm->cfg.rms_eps;
+// and the head input h = x_L W_out^T at the end); embed_scratch the fp32 rows before they are split.
+int opt_postln_forward_fp32(SkLm* lm, const FwdArgs& fa, const WsLayout& w, cudaStream_t s) {
+  const int B = fa.B, T = fa.T, M = B * T, d = lm->d, F = lm->F, L = lm->L, Q = lm->qkv_dim, K = head_k(lm);
+  const int64_t* ids = fa.ids;
+  const float eps = lm->eps;
   const float* P32 = lm->params32;
   auto pair = [&](int64_t off, int64_t stride) { return Pair{wsp<bf16>(lm, off), wsp<bf16>(lm, off + stride)}; };
   const Pair x = pair(w.X, w.sX), xm = pair(w.xmid, w.sX), h = pair(w.h1, w.sX), qkv = pair(w.qkv, w.sqkv),
@@ -1279,11 +1135,12 @@ int opt_postln_forward_fp32(SkLm* lm, const int64_t* ids, int B, int T, const Ws
     SK_TRY(sk_split_f32_launch(e32, x.hi, x.lo, (long)M * d, s));
   }
   const float scale = 1.0f / sqrtf((float)lm->hd);
-  const size_t plane = (size_t)B * lm->H * T_cache * lm->hd;
+  const size_t plane = (size_t)B * lm->H * fa.T_cache * lm->hd;
   for (int l = 0; l < L; ++l) {
-    const OptLayerOff& o = lm->olo[l];
+    const LnLayerOff& o = lm->lnl[l];
     SK_TRY(linear_split(lm, M, Q, d, x, o.wqkv, o.bqkv, 0, nullptr, qkv, nullptr, Q, s));
-    if (kv) SK_TRY(sk_kv_prefill_f32_launch(qkv.hi, qkv.lo, Q, kv + (size_t)l * 2 * plane, lens, B, T, lm->H, T_cache, s));
+    if (fa.kv)
+      SK_TRY(sk_kv_prefill_f32_launch(qkv.hi, qkv.lo, Q, fa.kv + (size_t)l * 2 * plane, fa.lens, B, T, lm->H, fa.T_cache, s));
     SK_TRY(sk_attn_tc_fwd_split_launch(qkv.hi, qkv.lo, ao.hi, ao.lo, B, T, lm->H, Q, d, scale, s, 1));
     SK_TRY(linear_split(lm, M, d, d, ao, o.wo, o.bo, 0, &x, xm, nullptr, d, s));
     SK_TRY(sk_layernorm_hilo_launch(xm.hi, xm.lo, nullptr, nullptr, P32 + o.ln1w, P32 + o.ln1b, h.hi, h.lo, nullptr, M, d, eps, s));
@@ -1291,53 +1148,42 @@ int opt_postln_forward_fp32(SkLm* lm, const int64_t* ids, int B, int T, const Ws
     SK_TRY(linear_split(lm, M, d, F, a, o.w2, o.b2, 0, &h, xm, nullptr, d, s));
     SK_TRY(sk_layernorm_hilo_launch(xm.hi, xm.lo, nullptr, nullptr, P32 + o.ln2w, P32 + o.ln2b, x.hi, x.lo, nullptr, M, d, eps, s));
   }
-  Pair hin = x;
-  if (lm->proj) {
-    SK_TRY(linear_split(lm, M, K, d, x, lm->off_pout, -1, 0, nullptr, h, nullptr, K, s));
-    hin = h;
-  }
-  if (hin_out) *hin_out = hin;
+  if (lm->proj) SK_TRY(linear_split(lm, M, K, d, x, lm->off_pout, -1, 0, nullptr, h, nullptr, K, s));
   lm->last_B = B;
   lm->last_T = T;
-  if (!with_head) return 0;
-  return linear_split(lm, M, lm->Vp, K, hin, lm->off_head, -1, 0, nullptr, Pair{nullptr, nullptr}, wsp<float>(lm, w.logits),
-                      lm->Vp, s);
+  if (!fa.with_head) return 0;
+  return linear_split(lm, M, lm->Vp, K, head_in_fp32(lm, w), lm->off_head, -1, 0, nullptr, Pair{nullptr, nullptr},
+                      wsp<float>(lm, w.logits), lm->Vp, s);
 }
 
 // Post-LN fp32 decode step: the slots of opt_decode_step_fp32, with h holding e at the start and the head input at the end
 int opt_postln_decode_step_fp32(SkLm* lm, const int64_t* tokens, const int32_t* pos, int B, float* kv, int T_cache,
-                                float* logits, int ldl, uint8_t* dws, const DecLayout& dl, cudaStream_t s) {
+                                float* logits, int ldl, const DecBufs& b, cudaStream_t s) {
   const int d = lm->d, F = lm->F, Q = lm->qkv_dim, K = head_k(lm);
-  const float eps = lm->cfg.rms_eps;
+  const float eps = lm->eps;
   const float* P32 = lm->params32;
-  auto pair = [&](int64_t off, int64_t n) {
-    bf16* hi = reinterpret_cast<bf16*>(dws + off);
-    return Pair{hi, hi + n};
-  };
-  const Pair x = pair(dl.x0, (int64_t)B * d), xm = pair(dl.x1, (int64_t)B * d), h = pair(dl.h, (int64_t)B * d),
-             qkv = pair(dl.qkv, (int64_t)B * Q), ao = pair(dl.ao, (int64_t)B * d), a = pair(dl.gu, (int64_t)B * F);
-  int32_t* lens = reinterpret_cast<int32_t*>(dws + dl.lens);
-  float* partial = reinterpret_cast<float*>(dws + dl.partial);
-  float* e32 = reinterpret_cast<float*>(dws + dl.e32);
+  auto pair = [&](bf16* hi, int64_t n) { return Pair{hi, hi + n}; };
+  const Pair x = pair(b.x0, (int64_t)B * d), xm = pair(b.x1, (int64_t)B * d), h = pair(b.h, (int64_t)B * d),
+             qkv = pair(b.qkv, (int64_t)B * Q), ao = pair(b.ao, (int64_t)B * d), a = pair(b.gu, (int64_t)B * F);
   const size_t plane = (size_t)B * lm->H * T_cache * lm->hd;
   const float scale = 1.0f / sqrtf((float)lm->hd);
   if (lm->proj) {
-    SK_TRY(sk_opt_embed_fwd_f32_launch(tokens, pos, nullptr, P32 + lm->off_pos, e32, B, 1, d, lm->V, lm->n_pos, s));
-    SK_TRY(sk_split_f32_launch(e32, xm.hi, xm.lo, (long)B * d, s));
-    SK_TRY(sk_opt_embed_fwd_f32_launch(tokens, pos, P32 + lm->off_embed, nullptr, e32, B, 1, K, lm->V, lm->n_pos, s));
-    SK_TRY(sk_split_f32_launch(e32, h.hi, h.lo, (long)B * K, s));
+    SK_TRY(sk_opt_embed_fwd_f32_launch(tokens, pos, nullptr, P32 + lm->off_pos, b.e32, B, 1, d, lm->V, lm->n_pos, s));
+    SK_TRY(sk_split_f32_launch(b.e32, xm.hi, xm.lo, (long)B * d, s));
+    SK_TRY(sk_opt_embed_fwd_f32_launch(tokens, pos, P32 + lm->off_embed, nullptr, b.e32, B, 1, K, lm->V, lm->n_pos, s));
+    SK_TRY(sk_split_f32_launch(b.e32, h.hi, h.lo, (long)B * K, s));
     SK_TRY(linear_split(lm, B, d, K, h, lm->off_pin, -1, 0, &xm, x, nullptr, d, s));
   } else {
-    SK_TRY(sk_opt_embed_fwd_f32_launch(tokens, pos, P32 + lm->off_embed, P32 + lm->off_pos, e32, B, 1, d, lm->V, lm->n_pos, s));
-    SK_TRY(sk_split_f32_launch(e32, x.hi, x.lo, (long)B * d, s));
+    SK_TRY(sk_opt_embed_fwd_f32_launch(tokens, pos, P32 + lm->off_embed, P32 + lm->off_pos, b.e32, B, 1, d, lm->V, lm->n_pos, s));
+    SK_TRY(sk_split_f32_launch(b.e32, x.hi, x.lo, (long)B * d, s));
   }
   for (int l = 0; l < lm->L; ++l) {
-    const OptLayerOff& o = lm->olo[l];
+    const LnLayerOff& o = lm->lnl[l];
     float* kc = kv + (size_t)l * 2 * plane;
     float* vc = kc + plane;
     SK_TRY(linear_split(lm, B, Q, d, x, o.wqkv, o.bqkv, 0, nullptr, qkv, nullptr, Q, s));
-    SK_TRY(sk_kv_append_f32_launch(qkv.hi, qkv.lo, Q, kc, vc, pos, lens, B, lm->H, T_cache, s));
-    SK_TRY(sk_attn_decode_f32_launch(qkv.hi, qkv.lo, Q, kc, vc, lens, ao.hi, ao.lo, d, partial, B, lm->H, T_cache, scale, s));
+    SK_TRY(sk_kv_append_f32_launch(qkv.hi, qkv.lo, Q, kc, vc, pos, b.lens, B, lm->H, T_cache, s));
+    SK_TRY(sk_attn_decode_f32_launch(qkv.hi, qkv.lo, Q, kc, vc, b.lens, ao.hi, ao.lo, d, b.partial, B, lm->H, T_cache, scale, s));
     SK_TRY(linear_split(lm, B, d, d, ao, o.wo, o.bo, 0, &x, xm, nullptr, d, s));
     SK_TRY(sk_layernorm_hilo_launch(xm.hi, xm.lo, nullptr, nullptr, P32 + o.ln1w, P32 + o.ln1b, h.hi, h.lo, nullptr, B, d, eps, s));
     SK_TRY(linear_split(lm, B, F, d, h, o.w1, o.b1, 2, nullptr, a, nullptr, F, s));
@@ -1352,12 +1198,10 @@ int opt_postln_decode_step_fp32(SkLm* lm, const int64_t* tokens, const int32_t* 
   return linear_split(lm, B, lm->Vp, K, hin, lm->off_head, -1, 0, nullptr, Pair{nullptr, nullptr}, logits, ldl, s);
 }
 
-// kv (optional, prefill): the fp32 cache of T_cache positions that receives the K / V of positions < lens[b]
-int opt_forward_fp32(SkLm* lm, const int64_t* ids, int B, int T, const WsLayout& w, cudaStream_t s, bool with_head,
-                     float* kv = nullptr, const int32_t* lens = nullptr, int T_cache = 0, Pair* hin_out = nullptr) {
-  if (lm->post_ln) return opt_postln_forward_fp32(lm, ids, B, T, w, s, with_head, kv, lens, T_cache, hin_out);
-  const int M = B * T, d = lm->d, F = lm->F, L = lm->L, Q = lm->qkv_dim;
-  const float eps = lm->cfg.rms_eps;
+int opt_forward_fp32(SkLm* lm, const FwdArgs& fa, const WsLayout& w, cudaStream_t s) {
+  const int B = fa.B, T = fa.T, M = B * T, d = lm->d, F = lm->F, L = lm->L, Q = lm->qkv_dim;
+  const int64_t* ids = fa.ids;
+  const float eps = lm->eps;
   const float* P32 = lm->params32;
   auto pair = [&](int64_t off, int64_t stride) { return Pair{wsp<bf16>(lm, off), wsp<bf16>(lm, off + stride)}; };
   const Pair x = pair(w.X, w.sX), xm = pair(w.xmid, w.sX), h = pair(w.h1, w.sX), qkv = pair(w.qkv, w.sqkv),
@@ -1367,12 +1211,13 @@ int opt_forward_fp32(SkLm* lm, const int64_t* ids, int B, int T, const WsLayout&
   SK_TRY(sk_split_f32_launch(e32, x.hi, x.lo, (long)M * d, s));
   // q * head_dim^-0.5 = q / 8 (HF:modeling_opt.py:146): a power of two, folded into the softmax scale exactly
   const float scale = 1.0f / sqrtf((float)lm->hd);
-  const size_t plane = (size_t)B * lm->H * T_cache * lm->hd;
+  const size_t plane = (size_t)B * lm->H * fa.T_cache * lm->hd;
   for (int l = 0; l < L; ++l) {
-    const OptLayerOff& o = lm->olo[l];
+    const LnLayerOff& o = lm->lnl[l];
     SK_TRY(sk_layernorm_hilo_launch(x.hi, x.lo, nullptr, nullptr, P32 + o.ln1w, P32 + o.ln1b, h.hi, h.lo, nullptr, M, d, eps, s));
     SK_TRY(linear_split(lm, M, Q, d, h, o.wqkv, o.bqkv, 0, nullptr, qkv, nullptr, Q, s));
-    if (kv) SK_TRY(sk_kv_prefill_f32_launch(qkv.hi, qkv.lo, Q, kv + (size_t)l * 2 * plane, lens, B, T, lm->H, T_cache, s));
+    if (fa.kv)
+      SK_TRY(sk_kv_prefill_f32_launch(qkv.hi, qkv.lo, Q, fa.kv + (size_t)l * 2 * plane, fa.lens, B, T, lm->H, fa.T_cache, s));
     SK_TRY(sk_attn_tc_fwd_split_launch(qkv.hi, qkv.lo, ao.hi, ao.lo, B, T, lm->H, Q, d, scale, s, 1));
     SK_TRY(linear_split(lm, M, d, d, ao, o.wo, o.bo, 0, &x, xm, nullptr, d, s));
     SK_TRY(sk_layernorm_hilo_launch(xm.hi, xm.lo, nullptr, nullptr, P32 + o.ln2w, P32 + o.ln2b, h.hi, h.lo, nullptr, M, d, eps, s));
@@ -1381,42 +1226,34 @@ int opt_forward_fp32(SkLm* lm, const int64_t* ids, int B, int T, const WsLayout&
   }
   SK_TRY(sk_layernorm_hilo_launch(x.hi, x.lo, nullptr, nullptr, P32 + lm->off_final_norm, P32 + lm->off_final_norm_b, h.hi,
                                   h.lo, nullptr, M, d, eps, s));
-  if (hin_out) *hin_out = h;
   lm->last_B = B;
   lm->last_T = T;
-  if (!with_head) return 0;
+  if (!fa.with_head) return 0;
   return linear_split(lm, M, lm->Vp, d, h, lm->off_head, -1, 0, nullptr, Pair{nullptr, nullptr}, wsp<float>(lm, w.logits),
                       lm->Vp, s);
 }
 
 // One token per row at position pos[b] on the fp32 cache ([K|V][B][H][T_cache][64] fp32 per layer); fp32 logits [B, ldl]
 int opt_decode_step_fp32(SkLm* lm, const int64_t* tokens, const int32_t* pos, int B, float* kv, int T_cache, float* logits,
-                         int ldl, uint8_t* dws, const DecLayout& dl, cudaStream_t s) {
-  if (lm->post_ln) return opt_postln_decode_step_fp32(lm, tokens, pos, B, kv, T_cache, logits, ldl, dws, dl, s);
+                         int ldl, const DecBufs& b, cudaStream_t s) {
   const int d = lm->d, F = lm->F, Q = lm->qkv_dim;
-  const float eps = lm->cfg.rms_eps;
+  const float eps = lm->eps;
   const float* P32 = lm->params32;
-  auto pair = [&](int64_t off, int64_t n) {
-    bf16* hi = reinterpret_cast<bf16*>(dws + off);
-    return Pair{hi, hi + n};
-  };
-  const Pair x = pair(dl.x0, (int64_t)B * d), xm = pair(dl.x1, (int64_t)B * d), h = pair(dl.h, (int64_t)B * d),
-             qkv = pair(dl.qkv, (int64_t)B * Q), ao = pair(dl.ao, (int64_t)B * d), a = pair(dl.gu, (int64_t)B * F);
-  int32_t* lens = reinterpret_cast<int32_t*>(dws + dl.lens);
-  float* partial = reinterpret_cast<float*>(dws + dl.partial);
-  float* e32 = reinterpret_cast<float*>(dws + dl.e32);
+  auto pair = [&](bf16* hi, int64_t n) { return Pair{hi, hi + n}; };
+  const Pair x = pair(b.x0, (int64_t)B * d), xm = pair(b.x1, (int64_t)B * d), h = pair(b.h, (int64_t)B * d),
+             qkv = pair(b.qkv, (int64_t)B * Q), ao = pair(b.ao, (int64_t)B * d), a = pair(b.gu, (int64_t)B * F);
   const size_t plane = (size_t)B * lm->H * T_cache * lm->hd;
   const float scale = 1.0f / sqrtf((float)lm->hd);
-  SK_TRY(sk_opt_embed_fwd_f32_launch(tokens, pos, P32 + lm->off_embed, P32 + lm->off_pos, e32, B, 1, d, lm->V, lm->n_pos, s));
-  SK_TRY(sk_split_f32_launch(e32, x.hi, x.lo, (long)B * d, s));
+  SK_TRY(sk_opt_embed_fwd_f32_launch(tokens, pos, P32 + lm->off_embed, P32 + lm->off_pos, b.e32, B, 1, d, lm->V, lm->n_pos, s));
+  SK_TRY(sk_split_f32_launch(b.e32, x.hi, x.lo, (long)B * d, s));
   for (int l = 0; l < lm->L; ++l) {
-    const OptLayerOff& o = lm->olo[l];
+    const LnLayerOff& o = lm->lnl[l];
     float* kc = kv + (size_t)l * 2 * plane;
     float* vc = kc + plane;
     SK_TRY(sk_layernorm_hilo_launch(x.hi, x.lo, nullptr, nullptr, P32 + o.ln1w, P32 + o.ln1b, h.hi, h.lo, nullptr, B, d, eps, s));
     SK_TRY(linear_split(lm, B, Q, d, h, o.wqkv, o.bqkv, 0, nullptr, qkv, nullptr, Q, s));
-    SK_TRY(sk_kv_append_f32_launch(qkv.hi, qkv.lo, Q, kc, vc, pos, lens, B, lm->H, T_cache, s));
-    SK_TRY(sk_attn_decode_f32_launch(qkv.hi, qkv.lo, Q, kc, vc, lens, ao.hi, ao.lo, d, partial, B, lm->H, T_cache, scale, s));
+    SK_TRY(sk_kv_append_f32_launch(qkv.hi, qkv.lo, Q, kc, vc, pos, b.lens, B, lm->H, T_cache, s));
+    SK_TRY(sk_attn_decode_f32_launch(qkv.hi, qkv.lo, Q, kc, vc, b.lens, ao.hi, ao.lo, d, b.partial, B, lm->H, T_cache, scale, s));
     SK_TRY(linear_split(lm, B, d, d, ao, o.wo, o.bo, 0, &x, xm, nullptr, d, s));
     SK_TRY(sk_layernorm_hilo_launch(xm.hi, xm.lo, nullptr, nullptr, P32 + o.ln2w, P32 + o.ln2b, h.hi, h.lo, nullptr, B, d, eps, s));
     SK_TRY(linear_split(lm, B, F, d, h, o.w1, o.b1, 2, nullptr, a, nullptr, F, s));
@@ -1431,8 +1268,10 @@ int opt_decode_step_fp32(SkLm* lm, const int64_t* tokens, const int32_t* pos, in
   SK_REQUIRE(!(lm)->fp32, who ": this handle runs fp32 inference (sk_lm_set_fp32), which is forward only; train with a " \
                           "bf16 or master-weights handle")
 
-// gradient-norm groups (one per HF parameter) and their device chunk tables; `groups` lists (offset, n) ranges
-int upload_norm_groups(SkLm* lm, const std::vector<std::vector<std::pair<int64_t, int64_t>>>& groups) {
+// gradient-norm groups and their device chunk tables.  A group is one HF parameter, a list of (offset, n) element ranges
+// of the flat buffer; chunks are listed group by group, so a group is a contiguous run of the chunk table.
+using NormGroups = std::vector<std::vector<std::pair<int64_t, int64_t>>>;
+int upload_norm_groups(SkLm* lm, const NormGroups& groups) {
   std::vector<long> cs;
   std::vector<int> cl, tb;
   for (const auto& g : groups) {
@@ -1454,6 +1293,110 @@ int upload_norm_groups(SkLm* lm, const std::vector<std::vector<std::pair<int64_t
   SK_CUDA_CHECK(cudaMemcpy(lm->d_chunk_len, cl.data(), cl.size() * sizeof(int), cudaMemcpyHostToDevice));
   SK_CUDA_CHECK(cudaMemcpy(lm->d_tensor_chunk_begin, tb.data(), tb.size() * sizeof(int), cudaMemcpyHostToDevice));
   return 0;
+}
+
+// A handle with the shape fields every decoder shares (head_dim 64); the caller has checked the shapes
+SkLm* new_lm(int arch, int V, int d, int L, int H, int KVH, int F, int max_pos, float eps, bool tie, bool qkv_bias) {
+  SkLm* lm = new SkLm();
+  lm->arch = arch;
+  lm->d = d;
+  lm->F = F;
+  lm->H = H;
+  lm->KVH = KVH;
+  lm->hd = 64;
+  lm->L = L;
+  lm->V = V;
+  lm->Vp = (V + 63) / 64 * 64;
+  lm->qkv_dim = (H + 2 * KVH) * lm->hd;
+  lm->max_pos = max_pos;
+  lm->eps = eps;
+  lm->tie = tie;
+  lm->qkv_bias = qkv_bias;
+  // text+unit vocabularies: chunked lm_head + CE (SK_HEAD_CHUNK=rows overrides, 0 turns it off)
+  lm->head_chunk = lm->Vp > 8192 ? 2048 : 0;
+  if (const char* e = getenv("SK_HEAD_CHUNK")) lm->head_chunk = (atoi(e) / 128) * 128;
+  return lm;
+}
+
+// upload the norm groups and hand the handle out, or free it
+int publish(SkLm* lm, const NormGroups& groups, SkLm** out) {
+  const int rc = upload_norm_groups(lm, groups);
+  if (rc) {
+    sk_lm_destroy(lm);
+    return rc;
+  }
+  *out = lm;
+  return 0;
+}
+
+// One token per row at position pos[b] (read on the device: the step is graph-capturable)
+int qwen2_decode_step(SkLm* lm, const int64_t* tokens, const int32_t* pos, int B, void* kv_cache, int T_cache, void* logits,
+                      int ldl, const DecBufs& b, cudaStream_t s) {
+  const int d = lm->d, F = lm->F, Q = lm->qkv_dim;
+  const bf16* P = lm->params;
+  bf16* x = b.x0;
+  bf16* xm = b.x1;
+  bf16* h = b.h;
+  bf16* qkv = b.qkv;
+  bf16* ao = b.ao;
+  bf16* gu = b.gu;
+  bf16* act = b.act;
+  const size_t plane = (size_t)B * lm->KVH * T_cache * lm->hd;
+  const float scale = 1.0f / sqrtf((float)lm->hd);
+  SK_TRY(sk_embed_fwd_launch(tokens, P + lm->off_embed, x, B, d, lm->V, s));
+  for (int l = 0; l < lm->L; ++l) {
+    const LayerOff& o = lm->lo[l];
+    bf16* kc = reinterpret_cast<bf16*>(kv_cache) + (size_t)l * 2 * plane;
+    bf16* vc = kc + plane;
+    SK_TRY(sk_rmsnorm_fwd_launch(x, P + o.ln1, h, nullptr, B, d, lm->eps, s));
+    SK_TRY(sk_linear_rope_launch(B, Q, d, h, P + o.wqkv, lm->qkv_bias ? P + o.bqkv : nullptr, qkv, lm->rope_cos,
+                                 lm->rope_sin, pos, 1, (lm->H + lm->KVH) * lm->hd, lm->max_pos, s));
+    SK_TRY(sk_kv_append_launch(qkv, Q, kc, vc, pos, b.lens, B, lm->H, lm->KVH, T_cache, s));
+    SK_TRY(sk_attn_decode_launch(qkv, Q, kc, vc, b.lens, ao, d, b.partial, B, lm->H, lm->KVH, T_cache, scale, s));
+    SK_TRY(linear_fwd(B, d, d, ao, P + o.wo, xm, nullptr, x, s));
+    SK_TRY(sk_rmsnorm_fwd_launch(xm, P + o.ln2, h, nullptr, B, d, lm->eps, s));
+    SK_TRY(sk_linear_swiglu_fwd_launch(B, F, d, h, P + o.wgu, gu, act, s));
+    // down projection added in place (residual == output): with M = B there is a single row of output tiles, so the
+    // scratch lets the GEMM split its long K loop over idle SMs (fixed-order reduction); rounded before the residual
+    // add like the forward pass's down projection
+    SK_TRY(sk_gemm_launch(B, d, F, act, F, 0, P + o.wd, F, 0, xm, d, 0, nullptr, xm, d, 1, 0, 0, s, b.gemm, b.gemm_bytes));
+    std::swap(x, xm);
+  }
+  SK_TRY(sk_rmsnorm_fwd_launch(x, P + lm->off_final_norm, h, nullptr, B, d, lm->eps, s));
+  return sk_gemm_launch(B, lm->Vp, d, h, d, 0, P + lm->off_head, d, 0, logits, ldl, 0, nullptr, nullptr, 0, 0, 0, 0, s);
+}
+
+// ---- the decoder variant: (fp32 inference) -> architecture -> (post-LN) -> (master weights), the only place that picks
+// one.  Master weights are never post-LN, fp32 inference is OPT forward only, and master handles do not decode.
+int forward(SkLm* lm, const FwdArgs& a, const WsLayout& w, cudaStream_t s) {
+  if (lm->fp32) return lm->post_ln ? opt_postln_forward_fp32(lm, a, w, s) : opt_forward_fp32(lm, a, w, s);
+  if (lm->arch == SK_ARCH_QWEN2) return qwen2_forward(lm, a, w, s);
+  if (lm->arch == SK_ARCH_NEOX) return neox_forward(lm, a, w, s);
+  if (lm->post_ln) return opt_postln_forward(lm, a, w, s);
+  if (lm->master) return opt_master_forward(lm, a, w, s);
+  return opt_forward(lm, a, w, s);
+}
+
+int backward(SkLm* lm, const FwdArgs& a, int accumulate, const WsLayout& w, cudaStream_t s) {
+  if (lm->arch == SK_ARCH_QWEN2) return qwen2_backward(lm, a, accumulate, w, s);
+  if (lm->arch == SK_ARCH_NEOX) return neox_backward(lm, a, accumulate, w, s);
+  if (lm->post_ln) return opt_postln_backward(lm, a, accumulate, w, s);
+  if (lm->master) return opt_master_backward(lm, a, accumulate, w, s);
+  return opt_backward(lm, a, accumulate, w, s);
+}
+
+int decode_step(SkLm* lm, const int64_t* tokens, const int32_t* pos, int B, void* kv_cache, int T_cache, void* logits, int ldl,
+                const DecBufs& b, cudaStream_t s) {
+  if (lm->fp32) {
+    float* kv = reinterpret_cast<float*>(kv_cache);
+    float* lg = reinterpret_cast<float*>(logits);
+    return lm->post_ln ? opt_postln_decode_step_fp32(lm, tokens, pos, B, kv, T_cache, lg, ldl, b, s)
+                       : opt_decode_step_fp32(lm, tokens, pos, B, kv, T_cache, lg, ldl, b, s);
+  }
+  if (lm->arch == SK_ARCH_QWEN2) return qwen2_decode_step(lm, tokens, pos, B, kv_cache, T_cache, logits, ldl, b, s);
+  if (lm->arch == SK_ARCH_NEOX) return neox_decode_step(lm, tokens, pos, B, kv_cache, T_cache, logits, ldl, b, s);
+  if (lm->post_ln) return opt_postln_decode_step(lm, tokens, pos, B, kv_cache, T_cache, logits, ldl, b, s);
+  return opt_decode_step(lm, tokens, pos, B, kv_cache, T_cache, logits, ldl, b, s);
 }
 
 }  // namespace
@@ -1481,27 +1424,29 @@ int sk_lm_prefill(SkLm* lm, const int64_t* ids, const int32_t* lens, int B, int 
   const WsLayout w = layout_of(lm, B, T);
   SK_TRY(check_bound(lm, B, T, w, nullptr));
   cudaStream_t s = (cudaStream_t)stream;
-  uint8_t* dws = reinterpret_cast<uint8_t*>(decode_ws);
-  SK_CUDA_CHECK(cudaMemsetAsync(dws + dl.gemm + dl.gemm_bytes - 4096, 0, 4096, s));
+  const DecBufs b = dec_bufs(decode_ws, dl);
+  SK_CUDA_CHECK(cudaMemsetAsync(reinterpret_cast<uint8_t*>(b.gemm) + b.gemm_bytes - 4096, 0, 4096, s));
+  FwdArgs a{ids, nullptr, nullptr, B, T};
+  a.with_head = false;
+  if (lm->fp32) {
+    a.kv = reinterpret_cast<float*>(kv_cache);
+    a.lens = lens;
+    a.T_cache = T_cache;
+  }
+  SK_TRY(forward(lm, a, w, s));
   const int K = head_k(lm);
   if (lm->fp32) {
-    Pair hf{nullptr, nullptr};   // the head input rows
-    SK_TRY(opt_forward_fp32(lm, ids, B, T, w, s, false, reinterpret_cast<float*>(kv_cache), lens, T_cache, &hf));
-    const int64_t n = (int64_t)B * lm->d;
-    const Pair hl{reinterpret_cast<bf16*>(dws + dl.h), reinterpret_cast<bf16*>(dws + dl.h) + n};
+    const Pair hf = head_in_fp32(lm, w);
+    const Pair hl{b.h, b.h + (int64_t)B * lm->d};
     SK_TRY(sk_gather_last_launch(hf.hi, lens, hl.hi, B, T, K, s));
     SK_TRY(sk_gather_last_launch(hf.lo, lens, hl.lo, B, T, K, s));
     return linear_split(lm, B, lm->Vp, K, hl, lm->off_head, -1, 0, nullptr, Pair{nullptr, nullptr},
                         reinterpret_cast<float*>(logits), ldl, s);
   }
-  if (lm->arch == SK_ARCH_OPT)       SK_TRY(opt_forward(lm, ids, nullptr, nullptr, B, T, 0.f, 1.f, false, nullptr, w, s, nullptr, false));
-  else if (lm->arch == SK_ARCH_NEOX) SK_TRY(neox_forward(lm, ids, nullptr, nullptr, B, T, 0.f, 1.f, false, nullptr, w, s, nullptr, false));
-  else                               SK_TRY(forward_impl(lm, ids, nullptr, nullptr, B, T, 0.f, 1.f, false, nullptr, w, s, nullptr, false));
   SK_TRY(sk_kv_prefill_launch(wsp<bf16>(lm, w.qkv), w.sqkv / 2, lm->qkv_dim, reinterpret_cast<bf16*>(kv_cache), lens, lm->L, B,
                               T, lm->H, lm->KVH, T_cache, s));
-  bf16* hl = reinterpret_cast<bf16*>(dws + dl.h);
-  SK_TRY(sk_gather_last_launch(head_in(lm, w), lens, hl, B, T, K, s));
-  return sk_gemm_launch(B, lm->Vp, K, hl, K, 0, lm->params + lm->off_head, K, 0, logits, ldl, 0, nullptr, nullptr,
+  SK_TRY(sk_gather_last_launch(head_in(lm, w), lens, b.h, B, T, K, s));
+  return sk_gemm_launch(B, lm->Vp, K, b.h, K, 0, lm->params + lm->off_head, K, 0, logits, ldl, 0, nullptr, nullptr,
                         0, 0, 0, 0, s);
 }
 
@@ -1519,51 +1464,7 @@ int sk_lm_decode_step(SkLm* lm, const int64_t* tokens, const int32_t* pos, int B
                           "saved checkpoint with a handle that has no master weights");
   const DecLayout dl = make_dec_layout(lm, B, T_cache);
   SK_TRY(check_decode(lm, B, T_cache, ldl, kv_cache, logits, decode_ws, decode_ws_bytes, dl));
-  cudaStream_t s = (cudaStream_t)stream;
-  if (lm->fp32)
-    return opt_decode_step_fp32(lm, tokens, pos, B, reinterpret_cast<float*>(kv_cache), T_cache, reinterpret_cast<float*>(logits),
-                                ldl, reinterpret_cast<uint8_t*>(decode_ws), dl, s);
-  if (lm->arch == SK_ARCH_OPT)
-    return opt_decode_step(lm, tokens, pos, B, kv_cache, T_cache, logits, ldl, reinterpret_cast<uint8_t*>(decode_ws), dl, s);
-  if (lm->arch == SK_ARCH_NEOX)
-    return neox_decode_step(lm, tokens, pos, B, kv_cache, T_cache, logits, ldl, reinterpret_cast<uint8_t*>(decode_ws), dl, s);
-  const int d = lm->d, F = lm->F, Q = lm->qkv_dim;
-  const bf16* P = lm->params;
-  uint8_t* dws = reinterpret_cast<uint8_t*>(decode_ws);
-  bf16* x = reinterpret_cast<bf16*>(dws + dl.x0);
-  bf16* xm = reinterpret_cast<bf16*>(dws + dl.x1);
-  bf16* h = reinterpret_cast<bf16*>(dws + dl.h);
-  bf16* qkv = reinterpret_cast<bf16*>(dws + dl.qkv);
-  bf16* ao = reinterpret_cast<bf16*>(dws + dl.ao);
-  bf16* gu = reinterpret_cast<bf16*>(dws + dl.gu);
-  bf16* act = reinterpret_cast<bf16*>(dws + dl.act);
-  int32_t* lens = reinterpret_cast<int32_t*>(dws + dl.lens);
-  float* partial = reinterpret_cast<float*>(dws + dl.partial);
-  void* gemm_ws = dws + dl.gemm;
-  const size_t plane = (size_t)B * lm->KVH * T_cache * lm->hd;
-  const float scale = 1.0f / sqrtf((float)lm->hd);
-  SK_TRY(sk_embed_fwd_launch(tokens, P + lm->off_embed, x, B, d, lm->V, s));
-  for (int l = 0; l < lm->L; ++l) {
-    const LayerOff& o = lm->lo[l];
-    bf16* kc = reinterpret_cast<bf16*>(kv_cache) + (size_t)l * 2 * plane;
-    bf16* vc = kc + plane;
-    SK_TRY(sk_rmsnorm_fwd_launch(x, P + o.ln1, h, nullptr, B, d, lm->cfg.rms_eps, s));
-    SK_TRY(sk_linear_rope_launch(B, Q, d, h, P + o.wqkv, lm->cfg.qkv_bias ? P + o.bqkv : nullptr, qkv, lm->rope_cos,
-                                 lm->rope_sin, pos, 1, (lm->H + lm->KVH) * lm->hd, lm->cfg.max_positions, s));
-    SK_TRY(sk_kv_append_launch(qkv, Q, kc, vc, pos, lens, B, lm->H, lm->KVH, T_cache, s));
-    SK_TRY(sk_attn_decode_launch(qkv, Q, kc, vc, lens, ao, d, partial, B, lm->H, lm->KVH, T_cache, scale, s));
-    SK_TRY(linear_fwd(B, d, d, ao, P + o.wo, xm, nullptr, x, s));
-    SK_TRY(sk_rmsnorm_fwd_launch(xm, P + o.ln2, h, nullptr, B, d, lm->cfg.rms_eps, s));
-    SK_TRY(sk_linear_swiglu_fwd_launch(B, F, d, h, P + o.wgu, gu, act, s));
-    // down projection added in place (residual == output): with M = B there is a single row of output tiles, so the
-    // scratch lets the GEMM split its long K loop over idle SMs (fixed-order reduction); rounded before the residual
-    // add like the forward pass's down projection
-    SK_TRY(sk_gemm_launch(B, d, F, act, F, 0, P + o.wd, F, 0, xm, d, 0, nullptr, xm, d, 1, 0, 0, s, gemm_ws,
-                          (size_t)dl.gemm_bytes));
-    std::swap(x, xm);
-  }
-  SK_TRY(sk_rmsnorm_fwd_launch(x, P + lm->off_final_norm, h, nullptr, B, d, lm->cfg.rms_eps, s));
-  return sk_gemm_launch(B, lm->Vp, d, h, d, 0, P + lm->off_head, d, 0, logits, ldl, 0, nullptr, nullptr, 0, 0, 0, 0, s);
+  return decode_step(lm, tokens, pos, B, kv_cache, T_cache, logits, ldl, dec_bufs(decode_ws, dl), (cudaStream_t)stream);
 }
 
 int sk_lm_create(const SkLmConfig* cfg, SkLm** out) {
@@ -1574,85 +1475,55 @@ int sk_lm_create(const SkLmConfig* cfg, SkLm** out) {
   SK_REQUIRE(cfg->n_heads % cfg->n_kv_heads == 0, "sk_lm_create: n_heads must be a multiple of n_kv_heads");
   SK_REQUIRE(cfg->vocab_size > 0 && cfg->vocab_size <= (1 << 20),
              "sk_lm_create: vocab_size must be in [1, 2^20] (unit vocabularies are ~502, interleaved text+unit ones ~152 k)");
-  SkLm* lm = new SkLm();
-  lm->cfg = *cfg;
-  lm->d = cfg->hidden;
-  lm->F = cfg->ffn;
-  lm->H = cfg->n_heads;
-  lm->KVH = cfg->n_kv_heads;
-  lm->hd = cfg->head_dim;
-  lm->L = cfg->n_layers;
-  lm->V = cfg->vocab_size;
-  lm->Vp = (cfg->vocab_size + 63) / 64 * 64;
-  lm->qkv_dim = (lm->H + 2 * lm->KVH) * lm->hd;
-  // text+unit vocabularies: chunked lm_head + CE (SK_HEAD_CHUNK=rows overrides, 0 turns it off)
-  lm->head_chunk = lm->Vp > 8192 ? 2048 : 0;
-  if (const char* e = getenv("SK_HEAD_CHUNK")) lm->head_chunk = (atoi(e) / 128) * 128;
+  SK_REQUIRE(cfg->n_heads * cfg->head_dim == cfg->hidden, "sk_lm_create: n_heads*head_dim must equal hidden");
+  SkLm* lm = new_lm(SK_ARCH_QWEN2, cfg->vocab_size, cfg->hidden, cfg->n_layers, cfg->n_heads, cfg->n_kv_heads, cfg->ffn,
+                    cfg->max_positions, cfg->rms_eps, cfg->tie_embeddings != 0, cfg->qkv_bias != 0);
+  const int d = lm->d, F = lm->F;
   lm->lo.resize(lm->L);
   for (int l = 0; l < lm->L; ++l) {
     const std::string p = "layers." + std::to_string(l) + ".";
     LayerOff& o = lm->lo[l];
-    o.ln1 = add_tensor(lm, p + "ln1", 1, lm->d);
-    o.wqkv = add_tensor(lm, p + "wqkv", lm->qkv_dim, lm->d);
+    o.ln1 = add_tensor(lm, p + "ln1", 1, d);
+    o.wqkv = add_tensor(lm, p + "wqkv", lm->qkv_dim, d);
     o.bqkv = add_tensor(lm, p + "bqkv", 1, lm->qkv_dim);
-    o.wo = add_tensor(lm, p + "wo", lm->d, lm->H * lm->hd);
-    o.ln2 = add_tensor(lm, p + "ln2", 1, lm->d);
-    o.wgu = add_tensor(lm, p + "wgu", 2 * lm->F, lm->d);
-    o.wd = add_tensor(lm, p + "wd", lm->d, lm->F);
+    o.wo = add_tensor(lm, p + "wo", d, lm->H * lm->hd);
+    o.ln2 = add_tensor(lm, p + "ln2", 1, d);
+    o.wgu = add_tensor(lm, p + "wgu", 2 * F, d);
+    o.wd = add_tensor(lm, p + "wd", d, F);
   }
-  lm->off_final_norm = add_tensor(lm, "final_norm", 1, lm->d);
-  lm->off_embed = add_tensor(lm, "embed", lm->Vp, lm->d);
-  lm->off_head = cfg->tie_embeddings ? lm->off_embed : add_tensor(lm, "lm_head", lm->Vp, lm->d);
-  SK_REQUIRE(lm->H * lm->hd == lm->d, "sk_lm_create: n_heads*head_dim must equal hidden");
+  lm->off_final_norm = add_tensor(lm, "final_norm", 1, d);
+  lm->off_embed = add_tensor(lm, "embed", lm->Vp, d);
+  lm->off_head = lm->tie ? lm->off_embed : add_tensor(lm, "lm_head", lm->Vp, d);
 
-  // gradient-norm chunk tables.  torch.nn.utils.clip_grad_norm_ takes one norm per PARAMETER (rounded to bf16 on bf16
-  // gradients), and HF keeps q/k/v and gate/up as separate parameters: a norm group here is one HF parameter, i.e. a
-  // list of element ranges of the flat buffer (q, k, v are row ranges of wqkv / bqkv; gate and up alternate in 128-row
-  // blocks of wgu).  Chunks are listed group by group, so a group is a contiguous run of the chunk table.
-  std::vector<long> cs;
-  std::vector<int> cl, tb;
-  auto add_range = [&](int64_t off, int64_t n) {
-    for (int64_t o = 0; o < n; o += GN_CHUNK) {
-      cs.push_back((long)(off + o));
-      cl.push_back((int)((n - o) < GN_CHUNK ? (n - o) : GN_CHUNK));
-    }
-  };
-  auto begin_group = [&]() { tb.push_back((int)cs.size()); };
+  // torch.nn.utils.clip_grad_norm_ takes one norm per PARAMETER (rounded to bf16 on bf16 gradients), and HF keeps q/k/v
+  // and gate/up as separate parameters: q, k, v are row ranges of wqkv / bqkv; gate and up alternate in 128-row blocks
+  // of wgu
+  NormGroups groups;
+  auto one = [&](int64_t off, int64_t n) { groups.push_back({{off, n}}); };
   const int64_t qd = (int64_t)lm->H * lm->hd, kvd = (int64_t)lm->KVH * lm->hd;
   for (int l = 0; l < lm->L; ++l) {
     const LayerOff& o = lm->lo[l];
-    begin_group(); add_range(o.ln1, lm->d);
-    begin_group(); add_range(o.wqkv, qd * lm->d);
-    begin_group(); add_range(o.wqkv + qd * lm->d, kvd * lm->d);
-    begin_group(); add_range(o.wqkv + (qd + kvd) * lm->d, kvd * lm->d);
-    if (cfg->qkv_bias) {
-      begin_group(); add_range(o.bqkv, qd);
-      begin_group(); add_range(o.bqkv + qd, kvd);
-      begin_group(); add_range(o.bqkv + qd + kvd, kvd);
+    one(o.ln1, d);
+    one(o.wqkv, qd * d);
+    one(o.wqkv + qd * d, kvd * d);
+    one(o.wqkv + (qd + kvd) * d, kvd * d);
+    if (lm->qkv_bias) {
+      one(o.bqkv, qd);
+      one(o.bqkv + qd, kvd);
+      one(o.bqkv + qd + kvd, kvd);
     }
-    begin_group(); add_range(o.wo, (int64_t)lm->d * lm->d);
-    begin_group(); add_range(o.ln2, lm->d);
+    one(o.wo, (int64_t)d * d);
+    one(o.ln2, d);
     for (int half = 0; half < 2; ++half) {   // gate, then up
-      begin_group();
-      for (int b = 0; b < lm->F / 128; ++b) add_range(o.wgu + ((int64_t)b * 256 + half * 128) * lm->d, (int64_t)128 * lm->d);
+      groups.emplace_back();
+      for (int b = 0; b < F / 128; ++b) groups.back().push_back({o.wgu + ((int64_t)b * 256 + half * 128) * d, (int64_t)128 * d});
     }
-    begin_group(); add_range(o.wd, (int64_t)lm->d * lm->F);
+    one(o.wd, (int64_t)d * F);
   }
-  begin_group(); add_range(lm->off_final_norm, lm->d);
-  begin_group(); add_range(lm->off_embed, (int64_t)lm->Vp * lm->d);
-  if (!cfg->tie_embeddings) { begin_group(); add_range(lm->off_head, (int64_t)lm->Vp * lm->d); }
-  lm->n_norm_groups = (int)tb.size();
-  tb.push_back((int)cs.size());
-  lm->n_chunks = (int)cs.size();
-  SK_CUDA_CHECK(cudaMalloc(&lm->d_chunk_start, cs.size() * sizeof(long)));
-  SK_CUDA_CHECK(cudaMalloc(&lm->d_chunk_len, cl.size() * sizeof(int)));
-  SK_CUDA_CHECK(cudaMalloc(&lm->d_tensor_chunk_begin, tb.size() * sizeof(int)));
-  SK_CUDA_CHECK(cudaMalloc(&lm->d_chunk_partial, cs.size() * sizeof(float)));
-  SK_CUDA_CHECK(cudaMemcpy(lm->d_chunk_start, cs.data(), cs.size() * sizeof(long), cudaMemcpyHostToDevice));
-  SK_CUDA_CHECK(cudaMemcpy(lm->d_chunk_len, cl.data(), cl.size() * sizeof(int), cudaMemcpyHostToDevice));
-  SK_CUDA_CHECK(cudaMemcpy(lm->d_tensor_chunk_begin, tb.data(), tb.size() * sizeof(int), cudaMemcpyHostToDevice));
-  *out = lm;
-  return 0;
+  one(lm->off_final_norm, d);
+  one(lm->off_embed, (int64_t)lm->Vp * d);
+  if (!lm->tie) one(lm->off_head, (int64_t)lm->Vp * d);
+  return publish(lm, groups, out);
 }
 
 int sk_lm_create_opt(const SkOptConfig* cfg, SkLm** out) {
@@ -1669,38 +1540,17 @@ int sk_lm_create_opt(const SkOptConfig* cfg, SkLm** out) {
                                     "the post-LayerNorm decoder only (post_ln = 1)", cfg->proj_dim, cfg->hidden);
   SK_REQUIRE(!proj || (cfg->proj_dim > 0 && cfg->proj_dim % 64 == 0 && cfg->proj_dim < cfg->hidden),
              "sk_lm_create_opt: proj_dim must be a positive multiple of 64 below hidden (got %d)", cfg->proj_dim);
-  SkLm* lm = new SkLm();
-  lm->arch = SK_ARCH_OPT;
+  SkLm* lm = new_lm(SK_ARCH_OPT, cfg->vocab_size, cfg->hidden, cfg->n_layers, cfg->n_heads, cfg->n_heads, cfg->ffn,
+                    cfg->max_positions, cfg->ln_eps, cfg->tie_embeddings != 0, true);
   lm->post_ln = cfg->post_ln != 0;
   lm->proj = proj;
   lm->pw = proj ? cfg->proj_dim : cfg->hidden;
-  lm->cfg.vocab_size = cfg->vocab_size;
-  lm->cfg.hidden = cfg->hidden;
-  lm->cfg.n_layers = cfg->n_layers;
-  lm->cfg.n_heads = cfg->n_heads;
-  lm->cfg.n_kv_heads = cfg->n_heads;
-  lm->cfg.head_dim = 64;
-  lm->cfg.ffn = cfg->ffn;
-  lm->cfg.max_positions = cfg->max_positions;
-  lm->cfg.rms_eps = cfg->ln_eps;
-  lm->cfg.tie_embeddings = cfg->tie_embeddings;
-  lm->cfg.qkv_bias = 1;
-  lm->d = cfg->hidden;
-  lm->F = cfg->ffn;
-  lm->H = lm->KVH = cfg->n_heads;
-  lm->hd = 64;
-  lm->L = cfg->n_layers;
-  lm->V = cfg->vocab_size;
-  lm->Vp = (cfg->vocab_size + 63) / 64 * 64;
-  lm->qkv_dim = 3 * lm->d;
   lm->n_pos = cfg->max_positions + 2;   // OPTLearnedPositionalEmbedding: offset 2
-  lm->head_chunk = lm->Vp > 8192 ? 2048 : 0;
-  if (const char* e = getenv("SK_HEAD_CHUNK")) lm->head_chunk = (atoi(e) / 128) * 128;
-  const int d = lm->d, F = lm->F;
-  lm->olo.resize(lm->L);
+  const int d = lm->d, F = lm->F, pw = lm->pw;
+  lm->lnl.resize(lm->L);
   for (int l = 0; l < lm->L; ++l) {
     const std::string p = "layers." + std::to_string(l) + ".";
-    OptLayerOff& o = lm->olo[l];
+    LnLayerOff& o = lm->lnl[l];
     o.ln1w = add_tensor(lm, p + "ln1", 1, d);
     o.ln1b = add_tensor(lm, p + "ln1_b", 1, d);
     o.wqkv = add_tensor(lm, p + "wqkv", 3 * d, d);
@@ -1714,7 +1564,6 @@ int sk_lm_create_opt(const SkOptConfig* cfg, SkLm** out) {
     o.w2 = add_tensor(lm, p + "w2", d, F);
     o.b2 = add_tensor(lm, p + "b2", 1, d);
   }
-  const int pw = lm->pw;
   if (!lm->post_ln) {   // post-LN OPT has no decoder-level final LayerNorm
     lm->off_final_norm = add_tensor(lm, "final_norm", 1, d);
     lm->off_final_norm_b = add_tensor(lm, "final_norm_b", 1, d);
@@ -1725,10 +1574,10 @@ int sk_lm_create_opt(const SkOptConfig* cfg, SkLm** out) {
     lm->off_pin = add_tensor(lm, "proj_in", d, pw);
     lm->off_pout = add_tensor(lm, "proj_out", pw, d);
   }
-  lm->off_head = cfg->tie_embeddings ? lm->off_embed : add_tensor(lm, "lm_head", lm->Vp, pw);
+  lm->off_head = lm->tie ? lm->off_embed : add_tensor(lm, "lm_head", lm->Vp, pw);
   // one gradient-norm group per HF parameter, weights and biases apart (torch clip_grad_norm_ over OPTForCausalLM, whose
   // decoder lists embed_tokens, embed_positions, project_out, project_in, then the layers)
-  std::vector<std::vector<std::pair<int64_t, int64_t>>> groups;
+  NormGroups groups;
   auto one = [&](int64_t off, int64_t n) { groups.push_back({{off, n}}); };
   const int64_t dd = (int64_t)d * d;
   one(lm->off_embed, (int64_t)lm->Vp * pw);
@@ -1738,7 +1587,7 @@ int sk_lm_create_opt(const SkOptConfig* cfg, SkLm** out) {
     one(lm->off_pin, (int64_t)d * pw);
   }
   for (int l = 0; l < lm->L; ++l) {
-    const OptLayerOff& o = lm->olo[l];
+    const LnLayerOff& o = lm->lnl[l];
     for (int j = 0; j < 3; ++j) {   // q, k, v
       one(o.wqkv + j * dd, dd);
       one(o.bqkv + (int64_t)j * d, d);
@@ -1753,14 +1602,8 @@ int sk_lm_create_opt(const SkOptConfig* cfg, SkLm** out) {
     one(lm->off_final_norm, d);
     one(lm->off_final_norm_b, d);
   }
-  if (!cfg->tie_embeddings) one(lm->off_head, (int64_t)lm->Vp * pw);
-  const int rc = upload_norm_groups(lm, groups);
-  if (rc) {
-    sk_lm_destroy(lm);
-    return rc;
-  }
-  *out = lm;
-  return 0;
+  if (!lm->tie) one(lm->off_head, (int64_t)lm->Vp * pw);
+  return publish(lm, groups, out);
 }
 
 int sk_lm_create_neox(const SkNeoxConfig* cfg, SkLm** out) {
@@ -1773,35 +1616,14 @@ int sk_lm_create_neox(const SkNeoxConfig* cfg, SkLm** out) {
              "sk_lm_create_neox: rot_dims (rotary_ndims) must be 16, 32 or 64 (got %d)", cfg->rot_dims);
   SK_REQUIRE(cfg->n_layers > 0 && cfg->max_positions > 0, "sk_lm_create_neox: n_layers and max_positions must be positive");
   SK_REQUIRE(cfg->vocab_size > 0 && cfg->vocab_size <= (1 << 20), "sk_lm_create_neox: vocab_size must be in [1, 2^20]");
-  SkLm* lm = new SkLm();
-  lm->arch = SK_ARCH_NEOX;
-  lm->cfg.vocab_size = cfg->vocab_size;
-  lm->cfg.hidden = cfg->hidden;
-  lm->cfg.n_layers = cfg->n_layers;
-  lm->cfg.n_heads = cfg->n_heads;
-  lm->cfg.n_kv_heads = cfg->n_heads;
-  lm->cfg.head_dim = 64;
-  lm->cfg.ffn = cfg->ffn;
-  lm->cfg.max_positions = cfg->max_positions;
-  lm->cfg.rms_eps = cfg->ln_eps;
-  lm->cfg.tie_embeddings = 0;
-  lm->cfg.qkv_bias = 1;
-  lm->d = cfg->hidden;
-  lm->F = cfg->ffn;
-  lm->H = lm->KVH = cfg->n_heads;
-  lm->hd = 64;
+  SkLm* lm = new_lm(SK_ARCH_NEOX, cfg->vocab_size, cfg->hidden, cfg->n_layers, cfg->n_heads, cfg->n_heads, cfg->ffn,
+                    cfg->max_positions, cfg->ln_eps, false, true);
   lm->rot = cfg->rot_dims;
-  lm->L = cfg->n_layers;
-  lm->V = cfg->vocab_size;
-  lm->Vp = (cfg->vocab_size + 63) / 64 * 64;
-  lm->qkv_dim = 3 * lm->d;
-  lm->head_chunk = lm->Vp > 8192 ? 2048 : 0;
-  if (const char* e = getenv("SK_HEAD_CHUNK")) lm->head_chunk = (atoi(e) / 128) * 128;
   const int d = lm->d, F = lm->F;
-  lm->nlo.resize(lm->L);
+  lm->lnl.resize(lm->L);
   for (int l = 0; l < lm->L; ++l) {
     const std::string p = "layers." + std::to_string(l) + ".";
-    NeoxLayerOff& o = lm->nlo[l];
+    LnLayerOff& o = lm->lnl[l];
     o.ln1w = add_tensor(lm, p + "ln1", 1, d);
     o.ln1b = add_tensor(lm, p + "ln1_b", 1, d);
     o.ln2w = add_tensor(lm, p + "ln2", 1, d);
@@ -1820,12 +1642,12 @@ int sk_lm_create_neox(const SkNeoxConfig* cfg, SkLm** out) {
   lm->off_embed = add_tensor(lm, "embed", lm->Vp, d);
   lm->off_head = add_tensor(lm, "lm_head", lm->Vp, d);
   // one gradient-norm group per HF parameter, in GPTNeoXForCausalLM.parameters() order (query_key_value is one tensor)
-  std::vector<std::vector<std::pair<int64_t, int64_t>>> groups;
+  NormGroups groups;
   auto one = [&](int64_t off, int64_t n) { groups.push_back({{off, n}}); };
   const int64_t dd = (int64_t)d * d;
   one(lm->off_embed, (int64_t)lm->Vp * d);
   for (int l = 0; l < lm->L; ++l) {
-    const NeoxLayerOff& o = lm->nlo[l];
+    const LnLayerOff& o = lm->lnl[l];
     one(o.ln1w, d); one(o.ln1b, d);
     one(o.ln2w, d); one(o.ln2b, d);
     one(o.wqkv, 3 * dd); one(o.bqkv, 3 * d);
@@ -1836,13 +1658,7 @@ int sk_lm_create_neox(const SkNeoxConfig* cfg, SkLm** out) {
   one(lm->off_final_norm, d);
   one(lm->off_final_norm_b, d);
   one(lm->off_head, (int64_t)lm->Vp * d);
-  const int rc = upload_norm_groups(lm, groups);
-  if (rc) {
-    sk_lm_destroy(lm);
-    return rc;
-  }
-  *out = lm;
-  return 0;
+  return publish(lm, groups, out);
 }
 
 void sk_lm_destroy(SkLm* lm) {
@@ -1917,12 +1733,12 @@ int sk_lm_set_master(SkLm* lm, float* params32, float* grads32) {
     // the layout), plus an untied lm_head; the tied lm_head's gradient is folded into the embedding's
     std::vector<std::pair<int64_t, int64_t>> ranges;
     for (int l = 0; l < lm->L; ++l) {
-      const OptLayerOff& o = lm->olo[l];
+      const LnLayerOff& o = lm->lnl[l];
       ranges.push_back({o.wqkv, o.ln2w - o.wqkv});
-      const int64_t end = l + 1 < lm->L ? lm->olo[l + 1].ln1w : lm->off_final_norm;
+      const int64_t end = l + 1 < lm->L ? lm->lnl[l + 1].ln1w : lm->off_final_norm;
       ranges.push_back({o.w1, end - o.w1});
     }
-    if (!lm->cfg.tie_embeddings) ranges.push_back({lm->off_head, lm->n_params - lm->off_head});
+    if (!lm->tie) ranges.push_back({lm->off_head, lm->n_params - lm->off_head});
     std::vector<long> cs;
     std::vector<int> cl;
     for (const auto& r : ranges)
@@ -1980,20 +1796,15 @@ int sk_lm_forward(SkLm* lm, const int64_t* ids, const int64_t* labels, const int
                   float num_items, float* stats, void* stream) {
   SK_REQUIRE(lm && ids, "sk_lm_forward: null argument");
   SK_REQUIRE(labels == nullptr || stats != nullptr, "sk_lm_forward: stats is required when labels are given");
-  if (lm->fp32) {
-    SK_REQUIRE(labels == nullptr && pos_ids == nullptr, "sk_lm_forward: an fp32 inference handle (sk_lm_set_fp32) takes "
-                                                        "neither labels (score with sk_seq_loglik_f32) nor position_ids");
-    const WsLayout w = layout_of(lm, B, T);
-    SK_TRY(check_bound(lm, B, T, w, nullptr));
-    return opt_forward_fp32(lm, ids, B, T, w, (cudaStream_t)stream, true);
-  }
+  SK_REQUIRE(!lm->fp32 || (labels == nullptr && pos_ids == nullptr), "sk_lm_forward: an fp32 inference handle (sk_lm_set_fp32) "
+                                                                     "takes neither labels (score with sk_seq_loglik_f32) nor "
+                                                                     "position_ids");
   const WsLayout w = layout_of(lm, B, T);
   SK_TRY(check_bound(lm, B, T, w, pos_ids));
-  if (lm->arch == SK_ARCH_OPT)
-    return opt_forward(lm, ids, labels, pos_ids, B, T, num_items, 1.0f, false, stats, w, (cudaStream_t)stream);
-  if (lm->arch == SK_ARCH_NEOX)
-    return neox_forward(lm, ids, labels, pos_ids, B, T, num_items, 1.0f, false, stats, w, (cudaStream_t)stream);
-  return forward_impl(lm, ids, labels, pos_ids, B, T, num_items, 1.0f, false, stats, w, (cudaStream_t)stream);
+  FwdArgs a{ids, labels, pos_ids, B, T};
+  a.num_items = num_items;
+  a.stats = stats;
+  return forward(lm, a, w, (cudaStream_t)stream);
 }
 
 int sk_lm_forward_backward(SkLm* lm, const int64_t* ids, const int64_t* labels, const int32_t* pos_ids, int B, int T,
@@ -2004,34 +1815,13 @@ int sk_lm_forward_backward(SkLm* lm, const int64_t* ids, const int64_t* labels, 
   SK_REQUIRE(!lm->master || lm->grads32, "sk_lm_forward_backward: no fp32 gradient buffer given to sk_lm_set_master");
   const WsLayout w = layout_of(lm, B, T);
   SK_TRY(check_bound(lm, B, T, w, pos_ids));
-  if (lm->arch == SK_ARCH_OPT) {
-    cudaStream_t s = (cudaStream_t)stream;
-    if (lm->head_chunk > 0) {
-      SK_TRY(opt_forward(lm, ids, labels, pos_ids, B, T, num_items, dloss, true, stats, w, s, nullptr, false));
-      // master weights: the bf16 gradient buffer holds one micro-batch (grads32 accumulates)
-      SK_TRY(head_chunked(lm, labels, B, T, num_items, dloss, lm->master ? 0 : accumulate, stats, w, s));
-      return opt_backward(lm, ids, pos_ids, B, T, accumulate, w, s, false);
-    }
-    SK_TRY(opt_forward(lm, ids, labels, pos_ids, B, T, num_items, dloss, true, stats, w, s));
-    return opt_backward(lm, ids, pos_ids, B, T, accumulate, w, s);
-  }
-  if (lm->arch == SK_ARCH_NEOX) {
-    cudaStream_t s = (cudaStream_t)stream;
-    if (lm->head_chunk > 0) {
-      SK_TRY(neox_forward(lm, ids, labels, pos_ids, B, T, num_items, dloss, true, stats, w, s, nullptr, false));
-      SK_TRY(head_chunked(lm, labels, B, T, num_items, dloss, accumulate, stats, w, s));
-      return neox_backward(lm, ids, pos_ids, B, T, accumulate, w, s, false);
-    }
-    SK_TRY(neox_forward(lm, ids, labels, pos_ids, B, T, num_items, dloss, true, stats, w, s));
-    return neox_backward(lm, ids, pos_ids, B, T, accumulate, w, s);
-  }
-  if (lm->head_chunk > 0) {
-    SK_TRY(forward_impl(lm, ids, labels, pos_ids, B, T, num_items, dloss, true, stats, w, (cudaStream_t)stream, nullptr, false));
-    SK_TRY(head_chunked(lm, labels, B, T, num_items, dloss, accumulate, stats, w, (cudaStream_t)stream));
-    return backward_impl(lm, ids, pos_ids, B, T, accumulate, w, (cudaStream_t)stream, false);
-  }
-  SK_TRY(forward_impl(lm, ids, labels, pos_ids, B, T, num_items, dloss, true, stats, w, (cudaStream_t)stream));
-  return backward_impl(lm, ids, pos_ids, B, T, accumulate, w, (cudaStream_t)stream);
+  cudaStream_t s = (cudaStream_t)stream;
+  FwdArgs a{ids, labels, pos_ids, B, T, num_items, dloss, true, stats};
+  a.with_head = lm->head_chunk == 0;
+  SK_TRY(forward(lm, a, w, s));
+  // master weights: the bf16 gradient buffer holds one micro-batch (grads32 accumulates)
+  if (!a.with_head) SK_TRY(head_chunked(lm, a, lm->master ? 0 : accumulate, w, s));
+  return backward(lm, a, accumulate, w, s);
 }
 
 int sk_lm_set_backward_events(SkLm* lm, void* const* events, int n) {
@@ -2052,11 +1842,8 @@ int sk_lm_forward_rows(SkLm* lm, const int64_t* ids, const int64_t* labels, cons
   SK_REFUSE_FP32(lm, "sk_lm_forward_rows");
   const WsLayout w = layout_of(lm, B, T);
   SK_TRY(check_bound(lm, B, T, w, pos_ids));
-  if (lm->arch == SK_ARCH_OPT)
-    return opt_forward(lm, ids, labels, pos_ids, B, T, 1.0f, 1.0f, false, stats, w, (cudaStream_t)stream, row_nll);
-  if (lm->arch == SK_ARCH_NEOX)
-    return neox_forward(lm, ids, labels, pos_ids, B, T, 1.0f, 1.0f, false, stats, w, (cudaStream_t)stream, row_nll);
-  return forward_impl(lm, ids, labels, pos_ids, B, T, 1.0f, 1.0f, false, stats, w, (cudaStream_t)stream, row_nll);
+  FwdArgs a{ids, labels, pos_ids, B, T, 1.0f, 1.0f, false, stats, row_nll};
+  return forward(lm, a, w, (cudaStream_t)stream);
 }
 
 int sk_lm_backward_weighted(SkLm* lm, const int64_t* ids, const int64_t* labels, const int32_t* pos_ids, int B, int T,
@@ -2073,9 +1860,7 @@ int sk_lm_backward_weighted(SkLm* lm, const int64_t* ids, const int64_t* labels,
   // the workspace (num_items = 1, dloss = 1: the caller's weights carry every scale factor)
   SK_TRY(sk_ce_launch(wsp<bf16>(lm, w.logits), labels, wsp<bf16>(lm, w.dlogits), wsp<float>(lm, w.ce_partial), nullptr,
                       stats, B * T, T, lm->V, lm->Vp, 1.0f, 1.0f, s, row_weight));
-  if (lm->arch == SK_ARCH_OPT) return opt_backward(lm, ids, pos_ids, B, T, accumulate, w, s);
-  if (lm->arch == SK_ARCH_NEOX) return neox_backward(lm, ids, pos_ids, B, T, accumulate, w, s);
-  return backward_impl(lm, ids, pos_ids, B, T, accumulate, w, s);
+  return backward(lm, FwdArgs{ids, labels, pos_ids, B, T}, accumulate, w, s);
 }
 
 const void* sk_lm_logits(const SkLm* lm) {
