@@ -134,8 +134,9 @@ int sk_linear_gelu_fwd(int M, int F, int K, const void* x, const void* w1, const
 int sk_linear_gelu_bwd(int M, int N, int F, const void* dy, const void* w2, const void* pre, void* dpre, void* stream);
 int sk_linear_res2(int M, int N, int K, const void* x, const void* w, const void* bias, const void* res2, const void* res,
                    void* out, void* ws, int64_t ws_bytes, void* stream);
-/* Test hook: the schedule of the four launches above (kind 0 rope_partial, 1 gelu_fwd, 2 gelu_bwd, 3 res2 with the
- * scratch of sk_gemm_ws_bytes() when with_ws), for an M x N x K problem; nothing is launched. */
+/* Test hook: the schedule of a fused linear for an M x N x K problem (the GEMM's own M, N, K); nothing is launched.
+ * kind 0 rope_partial, 1 gelu_fwd, 2 gelu_bwd, 3 res2 with the scratch of sk_gemm_ws_bytes() when with_ws;
+ * 4 sk_linear_swiglu_fwd (N = 2F), 5 sk_linear_swiglu_bwd (N = F, K = the dy width), 6 sk_linear_rope. */
 int sk_neox_gemm_plan(int kind, int M, int N, int K, int with_ws, SkGemmPlan* plan);
 
 /* ---- causal-LM element-wise / reduction kernels (path (ii)) --------------------------------------------------- */

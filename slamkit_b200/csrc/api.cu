@@ -142,7 +142,7 @@ int sk_linear_res2(int M, int N, int K, const void* x, const void* w, const void
   return sk_linear_res2_launch(M, N, K, x, w, bias, res2, res, out, S(stream), ws, (size_t)ws_bytes);
 }
 int sk_neox_gemm_plan(int kind, int M, int N, int K, int with_ws, SkGemmPlan* plan) {
-  SK_REQUIRE(plan && kind >= 0 && kind <= 3, "sk_neox_gemm_plan: kind must be 0..3");
+  SK_REQUIRE(plan && kind >= 0 && kind <= 6, "sk_neox_gemm_plan: kind must be 0..6");
   // stand-in operands: 256-byte aligned, never dereferenced by the planner
   void* p = reinterpret_cast<void*>((uintptr_t)1 << 20);
   SkGemmEx g;
@@ -156,6 +156,16 @@ int sk_neox_gemm_plan(int kind, int M, int N, int K, int with_ws, SkGemmPlan* pl
     g.bias = p; g.epi = 4; g.aux_out = p; g.ld_aux_out = N;
   } else if (kind == 2) {
     g.ldb = N; g.b_mn = 1; g.epi = 5; g.aux = p; g.ld_aux = N;
+  } else if (kind == 4) {
+    // sk_linear_swiglu_fwd: N = 2F gate|up columns, act [M, F]
+    g.epi = 1; g.aux_out = p; g.ld_aux_out = N / 2;
+  } else if (kind == 5) {
+    // sk_linear_swiglu_bwd: N = F, d_gu [M, 2F] from the saved gu [M, 2F]
+    g.ldb = N; g.b_mn = 1; g.ldc = 2 * N; g.epi = 2; g.aux = p; g.ld_aux = 2 * N;
+  } else if (kind == 6) {
+    // sk_linear_rope, the Qwen2 q|k|v projection: full-rotary 64-column heads (rope_rot 0 = 64); the plan does not
+    // depend on how many of them rotate
+    g.bias = p; g.epi = 3; g.rope_cos = p; g.rope_sin = p; g.rope_T = 1; g.rope_cols = N; g.rope_maxpos = 1;
   } else {
     g.bias = p; g.residual = p; g.ldr = N; g.round_before_res = 1; g.epi = 6; g.aux = p; g.ld_aux = N;
     if (with_ws) { g.splitk_ws = p; g.splitk_ws_bytes = sk_gemm_ws_min_bytes(); }

@@ -160,11 +160,15 @@ SK_DEVINL float ex2_approx(float x) {
   return y;
 }
 
-// sigmoid / SiLU via ex2.approx + rcp.approx (relative error ~2e-7, far inside the bf16 rounding every use ends in)
+// sigmoid / SiLU via ex2.approx + rcp.approx (relative error ~2e-7, far inside the bf16 rounding every use ends in).
+// For x in (-88.72, -87.34) the sigmoid is an fp32 subnormal, which rcp.approx.ftz would flush to 0 (silu(x) = -0 where
+// torch's x / (1 + exp(-x)) is a normal number: -87.5, -88 and -88.5 in bf16).  So the reciprocal is taken of
+// (1 + e) * 2^-32 -- one fma, exact scaling, a normal result for every finite e -- and scaled back by a multiply that
+// keeps subnormals; e = inf (torch's exp overflow) still gives 0.  Cheaper than rcp.approx.f32's subnormal fix-up.
 SK_DEVINL float sigmoid_f(float x) {
   float r;
-  asm("rcp.approx.ftz.f32 %0, %1;" : "=f"(r) : "f"(1.0f + ex2_approx(x * -1.4426950408889634f)));
-  return r;
+  asm("rcp.approx.ftz.f32 %0, %1;" : "=f"(r) : "f"(fmaf(ex2_approx(x * -1.4426950408889634f), 0x1p-32f, 0x1p-32f)));
+  return r * 0x1p-32f;
 }
 SK_DEVINL float silu_f(float x) { return x * sigmoid_f(x); }
 
