@@ -104,21 +104,23 @@ int sk_gemm_bf16(int M, int N, int K, const void* A, int lda, int a_mn, const vo
                  int ldc, int out_f32, const void* bias, const void* residual, int ldr, int round_before_res, int act,
                  int force_bn, void* stream) {
   SK_REQUIRE(A && B && C, "sk_gemm_bf16: null operand");
-  return sk_gemm_launch(M, N, K, A, lda, a_mn, B, ldb, b_mn, C, ldc, out_f32, bias, residual, ldr, round_before_res, act,
-                        force_bn, S(stream));
+  return sk_gemm_ex_launch(sk_gemm_desc(M, N, K, A, lda, a_mn, B, ldb, b_mn, C, ldc, out_f32, bias, residual, ldr,
+                                        round_before_res, act, force_bn, nullptr, 0),
+                           S(stream));
 }
 int sk_linear_swiglu_fwd(int M, int F, int K, const void* x, const void* w_gu, void* gu, void* act, void* stream) {
   SK_REQUIRE(x && w_gu && gu && act, "sk_linear_swiglu_fwd: null operand");
-  return sk_linear_swiglu_fwd_launch(M, F, K, x, w_gu, gu, act, S(stream));
+  return sk_gemm_ex_launch(sk_gemm_swiglu_fwd(M, F, K, x, w_gu, gu, act), S(stream));
 }
 int sk_linear_swiglu_bwd(int M, int N, int F, const void* dy, const void* w_down, const void* gu, void* dgu, void* stream) {
   SK_REQUIRE(dy && w_down && gu && dgu, "sk_linear_swiglu_bwd: null operand");
-  return sk_linear_swiglu_bwd_launch(M, N, F, dy, w_down, gu, dgu, S(stream));
+  return sk_gemm_ex_launch(sk_gemm_swiglu_bwd(M, N, F, dy, w_down, gu, dgu), S(stream));
 }
 int sk_linear_rope(int M, int N, int K, const void* x, const void* w, const void* bias, void* out, const void* cos_t,
                    const void* sin_t, const int32_t* pos_ids, int T, int rope_cols, int max_positions, void* stream) {
   SK_REQUIRE(x && w && out && cos_t && sin_t, "sk_linear_rope: null operand");
-  return sk_linear_rope_launch(M, N, K, x, w, bias, out, cos_t, sin_t, pos_ids, T, rope_cols, max_positions, S(stream));
+  return sk_gemm_ex_launch(sk_gemm_rope(M, N, K, x, w, bias, out, cos_t, sin_t, pos_ids, T, rope_cols, max_positions, 0),
+                           S(stream));
 }
 int sk_linear_rope_partial(int M, int N, int K, const void* x, const void* w, const void* bias, void* out, const void* cos_t,
                            const void* sin_t, const int32_t* pos_ids, int T, int rope_cols, int max_positions, int rot_dims,
@@ -126,65 +128,58 @@ int sk_linear_rope_partial(int M, int N, int K, const void* x, const void* w, co
   SK_REQUIRE(x && w && out && cos_t && sin_t, "sk_linear_rope_partial: null operand");
   SK_REQUIRE(rot_dims == 16 || rot_dims == 32 || rot_dims == 64,
              "sk_linear_rope_partial: rot_dims=%d is not supported (16, 32 or 64)", rot_dims);
-  return sk_linear_rope_launch(M, N, K, x, w, bias, out, cos_t, sin_t, pos_ids, T, rope_cols, max_positions, S(stream), rot_dims);
+  return sk_gemm_ex_launch(sk_gemm_rope(M, N, K, x, w, bias, out, cos_t, sin_t, pos_ids, T, rope_cols, max_positions, rot_dims),
+                           S(stream));
 }
 int sk_linear_gelu_fwd(int M, int F, int K, const void* x, const void* w1, const void* b1, void* pre, void* act, void* stream) {
   SK_REQUIRE(x && w1 && pre && act, "sk_linear_gelu_fwd: null operand");
-  return sk_linear_gelu_fwd_launch(M, F, K, x, w1, b1, pre, act, S(stream));
+  return sk_gemm_ex_launch(sk_gemm_gelu_fwd(M, F, K, x, w1, b1, pre, act), S(stream));
 }
 int sk_linear_gelu_bwd(int M, int N, int F, const void* dy, const void* w2, const void* pre, void* dpre, void* stream) {
   SK_REQUIRE(dy && w2 && pre && dpre, "sk_linear_gelu_bwd: null operand");
-  return sk_linear_gelu_bwd_launch(M, N, F, dy, w2, pre, dpre, S(stream));
+  return sk_gemm_ex_launch(sk_gemm_gelu_bwd(M, N, F, dy, w2, pre, dpre), S(stream));
 }
 int sk_linear_res2(int M, int N, int K, const void* x, const void* w, const void* bias, const void* res2, const void* res,
                    void* out, void* ws, int64_t ws_bytes, void* stream) {
   SK_REQUIRE(x && w && res2 && res && out, "sk_linear_res2: null operand");
-  return sk_linear_res2_launch(M, N, K, x, w, bias, res2, res, out, S(stream), ws, (size_t)ws_bytes);
+  return sk_gemm_ex_launch(sk_gemm_res2(M, N, K, x, w, bias, res2, res, out, ws, (size_t)ws_bytes), S(stream));
 }
 int sk_neox_gemm_plan(int kind, int M, int N, int K, int with_ws, SkGemmPlan* plan) {
   SK_REQUIRE(plan && kind >= 0 && kind <= 6, "sk_neox_gemm_plan: kind must be 0..6");
-  // stand-in operands: 256-byte aligned, never dereferenced by the planner
+  // the descriptor each fused linear launches, on stand-in operands: 256-byte aligned, never dereferenced by the planner
   void* p = reinterpret_cast<void*>((uintptr_t)1 << 20);
   SkGemmEx g;
-  memset(&g, 0, sizeof(g));
-  g.M = M; g.N = N; g.K = K; g.batch = 1; g.passes = 1; g.pdl = 1;
-  g.A = p; g.lda = K; g.B = p; g.ldb = K; g.C = p; g.ldc = N;
-  if (kind == 0) {
-    // the fused q|k|v projection: q and k heads rotate
-    g.bias = p; g.epi = 3; g.rope_cos = p; g.rope_sin = p; g.rope_T = 1; g.rope_cols = N / 3 * 2; g.rope_maxpos = 1; g.rope_rot = 16;
-  } else if (kind == 1) {
-    g.bias = p; g.epi = 4; g.aux_out = p; g.ld_aux_out = N;
-  } else if (kind == 2) {
-    g.ldb = N; g.b_mn = 1; g.epi = 5; g.aux = p; g.ld_aux = N;
-  } else if (kind == 4) {
-    // sk_linear_swiglu_fwd: N = 2F gate|up columns, act [M, F]
-    g.epi = 1; g.aux_out = p; g.ld_aux_out = N / 2;
-  } else if (kind == 5) {
-    // sk_linear_swiglu_bwd: N = F, d_gu [M, 2F] from the saved gu [M, 2F]
-    g.ldb = N; g.b_mn = 1; g.ldc = 2 * N; g.epi = 2; g.aux = p; g.ld_aux = 2 * N;
-  } else if (kind == 6) {
-    // sk_linear_rope, the Qwen2 q|k|v projection: full-rotary 64-column heads (rope_rot 0 = 64); the plan does not
-    // depend on how many of them rotate
-    g.bias = p; g.epi = 3; g.rope_cos = p; g.rope_sin = p; g.rope_T = 1; g.rope_cols = N; g.rope_maxpos = 1;
-  } else {
-    g.bias = p; g.residual = p; g.ldr = N; g.round_before_res = 1; g.epi = 6; g.aux = p; g.ld_aux = N;
-    if (with_ws) { g.splitk_ws = p; g.splitk_ws_bytes = sk_gemm_ws_min_bytes(); }
+  switch (kind) {
+    case 0:   // sk_linear_rope_partial on the fused q|k|v projection: q and k heads rotate
+      g = sk_gemm_rope(M, N, K, p, p, p, p, p, p, nullptr, 1, N / 3 * 2, 1, 16);
+      break;
+    case 1: g = sk_gemm_gelu_fwd(M, N, K, p, p, p, p, p); break;
+    case 2: g = sk_gemm_gelu_bwd(M, K, N, p, p, p, p); break;       // the builder takes dy's width K and F = N
+    case 3: g = sk_gemm_res2(M, N, K, p, p, p, p, p, p, with_ws ? p : nullptr, with_ws ? sk_gemm_ws_min_bytes() : 0); break;
+    case 4: g = sk_gemm_swiglu_fwd(M, N / 2, K, p, p, p, p); break;   // N = 2F gate|up columns
+    case 5: g = sk_gemm_swiglu_bwd(M, K, N, p, p, p, p); break;       // likewise; d_gu [M, 2F] from the saved gu [M, 2F]
+    default:
+      // sk_linear_rope, the Qwen2 q|k|v projection: full-rotary 64-column heads; the plan does not depend on how many of
+      // them rotate
+      g = sk_gemm_rope(M, N, K, p, p, p, p, p, p, nullptr, 1, N, 1, 0);
   }
   return sk_gemm_plan_ex(g, plan);
 }
 int sk_gemm_bf16_splitk(int M, int N, int K, const void* A, int lda, int a_mn, const void* B, int ldb, int b_mn, void* C,
                         int ldc, int accumulate, void* splitk_ws, int64_t splitk_ws_bytes, void* stream) {
   SK_REQUIRE(A && B && C, "sk_gemm_bf16_splitk: null operand");
-  return sk_gemm_launch(M, N, K, A, lda, a_mn, B, ldb, b_mn, C, ldc, 0, nullptr, accumulate ? C : nullptr, ldc, 1, 0, 0,
-                        S(stream), splitk_ws, (size_t)splitk_ws_bytes);
+  return sk_gemm_ex_launch(sk_gemm_desc(M, N, K, A, lda, a_mn, B, ldb, b_mn, C, ldc, 0, nullptr, accumulate ? C : nullptr, ldc,
+                                        1, SK_ACT_NONE, 0, splitk_ws, (size_t)splitk_ws_bytes),
+                           S(stream));
 }
 int sk_gemm_bf16_ws(int M, int N, int K, const void* A, int lda, int a_mn, const void* B, int ldb, int b_mn, void* C,
                     int ldc, int out_f32, const void* bias, const void* residual, int ldr, int round_before_res, int act,
                     int force_bn, void* ws, int64_t ws_bytes, void* stream) {
   SK_REQUIRE(A && B && C, "sk_gemm_bf16_ws: null operand");
   SK_REQUIRE(ws == nullptr || (((uintptr_t)ws & 15) == 0 && ws_bytes % 16 == 0), "sk_gemm_bf16_ws: scratch must be 16-byte aligned");
-  return sk_gemm_launch(M, N, K, A, lda, a_mn, B, ldb, b_mn, C, ldc, out_f32, bias, residual, ldr, round_before_res, act,
-                        force_bn, S(stream), ws, (size_t)ws_bytes);
+  return sk_gemm_ex_launch(sk_gemm_desc(M, N, K, A, lda, a_mn, B, ldb, b_mn, C, ldc, out_f32, bias, residual, ldr,
+                                        round_before_res, act, force_bn, ws, (size_t)ws_bytes),
+                           S(stream));
 }
 int64_t sk_gemm_ws_bytes(void) { return (int64_t)sk_gemm_ws_min_bytes(); }
 int sk_gemm_plan(int M, int N, int K, const void* A, int lda, int a_mn, const void* B, int ldb, int b_mn, const void* C,
@@ -199,9 +194,8 @@ int sk_gemm_plan(int M, int N, int K, const void* A, int lda, int a_mn, const vo
 
 namespace {
 SkGemmEx split_desc_to_ex(const SkGemmSplitDesc& d) {
-  SkGemmEx g;
-  memset(&g, 0, sizeof(g));
-  g.M = d.M; g.N = d.N; g.K = d.K; g.batch = d.batch; g.a_mode = d.a_mode; g.passes = d.passes;
+  SkGemmEx g = sk_gemm_base(d.M, d.N, d.K);
+  g.batch = d.batch; g.a_mode = d.a_mode; g.passes = d.passes;
   g.A = d.A; g.A_lo = d.A_lo; g.lda = d.lda; g.a_mn = d.a_mn;
   g.a_inner = (long)d.a_inner; g.a_rows = (long)d.a_rows; g.a_row_stride = (long)d.a_row_stride;
   g.a_batch_stride = (long)d.a_batch_stride;

@@ -328,7 +328,7 @@ SK_DEVINL void epi_bias_act(float (&v)[8], const GemmParams& p, int col) {
 
 // residual (hi, and lo when present) read at output column `ocol` of row `row`
 SK_DEVINL void epi_residual(float (&v)[8], const GemmParams& p, size_t row, int ocol) {
-  if (p.epi == 6) {   // mlp + attn first, rounded (then + x below with round_before_res)
+  if (p.epi == SK_EPI_RES2) {   // mlp + attn first, rounded (then + x below with round_before_res)
     const uint4 av = *reinterpret_cast<const uint4*>(p.aux + row * p.ld_aux + ocol);
     const uint32_t aw[4] = {av.x, av.y, av.z, av.w};
 #pragma unroll
@@ -542,7 +542,7 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
             ++store_cnt;
           };
           auto pair_bf16 = [&](int j, int h) { return pack_bf16(acc[4 * j + 2 * h], acc[4 * j + 2 * h + 1]); };
-          if (p.epi == 1) {
+          if (p.epi == SK_EPI_SWIGLU_FWD) {
             // SwiGLU forward: tile columns [0,128) = gate, [128,256) = up of the same 128 hidden units; gate, up and
             // act = bf16(bf16(silu(gate)) * up) -- the unfused swiglu_fwd_kernel's rounding points
             if constexpr (BN == 256) {
@@ -665,7 +665,7 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
       const int rr = w.tile - bidx * tiles_per_batch;
       const int m0 = (rr / p.tiles_n) * BM;
       const int n0 = (rr % p.tiles_n) * BN;
-      if (!SK && p.tma_store && p.epi == 2) {
+      if (!SK && p.tma_store && p.epi == SK_EPI_SWIGLU_BWD) {
         // ===== SwiGLU backward epilogue: acc = d_act; d_gate = bf16(bf16(d_act*u) * silu'(g)), d_up = bf16(d_act * bf16(silu(g)))
         // The accumulator arrives one ROW per thread, but gu / d_gu must move with coalesced accesses (a thread walking
         // its own row issues 32 scattered 16-byte requests per instruction: measured slower than the unfused kernels).
@@ -828,7 +828,7 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
           for (int c2 = chalf * (NC64 / CS); c2 < (chalf + 1) * (NC64 / CS); ++c2) body(std::false_type{}, c2);
           if constexpr (TAIL) body(std::true_type{}, NC64);
         };
-        if (!SK && p.tma_store && p.epi == 1) {
+        if (!SK && p.tma_store && p.epi == SK_EPI_SWIGLU_FWD) {
           // ---- SwiGLU forward: tile columns [0,128) = gate, [128,256) = up of the same 128 hidden units ----
           if constexpr (BN == 256) {
 #pragma unroll 1
@@ -866,7 +866,7 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
               stage_store(&tmAux, gpk, (n0 >> 1) + i * 64, std::false_type{});
             }
           }
-        } else if (!SK && p.tma_store && p.epi == 3 && p.rope_rot < 64) {
+        } else if (!SK && p.tma_store && p.epi == SK_EPI_BIAS_ROPE && p.rope_rot < 64) {
           // ---- bias + partial RoPE (GPT-NeoX): in each head, element i < rope_rot/2 pairs with i + rope_rot/2; the
           // columns from rope_rot on get the bias only.  Same rounding points as the whole-head form below ----
           const int half = p.rope_rot >> 1;   // 8 or 16
@@ -938,7 +938,7 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
             }
             stage_store(&tmC, pk, col64, std::false_type{});
           }
-        } else if (!SK && p.tma_store && p.epi == 4) {
+        } else if (!SK && p.tma_store && p.epi == SK_EPI_GELU_FWD) {
           // ---- GELU forward (GPT-NeoX dense_h_to_4h): pre = bf16(acc + bias) -> C, bf16(gelu(pre)) -> aux_out ----
 #pragma unroll 1
           for (int c2 = chalf * (BN / 64 / CS); c2 < (chalf + 1) * (BN / 64 / CS); ++c2) {
@@ -965,7 +965,7 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
             }
             stage_store(&tmAux, pk, col64, std::false_type{});
           }
-        } else if (!SK && p.tma_store && p.epi == 5) {
+        } else if (!SK && p.tma_store && p.epi == SK_EPI_GELU_BWD) {
           // ---- GELU backward (input gradient of dense_4h_to_h): d_pre = bf16(bf16(d_act) * gelu'(pre)) ----
 #pragma unroll 1
           for (int c2 = chalf * (BN / 64 / CS); c2 < (chalf + 1) * (BN / 64 / CS); ++c2) {
@@ -991,7 +991,7 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
             }
             stage_store(&tmC, pk, col64, std::false_type{});
           }
-        } else if (!SK && p.tma_store && p.epi == 3) {
+        } else if (!SK && p.tma_store && p.epi == SK_EPI_BIAS_ROPE) {
           // ---- bias + RoPE: a 64-column chunk is one attention head; element i pairs with element i + 32 ----
           uint32_t cw[16], sw[16];
           {
@@ -1340,6 +1340,11 @@ int dispatch_major(bool a_mn, bool b_mn, const CUtensorMap* tm, const GemmParams
 inline int tile_cost(int bn) { return bn >= 256 ? 100 : (bn > 128 ? 61 + (bn - 128) * 39 / 128 : (bn == 128 ? 61 : 54)); }
 
 constexpr size_t SK_FLAG_BYTES = 4096;   // tail of the scratch buffer: stream-K publish flags ([CTA][32-row quadrant])
+// stream-K balancing pays when whole-tile waves would leave at least this share (%) of the SM-time idle and the K loop
+// is at least this many k-blocks long; with less idle time or shorter K the fix-up traffic eats the gain
+constexpr int STREAMK_MIN_IDLE_PCT = 20;
+constexpr int STREAMK_MIN_KB = 32;
+constexpr int STREAMK_RANGES = 4;   // row units: each leftover unit is cut into at most ~this many K ranges
 
 }  // namespace
 
@@ -1405,31 +1410,27 @@ int plan_gemm(const SkGemmEx& g, GemmParams& p, int& BN, int& ew, int& grid) {
   SK_REQUIRE(use3d || g.lda >= (g.a_mn ? g.M : g.K), "gemm: lda=%d is smaller than the %s of A", g.lda, g.a_mn ? "M" : "K");
   SK_REQUIRE(g.ldb >= (g.b_mn ? g.N : g.K), "gemm: ldb=%d is smaller than the %s of B", g.ldb, g.b_mn ? "N" : "K");
   if (g.col_gin == 0) {   // (compacted columns are narrower than N)
-    const int out_cols = g.epi == 2 ? 2 * g.N : g.N;
+    const int out_cols = g.epi == SK_EPI_SWIGLU_BWD ? 2 * g.N : g.N;
     SK_REQUIRE(g.ldc >= out_cols, "gemm: ldc=%d is smaller than the %d output columns", g.ldc, out_cols);
     SK_REQUIRE(g.residual == nullptr || g.ldr >= g.N, "gemm: ldr=%d is smaller than N=%d", g.ldr, g.N);
   }
   const int nsm = sk_num_sms();
   // stream-K needs the plain 2-D form and a scratch buffer of sk_gemm_ws_min_bytes() whose last 4 KB (flags) are zero
   static const int sk_env = [] { const char* e = getenv("SK_STREAMK"); return e ? atoi(e) : 1; }();
-  // balancing pays when whole-tile waves would leave a good part (default >= 20 %) of the SM-time idle; with less idle
-  // time the fix-up traffic eats the gain
-  static const int sk_min_idle = [] { const char* e = getenv("SK_STREAMK_MIN_IDLE"); return e ? atoi(e) : 20; }();
-  static const int sk_min_kb = [] { const char* e = getenv("SK_STREAMK_MIN_KB"); return e ? atoi(e) : 32; }();
   const bool sk_ok = sk_env != 0 && g.batch == 1 && !use3d && g.passes == 1 && g.a_mode == 0 && g.splitk_ws != nullptr &&
                      g.splitk_ws_bytes >= sk_gemm_ws_min_bytes();
   const size_t ws_data_bytes = g.splitk_ws_bytes > SK_FLAG_BYTES ? g.splitk_ws_bytes - SK_FLAG_BYTES : 0;
   // the SwiGLU epilogues need both halves of a [128 gate | 128 up] block in one tile.  The 192 / 224 widths are for
   // plain one-pass 2-D problems; the auto planner leaves them to GEMMs without stream-K scratch (forward and dgrad):
   // with scratch, split-K / stream-K balance the last wave at the widths they were tuned for
-  // (the GELU epilogues 4 / 5 also stay on whole 64-column chunks: epi 4's second output leaves through tmAux)
-  const bool fit = g.passes == 1 && g.batch == 1 && !use3d && g.a_mode == 0 && g.epi != 1 && g.epi != 2 && g.epi != 4 &&
-                   g.epi != 5;
-  SK_REQUIRE((g.force_bn != 192 && g.force_bn != 224) || (fit && !(g.force_bn == 224 && g.epi == 3)),
+  // (the GELU epilogues also stay on whole 64-column chunks: the forward's second output leaves through tmAux)
+  const bool fit = g.passes == 1 && g.batch == 1 && !use3d && g.a_mode == 0 && g.epi != SK_EPI_SWIGLU_FWD &&
+                   g.epi != SK_EPI_SWIGLU_BWD && g.epi != SK_EPI_GELU_FWD && g.epi != SK_EPI_GELU_BWD;
+  SK_REQUIRE((g.force_bn != 192 && g.force_bn != 224) || (fit && !(g.force_bn == 224 && g.epi == SK_EPI_BIAS_ROPE)),
              "gemm: force_bn=%d needs a one-pass 2-D problem (and whole 64-column heads for RoPE)", g.force_bn);
+  const bool swiglu = g.epi == SK_EPI_SWIGLU_FWD || g.epi == SK_EPI_SWIGLU_BWD;
   BN = (g.a_mode == 1) ? 64
-                       : sk_pick_bn(g.M * g.batch, g.N, (g.epi == 1 || g.epi == 2) ? 256 : g.force_bn, fit,
-                                    fit && !sk_ok, g.epi == 3);
+                       : sk_pick_bn(g.M * g.batch, g.N, swiglu ? 256 : g.force_bn, fit, fit && !sk_ok, g.epi == SK_EPI_BIAS_ROPE);
   memset(&p, 0, sizeof(p));
   p.M = g.M; p.N = g.N; p.K = g.K;
   p.batch = g.batch;
@@ -1452,9 +1453,7 @@ int plan_gemm(const SkGemmEx& g, GemmParams& p, int& BN, int& ew, int& grid) {
   p.splits = 1;
   p.splitk_ws = nullptr;
   const int num_kb = (g.K + BK - 1) / BK;
-  static const int splitk_env = [] { const char* e = getenv("SK_SPLITK"); return e ? atoi(e) : 1; }();
-  static const int sk_ranges = [] { const char* e = getenv("SK_STREAMK_RANGES"); return e ? atoi(e) : 4; }();
-  if (splitk_env && g.splitk_ws && g.batch == 1 && g.passes == 1 && !g.out_f32 && !g.bias && !g.act && !g.C_lo && g.col_gin == 0 &&
+  if (g.splitk_ws && g.batch == 1 && g.passes == 1 && !g.out_f32 && !g.bias && !g.act && !g.C_lo && g.col_gin == 0 &&
       g.epi == 0 &&
       (g.residual == nullptr || g.residual == g.C) && tiles * 2 <= nsm && num_kb >= 16) {
     int sp = (int)(nsm / tiles);
@@ -1481,7 +1480,7 @@ int plan_gemm(const SkGemmEx& g, GemmParams& p, int& BN, int& ew, int& grid) {
   p.rope_pos = g.rope_pos;
   p.rope_T = g.rope_T; p.rope_cols = g.rope_cols; p.rope_maxpos = g.rope_maxpos;
   p.rope_rot = g.rope_rot == 0 ? 64 : g.rope_rot;
-  if (g.epi == 6) {
+  if (g.epi == SK_EPI_RES2) {
     // two residuals: runs on every output path (epi_residual), stream-K included; split-K is not planned for it
     SK_REQUIRE(g.passes == 1 && g.batch == 1 && !use3d && g.residual && g.aux && !g.residual_lo && !g.act && !g.out_f32 &&
                    !g.C_lo && g.col_gin == 0 && g.round_before_res && g.ld_aux >= g.N && g.ld_aux % 8 == 0 &&
@@ -1491,23 +1490,23 @@ int plan_gemm(const SkGemmEx& g, GemmParams& p, int& BN, int& ew, int& grid) {
   } else if (g.epi != 0) {
     SK_REQUIRE(p.tma_store && g.passes == 1 && !g.residual && !g.act && g.splitk_ws == nullptr,
                "gemm: fused epilogue %d needs the plain bf16 TMA-store path (no residual / activation / scratch)", g.epi);
-    if (g.epi == 1) {
+    if (g.epi == SK_EPI_SWIGLU_FWD) {
       SK_REQUIRE(BN == 256 && g.N % 256 == 0 && g.aux_out && g.ld_aux_out % 8 == 0 && !g.bias,
                  "gemm: SwiGLU-forward epilogue needs N = 2F with F %% 128 == 0 and an act output");
-    } else if (g.epi == 2) {
+    } else if (g.epi == SK_EPI_SWIGLU_BWD) {
       SK_REQUIRE(BN == 256 && g.N % 128 == 0 && g.aux && g.ld_aux % 8 == 0 && !g.bias,
                  "gemm: SwiGLU-backward epilogue needs N = F with F %% 128 == 0 and the saved gu activation");
-    } else if (g.epi == 3) {
+    } else if (g.epi == SK_EPI_BIAS_ROPE) {
       SK_REQUIRE(g.rope_cos && g.rope_sin && g.rope_T > 0 && g.rope_maxpos > 0 && g.rope_cols % 64 == 0 && g.N % 64 == 0 &&
                      !g.bias_f32,
                  "gemm: RoPE epilogue needs cos/sin tables, 64-column heads and a bf16 bias");
       SK_REQUIRE(p.rope_rot == 16 || p.rope_rot == 32 || p.rope_rot == 64,
                  "gemm: RoPE epilogue rotary width rope_rot=%d is not supported (16, 32 or 64)", g.rope_rot);
-    } else if (g.epi == 4) {
+    } else if (g.epi == SK_EPI_GELU_FWD) {
       SK_REQUIRE(BN % 64 == 0 && g.N % 64 == 0 && g.aux_out && g.ld_aux_out >= g.N && g.ld_aux_out % 8 == 0 && !g.bias_f32 &&
                      (reinterpret_cast<uintptr_t>(g.aux_out) & 15) == 0,
                  "gemm: GELU-forward epilogue needs N %% 64 == 0, an act output (pitch >= N) and a bf16 bias");
-    } else if (g.epi == 5) {
+    } else if (g.epi == SK_EPI_GELU_BWD) {
       SK_REQUIRE(BN % 64 == 0 && g.N % 64 == 0 && g.aux && g.ld_aux >= g.N && g.ld_aux % 8 == 0 && !g.bias &&
                      (reinterpret_cast<uintptr_t>(g.aux) & 15) == 0,
                  "gemm: GELU-backward epilogue needs N %% 64 == 0, the saved pre-activation (pitch >= N) and no bias");
@@ -1522,7 +1521,7 @@ int plan_gemm(const SkGemmEx& g, GemmParams& p, int& BN, int& ew, int& grid) {
   // units and a unit is cut into at most two ranges, the second continuing from the first's accumulator (carry-in: the
   // weight gradient comes out bit-identical to whole tiles).  SK_STREAMK=2 also takes single-wave shapes.
   p.sk_G = 1;
-  if (sk_ok && BN == 256 && p.splits == 1 && num_kb >= sk_min_kb && (p.tiles_n <= 8 || p.tiles_m <= 8)) {
+  if (sk_ok && BN == 256 && p.splits == 1 && num_kb >= STREAMK_MIN_KB && (p.tiles_n <= 8 || p.tiles_m <= 8)) {
     const int colunits = p.tiles_n <= 8 ? 0 : 1;
     const int G = colunits ? p.tiles_m : p.tiles_n;
     const int units = colunits ? p.tiles_n : p.tiles_m;
@@ -1530,7 +1529,7 @@ int plan_gemm(const SkGemmEx& g, GemmParams& p, int& BN, int& ew, int& grid) {
     const int rem = units % n_groups;
     const long slots = ((long)(units + n_groups - 1) / n_groups) * n_groups;
     const bool multiwave = units > n_groups;
-    if (n_groups >= 1 && rem != 0 && (slots - units) * 100 >= slots * sk_min_idle &&   // enough SM-time would idle
+    if (n_groups >= 1 && rem != 0 && (slots - units) * 100 >= slots * STREAMK_MIN_IDLE_PCT &&   // enough SM-time would idle
         (!colunits || multiwave || sk_env >= 2)) {
       if (colunits && multiwave) {
         p.sk_units = rem + n_groups;
@@ -1538,7 +1537,7 @@ int plan_gemm(const SkGemmEx& g, GemmParams& p, int& BN, int& ew, int& grid) {
         p.sk_carry = 1;
       } else {
         p.sk_units = rem;
-        p.sk_groups = n_groups < rem * sk_ranges ? n_groups : rem * sk_ranges;          // a unit is cut into at most ~4 ranges
+        p.sk_groups = n_groups < rem * STREAMK_RANGES ? n_groups : rem * STREAMK_RANGES;
       }
       p.sk_G = G;
       p.sk_colunits = colunits;
@@ -1553,10 +1552,13 @@ int plan_gemm(const SkGemmEx& g, GemmParams& p, int& BN, int& ew, int& grid) {
   // 8 epilogue warps (two per 32-row quadrant) where the epilogue does real work per element; the plain
   // convert-and-store epilogue is faster with 4 (fewer warps contending with the TMA / MMA issue threads)
   static const int ew_env = [] { const char* e = getenv("SK_GEMM_EW"); return e ? atoi(e) : 0; }();
-  ew = (p.sk_units == 0 && BN == 256 && p.tma_store && (ew_env == 8 || (ew_env == 0 && (g.epi == 2 || g.epi == 3 || g.epi == 4 || g.epi == 5)))) ? 8 : 4;
+  const bool heavy_epi = g.epi == SK_EPI_SWIGLU_BWD || g.epi == SK_EPI_BIAS_ROPE || g.epi == SK_EPI_GELU_FWD ||
+                         g.epi == SK_EPI_GELU_BWD;
+  ew = (p.sk_units == 0 && BN == 256 && p.tma_store && (ew_env == 8 || (ew_env == 0 && heavy_epi))) ? 8 : 4;
   // the register epilogue takes the one-pass TMA-store tiles whose epilogue reads no operand (plain convert and SwiGLU
   // forward) on the 4-epilogue-warp kernels; the others keep the parked accumulator
-  p.reg_epi = (p.tma_store && p.sk_units == 0 && ew == 4 && !g.bias && !g.act && !g.residual && (g.epi == 0 || g.epi == 1)) ? 1 : 0;
+  p.reg_epi = (p.tma_store && p.sk_units == 0 && ew == 4 && !g.bias && !g.act && !g.residual &&
+               (g.epi == 0 || g.epi == SK_EPI_SWIGLU_FWD)) ? 1 : 0;
   return 0;
 }
 
@@ -1611,15 +1613,16 @@ int sk_gemm_ex_launch(const SkGemmEx& g, cudaStream_t stream) {
   // warp's quadrant) otherwise
   const uint32_t box_rows = p.reg_epi ? 16 : 32;
   if (p.tma_store) {
-    // epi 2 writes d_gu [M, 2N] (the accumulator tile is d_act [M, N])
-    const int rc2 = sk_make_tmap_2d(&tm[4], g.C, 2, (uint64_t)(g.epi == 2 ? 2 * g.N : g.N), (uint64_t)g.M, (uint64_t)g.ldc, 64, box_rows);
+    // the SwiGLU backward writes d_gu [M, 2N] (the accumulator tile is d_act [M, N])
+    const int rc2 = sk_make_tmap_2d(&tm[4], g.C, 2, (uint64_t)(g.epi == SK_EPI_SWIGLU_BWD ? 2 * g.N : g.N), (uint64_t)g.M,
+                                    (uint64_t)g.ldc, 64, box_rows);
     if (rc2) return rc2;
   }
   tm[5] = tm[4];
-  if (g.epi == 1) {
+  if (g.epi == SK_EPI_SWIGLU_FWD) {
     const int rc3 = sk_make_tmap_2d(&tm[5], g.aux_out, 2, (uint64_t)g.N / 2, (uint64_t)g.M, (uint64_t)g.ld_aux_out, 64, box_rows);
     if (rc3) return rc3;
-  } else if (g.epi == 4) {   // the GELU output, same shape as C
+  } else if (g.epi == SK_EPI_GELU_FWD) {   // the GELU output, same shape as C
     const int rc3 = sk_make_tmap_2d(&tm[5], g.aux_out, 2, (uint64_t)g.N, (uint64_t)g.M, (uint64_t)g.ld_aux_out, 64, 32);
     if (rc3) return rc3;
   } else if (p.tma_store && BN % 64 != 0) {   // the 32-column tail chunk of a 224-wide tile
@@ -1654,104 +1657,4 @@ int sk_gemm_ex_launch(const SkGemmEx& g, cudaStream_t stream) {
     SK_LAUNCH_CHECK();
   }
   return 0;
-}
-
-// Plain entry point.  A: [M,K] (a_mn=0, lda = row pitch of the [M,K] array) or stored [K,M] (a_mn=1, lda = row pitch of
-// the [K,M] array).  B: [N,K] (b_mn=0) or stored [K,N] (b_mn=1).
-SkGemmEx sk_gemm_desc(int M, int N, int K, const void* A, int lda, int a_mn, const void* B, int ldb, int b_mn, void* C,
-                      int ldc, int out_f32, const void* bias, const void* residual, int ldr, int round_before_res, int act,
-                      int force_bn, void* splitk_ws, size_t splitk_ws_bytes) {
-  SkGemmEx g;
-  memset(&g, 0, sizeof(g));
-  g.M = M; g.N = N; g.K = K; g.batch = 1; g.passes = 1;
-  g.A = A; g.lda = lda; g.a_mn = a_mn;
-  g.B = B; g.ldb = ldb; g.b_mn = b_mn;
-  g.C = C; g.ldc = ldc; g.out_f32 = out_f32;
-  g.bias = bias; g.residual = residual; g.ldr = ldr; g.round_before_res = round_before_res; g.act = act;
-  g.force_bn = force_bn;
-  g.pdl = 1;
-  g.splitk_ws = splitk_ws;
-  g.splitk_ws_bytes = splitk_ws_bytes;
-  return g;
-}
-int sk_gemm_launch(int M, int N, int K, const void* A, int lda, int a_mn, const void* B, int ldb, int b_mn, void* C,
-                   int ldc, int out_f32, const void* bias, const void* residual, int ldr, int round_before_res, int act,
-                   int force_bn, cudaStream_t stream, void* splitk_ws, size_t splitk_ws_bytes) {
-  return sk_gemm_ex_launch(sk_gemm_desc(M, N, K, A, lda, a_mn, B, ldb, b_mn, C, ldc, out_f32, bias, residual, ldr,
-                                        round_before_res, act, force_bn, splitk_ws, splitk_ws_bytes),
-                           stream);
-}
-
-// ---- fused linears of the LM step (SkGemmEx::epi) ------------------------------------------------------------------
-// gu[M,2F] = x[M,K] * Wgu[2F,K]^T with Wgu (and gu) in [128 gate | 128 up] blocks, and act[M,F] = bf16(bf16(silu(gate)) * up)
-// written by the same epilogue (HF Qwen2MLP, HF:models/qwen2/modeling_qwen2.py:35-48)
-int sk_linear_swiglu_fwd_launch(int M, int F, int K, const void* x, const void* Wgu, void* gu, void* act, cudaStream_t s) {
-  SkGemmEx g;
-  memset(&g, 0, sizeof(g));
-  g.M = M; g.N = 2 * F; g.K = K; g.batch = 1; g.passes = 1;
-  g.A = x; g.lda = K; g.B = Wgu; g.ldb = K;
-  g.C = gu; g.ldc = 2 * F;
-  g.epi = 1; g.aux_out = act; g.ld_aux_out = F;
-  g.pdl = 1;
-  return sk_gemm_ex_launch(g, s);
-}
-// d_gu[M,2F] from d_act = dy[M,N] * Wd[N,F] without materialising d_act: the epilogue turns each accumulator tile into
-// d_gate / d_up with the saved gu (autograd of the SwiGLU above, same bf16 rounding points as the unfused kernels)
-int sk_linear_swiglu_bwd_launch(int M, int N, int F, const void* dy, const void* Wd, const void* gu, void* dgu, cudaStream_t s) {
-  SkGemmEx g;
-  memset(&g, 0, sizeof(g));
-  g.M = M; g.N = F; g.K = N; g.batch = 1; g.passes = 1;
-  g.A = dy; g.lda = N; g.B = Wd; g.ldb = F; g.b_mn = 1;
-  g.C = dgu; g.ldc = 2 * F;
-  g.epi = 2; g.aux = gu; g.ld_aux = 2 * F;
-  g.pdl = 1;
-  return sk_gemm_ex_launch(g, s);
-}
-// out[M,N] = x[M,K] * W[N,K]^T + bias, 64-column heads below rope_cols rotated in the epilogue (HF apply_rotary_pos_emb,
-// HF:models/qwen2/modeling_qwen2.py:102-146)
-int sk_linear_rope_launch(int M, int N, int K, const void* x, const void* W, const void* bias, void* out, const void* cos_t,
-                          const void* sin_t, const int32_t* pos_ids, int T, int rope_cols, int max_positions, cudaStream_t s,
-                          int rope_rot) {
-  SkGemmEx g;
-  memset(&g, 0, sizeof(g));
-  g.M = M; g.N = N; g.K = K; g.batch = 1; g.passes = 1;
-  g.A = x; g.lda = K; g.B = W; g.ldb = K;
-  g.C = out; g.ldc = N;
-  g.bias = bias;
-  g.epi = 3; g.rope_cos = cos_t; g.rope_sin = sin_t; g.rope_pos = pos_ids; g.rope_T = T;
-  g.rope_cols = rope_cols; g.rope_maxpos = max_positions; g.rope_rot = rope_rot;
-  g.pdl = 1;
-  return sk_gemm_ex_launch(g, s);
-}
-// GPT-NeoX MLP (HF GPTNeoXMLP): pre[M,F] = bf16(x W1^T + b1) and act = bf16(gelu(pre)) from one epilogue
-int sk_linear_gelu_fwd_launch(int M, int F, int K, const void* x, const void* W1, const void* b1, void* pre, void* act,
-                              cudaStream_t s) {
-  SkGemmEx g;
-  memset(&g, 0, sizeof(g));
-  g.M = M; g.N = F; g.K = K; g.batch = 1; g.passes = 1;
-  g.A = x; g.lda = K; g.B = W1; g.ldb = K;
-  g.C = pre; g.ldc = F;
-  g.bias = b1;
-  g.epi = 4; g.aux_out = act; g.ld_aux_out = F;
-  g.pdl = 1;
-  return sk_gemm_ex_launch(g, s);
-}
-// d_pre[M,F] = bf16(bf16(dy W2) * gelu'(pre)): d_act never reaches memory
-int sk_linear_gelu_bwd_launch(int M, int N, int F, const void* dy, const void* W2, const void* pre, void* dpre, cudaStream_t s) {
-  SkGemmEx g;
-  memset(&g, 0, sizeof(g));
-  g.M = M; g.N = F; g.K = N; g.batch = 1; g.passes = 1;
-  g.A = dy; g.lda = N; g.B = W2; g.ldb = F; g.b_mn = 1;
-  g.C = dpre; g.ldc = F;
-  g.epi = 5; g.aux = pre; g.ld_aux = F;
-  g.pdl = 1;
-  return sk_gemm_ex_launch(g, s);
-}
-// out[M,N] = bf16(bf16(bf16(x W^T + bias) + res2) + res): GPT-NeoX's `mlp_output + attn_output + hidden_states`, rounded
-// at each add in that order.  out may alias res (each element reads its residuals before it is stored).
-int sk_linear_res2_launch(int M, int N, int K, const void* x, const void* W, const void* bias, const void* res2, const void* res,
-                          void* out, cudaStream_t s, void* splitk_ws, size_t splitk_ws_bytes) {
-  SkGemmEx g = sk_gemm_desc(M, N, K, x, K, 0, W, K, 0, out, N, 0, bias, res, N, 1, 0, 0, splitk_ws, splitk_ws_bytes);
-  g.epi = 6; g.aux = res2; g.ld_aux = N;
-  return sk_gemm_ex_launch(g, s);
 }

@@ -118,8 +118,10 @@ HiLo hl(const SkHubert* h, int64_t off, int64_t elems) {
 // y(hi,lo)[M,N] = act(x(hi,lo)[M,K] * W(hi,lo)[N,K]^T + bias) (+ residual(hi,lo)), split-bf16 3-pass
 int linear_split(const SkHubert* h, int M, int N, int K, HiLo x, int64_t w_off, int64_t b_off, int act, const HiLo* res,
                  HiLo y, float* y_f32, int ldy, cudaStream_t s) {
-  return sk_linear_split_launch(M, N, K, x.hi, x.lo, h->w_hi + w_off, h->w_lo + w_off, b_off >= 0 ? h->w32 + b_off : nullptr,
-                                act, res ? res->hi : nullptr, res ? res->lo : nullptr, y.hi, y.lo, y_f32, ldy, s);
+  return sk_gemm_ex_launch(sk_gemm_linear_split(M, N, K, x.hi, x.lo, h->w_hi + w_off, h->w_lo + w_off,
+                                                b_off >= 0 ? h->w32 + b_off : nullptr, act, res ? res->hi : nullptr,
+                                                res ? res->lo : nullptr, y.hi, y.lo, y_f32, ldy),
+                           s);
 }
 
 // dbg_stage (tests only): 100+i = output of conv layer i, 200 = projection, 201 = positional conv (post-GELU),
@@ -151,9 +153,8 @@ int forward_impl(SkHubert* h, const float* wav, const int64_t* lens, int B, int 
   int cur = 0;
   for (int i = 1; i < h->nconv; ++i) {
     const int k = h->cfg.conv_kernel[i], st = h->cfg.conv_stride[i];
-    SkGemmEx g;
-    memset(&g, 0, sizeof(g));
-    g.M = T[i]; g.N = C; g.K = k * C; g.batch = B; g.passes = 3;
+    SkGemmEx g = sk_gemm_base(T[i], C, k * C);
+    g.batch = B; g.passes = 3;
     g.A = act[cur].hi; g.A_lo = act[cur].lo;
     g.a_inner = (long)k * C; g.a_rows = T[i]; g.a_row_stride = (long)st * C; g.a_batch_stride = (long)T[i - 1] * C;
     g.B = h->w_hi + h->conv_w[i]; g.B_lo = h->w_lo + h->conv_w[i]; g.ldb = k * C;
@@ -161,7 +162,7 @@ int forward_impl(SkHubert* h, const float* wav, const int64_t* lens, int B, int 
     HiLo out = act[cur ^ 1];
     if (i >= 2) out = hl(h, (cur ^ 1) == 0 ? w.act0 : w.act1, (int64_t)B * T[i] * C);
     g.C = out.hi; g.C_lo = out.lo; g.ldc = C;
-    g.act = 1;
+    g.act = SK_ACT_GELU;
     SK_TRY(sk_gemm_ex_launch(g, s));
     act[cur ^ 1] = out;
     cur ^= 1;
@@ -171,22 +172,21 @@ int forward_impl(SkHubert* h, const float* wav, const int64_t* lens, int B, int 
   HiLo lnc = hl(h, w.lnc, (int64_t)M * C), x = hl(h, w.x, (int64_t)M * H);
   SK_TRY(sk_layernorm_hilo_launch(act[cur].hi, act[cur].lo, nullptr, nullptr, h->w32 + h->fp_lng, h->w32 + h->fp_lnb,
                                   lnc.hi, lnc.lo, nullptr, M, C, eps, s));
-  SK_TRY(linear_split(h, M, H, C, lnc, h->fp_w, h->fp_b, 0, nullptr, x, nullptr, H, s));
+  SK_TRY(linear_split(h, M, H, C, lnc, h->fp_w, h->fp_b, SK_ACT_NONE, nullptr, x, nullptr, H, s));
   if (dbg_stage == 200) return sk_hilo_to_f32_launch(x.hi, x.lo, feat_out, (long)M * H, s);
   // positional conv (grouped, weight-norm folded on the host) + GELU, then x + pos -> LayerNorm
   const int Tp = Tf + 2 * h->halo, GP = h->G * GROUP_PAD;
   HiLo xp = hl(h, w.xp, (int64_t)B * Tp * GP), pc = hl(h, w.pc, (int64_t)M * H);
   SK_TRY(sk_regroup_pad_launch(x.hi, x.lo, xp.hi, xp.lo, B, Tf, h->halo, h->G, h->cg, GROUP_PAD, s));
   {
-    SkGemmEx g;
-    memset(&g, 0, sizeof(g));
-    g.M = Tf; g.N = GP; g.K = h->Kpos * GROUP_PAD; g.batch = B; g.passes = 3; g.a_mode = 1;
+    SkGemmEx g = sk_gemm_base(Tf, GP, h->Kpos * GROUP_PAD);
+    g.batch = B; g.passes = 3; g.a_mode = 1;
     g.A = xp.hi; g.A_lo = xp.lo;
     g.a_inner = GP; g.a_rows = Tp; g.a_row_stride = GP; g.a_batch_stride = (long)Tp * GP;
     g.B = h->w_hi + h->pos_w; g.B_lo = h->w_lo + h->pos_w; g.ldb = h->Kpos * GROUP_PAD;
     g.C = pc.hi; g.C_lo = pc.lo; g.ldc = H;
     g.bias = h->w32 + h->pos_b; g.bias_f32 = 1;
-    g.act = 1;
+    g.act = SK_ACT_GELU;
     g.col_gin = GROUP_PAD; g.col_gout = h->cg;
     SK_TRY(sk_gemm_ex_launch(g, s));
   }
@@ -212,18 +212,18 @@ int forward_impl(SkHubert* h, const float* wav, const int64_t* lens, int B, int 
   for (int l = 0; l < h->cfg.n_layers; ++l) {
     const LayerOff& o = h->lo[l];
     const bool last = (l == h->cfg.n_layers - 1) || (dbg_stage == l + 1);
-    SK_TRY(linear_split(h, M, 3 * H, H, hb[0], o.wqkv, o.bqkv, 0, nullptr, qkv, nullptr, 3 * H, s));
+    SK_TRY(linear_split(h, M, 3 * H, H, hb[0], o.wqkv, o.bqkv, SK_ACT_NONE, nullptr, qkv, nullptr, 3 * H, s));
     SK_TAP(l, 0, qkv, 3 * H);
     SK_TRY(sk_attn_tc_fwd_split_launch(qkv.hi, qkv.lo, ao.hi, ao.lo, B, Tf, h->cfg.n_heads, 3 * H, H, scale, s));
     SK_TAP(l, 1, ao, H);
-    SK_TRY(linear_split(h, M, H, H, ao, o.wo, o.bo, 0, &hb[0], t1, nullptr, H, s));
+    SK_TRY(linear_split(h, M, H, H, ao, o.wo, o.bo, SK_ACT_NONE, &hb[0], t1, nullptr, H, s));
     SK_TAP(l, 2, t1, H);
     SK_TRY(sk_layernorm_hilo_launch(t1.hi, t1.lo, nullptr, nullptr, h->w32 + o.ln1g, h->w32 + o.ln1b, hb[1].hi, hb[1].lo,
                                     nullptr, M, H, eps, s));
     SK_TAP(l, 3, hb[1], H);
-    SK_TRY(linear_split(h, M, F, H, hb[1], o.w1, o.b1, 1, nullptr, ff, nullptr, F, s));
+    SK_TRY(linear_split(h, M, F, H, hb[1], o.w1, o.b1, SK_ACT_GELU, nullptr, ff, nullptr, F, s));
     SK_TAP(l, 4, ff, F);
-    SK_TRY(linear_split(h, M, H, F, ff, o.w2, o.b2, 0, &hb[1], t1, nullptr, H, s));
+    SK_TRY(linear_split(h, M, H, F, ff, o.w2, o.b2, SK_ACT_NONE, &hb[1], t1, nullptr, H, s));
     SK_TAP(l, 5, t1, H);
     SK_TRY(sk_layernorm_hilo_launch(t1.hi, t1.lo, nullptr, nullptr, h->w32 + o.ln2g, h->w32 + o.ln2b, hb[0].hi, hb[0].lo,
                                     last ? feat_out : nullptr, M, H, eps, s));
@@ -232,7 +232,7 @@ int forward_impl(SkHubert* h, const float* wav, const int64_t* lens, int B, int 
 #undef SK_TAP
   if (ids) {
     float* dot = reinterpret_cast<float*>(h->ws + w.dot);
-    SK_TRY(linear_split(h, M, h->Upad, H, hb[0], h->km_c, -1, 0, nullptr, HiLo{nullptr, nullptr}, dot, h->Upad, s));
+    SK_TRY(linear_split(h, M, h->Upad, H, hb[0], h->km_c, -1, SK_ACT_NONE, nullptr, HiLo{nullptr, nullptr}, dot, h->Upad, s));
     SK_TRY(sk_kmeans_argmin_launch(dot, h->csq, ids, M, h->U, h->Upad, s));
   }
   if (n_frames) SK_TRY(sk_rel_len_launch(lens, n_frames, B, S, Tf, s));

@@ -2,7 +2,6 @@
 // (The public, C-ABI surface is include/slamkit_b200.h.)
 #pragma once
 #include "common.cuh"
-#include <string.h>
 
 // gemm_tcgen05.cu
 int sk_make_tmap_2d(CUtensorMap* out, const void* ptr, int elem_bytes, uint64_t inner, uint64_t outer, uint64_t ld,
@@ -11,8 +10,23 @@ int sk_make_tmap_3d(CUtensorMap* out, const void* ptr, uint64_t inner, uint64_t 
                     uint64_t batch_stride, uint32_t box_rows);
 int sk_pick_bn(int M, int N, int force_bn, bool fit_forced, bool fit, bool whole_heads);
 size_t sk_gemm_ws_min_bytes(void);   // scratch size that enables stream-K (last 4 KB = flag words, zero on first use)
+// SkGemmEx::act
+constexpr int SK_ACT_NONE = 0, SK_ACT_GELU = 1, SK_ACT_RELU = 2;
+// SkGemmEx::epi, the fused epilogues of the LM step (0 = none):
+//   SwiGLU forward : B = gate/up weight in [128 gate rows | 128 up rows] blocks, N = 2F; C = gu [M,2F] (same block
+//                    layout) and aux_out = act [M,F] = bf16(bf16(silu(gate)) * up)
+//   SwiGLU backward: N = F, acc = d_act; aux = gu [M,2F]; C = d_gu [M,2F] (ldc = its pitch)
+//   bias + RoPE    : 64-column heads with column < rope_cols are rotated with cos/sin[pos] (pos = rope_pos[row] or
+//                    row % rope_T, clamped to [0, rope_maxpos)); the first rope_rot columns of each head rotate
+//                    (0 or 64: the whole head, tables [maxpos, 32]; 16 / 32: partial rotary, tables [maxpos, rope_rot/2])
+//   GELU forward   : C = pre = bf16(acc + bias) and aux_out = bf16(gelu_erf(pre)) (same shape, ld_aux_out)
+//   GELU backward  : acc = d_act; aux = the saved pre; C = bf16(bf16(acc) * gelu'(pre))
+//   two residuals  : C = bf16(bf16(bf16(acc + bias) + aux) + residual) (GPT-NeoX parallel residual: mlp + attn + x)
+constexpr int SK_EPI_SWIGLU_FWD = 1, SK_EPI_SWIGLU_BWD = 2, SK_EPI_BIAS_ROPE = 3, SK_EPI_GELU_FWD = 4,
+              SK_EPI_GELU_BWD = 5, SK_EPI_RES2 = 6;
 // Extended GEMM description (HuBERT path): batched / strided-window A operands (convolutions as GEMMs without an
 // im2col copy), split-bf16 3-pass accumulation, fp32 bias, hi/lo residual and outputs, grouped column compaction.
+// The sk_gemm_* builders below fill it for each kind of GEMM the library launches.
 struct SkGemmEx {
   int M, N, K;              // M: rows per batch item
   int batch;                // >= 1
@@ -34,17 +48,7 @@ struct SkGemmEx {
   void* splitk_ws;          // optional scratch: deterministic split-K (few tiles, long K) and stream-K load balancing
   size_t splitk_ws_bytes;
   int pdl;                  // 1: launch with programmatic stream serialization (the LM step's short back-to-back GEMMs)
-  // Fused epilogues of the LM step (0 = none):
-  //   1 SwiGLU forward : B = gate/up weight in [128 gate rows | 128 up rows] blocks, N = 2F; C = gu [M,2F] (same block
-  //                      layout) and aux_out = act [M,F] = bf16(bf16(silu(gate)) * up)
-  //   2 SwiGLU backward: N = F, acc = d_act; aux = gu [M,2F]; C = d_gu [M,2F] (ldc = its pitch)
-  //   3 bias + RoPE    : 64-column heads with column < rope_cols are rotated with cos/sin[pos] (pos = rope_pos[row] or
-  //                      row % rope_T, clamped to [0, rope_maxpos)); the first rope_rot columns of each head rotate
-  //                      (0 or 64: the whole head, tables [maxpos, 32]; 16 / 32: partial rotary, tables [maxpos, rope_rot/2])
-  //   4 GELU forward   : C = pre = bf16(acc + bias) and aux_out = bf16(gelu_erf(pre)) (same shape, ld_aux_out)
-  //   5 GELU backward  : acc = d_act; aux = the saved pre; C = bf16(bf16(acc) * gelu'(pre))
-  //   6 two residuals  : C = bf16(bf16(bf16(acc + bias) + aux) + residual) (GPT-NeoX parallel residual: mlp + attn + x)
-  int epi;
+  int epi;                  // fused epilogue of the LM step: SK_EPI_* (0 = none)
   const void* aux;
   int ld_aux;
   void* aux_out;
@@ -55,15 +59,125 @@ struct SkGemmEx {
   int rope_rot;
 };
 int sk_gemm_ex_launch(const SkGemmEx& g, cudaStream_t stream);
+struct SkGemmPlan;
+int sk_gemm_plan_ex(const SkGemmEx& g, SkGemmPlan* out);   // the decisions sk_gemm_ex_launch makes for g, nothing launched
+
+// ---- descriptor builders: host-only, no CUDA call.  A residual's pitch (ldr) and round_before_res are set only
+// together with the residual.
+// A zeroed one-pass M x N x K descriptor, the start of every builder
+inline SkGemmEx sk_gemm_base(int M, int N, int K) {
+  SkGemmEx g{};
+  g.M = M; g.N = N; g.K = K; g.batch = 1; g.passes = 1;
+  return g;
+}
+// The plain GEMM of the C ABI (sk_gemm_bf16*, sk_gemm_plan).  A: [M,K] (a_mn=0, lda = row pitch of the [M,K] array) or
+// stored [K,M] (a_mn=1, lda = row pitch of the [K,M] array).  B: [N,K] (b_mn=0) or stored [K,N] (b_mn=1).
+inline SkGemmEx sk_gemm_desc(int M, int N, int K, const void* A, int lda, int a_mn, const void* B, int ldb, int b_mn, void* C,
+                             int ldc, int out_f32, const void* bias, const void* residual, int ldr, int round_before_res,
+                             int act, int force_bn, void* splitk_ws, size_t splitk_ws_bytes) {
+  SkGemmEx g = sk_gemm_base(M, N, K);
+  g.A = A; g.lda = lda; g.a_mn = a_mn;
+  g.B = B; g.ldb = ldb; g.b_mn = b_mn;
+  g.C = C; g.ldc = ldc; g.out_f32 = out_f32;
+  g.bias = bias; g.residual = residual; g.ldr = ldr; g.round_before_res = round_before_res; g.act = act;
+  g.force_bn = force_bn;
+  g.pdl = 1;
+  g.splitk_ws = splitk_ws;
+  g.splitk_ws_bytes = splitk_ws_bytes;
+  return g;
+}
+// The linears of the LM step (launched with programmatic stream serialization).
+// y[M,N] (pitch ldy) = act(x[M,K] W[N,K]^T + bias) (+ res, same pitch as y, added to the bf16-rounded product)
+inline SkGemmEx sk_gemm_linear(int M, int N, int K, const void* x, const void* W, void* y, int ldy, const void* bias,
+                               const void* res, int act, void* splitk_ws = nullptr, size_t splitk_ws_bytes = 0) {
+  SkGemmEx g = sk_gemm_base(M, N, K);
+  g.A = x; g.lda = K;
+  g.B = W; g.ldb = K;
+  g.C = y; g.ldc = ldy;
+  g.bias = bias;
+  if (res) { g.residual = res; g.ldr = ldy; g.round_before_res = 1; }
+  g.act = act;
+  g.pdl = 1;
+  g.splitk_ws = splitk_ws;
+  g.splitk_ws_bytes = splitk_ws_bytes;
+  return g;
+}
+// dx[M,K] = dy[M,N] W[N,K] (+ res [M,K], added to the bf16-rounded product)
+inline SkGemmEx sk_gemm_dgrad(int M, int N, int K, const void* dy, const void* W, void* dx, const void* res = nullptr) {
+  SkGemmEx g = sk_gemm_base(M, K, N);
+  g.A = dy; g.lda = N;
+  g.B = W; g.ldb = K; g.b_mn = 1;
+  g.C = dx; g.ldc = K;
+  if (res) { g.residual = res; g.ldr = K; g.round_before_res = 1; }
+  g.pdl = 1;
+  return g;
+}
+// dW[N,K] (+)= dy[M,N]^T x[M,K]; accumulating adds the bf16-rounded product to dW.  Scratch: split-K for the small
+// weight gradients, stream-K balancing for the large ones
+inline SkGemmEx sk_gemm_wgrad(int M, int N, int K, const void* dy, const void* x, void* dW, bool accumulate, void* splitk_ws,
+                              size_t splitk_ws_bytes) {
+  SkGemmEx g = sk_gemm_base(N, K, M);
+  g.A = dy; g.lda = N; g.a_mn = 1;
+  g.B = x; g.ldb = K; g.b_mn = 1;
+  g.C = dW; g.ldc = K;
+  if (accumulate) { g.residual = dW; g.ldr = K; g.round_before_res = 1; }
+  g.pdl = 1;
+  g.splitk_ws = splitk_ws;
+  g.splitk_ws_bytes = splitk_ws_bytes;
+  return g;
+}
+// gu[M,2F] = x[M,K] * Wgu[2F,K]^T with Wgu (and gu) in [128 gate | 128 up] blocks, and act[M,F] = bf16(bf16(silu(gate)) * up)
+// written by the same epilogue (HF Qwen2MLP, HF:models/qwen2/modeling_qwen2.py:35-48)
+inline SkGemmEx sk_gemm_swiglu_fwd(int M, int F, int K, const void* x, const void* Wgu, void* gu, void* act) {
+  SkGemmEx g = sk_gemm_linear(M, 2 * F, K, x, Wgu, gu, 2 * F, nullptr, nullptr, SK_ACT_NONE);
+  g.epi = SK_EPI_SWIGLU_FWD; g.aux_out = act; g.ld_aux_out = F;
+  return g;
+}
+// d_gu[M,2F] from d_act = dy[M,N] * Wd[N,F] without materialising d_act: the epilogue turns each accumulator tile into
+// d_gate / d_up with the saved gu (autograd of the SwiGLU above, same bf16 rounding points as the unfused kernels)
+inline SkGemmEx sk_gemm_swiglu_bwd(int M, int N, int F, const void* dy, const void* Wd, const void* gu, void* dgu) {
+  SkGemmEx g = sk_gemm_dgrad(M, N, F, dy, Wd, dgu);
+  g.ldc = 2 * F;
+  g.epi = SK_EPI_SWIGLU_BWD; g.aux = gu; g.ld_aux = 2 * F;
+  return g;
+}
+// out[M,N] = x[M,K] * W[N,K]^T + bias, 64-column heads below rope_cols rotated in the epilogue (HF apply_rotary_pos_emb,
+// HF:models/qwen2/modeling_qwen2.py:102-146); rope_rot: rotated columns per head (0 = all 64)
+inline SkGemmEx sk_gemm_rope(int M, int N, int K, const void* x, const void* W, const void* bias, void* out, const void* cos_t,
+                             const void* sin_t, const int32_t* pos_ids, int T, int rope_cols, int max_positions, int rope_rot) {
+  SkGemmEx g = sk_gemm_linear(M, N, K, x, W, out, N, bias, nullptr, SK_ACT_NONE);
+  g.epi = SK_EPI_BIAS_ROPE; g.rope_cos = cos_t; g.rope_sin = sin_t; g.rope_pos = pos_ids; g.rope_T = T;
+  g.rope_cols = rope_cols; g.rope_maxpos = max_positions; g.rope_rot = rope_rot;
+  return g;
+}
+// GPT-NeoX MLP (HF GPTNeoXMLP): pre[M,F] = bf16(x W1^T + b1) and act = bf16(gelu(pre)) from one epilogue
+inline SkGemmEx sk_gemm_gelu_fwd(int M, int F, int K, const void* x, const void* W1, const void* b1, void* pre, void* act) {
+  SkGemmEx g = sk_gemm_linear(M, F, K, x, W1, pre, F, b1, nullptr, SK_ACT_NONE);
+  g.epi = SK_EPI_GELU_FWD; g.aux_out = act; g.ld_aux_out = F;
+  return g;
+}
+// d_pre[M,F] = bf16(bf16(dy W2) * gelu'(pre)): d_act never reaches memory
+inline SkGemmEx sk_gemm_gelu_bwd(int M, int N, int F, const void* dy, const void* W2, const void* pre, void* dpre) {
+  SkGemmEx g = sk_gemm_dgrad(M, N, F, dy, W2, dpre);
+  g.epi = SK_EPI_GELU_BWD; g.aux = pre; g.ld_aux = F;
+  return g;
+}
+// out[M,N] = bf16(bf16(bf16(x W^T + bias) + res2) + res): GPT-NeoX's `mlp_output + attn_output + hidden_states`, rounded
+// at each add in that order.  out may alias res (each element reads its residuals before it is stored).
+inline SkGemmEx sk_gemm_res2(int M, int N, int K, const void* x, const void* W, const void* bias, const void* res2,
+                             const void* res, void* out, void* splitk_ws = nullptr, size_t splitk_ws_bytes = 0) {
+  SkGemmEx g = sk_gemm_linear(M, N, K, x, W, out, N, bias, res, SK_ACT_NONE, splitk_ws, splitk_ws_bytes);
+  g.epi = SK_EPI_RES2; g.aux = res2; g.ld_aux = N;
+  return g;
+}
 // The fp32-grade linear of the HuBERT encoder and of fp32 OPT inference: y[M,N] = act(x[M,K] W[N,K]^T + bias) (+ res),
 // split-bf16 3-pass on (hi, lo) pairs of x and W, fp32 bias (or none), optional (hi, lo) residual [M, N]; the result as a
 // (hi, lo) pair y_hi / y_lo, or fp32 into y32 when y32 is given; output pitch ldy.
-inline int sk_linear_split_launch(int M, int N, int K, const bf16* x_hi, const bf16* x_lo, const bf16* w_hi, const bf16* w_lo,
-                                  const float* bias, int act, const bf16* res_hi, const bf16* res_lo, bf16* y_hi, bf16* y_lo,
-                                  float* y32, int ldy, cudaStream_t s) {
-  SkGemmEx g;
-  memset(&g, 0, sizeof(g));
-  g.M = M; g.N = N; g.K = K; g.batch = 1; g.passes = 3;
+inline SkGemmEx sk_gemm_linear_split(int M, int N, int K, const bf16* x_hi, const bf16* x_lo, const bf16* w_hi,
+                                     const bf16* w_lo, const float* bias, int act, const bf16* res_hi, const bf16* res_lo,
+                                     bf16* y_hi, bf16* y_lo, float* y32, int ldy) {
+  SkGemmEx g = sk_gemm_base(M, N, K);
+  g.passes = 3;
   g.A = x_hi; g.A_lo = x_lo; g.lda = K;
   g.B = w_hi; g.B_lo = w_lo; g.ldb = K;
   if (y32) { g.C = y32; g.out_f32 = 1; } else { g.C = y_hi; g.C_lo = y_lo; }
@@ -71,29 +185,8 @@ inline int sk_linear_split_launch(int M, int N, int K, const bf16* x_hi, const b
   if (bias) { g.bias = bias; g.bias_f32 = 1; }
   if (res_hi) { g.residual = res_hi; g.residual_lo = res_lo; g.ldr = N; }
   g.act = act;
-  return sk_gemm_ex_launch(g, s);
+  return g;
 }
-struct SkGemmPlan;
-int sk_gemm_plan_ex(const SkGemmEx& g, SkGemmPlan* out);   // the decisions sk_gemm_ex_launch makes for g, nothing launched
-int sk_gemm_launch(int M, int N, int K, const void* A, int lda, int a_mn, const void* B, int ldb, int b_mn, void* C,
-                   int ldc, int out_f32, const void* bias, const void* residual, int ldr, int round_before_res, int act,
-                   int force_bn, cudaStream_t stream, void* splitk_ws = nullptr, size_t splitk_ws_bytes = 0);
-// the SkGemmEx that sk_gemm_launch runs
-SkGemmEx sk_gemm_desc(int M, int N, int K, const void* A, int lda, int a_mn, const void* B, int ldb, int b_mn, void* C,
-                      int ldc, int out_f32, const void* bias, const void* residual, int ldr, int round_before_res, int act,
-                      int force_bn, void* splitk_ws, size_t splitk_ws_bytes);
-int sk_linear_swiglu_fwd_launch(int M, int F, int K, const void* x, const void* Wgu, void* gu, void* act, cudaStream_t s);
-int sk_linear_swiglu_bwd_launch(int M, int N, int F, const void* dy, const void* Wd, const void* gu, void* dgu, cudaStream_t s);
-int sk_linear_rope_launch(int M, int N, int K, const void* x, const void* W, const void* bias, void* out, const void* cos_t,
-                          const void* sin_t, const int32_t* pos_ids, int T, int rope_cols, int max_positions, cudaStream_t s,
-                          int rope_rot = 0);
-// GPT-NeoX MLP: pre[M,F] = x * W1^T + b1 and act = bf16(gelu(pre)) in one epilogue; d_pre[M,F] from d_act = dy * W2
-// without materialising d_act; out = bf16(bf16(bf16(x * W^T + b) + res2) + res) (mlp + attn + x)
-int sk_linear_gelu_fwd_launch(int M, int F, int K, const void* x, const void* W1, const void* b1, void* pre, void* act,
-                              cudaStream_t s);
-int sk_linear_gelu_bwd_launch(int M, int N, int F, const void* dy, const void* W2, const void* pre, void* dpre, cudaStream_t s);
-int sk_linear_res2_launch(int M, int N, int K, const void* x, const void* W, const void* bias, const void* res2, const void* res,
-                          void* out, cudaStream_t s, void* splitk_ws = nullptr, size_t splitk_ws_bytes = 0);
 
 // lm_kernels.cu
 int sk_embed_fwd_launch(const int64_t* ids, const bf16* E, bf16* out, int M, int D, int V, cudaStream_t s);

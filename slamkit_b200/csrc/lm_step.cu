@@ -192,28 +192,34 @@ bf16* head_in(const SkLm* lm, const WsLayout& w) {
   return wsp<bf16>(lm, w.hf);
 }
 
-// y[M,N] = x[M,K] * W[N,K]^T (+bias) (+residual)
+// y[M,N] = act(x[M,K] * W[N,K]^T + bias) (+ res)
 // (forward and dgrad GEMMs get no scratch: whole-tile scheduling keeps every output row's fp32 summation order
-//  independent of the batch it sits in -- logits of a sequence are bit-identical alone or inside a batch)
+//  independent of the batch it sits in -- logits of a sequence are bit-identical alone or inside a batch; only the
+//  decode steps' down-projections, one row of output tiles, take scratch)
 int linear_fwd(int M, int N, int K, const bf16* x, const bf16* W, bf16* y, const bf16* bias, const bf16* res,
-               cudaStream_t s) {
-  return sk_gemm_launch(M, N, K, x, K, 0, W, K, 0, y, N, 0, bias, res, N, res ? 1 : 0, 0, 0, s);
+               cudaStream_t s, int act = SK_ACT_NONE, void* splitk_ws = nullptr, size_t splitk_bytes = 0) {
+  return sk_gemm_ex_launch(sk_gemm_linear(M, N, K, x, W, y, N, bias, res, act, splitk_ws, splitk_bytes), s);
 }
-// dx[M,K] = dy[M,N] * W[N,K]
-int linear_dgrad(int M, int N, int K, const bf16* dy, const bf16* W, bf16* dx, cudaStream_t s) {
-  return sk_gemm_launch(M, K, N, dy, N, 0, W, K, 1, dx, K, 0, nullptr, nullptr, 0, 0, 0, 0, s);
+// dx[M,K] = dy[M,N] * W[N,K] (+ res)
+int linear_dgrad(int M, int N, int K, const bf16* dy, const bf16* W, bf16* dx, cudaStream_t s, const bf16* res = nullptr) {
+  return sk_gemm_ex_launch(sk_gemm_dgrad(M, N, K, dy, W, dx, res), s);
 }
 // dW[N,K] (+)= dy[M,N]^T * x[M,K]   (scratch: split-K for the small wgrads, stream-K balancing for the large ones)
-int linear_wgrad(int M, int N, int K, const bf16* dy, const bf16* x, bf16* dW, int accumulate, cudaStream_t s,
+int linear_wgrad(int M, int N, int K, const bf16* dy, const bf16* x, bf16* dW, bool accumulate, cudaStream_t s,
                  void* splitk_ws, size_t splitk_bytes) {
-  return sk_gemm_launch(N, K, M, dy, N, 1, x, K, 1, dW, K, 0, nullptr, accumulate ? dW : nullptr, K, 1, 0, 0, s,
-                        splitk_ws, splitk_bytes);
+  return sk_gemm_ex_launch(sk_gemm_wgrad(M, N, K, dy, x, dW, accumulate, splitk_ws, splitk_bytes), s);
+}
+// logits [M, Vp] at pitch ldl: the lm_head on the rows h [M, K]
+int head_logits(const SkLm* lm, int M, int K, const bf16* h, void* logits, int ldl, cudaStream_t s) {
+  return sk_gemm_ex_launch(
+      sk_gemm_linear(M, lm->Vp, K, h, lm->params + lm->off_head, logits, ldl, nullptr, nullptr, SK_ACT_NONE), s);
 }
 
 int linear_qkv_rope(const SkLm* lm, int M, int T, const bf16* x, const bf16* W, const bf16* bias, bf16* qkv,
                     const int32_t* pos_ids, cudaStream_t s) {
-  return sk_linear_rope_launch(M, lm->qkv_dim, lm->d, x, W, bias, qkv, lm->rope_cos, lm->rope_sin, pos_ids, T,
-                               (lm->H + lm->KVH) * lm->hd, lm->max_pos, s);
+  return sk_gemm_ex_launch(sk_gemm_rope(M, lm->qkv_dim, lm->d, x, W, bias, qkv, lm->rope_cos, lm->rope_sin, pos_ids, T,
+                                        (lm->H + lm->KVH) * lm->hd, lm->max_pos, 0),
+                           s);
 }
 
 int check_bound(const SkLm* lm, int B, int T, const WsLayout& w, const int32_t* pos_ids) {
@@ -258,7 +264,7 @@ int head_forward(SkLm* lm, const WsLayout& w, const FwdArgs& a, const bf16* hin,
   if (!a.with_head) return 0;
   const int M = a.B * a.T;
   bf16* logits = wsp<bf16>(lm, w.logits);
-  SK_TRY(linear_fwd(M, lm->Vp, K, hin, lm->params + lm->off_head, logits, nullptr, nullptr, s));
+  SK_TRY(head_logits(lm, M, K, hin, logits, lm->Vp, s));
   if (!a.labels) return 0;
   return sk_ce_launch(logits, a.labels, a.want_dlogits ? wsp<bf16>(lm, w.dlogits) : nullptr, wsp<float>(lm, w.ce_partial),
                       a.row_nll, a.stats, M, a.T, lm->V, lm->Vp, a.num_items, a.dloss, s);
@@ -301,7 +307,7 @@ int qwen2_forward(SkLm* lm, const FwdArgs& a, const WsLayout& w, cudaStream_t s)
     SK_TRY(sk_attn_tc_fwd_launch(qkv, ao, lse, B, T, lm->H, lm->KVH, lm->qkv_dim, d, 1, scale, s, seg_start));
     SK_TRY(linear_fwd(M, d, d, ao, P + o.wo, xmid, nullptr, x, s));
     SK_TRY(sk_rmsnorm_fwd_launch(xmid, P + o.ln2, h2, r2, M, d, lm->eps, s));
-    SK_TRY(sk_linear_swiglu_fwd_launch(M, F, d, h2, P + o.wgu, gu, act, s));
+    SK_TRY(sk_gemm_ex_launch(sk_gemm_swiglu_fwd(M, F, d, h2, P + o.wgu, gu, act), s));
     SK_TRY(linear_fwd(M, d, F, act, P + o.wd, xn, nullptr, xmid, s));
   }
   bf16* xL = wsp<bf16>(lm, w.X + w.sX * L);
@@ -373,7 +379,7 @@ int qwen2_backward(SkLm* lm, const FwdArgs& a, int accumulate, const WsLayout& w
     bf16* act = wsp<bf16>(lm, w.act + w.sact * l);
 
     // MLP
-    SK_TRY(sk_linear_swiglu_bwd_launch(M, d, F, dxA, P + o.wd, gu, dgu, s));
+    SK_TRY(sk_gemm_ex_launch(sk_gemm_swiglu_bwd(M, d, F, dxA, P + o.wd, gu, dgu), s));
     SK_TRY(linear_wgrad(M, d, F, dxA, act, G + o.wd, accumulate, s, lm->ws + w.splitk, (size_t)w.splitk_bytes));
     SK_TRY(linear_dgrad(M, 2 * F, d, dgu, P + o.wgu, dh, s));
     SK_TRY(linear_wgrad(M, 2 * F, d, dgu, h2, G + o.wgu, accumulate, s, lm->ws + w.splitk, (size_t)w.splitk_bytes));
@@ -531,12 +537,13 @@ int neox_forward(SkLm* lm, const FwdArgs& a, const WsLayout& w, cudaStream_t s) 
     bf16* act = wsp<bf16>(lm, w.act + w.sact * l);
 
     SK_TRY(sk_layernorm2_fwd_launch(x, P + o.ln1w, P + o.ln1b, P + o.ln2w, P + o.ln2b, h1, h2, st, st + M, M, d, eps, s));
-    SK_TRY(sk_linear_rope_launch(M, Q, d, h1, P + o.wqkv, P + o.bqkv, qkv, lm->rope_cos, lm->rope_sin, pos_ids, T, 2 * d,
-                                 lm->max_pos, s, lm->rot));
+    SK_TRY(sk_gemm_ex_launch(sk_gemm_rope(M, Q, d, h1, P + o.wqkv, P + o.bqkv, qkv, lm->rope_cos, lm->rope_sin, pos_ids, T,
+                                          2 * d, lm->max_pos, lm->rot),
+                             s));
     SK_TRY(sk_attn_tc_fwd_launch(qkv, ao, lse, B, T, lm->H, lm->H, Q, d, 1, scale, s, seg_start));
     SK_TRY(linear_fwd(M, d, d, ao, P + o.wo, attn, P + o.bo, nullptr, s));
-    SK_TRY(sk_linear_gelu_fwd_launch(M, F, d, h2, P + o.w1, P + o.b1, pre, act, s));
-    SK_TRY(sk_linear_res2_launch(M, d, F, act, P + o.w2, P + o.b2, attn, x, xn, s));
+    SK_TRY(sk_gemm_ex_launch(sk_gemm_gelu_fwd(M, F, d, h2, P + o.w1, P + o.b1, pre, act), s));
+    SK_TRY(sk_gemm_ex_launch(sk_gemm_res2(M, d, F, act, P + o.w2, P + o.b2, attn, x, xn), s));
   }
   float* stf = wsp<float>(lm, w.rstdf);
   SK_TRY(sk_layernorm_fwd_launch(wsp<bf16>(lm, w.X + w.sX * L), P + lm->off_final_norm, P + lm->off_final_norm_b,
@@ -585,7 +592,7 @@ int neox_backward(SkLm* lm, const FwdArgs& a, int accumulate, const WsLayout& w,
     const bf16* act = wsp<bf16>(lm, w.act + w.sact * l);
 
     // MLP: d_pre = bf16(bf16(dy W2) * gelu'(pre)) from the GEMM epilogue; dh2 -> dh
-    SK_TRY(sk_linear_gelu_bwd_launch(M, d, F, dy, P + o.w2, pre, dpre, s));
+    SK_TRY(sk_gemm_ex_launch(sk_gemm_gelu_bwd(M, d, F, dy, P + o.w2, pre, dpre), s));
     SK_TRY(linear_wgrad(M, d, F, dy, act, G + o.w2, accumulate, s, sws, swb));
     SK_TRY(sk_colsum_launch(dy, G + o.b2, csp, M, d, d, accumulate, s));
     SK_TRY(linear_dgrad(M, F, d, dpre, P + o.w1, dh, s));
@@ -634,17 +641,18 @@ int neox_decode_step(SkLm* lm, const int64_t* tokens, const int32_t* pos, int B,
     bf16* kc = reinterpret_cast<bf16*>(kv_cache) + (size_t)l * 2 * plane;
     bf16* vc = kc + plane;
     SK_TRY(sk_layernorm2_fwd_launch(x, P + o.ln1w, P + o.ln1b, P + o.ln2w, P + o.ln2b, h, h2, nullptr, nullptr, B, d, eps, s));
-    SK_TRY(sk_linear_rope_launch(B, Q, d, h, P + o.wqkv, P + o.bqkv, qkv, lm->rope_cos, lm->rope_sin, pos, 1, 2 * d,
-                                 lm->max_pos, s, lm->rot));
+    SK_TRY(sk_gemm_ex_launch(
+        sk_gemm_rope(B, Q, d, h, P + o.wqkv, P + o.bqkv, qkv, lm->rope_cos, lm->rope_sin, pos, 1, 2 * d, lm->max_pos, lm->rot),
+        s));
     SK_TRY(sk_kv_append_launch(qkv, Q, kc, vc, pos, b.lens, B, lm->H, lm->H, T_cache, s));
     SK_TRY(sk_attn_decode_launch(qkv, Q, kc, vc, b.lens, ao, d, b.partial, B, lm->H, lm->H, T_cache, scale, s));
     SK_TRY(linear_fwd(B, d, d, ao, P + o.wo, attn, P + o.bo, nullptr, s));
-    SK_TRY(sk_linear_gelu_fwd_launch(B, F, d, h2, P + o.w1, P + o.b1, pre, act, s));
+    SK_TRY(sk_gemm_ex_launch(sk_gemm_gelu_fwd(B, F, d, h2, P + o.w1, P + o.b1, pre, act), s));
     // with M = B the scratch lets stream-K spread dense_4h_to_h's long K loop over idle SMs
-    SK_TRY(sk_linear_res2_launch(B, d, F, act, P + o.w2, P + o.b2, attn, x, x, s, b.gemm, b.gemm_bytes));
+    SK_TRY(sk_gemm_ex_launch(sk_gemm_res2(B, d, F, act, P + o.w2, P + o.b2, attn, x, x, b.gemm, b.gemm_bytes), s));
   }
   SK_TRY(sk_layernorm_fwd_launch(x, P + lm->off_final_norm, P + lm->off_final_norm_b, h, nullptr, nullptr, B, d, eps, s));
-  return sk_gemm_launch(B, lm->Vp, d, h, d, 0, P + lm->off_head, d, 0, logits, ldl, 0, nullptr, nullptr, 0, 0, 0, 0, s);
+  return head_logits(lm, B, d, h, logits, ldl, s);
 }
 
 // ---- OPT with fp32 master weights (sk_lm_set_master): HF OPTForCausalLM with fp32 parameters under
@@ -684,7 +692,7 @@ int opt_master_forward(SkLm* lm, const FwdArgs& a, const WsLayout& w, cudaStream
     SK_TRY(sk_attn_tc_fwd_launch(qkv, ao, lse, B, T, lm->H, lm->H, Q, d, 1, scale, s, seg_start));
     SK_TRY(linear_fwd(M, d, d, ao, P + o.wo, y, P + o.bo, nullptr, s));
     SK_TRY(sk_add_layernorm_f32_launch(x, y, P32 + o.ln2w, P32 + o.ln2b, xmid, h2, st2, st2 + M, M, d, eps, s));
-    SK_TRY(sk_gemm_launch(M, F, d, h2, d, 0, P + o.w1, d, 0, a, F, 0, P + o.b1, nullptr, 0, 0, 2, 0, s));   // relu(fc1)
+    SK_TRY(linear_fwd(M, F, d, h2, P + o.w1, a, P + o.b1, nullptr, s, SK_ACT_RELU));   // relu(fc1)
     SK_TRY(linear_fwd(M, d, F, a, P + o.w2, y, P + o.b2, nullptr, s));
   }
   float* stf = wsp<float>(lm, w.rstdf);
@@ -740,22 +748,22 @@ int opt_master_backward(SkLm* lm, const FwdArgs& a, int accumulate, const WsLayo
     // MLP on bf16(dres)
     SK_TRY(linear_dgrad(M, d, F, dr16, P + o.w2, da, s));
     SK_TRY(sk_relu_bwd_launch(da, a, (long)M * F, s));
-    SK_TRY(linear_wgrad(M, d, F, dr16, a, G + o.w2, 0, s, sws, swb));
+    SK_TRY(linear_wgrad(M, d, F, dr16, a, G + o.w2, false, s, sws, swb));
     SK_TRY(sk_colsum_launch(dr16, G + o.b2, csp, M, d, d, 0, s));
     SK_TRY(linear_dgrad(M, F, d, da, P + o.w1, dh, s));
-    SK_TRY(linear_wgrad(M, F, d, da, h2, G + o.w1, 0, s, sws, swb));
+    SK_TRY(linear_wgrad(M, F, d, da, h2, G + o.w1, false, s, sws, swb));
     SK_TRY(sk_colsum_launch(da, G + o.b1, csp, M, F, F, 0, s));
     SK_TRY(sk_layernorm_bwd_f32_launch(dh, xmid, P32 + o.ln2w, st2, st2 + M, dres, dres, dr16, G32 + o.ln2w, G32 + o.ln2b, lnp, M,
                                        d, accumulate, s));
     // attention on bf16(dres)
     SK_TRY(linear_dgrad(M, d, d, dr16, P + o.wo, dao, s));
-    SK_TRY(linear_wgrad(M, d, d, dr16, ao, G + o.wo, 0, s, sws, swb));
+    SK_TRY(linear_wgrad(M, d, d, dr16, ao, G + o.wo, false, s, sws, swb));
     SK_TRY(sk_colsum_launch(dr16, G + o.bo, csp, M, d, d, 0, s));
     SK_TRY(sk_attn_tc_bwd_launch(qkv, ao, dao, lse, wsp<float>(lm, w.delta), nullptr, dqkv, B, T, lm->H, lm->H, Q, d, Q, 1,
                                  scale, s, seg_start, seg_end));
     SK_TRY(sk_colsum_launch(dqkv, G + o.bqkv, csp, M, Q, Q, 0, s));
     SK_TRY(linear_dgrad(M, Q, d, dqkv, P + o.wqkv, dh, s));
-    SK_TRY(linear_wgrad(M, Q, d, dqkv, h1, G + o.wqkv, 0, s, sws, swb));
+    SK_TRY(linear_wgrad(M, Q, d, dqkv, h1, G + o.wqkv, false, s, sws, swb));
     SK_TRY(sk_layernorm_bwd_f32_launch(dh, x, P32 + o.ln1w, st1, st1 + M, dres, dres, dr16, G32 + o.ln1w, G32 + o.ln1b, lnp, M, d,
                                        accumulate, s));
     if (!lm->bwd_events.empty()) SK_CUDA_CHECK(cudaEventRecord(lm->bwd_events[l], s));
@@ -812,7 +820,7 @@ int opt_postln_forward(SkLm* lm, const FwdArgs& a, const WsLayout& w, cudaStream
     SK_TRY(sk_attn_tc_fwd_launch(qkv, ao, lse, B, T, lm->H, lm->H, Q, d, 1, scale, s, seg_start));
     SK_TRY(linear_fwd(M, d, d, ao, P + o.wo, s1, P + o.bo, x, s));
     SK_TRY(sk_layernorm_fwd_launch(s1, P + o.ln1w, P + o.ln1b, y1, st1, st1 + M, M, d, eps, s));
-    SK_TRY(sk_gemm_launch(M, F, d, y1, d, 0, P + o.w1, d, 0, a, F, 0, P + o.b1, nullptr, 0, 0, 2, 0, s));   // relu(fc1)
+    SK_TRY(linear_fwd(M, F, d, y1, P + o.w1, a, P + o.b1, nullptr, s, SK_ACT_RELU));   // relu(fc1)
     SK_TRY(linear_fwd(M, d, F, a, P + o.w2, s2, P + o.b2, y1, s));
     SK_TRY(sk_layernorm_fwd_launch(s2, P + o.ln2w, P + o.ln2b, xn, st2, st2 + M, M, d, eps, s));
   }
@@ -873,7 +881,7 @@ int opt_postln_backward(SkLm* lm, const FwdArgs& a, int accumulate, const WsLayo
     SK_TRY(linear_wgrad(M, d, F, dxB, a, G + o.w2, accumulate, s, sws, swb));
     SK_TRY(sk_colsum_launch(dxB, G + o.b2, csp, M, d, d, accumulate, s));
     // dy1 = bf16(ds2 + bf16(da W_1)) -> dxA: fc1's dgrad with the skip path's gradient as its residual
-    SK_TRY(sk_gemm_launch(M, d, F, da, F, 0, P + o.w1, d, 1, dxA, d, 0, nullptr, dxB, d, 1, 0, 0, s));
+    SK_TRY(linear_dgrad(M, F, d, da, P + o.w1, dxA, s, dxB));
     SK_TRY(linear_wgrad(M, F, d, da, y1, G + o.w1, accumulate, s, sws, swb));
     SK_TRY(sk_colsum_launch(da, G + o.b1, csp, M, F, F, accumulate, s));
     // LN1 backward from s1: ds1 -> dxB
@@ -887,7 +895,7 @@ int opt_postln_backward(SkLm* lm, const FwdArgs& a, int accumulate, const WsLayo
                                  scale, s, seg_start, seg_end));
     SK_TRY(sk_colsum_launch(dqkv, G + o.bqkv, csp, M, Q, Q, accumulate, s));
     // dx = bf16(ds1 + bf16(dqkv W_qkv)) -> dxA
-    SK_TRY(sk_gemm_launch(M, d, Q, dqkv, Q, 0, P + o.wqkv, d, 1, dxA, d, 0, nullptr, dxB, d, 1, 0, 0, s));
+    SK_TRY(linear_dgrad(M, Q, d, dqkv, P + o.wqkv, dxA, s, dxB));
     SK_TRY(linear_wgrad(M, Q, d, dqkv, x, G + o.wqkv, accumulate, s, sws, swb));
     if (!lm->bwd_events.empty()) SK_CUDA_CHECK(cudaEventRecord(lm->bwd_events[l], s));
   }
@@ -933,7 +941,7 @@ int opt_forward(SkLm* lm, const FwdArgs& a, const WsLayout& w, cudaStream_t s) {
     SK_TRY(sk_attn_tc_fwd_launch(qkv, ao, lse, B, T, lm->H, lm->H, Q, d, 1, scale, s, seg_start));
     SK_TRY(linear_fwd(M, d, d, ao, P + o.wo, xmid, P + o.bo, x, s));
     SK_TRY(sk_layernorm_fwd_launch(xmid, P + o.ln2w, P + o.ln2b, h2, st2, st2 + M, M, d, eps, s));
-    SK_TRY(sk_gemm_launch(M, F, d, h2, d, 0, P + o.w1, d, 0, a, F, 0, P + o.b1, nullptr, 0, 0, 2, 0, s));   // relu(fc1)
+    SK_TRY(linear_fwd(M, F, d, h2, P + o.w1, a, P + o.b1, nullptr, s, SK_ACT_RELU));   // relu(fc1)
     SK_TRY(linear_fwd(M, d, F, a, P + o.w2, xn, P + o.b2, xmid, s));
   }
   float* stf = wsp<float>(lm, w.rstdf);
@@ -1041,8 +1049,8 @@ int opt_postln_decode_step(SkLm* lm, const int64_t* tokens, const int32_t* pos, 
     SK_TRY(sk_attn_decode_launch(qkv, Q, kc, vc, b.lens, ao, d, b.partial, B, lm->H, lm->H, T_cache, scale, s));
     SK_TRY(linear_fwd(B, d, d, ao, P + o.wo, xm, P + o.bo, x, s));
     SK_TRY(sk_layernorm_fwd_launch(xm, P + o.ln1w, P + o.ln1b, h, nullptr, nullptr, B, d, eps, s));
-    SK_TRY(sk_gemm_launch(B, F, d, h, d, 0, P + o.w1, d, 0, a, F, 0, P + o.b1, nullptr, 0, 0, 2, 0, s));
-    SK_TRY(sk_gemm_launch(B, d, F, a, F, 0, P + o.w2, F, 0, xm, d, 0, P + o.b2, h, d, 1, 0, 0, s, b.gemm, b.gemm_bytes));
+    SK_TRY(linear_fwd(B, F, d, h, P + o.w1, a, P + o.b1, nullptr, s, SK_ACT_RELU));
+    SK_TRY(linear_fwd(B, d, F, a, P + o.w2, xm, P + o.b2, h, s, SK_ACT_NONE, b.gemm, b.gemm_bytes));
     SK_TRY(sk_layernorm_fwd_launch(xm, P + o.ln2w, P + o.ln2b, x, nullptr, nullptr, B, d, eps, s));
   }
   const bf16* hin = x;
@@ -1050,7 +1058,7 @@ int opt_postln_decode_step(SkLm* lm, const int64_t* tokens, const int32_t* pos, 
     SK_TRY(linear_fwd(B, K, d, x, P + lm->off_pout, h, nullptr, nullptr, s));
     hin = h;
   }
-  return sk_gemm_launch(B, lm->Vp, K, hin, K, 0, P + lm->off_head, K, 0, logits, ldl, 0, nullptr, nullptr, 0, 0, 0, 0, s);
+  return head_logits(lm, B, K, hin, logits, ldl, s);
 }
 
 // One token per row at position pos[b] (read on the device: the step is graph-capturable).  The KV cache layout is the
@@ -1079,13 +1087,13 @@ int opt_decode_step(SkLm* lm, const int64_t* tokens, const int32_t* pos, int B, 
     SK_TRY(sk_attn_decode_launch(qkv, Q, kc, vc, b.lens, ao, d, b.partial, B, lm->H, lm->H, T_cache, scale, s));
     SK_TRY(linear_fwd(B, d, d, ao, P + o.wo, xm, P + o.bo, x, s));
     SK_TRY(sk_layernorm_fwd_launch(xm, P + o.ln2w, P + o.ln2b, h, nullptr, nullptr, B, d, eps, s));
-    SK_TRY(sk_gemm_launch(B, F, d, h, d, 0, P + o.w1, d, 0, a, F, 0, P + o.b1, nullptr, 0, 0, 2, 0, s));
+    SK_TRY(linear_fwd(B, F, d, h, P + o.w1, a, P + o.b1, nullptr, s, SK_ACT_RELU));
     // fc2 + bias + residual into x (not in place): with M = B the scratch lets stream-K spread the long K loop over idle
     // SMs; rounded before the residual add like the forward pass
-    SK_TRY(sk_gemm_launch(B, d, F, a, F, 0, P + o.w2, F, 0, x, d, 0, P + o.b2, xm, d, 1, 0, 0, s, b.gemm, b.gemm_bytes));
+    SK_TRY(linear_fwd(B, d, F, a, P + o.w2, x, P + o.b2, xm, s, SK_ACT_NONE, b.gemm, b.gemm_bytes));
   }
   SK_TRY(sk_layernorm_fwd_launch(x, P + lm->off_final_norm, P + lm->off_final_norm_b, h, nullptr, nullptr, B, d, eps, s));
-  return sk_gemm_launch(B, lm->Vp, d, h, d, 0, P + lm->off_head, d, 0, logits, ldl, 0, nullptr, nullptr, 0, 0, 0, 0, s);
+  return head_logits(lm, B, d, h, logits, ldl, s);
 }
 
 // ---- OPT fp32 inference (sk_lm_set_fp32): HF OPTForCausalLM in fp32, as the reference scores and generates a float32
@@ -1098,12 +1106,13 @@ struct Pair {
   bf16* lo;
 };
 
-// sk_linear_split_launch on the split weights at w_off (bias fp32 at b_off >= 0)
+// sk_gemm_linear_split on the split weights at w_off (bias fp32 at b_off >= 0)
 int linear_split(const SkLm* lm, int M, int N, int K, Pair x, int64_t w_off, int64_t b_off, int act, const Pair* res, Pair y,
                  float* y32, int ldy, cudaStream_t s) {
-  return sk_linear_split_launch(M, N, K, x.hi, x.lo, lm->w_hi + w_off, lm->w_lo + w_off,
-                                b_off >= 0 ? lm->params32 + b_off : nullptr, act, res ? res->hi : nullptr,
-                                res ? res->lo : nullptr, y.hi, y.lo, y32, ldy, s);
+  return sk_gemm_ex_launch(sk_gemm_linear_split(M, N, K, x.hi, x.lo, lm->w_hi + w_off, lm->w_lo + w_off,
+                                                b_off >= 0 ? lm->params32 + b_off : nullptr, act, res ? res->hi : nullptr,
+                                                res ? res->lo : nullptr, y.hi, y.lo, y32, ldy),
+                           s);
 }
 
 // the lm_head's input rows [M, head_k] of fp32 inference: the final LayerNorm's output in h1, or for post-LN OPT the last
@@ -1129,7 +1138,7 @@ int opt_postln_forward_fp32(SkLm* lm, const FwdArgs& fa, const WsLayout& w, cuda
     SK_TRY(sk_split_f32_launch(e32, xm.hi, xm.lo, (long)M * d, s));
     SK_TRY(sk_opt_embed_fwd_f32_launch(ids, nullptr, P32 + lm->off_embed, nullptr, e32, M, T, K, lm->V, lm->n_pos, s));
     SK_TRY(sk_split_f32_launch(e32, h.hi, h.lo, (long)M * K, s));
-    SK_TRY(linear_split(lm, M, d, K, h, lm->off_pin, -1, 0, &xm, x, nullptr, d, s));
+    SK_TRY(linear_split(lm, M, d, K, h, lm->off_pin, -1, SK_ACT_NONE, &xm, x, nullptr, d, s));
   } else {
     SK_TRY(sk_opt_embed_fwd_f32_launch(ids, nullptr, P32 + lm->off_embed, P32 + lm->off_pos, e32, M, T, d, lm->V, lm->n_pos, s));
     SK_TRY(sk_split_f32_launch(e32, x.hi, x.lo, (long)M * d, s));
@@ -1138,21 +1147,21 @@ int opt_postln_forward_fp32(SkLm* lm, const FwdArgs& fa, const WsLayout& w, cuda
   const size_t plane = (size_t)B * lm->H * fa.T_cache * lm->hd;
   for (int l = 0; l < L; ++l) {
     const LnLayerOff& o = lm->lnl[l];
-    SK_TRY(linear_split(lm, M, Q, d, x, o.wqkv, o.bqkv, 0, nullptr, qkv, nullptr, Q, s));
+    SK_TRY(linear_split(lm, M, Q, d, x, o.wqkv, o.bqkv, SK_ACT_NONE, nullptr, qkv, nullptr, Q, s));
     if (fa.kv)
       SK_TRY(sk_kv_prefill_f32_launch(qkv.hi, qkv.lo, Q, fa.kv + (size_t)l * 2 * plane, fa.lens, B, T, lm->H, fa.T_cache, s));
     SK_TRY(sk_attn_tc_fwd_split_launch(qkv.hi, qkv.lo, ao.hi, ao.lo, B, T, lm->H, Q, d, scale, s, 1));
-    SK_TRY(linear_split(lm, M, d, d, ao, o.wo, o.bo, 0, &x, xm, nullptr, d, s));
+    SK_TRY(linear_split(lm, M, d, d, ao, o.wo, o.bo, SK_ACT_NONE, &x, xm, nullptr, d, s));
     SK_TRY(sk_layernorm_hilo_launch(xm.hi, xm.lo, nullptr, nullptr, P32 + o.ln1w, P32 + o.ln1b, h.hi, h.lo, nullptr, M, d, eps, s));
-    SK_TRY(linear_split(lm, M, F, d, h, o.w1, o.b1, 2, nullptr, a, nullptr, F, s));   // relu(fc1)
-    SK_TRY(linear_split(lm, M, d, F, a, o.w2, o.b2, 0, &h, xm, nullptr, d, s));
+    SK_TRY(linear_split(lm, M, F, d, h, o.w1, o.b1, SK_ACT_RELU, nullptr, a, nullptr, F, s));   // relu(fc1)
+    SK_TRY(linear_split(lm, M, d, F, a, o.w2, o.b2, SK_ACT_NONE, &h, xm, nullptr, d, s));
     SK_TRY(sk_layernorm_hilo_launch(xm.hi, xm.lo, nullptr, nullptr, P32 + o.ln2w, P32 + o.ln2b, x.hi, x.lo, nullptr, M, d, eps, s));
   }
-  if (lm->proj) SK_TRY(linear_split(lm, M, K, d, x, lm->off_pout, -1, 0, nullptr, h, nullptr, K, s));
+  if (lm->proj) SK_TRY(linear_split(lm, M, K, d, x, lm->off_pout, -1, SK_ACT_NONE, nullptr, h, nullptr, K, s));
   lm->last_B = B;
   lm->last_T = T;
   if (!fa.with_head) return 0;
-  return linear_split(lm, M, lm->Vp, K, head_in_fp32(lm, w), lm->off_head, -1, 0, nullptr, Pair{nullptr, nullptr},
+  return linear_split(lm, M, lm->Vp, K, head_in_fp32(lm, w), lm->off_head, -1, SK_ACT_NONE, nullptr, Pair{nullptr, nullptr},
                       wsp<float>(lm, w.logits), lm->Vp, s);
 }
 
@@ -1172,7 +1181,7 @@ int opt_postln_decode_step_fp32(SkLm* lm, const int64_t* tokens, const int32_t* 
     SK_TRY(sk_split_f32_launch(b.e32, xm.hi, xm.lo, (long)B * d, s));
     SK_TRY(sk_opt_embed_fwd_f32_launch(tokens, pos, P32 + lm->off_embed, nullptr, b.e32, B, 1, K, lm->V, lm->n_pos, s));
     SK_TRY(sk_split_f32_launch(b.e32, h.hi, h.lo, (long)B * K, s));
-    SK_TRY(linear_split(lm, B, d, K, h, lm->off_pin, -1, 0, &xm, x, nullptr, d, s));
+    SK_TRY(linear_split(lm, B, d, K, h, lm->off_pin, -1, SK_ACT_NONE, &xm, x, nullptr, d, s));
   } else {
     SK_TRY(sk_opt_embed_fwd_f32_launch(tokens, pos, P32 + lm->off_embed, P32 + lm->off_pos, b.e32, B, 1, d, lm->V, lm->n_pos, s));
     SK_TRY(sk_split_f32_launch(b.e32, x.hi, x.lo, (long)B * d, s));
@@ -1181,21 +1190,21 @@ int opt_postln_decode_step_fp32(SkLm* lm, const int64_t* tokens, const int32_t* 
     const LnLayerOff& o = lm->lnl[l];
     float* kc = kv + (size_t)l * 2 * plane;
     float* vc = kc + plane;
-    SK_TRY(linear_split(lm, B, Q, d, x, o.wqkv, o.bqkv, 0, nullptr, qkv, nullptr, Q, s));
+    SK_TRY(linear_split(lm, B, Q, d, x, o.wqkv, o.bqkv, SK_ACT_NONE, nullptr, qkv, nullptr, Q, s));
     SK_TRY(sk_kv_append_f32_launch(qkv.hi, qkv.lo, Q, kc, vc, pos, b.lens, B, lm->H, T_cache, s));
     SK_TRY(sk_attn_decode_f32_launch(qkv.hi, qkv.lo, Q, kc, vc, b.lens, ao.hi, ao.lo, d, b.partial, B, lm->H, T_cache, scale, s));
-    SK_TRY(linear_split(lm, B, d, d, ao, o.wo, o.bo, 0, &x, xm, nullptr, d, s));
+    SK_TRY(linear_split(lm, B, d, d, ao, o.wo, o.bo, SK_ACT_NONE, &x, xm, nullptr, d, s));
     SK_TRY(sk_layernorm_hilo_launch(xm.hi, xm.lo, nullptr, nullptr, P32 + o.ln1w, P32 + o.ln1b, h.hi, h.lo, nullptr, B, d, eps, s));
-    SK_TRY(linear_split(lm, B, F, d, h, o.w1, o.b1, 2, nullptr, a, nullptr, F, s));
-    SK_TRY(linear_split(lm, B, d, F, a, o.w2, o.b2, 0, &h, xm, nullptr, d, s));
+    SK_TRY(linear_split(lm, B, F, d, h, o.w1, o.b1, SK_ACT_RELU, nullptr, a, nullptr, F, s));
+    SK_TRY(linear_split(lm, B, d, F, a, o.w2, o.b2, SK_ACT_NONE, &h, xm, nullptr, d, s));
     SK_TRY(sk_layernorm_hilo_launch(xm.hi, xm.lo, nullptr, nullptr, P32 + o.ln2w, P32 + o.ln2b, x.hi, x.lo, nullptr, B, d, eps, s));
   }
   Pair hin = x;
   if (lm->proj) {
-    SK_TRY(linear_split(lm, B, K, d, x, lm->off_pout, -1, 0, nullptr, h, nullptr, K, s));
+    SK_TRY(linear_split(lm, B, K, d, x, lm->off_pout, -1, SK_ACT_NONE, nullptr, h, nullptr, K, s));
     hin = h;
   }
-  return linear_split(lm, B, lm->Vp, K, hin, lm->off_head, -1, 0, nullptr, Pair{nullptr, nullptr}, logits, ldl, s);
+  return linear_split(lm, B, lm->Vp, K, hin, lm->off_head, -1, SK_ACT_NONE, nullptr, Pair{nullptr, nullptr}, logits, ldl, s);
 }
 
 int opt_forward_fp32(SkLm* lm, const FwdArgs& fa, const WsLayout& w, cudaStream_t s) {
@@ -1215,22 +1224,22 @@ int opt_forward_fp32(SkLm* lm, const FwdArgs& fa, const WsLayout& w, cudaStream_
   for (int l = 0; l < L; ++l) {
     const LnLayerOff& o = lm->lnl[l];
     SK_TRY(sk_layernorm_hilo_launch(x.hi, x.lo, nullptr, nullptr, P32 + o.ln1w, P32 + o.ln1b, h.hi, h.lo, nullptr, M, d, eps, s));
-    SK_TRY(linear_split(lm, M, Q, d, h, o.wqkv, o.bqkv, 0, nullptr, qkv, nullptr, Q, s));
+    SK_TRY(linear_split(lm, M, Q, d, h, o.wqkv, o.bqkv, SK_ACT_NONE, nullptr, qkv, nullptr, Q, s));
     if (fa.kv)
       SK_TRY(sk_kv_prefill_f32_launch(qkv.hi, qkv.lo, Q, fa.kv + (size_t)l * 2 * plane, fa.lens, B, T, lm->H, fa.T_cache, s));
     SK_TRY(sk_attn_tc_fwd_split_launch(qkv.hi, qkv.lo, ao.hi, ao.lo, B, T, lm->H, Q, d, scale, s, 1));
-    SK_TRY(linear_split(lm, M, d, d, ao, o.wo, o.bo, 0, &x, xm, nullptr, d, s));
+    SK_TRY(linear_split(lm, M, d, d, ao, o.wo, o.bo, SK_ACT_NONE, &x, xm, nullptr, d, s));
     SK_TRY(sk_layernorm_hilo_launch(xm.hi, xm.lo, nullptr, nullptr, P32 + o.ln2w, P32 + o.ln2b, h.hi, h.lo, nullptr, M, d, eps, s));
-    SK_TRY(linear_split(lm, M, F, d, h, o.w1, o.b1, 2, nullptr, a, nullptr, F, s));   // relu(fc1)
-    SK_TRY(linear_split(lm, M, d, F, a, o.w2, o.b2, 0, &xm, x, nullptr, d, s));
+    SK_TRY(linear_split(lm, M, F, d, h, o.w1, o.b1, SK_ACT_RELU, nullptr, a, nullptr, F, s));   // relu(fc1)
+    SK_TRY(linear_split(lm, M, d, F, a, o.w2, o.b2, SK_ACT_NONE, &xm, x, nullptr, d, s));
   }
   SK_TRY(sk_layernorm_hilo_launch(x.hi, x.lo, nullptr, nullptr, P32 + lm->off_final_norm, P32 + lm->off_final_norm_b, h.hi,
                                   h.lo, nullptr, M, d, eps, s));
   lm->last_B = B;
   lm->last_T = T;
   if (!fa.with_head) return 0;
-  return linear_split(lm, M, lm->Vp, d, h, lm->off_head, -1, 0, nullptr, Pair{nullptr, nullptr}, wsp<float>(lm, w.logits),
-                      lm->Vp, s);
+  return linear_split(lm, M, lm->Vp, d, h, lm->off_head, -1, SK_ACT_NONE, nullptr, Pair{nullptr, nullptr},
+                      wsp<float>(lm, w.logits), lm->Vp, s);
 }
 
 // One token per row at position pos[b] on the fp32 cache ([K|V][B][H][T_cache][64] fp32 per layer); fp32 logits [B, ldl]
@@ -1251,17 +1260,17 @@ int opt_decode_step_fp32(SkLm* lm, const int64_t* tokens, const int32_t* pos, in
     float* kc = kv + (size_t)l * 2 * plane;
     float* vc = kc + plane;
     SK_TRY(sk_layernorm_hilo_launch(x.hi, x.lo, nullptr, nullptr, P32 + o.ln1w, P32 + o.ln1b, h.hi, h.lo, nullptr, B, d, eps, s));
-    SK_TRY(linear_split(lm, B, Q, d, h, o.wqkv, o.bqkv, 0, nullptr, qkv, nullptr, Q, s));
+    SK_TRY(linear_split(lm, B, Q, d, h, o.wqkv, o.bqkv, SK_ACT_NONE, nullptr, qkv, nullptr, Q, s));
     SK_TRY(sk_kv_append_f32_launch(qkv.hi, qkv.lo, Q, kc, vc, pos, b.lens, B, lm->H, T_cache, s));
     SK_TRY(sk_attn_decode_f32_launch(qkv.hi, qkv.lo, Q, kc, vc, b.lens, ao.hi, ao.lo, d, b.partial, B, lm->H, T_cache, scale, s));
-    SK_TRY(linear_split(lm, B, d, d, ao, o.wo, o.bo, 0, &x, xm, nullptr, d, s));
+    SK_TRY(linear_split(lm, B, d, d, ao, o.wo, o.bo, SK_ACT_NONE, &x, xm, nullptr, d, s));
     SK_TRY(sk_layernorm_hilo_launch(xm.hi, xm.lo, nullptr, nullptr, P32 + o.ln2w, P32 + o.ln2b, h.hi, h.lo, nullptr, B, d, eps, s));
-    SK_TRY(linear_split(lm, B, F, d, h, o.w1, o.b1, 2, nullptr, a, nullptr, F, s));
-    SK_TRY(linear_split(lm, B, d, F, a, o.w2, o.b2, 0, &xm, x, nullptr, d, s));
+    SK_TRY(linear_split(lm, B, F, d, h, o.w1, o.b1, SK_ACT_RELU, nullptr, a, nullptr, F, s));
+    SK_TRY(linear_split(lm, B, d, F, a, o.w2, o.b2, SK_ACT_NONE, &xm, x, nullptr, d, s));
   }
   SK_TRY(sk_layernorm_hilo_launch(x.hi, x.lo, nullptr, nullptr, P32 + lm->off_final_norm, P32 + lm->off_final_norm_b, h.hi,
                                   h.lo, nullptr, B, d, eps, s));
-  return linear_split(lm, B, lm->Vp, d, h, lm->off_head, -1, 0, nullptr, Pair{nullptr, nullptr}, logits, ldl, s);
+  return linear_split(lm, B, lm->Vp, d, h, lm->off_head, -1, SK_ACT_NONE, nullptr, Pair{nullptr, nullptr}, logits, ldl, s);
 }
 
 #define SK_REFUSE_FP32(lm, who)                                                                                          \
@@ -1349,21 +1358,20 @@ int qwen2_decode_step(SkLm* lm, const int64_t* tokens, const int32_t* pos, int B
     bf16* kc = reinterpret_cast<bf16*>(kv_cache) + (size_t)l * 2 * plane;
     bf16* vc = kc + plane;
     SK_TRY(sk_rmsnorm_fwd_launch(x, P + o.ln1, h, nullptr, B, d, lm->eps, s));
-    SK_TRY(sk_linear_rope_launch(B, Q, d, h, P + o.wqkv, lm->qkv_bias ? P + o.bqkv : nullptr, qkv, lm->rope_cos,
-                                 lm->rope_sin, pos, 1, (lm->H + lm->KVH) * lm->hd, lm->max_pos, s));
+    SK_TRY(linear_qkv_rope(lm, B, 1, h, P + o.wqkv, lm->qkv_bias ? P + o.bqkv : nullptr, qkv, pos, s));
     SK_TRY(sk_kv_append_launch(qkv, Q, kc, vc, pos, b.lens, B, lm->H, lm->KVH, T_cache, s));
     SK_TRY(sk_attn_decode_launch(qkv, Q, kc, vc, b.lens, ao, d, b.partial, B, lm->H, lm->KVH, T_cache, scale, s));
     SK_TRY(linear_fwd(B, d, d, ao, P + o.wo, xm, nullptr, x, s));
     SK_TRY(sk_rmsnorm_fwd_launch(xm, P + o.ln2, h, nullptr, B, d, lm->eps, s));
-    SK_TRY(sk_linear_swiglu_fwd_launch(B, F, d, h, P + o.wgu, gu, act, s));
+    SK_TRY(sk_gemm_ex_launch(sk_gemm_swiglu_fwd(B, F, d, h, P + o.wgu, gu, act), s));
     // down projection added in place (residual == output): with M = B there is a single row of output tiles, so the
     // scratch lets the GEMM split its long K loop over idle SMs (fixed-order reduction); rounded before the residual
     // add like the forward pass's down projection
-    SK_TRY(sk_gemm_launch(B, d, F, act, F, 0, P + o.wd, F, 0, xm, d, 0, nullptr, xm, d, 1, 0, 0, s, b.gemm, b.gemm_bytes));
+    SK_TRY(linear_fwd(B, d, F, act, P + o.wd, xm, nullptr, xm, s, SK_ACT_NONE, b.gemm, b.gemm_bytes));
     std::swap(x, xm);
   }
   SK_TRY(sk_rmsnorm_fwd_launch(x, P + lm->off_final_norm, h, nullptr, B, d, lm->eps, s));
-  return sk_gemm_launch(B, lm->Vp, d, h, d, 0, P + lm->off_head, d, 0, logits, ldl, 0, nullptr, nullptr, 0, 0, 0, 0, s);
+  return head_logits(lm, B, d, h, logits, ldl, s);
 }
 
 // ---- the decoder variant: (fp32 inference) -> architecture -> (post-LN) -> (master weights), the only place that picks
@@ -1440,14 +1448,13 @@ int sk_lm_prefill(SkLm* lm, const int64_t* ids, const int32_t* lens, int B, int 
     const Pair hl{b.h, b.h + (int64_t)B * lm->d};
     SK_TRY(sk_gather_last_launch(hf.hi, lens, hl.hi, B, T, K, s));
     SK_TRY(sk_gather_last_launch(hf.lo, lens, hl.lo, B, T, K, s));
-    return linear_split(lm, B, lm->Vp, K, hl, lm->off_head, -1, 0, nullptr, Pair{nullptr, nullptr},
+    return linear_split(lm, B, lm->Vp, K, hl, lm->off_head, -1, SK_ACT_NONE, nullptr, Pair{nullptr, nullptr},
                         reinterpret_cast<float*>(logits), ldl, s);
   }
   SK_TRY(sk_kv_prefill_launch(wsp<bf16>(lm, w.qkv), w.sqkv / 2, lm->qkv_dim, reinterpret_cast<bf16*>(kv_cache), lens, lm->L, B,
                               T, lm->H, lm->KVH, T_cache, s));
   SK_TRY(sk_gather_last_launch(head_in(lm, w), lens, b.h, B, T, K, s));
-  return sk_gemm_launch(B, lm->Vp, K, b.h, K, 0, lm->params + lm->off_head, K, 0, logits, ldl, 0, nullptr, nullptr,
-                        0, 0, 0, 0, s);
+  return head_logits(lm, B, K, b.h, logits, ldl, s);
 }
 
 int sk_lm_kv_fanout(const SkLm* lm, const void* src_cache, int B, int k, void* dst_cache, int T_cache, const int32_t* lens,

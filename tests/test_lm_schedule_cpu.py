@@ -78,7 +78,7 @@ def launcher_stubs():
     """kernels.h's launchers that lm_step.cu calls, each defined to print its arguments"""
     header = _strip_comments(open(os.path.join(CSRC, "kernels.h")).read())
     used = set(re.findall(r"\b(sk_\w+)\s*\(", open(os.path.join(CSRC, "lm_step.cu")).read()))
-    used.add("sk_gemm_ex_launch")   # behind the inline sk_linear_split_launch
+    used.add("sk_gemm_ex_launch")   # the launcher behind every GEMM descriptor builder
     out = ['#include "kernels.h"', '#include "trace.h"', ""]
     decls = re.finditer(r"^(extern \"C\" )?(int|size_t|SkGemmEx)\s+(sk_\w+)\(([^)]*)\)\s*;", header, re.M)
     for m in decls:
