@@ -118,7 +118,8 @@ def main(argv=None):
 
 
 def generate_max_seq(cfg, tokeniser, dataset) -> int:
-    """LM rows needed by `metric=generate`: BOS + the units of the longest prompt (at most one per HuBERT frame) +
+    """LM rows needed by `metric=generate`: the units of the longest prompt (at most one per HuBERT frame), what the
+    tokeniser puts around them (the unit tokeniser's BOS; the interleaved tokeniser's prefix and `<speech>` marker) and
     max_new_tokens."""
     from slamkit_b200.audio_io import audio_info
     sr = tokeniser.fe_sample_rate
@@ -129,7 +130,8 @@ def generate_max_seq(cfg, tokeniser, dataset) -> int:
         cut = dataset.crop(i)
         longest = max(longest, n if cut is None else min(n, cut))
     new = int(cfg.metric.get("generate_kwargs", {}).get("max_new_tokens", 20))
-    return tokeniser.model.frames(max(longest, 1)) + 1 + new
+    extra = len(tokeniser.prompt_layout()["prefix"]) + 1 if hasattr(tokeniser, "prompt_layout") else 1
+    return tokeniser.model.frames(max(longest, 1)) + extra + new
 
 
 def run_generate(cfg, tokeniser, device: str) -> dict:
@@ -150,6 +152,9 @@ def run_generate(cfg, tokeniser, device: str) -> dict:
     n_ret = int(m.get("generate_kwargs", {}).get("num_return_sequences", None) or 1)
     vocoder = vocoder_b200_from_cfg(cfg.vocoder, device=device, max_rows=cfg.batch_size * n_ret)
     model = B200SpeechLM(load_model(cfg, device, max_seq=generate_max_seq(cfg, tokeniser, ds)), tokeniser, vocoder=vocoder)
+    if len(tokeniser) > model.model.config.vocab_size:
+        raise ValueError(f"the tokeniser has {len(tokeniser)} ids but the model's vocabulary is "
+                         f"{model.model.config.vocab_size}")
     res = M.generate(model, path, cfg.batch_size, m.get("used_token_modality", None), m.prompt_length,
                      m.get("min_file_length", None), m.get("alignment_folder", None), m.get("use_alignment", False),
                      tokeniser.fe_sample_rate, m.num_files, cfg.num_workers, cfg.pin_memory, **m.get("generate_kwargs", {}))

@@ -467,6 +467,20 @@ int sk_lm_prefill(SkLm* lm, const int64_t* ids, const int32_t* lens, int B, int 
  * RMSNorm -> SwiGLU GEMM -> down-proj + residual; final norm, head -> logits [B, ldl]. */
 int sk_lm_decode_step(SkLm* lm, const int64_t* tokens, const int32_t* pos, int B, void* kv_cache, int T_cache,
                       void* logits, int ldl, void* decode_ws, int64_t decode_ws_bytes, void* stream);
+/* Decoding restricted to n allowed ids (generate's allowed_token_ids): the compact head is rows ids[0 .. n) of the
+ * handle's head (the token table when tied, else lm_head / embed_out; post-LN OPT with project_out: the proj_dim-wide
+ * table) gathered into head bf16 [n_pad, head width], rows n .. n_pad - 1 zero; n_pad a multiple of 64 <= the padded
+ * vocabulary.  ids int32, ascending, in [0, vocab).  Run once per generate call (not per step). */
+int sk_lm_gather_head(const SkLm* lm, const int32_t* ids, int n, int n_pad, void* head, void* stream);
+/* sk_lm_prefill / sk_lm_decode_step with the final GEMM on the compact head: logits [B, ld_sub] (ld_sub >= n_pad, a
+ * multiple of 8), column c = the logit of ids[c], bit-identical to that id's column of the full-vocabulary call (the
+ * same whole-tile GEMM, same K order per element).  Every other launch is the full call's.  bf16 handles only. */
+int sk_lm_prefill_sub(SkLm* lm, const int64_t* ids, const int32_t* lens, int B, int T, void* kv_cache, int T_cache,
+                      const void* head, int n_pad, void* logits, int ld_sub, void* decode_ws, int64_t decode_ws_bytes,
+                      void* stream);
+int sk_lm_decode_step_sub(SkLm* lm, const int64_t* tokens, const int32_t* pos, int B, void* kv_cache, int T_cache,
+                          const void* head, int n_pad, void* logits, int ld_sub, void* decode_ws, int64_t decode_ws_bytes,
+                          void* stream);
 /* Prompt fan-out for num_return_sequences: copies positions t < lens[b] of every layer's K and V of row b of src_cache
  * (B rows) into rows b*k .. b*k + k - 1 of dst_cache (B*k rows), both with the same T_cache and the handle's layout
  * ([L][K|V][rows][KVH][T_cache][head_dim], bf16, or fp32 on fp32 inference handles).  Positions >= lens[b] of the
@@ -518,6 +532,11 @@ int sk_select_next(const void* logits, int ldl, int V, int B, const uint32_t* ba
                    const float* uniforms, const SkDecodeState* state, void* stream);
 /* sk_select_next on fp32 logits [B, ldl] (fp32 inference handles); logits 16-byte aligned. */
 int sk_select_next_f32(const float* logits, int ldl, int V, int B, const uint32_t* ban_bits, const SkSampling* cfg,
+                       const float* uniforms, const SkDecodeState* state, void* stream);
+/* sk_select_next over compact bf16 logits [B, ld_sub]: column c is token ids[c] (int32 [n], ascending, in [0, V)) and
+ * every other id of the V-token vocabulary is banned.  Picks the token sk_select_next picks on the full logits with the
+ * complement in ban_bits (the same per-thread sums and tie breaks); writes the token id, not the column. */
+int sk_select_next_sub(const void* logits, int ld_sub, const int32_t* ids, int n, int V, int B, const SkSampling* cfg,
                        const float* uniforms, const SkDecodeState* state, void* stream);
 /* History-dependent logits processors (HF GenerationConfig repetition_penalty, no_repeat_ngram_size, min_new_tokens /
  * min_length).  Row b's history is history[b, 0 .. prompt_len + step): the padded prompt exactly as the caller passed
@@ -572,6 +591,13 @@ int sk_seq_loglik_f32(const float* logits, int ldl, int V, const int64_t* ids, i
  * T_out = max(counts) + 2 gives the batch tokenise() builds. */
 int sk_units_to_tokens(const int32_t* units, const int32_t* counts, int B, int T_units, int offset, int bos, int eos, int pad,
                        int64_t* ids, int T_out, void* stream);
+/* InterleavingTokeniser.build_prompt (SPEECH output) on the device, left-padded: row b of ids int64 [B, T_out] is
+ * [pad..., prefix[0 .. n_prefix), unit_id[units[b, j]] for j < counts[b], marker] and mask int64 [B, T_out] is 0 on the
+ * pads, 1 elsewhere.  unit_id int32 [n_units] (device) maps unit u to the id of `<Un u>`; prefix int32 (device) holds what
+ * the text tokenizer puts before a string.  T_out >= n_prefix + max(counts) + 1. */
+int sk_units_to_prompt(const int32_t* units, const int32_t* counts, int B, int T_units, const int32_t* unit_id, int n_units,
+                       const int32_t* prefix, int n_prefix, int marker, int pad, int64_t* ids, int64_t* mask, int T_out,
+                       void* stream);
 /* ---- HuBERT unit extraction (path (i)) ------------------------------------------------------------------------------
  * One object per device; replaces HubertFeatureExtractor.extract + batch_cluster
  * (slamkit/feature_extractor/hubert_feature_extractor.py:40-50,73-81): F.pad(40,40) -> HF HubertModel conv encoder,

@@ -325,6 +325,17 @@ SK_DEVINL T block_exclusive_scan(T v, T* red, T& total) {
 SK_DEVINL float logit_at(const bf16* row, int i) { return __bfloat162float(row[i]); }
 SK_DEVINL float logit_at(const float* row, int i) { return row[i]; }
 
+// first index of the ascending a[0, n) whose value is >= x (n if none)
+SK_DEVINL int lower_bound_i32(const int32_t* a, int n, int x) {
+  int lo = 0, hi = n;
+  while (lo < hi) {
+    const int mid = (lo + hi) >> 1;
+    if (a[mid] < x) lo = mid + 1;
+    else hi = mid;
+  }
+  return lo;
+}
+
 SK_DEVINL bool bit_set(const uint32_t* bits, int i) { return (bits[i >> 5] >> (i & 31)) & 1u; }
 
 // RULES: the SkLogitRules processors of one row.  `dyn` holds this step's n-gram and min-length bans (NULL when there
@@ -392,12 +403,14 @@ SK_DEVINL const uint32_t* rules_bans(const SkLogitRules& r, const SkSampling& cf
 // greedy = argmax of the banned scores, lowest id on ties.  Each thread owns the contiguous id range
 // [tid * chunk, (tid + 1) * chunk), so per-thread partial sums are in token order and every sum is taken in a fixed order.
 // LT: bf16 logits, or fp32 ones (fp32 OPT inference).  RULES: apply `rules` (sk_select_next_ex) and append to the
-// history; without, `rules` is not read.
-template <typename LT, bool RULES>
-__global__ void __launch_bounds__(SEL_THREADS) select_next_kernel(const LT* __restrict__ logits, int ldl, int V,
-                                                                  const uint32_t* __restrict__ ban, SkSampling cfg,
-                                                                  const float* __restrict__ uniforms, SkDecodeState st,
-                                                                  SkLogitRules rules) {
+// history; without, `rules` is not read.  SUB (sk_select_next_sub): column c of the logits is token sub_ids[c] (ascending)
+// and every other id is banned.  A thread then owns the columns whose ids fall in its id range, so each partial sum, scan
+// and tie break sees the same values in the same order as the full-vocabulary kernel with those ids banned, and picks
+// the same token.
+template <typename LT, bool RULES, bool SUB>
+SK_DEVINL void select_next_row(const LT* __restrict__ logits, int ldl, int V, const uint32_t* __restrict__ ban,
+                               const SkSampling& cfg, const float* __restrict__ uniforms, const SkDecodeState& st,
+                               const SkLogitRules& rules, const int32_t* __restrict__ sub_ids, int n_sub) {
   __shared__ float red_f[SEL_WARPS];
   __shared__ int red_i[SEL_WARPS];
   __shared__ unsigned long long red_u[SEL_WARPS];
@@ -429,6 +442,13 @@ __global__ void __launch_bounds__(SEL_THREADS) select_next_kernel(const LT* __re
   }
   const int chunk = (V + SEL_THREADS - 1) / SEL_THREADS;
   const int i0 = min(tid * chunk, V), i1 = min(i0 + chunk, V);
+  // the thread's columns [c0, c1) and the id of a column
+  int c0 = i0, c1 = i1;
+  if constexpr (SUB) {
+    c0 = lower_bound_i32(sub_ids, n_sub, i0);
+    c1 = lower_bound_i32(sub_ids, n_sub, i1);
+  }
+  const int n_cols = SUB ? n_sub : V;
   SelRow<LT, RULES> R{logits + (size_t)b * ldl, ban, cfg.temperature, cfg.do_sample != 0 && cfg.temperature != 1.0f,
                       nullptr, nullptr, 1.f};
   if constexpr (RULES) {
@@ -443,8 +463,9 @@ __global__ void __launch_bounds__(SEL_THREADS) select_next_kernel(const LT* __re
     // argmax, lowest id among equal maxima
     float bv = -INFINITY;
     int bi = 0x7fffffff;
-    for (int i = i0; i < i1; ++i) {
-      const float v = R.score(i);
+    for (int c = c0; c < c1; ++c) {
+      const float v = R.score(c);
+      const int i = (SUB ? (int)sub_ids[c] : c);
       if (v > bv || (v == bv && i < bi)) { bv = v; bi = i; }
     }
     // pack (ordered value, inverted id) so that one max picks the largest value, then the smallest id
@@ -454,16 +475,17 @@ __global__ void __launch_bounds__(SEL_THREADS) select_next_kernel(const LT* __re
     if (tok >= V) tok = 0;
   } else {
     // top-k: the k-th largest score by radix select on order-preserving keys (HF keeps every score >= it)
-    const int k = cfg.top_k > 0 ? min(cfg.top_k, V) : V;
+    // (SUB: with k >= n_sub the full kernel's k-th score is a banned -inf, which keeps every allowed id, as kth = 0 does)
+    const int k = cfg.top_k > 0 ? min(cfg.top_k, n_cols) : n_cols;
     uint32_t kth = 0;
-    if (k < V) {
+    if (k < n_cols) {
       uint32_t prefix = 0, mask = 0;
       int rank = k;
       for (int shift = 24; shift >= 0; shift -= 8) {
         for (int i = tid; i < 256; i += SEL_THREADS) hist[i] = 0;
         __syncthreads();
-        for (int i = i0; i < i1; ++i) {
-          const uint32_t key = ordered_key(R.score(i));
+        for (int c = c0; c < c1; ++c) {
+          const uint32_t key = ordered_key(R.score(c));
           if ((key & mask) == prefix) atomicAdd(&hist[(key >> shift) & 255u], 1);
         }
         __syncthreads();
@@ -487,8 +509,8 @@ __global__ void __launch_bounds__(SEL_THREADS) select_next_kernel(const LT* __re
     }
     // softmax over the kept scores
     float mx = -INFINITY;
-    for (int i = i0; i < i1; ++i) {
-      const float v = R.score(i);
+    for (int c = c0; c < c1; ++c) {
+      const float v = R.score(c);
       if (ordered_key(v) >= kth) mx = fmaxf(mx, v);
     }
     mx = block_reduce(mx, red_f, [](float a, float c) { return fmaxf(a, c); });
@@ -501,16 +523,16 @@ __global__ void __launch_bounds__(SEL_THREADS) select_next_kernel(const LT* __re
     if (cfg.top_p < 1.0) {
       const float thr = (float)(1.0 - cfg.top_p);
       float z = 0.f;
-      for (int i = i0; i < i1; ++i) {
-        const float v = R.score(i);
+      for (int c = c0; c < c1; ++c) {
+        const float v = R.score(c);
         if (ordered_key(v) >= kth) z += expf(v - mx);
       }
       float ztot;
       block_exclusive_scan(z, red_f, ztot);
       auto mass_le = [&](uint32_t K) {
         float m = 0.f;
-        for (int i = i0; i < i1; ++i) {
-          const float v = R.score(i);
+        for (int c = c0; c < c1; ++c) {
+          const float v = R.score(c);
           const uint32_t key = ordered_key(v);
           if (key >= kth && key <= K) m += expf(v - mx);
         }
@@ -528,8 +550,8 @@ __global__ void __launch_bounds__(SEL_THREADS) select_next_kernel(const LT* __re
       // the tie group at K*: count, and the mass strictly below it
       int cnt = 0, first_in_chunk = 0;
       float q = 0.f;
-      for (int i = i0; i < i1; ++i) {
-        const float v = R.score(i);
+      for (int c = c0; c < c1; ++c) {
+        const float v = R.score(c);
         if (ordered_key(v) == cut_key) { ++cnt; q = expf(v - mx); }
       }
       int cnt_tot;
@@ -543,8 +565,8 @@ __global__ void __launch_bounds__(SEL_THREADS) select_next_kernel(const LT* __re
         // id of the drop-th member of the group (1-based) in id order
         int id = -1, seen = first_in_chunk;
         if (seen < drop && seen + cnt >= drop) {
-          for (int i = i0; i < i1; ++i) {
-            if (ordered_key(R.score(i)) == cut_key && ++seen == drop) { id = i; break; }
+          for (int c = c0; c < c1; ++c) {
+            if (ordered_key(R.score(c)) == cut_key && ++seen == drop) { id = (SUB ? (int)sub_ids[c] : c); break; }
           }
         }
         cut_id = block_reduce(id, red_i, [](int a, int c) { return a > c ? a : c; });
@@ -565,8 +587,9 @@ __global__ void __launch_bounds__(SEL_THREADS) select_next_kernel(const LT* __re
     }
     float e = 0.f;
     int last = -1;
-    for (int i = i0; i < i1; ++i) {
-      const float v = R.score(i);
+    for (int c = c0; c < c1; ++c) {
+      const float v = R.score(c);
+      const int i = (SUB ? (int)sub_ids[c] : c);
       if (kept(i, v)) { e += expf(v - mx); last = i; }
     }
     float etot;
@@ -577,8 +600,9 @@ __global__ void __launch_bounds__(SEL_THREADS) select_next_kernel(const LT* __re
     __syncthreads();
     if (e > 0.f && before <= target && target < before + e) {
       float run = before;
-      for (int i = i0; i < i1; ++i) {
-        const float v = R.score(i);
+      for (int c = c0; c < c1; ++c) {
+        const float v = R.score(c);
+        const int i = (SUB ? (int)sub_ids[c] : c);
         if (kept(i, v)) {
           run += expf(v - mx);
           if (run > target) { atomicMin(&s_tok, i); break; }
@@ -600,6 +624,20 @@ __global__ void __launch_bounds__(SEL_THREADS) select_next_kernel(const LT* __re
   }
 }
 
+template <typename LT, bool RULES>
+__global__ void __launch_bounds__(SEL_THREADS) select_next_kernel(const LT* __restrict__ logits, int ldl, int V,
+                                                                  const uint32_t* __restrict__ ban, SkSampling cfg,
+                                                                  const float* __restrict__ uniforms, SkDecodeState st,
+                                                                  SkLogitRules rules) {
+  select_next_row<LT, RULES, false>(logits, ldl, V, ban, cfg, uniforms, st, rules, nullptr, 0);
+}
+__global__ void __launch_bounds__(SEL_THREADS) select_next_sub_kernel(const bf16* __restrict__ logits, int ld_sub, int V,
+                                                                         SkSampling cfg, const float* __restrict__ uniforms,
+                                                                         SkDecodeState st, const int32_t* __restrict__ ids,
+                                                                         int n) {
+  select_next_row<bf16, false, true>(logits, ld_sub, V, nullptr, cfg, uniforms, st, SkLogitRules{}, ids, n);
+}
+
 // presence[b] = bitmap of history[b, 0 .. T).  grid B
 __global__ void presence_init_kernel(const int64_t* __restrict__ history, int hist_ld, int T, int V,
                                      uint32_t* __restrict__ presence) {
@@ -612,6 +650,18 @@ __global__ void presence_init_kernel(const int64_t* __restrict__ history, int hi
     const int64_t id = history[(size_t)b * hist_ld + t];
     if (id >= 0 && id < V) atomicOr(&p[id >> 5], 1u << (id & 31));
   }
+}
+
+// compact head: row r < n of dst [n_pad, K] is row ids[r] of src [V, K] (zeros for an id outside [0, V)), rows
+// n .. n_pad - 1 are zeros.  grid n_pad
+__global__ void gather_rows_kernel(const bf16* __restrict__ src, const int32_t* __restrict__ ids, int n, int V, int K,
+                                   bf16* __restrict__ dst) {
+  const int r = blockIdx.x;
+  const int id = r < n ? ids[r] : -1;
+  const bool ok = id >= 0 && id < V;
+  const uint4* s = reinterpret_cast<const uint4*>(src + (size_t)(ok ? id : 0) * K);
+  uint4* d = reinterpret_cast<uint4*>(dst + (size_t)r * K);
+  for (int c = threadIdx.x; c < K / 8; c += blockDim.x) d[c] = ok ? s[c] : make_uint4(0u, 0u, 0u, 0u);
 }
 
 // prompt fan-out: the first lens[b] rows of the [T_cache][row_bytes] plane of (layer | K/V, row b, kv head) go to rows
@@ -749,6 +799,15 @@ int sk_select_next_launch(const bf16* logits, int ldl, int V, int B, const uint3
   return select_next<bf16>(logits, ldl, V, B, ban, cfg, uniforms, st, s);
 }
 
+int sk_gather_rows_launch(const bf16* src, const int32_t* ids, int n, int n_pad, int V, int K, bf16* dst, cudaStream_t s) {
+  SK_REQUIRE(src && ids && dst && n > 0 && n <= n_pad && K > 0 && K % 8 == 0, "gather_rows: bad arguments n=%d n_pad=%d K=%d",
+             n, n_pad, K);
+  SK_REQUIRE((((uintptr_t)src | (uintptr_t)dst) & 15) == 0, "gather_rows: rows must be 16-byte aligned");
+  gather_rows_kernel<<<n_pad, 128, 0, s>>>(src, ids, n, V, K, dst);
+  SK_LAUNCH_CHECK();
+  return 0;
+}
+
 extern "C" {
 
 int64_t sk_attn_decode_partial_bytes(int B, int H, int T_cache) {
@@ -790,6 +849,22 @@ int sk_select_next_ex_f32(const float* logits, int ldl, int V, int B, const uint
   SK_REQUIRE(logits && cfg && state && rules, "sk_select_next_ex_f32: null argument");
   SK_REQUIRE(((uintptr_t)logits & 15) == 0, "sk_select_next_ex_f32: logits must be 16-byte aligned");
   return select_next<float>(logits, ldl, V, B, ban_bits, *cfg, uniforms, *state, (cudaStream_t)stream, rules);
+}
+
+int sk_select_next_sub(const void* logits, int ld_sub, const int32_t* ids, int n, int V, int B, const SkSampling* cfg,
+                       const float* uniforms, const SkDecodeState* state, void* stream) {
+  SK_REQUIRE(logits && ids && cfg && state, "sk_select_next_sub: null argument");
+  SK_REQUIRE(B > 0 && n > 0 && n <= V && ld_sub >= n, "sk_select_next_sub: bad shape B=%d n=%d V=%d ld_sub=%d", B, n, V,
+             ld_sub);
+  SK_REQUIRE(cfg->n_eos >= 0 && cfg->n_eos <= 8, "sk_select_next_sub: at most 8 eos ids");
+  SK_REQUIRE(!cfg->do_sample || cfg->temperature > 0.f, "sk_select_next_sub: temperature must be > 0");
+  const SkDecodeState& st = *state;
+  SK_REQUIRE(st.tokens && st.pos && st.finished && st.n_gen && st.out && st.step && st.max_new > 0,
+             "sk_select_next_sub: incomplete decode state");
+  SK_CUDA_CHECK(sk_launch_pdl(select_next_sub_kernel, dim3(B), dim3(SEL_THREADS), (size_t)0, (cudaStream_t)stream,
+                              reinterpret_cast<const bf16*>(logits), ld_sub, V, *cfg, uniforms, st, ids, n));
+  SK_LAUNCH_CHECK();
+  return 0;
 }
 
 int sk_presence_init(const int64_t* history, int hist_ld, int prompt_len, int B, int V, uint32_t* presence, void* stream) {

@@ -290,6 +290,8 @@ int sk_kv_prefill_launch(const bf16* qkv, long layer_stride, int ldq, bf16* cach
 int sk_kv_append_launch(const bf16* qkv, int ldq, bf16* kc, bf16* vc, const int32_t* pos, int32_t* lens, int B, int H,
                         int KVH, int T_cache, cudaStream_t s);
 int sk_gather_last_launch(const bf16* x, const int32_t* lens, bf16* out, int B, int T, int D, cudaStream_t s);
+// rows ids[0 .. n) of src [V, K] into dst [n_pad, K], zero rows after them (the compact head of sk_lm_gather_head)
+int sk_gather_rows_launch(const bf16* src, const int32_t* ids, int n, int n_pad, int V, int K, bf16* dst, cudaStream_t s);
 // fp32 OPT inference: an fp32 cache ([K|V][B][H][T_cache][64] per layer) filled from the (hi, lo) projections of one layer,
 // decode attention with a (hi, lo) query and output
 int sk_kv_prefill_f32_launch(const bf16* qkv_hi, const bf16* qkv_lo, int ldq, float* cache, const int32_t* lens, int B, int T,

@@ -437,13 +437,14 @@ DecLayout make_dec_layout(const SkLm* lm, int B, int T_cache) {
   return w;
 }
 
-int check_decode(const SkLm* lm, int B, int T_cache, int ldl, const void* kv_cache, const void* logits, const void* ws,
-                 int64_t ws_bytes, const DecLayout& w) {
+// n_cols: the logits columns the head writes (Vp, or the compact head's rows)
+int check_decode(const SkLm* lm, int B, int T_cache, int ldl, int n_cols, const void* kv_cache, const void* logits,
+                 const void* ws, int64_t ws_bytes, const DecLayout& w) {
   SK_REQUIRE(lm->params && lm->ws, "sk_lm: sk_lm_bind has not been called");
   SK_REQUIRE(kv_cache && logits && ws, "sk_lm decode: null argument");
   SK_REQUIRE(B > 0 && T_cache > 0 && T_cache <= lm->max_pos, "sk_lm decode: bad shape B=%d T_cache=%d (max_positions=%d)",
              B, T_cache, lm->max_pos);
-  SK_REQUIRE(ldl >= lm->Vp && ldl % 8 == 0, "sk_lm decode: ldl must be >= %d and a multiple of 8 (got %d)", lm->Vp, ldl);
+  SK_REQUIRE(ldl >= n_cols && ldl % 8 == 0, "sk_lm decode: ldl must be >= %d and a multiple of 8 (got %d)", n_cols, ldl);
   SK_REQUIRE(((uintptr_t)ws & 255) == 0 && ((uintptr_t)kv_cache & 15) == 0 && ((uintptr_t)logits & 15) == 0,
              "sk_lm decode: decode workspace must be 256-byte, cache and logits 16-byte aligned");
   SK_REQUIRE(ws_bytes >= w.total, "sk_lm decode: decode workspace too small: need %lld bytes, got %lld", (long long)w.total,
@@ -459,6 +460,9 @@ struct DecBufs {
   float* e32;
   void* gemm;
   size_t gemm_bytes;
+  // compact head of sk_lm_prefill_sub / sk_lm_decode_step_sub: rows [head_n, head_k] (nullptr: the model's head)
+  const bf16* head = nullptr;
+  int head_n = 0;
 };
 
 DecBufs dec_bufs(void* ws, const DecLayout& dl) {
@@ -467,6 +471,14 @@ DecBufs dec_bufs(void* ws, const DecLayout& dl) {
   return DecBufs{b16(dl.x0), b16(dl.x1), b16(dl.h), b16(dl.qkv), b16(dl.ao), b16(dl.gu), b16(dl.act),
                  reinterpret_cast<int32_t*>(p + dl.lens), reinterpret_cast<float*>(p + dl.partial),
                  reinterpret_cast<float*>(p + dl.e32), p + dl.gemm, (size_t)dl.gemm_bytes};
+}
+
+// logits [B, ldl] of a bf16 decode step or prefill from the head input h [B, K]: the model's head, or the compact head.
+// The compact GEMM is the same whole-tile plan as the full head (no scratch: no split-K, no stream-K), so every logit
+// is the same K-ordered fp32 sum as the column of its id in the full step, only the tile width follows N.
+int dec_head(const SkLm* lm, const DecBufs& b, int B, int K, const bf16* h, void* logits, int ldl, cudaStream_t s) {
+  if (!b.head) return head_logits(lm, B, K, h, logits, ldl, s);
+  return sk_gemm_ex_launch(sk_gemm_linear(B, b.head_n, K, h, b.head, logits, ldl, nullptr, nullptr, SK_ACT_NONE), s);
 }
 
 // ---- OPT decoder (HF:models/opt/modeling_opt.py:45-70 positions, :100-182 attention, :185-260 decoder layer,
@@ -652,7 +664,7 @@ int neox_decode_step(SkLm* lm, const int64_t* tokens, const int32_t* pos, int B,
     SK_TRY(sk_gemm_ex_launch(sk_gemm_res2(B, d, F, act, P + o.w2, P + o.b2, attn, x, x, b.gemm, b.gemm_bytes), s));
   }
   SK_TRY(sk_layernorm_fwd_launch(x, P + lm->off_final_norm, P + lm->off_final_norm_b, h, nullptr, nullptr, B, d, eps, s));
-  return head_logits(lm, B, d, h, logits, ldl, s);
+  return dec_head(lm, b, B, d, h, logits, ldl, s);
 }
 
 // ---- OPT with fp32 master weights (sk_lm_set_master): HF OPTForCausalLM with fp32 parameters under
@@ -1058,7 +1070,7 @@ int opt_postln_decode_step(SkLm* lm, const int64_t* tokens, const int32_t* pos, 
     SK_TRY(linear_fwd(B, K, d, x, P + lm->off_pout, h, nullptr, nullptr, s));
     hin = h;
   }
-  return head_logits(lm, B, K, hin, logits, ldl, s);
+  return dec_head(lm, b, B, K, hin, logits, ldl, s);
 }
 
 // One token per row at position pos[b] (read on the device: the step is graph-capturable).  The KV cache layout is the
@@ -1093,7 +1105,7 @@ int opt_decode_step(SkLm* lm, const int64_t* tokens, const int32_t* pos, int B, 
     SK_TRY(linear_fwd(B, d, F, a, P + o.w2, x, P + o.b2, xm, s, SK_ACT_NONE, b.gemm, b.gemm_bytes));
   }
   SK_TRY(sk_layernorm_fwd_launch(x, P + lm->off_final_norm, P + lm->off_final_norm_b, h, nullptr, nullptr, B, d, eps, s));
-  return head_logits(lm, B, d, h, logits, ldl, s);
+  return dec_head(lm, b, B, d, h, logits, ldl, s);
 }
 
 // ---- OPT fp32 inference (sk_lm_set_fp32): HF OPTForCausalLM in fp32, as the reference scores and generates a float32
@@ -1371,7 +1383,7 @@ int qwen2_decode_step(SkLm* lm, const int64_t* tokens, const int32_t* pos, int B
     std::swap(x, xm);
   }
   SK_TRY(sk_rmsnorm_fwd_launch(x, P + lm->off_final_norm, h, nullptr, B, d, lm->eps, s));
-  return head_logits(lm, B, d, h, logits, ldl, s);
+  return dec_head(lm, b, B, d, h, logits, ldl, s);
 }
 
 // ---- the decoder variant: (fp32 inference) -> architecture -> (post-LN) -> (master weights), the only place that picks
@@ -1407,32 +1419,21 @@ int decode_step(SkLm* lm, const int64_t* tokens, const int32_t* pos, int B, void
   return opt_decode_step(lm, tokens, pos, B, kv_cache, T_cache, logits, ldl, b, s);
 }
 
-}  // namespace
-
-extern "C" {
-
-int64_t sk_lm_kv_cache_bytes(const SkLm* lm, int B, int T_cache) {
-  if (!lm || B <= 0 || T_cache <= 0) return 0;
-  return (int64_t)lm->L * 2 * B * lm->KVH * T_cache * lm->hd * (lm->fp32 ? 4 : 2);
-}
-
-int64_t sk_lm_decode_workspace_bytes(const SkLm* lm, int B, int T_cache) {
-  if (!lm || B <= 0 || T_cache <= 0) return 0;
-  return make_dec_layout(lm, B, T_cache).total;
-}
-
-int sk_lm_prefill(SkLm* lm, const int64_t* ids, const int32_t* lens, int B, int T, void* kv_cache, int T_cache,
-                  void* logits, int ldl, void* decode_ws, int64_t decode_ws_bytes, void* stream) {
-  SK_REQUIRE(lm && ids && lens, "sk_lm_prefill: null argument");
-  SK_REQUIRE(!lm->master, "sk_lm_prefill: this handle trains fp32 master weights (sk_lm_set_master); generate from its saved "
-                          "checkpoint with a handle that has no master weights");
+// sk_lm_prefill, or with head != nullptr sk_lm_prefill_sub (its caller has checked the compact head)
+int prefill(const char* who, SkLm* lm, const int64_t* ids, const int32_t* lens, int B, int T, void* kv_cache, int T_cache,
+            const bf16* head, int head_n, void* logits, int ldl, void* decode_ws, int64_t decode_ws_bytes, void* stream) {
+  SK_REQUIRE(lm && ids && lens, "%s: null argument", who);
+  SK_REQUIRE(!lm->master, "%s: this handle trains fp32 master weights (sk_lm_set_master); generate from its saved "
+                          "checkpoint with a handle that has no master weights", who);
   const DecLayout dl = make_dec_layout(lm, B, T_cache);
-  SK_TRY(check_decode(lm, B, T_cache, ldl, kv_cache, logits, decode_ws, decode_ws_bytes, dl));
-  SK_REQUIRE(T > 0 && T <= T_cache, "sk_lm_prefill: prompt width T=%d must be in [1, T_cache=%d]", T, T_cache);
+  SK_TRY(check_decode(lm, B, T_cache, ldl, head ? head_n : lm->Vp, kv_cache, logits, decode_ws, decode_ws_bytes, dl));
+  SK_REQUIRE(T > 0 && T <= T_cache, "%s: prompt width T=%d must be in [1, T_cache=%d]", who, T, T_cache);
   const WsLayout w = layout_of(lm, B, T);
   SK_TRY(check_bound(lm, B, T, w, nullptr));
   cudaStream_t s = (cudaStream_t)stream;
-  const DecBufs b = dec_bufs(decode_ws, dl);
+  DecBufs b = dec_bufs(decode_ws, dl);
+  b.head = head;
+  b.head_n = head_n;
   SK_CUDA_CHECK(cudaMemsetAsync(reinterpret_cast<uint8_t*>(b.gemm) + b.gemm_bytes - 4096, 0, 4096, s));
   FwdArgs a{ids, nullptr, nullptr, B, T};
   a.with_head = false;
@@ -1454,7 +1455,81 @@ int sk_lm_prefill(SkLm* lm, const int64_t* ids, const int32_t* lens, int B, int 
   SK_TRY(sk_kv_prefill_launch(wsp<bf16>(lm, w.qkv), w.sqkv / 2, lm->qkv_dim, reinterpret_cast<bf16*>(kv_cache), lens, lm->L, B,
                               T, lm->H, lm->KVH, T_cache, s));
   SK_TRY(sk_gather_last_launch(head_in(lm, w), lens, b.h, B, T, K, s));
-  return head_logits(lm, B, K, b.h, logits, ldl, s);
+  return dec_head(lm, b, B, K, b.h, logits, ldl, s);
+}
+
+// sk_lm_decode_step, or with head != nullptr sk_lm_decode_step_sub
+int decode(const char* who, SkLm* lm, const int64_t* tokens, const int32_t* pos, int B, void* kv_cache, int T_cache,
+           const bf16* head, int head_n, void* logits, int ldl, void* decode_ws, int64_t decode_ws_bytes, void* stream) {
+  SK_REQUIRE(lm && tokens && pos, "%s: null argument", who);
+  SK_REQUIRE(!lm->master, "%s: this handle trains fp32 master weights (sk_lm_set_master); generate from its "
+                          "saved checkpoint with a handle that has no master weights", who);
+  const DecLayout dl = make_dec_layout(lm, B, T_cache);
+  SK_TRY(check_decode(lm, B, T_cache, ldl, head ? head_n : lm->Vp, kv_cache, logits, decode_ws, decode_ws_bytes, dl));
+  DecBufs b = dec_bufs(decode_ws, dl);
+  b.head = head;
+  b.head_n = head_n;
+  return decode_step(lm, tokens, pos, B, kv_cache, T_cache, logits, ldl, b, (cudaStream_t)stream);
+}
+
+// the compact head of the _sub entry points: n_pad rows of head_k(lm) bf16 (sk_lm_gather_head), bf16 handles only
+int check_sub_head(const char* who, const SkLm* lm, const void* head, int n_pad) {
+  SK_REQUIRE(lm, "%s: null argument", who);
+  SK_REQUIRE(!lm->fp32, "%s: fp32 inference handles decode with the full head (sk_lm_decode_step)", who);
+  SK_REQUIRE(head && ((uintptr_t)head & 15) == 0, "%s: the compact head must be a 16-byte aligned device buffer", who);
+  SK_REQUIRE(n_pad > 0 && n_pad % 64 == 0 && n_pad <= lm->Vp, "%s: n_pad=%d must be a positive multiple of 64, at most %d",
+             who, n_pad, lm->Vp);
+  return 0;
+}
+
+}  // namespace
+
+extern "C" {
+
+int64_t sk_lm_kv_cache_bytes(const SkLm* lm, int B, int T_cache) {
+  if (!lm || B <= 0 || T_cache <= 0) return 0;
+  return (int64_t)lm->L * 2 * B * lm->KVH * T_cache * lm->hd * (lm->fp32 ? 4 : 2);
+}
+
+int64_t sk_lm_decode_workspace_bytes(const SkLm* lm, int B, int T_cache) {
+  if (!lm || B <= 0 || T_cache <= 0) return 0;
+  return make_dec_layout(lm, B, T_cache).total;
+}
+
+int sk_lm_prefill(SkLm* lm, const int64_t* ids, const int32_t* lens, int B, int T, void* kv_cache, int T_cache,
+                  void* logits, int ldl, void* decode_ws, int64_t decode_ws_bytes, void* stream) {
+  return prefill("sk_lm_prefill", lm, ids, lens, B, T, kv_cache, T_cache, nullptr, 0, logits, ldl, decode_ws,
+                 decode_ws_bytes, stream);
+}
+
+int sk_lm_prefill_sub(SkLm* lm, const int64_t* ids, const int32_t* lens, int B, int T, void* kv_cache, int T_cache,
+                      const void* head, int n_pad, void* logits, int ld_sub, void* decode_ws, int64_t decode_ws_bytes,
+                      void* stream) {
+  SK_TRY(check_sub_head("sk_lm_prefill_sub", lm, head, n_pad));
+  return prefill("sk_lm_prefill_sub", lm, ids, lens, B, T, kv_cache, T_cache, reinterpret_cast<const bf16*>(head), n_pad,
+                 logits, ld_sub, decode_ws, decode_ws_bytes, stream);
+}
+
+int sk_lm_decode_step(SkLm* lm, const int64_t* tokens, const int32_t* pos, int B, void* kv_cache, int T_cache,
+                      void* logits, int ldl, void* decode_ws, int64_t decode_ws_bytes, void* stream) {
+  return decode("sk_lm_decode_step", lm, tokens, pos, B, kv_cache, T_cache, nullptr, 0, logits, ldl, decode_ws,
+                decode_ws_bytes, stream);
+}
+
+int sk_lm_decode_step_sub(SkLm* lm, const int64_t* tokens, const int32_t* pos, int B, void* kv_cache, int T_cache,
+                          const void* head, int n_pad, void* logits, int ld_sub, void* decode_ws, int64_t decode_ws_bytes,
+                          void* stream) {
+  SK_TRY(check_sub_head("sk_lm_decode_step_sub", lm, head, n_pad));
+  return decode("sk_lm_decode_step_sub", lm, tokens, pos, B, kv_cache, T_cache, reinterpret_cast<const bf16*>(head), n_pad,
+                logits, ld_sub, decode_ws, decode_ws_bytes, stream);
+}
+
+int sk_lm_gather_head(const SkLm* lm, const int32_t* ids, int n, int n_pad, void* head, void* stream) {
+  SK_TRY(check_sub_head("sk_lm_gather_head", lm, head, n_pad));
+  SK_REQUIRE(ids && n > 0 && n <= n_pad, "sk_lm_gather_head: need 1 <= n=%d <= n_pad=%d ids", n, n_pad);
+  SK_REQUIRE(lm->params, "sk_lm: sk_lm_bind has not been called");
+  return sk_gather_rows_launch(lm->params + lm->off_head, ids, n, n_pad, lm->V, head_k(lm), reinterpret_cast<bf16*>(head),
+                               (cudaStream_t)stream);
 }
 
 int sk_lm_kv_fanout(const SkLm* lm, const void* src_cache, int B, int k, void* dst_cache, int T_cache, const int32_t* lens,
@@ -1462,16 +1537,6 @@ int sk_lm_kv_fanout(const SkLm* lm, const void* src_cache, int B, int k, void* d
   SK_REQUIRE(lm && src_cache && dst_cache && lens, "sk_lm_kv_fanout: null argument");
   return sk_kv_fanout_launch(src_cache, dst_cache, lens, lm->L, B, k, lm->KVH, T_cache, lm->hd * (lm->fp32 ? 4 : 2),
                              (cudaStream_t)stream);
-}
-
-int sk_lm_decode_step(SkLm* lm, const int64_t* tokens, const int32_t* pos, int B, void* kv_cache, int T_cache,
-                      void* logits, int ldl, void* decode_ws, int64_t decode_ws_bytes, void* stream) {
-  SK_REQUIRE(lm && tokens && pos, "sk_lm_decode_step: null argument");
-  SK_REQUIRE(!lm->master, "sk_lm_decode_step: this handle trains fp32 master weights (sk_lm_set_master); generate from its "
-                          "saved checkpoint with a handle that has no master weights");
-  const DecLayout dl = make_dec_layout(lm, B, T_cache);
-  SK_TRY(check_decode(lm, B, T_cache, ldl, kv_cache, logits, decode_ws, decode_ws_bytes, dl));
-  return decode_step(lm, tokens, pos, B, kv_cache, T_cache, logits, ldl, dec_bufs(decode_ws, dl), (cudaStream_t)stream);
 }
 
 int sk_lm_create(const SkLmConfig* cfg, SkLm** out) {

@@ -221,6 +221,29 @@ __global__ void units_to_tokens_kernel(const int32_t* __restrict__ units, const 
   ids[i] = v;
 }
 
+// left-padded generation prompt of the interleaved tokeniser: row b = [pad..., prefix..., unit_id[u]..., marker] with the
+// attention mask 0 on the pads, 1 elsewhere.  A unit outside [0, n_units) becomes pad (it has no id).
+__global__ void units_to_prompt_kernel(const int32_t* __restrict__ units, const int32_t* __restrict__ counts, int B,
+                                       int T_units, const int32_t* __restrict__ unit_id, int n_units,
+                                       const int32_t* __restrict__ prefix, int n_prefix, int marker, int pad,
+                                       int64_t* __restrict__ ids, int64_t* __restrict__ mask, int T_out) {
+  const long i = (long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= (long)B * T_out) return;
+  const int b = (int)(i / T_out), t = (int)(i % T_out);
+  const int n = min(max(counts[b], 0), T_units);
+  const int start = T_out - (n_prefix + n + 1);
+  const int j = t - start;
+  long v;
+  if (j < 0) v = pad;
+  else if (j < n_prefix) v = prefix[j];
+  else if (j < n_prefix + n) {
+    const int u = units[(size_t)b * T_units + j - n_prefix];
+    v = u >= 0 && u < n_units ? unit_id[u] : pad;
+  } else v = marker;
+  ids[i] = v;
+  mask[i] = j >= 0 ? 1 : 0;
+}
+
 // LT: logits element type; OT: ll_out element type; ROUND: the bf16 model's roundings
 template <typename LT, typename OT, bool ROUND>
 int seq_loglik(const char* who, const void* logits, int ldl, int V, const int64_t* ids, int B, int T, int pad_id,
@@ -273,6 +296,21 @@ int sk_units_to_tokens(const int32_t* units, const int32_t* counts, int B, int T
   const long n = (long)B * T_out;
   units_to_tokens_kernel<<<(unsigned)((n + 255) / 256), 256, 0, (cudaStream_t)stream>>>(units, counts, B, T_units, offset, bos,
                                                                                           eos, pad, ids, T_out);
+  SK_LAUNCH_CHECK();
+  return 0;
+}
+
+int sk_units_to_prompt(const int32_t* units, const int32_t* counts, int B, int T_units, const int32_t* unit_id, int n_units,
+                       const int32_t* prefix, int n_prefix, int marker, int pad, int64_t* ids, int64_t* mask, int T_out,
+                       void* stream) {
+  SK_REQUIRE(units && counts && unit_id && ids && mask && (prefix || n_prefix == 0), "sk_units_to_prompt: null argument");
+  SK_REQUIRE(B > 0 && T_units >= 0 && n_units > 0 && n_prefix >= 0 && T_out >= n_prefix + 1,
+             "sk_units_to_prompt: bad shape B=%d T_units=%d n_units=%d n_prefix=%d T_out=%d", B, T_units, n_units, n_prefix,
+             T_out);
+  SK_REQUIRE((long)B * T_out < (1L << 31), "sk_units_to_prompt: B*T_out too large");
+  const long n = (long)B * T_out;
+  units_to_prompt_kernel<<<(unsigned)((n + 255) / 256), 256, 0, (cudaStream_t)stream>>>(
+      units, counts, B, T_units, unit_id, n_units, prefix, n_prefix, marker, pad, ids, mask, T_out);
   SK_LAUNCH_CHECK();
   return 0;
 }

@@ -838,7 +838,13 @@ class B200UnitLM:
         Prompt plus continuation is bounded by `max_positions`.  `repetition_penalty`, `no_repeat_ngram_size` and
         `min_length` / `min_new_tokens` run inside the selection kernel on a device copy of each row's history;
         `num_return_sequences = k` prefills each prompt once and copies its KV cache to k rows (output [B*k, ...],
-        rows of one prompt adjacent, as HF orders them)."""
+        rows of one prompt adjacent, as HF orders them).
+
+        `allowed_token_ids = A` restricts every step to the ids in A: the result is that of
+        `bad_words_ids=[[i] for i not in A]`.  The decode steps then run the head GEMM on the rows of A only and select
+        over those columns (`sk_lm_decode_step_sub`, `sk_select_next_sub`); with history rules (repetition_penalty,
+        no_repeat_ngram_size, min_length / min_new_tokens) or on an fp32 inference handle they ban the complement on the
+        full vocabulary instead."""
         if self.master:
             raise NotImplementedError("generate: this model trains fp32 master weights; generate from its saved checkpoint "
                                       "(B200UnitLM.from_pretrained without master_weights)")
@@ -849,7 +855,7 @@ class B200UnitLM:
             raise ValueError("generate: no prompt (inputs / input_ids)")
         keys = ("max_new_tokens", "max_length", "do_sample", "temperature", "top_k", "top_p", "eos_token_id", "pad_token_id",
                 "bad_words_ids", "repetition_penalty", "no_repeat_ngram_size", "min_length", "min_new_tokens",
-                "num_return_sequences")
+                "num_return_sequences", "allowed_token_ids")
         opts = {}
         if generation_config is not None:
             for k in keys:
@@ -869,19 +875,39 @@ class B200UnitLM:
         if unknown:
             raise NotImplementedError(f"generate: unsupported arguments {unknown} (greedy / sampling with temperature, top_k, "
                                       "top_p, bad_words_ids, repetition_penalty, no_repeat_ngram_size, min_length, "
-                                      "min_new_tokens, num_return_sequences, eos / pad ids and length limits are "
-                                      "implemented)")
+                                      "min_new_tokens, num_return_sequences, allowed_token_ids, eos / pad ids and "
+                                      "length limits are implemented)")
         opts.setdefault("eos_token_id", getattr(self.config, "eos_token_id", 1))      # UnitTokeniser: bos = eos = 1
         opts.setdefault("pad_token_id", self.config.pad_token_id)
         if opts.get("do_sample") and "top_k" not in opts:
             opts["top_k"] = 50                                    # transformers' GenerationConfig default
         return self._generate_cached(inputs, attention_mask, generator=generator, **opts)
 
+    def _allowed_ids(self, allowed_token_ids, with_bans: bool) -> Optional[torch.Tensor]:
+        """allowed_token_ids as ascending int64 ids, after the checks generate makes (None when not given)."""
+        if allowed_token_ids is None:
+            return None
+        if with_bans:
+            raise ValueError("generate: pass allowed_token_ids or bad_words_ids, not both")
+        ids = torch.as_tensor(allowed_token_ids).reshape(-1)
+        if ids.numel() == 0:
+            raise ValueError("generate: allowed_token_ids is empty")
+        if ids.is_floating_point() or ids.dtype == torch.bool:
+            raise ValueError("generate: allowed_token_ids must be integer token ids")
+        ids = ids.to("cpu", torch.long)
+        V = self.config.vocab_size
+        if bool(((ids < 0) | (ids >= V)).any()):
+            raise ValueError(f"generate: allowed_token_ids must be in [0, {V})")
+        ids = ids.sort().values
+        if bool((ids[1:] == ids[:-1]).any()):
+            raise ValueError("generate: allowed_token_ids has duplicate ids")
+        return ids
+
     def _generate_cached(self, inputs: torch.Tensor, attention_mask: Optional[torch.Tensor], max_new_tokens=None,
                          max_length=None, do_sample=False, temperature=None, top_k=None, top_p=None, eos_token_id=None,
                          pad_token_id=None, bad_words_ids=None, generator=None, repetition_penalty=None,
                          no_repeat_ngram_size=None, min_length=None, min_new_tokens=None,
-                         num_return_sequences=None) -> torch.Tensor:
+                         num_return_sequences=None, allowed_token_ids=None) -> torch.Tensor:
         from .generation import _single_token_bans, ban_bitmask, min_step
         if inputs.dim() != 2:
             raise ValueError("generate: inputs must be [batch, time]")
@@ -909,6 +935,7 @@ class B200UnitLM:
             pad_token_id = min(eos)                                   # HF: "Setting pad_token_id to eos_token_id"
         fill = int(pad_token_id) if pad_token_id is not None else 0
         banned = _single_token_bans(bad_words_ids)
+        allowed = self._allowed_ids(allowed_token_ids, bool(banned))
         lens = torch.full((B,), T, dtype=torch.long)
         if attention_mask is not None:
             m = attention_mask.to("cpu").bool()
@@ -919,6 +946,9 @@ class B200UnitLM:
         bound = min_step(T, min_length, min_new_tokens) if eos else 0
         rules = penalty != 1.0 or ngram > 0 or bound > 0
         V = self.config.vocab_size
+        if allowed is not None and (rules or self.fp32):
+            keep = set(allowed.tolist())                 # the same result through the full-vocabulary ban bitmask
+            banned, allowed = [i for i in range(V) if i not in keep], None
         if rules and B and bool(((inputs < 0) | (inputs >= V)).any()):
             raise ValueError(f"generate: repetition_penalty / no_repeat_ngram_size read every prompt id, pads included; "
                              f"all must be in [0, {V})")
@@ -947,7 +977,7 @@ class B200UnitLM:
             cfg.eos[i] = e
         if do_sample and cfg.temperature <= 0:
             raise ValueError("temperature must be > 0")
-        sess = DecodeSession(self, B * k, T_cache, max_new_tokens, fill)
+        sess = DecodeSession(self, B * k, T_cache, max_new_tokens, fill, allowed)
         if rules:
             sess.set_rules(inputs.repeat_interleave(k, dim=0), penalty, ngram, bound)
         ban = ban_bitmask(banned, V).to(self.device) if banned else None
@@ -990,10 +1020,20 @@ class DecodeSession:
     current stream.  `step` and `select` take the same arguments every call, so they can be captured in a CUDA graph.
     After `set_rules`, `select` runs `sk_select_next_ex` over the rows' device history instead."""
 
-    def __init__(self, model: B200UnitLM, B: int, T_cache: int, max_new: int, pad_token_id: int = 0):
+    def __init__(self, model: B200UnitLM, B: int, T_cache: int, max_new: int, pad_token_id: int = 0,
+                 allowed: Optional[torch.Tensor] = None):
         self.m, self.B, self.T_cache = model, B, T_cache
         lib, h, dev = model.lib, model._h, model.device
         self.ldl = model.vocab_padded
+        # allowed ids (ascending): the head is gathered once into `head` [n_pad, width] and the logits are [B, n_pad]
+        self.sub_ids, self.head = None, None
+        if allowed is not None:
+            n = int(allowed.numel())
+            self.ldl = (n + 63) // 64 * 64
+            self.sub_ids = allowed.to(dev, torch.int32)
+            width = model.tensors.get("lm_head", model.tensors["embed"])[2]
+            self.head = torch.empty(self.ldl, width, device=dev, dtype=torch.bfloat16)
+            L.check(lib.sk_lm_gather_head(h, L.ptr(self.sub_ids), n, self.ldl, L.ptr(self.head), L.stream_ptr()))
         self.kv = torch.empty(int(lib.sk_lm_kv_cache_bytes(h, B, T_cache)), device=dev, dtype=torch.uint8)
         self.ws = torch.empty(int(lib.sk_lm_decode_workspace_bytes(h, B, T_cache)), device=dev, dtype=torch.uint8)
         self.logits_buf = torch.empty(B, self.ldl, device=dev, dtype=torch.float32 if model.fp32 else torch.bfloat16)
@@ -1024,7 +1064,10 @@ class DecodeSession:
 
     @property
     def logits(self) -> torch.Tensor:
-        """[B, vocab_size] logits of the last prefill / decode step (bf16; fp32 with fp32 inference)."""
+        """[B, vocab_size] logits of the last prefill / decode step (bf16; fp32 with fp32 inference); with allowed ids,
+        [B, n]: column c is the logit of sub_ids[c]."""
+        if self.sub_ids is not None:
+            return self.logits_buf[:, :self.sub_ids.numel()]
         return self.logits_buf[:, :self.m.config.vocab_size]
 
     def prefill(self, ids: torch.Tensor, lens: torch.Tensor, k: int = 1) -> torch.Tensor:
@@ -1042,9 +1085,14 @@ class DecodeSession:
         tok = ids_d.gather(1, (lens_d.long() - 1).clamp(min=0)[:, None])[:, 0]
         kv = self.kv if k == 1 else torch.empty(int(m.lib.sk_lm_kv_cache_bytes(m._h, B, self.T_cache)), device=m.device,
                                                 dtype=torch.uint8)
-        L.check(m.lib.sk_lm_prefill(m._h, L.ptr(ids_d), L.ptr(lens_d), B, T, L.ptr(kv), self.T_cache,
-                                    L.ptr(self.logits_buf), self.ldl, L.ptr(self.ws), C.c_int64(self.ws.numel()),
-                                    L.stream_ptr()))
+        if self.head is None:
+            L.check(m.lib.sk_lm_prefill(m._h, L.ptr(ids_d), L.ptr(lens_d), B, T, L.ptr(kv), self.T_cache,
+                                        L.ptr(self.logits_buf), self.ldl, L.ptr(self.ws), C.c_int64(self.ws.numel()),
+                                        L.stream_ptr()))
+        else:
+            L.check(m.lib.sk_lm_prefill_sub(m._h, L.ptr(ids_d), L.ptr(lens_d), B, T, L.ptr(kv), self.T_cache,
+                                            L.ptr(self.head), self.ldl, L.ptr(self.logits_buf), self.ldl, L.ptr(self.ws),
+                                            C.c_int64(self.ws.numel()), L.stream_ptr()))
         if k > 1:
             L.check(m.lib.sk_lm_kv_fanout(m._h, L.ptr(kv), B, k, L.ptr(self.kv), self.T_cache, L.ptr(lens_d),
                                           L.stream_ptr()))
@@ -1062,13 +1110,25 @@ class DecodeSession:
         m = self.m
         t = self.tokens if tokens is None else tokens
         p = self.pos if pos is None else pos
-        L.check(m.lib.sk_lm_decode_step(m._h, L.ptr(t), L.ptr(p), self.B, L.ptr(self.kv), self.T_cache,
-                                        L.ptr(self.logits_buf), self.ldl, L.ptr(self.ws), C.c_int64(self.ws.numel()),
-                                        L.stream_ptr()))
+        if self.head is None:
+            L.check(m.lib.sk_lm_decode_step(m._h, L.ptr(t), L.ptr(p), self.B, L.ptr(self.kv), self.T_cache,
+                                            L.ptr(self.logits_buf), self.ldl, L.ptr(self.ws), C.c_int64(self.ws.numel()),
+                                            L.stream_ptr()))
+        else:
+            L.check(m.lib.sk_lm_decode_step_sub(m._h, L.ptr(t), L.ptr(p), self.B, L.ptr(self.kv), self.T_cache,
+                                                L.ptr(self.head), self.ldl, L.ptr(self.logits_buf), self.ldl,
+                                                L.ptr(self.ws), C.c_int64(self.ws.numel()), L.stream_ptr()))
         return self.logits
 
     def select(self, cfg: "L.SkSampling", ban: Optional[torch.Tensor] = None, uniforms: Optional[torch.Tensor] = None) -> None:
         m = self.m
+        if self.sub_ids is not None:
+            if ban is not None or self.rules is not None:
+                raise ValueError("select: a session with allowed ids takes no ban bitmask or rules")
+            L.check(m.lib.sk_select_next_sub(L.ptr(self.logits_buf), self.ldl, L.ptr(self.sub_ids), self.sub_ids.numel(),
+                                             m.config.vocab_size, self.B, C.byref(cfg), L.ptr(uniforms),
+                                             C.byref(self.state), L.stream_ptr()))
+            return
         args = (L.ptr(self.logits_buf), self.ldl, m.config.vocab_size, self.B, L.ptr(ban), C.byref(cfg), L.ptr(uniforms),
                 C.byref(self.state))
         if self.rules is None:

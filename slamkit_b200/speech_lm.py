@@ -4,7 +4,9 @@ an audio tokeniser and, optionally, a unit vocoder, scoring and continuing zero-
 With the unit tokeniser the whole chain runs on the device: HuBERT units (`sk_hubert_units`) -> dedup (`sk_rle`) ->
 token ids (`sk_units_to_tokens`) -> LM forward (`sk_lm_forward`) -> per-sequence scores (`sk_seq_loglik`).  `generate`
 continues left-padded prompts with the cached decoder and vocodes every row in one batched `sk_vocoder_run` call.  The
-interleaved tokeniser builds its ids through the text tokenizer on the host, as the reference does."""
+interleaved tokeniser scores through the text tokenizer on the host, as the reference does; it continues speech on the
+device: `sk_units_to_prompt` builds the prompts and the decode steps compute only the head rows of the ids a SPEECH
+continuation may emit (`allowed_token_ids`)."""
 from __future__ import annotations
 
 from typing import List, Optional
@@ -42,18 +44,24 @@ class B200SpeechLM:
         tensor for an empty continuation), otherwise the decoded unit ids.  With `num_return_sequences = k` there are
         B*k rows, the k continuations of each prompt adjacent (HF's order)."""
         if not hasattr(self.tokeniser, "build_prompt"):
-            raise NotImplementedError("generate needs the unit tokeniser: interleaved (speech + text) prompts are not "
-                                      "supported")
+            raise NotImplementedError(f"generate: {type(self.tokeniser).__name__} cannot build generation prompts "
+                                      "(build_prompt); use the unit or the interleaved tokeniser")
         if output_modality is None or output_modality.upper() != "SPEECH":
             raise NotImplementedError(f"output_modality={output_modality!r}: only SPEECH continuations are supported")
         tokens = self.tokeniser.build_prompt(wavs, lens, output_modality=output_modality)
-        ignore = self.tokeniser.get_ignore_tokens(output_modality)
-        if ignore is not None:
-            ignore = [[tok] for tok in ignore]
-        conts = self.model.generate(tokens["input_ids"], attention_mask=tokens["attention_mask"], bad_words_ids=ignore,
-                                    **kwargs)
+        if hasattr(self.tokeniser, "allowed_ids"):
+            # the reference bans every id of get_ignore_tokens; the same continuation from the allowed ids' head rows
+            kwargs["allowed_token_ids"] = self.tokeniser.allowed_ids(output_modality, self.model.config.vocab_size)
+        else:
+            ignore = self.tokeniser.get_ignore_tokens(output_modality)
+            kwargs["bad_words_ids"] = [[tok] for tok in ignore] if ignore is not None else None
+        conts = self.model.generate(tokens["input_ids"], attention_mask=tokens["attention_mask"], **kwargs)
         if remove_prompt:
             conts = conts[..., tokens["input_ids"].size(1):]
+        if hasattr(self.tokeniser, "decode_units") and self.vocoder is not None:
+            wave, wl = self.vocoder.vocode_batch(self.tokeniser.decode_units(conts))
+            return [wave[i, :int(wl[i])] if int(wl[i]) > 0 else torch.zeros(0, device=wave.device)
+                    for i in range(conts.shape[0])]
         decoded = [self.tokeniser.decode_sample(c, output_modality=output_modality) for c in conts]
         if self.vocoder is None:
             return decoded

@@ -207,6 +207,111 @@ class B200InterleavingTokeniser:
         strs = self.stringify_representation(self.audio_represent(wav, lens))
         return self.string_tokenise(strs, return_tensors="pt", padding=True)
 
+    def _check_speech_output(self, wav, output_modality: Optional[str]) -> None:
+        if not isinstance(wav, torch.Tensor):
+            raise NotImplementedError("interleaved (speech + text) inputs are not supported: pass a speech-only wav batch")
+        if output_modality is None or output_modality.upper() != "SPEECH":
+            raise NotImplementedError(f"output_modality={output_modality!r}: only SPEECH continuations are supported")
+
+    def prompt_layout(self) -> Dict[str, object]:
+        """What build_prompt puts around the units, read off the text tokenizer once: `prefix` (the ids it adds before a
+        string with add_special_tokens=True: a bos for OPT-style tokenizers, nothing for Qwen2 / NeoX ones), `unit_id` (the
+        id of `<Un i>`, i < num_units) and `marker` (the id of `<speech>`).  A trailing eos the tokenizer appends is
+        dropped, as interleaving_tokeniser.py:260-262 drops it."""
+        lay = self.__dict__.get("_prompt_layout")
+        if lay is None:
+            tk = self.text_tokeniser
+            plain = tk("<Un0>", add_special_tokens=False)["input_ids"]
+            full = tk("<Un0>", add_special_tokens=True)["input_ids"]
+            at = next((i for i in range(len(full) - len(plain) + 1) if full[i:i + len(plain)] == plain), None)
+            if len(plain) != 1 or at is None:
+                raise NotImplementedError("the text tokenizer does not encode `<Un0>` as one token")
+            suffix = full[at + 1:]
+            if suffix and not (len(suffix) == 1 and tk.eos_token_id is not None and suffix[0] == tk.eos_token_id):
+                raise NotImplementedError(f"the text tokenizer appends {suffix} after a string; only a trailing eos "
+                                          "(dropped) is supported")
+            lay = {"prefix": list(full[:at]),
+                   "unit_id": tk.convert_tokens_to_ids([f"<Un{u}>" for u in range(self.num_units)]),
+                   "marker": tk.convert_tokens_to_ids(SPEECH_TOKEN)}
+            self._prompt_layout = lay
+        return lay
+
+    def _device_tables(self, device) -> Dict[str, torch.Tensor]:
+        key = ("_tables", str(device))
+        t = self.__dict__.get(key)
+        if t is None:
+            lay = self.prompt_layout()
+            tk = self.text_tokeniser
+            n = len(tk)
+            unit_of = torch.full((n,), -1, dtype=torch.long)
+            unit_of[torch.tensor(lay["unit_id"], dtype=torch.long)] = torch.arange(self.num_units)
+            # decode_sample drops pad / bos / eos and the markers before it looks for units
+            drop = [i for i in (tk.pad_token_id, tk.bos_token_id, tk.eos_token_id) if i is not None]
+            drop += [tk.encode(SPEECH_TOKEN)[0], tk.encode(TEXT_TOKEN)[0]]
+            unit_of[torch.tensor(drop, dtype=torch.long)] = -1
+            t = {"unit_id": torch.tensor(lay["unit_id"], dtype=torch.int32, device=device),
+                 "prefix": torch.tensor(lay["prefix"] or [0], dtype=torch.int32, device=device),
+                 "unit_of": unit_of.to(device)}
+            self.__dict__[key] = t
+        return t
+
+    def prompt_ids(self, units: torch.Tensor, counts: torch.Tensor) -> Dict[str, torch.Tensor]:
+        """The SPEECH generation prompt of interleaving_tokeniser.py:242-263, left-padded as SpeechLM.generate pads it,
+        from sk_rle's units int32 [B, T_units] and counts int32 [B] (device): row b is
+        `[pad..., prefix..., <Un u>..., <speech>]` with its attention mask (`sk_units_to_prompt`)."""
+        from . import _lib as L
+        lay, tab = self.prompt_layout(), self._device_tables(units.device)
+        B, T_units = units.shape
+        units, counts = units.to(torch.int32).contiguous(), counts.to(units.device, torch.int32).contiguous()
+        T = len(lay["prefix"]) + (int(counts.max()) if B else 0) + 1
+        ids = torch.empty((B, T), dtype=torch.int64, device=units.device)
+        mask = torch.empty_like(ids)
+        if B:
+            L.check(L.load().sk_units_to_prompt(L.ptr(units), L.ptr(counts), B, T_units, L.ptr(tab["unit_id"]),
+                                                self.num_units, L.ptr(tab["prefix"]), len(lay["prefix"]),
+                                                int(lay["marker"]), int(self.text_tokeniser.pad_token_id), L.ptr(ids),
+                                                L.ptr(mask), T, L.stream_ptr()))
+        return {"input_ids": ids, "attention_mask": mask}
+
+    @torch.inference_mode()
+    def build_prompt(self, wav: torch.Tensor, lens: Optional[torch.Tensor] = None,
+                     output_modality: Optional[str] = "SPEECH") -> Dict[str, torch.Tensor]:
+        """interleaving_tokeniser.py:242-263 for a speech-only batch and SPEECH output, on the device: HuBERT units ->
+        dedup (`sk_rle`) -> left-padded `[prefix, <Un u>..., <speech>]` rows."""
+        self._check_speech_output(wav, output_modality)
+        fe = self.model
+        if fe is None:
+            raise RuntimeError("This tokeniser does not have a feature extractor")
+        ids, nf = fe.units_device(wav, lens)
+        if self.dedup:
+            ids, _, nf = fe.dedup_device(ids, nf)
+        return self.prompt_ids(ids, nf)
+
+    def allowed_ids(self, output_modality: str = "SPEECH", vocab_size: Optional[int] = None) -> List[int]:
+        """The ids a SPEECH continuation may emit: the complement of get_ignore_tokens('SPEECH') in a model vocabulary
+        of `vocab_size` ids (default: the tokenizer's): the units, the tokenizer's bos / eos, whatever the reference's ban
+        list leaves, and the model's ids past the tokenizer's, which the ban list does not cover."""
+        if output_modality is None or output_modality.upper() != "SPEECH":
+            raise NotImplementedError(f"output_modality={output_modality!r}: only SPEECH continuations are supported")
+        ban = set(self.get_ignore_tokens("SPEECH"))
+        n = len(self.text_tokeniser) if vocab_size is None else int(vocab_size)
+        return [i for i in range(n) if i not in ban]
+
+    def decode_units(self, tokens: torch.Tensor) -> torch.Tensor:
+        """Batched device form of decode_sample(·, 'SPEECH'): the unit index of every `<Un i>` id of tokens [N, T],
+        -1 elsewhere (pad, bos, eos, markers, text and ids outside the tokenizer).  `vocode_batch` drops the -1s."""
+        unit_of = self._device_tables(tokens.device)["unit_of"]
+        t = tokens.long()
+        ok = (t >= 0) & (t < unit_of.numel())
+        return torch.where(ok, unit_of[t.clamp(0, unit_of.numel() - 1)], torch.full_like(t, -1))
+
+    def decode_sample(self, tokens: torch.Tensor, output_modality: str = "SPEECH") -> torch.Tensor:
+        """interleaving_tokeniser.py:268-287 for SPEECH: the `<Un i>` units of tokens, in order."""
+        if output_modality is None or output_modality.upper() != "SPEECH":
+            raise NotImplementedError(f"output_modality={output_modality!r}: only SPEECH continuations are supported")
+        u = self.decode_units(tokens.reshape(-1))
+        return u[u >= 0]
+
     def get_ignore_tokens(self, used_token_modality: Optional[str]) -> Optional[List[int]]:
         """interleaving_tokeniser.py:295-310: ids excluded from the log-likelihood.  SPEECH bans every text id except
         bos / eos, plus `<speech>` / `<text>`; TEXT bans the unit ids (not the two markers); anything else bans nothing."""
