@@ -742,10 +742,10 @@ int sk_flac_decode_i32(const char* path, int32_t* pcm_host, int64_t capacity, in
 /* ---- data-parallel gradient all-reduce over NVLink peer memory (single NVSwitch node) ----------------------------------
  * Replaces the per-bucket NCCL all-reduce of accelerate's DDP wrapper around `training_step` (HF:trainer.py:1867-2014;
  * config/training_args/default.yaml:18) for ranks that share a node: every rank maps every other rank's flat bf16
- * gradient buffer and a small flag array with CUDA IPC, and one small-footprint kernel per bucket (64-thread CTAs, no
- * shared memory: they co-reside with the GEMM / attention CTAs of the backward pass) reduce-scatters and all-gathers in
- * one pass -- rank r sums the W copies of its 1/W of the bucket in rank order (fp32, one rounding: bit-identical on all
- * ranks) and stores the result into all W buffers.  Protocol per bucket (all on one side stream):
+ * gradient buffer and a small flag array with CUDA IPC, and one small-footprint kernel per bucket (128-thread CTAs of
+ * <= 32 registers per thread, no shared memory: they co-reside with the GEMM / attention CTAs of the backward pass)
+ * reduce-scatters and all-gathers in one pass -- rank r sums the W copies of its 1/W of the bucket in rank order (fp32,
+ * one rounding: bit-identical on all ranks) and stores the result into all W buffers.  Protocol per bucket (all on one side stream):
  *   sk_p2p_signal(slot, epoch)  this rank's gradients of the bucket are final (READY flag to every peer)
  *   sk_p2p_allreduce_bf16(...)  waits for every peer's READY, reduces, tells every peer when its share is written
  *   sk_p2p_wait(slots, epoch)   returns (in stream order) when every peer's share of those slots has arrived in this
@@ -766,7 +766,7 @@ int sk_p2p_wait(void* const* flags, int rank, int world, int slot_lo, int n_slot
 /* Profiling hook: uint64 [257][4] device buffer that the kernels above fill with %globaltimer stamps per slot (0 READY sent,
  * 1 reduce kernel running, 2 peers ready, 3 last CTA done; row 256: wait kernel start / end); NULL switches it off. */
 int sk_p2p_set_trace(void* buf);
-/* Test hook: `ctas` CTAs with the reduce kernel's footprint (64 threads, <= 64 registers, no shared memory) that hold their
+/* Test hook: `ctas` CTAs with the reduce kernel's footprint (128 threads, <= 32 registers, no shared memory) that hold their
  * slot for `ns` nanoseconds; started_u32 counts the CTAs that got onto an SM. */
 int sk_p2p_debug_hog(int ctas, int64_t ns, void* started_u32, void* stream);
 

@@ -70,7 +70,7 @@ SK_DEVINL void st_peer128(void* p, uint4 v) {
   asm volatile("st.global.v4.u32 [%0], {%1, %2, %3, %4};" ::"l"(p), "r"(v.x), "r"(v.y), "r"(v.z), "r"(v.w) : "memory");
 }
 
-// optional timeline (tools/p2p_trace.py): [slot][4] globaltimer stamps -- 0 READY signalled, 1 first CTA of the reduce
+// optional timeline (sk_p2p_set_trace): [slot][4] globaltimer stamps -- 0 READY signalled, 1 first CTA of the reduce
 // kernel running, 2 peers ready, 3 last CTA done; row P2P_SLOTS: 0 wait kernel running, 1 all shares arrived
 __device__ unsigned long long* g_p2p_trace = nullptr;
 
@@ -174,7 +174,7 @@ p2p_allreduce_kernel(P2PPeers pr, uint32_t* own_flags, int rank, int world, size
   }
 }
 
-// Stand-in with exactly the reduce kernel's footprint (64 threads, <= 64 registers, no shared memory) that just occupies
+// Stand-in with exactly the reduce kernel's footprint (128 threads, <= 32 registers, no shared memory) that just occupies
 // its slot for `ns` nanoseconds: timing the backward kernels with and without it resident shows which of them share an SM
 // with the reduce kernel.
 __global__ void __launch_bounds__(P2P_THREADS, 16) p2p_hog_kernel(unsigned long long ns, unsigned* started, float* sink) {
@@ -311,7 +311,9 @@ int sk_p2p_signal_launch(void* const* flags, int rank, int world, int slot, uint
 int sk_p2p_wait_launch(void* const* flags, int rank, int world, int slot_lo, int n_slots, uint32_t epoch, int* err_flag, cudaStream_t s) {
   P2PPeers pr;
   if (int rc = fill_peers(pr, nullptr, flags, rank, world)) return rc;
-  SK_REQUIRE(slot_lo >= 0 && n_slots >= 1 && slot_lo + n_slots <= P2P_SLOTS, "p2p: slots [%d, +%d) out of range", slot_lo, n_slots);
+  // (n_slots <= P2P_SLOTS - slot_lo: slot_lo + n_slots could overflow int and pass the bound)
+  SK_REQUIRE(slot_lo >= 0 && slot_lo < P2P_SLOTS && n_slots >= 1 && n_slots <= P2P_SLOTS - slot_lo, "p2p: slots [%d, +%d) out of range",
+             slot_lo, n_slots);
   p2p_wait_kernel<<<1, 256, 0, s>>>(pr.flag[rank], rank, world, slot_lo, n_slots, epoch, err_flag);
   SK_LAUNCH_CHECK();
   return 0;

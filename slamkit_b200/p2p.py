@@ -2,9 +2,9 @@
 
 Takes the place of the NCCL all-reduce accelerate's DDP wrapper issues for the reference (`SLAMTrainer` under `torchrun`,
 HF:trainer.py:1867-2014): every rank maps every peer's gradient buffer and a flag array with CUDA IPC (handles travel
-through `torch.distributed.all_gather_object`, once, at construction) and a 64-thread-per-CTA kernel without shared
-memory reduces a bucket in one pass while the backward pass keeps all SMs busy.  Sums are taken in rank order in fp32 and
-rounded once, so every rank ends up with bit-identical gradients.
+through `torch.distributed.all_gather_object`, once, at construction) and a kernel of 128-thread CTAs with at most 32
+registers per thread and no shared memory reduces a bucket in one pass while the backward pass keeps all SMs busy.
+Sums are taken in rank order in fp32 and rounded once, so every rank ends up with bit-identical gradients.
 """
 from __future__ import annotations
 

@@ -1,5 +1,5 @@
 """Which kernels of the backward pass share an SM with the peer all-reduce kernel?  A stand-in with the reduce kernel's
-exact footprint (64 threads, <= 64 registers, no shared memory; sk_p2p_debug_hog) is parked on every SM for 30 ms on a
+exact footprint (128 threads, <= 32 registers, no shared memory; sk_p2p_debug_hog) is parked on every SM for 30 ms on a
 high-priority side stream; each kernel is timed alone and while the stand-ins are resident.  A kernel that cannot
 co-reside either waits for them (time jumps by milliseconds) or loses occupancy."""
 import ctypes as C, os, sys, time
